@@ -1,4 +1,4 @@
-/* speech_b200 — C ABI of the B200-native (sm_100a) hot path of awni/speech.
+/* speech_b200 — C ABI of the H100-native (sm_90a) hot path of awni/speech.
  *
  * Boundary rules (SURVEY.md §8b):
  *   - plain C symbols, raw pointers and sizes, no torch / C++ types in any signature;
@@ -54,7 +54,7 @@ int sb_ctc_fwd_bwd(const float* acts, float* grads, const int* labels, const int
                    void* stream);
 
 /* ---------------------------------------------------------------------------------------
- * Dense contraction on tcgen05 tensor cores:
+ * Dense contraction on wgmma tensor cores:
  *     C[M,N] (f32)  (+)=  A[M,K] (bf16, row-major) * B[N,K]^T (bf16, row-major)  (+ bias[N])
  * Replaces: the cuBLAS/cuDNN GEMMs reached through nn.GRU / nn.Linear
  *           (speech/models/model.py:35-39, 115-133).
@@ -350,10 +350,6 @@ int sb_log_specgram(const short* pcm, const long long* offsets, const int* n_sam
 /* Developer hook (not part of the drop-in surface): device buffer of >= 64*16 uint64 receiving a
  * globaltimer timeline of CTA 0 for the next sb_gru_fwd launches; NULL disables. */
 int sb_debug_gru_timeline(void* dev_buffer);
-/* Developer hook, kernel selection of sb_gemm_bf16_tn (default 1|4): bit 0 = no 256-row
- * single-CTA tile variant, bit 1 = register-store epilogue instead of TMA stores, bit 2 = allow
- * the CTA-pair (tcgen05 cta_group::2) kernel. */
-int sb_debug_gemm_mt1(int force);
 int sb_debug_umma_mn(int lbo_bytes, int sbo_bytes, int kadv_bytes);
 /* Developer hook, GRU kernel selection / timing knobs (0 = defaults): 8 / 16 = never / always use
  * the transposed-accumulator K-split kernels, 32 = no K-split forward kernel, 64 / 128 = polling

@@ -1,6 +1,6 @@
-"""speech_b200 - B200-native (sm_100a) replacement for the data-parallel hot path of awni/speech.
+"""speech_b200 - H100-native (sm_90a) replacement for the data-parallel hot path of awni/speech.
 
-Layout (SURVEY.md §8, DESIGN.md):
+Layout (SURVEY.md §8):
     csrc/        hand-written CUDA kernels + the C ABI (include/speech_b200.h), built in-tree
     _lib.py      ctypes binding of that ABI (no CPU fallback)
     functions/   operator-level drop-ins: functions.ctc.CTCLoss, transducer.* (reference imports)

@@ -78,7 +78,6 @@ SIGNATURES = {
     "sb_debug_gru_cluster": (_c_int, [_c_int]),
     "sb_debug_gru_ksplit": (_c_int, [_c_int]),
     "sb_debug_gru_flags": (_c_int, [_c_int]),
-    "sb_debug_gemm_mt1": (_c_int, [_c_int]),
     "sb_debug_umma_mn": (_c_int, [_c_int, _c_int, _c_int]),
     "sb_edit_distance": (_c_ll, [_vp, _c_ll, _vp, _c_ll]),
     "sb_log_specgram": (_c_int, [_vp, _vp, _vp, _c_int, _c_int, _c_int, ctypes.c_double, _fl, _vp,

@@ -1,4 +1,4 @@
-"""Build libspeech_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Build libspeech_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
     python -m speech_b200.csrc.build [--force] [--verbose]
 
@@ -17,7 +17,7 @@ LIB = os.path.join(os.path.dirname(HERE), "libspeech_b200.so")
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -76,7 +76,7 @@ def build(force=False, verbose=False):
         raise RuntimeError("speech_b200: CUDA build failed")
     newest = max(os.path.getmtime(o) for o in objs)
     if force or procs or not os.path.exists(LIB) or os.path.getmtime(LIB) < newest:
-        cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-lcudart"]
+        cmd = [NVCC] + FLAGS[:2] + ["-shared", "-o", LIB] + objs + ["-lcudart"]
         subprocess.check_call(cmd)
     return LIB
 

@@ -11,7 +11,7 @@
 //       pre-activation sign is available to the backward mask);
 //   im2col matrix A[m][(i*kw + j)*Ci + ci] bf16 (K padded to a multiple of 8 with zeros); the
 //       weights are permuted to the same K order on the host side (40 K elements);
-//   conv = sb_gemm_bf16_tn(A, Wp) + bias  on tcgen05.
+//   conv = sb_gemm_bf16_tn(A, Wp) + bias  on the wgmma GEMM.
 // Backward: dC (pre-activation grad, bf16) -> dW = dC^T A (GEMM on transposed copies, split-K),
 //   dA = dC Wp (GEMM), col2im as a GATHER (each input pixel sums its <= ceil(kh/s)*ceil(kw/s)
 //   taps; no atomics) fused with the ReLU mask of the layer below.

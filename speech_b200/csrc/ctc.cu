@@ -22,7 +22,7 @@
 // and the 1e-4 parity bar holds for long utterances.
 //
 // Roofline: nominally HBM (read logits + write grads = 2*B*T*V*4 bytes), in practice bound by
-// the T-step serial chain (see DESIGN.md).
+// the T-step serial chain.
 #include "common.cuh"
 #include <math.h>
 

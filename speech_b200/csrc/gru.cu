@@ -1,4 +1,4 @@
-// Persistent GRU recurrence kernels (forward and backward in time) for sm_100a.
+// Persistent GRU recurrence kernels (forward and backward in time) for sm_90a.
 //
 // Replaces the cuDNN RNN reached through nn.GRU in the reference encoder
 // (speech/models/model.py:35-39 construction, :73 call; gate order r,z,n; bidirectional halves
@@ -9,24 +9,25 @@
 // sb_gemm_bf16_tn; these kernels run the T-serial part.  One cooperative launch per layer covers
 // BOTH directions:
 //   * CTA c of direction d owns 16 hidden units j0..j0+15: its 48 rows of W_hh (r,z,n) stay
-//     resident in shared memory (bf16, UMMA K-major SWIZZLE_128B chunks) for all T steps;
+//     resident in shared memory (bf16, wgmma K-major SWIZZLE_128B chunks) for all T steps;
 //   * per step every CTA needs ALL of h_{t-1} (bf16, written by the CTAs of its direction in the
 //     previous step).  CTAs form thread-block clusters of up to 8; each CTA fetches 1/CS of the
 //     [Bp x 64] chunks with TMA and MULTICASTS them into the shared memory of all CTAs of its
 //     cluster, so L2 is read once per cluster instead of once per CTA (the un-multicast version
 //     was bound by 64 SMs hammering the same L2 lines: 4 us of a 13 us step);
-//   * one thread issues tcgen05.mma  D[batch(128) x 48] += h_{t-1}[batch x 64] * Wslice[48 x 64]^T
-//     per chunk as its mbarrier completes; accumulators live in TMEM;
-//   * 8 epilogue warps (thread = TMEM lane = batch row, 8 hidden units each) read the
-//     accumulators with tcgen05.ld, apply the gate math in fp32 (h_{t-1} of the thread's own units
+//   * one warpgroup issues wgmma  D[batch x 48] += h_{t-1}[batch x 64] * Wslice[48 x 64]^T
+//     (one m64 block per 64 batch rows) per chunk as its mbarrier completes, accumulates in
+//     registers and parks the finished product in shared memory;
+//   * 8 epilogue warps (thread = batch row, 8 hidden units each) read the product back, apply
+//     the gate math in fp32 (h_{t-1} of the thread's own units
 //     stays in registers across steps), publish the bf16 h_t, arrive on the per-direction grid
 //     barrier, and only then write the fp32 state / transposed copy / saved gates;
 //   * the grid barrier is one red.release.gpu + ld.acquire.gpu polling on a global counter.
 // The backward kernel has the same structure with W_hh^T resident (16 rows x 3H) and the
 // all-gather over the pre-activation gradients dgh_t (batch x 3H).
 //
-// Roofline: tensor work, but each step is bound by the all-gather + barrier latency; DESIGN.md
-// reports us/step next to the tensor-pipe share.
+// Roofline: tensor work, but each step is bound by the all-gather + barrier latency
+// (tools/gru_timeline.py prints the per-step timeline).
 #include "common.cuh"
 #include <cuda.h>
 #include <string.h>
@@ -40,7 +41,9 @@ static constexpr int GRU_HC = 16;            // hidden units per CTA
 static constexpr int GRU_UPT = 8;            // hidden units per epilogue thread
 static constexpr int GRU_MAX_RING = 16;      // smem ring slots for the gathered operand
 static constexpr int GRU_EPI = 256;          // warps 0..7: epilogue
-static constexpr int GRU_THREADS = GRU_EPI + 64;  // + warp 8: MMA issuer/TMEM owner, warp 9: TMA
+static constexpr int GRU_MMA_WARP = 8;       // warps 8..11: the wgmma warpgroup
+static constexpr int GRU_TMA_WARP = 12;      // warp 12: TMA producer
+static constexpr int GRU_THREADS = GRU_EPI + 128 + 32;
 
 typedef __nv_bfloat16 bf16;
 
@@ -133,13 +136,13 @@ SB_DEVINL void tma_load_2d_mc(void* smem_dst, const void* tmap, uint64_t* bar, i
         "r"(c0), "r"(c1), "h"(mask)
       : "memory");
 }
-// arrive (when all prior MMAs of this thread retire) on the mbarrier at this offset in every CTA
-// of `mask`
-SB_DEVINL void umma_commit_mc(uint64_t* bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64"
-      " [%0], %1;" ::"r"(smem_u32(bar)), "h"(mask)
-      : "memory");
+// arrive on the mbarrier at this offset in each of the first `cs` CTAs of the cluster
+SB_DEVINL void mbar_arrive_all_ctas(uint64_t* bar, uint32_t cs) {
+  for (uint32_t r = 0; r < cs; ++r) {
+    uint32_t ra;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(smem_u32(bar)), "r"(r));
+    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(ra) : "memory");
+  }
 }
 
 struct GruSmem {
@@ -149,8 +152,8 @@ struct GruSmem {
   uint64_t* full;   // [GRU_MAX_RING]
   uint64_t* empty;  // [GRU_MAX_RING]
   uint64_t* accfull;
-  uint32_t* tmem_slot;
   float* scratch;   // [64]
+  float* accbuf;    // [Bp][N + 4] the finished recurrent product, batch-major
 };
 
 SB_DEVINL GruSmem carve(uint8_t* raw, int ring_bytes, int wbytes) {
@@ -162,8 +165,8 @@ SB_DEVINL GruSmem carve(uint8_t* raw, int ring_bytes, int wbytes) {
   s.full = bars;
   s.empty = bars + GRU_MAX_RING;
   s.accfull = bars + 2 * GRU_MAX_RING;
-  s.tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * GRU_MAX_RING + 1);
   s.scratch = reinterpret_cast<float*>(bars + 2 * GRU_MAX_RING + 2);
+  s.accbuf = s.scratch + 64;
   return s;
 }
 
@@ -196,35 +199,48 @@ SB_DEVINL void tma_gather(const GruSmem& s, const CUtensorMap* tm, int row0, int
   }
 }
 
-// MMA thread: consume the step's chunks against the resident weight chunks.
-template <int N>
-SB_DEVINL void mma_consume(const GruSmem& s, uint32_t tmem_d, int nchunks, int wchunk_bytes,
-                           int Bp, int ring, int gc, int k, uint32_t cs) {
-  constexpr uint32_t idesc = umma_idesc_bf16_f32(128, N);
+// MMA warpgroup: consume the step's chunks against the resident weight chunks, one m64 block per
+// 64 batch rows, then park D[Bp x N] in s.accbuf (pitch N + 4) and arrive on s.accfull (count 128).
+// (TWO: Bp > 64, a second m64 block; a template parameter so that no wgmma sits under a branch.
+// The scale-d = 0 first MMA initialises the accumulators.)
+template <int N, bool TWO>
+SB_DEVINL void mma_consume(const GruSmem& s, int nchunks, int wchunk_bytes, int Bp, int ring,
+                           int gc, int k, uint32_t cs) {
   const int stride = Bp * 128;
   const int ngroups = nchunks / gc;
   const int upr = ngroups / ring;
-  const uint16_t mask = (uint16_t)((1u << cs) - 1u);
+  constexpr bool two = TWO;
+  float d0[N / 2], d1[N / 2];
   for (int g = 0; g < ngroups; ++g) {
     const int slot = g % ring;
     const unsigned int P = (unsigned int)(k * upr + g / ring);
     mbar_wait(&s.full[slot], P & 1u);
-    tc_fence_after_sync();
+    wgmma_fence();
     for (int i = 0; i < gc; ++i) {
       const int c = g * gc + i;
-      const uint64_t da = umma_desc_sw128_kmajor(smem_u32(s.ring + (slot * gc + i) * stride));
-      const uint64_t db = umma_desc_sw128_kmajor(smem_u32(s.wtile + c * wchunk_bytes));
+      const uint32_t sa = smem_u32(s.ring + (slot * gc + i) * stride);
+      const uint64_t da0 = gmma_desc_sw128_kmajor(sa);
+      const uint64_t da1 = gmma_desc_sw128_kmajor(sa + 64 * 128);
+      const uint64_t db = gmma_desc_sw128_kmajor(smem_u32(s.wtile + c * wchunk_bytes));
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk)
-        umma_bf16_ss(tmem_d, da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), idesc,
-                     (c > 0 || kk > 0) ? 1u : 0u);
+      for (int kk = 0; kk < 4; ++kk) {
+        const uint32_t acc = (c > 0 || kk > 0) ? 1u : 0u;
+        wgmma_bf16<N>(d0, da0 + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), acc);
+        if (two) wgmma_bf16<N>(d1, da1 + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), acc);
+      }
     }
-    if (ring < ngroups) {
-      if (cs > 1) umma_commit_mc(&s.empty[slot], mask);
-      else umma_commit(&s.empty[slot]);
+    wgmma_commit();
+    wgmma_wait<0>();
+    if (ring < ngroups && (threadIdx.x & 127) == 0) {
+      if (cs > 1) mbar_arrive_all_ctas(&s.empty[slot], cs);   // the slot is free in every CTA
+      else mbar_arrive(&s.empty[slot]);
     }
   }
-  umma_commit(s.accfull);
+  wgmma_fence_regs(d0);
+  wgmma_fence_regs(d1);
+  wg_store_rows<N>(d0, s.accbuf, N + 4, 0, Bp);
+  if (two) wg_store_rows<N>(d1, s.accbuf, N + 4, 64, Bp);
+  mbar_arrive(s.accfull);
 }
 
 SB_DEVINL float fast_sigmoid(float x) { return __fdividef(1.0f, 1.0f + __expf(-x)); }
@@ -257,14 +273,6 @@ SB_DEVINL uint4 pack8(const float (&v)[8]) {
   r.z = pack_bf16x2(v[4], v[5]); r.w = pack_bf16x2(v[6], v[7]);
   return r;
 }
-SB_DEVINL void tmem_ld_32x32b_x8(uint32_t taddr, uint32_t (&v)[8]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7])
-      : "r"(taddr)
-      : "memory");
-}
 
 // =============================================================================================
 // forward
@@ -289,7 +297,7 @@ gru_fwd_kernel(const __grid_constant__ CUtensorMap tm_d0, const __grid_constant_
   const CUtensorMap* tm = dir == 0 ? &tm_d0 : &tm_d1;
   const uint32_t crank = cluster_rank(), csize = cluster_size();
 
-  // ---- one-time setup: zero ring + weight region, stage the 48 weight rows, barriers, TMEM ----
+  // ---- one-time setup: zero ring + weight region, stage the 48 weight rows, barriers ----
   for (int k = tid; k < (ring_bytes + wbytes) / 16; k += GRU_THREADS)
     reinterpret_cast<uint4*>(s.ring)[k] = make_uint4(0, 0, 0, 0);
   __syncthreads();
@@ -315,20 +323,16 @@ gru_fwd_kernel(const __grid_constant__ CUtensorMap tm_d0, const __grid_constant_
       mbar_init(&s.full[i], 1);
       mbar_init(&s.empty[i], csize);
     }
-    mbar_init(s.accfull, 1);
+    mbar_init(s.accfull, 128);
     mbar_fence_init();
     tma_prefetch_desc(tm);
   }
-  if (warp == 8) tmem_alloc(s.tmem_slot, 64);
   fence_proxy_async_smem();
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
   cluster_sync_all();   // peers' barriers are initialised before anyone multicasts into them
-  const uint32_t tmem_base = *s.tmem_slot;
   unsigned int* ctr = p.barrier + dir * 32;   // one L2 line per direction
 
-  if (warp == 9) {
+  if (warp == GRU_TMA_WARP) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       for (int step = 1; step < T; ++step) {
@@ -341,17 +345,16 @@ gru_fwd_kernel(const __grid_constant__ CUtensorMap tm_d0, const __grid_constant_
         GRU_STAMP(1);
       }
     }
-  } else if (warp == 8) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      for (int step = 1; step < T; ++step) {
-        mma_consume<48>(s, tmem_base, nchunks, WCHUNK, Bp, p.ring, p.gc, step - 1, csize);
-        GRU_STAMP(2);
-      }
+  } else if (warp >= GRU_MMA_WARP) {
+    // ===================== MMA warpgroup =====================
+    for (int step = 1; step < T; ++step) {
+      if (Bp > 64) mma_consume<48, true>(s, nchunks, WCHUNK, Bp, p.ring, p.gc, step - 1, csize);
+      else mma_consume<48, false>(s, nchunks, WCHUNK, Bp, p.ring, p.gc, step - 1, csize);
+      if (tid == GRU_MMA_WARP * 32) GRU_STAMP(2);
     }
   } else {
     // ===================== epilogue: thread = (batch row, half of the 16 units) ==============
-    const int row = (warp & 3) * 32 + lane;      // TMEM lane this thread may read
+    const int row = (warp & 3) * 32 + lane;      // batch row
     const int uh = warp >> 2;                    // which 8 of the CTA's 16 units
     const int ju = j0 + uh * GRU_UPT;
     float hprev[GRU_UPT];
@@ -376,17 +379,11 @@ gru_fwd_kernel(const __grid_constant__ CUtensorMap tm_d0, const __grid_constant_
       if (step > 0) {
         mbar_wait(s.accfull, (step - 1) & 1);
         if (tid == 0) GRU_STAMP(3);
-        tc_fence_after_sync();
-        uint32_t v[8];
+        const float* ar = s.accbuf + row * (48 + 4) + uh * GRU_UPT;
 #pragma unroll
-        for (int gg = 0; gg < 3; ++gg) {
-          tmem_ld_32x32b_x8(tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + gg * 16 + uh * GRU_UPT,
-                            v);
-          tmem_ld_wait();
+        for (int gg = 0; gg < 3; ++gg)
 #pragma unroll
-          for (int jj = 0; jj < GRU_UPT; ++jj) acc[gg][jj] = __uint_as_float(v[jj]);
-        }
-        tc_fence_before_sync();
+          for (int jj = 0; jj < GRU_UPT; ++jj) acc[gg][jj] = active ? ar[gg * 16 + jj] : 0.f;
         if (tid == 0) GRU_STAMP(4);
       } else {
 #pragma unroll
@@ -437,13 +434,8 @@ gru_fwd_kernel(const __grid_constant__ CUtensorMap tm_d0, const __grid_constant_
     }
   }
 
-  tc_fence_before_sync();
   __syncthreads();
   cluster_sync_all();   // no CTA leaves while peers may still signal its barriers
-  if (warp == 8) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 64);
-  }
 }
 
 // =============================================================================================
@@ -491,20 +483,16 @@ gru_bwd_kernel(const __grid_constant__ CUtensorMap tm_d0, const __grid_constant_
       mbar_init(&s.full[i], 1);
       mbar_init(&s.empty[i], csize);
     }
-    mbar_init(s.accfull, 1);
+    mbar_init(s.accfull, 128);
     mbar_fence_init();
     tma_prefetch_desc(tm);
   }
-  if (warp == 8) tmem_alloc(s.tmem_slot, 32);
   fence_proxy_async_smem();
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
   cluster_sync_all();
-  const uint32_t tmem_base = *s.tmem_slot;
   unsigned int* ctr = p.barrier + dir * 32;   // one L2 line per direction
 
-  if (warp == 9) {
+  if (warp == GRU_TMA_WARP) {
     if (lane == 0) {
       // the recurrent product is needed for every step except the last one processed
       for (int step = 0; step + 1 < T; ++step) {
@@ -514,12 +502,11 @@ gru_bwd_kernel(const __grid_constant__ CUtensorMap tm_d0, const __grid_constant_
         GRU_STAMP(1);
       }
     }
-  } else if (warp == 8) {
-    if (lane == 0) {
-      for (int step = 0; step + 1 < T; ++step) {
-        mma_consume<16>(s, tmem_base, nchunks, WCHUNK, Bp, p.ring, p.gc, step, csize);
-        GRU_STAMP(2);
-      }
+  } else if (warp >= GRU_MMA_WARP) {
+    for (int step = 0; step + 1 < T; ++step) {
+      if (Bp > 64) mma_consume<16, true>(s, nchunks, WCHUNK, Bp, p.ring, p.gc, step, csize);
+      else mma_consume<16, false>(s, nchunks, WCHUNK, Bp, p.ring, p.gc, step, csize);
+      if (tid == GRU_MMA_WARP * 32) GRU_STAMP(2);
     }
   } else {
     const int row = (warp & 3) * 32 + lane;
@@ -560,14 +547,10 @@ gru_bwd_kernel(const __grid_constant__ CUtensorMap tm_d0, const __grid_constant_
       if (step > 0) {
         mbar_wait(s.accfull, (step - 1) & 1);
         if (tid == 0) GRU_STAMP(3);
-        tc_fence_after_sync();
-        uint32_t v[8];
-        tmem_ld_32x32b_x8(tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + uh * GRU_UPT, v);
-        tmem_ld_wait();
-        tc_fence_before_sync();
+        const float* ar = s.accbuf + row * (16 + 4) + uh * GRU_UPT;
         if (tid == 0) GRU_STAMP(4);
 #pragma unroll
-        for (int jj = 0; jj < GRU_UPT; ++jj) dh_rec[jj] += __uint_as_float(v[jj]);
+        for (int jj = 0; jj < GRU_UPT; ++jj) dh_rec[jj] += active ? ar[jj] : 0.f;
       }
       float dr[GRU_UPT], dz[GRU_UPT], dn[GRU_UPT], dnr[GRU_UPT];
       if (active) {
@@ -640,13 +623,8 @@ gru_bwd_kernel(const __grid_constant__ CUtensorMap tm_d0, const __grid_constant_
     }
   }
 
-  tc_fence_before_sync();
   __syncthreads();
   cluster_sync_all();
-  if (warp == 8) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 32);
-  }
 }
 
 // =============================================================================================
@@ -735,7 +713,6 @@ gru_bwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
   uint64_t* full = bars;          // [4] groups
   uint64_t* accfull = bars + 4;
   uint64_t* recvbar = bars + 5;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 6);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int D = p.ndir * H;
   const CUtensorMap* tm = dir == 0 ? &tm_d0 : &tm_d1;
@@ -763,21 +740,17 @@ gru_bwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
   }
   if (tid == 0) {
     for (int i = 0; i < 4; ++i) mbar_init(&full[i], 1);
-    mbar_init(accfull, 1);
+    mbar_init(accfull, 128);
     mbar_init(recvbar, 1);   // one local arrive.expect_tx per step; the peers' copies complete_tx
     mbar_fence_init();
     tma_prefetch_desc(tm);
   }
-  if (warp == 8) tmem_alloc(tmem_slot, 64);
   fence_proxy_async_smem();
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
   cluster_sync_all();
-  const uint32_t tmem_base = *tmem_slot;
   unsigned int* ctr = p.barrier + dir * 32;   // one L2 line per direction
 
-  if (warp == 9) {
+  if (warp == GRU_TMA_WARP) {
     if (lane == 0) {
       for (int step = 0; step + 1 < T; ++step) {
         grid_wait(ctr, (unsigned int)nC * (step + 1), p.ablate & 192);   // dgh of this step is complete
@@ -791,25 +764,47 @@ gru_bwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
         }
       }
     }
-  } else if (warp == 8) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16_f32(128, 64);
-      for (int step = 0; step + 1 < T; ++step) {
-        for (int g = 0; g < ngroups; ++g) {
-          mbar_wait(&full[g], step & 1);
-          tc_fence_after_sync();
-          for (int i = 0; i < gc; ++i) {
-            const int c = g * gc + i;
-            const uint64_t da = umma_desc_sw128_kmajor(smem_u32(ring + c * stride));
-            const uint64_t db = umma_desc_sw128_kmajor(smem_u32(wtile + c * WCHUNK));
+  } else if (warp >= GRU_MMA_WARP) {
+    // ===================== MMA warpgroup: D[Bp x 64 units] for this K quarter ===============
+    // The product is written straight into the reduce-scatter buffers: the 16 columns of peer pr
+    // into stage[pr], the CTA's own 16 columns into recv[crank] (which no peer writes).
+    const int t = tid & 127;
+    const bool two = Bp > 64;                 // batch rows 64..127: a second m64 block
+    for (int step = 0; step + 1 < T; ++step) {
+      float d[2][32];   // initialised by the scale-d = 0 first MMA (d[1] only used if two)
+      for (int g = 0; g < ngroups; ++g) {
+        mbar_wait(&full[g], step & 1);
+        wgmma_fence();
+        for (int i = 0; i < gc; ++i) {
+          const int c = g * gc + i;
+          const uint32_t sa = smem_u32(ring + c * stride);
+          const uint64_t da0 = gmma_desc_sw128_kmajor(sa);
+          const uint64_t da1 = gmma_desc_sw128_kmajor(sa + 64 * 128);
+          const uint64_t db = gmma_desc_sw128_kmajor(smem_u32(wtile + c * WCHUNK));
 #pragma unroll
-            for (int kk = 0; kk < 4; ++kk)
-              umma_bf16_ss(tmem_base, da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), idesc,
-                           (c > 0 || kk > 0) ? 1u : 0u);
+          for (int kk = 0; kk < 4; ++kk) {
+            const uint32_t acc = (c > 0 || kk > 0) ? 1u : 0u;
+            wgmma_bf16<64>(d[0], da0 + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), acc);
+            if (two) wgmma_bf16<64>(d[1], da1 + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), acc);
           }
         }
-        umma_commit(accfull);
+        wgmma_commit();
       }
+      wgmma_wait<0>();
+      wgmma_fence_regs(d[0]);
+      wgmma_fence_regs(d[1]);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int i = 0; i < 32; ++i) {
+          const int r = h * 64 + wg_frag_row(t, i), col = wg_frag_col(t, i);
+          const uint32_t pr = (uint32_t)(col >> 4);
+          if (r < Bp)
+            (pr == crank ? recv : stage)[((size_t)pr * Bp + r) * 16 + (col & 15)] = d[h][i];
+        }
+      }
+      fence_proxy_async_smem();   // generic st.shared -> the bulk copies (async proxy) to the peers
+      mbar_arrive(accfull);
     }
   } else {
     const int row = (warp & 3) * 32 + lane;
@@ -848,47 +843,22 @@ gru_bwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
       if (step > 0) {
         mbar_wait(accfull, (step - 1) & 1);
         if (tid == 0) GRU_STAMP(3);
-        tc_fence_after_sync();
-        float own[GRU_UPT];
-        if (tid == 0) mbar_expect_tx(recvbar, (uint32_t)((KS - 1) * Bp * 16 * 4));
-        // the peers' slices first, each staged and sent as soon as it is complete (see
-        // gru_fwd_ks_kernel); the own slice last
-#pragma unroll 1
-        for (int q = 1; q <= KS; ++q) {
-          const uint32_t pr = (crank + (uint32_t)q) % KS;      // q == KS: own slice
-          uint32_t v[8];
-          tmem_ld_32x32b_x8(tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + pr * 16 +
-                                uh * GRU_UPT, v);
-          tmem_ld_wait();
-          if (q == KS) {
-#pragma unroll
-            for (int jj = 0; jj < GRU_UPT; ++jj) own[jj] = __uint_as_float(v[jj]);
-          } else {
-            if (active) {
-              float4* sp = reinterpret_cast<float4*>(stage + ((size_t)pr * Bp + row) * 16 +
-                                                     uh * GRU_UPT);
-              sp[0] = make_float4(__uint_as_float(v[0]), __uint_as_float(v[1]),
-                                  __uint_as_float(v[2]), __uint_as_float(v[3]));
-              sp[1] = make_float4(__uint_as_float(v[4]), __uint_as_float(v[5]),
-                                  __uint_as_float(v[6]), __uint_as_float(v[7]));
-            }
-            fence_proxy_async_smem();
-            epi_barrier();
-            if (tid == 0)
-              bulk_s2peer(mapa_shared(smem_u32(recv + (size_t)crank * Bp * 16), pr),
-                          stage + (size_t)pr * Bp * 16, (uint32_t)(Bp * 16 * 4),
-                          mapa_shared(smem_u32(recvbar), pr));
+        // the MMA warpgroup staged the peers' slices: one bulk copy into each peer's receive
+        // buffer; the own slice already sits in recv[crank]
+        if (tid == 0) {
+          mbar_expect_tx(recvbar, (uint32_t)((KS - 1) * Bp * 16 * 4));
+          for (uint32_t q = 1; q < KS; ++q) {
+            const uint32_t pr = (crank + q) % KS;
+            bulk_s2peer(mapa_shared(smem_u32(recv + (size_t)crank * Bp * 16), pr),
+                        stage + (size_t)pr * Bp * 16, (uint32_t)(Bp * 16 * 4),
+                        mapa_shared(smem_u32(recvbar), pr));
           }
         }
-        tc_fence_before_sync();
         if (tid == 0) GRU_STAMP(4);
         mbar_wait(recvbar, (step - 1) & 1);
-#pragma unroll
-        for (int jj = 0; jj < GRU_UPT; ++jj) dh_rec[jj] += own[jj];
         if (active) {
 #pragma unroll
           for (int src = 0; src < KS; ++src) {
-            if ((uint32_t)src == crank) continue;
             const float4* rp = reinterpret_cast<const float4*>(
                 recv + ((size_t)src * Bp + row) * 16 + uh * GRU_UPT);
             const float4 a = rp[0], b = rp[1];
@@ -957,13 +927,8 @@ gru_bwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
     }
   }
 
-  tc_fence_before_sync();
   __syncthreads();
   cluster_sync_all();
-  if (warp == 8) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 64);
-  }
 }
 
 // =============================================================================================
@@ -1014,7 +979,6 @@ gru_fwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
   uint64_t* full = bars;
   uint64_t* accfull = bars + 1;
   uint64_t* recvbar = bars + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3);
   float* bias_s = reinterpret_cast<float*>(bars + 4);             // [48]
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int D = p.ndir * H;
@@ -1041,21 +1005,17 @@ gru_fwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
   }
   if (tid == 0) {
     mbar_init(full, 1);
-    mbar_init(accfull, 1);
+    mbar_init(accfull, 128);
     mbar_init(recvbar, 1);   // one local arrive.expect_tx per step; the peers' copies complete_tx
     mbar_fence_init();
     tma_prefetch_desc(tm);
   }
-  if (warp == 8) tmem_alloc(tmem_slot, 256);
   fence_proxy_async_smem();
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
   cluster_sync_all();
-  const uint32_t tmem_base = *tmem_slot;
   unsigned int* ctr = p.barrier + dir * 32;   // one L2 line per direction
 
-  if (warp == 9) {
+  if (warp == GRU_TMA_WARP) {
     // ===================== TMA producer: this CTA's K quarter of h_{t-1} =====================
     if (lane == 0) {
       for (int step = 1; step < T; ++step) {
@@ -1070,24 +1030,37 @@ gru_fwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
         GRU_STAMP(1);
       }
     }
-  } else if (warp == 8) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16_f32(128, NCOL);
-      for (int step = 1; step < T; ++step) {
-        mbar_wait(full, (step - 1) & 1);
-        tc_fence_after_sync();
-        for (int c = 0; c < nchunks; ++c) {
-          const uint64_t da = umma_desc_sw128_kmajor(smem_u32(ring + c * stride));
-          const uint64_t db = umma_desc_sw128_kmajor(smem_u32(wtile + c * WCHUNK));
+  } else if (warp >= GRU_MMA_WARP) {
+    // ===================== MMA warpgroup: D[Bp x (gate, 64 units)] for this K quarter ========
+    // Column gg*64 + pr*16 + u belongs to unit u of peer pr: it is written straight into
+    // stage[pr] (row pitch RW = 48, gate-major), the CTA's own columns into recv[crank].
+    const int t = tid & 127;
+    for (int step = 1; step < T; ++step) {
+      float d[NCOL / 2];   // initialised by the scale-d = 0 first MMA
+      mbar_wait(full, (step - 1) & 1);
+      wgmma_fence();
+      for (int c = 0; c < nchunks; ++c) {
+        const uint64_t da = gmma_desc_sw128_kmajor(smem_u32(ring + c * stride));
+        const uint64_t db = gmma_desc_sw128_kmajor(smem_u32(wtile + c * WCHUNK));
 #pragma unroll
-          for (int kk = 0; kk < 4; ++kk)
-            umma_bf16_ss(tmem_base, da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), idesc,
-                         (c > 0 || kk > 0) ? 1u : 0u);
-        }
-        umma_commit(accfull);
-        GRU_STAMP(2);
+        for (int kk = 0; kk < 4; ++kk)
+          wgmma_bf16<NCOL>(d, da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2),
+                           (c > 0 || kk > 0) ? 1u : 0u);
       }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(d);
+#pragma unroll
+      for (int i = 0; i < NCOL / 2; ++i) {
+        const int r = wg_frag_row(t, i), col = wg_frag_col(t, i);
+        const int gg = col >> 6, u = col & 15;
+        const uint32_t pr = (uint32_t)((col >> 4) & 3);
+        if (r < Bp)
+          (pr == crank ? recv : stage)[((size_t)pr * Bp + r) * RW + gg * GRU_HC + u] = d[i];
+      }
+      fence_proxy_async_smem();   // generic st.shared -> the bulk copies (async proxy) to the peers
+      mbar_arrive(accfull);
+      if (t == 0) GRU_STAMP(2);
     }
   } else {
     // ===================== epilogue: thread = (batch row, half of the CTA's 16 units) ==========
@@ -1120,53 +1093,23 @@ gru_fwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
       if (step > 0) {
         mbar_wait(accfull, (step - 1) & 1);
         if (tid == 0) GRU_STAMP(3);
-        tc_fence_after_sync();
-        // ---- reduce-scatter of the four partial products.  The three slices that belong to
-        // the peers go first, one at a time: TMEM -> registers -> local staging -> (named barrier)
-        // -> ONE bulk copy into the peer's receive buffer, so the first copy is in flight while
-        // the next slice is still being staged; the CTA's own slice is read last ----
-        if (tid == 0) mbar_expect_tx(recvbar, (uint32_t)((KS - 1) * Bp * RW * 4));
-#pragma unroll 1
-        for (int q = 1; q <= KS; ++q) {
-          const uint32_t pr = (crank + (uint32_t)q) % KS;      // q == KS: own slice
-          uint32_t v[3][8];
-#pragma unroll
-          for (int gg = 0; gg < 3; ++gg)
-            tmem_ld_32x32b_x8(tmem_base + ((uint32_t)((warp & 3) * 32) << 16) +
-                                  gg * (KS * GRU_HC) + pr * GRU_HC + uh * GRU_UPT, v[gg]);
-          tmem_ld_wait();
-          if (q == KS) {
-#pragma unroll
-            for (int gg = 0; gg < 3; ++gg)
-#pragma unroll
-              for (int jj = 0; jj < GRU_UPT; ++jj) acc[gg][jj] = __uint_as_float(v[gg][jj]);
-          } else {
-            if (active) {
-              float* sp = stage + ((size_t)pr * Bp + row) * RW + uh * GRU_UPT;
-#pragma unroll
-              for (int gg = 0; gg < 3; ++gg) {
-                float4* o = reinterpret_cast<float4*>(sp + gg * GRU_HC);
-                o[0] = make_float4(__uint_as_float(v[gg][0]), __uint_as_float(v[gg][1]),
-                                   __uint_as_float(v[gg][2]), __uint_as_float(v[gg][3]));
-                o[1] = make_float4(__uint_as_float(v[gg][4]), __uint_as_float(v[gg][5]),
-                                   __uint_as_float(v[gg][6]), __uint_as_float(v[gg][7]));
-              }
-            }
-            fence_proxy_async_smem();   // generic st.shared -> the copy engine's (async proxy) reads
-            epi_barrier();              // this peer's slice is completely staged
-            if (tid == 0)
-              bulk_s2peer(mapa_shared(smem_u32(recv + (size_t)crank * Bp * RW), pr),
-                          stage + (size_t)pr * Bp * RW, (uint32_t)(Bp * RW * 4),
-                          mapa_shared(smem_u32(recvbar), pr));
+        // ---- reduce-scatter of the four partial products: the MMA warpgroup staged the three
+        // slices that belong to the peers, each leaves as ONE bulk copy into the peer's receive
+        // buffer; the CTA's own slice already sits in recv[crank] ----
+        if (tid == 0) {
+          mbar_expect_tx(recvbar, (uint32_t)((KS - 1) * Bp * RW * 4));
+          for (uint32_t q = 1; q < KS; ++q) {
+            const uint32_t pr = (crank + q) % KS;
+            bulk_s2peer(mapa_shared(smem_u32(recv + (size_t)crank * Bp * RW), pr),
+                        stage + (size_t)pr * Bp * RW, (uint32_t)(Bp * RW * 4),
+                        mapa_shared(smem_u32(recvbar), pr));
           }
         }
-        tc_fence_before_sync();
         if (tid == 0) GRU_STAMP(4);
         mbar_wait(recvbar, (step - 1) & 1);
         if (active) {
 #pragma unroll
           for (int src = 0; src < KS; ++src) {
-            if ((uint32_t)src == crank) continue;
             const float* rp = recv + ((size_t)src * Bp + row) * RW + uh * GRU_UPT;
 #pragma unroll
             for (int gg = 0; gg < 3; ++gg) {
@@ -1216,13 +1159,8 @@ gru_fwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
     }
   }
 
-  tc_fence_before_sync();
   __syncthreads();
   cluster_sync_all();
-  if (warp == 8) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 256);
-  }
 }
 
 // =============================================================================================
@@ -1230,17 +1168,15 @@ gru_fwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
 //
 // Same partition as gru_fwd_ks_kernel (cluster of 4 owns 64 units, CTA r contracts K quarter r),
 // but the resident weight slice is the M-side operand and h_{t-1} the N-side one:
-//     D0[128 x Bp] = W[(r|z) x 64 units, quarter r] * h_{t-1}[:, quarter r]^T     (TMEM cols 0..)
-//     D1[ 64 x Bp] = W[ n    x 64 units, quarter r] * h_{t-1}[:, quarter r]^T     (TMEM cols 64..)
-// An MMA of N = Bp costs Bp/256 of the N = 192 one, so the tensor-core share of the step falls
-// from 16 x 96 to 32 x (Bp/8) cycles (1536 -> 1024 at 64 rows, -> 128 at 8 rows), and every
-// accumulator lane is a weight row, so all 128 lanes (all four TMEM sub-partitions) carry data
-// whatever the batch is.  The weight rows are ordered by OWNER: tile 0 rows 32q..32q+31 are the
-// r and z rows of the 16 units CTA q of the cluster owns, tile 1 rows 16q..16q+15 its n rows, so
-// an epilogue thread's accumulator row goes to exactly one peer: it is written as one row of
-// [48][Bp] (pitch Bp+4: conflict-free) into the staging slice for that peer, the three slices leave
-// as one bulk copy each, and the gate math then runs on ALL 256 epilogue threads
-// (thread = batch row x UPT units) from the four received slices.
+//     D[192 x NB] = W[(r|z|n) x 64 units, quarter r] * h_{t-1}[:, quarter r]^T
+// issued as three wgmma m64 blocks of weight rows with N = NB (the batch rounded up to 16).  The
+// batch-major form needs M >= 64 batch rows per m64 block whatever the batch is, so at 8 rows it
+// spends 8x the tensor work of this one (N = 192 on 64 mostly empty rows).  The weight rows are
+// ordered by OWNER: rows 32q..32q+31 are the r and z rows of the 16 units CTA q of the cluster
+// owns, rows 128+16q..128+16q+15 its n rows, so every accumulator row goes to exactly one peer:
+// the MMA warpgroup writes it as one row of [48][Bp] (pitch Bp+4) into the staging slice for
+// that peer, the three slices leave as one bulk copy each, and the gate math then runs on ALL 256
+// epilogue threads (thread = batch row x UPT units) from the four received slices.
 // Requires cluster size 4, H % 256 == 0, Bp <= 64 (Bp % 8 == 0 as everywhere).
 // =============================================================================================
 template <int UPT>
@@ -1272,6 +1208,92 @@ SB_DEVINL void st_bf16u(bf16* p, const float (&v)[UPT]) {
   }
 }
 
+// Owner-major staging of the transposed accumulators: slice of peer q (the own slice lives in
+// recv[crank], the others in stage[(q - crank) mod KS - 1]), row srow, column = batch row.
+SB_DEVINL float* kt_slice(float* recv, float* stage, int slice, uint32_t q, uint32_t crank) {
+  const uint32_t q0 = (q + KS - crank) % KS;
+  return q0 == 0 ? recv + (size_t)crank * slice : stage + (size_t)(q0 - 1) * slice;
+}
+
+// MMA warpgroup of gru_fwd_kt_kernel, one step per iteration: three m64 blocks of weight rows
+// (r,z of the cluster's 64 units | n of them) x NB batch rows; the scale-d = 0 first MMA
+// initialises the accumulators.
+template <int NB>
+SB_DEVINL void fwd_kt_mma(uint8_t* ring, uint8_t* wtile, float* recv, float* stage, uint64_t* full,
+                          uint64_t* accfull, int nchunks, int stride, int Bp, int P, int slice,
+                          uint32_t crank, int T) {
+  constexpr int WCHUNK = 3 * KS * GRU_HC * 128;
+  const int t = threadIdx.x & 127;
+  for (int step = 1; step < T; ++step) {
+    float d[3][NB / 2];
+    mbar_wait(full, (step - 1) & 1);
+    wgmma_fence();
+    for (int c = 0; c < nchunks; ++c) {
+      const uint32_t wa = smem_u32(wtile + c * WCHUNK);
+      const uint64_t db = gmma_desc_sw128_kmajor(smem_u32(ring + c * stride));
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
+        const uint32_t acc = (c > 0 || kk > 0) ? 1u : 0u;
+#pragma unroll
+        for (int j = 0; j < 3; ++j)
+          wgmma_bf16<NB>(d[j], gmma_desc_sw128_kmajor(wa + j * 64 * 128) + (uint64_t)(kk * 2),
+                         db + (uint64_t)(kk * 2), acc);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int j = 0; j < 3; ++j) wgmma_fence_regs(d[j]);
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+#pragma unroll
+      for (int i = 0; i < NB / 2; ++i) {
+        const int r = j * 64 + wg_frag_row(t, i), b = wg_frag_col(t, i);
+        const uint32_t q = r < 128 ? (uint32_t)(r >> 5) : (uint32_t)((r - 128) >> 4);
+        const int srow = r < 128 ? (r & 31) : 2 * GRU_HC + (r & 15);
+        if (b < Bp) kt_slice(recv, stage, slice, q, crank)[srow * P + b] = d[j][i];
+      }
+    }
+    fence_proxy_async_smem();   // generic st.shared -> the bulk copies (async proxy) to the peers
+    mbar_arrive(accfull);
+  }
+}
+
+// MMA warpgroup of gru_bwd_kt_kernel: one m64 block (the cluster's 64 units) x NB batch rows
+template <int NB>
+SB_DEVINL void bwd_kt_mma(uint8_t* ring, uint8_t* wtile, float* recv, float* stage, uint64_t* full,
+                          uint64_t* accfull, int ngroups, int gc, int stride, int Bp, int P,
+                          int slice, uint32_t crank, int T) {
+  constexpr int WCHUNK = 64 * 128;
+  const int t = threadIdx.x & 127;
+  for (int step = 0; step + 1 < T; ++step) {
+    float d[NB / 2];
+    for (int g = 0; g < ngroups; ++g) {
+      mbar_wait(&full[g], step & 1);
+      wgmma_fence();
+      for (int i = 0; i < gc; ++i) {
+        const int c = g * gc + i;
+        const uint64_t da = gmma_desc_sw128_kmajor(smem_u32(wtile + c * WCHUNK));
+        const uint64_t db = gmma_desc_sw128_kmajor(smem_u32(ring + c * stride));
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk)
+          wgmma_bf16<NB>(d, da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2),
+                         (c > 0 || kk > 0) ? 1u : 0u);
+      }
+      wgmma_commit();
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(d);
+#pragma unroll
+    for (int i = 0; i < NB / 2; ++i) {
+      const int r = wg_frag_row(t, i), b = wg_frag_col(t, i);
+      if (b < Bp) kt_slice(recv, stage, slice, (uint32_t)(r >> 4), crank)[(r & 15) * P + b] = d[i];
+    }
+    fence_proxy_async_smem();
+    mbar_arrive(accfull);
+  }
+}
+
 template <int UPT>
 __global__ void __launch_bounds__(GRU_THREADS, 1)
 gru_fwd_kt_kernel(const __grid_constant__ CUtensorMap tm_d0,
@@ -1296,9 +1318,8 @@ gru_fwd_kt_kernel(const __grid_constant__ CUtensorMap tm_d0,
   const int ring_bytes = nchunks * stride;            // the whole quarter is resident
   const int wbytes = nchunks * WCHUNK;
   // carve: ring | weights | recv | stage | barriers.  The N-side read of the last chunk may run
-  // up to 8 rows past the ring into the weights, and the 128-row M-side read of tile 1 runs 64
-  // rows past its 64 valid ones (into the next chunk / the receive buffer): both only feed
-  // accumulator columns / lanes that are never read.
+  // up to 8 rows past the ring into the weights: it only feeds accumulator columns >= Bp, which
+  // are never stored.
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint8_t* ring = base;
@@ -1309,7 +1330,6 @@ gru_fwd_kt_kernel(const __grid_constant__ CUtensorMap tm_d0,
   uint64_t* full = bars;
   uint64_t* accfull = bars + 1;
   uint64_t* recvbar = bars + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3);
   float* bias_s = reinterpret_cast<float*>(bars + 4);             // [48]
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int D = p.ndir * H;
@@ -1338,21 +1358,17 @@ gru_fwd_kt_kernel(const __grid_constant__ CUtensorMap tm_d0,
   }
   if (tid == 0) {
     mbar_init(full, 1);
-    mbar_init(accfull, 1);
+    mbar_init(accfull, 128);
     mbar_init(recvbar, 1);   // one local arrive.expect_tx per step; the peers' copies complete_tx
     mbar_fence_init();
     tma_prefetch_desc(tm);
   }
-  if (warp == 8) tmem_alloc(tmem_slot, 128);
   fence_proxy_async_smem();
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
   cluster_sync_all();
-  const uint32_t tmem_base = *tmem_slot;
   unsigned int* ctr = p.barrier + dir * 32;   // one L2 line per direction
 
-  if (warp == 9) {
+  if (warp == GRU_TMA_WARP) {
     // ===================== TMA producer: this CTA's K quarter of h_{t-1} =====================
     if (lane == 0) {
       for (int step = 1; step < T; ++step) {
@@ -1367,43 +1383,16 @@ gru_fwd_kt_kernel(const __grid_constant__ CUtensorMap tm_d0,
         GRU_STAMP(1);
       }
     }
-  } else if (warp == 8) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      const uint32_t idesc = umma_idesc_bf16_f32(128, (uint32_t)NB);
-      for (int step = 1; step < T; ++step) {
-        mbar_wait(full, (step - 1) & 1);
-        tc_fence_after_sync();
-        for (int c = 0; c < nchunks; ++c) {
-          const uint64_t da0 = umma_desc_sw128_kmajor(smem_u32(wtile + c * WCHUNK));
-          const uint64_t da1 = umma_desc_sw128_kmajor(smem_u32(wtile + c * WCHUNK + 128 * 128));
-          const uint64_t db = umma_desc_sw128_kmajor(smem_u32(ring + c * stride));
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) {
-            const uint32_t acc = (c > 0 || kk > 0) ? 1u : 0u;
-            umma_bf16_ss(tmem_base, da0 + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), idesc, acc);
-            umma_bf16_ss(tmem_base + 64, da1 + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), idesc,
-                         acc);
-          }
-        }
-        umma_commit(accfull);
-        GRU_STAMP(2);
-      }
+  } else if (warp >= GRU_MMA_WARP) {
+    // ===================== MMA warpgroup =====================
+    switch (NB) {
+      case 16: fwd_kt_mma<16>(ring, wtile, recv, stage, full, accfull, nchunks, stride, Bp, P, slice, crank, T); break;
+      case 32: fwd_kt_mma<32>(ring, wtile, recv, stage, full, accfull, nchunks, stride, Bp, P, slice, crank, T); break;
+      case 48: fwd_kt_mma<48>(ring, wtile, recv, stage, full, accfull, nchunks, stride, Bp, P, slice, crank, T); break;
+      default: fwd_kt_mma<64>(ring, wtile, recv, stage, full, accfull, nchunks, stride, Bp, P, slice, crank, T); break;
     }
   } else {
     // ===================== epilogue =====================
-    // phase A (scatter): warp w reads accumulator lanes 32*(w&3).. of tile 0 and, for w&3 < 2,
-    // of tile 1, for the column blocks (8 batch rows each) of its half (w>>2) of the batch
-    const int sub = warp & 3, hi = warp >> 2;
-    const int nblk = Bp >> 3;
-    const int blk0 = hi == 0 ? 0 : (nblk + 1) / 2;
-    const int myblk = hi == 0 ? (nblk + 1) / 2 : nblk / 2;          // <= 4
-    const uint32_t own0 = (uint32_t)sub;                            // owner of the tile-0 row
-    const uint32_t own1 = (uint32_t)(sub * 2 + (lane >> 4));        // owner of the tile-1 row
-    const uint32_t q0 = (own0 + KS - crank) % KS, q1 = (own1 + KS - crank) % KS;
-    float* dst0 = (q0 == 0 ? recv + crank * slice : stage + (q0 - 1) * slice) + lane * P;
-    float* dst1 = (q1 == 0 ? recv + crank * slice : stage + (q1 - 1) * slice) +
-                  (2 * GRU_HC + (lane & 15)) * P;
     // phase B (gate math): thread = (batch row b, UPT of the CTA's 16 units)
     const int b = tid % Bp, ug = tid / Bp;
     const bool active = ug * UPT < GRU_HC;
@@ -1434,45 +1423,8 @@ gru_fwd_kt_kernel(const __grid_constant__ CUtensorMap tm_d0,
       if (step > 0) {
         mbar_wait(accfull, (step - 1) & 1);
         if (tid == 0) GRU_STAMP(3);
-        tc_fence_after_sync();
+        // the MMA warpgroup staged the three outgoing slices (and the own one in recv[crank])
         if (tid == 0) mbar_expect_tx(recvbar, (uint32_t)((KS - 1) * slice * 4));
-        {
-          const uint32_t tl = tmem_base + ((uint32_t)(sub * 32) << 16) + (uint32_t)(blk0 * 8);
-#pragma unroll
-          for (int kb = 0; kb < 4; kb += 2) {
-            if (kb < myblk) {
-              uint32_t v0[2][8], v1[2][8];
-#pragma unroll
-              for (int k = 0; k < 2; ++k) {
-                if (kb + k < myblk) {
-                  tmem_ld_32x32b_x8(tl + (kb + k) * 8, v0[k]);
-                  if (sub < 2) tmem_ld_32x32b_x8(tl + 64 + (kb + k) * 8, v1[k]);
-                }
-              }
-              tmem_ld_wait();
-#pragma unroll
-              for (int k = 0; k < 2; ++k) {
-                if (kb + k < myblk) {
-                  float4* o = reinterpret_cast<float4*>(dst0 + (blk0 + kb + k) * 8);
-                  o[0] = make_float4(__uint_as_float(v0[k][0]), __uint_as_float(v0[k][1]),
-                                     __uint_as_float(v0[k][2]), __uint_as_float(v0[k][3]));
-                  o[1] = make_float4(__uint_as_float(v0[k][4]), __uint_as_float(v0[k][5]),
-                                     __uint_as_float(v0[k][6]), __uint_as_float(v0[k][7]));
-                  if (sub < 2) {
-                    float4* o1 = reinterpret_cast<float4*>(dst1 + (blk0 + kb + k) * 8);
-                    o1[0] = make_float4(__uint_as_float(v1[k][0]), __uint_as_float(v1[k][1]),
-                                        __uint_as_float(v1[k][2]), __uint_as_float(v1[k][3]));
-                    o1[1] = make_float4(__uint_as_float(v1[k][4]), __uint_as_float(v1[k][5]),
-                                        __uint_as_float(v1[k][6]), __uint_as_float(v1[k][7]));
-                  }
-                }
-              }
-            }
-          }
-        }
-        tc_fence_before_sync();
-        fence_proxy_async_smem();   // generic st.shared -> the copy engine's (async proxy) reads
-        epi_barrier();              // all three outgoing slices (and the own one) are staged
         if (lane == 0 && warp >= 1 && warp <= KS - 1) {
           const uint32_t pr = (crank + (uint32_t)warp) % KS;
           bulk_s2peer(mapa_shared(smem_u32(recv + (size_t)crank * slice), pr),
@@ -1530,21 +1482,16 @@ gru_fwd_kt_kernel(const __grid_constant__ CUtensorMap tm_d0,
     }
   }
 
-  tc_fence_before_sync();
   __syncthreads();
   cluster_sync_all();
-  if (warp == 8) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 128);
-  }
 }
 
 // =============================================================================================
 // backward, K split with the accumulator TRANSPOSED (see gru_fwd_kt_kernel):
 //     D^T[64 units x Bp] = W_hh^T[64 units of the cluster, quarter r of 3H] * dgh[:, quarter r]^T
-// The weight tile is the one of gru_bwd_ks_kernel (its 64 rows are already grouped by owner:
-// rows 16q..16q+15 belong to CTA q of the cluster); an accumulator lane is a unit, so its row
-// of Bp partial sums goes to exactly one peer, and the elementwise work runs on all 256
+// issued as one wgmma m64 block of weight rows with N = NB.  The weight tile is the one of
+// gru_bwd_ks_kernel (its 64 rows are already grouped by owner: rows 16q..16q+15 belong to CTA q
+// of the cluster); an accumulator row is a unit, so its Bp partial sums go to exactly one peer, and the elementwise work runs on all 256
 // epilogue threads (thread = batch row x UPT units).
 // =============================================================================================
 template <int UPT>
@@ -1580,30 +1527,24 @@ gru_bwd_kt_kernel(const __grid_constant__ CUtensorMap tm_d0,
   const int stride = Bp * 128;
   const int ring_bytes = nchunks * stride;            // the whole quarter is resident
   const int wbytes = nchunks * WCHUNK;
-  // carve: ring | weights | recv | stage | barriers.  The 128-row M-side read covers the next
-  // weight chunk (last chunk: the receive buffer) with its lanes 64..127, which are never read.
+  // carve: ring | weights | recv | stage | barriers
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint8_t* ring = base;
   uint8_t* wtile = ring + ring_bytes;
   float* recv = reinterpret_cast<float*>(wtile + wbytes);          // [KS src][16][P]
   float* stage = recv + KS * slice;                                // [KS-1 dst][16][P]
-  float* pad_end = stage + (KS - 1) * slice;
-  // the last chunk's 128-row read needs 8 KB after the weights: recv + stage cover it only for
-  // large batches, so reserve it explicitly
-  const int tail_floats = max(0, 2048 - (2 * KS - 1) * slice);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(pad_end + tail_floats);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(stage + (KS - 1) * slice);
   uint64_t* full = bars;          // [4] groups
   uint64_t* accfull = bars + 4;
   uint64_t* recvbar = bars + 5;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 6);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int D = p.ndir * H;
   const CUtensorMap* tm = dir == 0 ? &tm_d0 : &tm_d1;
   const int gc = (nchunks % 4 == 0) ? 4 : ((nchunks % 3 == 0) ? 3 : ((nchunks % 2 == 0) ? 2 : 1));
   const int ngroups = nchunks / gc;                   // <= 4 for H <= 1024 ... checked on host
 
-  for (int k = tid; k < (ring_bytes + wbytes + ((2 * KS - 1) * slice + tail_floats) * 4) / 16;
+  for (int k = tid; k < (ring_bytes + wbytes + (2 * KS - 1) * slice * 4) / 16;
        k += GRU_THREADS)
     reinterpret_cast<uint4*>(base)[k] = make_uint4(0, 0, 0, 0);
   __syncthreads();
@@ -1623,21 +1564,17 @@ gru_bwd_kt_kernel(const __grid_constant__ CUtensorMap tm_d0,
   }
   if (tid == 0) {
     for (int i = 0; i < 4; ++i) mbar_init(&full[i], 1);
-    mbar_init(accfull, 1);
+    mbar_init(accfull, 128);
     mbar_init(recvbar, 1);
     mbar_fence_init();
     tma_prefetch_desc(tm);
   }
-  if (warp == 8) tmem_alloc(tmem_slot, 64);
   fence_proxy_async_smem();
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
   cluster_sync_all();
-  const uint32_t tmem_base = *tmem_slot;
   unsigned int* ctr = p.barrier + dir * 32;   // one L2 line per direction
 
-  if (warp == 9) {
+  if (warp == GRU_TMA_WARP) {
     if (lane == 0) {
       for (int step = 0; step + 1 < T; ++step) {
         grid_wait(ctr, (unsigned int)nC * (step + 1), p.ablate & 192);   // dgh of this step is complete
@@ -1653,36 +1590,14 @@ gru_bwd_kt_kernel(const __grid_constant__ CUtensorMap tm_d0,
         GRU_STAMP(1);
       }
     }
-  } else if (warp == 8) {
-    if (lane == 0) {
-      const uint32_t idesc = umma_idesc_bf16_f32(128, (uint32_t)NB);
-      for (int step = 0; step + 1 < T; ++step) {
-        for (int g = 0; g < ngroups; ++g) {
-          mbar_wait(&full[g], step & 1);
-          tc_fence_after_sync();
-          for (int i = 0; i < gc; ++i) {
-            const int c = g * gc + i;
-            const uint64_t da = umma_desc_sw128_kmajor(smem_u32(wtile + c * WCHUNK));
-            const uint64_t db = umma_desc_sw128_kmajor(smem_u32(ring + c * stride));
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk)
-              umma_bf16_ss(tmem_base, da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), idesc,
-                           (c > 0 || kk > 0) ? 1u : 0u);
-          }
-        }
-        umma_commit(accfull);
-        GRU_STAMP(2);
-      }
+  } else if (warp >= GRU_MMA_WARP) {
+    switch (NB) {
+      case 16: bwd_kt_mma<16>(ring, wtile, recv, stage, full, accfull, ngroups, gc, stride, Bp, P, slice, crank, T); break;
+      case 32: bwd_kt_mma<32>(ring, wtile, recv, stage, full, accfull, ngroups, gc, stride, Bp, P, slice, crank, T); break;
+      case 48: bwd_kt_mma<48>(ring, wtile, recv, stage, full, accfull, ngroups, gc, stride, Bp, P, slice, crank, T); break;
+      default: bwd_kt_mma<64>(ring, wtile, recv, stage, full, accfull, ngroups, gc, stride, Bp, P, slice, crank, T); break;
     }
   } else {
-    // phase A (scatter): warps with (w&3) < 2 hold the 64 valid accumulator lanes
-    const int sub = warp & 3, hi = warp >> 2;
-    const int nblk = Bp >> 3;
-    const int blk0 = hi == 0 ? 0 : (nblk + 1) / 2;
-    const int myblk = hi == 0 ? (nblk + 1) / 2 : nblk / 2;          // <= 4
-    const uint32_t own = (uint32_t)(sub * 2 + (lane >> 4));
-    const uint32_t q0 = (own + KS - crank) % KS;
-    float* dst0 = (q0 == 0 ? recv + crank * slice : stage + (q0 - 1) * slice) + (lane & 15) * P;
     // phase B: thread = (batch row b, UPT of the CTA's 16 units)
     const int b = tid % Bp, ug = tid / Bp;
     const bool active = ug * UPT < GRU_HC;
@@ -1719,29 +1634,8 @@ gru_bwd_kt_kernel(const __grid_constant__ CUtensorMap tm_d0,
       if (step > 0) {
         mbar_wait(accfull, (step - 1) & 1);
         if (tid == 0) GRU_STAMP(3);
-        tc_fence_after_sync();
+        // the MMA warpgroup staged the three outgoing slices (and the own one in recv[crank])
         if (tid == 0) mbar_expect_tx(recvbar, (uint32_t)((KS - 1) * slice * 4));
-        if (sub < 2) {
-          const uint32_t tl = tmem_base + ((uint32_t)(sub * 32) << 16) + (uint32_t)(blk0 * 8);
-          uint32_t v[4][8];
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            if (k < myblk) tmem_ld_32x32b_x8(tl + k * 8, v[k]);
-          tmem_ld_wait();
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            if (k < myblk) {
-              float4* o = reinterpret_cast<float4*>(dst0 + (blk0 + k) * 8);
-              o[0] = make_float4(__uint_as_float(v[k][0]), __uint_as_float(v[k][1]),
-                                 __uint_as_float(v[k][2]), __uint_as_float(v[k][3]));
-              o[1] = make_float4(__uint_as_float(v[k][4]), __uint_as_float(v[k][5]),
-                                 __uint_as_float(v[k][6]), __uint_as_float(v[k][7]));
-            }
-          }
-        }
-        tc_fence_before_sync();
-        fence_proxy_async_smem();
-        epi_barrier();
         if (lane == 0 && warp >= 1 && warp <= KS - 1) {
           const uint32_t pr = (crank + (uint32_t)warp) % KS;
           bulk_s2peer(mapa_shared(smem_u32(recv + (size_t)crank * slice), pr),
@@ -1815,27 +1709,25 @@ gru_bwd_kt_kernel(const __grid_constant__ CUtensorMap tm_d0,
     }
   }
 
-  tc_fence_before_sync();
   __syncthreads();
   cluster_sync_all();
-  if (warp == 8) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 64);
-  }
 }
 
 int make_tmap_bf16_2d(CUtensorMap* map, const void* base, long long rows, long long cols,
                       long long ld, int box_rows);
 
 // chunks are grouped gc per mbarrier pair (gc = largest of 4,3,2,1 dividing nchunks); ring = the
-// largest divisor of ngroups (<= GRU_MAX_RING) whose slots fit next to the resident weights
-static int gru_ring_slots(int wbytes, int Bp, int nchunks, int* gc_out, size_t* smem_bytes) {
+// largest divisor of ngroups (<= GRU_MAX_RING) whose slots fit next to the resident weights and
+// the parked recurrent product of `acc_cols` columns
+static int gru_ring_slots(int wbytes, int Bp, int nchunks, int acc_cols, int* gc_out,
+                          size_t* smem_bytes) {
   int gc = 1;
   for (int g = 4; g >= 1; --g)
     if (nchunks % g == 0) { gc = g; break; }
   const int ngroups = nchunks / gc;
   const int slot = gc * Bp * 128;
-  const int fixed = wbytes + 1024 /*align*/ + (2 * GRU_MAX_RING + 2) * 8 + 256 /*scratch*/ + 64;
+  const int fixed = wbytes + 1024 /*align*/ + (2 * GRU_MAX_RING + 2) * 8 + 256 /*scratch*/ + 64 +
+                    Bp * (acc_cols + 4) * 4;
   int fit = (227 * 1024 - fixed) / slot;
   if (fit > GRU_MAX_RING) fit = GRU_MAX_RING;
   int ring = -1;
@@ -1912,14 +1804,17 @@ static unsigned long long* g_gru_dbg = nullptr;
 static int g_gru_ablate = 0;
 static int g_gru_ksplit = 1;   // developer knob: 0 disables the K-split backward kernel
 
-// Which K-split flavour: the transposed-accumulator kernels (gru_*_kt_kernel) win while the batch
-// is small.  Measured us/step at H = 1024 (kt | ks): forward 3.8 | 4.8 at 8 rows, 4.3 | 4.9 at 16,
-// 5.3 | 5.4 at 32, 7.9 | 7.1 at 64; backward 4.6 | 5.3 at 8, 5.4 | 5.4 at 16, 6.2 | 5.8 at 32,
-// 8.3 | 7.8 at 64.  Developer knob (sb_debug_gru_flags): 16 forces them, 8 disables them.
+// Which K-split flavour: the transposed-accumulator kernels (gru_*_kt_kernel) spend tensor work
+// in proportion to the batch (N = batch) instead of a whole m64 block of batch rows.  Measured on
+// an H100 80GB HBM3 (400 W power limit), one biGRU-1024 layer at T = 247 including its projection
+// GEMMs, ms (kt | ks): forward 2.12 | 2.14 at 8 rows, 2.10 | 2.46 at 16, 2.66 | 2.50 at 32,
+// 4.40 | 4.37 at 64; backward 3.03 | 2.98 at 8, 3.18 | 3.24 at 16, 6.24 | 6.23 at 32,
+// 8.30 | 7.88 at 64.  So kt runs the forward recurrence up to 16 rows; the backward stays on ks.
+// Developer knob (sb_debug_gru_flags): 16 forces them, 8 disables them.
 static bool gru_use_kt(int Bp, bool backward) {
   if (g_gru_ablate & 8) return false;
   if (g_gru_ablate & 16) return true;
-  return Bp <= (backward ? 8 : 32);
+  return !backward && Bp <= 16;
 }
 
 // cooperative launch with EXACTLY the given cluster size; fails if the grid is not co-resident
@@ -2030,7 +1925,7 @@ extern "C" int sb_gru_fwd(const float* gi, const void* whh_bf16, const float* bh
   int gc = 1;
   size_t smem = 0;
   const int ring =
-      gru_ring_slots(std::max(nchunks * 48 * 128, 16384 - Bp * 128), Bp, nchunks, &gc, &smem);
+      gru_ring_slots(std::max(nchunks * 48 * 128, 16384 - Bp * 128), Bp, nchunks, 48, &gc, &smem);
   if (ring < 0) return SB_ERR_UNSUPPORTED;
 
   // ---- preferred: K-split over 4-CTA clusters (H % 256 == 0, batch rows <= 64) ----
@@ -2140,10 +2035,9 @@ extern "C" int sb_gru_bwd(const float* dy, const float* y, const float* gates,
       }
       p.ring = nq; p.gc = 1;
       void* kargs[] = {(void*)&tq[0], (void*)&tq[1], (void*)&p};
-      const size_t ex = (size_t)(2 * KS - 1) * GRU_HC * (Bp + 4) * 4;
       const size_t kt_smem = (size_t)nq * Bp * 128 + (size_t)nq * 64 * 128 +
-                             std::max(ex, (size_t)8192) + 1024 + 256;
-      if (gru_use_kt(Bp, true) && kt_smem <= 227 * 1024) {
+                             (size_t)(2 * KS - 1) * GRU_HC * (Bp + 4) * 4 + 1024 + 256;
+      if (gru_use_kt(Bp, true) && Bp <= 64 && kt_smem <= 227 * 1024) {
         const void* kt = Bp > 32   ? (const void*)gru_bwd_kt_kernel<4>
                          : Bp > 16 ? (const void*)gru_bwd_kt_kernel<2>
                                    : (const void*)gru_bwd_kt_kernel<1>;
@@ -2154,7 +2048,8 @@ extern "C" int sb_gru_bwd(const float* dy, const float* y, const float* gates,
       if (rc == SB_OK) return SB_OK;
     }
   }
-  p.ring = gru_ring_slots(std::max(nchunks * 16 * 128, 16384 - Bp * 128), Bp, nchunks, &p.gc, &smem);
+  p.ring = gru_ring_slots(std::max(nchunks * 16 * 128, 16384 - Bp * 128), Bp, nchunks, 16, &p.gc,
+                          &smem);
   if (p.ring < 0) return SB_ERR_UNSUPPORTED;
   // per direction: the two parity buffers stacked as [2*Bp rows][3H cols]
   CUtensorMap tm[2];

@@ -9,12 +9,13 @@
 // lat[node] = {log p(blank), log p(label_u)} (8 bytes per node) and the hidden tensor only ever
 // exists as 16 KB operand tiles in shared memory:
 //   * 3 x 4 producer warps (thread = node row; the groups take the k-blocks in turn) build
-//     A tiles [128 nodes x 64] bf16 of relu(fx[b,t,:] + fy[b,u,:]) straight into the UMMA
+//     A tiles [128 nodes x 64] bf16 of relu(fx[b,t,:] + fy[b,u,:]) straight into the wgmma
 //     K-major SWIZZLE_128B layout (fx, fy: fp32 outputs of the fc1 GEMMs, L2 resident: 7.9 K
 //     and 3.2 K rows);
 //   * fc2's weight (V+1 <= 64 rows x H, bf16) stays resident in shared memory;
-//   * one thread issues tcgen05.mma  D[128 x NV] += A * W2^T  (accumulators in TMEM, 2 stages);
-//   * 4 epilogue warps (thread = node) add the bias, take the log-softmax over the V+1 classes
+//   * one consumer warpgroup issues wgmma  D[128 x NV] += A * W2^T  (two m64 halves, fp32
+//     accumulators in registers), parks the tile in shared memory and re-reads it as thread = node;
+//   * the same 4 warps (thread = node) add the bias, take the log-softmax over the V+1 classes
 //     in registers and write either the compact lattice (+ optionally the full log-probabilities,
 //     which `infer` needs for the beam search), or - in the backward recompute pass - the
 //     gradient w.r.t. the logits as bf16 rows [node][NV] from the per-arc gradients of the
@@ -31,13 +32,16 @@ namespace sb {
 
 typedef __nv_bfloat16 bf16;
 
-static constexpr int JT_STAGES = 6;
 // producer groups of 4 warps: 3 for the 32-class kernel, 2 for the 64-class one (whose epilogue
-// keeps 2 x 64 values per thread and would spill under the register cap of 17 warps)
+// keeps 2 x 64 values per thread and would spill under the register cap of 16 warps).  The
+// 64-class kernel keeps 4 ring stages so that fc2's weight (128 KB at H = 1024), the ring and the
+// accumulator tile fit in the 227 KB of shared memory of one block.
 template <int NV> struct JtCfg {
   static constexpr int kGroups = NV <= 32 ? 3 : 2;
   static constexpr int kPW = 4 * kGroups;              // producer warps
-  static constexpr int kThreads = 32 * (kPW + 5);      // producers | MMA warp | 4 epilogue warps
+  static constexpr int kThreads = 32 * (kPW + 4);      // producers | consumer warpgroup
+  static constexpr int kStages = NV <= 32 ? 6 : 4;
+  static constexpr int kAccPitch = NV + 1;             // floats per node row of the parked tile
 };
 
 struct JointParams {
@@ -58,6 +62,7 @@ struct JointParams {
 template <int NV>
 __global__ void __launch_bounds__(JtCfg<NV>::kThreads, 1) joint_kernel(const JointParams p) {
   constexpr int JT_GROUPS = JtCfg<NV>::kGroups, JT_PW = JtCfg<NV>::kPW, JT_THREADS = JtCfg<NV>::kThreads;
+  constexpr int JT_STAGES = JtCfg<NV>::kStages, ACC_LD = JtCfg<NV>::kAccPitch;
   extern __shared__ uint8_t smem_raw[];
   const int H = p.H;
   const int nkb = (H + 63) / 64;
@@ -67,17 +72,15 @@ __global__ void __launch_bounds__(JtCfg<NV>::kThreads, 1) joint_kernel(const Joi
                                              ~static_cast<uintptr_t>(1023));
   uint8_t* a_ring = base;
   uint8_t* wtile = a_ring + JT_STAGES * A_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(wtile + (size_t)nkb * WCHUNK);
+  float* acc_s = reinterpret_cast<float*>(wtile + (size_t)nkb * WCHUNK);   // [128][ACC_LD]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(acc_s + 128 * ACC_LD + 2);
   uint64_t* full = bars;                    // [JT_STAGES]  4 producer-warp arrivals
-  uint64_t* empty = bars + JT_STAGES;       // [JT_STAGES]
-  uint64_t* tfull = bars + 2 * JT_STAGES;   // [2]
-  uint64_t* tempty = tfull + 2;             // [2]          4 epilogue-warp arrivals
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
-  float* bias_s = reinterpret_cast<float*>(tmem_slot + 2);   // [NV]
+  uint64_t* empty = bars + JT_STAGES;       // [JT_STAGES]  1 consumer arrival
+  float* bias_s = reinterpret_cast<float*>(empty + JT_STAGES);   // [NV]
   float* db_s = bias_s + NV;                                  // [NV]
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
-  // ---- one-time: fc2 weight -> shared memory (UMMA K-major SWIZZLE_128B chunks), bias ----
+  // ---- one-time: fc2 weight -> shared memory (wgmma K-major SWIZZLE_128B chunks), bias ----
   for (int k = tid; k < nkb * WCHUNK / 16; k += JT_THREADS)
     reinterpret_cast<uint4*>(wtile)[k] = make_uint4(0, 0, 0, 0);
   __syncthreads();
@@ -100,18 +103,10 @@ __global__ void __launch_bounds__(JtCfg<NV>::kThreads, 1) joint_kernel(const Joi
       mbar_init(&full[s], 4);
       mbar_init(&empty[s], 1);
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull[s], 1);
-      mbar_init(&tempty[s], 4);
-    }
     mbar_fence_init();
   }
-  if (warp == JT_PW) tmem_alloc(tmem_slot, 2 * NV < 32 ? 32 : 2 * NV);
   fence_proxy_async_smem();
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
   const long long ntiles = (p.nodes + 127) / 128;
 
   if (warp < JT_PW) {
@@ -157,64 +152,57 @@ __global__ void __launch_bounds__(JtCfg<NV>::kThreads, 1) joint_kernel(const Joi
           }
           *reinterpret_cast<uint4*>(a + sw128_offset((uint32_t)rowt, (uint32_t)c16)) = o;
         }
-        fence_proxy_async_smem();     // generic st.shared -> tcgen05.mma (async proxy)
+        fence_proxy_async_smem();     // generic st.shared -> wgmma (async proxy)
         __syncwarp();
         if (lane == 0) mbar_arrive(&full[stage]);
       }
     }
-  } else if (warp == JT_PW) {
-    // ===================== MMA issuer =====================
-    constexpr uint32_t idesc = umma_idesc_bf16_f32(128, NV);
-    int stage = 0, acc = 0;
-    uint32_t phase = 0, acc_phase = 0;
-    for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-      if (lane == 0) {
-        mbar_wait(&tempty[acc], acc_phase ^ 1);
-        tc_fence_after_sync();
-        for (int kb = 0; kb < nkb; ++kb) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after_sync();
-          const uint64_t da = umma_desc_sw128_kmajor(smem_u32(a_ring + stage * A_BYTES));
-          const uint64_t db = umma_desc_sw128_kmajor(smem_u32(wtile + kb * WCHUNK));
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk)
-            umma_bf16_ss(tmem_base + acc * NV, da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2),
-                         idesc, (kb > 0 || kk > 0) ? 1u : 0u);
-          umma_commit(&empty[stage]);
-          if (kb == nkb - 1) umma_commit(&tfull[acc]);
-          if (++stage == JT_STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-      __syncwarp();
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
   } else {
-    // ===================== epilogue: thread = node =====================
-    const int sub = warp & 3;                  // TMEM sub-partition of this warp (warps 9..12)
-    const int row = sub * 32 + lane;
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    // ===================== consumer warpgroup: wgmma, then thread = node =====================
+    const int row = tid - 32 * JT_PW;          // 0..127
+    int stage = 0;
+    uint32_t phase = 0;
     float dbacc[NV];
 #pragma unroll
     for (int j = 0; j < NV; ++j) dbacc[j] = 0.f;
     for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
       const long long n = tile * 128 + row;
       const bool ok = n < p.nodes;
-      mbar_wait(&tfull[acc], acc_phase);
-      tc_fence_after_sync();
+      float d0[NV / 2], d1[NV / 2];            // node rows 0..63 | 64..127 of the tile
+#pragma unroll
+      for (int j = 0; j < NV / 2; ++j) { d0[j] = 0.f; d1[j] = 0.f; }
+      int prev = -1;
+      for (int kb = 0; kb < nkb; ++kb) {
+        mbar_wait(&full[stage], phase);
+        const uint32_t sa = smem_u32(a_ring + stage * A_BYTES);
+        const uint64_t da0 = gmma_desc_sw128_kmajor(sa);
+        const uint64_t da1 = gmma_desc_sw128_kmajor(sa + 64 * 128);
+        const uint64_t db = gmma_desc_sw128_kmajor(smem_u32(wtile + kb * WCHUNK));
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+          const uint32_t accum = (kb > 0 || kk > 0) ? 1u : 0u;
+          wgmma_bf16<NV>(d0, da0 + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), accum);
+          wgmma_bf16<NV>(d1, da1 + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), accum);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                       // the previous k-block's group has retired
+        if (prev >= 0 && row == 0) mbar_arrive(&empty[prev]);
+        prev = stage;
+        if (++stage == JT_STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(d0);
+      wgmma_fence_regs(d1);
+      if (prev >= 0 && row == 0) mbar_arrive(&empty[prev]);
+      // fragment layout -> thread = node row
+      wg_store_rows<NV>(d0, acc_s, ACC_LD, 0, 128);
+      wg_store_rows<NV>(d1, acc_s, ACC_LD, 64, 128);
+      asm volatile("bar.sync 1, 128;" ::: "memory");
       float v[NV];
 #pragma unroll
-      for (int c = 0; c < NV / 32; ++c) {
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(sub * 32) << 16) + acc * NV + c * 32, r);
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[c * 32 + j] = __uint_as_float(r[j]);
-      }
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[acc]);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+      for (int j = 0; j < NV; ++j) v[j] = acc_s[row * ACC_LD + j];
+      asm volatile("bar.sync 1, 128;" ::: "memory");   // the next tile may overwrite acc_s
       if (!ok) continue;
       float mx = -INFINITY;
 #pragma unroll
@@ -276,13 +264,8 @@ __global__ void __launch_bounds__(JtCfg<NV>::kThreads, 1) joint_kernel(const Joi
     }
   }
 
-  tc_fence_before_sync();
   __syncthreads();
   if (p.mode == 1 && tid < p.V1) atomicAdd(p.db2 + tid, db_s[tid]);
-  if (warp == JT_PW) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 2 * NV < 32 ? 32 : 2 * NV);
-  }
 }
 
 // ---- slab kernels of the backward pass -------------------------------------------------------
@@ -388,7 +371,10 @@ static int joint_launch(JointParams& p, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   const int nv = p.V1 <= 32 ? 32 : 64;
   const int nkb = (p.H + 63) / 64;
-  const size_t smem = (size_t)JT_STAGES * 128 * 128 + (size_t)nkb * nv * 128 + 1024 + 256 + 8 * nv;
+  const int stages = nv == 32 ? JtCfg<32>::kStages : JtCfg<64>::kStages;
+  // ring | fc2 weight | parked accumulator tile | barriers, bias, bias gradient
+  const size_t smem = (size_t)stages * 128 * 128 + (size_t)nkb * nv * 128 +
+                      (size_t)128 * (nv + 1) * 4 + 8 + 1024 + 16 * stages + 8 * nv;
   if (smem > 227 * 1024) return SB_ERR_UNSUPPORTED;
   const long long ntiles = (p.nodes + 127) / 128;
   int grid = device_sm_count();

@@ -27,7 +27,7 @@
 //   s2s_cell_bwd      d ix = d gi W_ih, d hx_{u-1} = d gh W_hh + z * d hx_u on transposed weights.
 // The output-projection backward (d o = dlogits W_fc) of ALL steps is one launch before the loop
 // (s2s_dout); the weight gradients of the cell, the embedding and fc are time-batched contractions
-// over all (u, b) rows and run once per sequence on the tcgen05 GEMM (SB_GEMM_A_MN | SB_GEMM_B_MN).
+// over all (u, b) rows and run once per sequence on the wgmma GEMM (SB_GEMM_A_MN | SB_GEMM_B_MN).
 // Everything is fp32 (the reference's arithmetic); roofline: L2 bandwidth on eh and the cell
 // weights per token (B*T*H*4 bytes forward, 3x that backward, + 24 H^2), in practice launch-bound.
 #include "common.cuh"

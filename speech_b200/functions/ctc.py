@@ -20,7 +20,7 @@ from .. import _lib
 
 
 def ctc_costs_and_grads(acts, labels, act_lens, label_lens, blank=None, need_grad=True):
-    """Run the fused sm_100a CTC kernel.  Returns (costs (B,), grads (B,T,V) or None)."""
+    """Run the fused sm_90a CTC kernel.  Returns (costs (B,), grads (B,T,V) or None)."""
     _lib.require_cuda(acts, "acts")
     lib = _lib.load()
     if acts.dtype != torch.float32:

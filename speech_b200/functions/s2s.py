@@ -2,7 +2,7 @@
 Seq2Seq.decode / decode_step / infer / beam_search (speech/models/seq2seq.py:78-227) and
 NNAttention.forward (:344-360) as two kernels per token (GRU cell; attention + output projection),
 with a hand-written backward (three kernels per token, the output-projection backward of all
-steps in one launch, the weight gradients time-batched on the tcgen05 GEMM), a greedy loop and a
+steps in one launch, the weight gradients time-batched on the wgmma GEMM), a greedy loop and a
 beam search that never leave the device: the host only enqueues kernels and reads the final
 hypothesis back once.
 """
@@ -195,7 +195,7 @@ class DecodeFunction(torch.autograd.Function):
             ops._launch("s2s_cell_bwd", 0.0, lambda: lib.sb_s2s_cell_bwd(
                 p_dgi + 3 * u * BH, p_dgh + 3 * u * BH, p_dhd, p_wihT, p_whhT, p_dix + u * BH,
                 p_dhp, B, H, sp))
-        # ---- time-batched weight gradients: contractions over all (u, b) rows on the tcgen05 GEMM
+        # ---- time-batched weight gradients: contractions over all (u, b) rows on the wgmma GEMM
         R = steps * B
 
         def wgrad(dy, x):          # dy (R, O) f32, x (R, K) f32 -> dy^T x  (O, K) f32

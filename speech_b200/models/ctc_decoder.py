@@ -1,7 +1,7 @@
 """CTC prefix beam search - drop-in for speech/models/ctc_decoder.py:38-113 (reference).
 
 `decode(probs, beam_size=10, blank=0)` keeps the reference's signature and return value
-((label tuple, negative log-likelihood)); the search itself runs in the sm_100a kernel
+((label tuple, negative log-likelihood)); the search itself runs in the sm_90a kernel
 sb_ctc_prefix_beam (csrc/decode.cu), one CTA per utterance.  `decode_batch` is the batched
 entry CTC.infer uses (the reference loops over utterances in Python, ctc_model.py:59-60).
 """

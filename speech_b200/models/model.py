@@ -4,7 +4,7 @@ Same constructor, attributes, state_dict key names (`conv.{0,2,..}.{weight,bias}
 `rnn.weight_ih_l{k}[_reverse]` ...) and picklability as the reference `Model`; the nn.Conv2d /
 nn.GRU modules are kept as PARAMETER CONTAINERS (identical construction order => identical
 initialisation under the same torch seed) while the arithmetic of `encode` runs in the
-hand-written sm_100a kernels (speech_b200/ops.py -> csrc/).  There is no CPU path: calling
+hand-written sm_90a kernels (speech_b200/ops.py -> csrc/).  There is no CPU path: calling
 `encode` on a CPU tensor raises.
 """
 import math
@@ -117,7 +117,7 @@ class LinearND(nn.Module):
         self.fc = nn.Linear(*args)
 
     def forward(self, x):
-        # time-batched projections run on the package's tcgen05 GEMM (forward and backward);
+        # time-batched projections run on the package's wgmma GEMM (forward and backward);
         # per-token rows of the attention decoder (a handful of rows) stay in fp32
         _lib.require_cuda(x, "LinearND input")
         if x.numel() // x.shape[-1] >= 128 and self.fc.out_features >= 8:

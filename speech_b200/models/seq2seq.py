@@ -1,7 +1,7 @@
 """Attention sequence-to-sequence model - host-side mirror of speech/models/seq2seq.py:14-248
 (Seq2Seq) and :331-360 (NNAttention, the only attention module the reference instantiates).
 
-The encoder runs on the sm_100a kernels (ops.conv_stack / ops.gru_stack).  The per-token decoder
+The encoder runs on the sm_90a kernels (ops.conv_stack / ops.gru_stack).  The per-token decoder
 (embedding + GRUCell + NNAttention + fc, seq2seq.py:92-108,114-137) keeps the reference's module
 structure and state_dict names (the nn modules are parameter containers); its arithmetic is two
 kernels per token, forward and backward (functions/s2s.py -> csrc/s2s.cu), and both the greedy

@@ -1,6 +1,6 @@
 """RNN-Transducer model - host-side mirror of speech/models/transducer_model.py:14-116.
 
-Encoder and prediction network run on the sm_100a GRU kernels (ops.gru_stack); the joint network
+Encoder and prediction network run on the sm_90a GRU kernels (ops.gru_stack); the joint network
 (fc1 shared by both streams, transducer_model.py:71-73), the log-softmax and the loss run fused
 (csrc/joint.cu + csrc/rnnt.cu): training never materialises the (B,T',U+1,H) hidden tensor nor the
 (B,T',U+1,V+1) log-probabilities, only a compact {blank, label} lattice; `forward` / `infer` still

@@ -1,7 +1,7 @@
 """Host-side operators over the C ABI: dense contraction and the (bi)GRU stack.
 
 PyTorch is used here for device memory, streams and autograd plumbing only; the arithmetic of
-the recurrence and of every projection runs in the hand-written sm_100a kernels of csrc/.
+the recurrence and of every projection runs in the hand-written sm_90a kernels of csrc/.
 Internal activations are TIME-MAJOR with the batch padded to a multiple of 8 (row m = t*Bp + b).
 """
 import ctypes
@@ -28,8 +28,6 @@ def _apply_env_knobs():
     lib = _lib.load()
     if os.environ.get("SB_GRU_KSPLIT") is not None:
         lib.sb_debug_gru_ksplit(int(os.environ["SB_GRU_KSPLIT"]))
-    if os.environ.get("SB_GEMM_MT1") is not None:
-        lib.sb_debug_gemm_mt1(int(os.environ["SB_GEMM_MT1"]))
     if os.environ.get("SB_GRU_CLUSTER") is not None:
         lib.sb_debug_gru_cluster(int(os.environ["SB_GRU_CLUSTER"]))
 
@@ -209,7 +207,7 @@ def encode_logits_parity(x, conv, rnn, fc):
 
 
 class LinearFunction(torch.autograd.Function):
-    """y = x W^T + b on the tcgen05 GEMM (bf16 operands, fp32 accumulate), forward and backward:
+    """y = x W^T + b on the wgmma GEMM (bf16 operands, fp32 accumulate), forward and backward:
     the arithmetic behind the reference's LinearND / nn.Linear (model.py:115-133).
     x (N, K) f32, W (O, K), b (O) -> (N, O) f32."""
 
@@ -253,7 +251,7 @@ class LinearFunction(torch.autograd.Function):
 
 
 def linear(x, w, b=None):
-    """nn.Linear semantics over the last dimension of an N-D CUDA tensor, on the tcgen05 GEMM."""
+    """nn.Linear semantics over the last dimension of an N-D CUDA tensor, on the wgmma GEMM."""
     lead = x.shape[:-1]
     out = LinearFunction.apply(x.reshape(-1, x.shape[-1]).float(), w, b)
     return out.view(*lead, out.shape[-1])
@@ -589,7 +587,7 @@ def gru_stack_logits(x, rnn, fc, dropout=0.0):
 
 
 def gru_stack(x, rnn, dropout=0.0):
-    """Run the sm_100a GRU stack with the parameters of an nn.GRU module (batch_first, h0 = 0)."""
+    """Run the sm_90a GRU stack with the parameters of an nn.GRU module (batch_first, h0 = 0)."""
     ndir, weights = _gru_weights(rnn)
     return _batch_chunks(x, lambda xc: GRUStackFunction.apply(
         xc, ndir, rnn.hidden_size, float(dropout), None, None, *weights))
@@ -615,7 +613,7 @@ def _transpose_bf16(src, rows_pad=8, out=None):
 
 
 class ConvStackFunction(torch.autograd.Function):
-    """Conv2d+ReLU stack as im2col + tcgen05 GEMM (csrc/conv.cu, csrc/gemm.cu).
+    """Conv2d+ReLU stack as im2col + wgmma GEMM (csrc/conv.cu, csrc/gemm.cu).
 
     forward(x (B,T,F) f32, specs ((kh,kw,s),...), w0, b0, w1, b1, ...) -> (B, T', C*F') f32 with
     the reference's channel-major feature order (model.py:66-71)."""
@@ -722,7 +720,7 @@ def conv_stack(x, conv, training):
     """Conv2d+ReLU(+Dropout) front-end of the encoder (reference model.py:19-29,60-71).
 
     x (B, T, F) -> (B, T', C*F') with the reference's channel-major feature flattening
-    (transpose(1,2) of (B,C,T',F') then view, model.py:66-71).  Runs on our im2col + tcgen05
+    (transpose(1,2) of (B,C,T',F') then view, model.py:66-71).  Runs on our im2col + wgmma
     kernels, including the Dropout after each ReLU when training.  Shapes the kernels do not
     cover go through the nn modules: grouped / dilated / padded convolutions and out_channels not
     a multiple of 8 (none of which the reference can express, model.py:21-23), and - only when a

@@ -1,5 +1,5 @@
 """Data-parallel gradient synchronisation: one process per GPU, minibatch sharded B/N per rank,
-the gradients summed over ranks once per step over NCCL (NVLink 5 / NVSwitch).
+the gradients summed over ranks once per step over NCCL (NVLink / NVSwitch).
 
 The reference has no multi-GPU path at all (train.py:92, SURVEY.md §2.4); this adds exactly the
 collective the north star names.  Gradients are SUMMED (not averaged): the reference's loss is a

@@ -1,4 +1,4 @@
-"""GPU parity: im2col + tcgen05 conv stack vs torch conv2d in fp64 on the CPU.
+"""GPU parity: im2col + wgmma conv stack vs torch conv2d in fp64 on the CPU.
 
 The kernels round the GEMM operands (inputs, weights, inter-layer activations) to bf16 and
 accumulate in fp32.  A ReLU mask is discontinuous, so a reference computed from UN-rounded operands

@@ -1,4 +1,4 @@
-"""GPU parity: fused sm_100a CTC kernel (through the C ABI) vs the CPU oracle.
+"""GPU parity: fused sm_90a CTC kernel (through the C ABI) vs the CPU oracle.
 
 Tolerance: loss and gradients within 1e-4 relative (BASELINE.json north_star), fp32 kernel vs
 float64 oracle.  Gradient tolerance is relative to the largest |grad| of the utterance (entries

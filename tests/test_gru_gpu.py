@@ -72,7 +72,7 @@ def test_gru_north_star_width_small_batches(cuda_lib, B):
 
 @pytest.mark.parametrize("B,H", [(96, 256), (128, 256), (128, 1024)])
 def test_gru_large_per_gpu_batch(cuda_lib, B, H):
-    """batches above 64 rows per GPU (all four TMEM lane quadrants; smaller smem ring at H=1024)."""
+    """batches above 64 rows per GPU (two m64 wgmma blocks per step; smaller smem ring at H=1024)."""
     rnn64, x64, y64, rnn_c, xc, yc = _ref_and_ours(B, 4, 64, H, 1, True, seed=B + H)
     assert (yc.double().cpu() - y64).abs().max().item() < 2e-2
     for (n, p64), (_, pc) in zip(rnn64.named_parameters(), rnn_c.named_parameters()):

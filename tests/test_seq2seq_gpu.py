@@ -99,7 +99,7 @@ def test_teacher_forced_decode_forward_and_backward(cuda_lib, B, T, H, V, U, log
             continue
         ref = rp[name].grad
         got = p.grad.double().cpu().reshape(ref.shape)
-        # time-batched on the tcgen05 GEMM (bf16 operands): cell weights and the output projection
+        # time-batched on the wgmma GEMM (bf16 operands): cell weights and the output projection
         tol = 2e-2 if name in ("dec_rnn.weight_ih", "dec_rnn.weight_hh", "fc.fc.weight") else 2e-3
         # the softmax is invariant to a shift of the scores, so d(attention bias) is EXACTLY zero:
         # what both sides hold is the rounding residue of sum_t d score_t (fp64: 1e-16, fp32: 1e-6)

@@ -1,4 +1,4 @@
-"""Developer tool: validate the MN-major UMMA operand path of sb_gemm_bf16_tn against torch.
+"""Developer tool: validate the MN-major wgmma operand path of sb_gemm_bf16_tn against torch.
 
 Sweeps the descriptor-field candidates (LBO, SBO, K advance) so that one GPU call settles the
 encoding; the defaults compiled into gemm.cu are the first row."""
