@@ -74,7 +74,8 @@ struct GruBwdParams {
   unsigned int* barrier;  // [ndir]
   unsigned long long* dbg;
   int T, Bp, H, ndir, ring, gc;
-  int ablate;          // developer knobs (polling mode bits 64 / 128)
+  int dir0;            // direction of CTA 0 (gru_bwd_ks_kernel launched for one direction: 0 or 1)
+  int ablate;          // developer knobs: see sb_debug_gru_flags
 };
 
 SB_DEVINL unsigned long long gtime() {
@@ -690,7 +691,7 @@ gru_bwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
   extern __shared__ uint8_t smem_raw[];
   const int H = p.H, Bp = p.Bp, T = p.T;
   const int nC = H / GRU_HC;
-  const int dir = blockIdx.x / nC;
+  const int dir = p.dir0 + blockIdx.x / nC;
   const int cta_in_dir = blockIdx.x % nC;
   const int j0 = cta_in_dir * GRU_HC;                 // own 16 units (elementwise work)
   const uint32_t crank = cluster_rank();              // == cta_in_dir % 4
@@ -752,16 +753,19 @@ gru_bwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
 
   if (warp == GRU_TMA_WARP) {
     if (lane == 0) {
-      for (int step = 0; step + 1 < T; ++step) {
-        grid_wait(ctr, (unsigned int)nC * (step + 1), p.ablate & 192);   // dgh of this step is complete
+      // step = the epilogue step that consumes the product (as in the forward kernels)
+      for (int step = 1; step < T; ++step) {
+        grid_wait(ctr, (unsigned int)nC * step, p.ablate & 192);   // dgh of step - 1 is complete
+        GRU_STAMP(0);
         for (int g = 0; g < ngroups; ++g) {
           mbar_expect_tx(&full[g], (uint32_t)(stride * gc));
           for (int i = 0; i < gc; ++i) {
             const int c = g * gc + i;
             tma_load_2d(ring + c * stride, tm, &full[g], (int)crank * KQ + c * 64,
-                        (step & 1) * Bp);
+                        ((step - 1) & 1) * Bp);
           }
         }
+        GRU_STAMP(1);
       }
     }
   } else if (warp >= GRU_MMA_WARP) {
@@ -770,10 +774,10 @@ gru_bwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
     // into stage[pr], the CTA's own 16 columns into recv[crank] (which no peer writes).
     const int t = tid & 127;
     const bool two = Bp > 64;                 // batch rows 64..127: a second m64 block
-    for (int step = 0; step + 1 < T; ++step) {
+    for (int step = 1; step < T; ++step) {
       float d[2][32];   // initialised by the scale-d = 0 first MMA (d[1] only used if two)
       for (int g = 0; g < ngroups; ++g) {
-        mbar_wait(&full[g], step & 1);
+        mbar_wait(&full[g], (step - 1) & 1);
         wgmma_fence();
         for (int i = 0; i < gc; ++i) {
           const int c = g * gc + i;
@@ -805,6 +809,7 @@ gru_bwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
       }
       fence_proxy_async_smem();   // generic st.shared -> the bulk copies (async proxy) to the peers
       mbar_arrive(accfull);
+      if (t == 0) GRU_STAMP(2);
     }
   } else {
     const int row = (warp & 3) * 32 + lane;
@@ -888,7 +893,7 @@ gru_bwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
           *reinterpret_cast<uint4*>(x + H) = pack8(dz);
           *reinterpret_cast<uint4*>(x + 2 * H) = pack8(dnr);
           if (tid == 0) GRU_STAMP(5);
-          fence_proxy_async_global();
+          if (!(p.ablate & 1)) fence_proxy_async_global();
           if (tid == 0) GRU_STAMP(6);
         }
       }
@@ -900,7 +905,7 @@ gru_bwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
           GRU_STAMP(9);
         }
       }
-      if (active) {
+      if (active && !(p.ablate & 2)) {
         bf16* o = p.dgi + m * (p.ndir * K3) + dir * K3 + ju;
         st_stream_u4(o, pack8(dr));
         st_stream_u4(o + H, pack8(dz));
@@ -1135,7 +1140,7 @@ gru_fwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
         // critical path: only the bf16 h_t that the other CTAs gather next step
         *reinterpret_cast<uint4*>(p.xn + m * D + dir * H + ju) = pack8(hprev);
         if (tid == 0) GRU_STAMP(5);
-        fence_proxy_async_global();   // generic writes -> other CTAs' TMA reads
+        if (!(p.ablate & 1)) fence_proxy_async_global();   // generic writes -> other CTAs' TMA reads
         if (tid == 0) GRU_STAMP(6);
       }
       epi_barrier();
@@ -1145,7 +1150,7 @@ gru_fwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
         grid_arrive(ctr);
         GRU_STAMP(9);
       }
-      if (active) {
+      if (active && !(p.ablate & 2)) {
         st8(p.y + m * D + dir * H + ju, hprev);
         if (p.gates) {
           float* go = p.gates + ((m * p.ndir + dir) * 4) * H + ju;
@@ -1805,11 +1810,15 @@ static int g_gru_ablate = 0;
 static int g_gru_ksplit = 1;   // developer knob: 0 disables the K-split backward kernel
 
 // Which K-split flavour: the transposed-accumulator kernels (gru_*_kt_kernel) spend tensor work
-// in proportion to the batch (N = batch) instead of a whole m64 block of batch rows.  Measured on
-// an H100 80GB HBM3 (400 W power limit), one biGRU-1024 layer at T = 247 including its projection
-// GEMMs, ms (kt | ks): forward 2.12 | 2.14 at 8 rows, 2.10 | 2.46 at 16, 2.66 | 2.50 at 32,
-// 4.40 | 4.37 at 64; backward 3.03 | 2.98 at 8, 3.18 | 3.24 at 16, 6.24 | 6.23 at 32,
-// 8.30 | 7.88 at 64.  So kt runs the forward recurrence up to 16 rows; the backward stays on ks.
+// in proportion to the batch (N = batch) instead of a whole m64 block of batch rows.
+// An H100 holds 30 clusters of 4 one-CTA-per-SM blocks (120 CTAs), so at H = 1024 the two
+// directions (128 CTAs) never fit as one K-split launch: the forward runs gru_fwd_kernel there
+// and the backward gru_bwd_ks_kernel once per direction.  Measured on an H100 80GB HBM3 (400 W
+// power limit), recurrence kernel alone, us per step at T = 247, ONE direction of H = 1024
+// (kt | ks): forward 4.12 | 4.17 at 8 rows, 4.59 | 4.34 at 16, 7.73 | 5.46 at 32, 14.68 | 8.38 at
+// 64; backward 3.17 | 4.28 at 8, 4.08 | 4.37 at 16, 6.09 | 5.12 at 32, 8.15 | 7.94 at 64.  Both
+// directions at 64 rows: gru_fwd_kernel 11.7; backward 23.4 with gru_bwd_kernel, 15.5 with the
+// two one-direction gru_bwd_ks_kernel launches.
 // Developer knob (sb_debug_gru_flags): 16 forces them, 8 disables them.
 static bool gru_use_kt(int Bp, bool backward) {
   if (g_gru_ablate & 8) return false;
@@ -1864,9 +1873,10 @@ extern "C" int sb_debug_gru_timeline(void* dev_buffer) {
   sb::g_gru_dbg = reinterpret_cast<unsigned long long*>(dev_buffer);
   return SB_OK;
 }
-// developer knobs: 1 / 2: gru_fwd_kernel without the proxy fence / the off-path stores (timing
-// only: results become wrong); 8 / 16: never / always use the transposed-accumulator K-split
-// kernels (default: by batch size, see gru_use_kt); 32: disable the K-split forward kernels;
+// developer knobs: 1 / 2: gru_fwd_kernel and the gru_*_ks_kernel without the proxy fence / the
+// off-path stores (timing only: results become wrong); 8 / 16: never / always use the
+// transposed-accumulator K-split kernels (default: by batch size, see gru_use_kt); 32: disable
+// the K-split forward kernels;
 // 64 / 128: polling mode of the grid barrier in the K-split kernels (see grid_wait)
 extern "C" int sb_debug_gru_flags(int flags) {
   sb::g_gru_ablate = flags;
@@ -1938,7 +1948,7 @@ extern "C" int sb_gru_fwd(const float* gi, const void* whh_bf16, const float* bh
       q.gi = gi; q.whh = reinterpret_cast<const bf16*>(whh_bf16); q.bhh = bhh; q.y = y;
       q.xn = reinterpret_cast<bf16*>(xn_bf16); q.xnT = nullptr; q.gates = gates;
       q.barrier = barrier; q.T = T; q.Bp = Bp; q.H = H; q.ndir = ndir;
-      q.dbg = g_gru_dbg; q.ablate = g_gru_ablate & 192; q.ring = nq; q.gc = 1;
+      q.dbg = g_gru_dbg; q.ablate = g_gru_ablate & 195; q.ring = nq; q.gc = 1;
       CUtensorMap tq[2];
       for (int d = 0; d < 2; ++d) {
         const int dd = d < ndir ? d : 0;
@@ -2013,7 +2023,8 @@ extern "C" int sb_gru_bwd(const float* dy, const float* y, const float* gates,
   p.xchg = reinterpret_cast<bf16*>(ws + gru_ws_counters_bytes(ndir));
   p.dbih = dbih; p.dbhh = dbhh; p.T = T; p.Bp = Bp; p.H = H; p.ndir = ndir;
   p.dbg = g_gru_dbg;
-  p.ablate = g_gru_ablate & 192;
+  p.dir0 = 0;
+  p.ablate = g_gru_ablate & 195;
   const int K3 = 3 * H;
   const int nchunks = (K3 + 63) / 64;
   size_t smem = 0;
@@ -2046,6 +2057,16 @@ extern "C" int sb_gru_bwd(const float* dy, const float* y, const float* gates,
       }
       rc = gru_launch_exact((const void*)gru_bwd_ks_kernel, ndir * nC_, KS, ks_smem, kargs, stream);
       if (rc == SB_OK) return SB_OK;
+      // Both directions do not fit as 4-CTA clusters (an H100 holds 30 of them, 120 CTAs, against
+      // 128 at H = 1024): run the directions one after the other, each with its own barrier
+      // counter.  Still faster than the plain kernel, whose every CTA gathers all of dgh_t.
+      if (rc == SB_ERR_UNSUPPORTED && ndir == 2) {
+        rc = gru_launch_exact((const void*)gru_bwd_ks_kernel, nC_, KS, ks_smem, kargs, stream);
+        if (rc == SB_OK) {
+          p.dir0 = 1;   // kernel parameters are copied at launch
+          return gru_launch_exact((const void*)gru_bwd_ks_kernel, nC_, KS, ks_smem, kargs, stream);
+        }
+      }
     }
   }
   p.ring = gru_ring_slots(std::max(nchunks * 16 * 128, 16384 - Bp * 128), Bp, nchunks, 16, &p.gc,

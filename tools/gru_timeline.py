@@ -38,9 +38,11 @@ else:
 print("mode:", MODE)
 raw = dbg.cpu().numpy()
 d = raw[:1024].reshape(64, 16)
-names = ["P:grid_wait done", "P:tma issued", "M:all mma committed", "E:accfull",
-         "E:tmem loaded (+reduce-scatter)", "E:xn stored", "E:proxy fence", "E:epi barrier", None,
-         "E:arrived", "E:offpath done"]
+# stamp index -> phase; P: producer warp, M: MMA warpgroup, E: epilogue thread 0.  The K-split
+# kernels stamp 4 after issuing the reduce-scatter bulk copies (the plain kernels: accbuf read).
+names = ["P:grid_wait done", "P:tma issued", "M:product staged", "E:accfull",
+         "E:reduce-scatter issued", "E:xn stored" if MODE == "fwd" else "E:dgh stored",
+         "E:proxy fence", "E:epi barrier", None, "E:arrived", "E:offpath done"]
 for step in (11, 40):
     base = d[step - 1][9]   # previous step's arrival by this CTA
     print("step %d (ns since this CTA's previous arrive):" % step)
