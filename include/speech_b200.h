@@ -295,7 +295,8 @@ int sb_rnnt_fwd_bwd_compact(const float* lat, float* garc, const int* labels,
  *   sb_rnnt_joint_build_slab / _reduce_slab: the hidden activations of Tc <= 8 frames
  *                           (z [B*Tc*U1][H] bf16) for the weight-gradient GEMMs, and the masked
  *                           reduction of dz [B*Tc*U1][H] f32 into dfx (=) and dfy (+=)
- * Constraints: H % 8 == 0, V1 <= 64.
+ * Constraints: H % 8 == 0, V1 <= 64.  Larger vocabularies (V1 > 64) go through the slab path
+ * below: build_slab, sb_gemm_bf16_tn for the logits, and sb_rnnt_joint_vocab_fwd_rows / _bwd_rows.
  * ------------------------------------------------------------------------------------- */
 int sb_rnnt_joint_fwd(const float* fx, const float* fy, const void* w2_bf16, const float* b2,
                       const int* ymat, float* lat, float* lp_full, int B, int T, int U1, int H,
@@ -307,6 +308,30 @@ int sb_rnnt_joint_build_slab(const float* fx, const float* fy, void* z_bf16, int
                              int H, int t0, int Tc, void* stream);
 int sb_rnnt_joint_reduce_slab(const float* dz, const void* z_bf16, float* dfx, float* dfy, int B,
                               int T, int U1, int H, int t0, int Tc, void* stream);
+
+/* ---------------------------------------------------------------------------------------
+ * Row kernels of the large-vocabulary joint (any V1; the models use them for V1 > 64, where fc2's
+ * weight does not fit the shared memory of the fused kernel).  The caller walks the lattice a slab
+ * of Tc frames at a time: z = sb_rnnt_joint_build_slab, logits = z W2^T + b2 with sb_gemm_bf16_tn
+ * into f32 rows [Tc*B*U1][ld]; row r of the slab is node n = t0*B*U1 + r.
+ *   sb_rnnt_joint_vocab_fwd_rows: per row, max and log-sum-exp over the first V1 columns ->
+ *       lat [nodes][2] = {v_blank - lse, v_label - lse} (label -inf at u = U1-1, as
+ *       sb_rnnt_joint_fwd), lse [nodes] (kept for the backward pass), and, if lp_full is not NULL,
+ *       the slab's rows of the batch-first (B, T, U1, V1) log-probabilities.
+ *   sb_rnnt_joint_vocab_bwd_rows: from the recomputed logits, lse and garc [nodes][2] ->
+ *       dlogits [Tc*B*U1][ldd] bf16, dlogit_k = g_b [k = blank] + g_l [k = label]
+ *       - (g_b + g_l) exp(v_k - lse), zero in columns V1 .. ldd-1;  db2 [V1] += its column sums.
+ * lat, lse and garc are the whole-lattice arrays (indexed by n), logits / dlogits the slab's rows.
+ * Constraints: 0 <= blank < V1, 0 <= t0, t0 + Tc <= T, ld and ldd >= V1 and multiples of 8,
+ * logits and dlogits 16-byte aligned.
+ * ------------------------------------------------------------------------------------- */
+int sb_rnnt_joint_vocab_fwd_rows(const float* logits, long long ld, const int* ymat, float* lat,
+                                 float* lse, float* lp_full, int B, int T, int U1, int V1, int blank,
+                                 int t0, int Tc, void* stream);
+int sb_rnnt_joint_vocab_bwd_rows(const float* logits, long long ld, const float* lse,
+                                 const float* garc, const int* ymat, void* dlogits_bf16,
+                                 long long ldd, float* db2, int B, int T, int U1, int V1, int blank,
+                                 int t0, int Tc, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Transducer beam search over a precomputed (teacher-forced) lattice, one CTA per utterance.

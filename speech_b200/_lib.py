@@ -70,6 +70,10 @@ SIGNATURES = {
                                           _c_int, _vp]),
     "sb_rnnt_joint_reduce_slab": (_c_int, [_vp, _vp, _vp, _vp, _c_int, _c_int, _c_int, _c_int,
                                            _c_int, _c_int, _vp]),
+    "sb_rnnt_joint_vocab_fwd_rows": (_c_int, [_vp, _c_ll, _vp, _vp, _vp, _vp, _c_int, _c_int, _c_int,
+                                              _c_int, _c_int, _c_int, _c_int, _vp]),
+    "sb_rnnt_joint_vocab_bwd_rows": (_c_int, [_vp, _c_ll, _vp, _vp, _vp, _vp, _c_ll, _vp, _c_int,
+                                              _c_int, _c_int, _c_int, _c_int, _c_int, _c_int, _vp]),
     "sb_rnnt_decode_static_workspace_size": (_c_int, [_c_int, _c_int, _c_int, _c_int,
                                                       ctypes.POINTER(_c_sz)]),
     "sb_rnnt_decode_static": (_c_int, [_vp, _vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int, _c_int,

@@ -92,6 +92,108 @@ class TransducerLoss(torch.nn.Module):
 # (transducer_model.py:71-76) never exist on the training path.
 # ------------------------------------------------------------------------------------------------
 JOINT_SLAB_FRAMES = 8     # frames whose hidden activations are materialised at a time in backward
+JOINT_RESIDENT_MAX_CLASSES = 64   # V+1 up to which fc2's weight stays resident in the fused kernel
+# Cap on one slab's fp32 logits in the large-vocabulary path.  Measured on an H100 80GB HBM3 at a
+# 700 W power limit (tools/joint_vocab_bench.py, B=32, T'=247, U+1=100, H=1024), forward + backward:
+#   V+1 = 1024: Tc = 1, 2, 4, 8 -> 40.8, 32.5, 27.0, 24.4 ms (host enqueue 30.5, 16.0, 8.1, 5.9 ms)
+#   V+1 = 4096: Tc = 1, 2, 4, 8 -> 100.6, 91.8, 84.8, 81.8 ms
+# (the same order on a card limited to 400 W: 40.8, 37.9, 32.6, 29.5 ms at V+1 = 1024).
+# Keeping a slab's logits in the 50 MB L2 (Tc <= 2 at V+1 = 1024) loses to the larger GEMMs and the
+# fewer launches of bigger slabs, so the cap only bounds memory: Tc = 8 up to V+1 = 5120 there.
+JOINT_VOCAB_SLAB_BYTES = 512 << 20
+
+
+def _round_up(x, m):
+    return (x + m - 1) // m * m
+
+
+def joint_vocab_slab_frames(B, U1, V1, budget=None):
+    """Frames per slab of the large-vocabulary joint (forward and backward): as many as keep one
+    slab's fp32 logits within `budget` bytes, at most JOINT_SLAB_FRAMES (the limit of
+    sb_rnnt_joint_reduce_slab); one frame when a single frame alone exceeds the budget."""
+    budget = JOINT_VOCAB_SLAB_BYTES if budget is None else budget
+    frame = B * U1 * _round_up(V1, 8) * 4
+    return max(1, min(JOINT_SLAB_FRAMES, budget // frame))
+
+
+def joint_vocab_forward(fxc, fyc, w2b, b2c, ym, blank, lp_full=None):
+    """Joint + log-softmax for any V1 (used for V1 > 64), a slab of frames at a time:
+    z = relu(fx + fy) (bf16) -> logits = z W2^T + b2 (f32, GEMM) -> per-row log-sum-exp.
+    fxc (B,T,H) f32, fyc (B,U1,H) f32, w2b (V1,H) bf16, b2c (V1,) f32, ym (B,U1-1) int32, all
+    contiguous on the device.  Fills lp_full (B,T,U1,V1) f32 if given.
+    -> lat (nodes, 2) {log p(blank), log p(label)}, lse (nodes,) log-sum-exp of every node."""
+    from .. import ops
+    lib = _lib.load()
+    B, T, H = fxc.shape
+    U1 = fyc.shape[1]
+    V1 = w2b.shape[0]
+    dev = fxc.device
+    ld = _round_up(V1, 8)
+    Tc = min(joint_vocab_slab_frames(B, U1, V1), T)
+    lat = torch.empty(T * B * U1, 2, dtype=torch.float32, device=dev)
+    lse = torch.empty(T * B * U1, dtype=torch.float32, device=dev)
+    z = torch.empty(Tc * B * U1, H, dtype=torch.bfloat16, device=dev)
+    logits = torch.empty(Tc * B * U1, ld, dtype=torch.float32, device=dev)
+    sp = _lib.stream_ptr()
+    for t0 in range(0, T, Tc):
+        tc = min(Tc, T - t0)
+        ops._launch("rnnt_joint_slab", 0.0,
+                    lambda: lib.sb_rnnt_joint_build_slab(fxc.data_ptr(), fyc.data_ptr(),
+                                                         z.data_ptr(), B, T, U1, H, t0, tc, sp))
+        ops.gemm_bf16_tn(z[:tc * B * U1], w2b, out=logits, bias=b2c)
+        ops._launch("rnnt_joint_rows", 0.0,
+                    lambda: lib.sb_rnnt_joint_vocab_fwd_rows(logits.data_ptr(), ld, ym.data_ptr(),
+                                                             lat.data_ptr(), lse.data_ptr(),
+                                                             _lib.ptr(lp_full), B, T, U1, V1,
+                                                             int(blank), t0, tc, sp))
+    return lat, lse
+
+
+def joint_vocab_backward(fxc, fyc, w2b, b2c, ym, garc, lse, blank):
+    """Backward of joint_vocab_forward from garc (nodes, 2), the gradient w.r.t. lat, and the
+    forward's lse.  Per slab: z, the logits again (same GEMM), dlogits (bf16) and db2 from the row
+    kernel, dW2 += dlogits^T z, dz = dlogits W2, then dz is reduced into dfx / dfy.
+    -> dfx (B,T,H), dfy (B,U1,H), dw2 (V1,H), db2 (V1,), all f32."""
+    from .. import ops
+    lib = _lib.load()
+    B, T, H = fxc.shape
+    U1 = fyc.shape[1]
+    V1 = w2b.shape[0]
+    dev = fxc.device
+    ld = _round_up(V1, 8)
+    Tc = min(joint_vocab_slab_frames(B, U1, V1), T)
+    rows_max = Tc * B * U1
+    z = torch.empty(rows_max, H, dtype=torch.bfloat16, device=dev)
+    logits = torch.empty(rows_max, ld, dtype=torch.float32, device=dev)
+    dl = torch.empty(rows_max, ld, dtype=torch.bfloat16, device=dev)
+    dz = torch.empty(rows_max, H, dtype=torch.float32, device=dev)
+    dw2 = torch.zeros(V1, H, dtype=torch.float32, device=dev)
+    db2 = torch.zeros(V1, dtype=torch.float32, device=dev)
+    dfx = torch.empty(B, T, H, dtype=torch.float32, device=dev)
+    dfy = torch.zeros(B, U1, H, dtype=torch.float32, device=dev)
+    sp = _lib.stream_ptr()
+    for t0 in range(0, T, Tc):
+        tc = min(Tc, T - t0)
+        rows = tc * B * U1
+        ops._launch("rnnt_joint_slab", 0.0,
+                    lambda: lib.sb_rnnt_joint_build_slab(fxc.data_ptr(), fyc.data_ptr(),
+                                                         z.data_ptr(), B, T, U1, H, t0, tc, sp))
+        ops.gemm_bf16_tn(z[:rows], w2b, out=logits, bias=b2c)
+        ops._launch("rnnt_joint_rows", 0.0,
+                    lambda: lib.sb_rnnt_joint_vocab_bwd_rows(logits.data_ptr(), ld, lse.data_ptr(),
+                                                             garc.data_ptr(), ym.data_ptr(),
+                                                             dl.data_ptr(), ld, db2.data_ptr(), B, T,
+                                                             U1, V1, int(blank), t0, tc, sp))
+        dlv = dl[:rows, :V1]
+        # dW2 (V1 x H) += dlogits^T z   (token-major operands, MN-major wgmma)
+        ops.gemm_bf16_tn(dlv, z[:rows], out=dw2, accumulate=True, a_mn=True, b_mn=True)
+        # dz (rows x H) = dlogits W2    (W2 is the [K][N] form of the B operand)
+        ops.gemm_bf16_tn(dlv, w2b, out=dz[:rows], b_mn=True)
+        ops._launch("rnnt_joint_slab", 0.0,
+                    lambda: lib.sb_rnnt_joint_reduce_slab(dz.data_ptr(), z.data_ptr(),
+                                                          dfx.data_ptr(), dfy.data_ptr(), B, T,
+                                                          U1, H, t0, tc, sp))
+    return dfx, dfy, dw2, db2
 
 
 def _pack_labels(labels, x_lens, y_lens, B, U1, dev):
@@ -123,6 +225,10 @@ def joint_log_probs(fx, fy, fc2, ymat, blank):
     w2 = fc2.weight.detach().to(torch.bfloat16).contiguous()
     b2 = fc2.bias.detach().float().contiguous()
     ym = ymat.detach().to(fx.device, torch.int32).contiguous()
+    if V1 > JOINT_RESIDENT_MAX_CLASSES:
+        out = torch.empty(B, T, U1, V1, dtype=torch.float32, device=fx.device)
+        joint_vocab_forward(fxc, fyc, w2, b2, ym, blank, lp_full=out)
+        return out
     lat = torch.empty(T * B * U1, 2, dtype=torch.float32, device=fx.device)
     out = torch.empty(B, T, U1, V1, dtype=torch.float32, device=fx.device)
     sp = _lib.stream_ptr()
@@ -149,12 +255,17 @@ class _JointLossFunction(torch.autograd.Function):
         ym = ymat.detach().to(dev, torch.int32).contiguous()
         lab, offs, ylen, xlen = _pack_labels(labels, x_lens, y_lens, B, U1, dev)
         nodes = T * B * U1
-        lat = torch.empty(nodes, 2, dtype=torch.float32, device=dev)
-        sp = _lib.stream_ptr()
-        ops._launch("rnnt_joint", 2.0 * nodes * H * V1,
-                    lambda: lib.sb_rnnt_joint_fwd(fxc.data_ptr(), fyc.data_ptr(), w2b.data_ptr(),
-                                                  b2c.data_ptr(), ym.data_ptr(), lat.data_ptr(),
-                                                  None, B, T, U1, H, V1, int(blank), sp))
+        lse = None
+        if V1 > JOINT_RESIDENT_MAX_CLASSES:
+            lat, lse = joint_vocab_forward(fxc, fyc, w2b, b2c, ym, blank)
+            sp = _lib.stream_ptr()
+        else:
+            lat = torch.empty(nodes, 2, dtype=torch.float32, device=dev)
+            sp = _lib.stream_ptr()
+            ops._launch("rnnt_joint", 2.0 * nodes * H * V1,
+                        lambda: lib.sb_rnnt_joint_fwd(fxc.data_ptr(), fyc.data_ptr(), w2b.data_ptr(),
+                                                      b2c.data_ptr(), ym.data_ptr(), lat.data_ptr(),
+                                                      None, B, T, U1, H, V1, int(blank), sp))
         need = any(ctx.needs_input_grad[:4])
         nbytes = ctypes.c_size_t(0)
         _lib.check(lib.sb_rnnt_workspace_size(B, T, U1, ctypes.byref(nbytes)), "ws")
@@ -171,6 +282,7 @@ class _JointLossFunction(torch.autograd.Function):
         scale = 1.0 / B if size_average else 1.0
         ctx.saved = (fxc, fyc, w2b, b2c, ym, garc)
         ctx.dims = (B, T, U1, H, V1, int(blank), scale)
+        ctx.lse = lse
         return loss * scale
 
     @staticmethod
@@ -184,6 +296,9 @@ class _JointLossFunction(torch.autograd.Function):
             return (None,) * 10
         garc = garc * (grad_out.reshape(1, 1).float() * scale)
         nodes = T * B * U1
+        if V1 > JOINT_RESIDENT_MAX_CLASSES:
+            dfx, dfy, dw2, db2 = joint_vocab_backward(fxc, fyc, w2b, b2c, ym, garc, ctx.lse, blank)
+            return dfx, dfy, dw2, db2, None, None, None, None, None, None
         NV = 32 if V1 <= 32 else 64
         dlog = torch.empty(nodes, NV, dtype=torch.bfloat16, device=dev)
         db2 = torch.zeros(V1, dtype=torch.float32, device=dev)

@@ -5,6 +5,9 @@ Encoder and prediction network run on the sm_90a GRU kernels (ops.gru_stack); th
 (csrc/joint.cu + csrc/rnnt.cu): training never materialises the (B,T',U+1,H) hidden tensor nor the
 (B,T',U+1,V+1) log-probabilities, only a compact {blank, label} lattice; `forward` / `infer` still
 return the reference's full log-probability tensor, written by the same fused kernel.
+The fused kernel keeps fc2's weight in shared memory, which holds up to V+1 = 64 classes; larger
+vocabularies run the same computation a slab of frames at a time (GEMM logits + row kernels of
+csrc/joint_vocab.cu), so only one slab's logits ever exist.
 """
 import torch
 import torch.nn as nn

@@ -25,4 +25,8 @@ print("seq2seq ok", l2.item(), [len(h) for h in s.infer((inputs, lab2), max_len=
 t = Transducer(80, 28, cfg).cuda()
 l3 = t.loss((inputs, labels)); l3.backward()
 print("transducer ok", l3.item())
+t2 = Transducer(80, 300, cfg).cuda()       # V+1 = 301: the large-vocabulary joint path
+labels2 = [np.random.randint(0, 300, 7 + i).tolist() for i in range(5)]
+l4 = t2.loss((inputs, labels2)); l4.backward()
+print("transducer V+1=301 ok", l4.item(), [len(p) for p in t2.infer((inputs, labels2))])
 torch.cuda.synchronize()
