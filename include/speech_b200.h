@@ -119,6 +119,20 @@ int sb_gru_bwd(const float* dy, const float* y, const float* gates, const void* 
                void* dgi_bf16, void* dghn_bf16, float* dbih, float* dbhh, void* workspace,
                size_t workspace_bytes, int T, int Bp, int H, int ndir, void* stream);
 
+/* Per-utterance time alignment of a block of columns of a time-major [T*Bp][ld] matrix (row
+ * m = t*Bp + b), for the exact-lengths mode of the GRU stack (csrc/lengths.cu):
+ *   right != 0: row (t, b) moves to (t + T - len_b, b)  (each utterance ends at frame T-1)
+ *   right == 0: row (t, b) moves to (t - T + len_b, b)  (the inverse: back to frame 0)
+ * Destination rows with no source row are zero-filled.  With right-aligned operands the reverse
+ * direction of sb_gru_fwd / sb_gru_bwd processes each utterance's real frames first and its
+ * padding last, so its real frames are those of the unpadded utterance.
+ *   src, dst    first element of the column block; ld_src / ld_dst in elements; out of place only
+ *   lens        (Bp) int32 valid frames per row b (device; clamped to [0, T]; give T for padding
+ *               rows of the batch)
+ *   cols        columns in the block;  elem_bytes 2 (bf16) or 4 (f32) */
+int sb_time_align(const void* src, long long ld_src, void* dst, long long ld_dst, const int* lens,
+                  int T, int Bp, int cols, int elem_bytes, int right, void* stream);
+
 /* ---------------------------------------------------------------------------------------
  * CTC prefix beam search, one CTA per utterance.
  * Replaces: speech.models.ctc_decoder.decode(probs, beam_size, blank)
@@ -236,6 +250,31 @@ int sb_s2s_attn_bwd(const float* eh, const float* hx, const float* hx_prev, cons
                     float* g_conv_wT, float* g_conv_b, float* g_lin_w, float* g_lin_b, int log_t,
                     int B, int T, int H, int Kc, void* workspace, size_t workspace_bytes,
                     void* stream);
+/* Length-masked variants (exact-lengths mode): `lens` (B) int32 on the device gives the frames
+ * row b attends over (clamped to [1, T]; NULL = all T, which is what the entry points above pass).
+ * Frames t >= lens[b] are left out of the softmax, so a_t = 0 exactly there, and out of the
+ * location conv's input; log_t scales by log(lens[b]); d eh stays untouched (zero) there.  CTAs
+ * whose frame tile lies wholly past lens[b] exit at once. */
+int sb_attn_step_len(const float* eh, const float* dhx, const float* ax_prev, const float* conv_wT,
+                     const float* conv_b, const float* lin_w, float lin_b, int log_t, int B, int T,
+                     int H, int Kc, float* sx, float* ax, const int* lens, void* workspace,
+                     size_t workspace_bytes, void* stream);
+int sb_s2s_attn_fwd_len(const float* eh, int eh_bcast, const float* hx, const float* ax_prev,
+                        const float* conv_wT, const float* conv_b, const float* lin_w, float lin_b,
+                        int log_t, int B, int T, int H, int Kc, float* sx, float* ax,
+                        const float* fc_w, const float* fc_b, int C, float* logits,
+                        long long logit_stride, float* logp, int* argmax, int* history,
+                        int hist_stride, int hist_col, int* end_count, int end_tok,
+                        const int* done, const int* lens, void* workspace,
+                        size_t workspace_bytes, void* stream);
+int sb_s2s_attn_bwd_len(const float* eh, const float* hx, const float* hx_prev,
+                        const float* ax_prev, const float* ax, const float* conv_wT,
+                        const float* conv_b, const float* lin_w, const float* d_o,
+                        const float* d_ix_next, const float* d_ax_next, const float* d_hx_next,
+                        const float* gates, float* d_eh, float* d_ax_prev, float* d_gi,
+                        float* d_gh, float* d_hx_direct, float* g_conv_wT, float* g_conv_b,
+                        float* g_lin_w, float* g_lin_b, int log_t, int B, int T, int H, int Kc,
+                        const int* lens, void* workspace, size_t workspace_bytes, void* stream);
 int sb_s2s_cell_bwd(const float* d_gi, const float* d_gh, const float* d_hx_direct,
                     const float* w_ihT, const float* w_hhT, float* d_ix, float* d_hx_prev, int B,
                     int H, void* stream);

@@ -46,6 +46,13 @@ SIGNATURES = {
     "sb_s2s_attn_fwd": (_c_int, [_vp, _c_int, _vp, _vp, _vp, _vp, _vp, _fl, _c_int, _c_int, _c_int,
                                  _c_int, _c_int, _vp, _vp, _vp, _vp, _c_int, _vp, _c_ll, _vp, _vp,
                                  _vp, _c_int, _c_int, _vp, _c_int, _vp, _vp, _c_sz, _vp]),
+    "sb_attn_step_len": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _fl, _c_int, _c_int, _c_int, _c_int,
+                                  _c_int, _vp, _vp, _vp, _vp, _c_sz, _vp]),
+    "sb_s2s_attn_fwd_len": (_c_int, [_vp, _c_int, _vp, _vp, _vp, _vp, _vp, _fl, _c_int, _c_int,
+                                     _c_int, _c_int, _c_int, _vp, _vp, _vp, _vp, _c_int, _vp, _c_ll,
+                                     _vp, _vp, _vp, _c_int, _c_int, _vp, _c_int, _vp, _vp, _vp,
+                                     _c_sz, _vp]),
+    "sb_s2s_attn_bwd_len": (_c_int, [_vp] * 22 + [_c_int] * 5 + [_vp, _vp, _c_sz, _vp]),
     "sb_s2s_dout": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _c_ll, _c_int, _c_int, _vp]),
     "sb_s2s_attn_bwd": (_c_int, [_vp] * 22 + [_c_int] * 5 + [_vp, _c_sz, _vp]),
     "sb_s2s_cell_bwd": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_int, _c_int, _vp]),
@@ -90,6 +97,8 @@ SIGNATURES = {
     "sb_gru_fwd": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_sz, _c_int, _c_int, _c_int,
                             _c_int, _vp]),
     "sb_gru_fwd_f32": (_c_int, [_vp, _vp, _vp, _vp, _vp, _c_int, _c_int, _c_int, _c_int, _vp]),
+    "sb_time_align": (_c_int, [_vp, _c_ll, _vp, _c_ll, _vp, _c_int, _c_int, _c_int, _c_int, _c_int,
+                               _vp]),
     "sb_gru_bwd_workspace_size": (_c_int, [_c_int, _c_int, _c_int, ctypes.POINTER(_c_sz)]),
     "sb_gru_bwd": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_sz, _c_int, _c_int,
                             _c_int, _c_int, _vp]),

@@ -246,9 +246,17 @@ struct AttnFwdParams {
   int* end_count;         // += 1 when this row's arg-max == end_tok (or null)
   int end_tok;
   const int* done;        // device flag: != 0 -> do nothing
+  const int* lens;        // (B) frames each row attends over, or null (all T)
   AttnWs ws;
   int B, T, H, Kc, C, log_t;
 };
+
+// Frames row b attends over: lens[b] clamped to [1, T], or T.  Frames >= this are left out of the
+// softmax (a_t = 0) and of the location conv's input, log_t scales by its log, and CTAs whose
+// frame tile lies wholly past it do nothing (they also stay out of the ticket count).
+SB_DEVINL int attn_frames(const int* lens, int b, int T) {
+  return lens ? min(max(__ldg(lens + b), 1), T) : T;
+}
 
 // the warp's alignment window: a[i] = ax_prev[tw + i - pad] (zero outside [0, T))
 SB_DEVINL void load_window(const float* ax_prev_b, int tw, int pad, int T, int Kc,
@@ -267,17 +275,19 @@ __global__ void __launch_bounds__(ATT_THREADS) s2s_attn_fwd_kernel(const AttnFwd
   const int b = blockIdx.y, ts = blockIdx.x, TS = gridDim.x;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int T = p.T, H = p.H, Kc = p.Kc, pad = (Kc - 1) / 2;
+  const int Tb = attn_frames(p.lens, b, T), TSb = (Tb + ATT_TT - 1) / ATT_TT;
+  if (ts >= TSb) return;
   float* wacc = att_smem;                      // [NW][H] per-warp weighted sums; later o, logits
   float* wst = wacc + ATT_NW * H;              // [NW][2] per-warp (max, sum)
   float* sct = wst + 2 * ATT_NW;               // [TS] scale of each CTA partial (final combine)
   const bool has_prev = p.ax_prev != nullptr;
-  const float tscale = p.log_t ? logf((float)T) : 1.0f;
+  const float tscale = p.log_t ? logf((float)Tb) : 1.0f;
   const float* eh = p.eh + (p.eh_bcast ? 0 : (size_t)b * T * H);
   const int tw = ts * ATT_TT + warp * ATT_FG;
-  const int nf = max(0, min(ATT_FG, T - tw));
+  const int nf = max(0, min(ATT_FG, Tb - tw));
 
   float a[ATT_WIN];
-  load_window(has_prev ? p.ax_prev + (size_t)b * T : nullptr, tw, pad, T, Kc, a);
+  load_window(has_prev ? p.ax_prev + (size_t)b * T : nullptr, tw, pad, Tb, Kc, a);
   // lanes over h in groups of four (16-byte loads): the h loop is a chain of L2 round trips, so it
   // has to be short - H/128 iterations
   const int H4 = H >> 2;
@@ -360,29 +370,29 @@ __global__ void __launch_bounds__(ATT_THREADS) s2s_attn_fwd_kernel(const AttnFwd
   if (tid == 0) { p.ws.m[slot] = m_c; p.ws.l[slot] = l_c; }
   __threadfence();
   __syncthreads();
-  if (tid == 0) s_last = (atomicAdd(p.ws.cnt + b, 1u) == (unsigned int)(TS - 1));
+  if (tid == 0) s_last = (atomicAdd(p.ws.cnt + b, 1u) == (unsigned int)(TSb - 1));
   __syncthreads();
   if (!s_last) return;
   __threadfence();
-  // ---- the utterance's last CTA: combine the TS partials in index order ----
+  // ---- the utterance's last CTA: combine the TSb partials in index order ----
   float m = -INFINITY;
-  for (int q = 0; q < TS; ++q) m = fmaxf(m, __ldcg(p.ws.m + (size_t)b * TS + q));
-  for (int q = tid; q < TS; q += ATT_THREADS) sct[q] = __expf(__ldcg(p.ws.m + (size_t)b * TS + q) - m);
+  for (int q = 0; q < TSb; ++q) m = fmaxf(m, __ldcg(p.ws.m + (size_t)b * TS + q));
+  for (int q = tid; q < TSb; q += ATT_THREADS) sct[q] = __expf(__ldcg(p.ws.m + (size_t)b * TS + q) - m);
   __syncthreads();
   float l = 0.f;
-  for (int q = 0; q < TS; ++q) l += __ldcg(p.ws.l + (size_t)b * TS + q) * sct[q];
+  for (int q = 0; q < TSb; ++q) l += __ldcg(p.ws.l + (size_t)b * TS + q) * sct[q];
   const float inv = 1.0f / l;
   float* o = wacc;                 // [H]   hx + sx
   float* lg = wacc + H;            // [C]
   for (int h = tid; h < H; h += ATT_THREADS) {
     float s = 0.f;
-    for (int q = 0; q < TS; ++q) s += __ldcg(p.ws.acc + ((size_t)b * TS + q) * H + h) * sct[q];
+    for (int q = 0; q < TSb; ++q) s += __ldcg(p.ws.acc + ((size_t)b * TS + q) * H + h) * sct[q];
     s *= inv;
     p.sx[(size_t)b * H + h] = s;
     o[h] = p.hx[(size_t)b * H + h] + s;
   }
   for (int t = tid; t < T; t += ATT_THREADS)
-    p.ax[(size_t)b * T + t] = __expf(__ldcg(p.ws.score + (size_t)b * T + t) - m) * inv;
+    p.ax[(size_t)b * T + t] = t < Tb ? __expf(__ldcg(p.ws.score + (size_t)b * T + t) - m) * inv : 0.f;
   if (tid == 0) p.ws.cnt[b] = 0u;
   if (!p.fc_w) return;
   // ---- output projection on o = hx + sx (seq2seq.py:108,131-132) ----
@@ -481,6 +491,7 @@ struct AttnBwdParams {
   float* g_conv_b;         // (B, H) +=
   float* g_lin_w;          // (B, H) +=
   float* g_lin_b;          // (B) +=
+  const int* lens;         // (B) frames of each utterance, or null (all T)
   AttnWs ws;
   int B, T, H, Kc, log_t;
 };
@@ -490,6 +501,8 @@ __global__ void __launch_bounds__(ATT_THREADS) s2s_attn_bwd_a_kernel(const AttnB
   const int b = blockIdx.y, ts = blockIdx.x, TS = gridDim.x;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int T = p.T, H = p.H;
+  const int Tb = attn_frames(p.lens, b, T);
+  if (ts * ATT_TT >= Tb) return;
   float* dsx = bwa_smem;             // [H]
   float* red = dsx + H;              // [NW]
   for (int h = tid; h < H; h += ATT_THREADS)
@@ -497,7 +510,7 @@ __global__ void __launch_bounds__(ATT_THREADS) s2s_attn_bwd_a_kernel(const AttnB
   __syncthreads();
   const float* eh = p.eh + (size_t)b * T * H;
   const int tw = ts * ATT_TT + warp * ATT_FG;
-  const int nf = max(0, min(ATT_FG, T - tw));
+  const int nf = max(0, min(ATT_FG, Tb - tw));
   float part[ATT_FG];
 #pragma unroll
   for (int f = 0; f < ATT_FG; ++f) part[f] = 0.f;
@@ -538,6 +551,8 @@ __global__ void __launch_bounds__(ATT_THREADS) s2s_attn_bwd_b_kernel(const AttnB
   const int b = blockIdx.y, ts = blockIdx.x, TS = gridDim.x;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int T = p.T, H = p.H, Kc = p.Kc, pad = (Kc - 1) / 2;
+  const int Tb = attn_frames(p.lens, b, T), TSb = (Tb + ATT_TT - 1) / ATT_TT;
+  if (ts >= TSb) return;
   float* dsx = bwb_smem;                         // [H]
   float* dpre_s = dsx + H;                       // [TT][H]  d pre of the CTA's frames
   float* glw_w = dpre_s + ATT_TT * H;            // [NW][H]  per-warp d lin_w
@@ -545,20 +560,20 @@ __global__ void __launch_bounds__(ATT_THREADS) s2s_attn_bwd_b_kernel(const AttnB
   float* axc = win_s + ATT_NW * ATT_WIN;         // [TT + KMAX - 1] the CTA's alignment window
   float* red = axc + ATT_TT + ATT_KMAX - 1;      // [NW]
   const bool has_prev = p.ax_prev != nullptr;
-  const float tscale = p.log_t ? logf((float)T) : 1.0f;
+  const float tscale = p.log_t ? logf((float)Tb) : 1.0f;
   const float* eh = p.eh + (size_t)b * T * H;
   float* deh = p.d_eh + (size_t)b * T * H;
   const int t0 = ts * ATT_TT;
   const int tw = t0 + warp * ATT_FG;
-  const int nf = max(0, min(ATT_FG, T - tw));
+  const int nf = max(0, min(ATT_FG, Tb - tw));
   for (int h = tid; h < H; h += ATT_THREADS)
     dsx[h] = p.d_o[(size_t)b * H + h] + (p.d_ix_next ? p.d_ix_next[(size_t)b * H + h] : 0.f);
   for (int j = tid; j < ATT_TT + ATT_KMAX - 1; j += ATT_THREADS) {
     const int tt = t0 - pad + j;
-    axc[j] = (has_prev && tt >= 0 && tt < T) ? p.ax_prev[(size_t)b * T + tt] : 0.f;
+    axc[j] = (has_prev && tt >= 0 && tt < Tb) ? p.ax_prev[(size_t)b * T + tt] : 0.f;
   }
   float S = 0.f;
-  for (int q = 0; q < TS; ++q) S += p.ws.s[(size_t)b * TS + q];
+  for (int q = 0; q < TSb; ++q) S += p.ws.s[(size_t)b * TS + q];
   __syncthreads();
   // ---- (i) warp per frame group ----
   float ds[ATT_FG], at[ATT_FG];
@@ -574,7 +589,7 @@ __global__ void __launch_bounds__(ATT_THREADS) s2s_attn_bwd_b_kernel(const AttnB
     }
   }
   float a[ATT_WIN];
-  load_window(has_prev ? p.ax_prev + (size_t)b * T : nullptr, tw, pad, T, Kc, a);
+  load_window(has_prev ? p.ax_prev + (size_t)b * T : nullptr, tw, pad, Tb, Kc, a);
   float dwin[ATT_WIN];
 #pragma unroll
   for (int i = 0; i < ATT_WIN; ++i) dwin[i] = 0.f;
@@ -647,7 +662,7 @@ __global__ void __launch_bounds__(ATT_THREADS) s2s_attn_bwd_b_kernel(const AttnB
         if (i >= 0 && i < ATT_FG + Kc - 1) s += win_s[q * ATT_WIN + i];
       }
       const int tt = t0 - pad + j;
-      if (tt >= 0 && tt < T) atomicAdd(p.d_ax_prev + (size_t)b * T + tt, s);
+      if (tt >= 0 && tt < Tb) atomicAdd(p.d_ax_prev + (size_t)b * T + tt, s);
     }
   }
   // ---- (iii) thread per h over the CTA's frames: partial sums, conv weight gradient ----
@@ -689,21 +704,21 @@ __global__ void __launch_bounds__(ATT_THREADS) s2s_attn_bwd_b_kernel(const AttnB
   }
   __threadfence();
   __syncthreads();
-  if (tid == 0) s_last = (atomicAdd(p.ws.cnt + b, 1u) == (unsigned int)(TS - 1));
+  if (tid == 0) s_last = (atomicAdd(p.ws.cnt + b, 1u) == (unsigned int)(TSb - 1));
   __syncthreads();
   if (!s_last) return;
   __threadfence();
   // ---- the utterance's last CTA: totals in index order, gate gradients of the cell ----
   if (tid == 0) {
     float s = 0.f;
-    for (int q = 0; q < TS; ++q) s += __ldcg(p.ws.s2 + (size_t)b * TS + q);
+    for (int q = 0; q < TSb; ++q) s += __ldcg(p.ws.s2 + (size_t)b * TS + q);
     p.g_lin_b[b] += s;
     p.ws.cnt[b] = 0u;
   }
   const float* gt = p.gates + (size_t)b * 4 * H;
   for (int h = tid; h < H; h += ATT_THREADS) {
     float gdh = 0.f, glw = 0.f;
-    for (int q = 0; q < TS; ++q) {
+    for (int q = 0; q < TSb; ++q) {
       gdh += __ldcg(p.ws.acc + ((size_t)b * TS + q) * H + h);
       glw += __ldcg(p.ws.aux + ((size_t)b * TS + q) * H + h);
     }
@@ -1017,14 +1032,15 @@ static int attn_dims_ok(int B, int T, int H, int Kc) {
   return SB_OK;
 }
 
-extern "C" int sb_s2s_attn_fwd(const float* eh, int eh_bcast, const float* hx, const float* ax_prev,
-                               const float* conv_wT, const float* conv_b, const float* lin_w,
-                               float lin_b, int log_t, int B, int T, int H, int Kc, float* sx,
-                               float* ax, const float* fc_w, const float* fc_b, int C,
-                               float* logits, long long logit_stride, float* logp, int* argmax,
-                               int* history, int hist_stride, int hist_col, int* end_count,
-                               int end_tok, const int* done, void* workspace,
-                               size_t workspace_bytes, void* stream_) {
+extern "C" int sb_s2s_attn_fwd_len(const float* eh, int eh_bcast, const float* hx,
+                                   const float* ax_prev, const float* conv_wT, const float* conv_b,
+                                   const float* lin_w, float lin_b, int log_t, int B, int T, int H,
+                                   int Kc, float* sx, float* ax, const float* fc_w,
+                                   const float* fc_b, int C, float* logits,
+                                   long long logit_stride, float* logp, int* argmax, int* history,
+                                   int hist_stride, int hist_col, int* end_count, int end_tok,
+                                   const int* done, const int* lens, void* workspace,
+                                   size_t workspace_bytes, void* stream_) {
   if (!eh || !hx || !conv_wT || !conv_b || !lin_w || !sx || !ax || !workspace) return SB_ERR_INVALID;
   int rc = attn_dims_ok(B, T, H, Kc);
   if (rc != SB_OK) return rc;
@@ -1042,21 +1058,45 @@ extern "C" int sb_s2s_attn_fwd(const float* eh, int eh_bcast, const float* hx, c
   p.conv_b = conv_b; p.lin_w = lin_w; p.lin_b = lin_b; p.sx = sx; p.ax = ax; p.fc_w = fc_w;
   p.fc_b = fc_b; p.logits = logits; p.logit_stride = logit_stride; p.logp = logp;
   p.argmax = argmax; p.history = history; p.hist_stride = hist_stride; p.hist_col = hist_col;
-  p.end_count = end_count; p.end_tok = end_tok; p.done = done;
+  p.end_count = end_count; p.end_tok = end_tok; p.done = done; p.lens = lens;
   p.ws = attn_ws_carve(workspace, B, T, H);
   p.B = B; p.T = T; p.H = H; p.Kc = Kc; p.C = C; p.log_t = log_t;
   s2s_attn_fwd_kernel<<<dim3((T + ATT_TT - 1) / ATT_TT, B), ATT_THREADS, smem, stream>>>(p);
   return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
 }
 
+extern "C" int sb_s2s_attn_fwd(const float* eh, int eh_bcast, const float* hx, const float* ax_prev,
+                               const float* conv_wT, const float* conv_b, const float* lin_w,
+                               float lin_b, int log_t, int B, int T, int H, int Kc, float* sx,
+                               float* ax, const float* fc_w, const float* fc_b, int C,
+                               float* logits, long long logit_stride, float* logp, int* argmax,
+                               int* history, int hist_stride, int hist_col, int* end_count,
+                               int end_tok, const int* done, void* workspace,
+                               size_t workspace_bytes, void* stream_) {
+  return sb_s2s_attn_fwd_len(eh, eh_bcast, hx, ax_prev, conv_wT, conv_b, lin_w, lin_b, log_t, B,
+                             T, H, Kc, sx, ax, fc_w, fc_b, C, logits, logit_stride, logp, argmax,
+                             history, hist_stride, hist_col, end_count, end_tok, done, nullptr,
+                             workspace, workspace_bytes, stream_);
+}
+
 // the standalone attention step (no output projection): NNAttention.forward on the decode path
+extern "C" int sb_attn_step_len(const float* eh, const float* dhx, const float* ax_prev,
+                                const float* conv_wT, const float* conv_b, const float* lin_w,
+                                float lin_b, int log_t, int B, int T, int H, int Kc, float* sx,
+                                float* ax, const int* lens, void* workspace,
+                                size_t workspace_bytes, void* stream_) {
+  return sb_s2s_attn_fwd_len(eh, 0, dhx, ax_prev, conv_wT, conv_b, lin_w, lin_b, log_t, B, T, H,
+                             Kc, sx, ax, nullptr, nullptr, 0, nullptr, 0, nullptr, nullptr,
+                             nullptr, 0, 0, nullptr, 0, nullptr, lens, workspace, workspace_bytes,
+                             stream_);
+}
+
 extern "C" int sb_attn_step(const float* eh, const float* dhx, const float* ax_prev,
                             const float* conv_wT, const float* conv_b, const float* lin_w,
                             float lin_b, int log_t, int B, int T, int H, int Kc, float* sx,
                             float* ax, void* workspace, size_t workspace_bytes, void* stream_) {
-  return sb_s2s_attn_fwd(eh, 0, dhx, ax_prev, conv_wT, conv_b, lin_w, lin_b, log_t, B, T, H, Kc,
-                         sx, ax, nullptr, nullptr, 0, nullptr, 0, nullptr, nullptr, nullptr, 0, 0,
-                         nullptr, 0, nullptr, workspace, workspace_bytes, stream_);
+  return sb_attn_step_len(eh, dhx, ax_prev, conv_wT, conv_b, lin_w, lin_b, log_t, B, T, H, Kc, sx,
+                          ax, nullptr, workspace, workspace_bytes, stream_);
 }
 
 extern "C" int sb_s2s_dout(const float* dlogits, const float* fc_w, const float* hx, const float* sx,
@@ -1069,15 +1109,16 @@ extern "C" int sb_s2s_dout(const float* dlogits, const float* fc_w, const float*
   return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
 }
 
-extern "C" int sb_s2s_attn_bwd(const float* eh, const float* hx, const float* hx_prev,
-                               const float* ax_prev, const float* ax, const float* conv_wT,
-                               const float* conv_b, const float* lin_w, const float* d_o,
-                               const float* d_ix_next, const float* d_ax_next,
-                               const float* d_hx_next, const float* gates, float* d_eh,
-                               float* d_ax_prev, float* d_gi, float* d_gh, float* d_hx_direct,
-                               float* g_conv_wT, float* g_conv_b, float* g_lin_w, float* g_lin_b,
-                               int log_t, int B, int T, int H, int Kc, void* workspace,
-                               size_t workspace_bytes, void* stream_) {
+extern "C" int sb_s2s_attn_bwd_len(const float* eh, const float* hx, const float* hx_prev,
+                                   const float* ax_prev, const float* ax, const float* conv_wT,
+                                   const float* conv_b, const float* lin_w, const float* d_o,
+                                   const float* d_ix_next, const float* d_ax_next,
+                                   const float* d_hx_next, const float* gates, float* d_eh,
+                                   float* d_ax_prev, float* d_gi, float* d_gh, float* d_hx_direct,
+                                   float* g_conv_wT, float* g_conv_b, float* g_lin_w,
+                                   float* g_lin_b, int log_t, int B, int T, int H, int Kc,
+                                   const int* lens, void* workspace, size_t workspace_bytes,
+                                   void* stream_) {
   if (!eh || !hx || !hx_prev || !ax || !conv_wT || !conv_b || !lin_w || !d_o || !gates || !d_eh ||
       !d_ax_prev || !d_gi || !d_gh || !d_hx_direct || !g_conv_wT || !g_conv_b || !g_lin_w ||
       !g_lin_b || !workspace)
@@ -1100,13 +1141,28 @@ extern "C" int sb_s2s_attn_bwd(const float* eh, const float* hx, const float* hx
   p.d_ix_next = d_ix_next; p.d_ax_next = d_ax_next;
   p.d_hx_next = d_hx_next; p.gates = gates; p.d_eh = d_eh; p.d_ax_prev = d_ax_prev; p.d_gi = d_gi;
   p.d_gh = d_gh; p.d_hx_direct = d_hx_direct; p.g_conv_wT = g_conv_wT;
-  p.g_conv_b = g_conv_b; p.g_lin_w = g_lin_w; p.g_lin_b = g_lin_b;
+  p.g_conv_b = g_conv_b; p.g_lin_w = g_lin_w; p.g_lin_b = g_lin_b; p.lens = lens;
   p.ws = attn_ws_carve(workspace, B, T, H);
   p.B = B; p.T = T; p.H = H; p.Kc = Kc; p.log_t = log_t;
   const dim3 grid((T + ATT_TT - 1) / ATT_TT, B);
   s2s_attn_bwd_a_kernel<<<grid, ATT_THREADS, smem_a, stream>>>(p);
   s2s_attn_bwd_b_kernel<<<grid, ATT_THREADS, smem_b, stream>>>(p);
   return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
+}
+
+extern "C" int sb_s2s_attn_bwd(const float* eh, const float* hx, const float* hx_prev,
+                               const float* ax_prev, const float* ax, const float* conv_wT,
+                               const float* conv_b, const float* lin_w, const float* d_o,
+                               const float* d_ix_next, const float* d_ax_next,
+                               const float* d_hx_next, const float* gates, float* d_eh,
+                               float* d_ax_prev, float* d_gi, float* d_gh, float* d_hx_direct,
+                               float* g_conv_wT, float* g_conv_b, float* g_lin_w, float* g_lin_b,
+                               int log_t, int B, int T, int H, int Kc, void* workspace,
+                               size_t workspace_bytes, void* stream_) {
+  return sb_s2s_attn_bwd_len(eh, hx, hx_prev, ax_prev, ax, conv_wT, conv_b, lin_w, d_o, d_ix_next,
+                             d_ax_next, d_hx_next, gates, d_eh, d_ax_prev, d_gi, d_gh, d_hx_direct,
+                             g_conv_wT, g_conv_b, g_lin_w, g_lin_b, log_t, B, T, H, Kc, nullptr,
+                             workspace, workspace_bytes, stream_);
 }
 
 extern "C" int sb_s2s_cell_bwd(const float* d_gi, const float* d_gh, const float* d_hx_direct,

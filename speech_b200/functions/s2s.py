@@ -65,28 +65,43 @@ def _cell_fwd(lib, w, tok, tok_stride, sx_prev, hx_prev, hx, ix_save, gates_save
 
 def _attn_fwd(lib, w, ws, eh, bcast, hx, ax_prev, sx, ax, B, T, sp, logits=None, logit_stride=0,
               logp=None, argmax=None, history=None, hist_stride=0, hist_col=0, end_count=None,
-              end_tok=-1, done=None, with_fc=True):
+              end_tok=-1, done=None, with_fc=True, lens=None):
     from .. import ops
     ops._launch("s2s_attn_fwd", 0.0,
-                lambda: lib.sb_s2s_attn_fwd(_a(eh), bcast, _a(hx), _a(ax_prev), w.p_conv_wT,
-                                            w.p_conv_b, w.p_lin_w, w.lin_b, w.log_t, B, T, w.H,
-                                            w.Kc, _a(sx), _a(ax),
-                                            w.p_fc_w if with_fc else None,
-                                            w.p_fc_b if with_fc else None, w.C,
-                                            logits, logit_stride, _a(logp), _a(argmax),
-                                            history, hist_stride, hist_col, end_count, end_tok,
-                                            done, _a(ws), ws.numel(), sp))
+                lambda: lib.sb_s2s_attn_fwd_len(_a(eh), bcast, _a(hx), _a(ax_prev), w.p_conv_wT,
+                                                w.p_conv_b, w.p_lin_w, w.lin_b, w.log_t, B, T, w.H,
+                                                w.Kc, _a(sx), _a(ax),
+                                                w.p_fc_w if with_fc else None,
+                                                w.p_fc_b if with_fc else None, w.C,
+                                                logits, logit_stride, _a(logp), _a(argmax),
+                                                history, hist_stride, hist_col, end_count,
+                                                end_tok, done, _a(lens), _a(ws), ws.numel(), sp))
+
+
+def attn_lens(lens, B, T, dev):
+    """(B,) int32 device frames per utterance for the length-masked attention kernels, or None
+    (every utterance attends over all T frames)."""
+    if lens is None:
+        return None
+    ln = torch.as_tensor(lens).detach().to("cpu", torch.int64).reshape(-1)
+    if ln.numel() != B:
+        raise ValueError("lens must have one entry per utterance (%d), got %d" % (B, ln.numel()))
+    if B and (int(ln.min()) < 1 or int(ln.max()) > T):
+        raise ValueError("attention lens must lie in [1, T] (T = %d)" % T)
+    if bool((ln == T).all()):
+        return None
+    return ln.to(torch.int32).to(dev)
 
 
 class DecodeFunction(torch.autograd.Function):
     """Teacher-forced decode (seq2seq.py:78-112): eh (B,T,H), tokens (B,U) -> logits (B,U-1,C),
     alignments (B,U-1,T).  sample_flags[u] (host bools, drawn by the caller from Python's `random`
     exactly as the reference does, :94): feed the arg-max of the previous step instead of the
-    label."""
+    label.  lens (optional, (B,) int32 device): frames each utterance attends over."""
 
     @staticmethod
-    def forward(ctx, eh, tokens, sample_flags, w, emb_w, w_ih, w_hh, b_ih, b_hh, conv_w, conv_b,
-                lin_w, lin_b, fc_w, fc_b):
+    def forward(ctx, eh, tokens, sample_flags, w, lens, emb_w, w_ih, w_hh, b_ih, b_hh, conv_w,
+                conv_b, lin_w, lin_b, fc_w, fc_b):
         _lib.require_cuda(eh, "encoder states")
         lib = _lib.load()
         ehc = _f(eh)
@@ -126,8 +141,9 @@ class DecodeFunction(torch.autograd.Function):
                       p_gt + 4 * u * BH if need else None, None, B, sp)
             _attn_fwd(lib, w, ws, ehc, 0, p_hx + (u + 1) * BH, p_ax + (u - 1) * BT if u > 0 else None,
                       p_sx + u * BH, p_ax + u * BT, B, T, sp, logits=p_logits + 4 * u * w.C,
-                      logit_stride=steps * w.C, argmax=p_amax)
+                      logit_stride=steps * w.C, argmax=p_amax, lens=lens)
         ctx.w = w
+        ctx.lens = lens
         ctx.saved = (ehc, hx_all, sx_all, ax_all, ix_all, gates_all, used)
         ctx.dims = (B, T, H, steps)
         ctx.vocab = emb_w.shape[0]
@@ -178,6 +194,7 @@ class DecodeFunction(torch.autograd.Function):
         p_gcw, p_gcb = g_conv_wT.data_ptr(), g_conv_b.data_ptr()
         p_glw, p_glb = g_lin_w.data_ptr(), g_lin_b.data_ptr()
         p_wihT, p_whhT, p_ws, n_ws = w_ihT.data_ptr(), w_hhT.data_ptr(), ws.data_ptr(), ws.numel()
+        p_lens = _a(ctx.lens)
         for u in reversed(range(steps)):
             last = (u == steps - 1)
             d_ax_next = None if last else p_dax[(u + 1) & 1]
@@ -186,12 +203,12 @@ class DecodeFunction(torch.autograd.Function):
                     d_ax_next = da_ext[u].data_ptr()
                 else:
                     d_ax[(u + 1) & 1].add_(da_ext[u])
-            ops._launch("s2s_attn_bwd", 0.0, lambda: lib.sb_s2s_attn_bwd(
+            ops._launch("s2s_attn_bwd", 0.0, lambda: lib.sb_s2s_attn_bwd_len(
                 p_eh, p_hx + (u + 1) * BH, p_hx + u * BH, p_ax + (u - 1) * BT if u > 0 else None,
                 p_ax + u * BT, w.p_conv_wT, w.p_conv_b, w.p_lin_w, p_do + u * BH,
                 None if last else p_dix + (u + 1) * BH, d_ax_next, None if last else p_dhp,
                 p_gt + 4 * u * BH, p_deh, p_dax[u & 1], p_dgi + 3 * u * BH, p_dgh + 3 * u * BH,
-                p_dhd, p_gcw, p_gcb, p_glw, p_glb, w.log_t, B, T, H, Kc, p_ws, n_ws, sp))
+                p_dhd, p_gcw, p_gcb, p_glw, p_glb, w.log_t, B, T, H, Kc, p_lens, p_ws, n_ws, sp))
             ops._launch("s2s_cell_bwd", 0.0, lambda: lib.sb_s2s_cell_bwd(
                 p_dgi + 3 * u * BH, p_dgh + 3 * u * BH, p_dhd, p_wihT, p_whhT, p_dix + u * BH,
                 p_dhp, B, H, sp))
@@ -221,22 +238,25 @@ class DecodeFunction(torch.autograd.Function):
         d_conv_b = g_conv_b.sum(0)
         d_lin_w = g_lin_w.sum(0).reshape(ctx.lin_shape)
         d_lin_b = g_lin_b.sum().reshape(1) if ctx.has_lin_b else None
-        return (d_eh, None, None, None, d_emb, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_conv_w, d_conv_b,
+        return (d_eh, None, None, None, None, d_emb, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_conv_w, d_conv_b,
                 d_lin_w, d_lin_b, d_fc_w, d_fc_b)
 
 
-def decode(m, eh, tokens, sample_flags):
-    """logits (B, U-1, C), alignments (B, U-1, T) with autograd through the kernels above."""
+def decode(m, eh, tokens, sample_flags, lens=None):
+    """logits (B, U-1, C), alignments (B, U-1, T) with autograd through the kernels above.
+    lens (optional): frames each utterance attends over (alignments are 0 past them)."""
     w = DecoderWeights(m)
     lin = m.attend.nn[1].fc
-    return DecodeFunction.apply(eh, tokens, sample_flags, w, m.embedding.weight,
+    ld = attn_lens(lens, eh.shape[0], eh.shape[1], eh.device)
+    return DecodeFunction.apply(eh, tokens, sample_flags, w, ld, m.embedding.weight,
                                 m.dec_rnn.weight_ih, m.dec_rnn.weight_hh, m.dec_rnn.bias_ih,
                                 m.dec_rnn.bias_hh, m.attend.conv.weight, m.attend.conv.bias,
                                 lin.weight, lin.bias, m.fc.fc.weight, m.fc.fc.bias)
 
 
-def decode_step(m, eh, y, state, softmax):
-    """One step (seq2seq.py:114-137), no autograd: y (B,1) tokens -> (out (B,C), (hx, ax, sx))."""
+def decode_step(m, eh, y, state, softmax, lens=None):
+    """One step (seq2seq.py:114-137), no autograd: y (B,1) tokens -> (out (B,C), (hx, ax, sx)).
+    lens (optional): frames each utterance attends over."""
     lib = _lib.load()
     w = DecoderWeights(m)
     ehc = _f(eh)
@@ -258,16 +278,18 @@ def decode_step(m, eh, y, state, softmax):
     logp = torch.empty(B, w.C, dtype=torch.float32, device=dev) if softmax else None
     sp = _lib.stream_ptr()
     ws = attn_workspace(lib, B, T, H, dev)
+    ld = attn_lens(lens, B, T, dev)
     _cell_fwd(lib, w, tok.data_ptr(), 1, sx_prev, hx_prev, hx, None, None, None, B, sp)
     _attn_fwd(lib, w, ws, ehc, 0, hx, ax_prev, sx, ax, B, T, sp, logits=out.data_ptr(),
-              logit_stride=w.C, logp=logp)
+              logit_stride=w.C, logp=logp, lens=ld)
     return (logp if softmax else out), (hx, ax, sx.unsqueeze(1))
 
 
-def greedy(m, eh, start, end_tok, max_len):
+def greedy(m, eh, start, end_tok, max_len, lens=None):
     """Greedy decode (seq2seq.py:145-178) without leaving the device: every kernel of every step
     is enqueued up front, kernels after the stop condition (all rows emitted end_tok in the same
-    step, :155-156) are no-ops, ONE device->host copy returns the tokens.  -> (B, steps+1) list."""
+    step, :155-156) are no-ops, ONE device->host copy returns the tokens.  -> (B, steps+1) list.
+    lens (optional): frames each utterance attends over."""
     lib = _lib.load()
     w = DecoderWeights(m)
     ehc = _f(eh)
@@ -282,6 +304,7 @@ def greedy(m, eh, start, end_tok, max_len):
     ax = [torch.empty(B, T, dtype=torch.float32, device=dev) for _ in range(2)]
     sp = _lib.stream_ptr()
     ws = attn_workspace(lib, B, T, H, dev)
+    ld = attn_lens(lens, B, T, dev)
     from .. import ops
     for e in range(max_len):
         cur, prv = e & 1, (e & 1) ^ 1
@@ -289,7 +312,8 @@ def greedy(m, eh, start, end_tok, max_len):
                   hx[prv], hx[cur], None, None, done.data_ptr(), B, sp)
         _attn_fwd(lib, w, ws, ehc, 0, hx[cur], ax[prv] if e > 0 else None, sx[cur], ax[cur], B, T, sp,
                   history=hist.data_ptr(), hist_stride=max_len + 1, hist_col=e + 1,
-                  end_count=ctl.data_ptr() + 4 * e, end_tok=int(end_tok), done=done.data_ptr())
+                  end_count=ctl.data_ptr() + 4 * e, end_tok=int(end_tok), done=done.data_ptr(),
+                  lens=ld)
         ops._launch("s2s_check_done", 0.0,
                     lambda: lib.sb_s2s_check_done(ctl.data_ptr() + 4 * e, B, done.data_ptr(),
                                                   nsteps.data_ptr(), e + 1, sp))

@@ -21,36 +21,45 @@ class CTC(model.Model):
             return batch.tensors()
         return self.collate(*batch)
 
+    def _forward_impl(self, x, lens, softmax=False):
+        # without lengths, the call the default mode has always made
+        if lens is None:
+            return self.forward_impl(x, softmax=softmax) if softmax else self.forward_impl(x)
+        return self.forward_impl(x, softmax=softmax, lens=lens)
+
     def forward(self, batch):
         x, y, x_lens, y_lens = self._collated(batch)
         with self._grad_ctx():
-            return self.forward_impl(x)
+            return self._forward_impl(x, self.exact_lens(x_lens))
 
-    def forward_impl(self, x, softmax=False):
+    def forward_impl(self, x, softmax=False, lens=None):
         if self.is_cuda:
             x = x.cuda(non_blocking=True)
-        x = self.encode_logits(x)
+        x = self.encode_logits(x) if lens is None else self.encode_logits(x, lens)
         if softmax:
             return torch.nn.functional.softmax(x, dim=2)
         return x
 
-    def encode_logits(self, x):
+    def encode_logits(self, x, lens=None):
         """encode + fc with the halves-sum and the projection fused into one contraction on the
-        bf16 top-layer output (same math as model.py:75-77 followed by ctc_model.py:29)."""
+        bf16 top-layer output (same math as model.py:75-77 followed by ctc_model.py:29).
+        lens (optional): valid frames per utterance (exact-lengths mode, Model.encode)."""
         from .. import _lib, ops
         _lib.require_cuda(x, "forward_impl() input")
         if getattr(self, "parity_mode", False) and not torch.is_grad_enabled():
+            if lens is not None:
+                raise NotImplementedError("parity_mode does not support exact_lengths")
             # reference-precision forward (split-bf16 GEMMs, fp32 recurrence): a measuring stick
             # for the bf16 operand path, see ops.encode_logits_parity
             return ops.encode_logits_parity(x, self.conv, self.rnn, self.fc.fc)
         x = ops.conv_stack(x, self.conv, self.training)
         p = self.rnn.dropout if self.training else 0.0
-        return ops.gru_stack_logits(x, self.rnn, self.fc.fc, dropout=p)
+        return ops.gru_stack_logits(x, self.rnn, self.fc.fc, dropout=p, lens=lens)
 
     def loss(self, batch):
         x, y, x_lens, y_lens = self._collated(batch)
         with self._grad_ctx():
-            out = self.forward_impl(x)
+            out = self._forward_impl(x, self.exact_lens(x_lens))
             return self.ctc_loss(out, y, x_lens, y_lens)
 
     def ctc_loss(self, out, y, x_lens, y_lens):
@@ -62,9 +71,10 @@ class CTC(model.Model):
 
     def infer(self, batch, beam_size=1):
         x, y, x_lens, y_lens = self._collated(batch)
+        lens = self.exact_lens(x_lens)
         with torch.no_grad():
-            probs = self.forward_impl(x, softmax=True)
-        return decode_batch(probs, beam_size=beam_size, blank=self.blank)
+            probs = self._forward_impl(x, lens, softmax=True)
+        return decode_batch(probs, beam_size=beam_size, blank=self.blank, lens=lens)
 
     @staticmethod
     def max_decode(pred, blank):

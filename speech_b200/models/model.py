@@ -18,6 +18,12 @@ from .. import _lib, ops
 
 class Model(nn.Module):
 
+    # Exact-lengths mode (config key "exact_lengths"; off by default, as in the reference): every
+    # utterance is encoded, scored and decoded over its own frames, len_b = conv_out_size(T_b, 0),
+    # so its results do not depend on the other utterances of its minibatch.  A class attribute,
+    # so that pickles written before the key existed read it as False.
+    exact_lengths = False
+
     def __init__(self, input_dim, config):
         super().__init__()
         self.input_dim = input_dim
@@ -41,6 +47,7 @@ class Model(nn.Module):
                           dropout=config["dropout"], bidirectional=rnn_cfg["bidirectional"])
         self._encoder_dim = rnn_cfg["dim"]
         self.volatile = False
+        self.exact_lengths = bool(config.get("exact_lengths", False))
 
     # reference: model.py:44-52 (valid convolution, ceil((n - k + 1) / s) per layer)
     def conv_out_size(self, n, dim):
@@ -59,12 +66,14 @@ class Model(nn.Module):
     def infer(self, batch):
         raise NotImplementedError
 
-    def encode(self, x):
-        """x (B, T, F) float32 on the CUDA device -> (B, T', encoder_dim)   (model.py:60-79)."""
+    def encode(self, x, lens=None):
+        """x (B, T, F) float32 on the CUDA device -> (B, T', encoder_dim)   (model.py:60-79).
+        lens (optional): valid output frames per utterance (x_lens of the exact-lengths mode);
+        states at frames < lens[b] are then those of the utterance alone, later frames are zero."""
         _lib.require_cuda(x, "encode() input")
         x = ops.conv_stack(x, self.conv, self.training)          # (B, T', C*F') c-major features
         p = self.rnn.dropout if self.training else 0.0
-        x = ops.gru_stack(x, self.rnn, dropout=p)                 # (B, T', ndir*H)
+        x = ops.gru_stack(x, self.rnn, dropout=p, lens=lens)     # (B, T', ndir*H)
         if self.rnn.bidirectional:
             half = x.shape[-1] // 2
             x = x[:, :, :half] + x[:, :, half:]
@@ -97,12 +106,28 @@ class Model(nn.Module):
     def lattice_batch(self, inputs, labels):
         """[x, flat int32 labels, x_lens, y_lens] as the CTC and transducer losses take them
         (ctc_model.py:42-53, transducer_model.py:79-90): every utterance is scored over the
-        padded T', labels and lengths stay on the host."""
-        frames = self.conv_out_size(max(i.shape[0] for i in inputs), 0)
-        x_lens = torch.full((len(inputs),), frames, dtype=torch.int32)
+        padded T' - or, in the exact-lengths mode, over its own conv_out_size(T_b) frames; labels
+        and lengths stay on the host."""
+        if self.exact_lengths:
+            # the valid conv makes these frames exact: output frame t reads input frames
+            # <= t*s + k - 1 <= T_b - 1 in every layer
+            x_lens = torch.tensor([max(0, self.conv_out_size(i.shape[0], 0)) for i in inputs],
+                                  dtype=torch.int32)
+        else:
+            frames = self.conv_out_size(max(i.shape[0] for i in inputs), 0)
+            x_lens = torch.full((len(inputs),), frames, dtype=torch.int32)
         y_lens = torch.tensor([len(seq) for seq in labels], dtype=torch.int32)
         flat = torch.tensor([int(tok) for seq in labels for tok in seq], dtype=torch.int32)
         return [self.stage_inputs(inputs), flat, x_lens, y_lens]
+
+    def _encode(self, x, lens):
+        # without lengths, call encode exactly as the default mode always has (callers may
+        # substitute a one-argument encode, e.g. to feed precomputed encoder states)
+        return self.encode(x) if lens is None else self.encode(x, lens)
+
+    def exact_lens(self, x_lens):
+        """x_lens for the encoder in the exact-lengths mode, else None (the reference's padding)."""
+        return x_lens if self.exact_lengths else None
 
     def _grad_ctx(self):
         # the reference marks eval batches `volatile`; on modern torch that is no_grad

@@ -49,44 +49,54 @@ class Seq2Seq(model.Model):
             y = y.cuda(non_blocking=True)
         return x, y
 
+    def input_lens(self, inputs):
+        """Exact-lengths mode: encoder frames conv_out_size(T_b) of every utterance, which the
+        encoder and the attention then keep to; None in the default (padded) mode."""
+        if not self.exact_lengths:
+            return None
+        return [max(0, self.conv_out_size(i.shape[0], 0)) for i in inputs]
+
     def loss(self, batch):
+        lens = self.input_lens(batch[0])
         x, y = self.collate(*batch)
         x, y = self._to_dev(x, y)
         with self._grad_ctx():
-            out, _ = self.forward_impl(x, y)
+            out, _ = self.forward_impl(x, y) if lens is None else self.forward_impl(x, y, lens)
             bsz, _, out_dim = out.shape
             ce = nn.functional.cross_entropy(out.reshape(-1, out_dim), y[:, 1:].reshape(-1),
                                              reduction="sum")
             # (1,)-shaped so that train.py:33 `loss.data[0]` works on current torch
             return (ce / bsz).reshape(1)
 
-    def forward_impl(self, x, y):
-        x = self.encode(x)
-        return self.decode(x, y)
+    def forward_impl(self, x, y, lens=None):
+        x = self._encode(x, lens)
+        return self.decode(x, y) if lens is None else self.decode(x, y, lens)
 
     def forward(self, batch):
+        lens = self.input_lens(batch[0])
         x, y = self.collate(*batch)
         x, y = self._to_dev(x, y)
         with self._grad_ctx():
-            return self.forward_impl(x, y)[0]
+            return (self.forward_impl(x, y) if lens is None else self.forward_impl(x, y, lens))[0]
 
-    def decode(self, x, y):
+    def decode(self, x, y, lens=None):
         """Teacher-forced decode (:78-112).  x (B, T', H); y (B, U) -> logits (B, U-1, V-1),
         alignments (B, U-1, T').  The scheduled-sampling coin flips are drawn here from Python's
         `random` in the reference's order (:93-94: one draw per step after the first, only while
-        sampling is on); the steps themselves run on the device."""
+        sampling is on); the steps themselves run on the device.  lens (optional): frames each
+        utterance attends over."""
         from ..functions import s2s
         steps = y.shape[1] - 1
         flags = [False] * max(steps, 1)
         if self.scheduled_sampling:
             for t in range(1, steps):
                 flags[t] = random.random() < self.sample_prob
-        return s2s.decode(self, x, y, flags)
+        return s2s.decode(self, x, y, flags, lens)
 
-    def decode_step(self, x, y, state=None, softmax=False):
+    def decode_step(self, x, y, state=None, softmax=False, lens=None):
         """One decoder step (:114-137).  y (B, 1) -> (logits (B, V-1), (hx, ax, sx))."""
         from ..functions import s2s
-        return s2s.decode_step(self, x, y, state, softmax)
+        return s2s.decode_step(self, x, y, state, softmax, lens)
 
     def predict(self, batch):
         probs = self(batch)
@@ -108,12 +118,13 @@ class Seq2Seq(model.Model):
         """Greedy decode (:162-178): the start token, then arg-max until every row emitted end in
         the same step; device-resident (functions/s2s.py: greedy)."""
         from ..functions import s2s
+        lens = self.input_lens(batch[0])
         x, y = self.collate(*batch)
         end_tok = int(y[0, -1])
         x, y = self._to_dev(x, y)
         with torch.no_grad():
-            x = self.encode(x)
-            return s2s.greedy(self, x, y[:, 0], end_tok, max_len)
+            x = self._encode(x, lens)
+            return s2s.greedy(self, x, y[:, 0], end_tok, max_len, lens)
 
     def beam_search(self, batch, beam_size=10, max_len=200):
         """Beam search for ONE utterance (:180-227).  Hypothesis scores are sums of log-softmax
@@ -146,7 +157,7 @@ class NNAttention(nn.Module):
         self.nn = nn.Sequential(nn.ReLU(), model.LinearND(n_channels, 1))
         self.log_t = log_t
 
-    def forward(self, eh, dhx, ax=None):
+    def forward(self, eh, dhx, ax=None, lens=None):
         """(sx (B,1,H), ax (B,T)) of one attention step on the fused kernel (csrc/s2s.cu).  The
         module is a parameter container for the decoder: training differentiates the whole
         decode through functions/s2s.py, so this stand-alone call carries no autograd."""
@@ -154,4 +165,4 @@ class NNAttention(nn.Module):
         if torch.is_grad_enabled() and (eh.requires_grad or dhx.requires_grad):
             raise RuntimeError("NNAttention.forward is inference-only; gradients flow through "
                                "Seq2Seq.decode (speech_b200.functions.s2s)")
-        return ops.attn_step(eh, dhx, ax, self.conv, self.nn[1].fc, self.log_t)
+        return ops.attn_step(eh, dhx, ax, self.conv, self.nn[1].fc, self.log_t, lens)

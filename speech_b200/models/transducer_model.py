@@ -36,13 +36,15 @@ class Transducer(model.Model):
         x, y, x_lens, y_lens = self.collate(*batch)
         y_mat = self.label_collate(batch[1])
         with self._grad_ctx():
-            return self.forward_impl(x, y_mat)
+            lens = self.exact_lens(x_lens)
+            return self.forward_impl(x, y_mat) if lens is None else \
+                self.forward_impl(x, y_mat, lens=lens)
 
-    def forward_impl(self, x, y):
+    def forward_impl(self, x, y, lens=None):
         if self.is_cuda:
             x = x.cuda(non_blocking=True)
             y = y.cuda(non_blocking=True)
-        return self.decode(self.encode(x), y)
+        return self.decode(self._encode(x, lens), y)
 
     def loss(self, batch):
         x, y, x_lens, y_lens = self.collate(*batch)
@@ -51,7 +53,10 @@ class Transducer(model.Model):
             if self.is_cuda:
                 x = x.cuda(non_blocking=True)
                 y_mat = y_mat.cuda(non_blocking=True)
-            fx, fy = self.joint_inputs(self.encode(x), y_mat)
+            # in the exact-lengths mode x_lens are the utterances' own frames: the loss gives
+            # frames >= x_lens[b] exactly zero gradient (sb_rnnt_fwd_bwd_compact), and so does
+            # the encoder
+            fx, fy = self.joint_inputs(self._encode(x, self.exact_lens(x_lens)), y_mat)
             fc2 = self.fc2.fc
             return transducer_fn.JointTransducerLoss(blank=self.blank)(
                 fx, fy, fc2.weight, fc2.bias, y_mat, y, x_lens, y_lens)
@@ -78,12 +83,16 @@ class Transducer(model.Model):
 
     def infer(self, batch, beam_size=4):
         """Beam search on the TEACHER-FORCED lattice, as the reference does (:92-101), including
-        its use of the un-subsampled input length as the time bound (clamped by slicing)."""
+        its use of the un-subsampled input length as the time bound (clamped by slicing); in the
+        exact-lengths mode the bound is each utterance's own conv_out_size(T_b) frames."""
         with torch.no_grad():
             out = self(batch)                                  # (B, T', U+1, V+1) on the device
         # the reference slices lp[:T, :U] per utterance with the UN-subsampled T (clamped by
         # numpy slicing to T') and U = labels + 1; the search itself runs batched on the GPU
-        tlens = [min(i.shape[0], out.shape[1]) for i in batch[0]]
+        if self.exact_lengths:
+            tlens = [max(0, self.conv_out_size(i.shape[0], 0)) for i in batch[0]]
+        else:
+            tlens = [min(i.shape[0], out.shape[1]) for i in batch[0]]
         ulens = [len(l) + 1 for l in batch[1]]
         preds, _ = decode_static_batch(out, tlens, ulens, beam_size, self.blank)
         return preds

@@ -330,6 +330,52 @@ def _grad_sink(param, rows=None):
     return g if rows is None else g[rows[0]:rows[1]]
 
 
+def time_align(src, lens_dev, T, Bp, right, out=None):
+    """Per-utterance shift of the rows of a time-major [T*Bp][cols] matrix (row m = t*Bp + b):
+    right=True moves row (t, b) to (t + T - len_b, b), right=False moves it back; vacated rows are
+    zero.  src / out may be column blocks of wider matrices; lens_dev: (Bp,) int32 on the device."""
+    lib = _lib.load()
+    M, cols = src.shape
+    assert M == T * Bp and src.stride(1) == 1 and src.dtype in (torch.bfloat16, torch.float32)
+    if out is None:
+        out = torch.empty(M, cols, dtype=src.dtype, device=src.device)
+    assert out.shape == src.shape and out.dtype == src.dtype and out.stride(1) == 1
+    sp = _lib.stream_ptr()
+    _launch("time_align", 0.0,
+            lambda: lib.sb_time_align(src.data_ptr(), src.stride(0), out.data_ptr(), out.stride(0),
+                                      lens_dev.data_ptr(), T, Bp, cols, src.element_size(),
+                                      1 if right else 0, sp))
+    return out
+
+
+def _align_reverse(a, lens_dev, T, Bp, half, right):
+    """[M][2*half] with its reverse-direction half (columns half..) aligned (see time_align)."""
+    out = torch.empty_like(a)
+    out[:, :half].copy_(a[:, :half])
+    time_align(a[:, half:], lens_dev, T, Bp, right, out=out[:, half:])
+    return out
+
+
+def _lens_operands(lens, B, T, Bp, dev):
+    """Exact-lengths mode of the GRU stack: (Bp,) int32 device lengths (padding rows of the batch
+    count as full length) and the (B, T, 1) f32 mask of valid frames, or None when every utterance
+    fills the padded T (nothing to align or mask)."""
+    if lens is None:
+        return None
+    ln = torch.as_tensor(lens).detach().to("cpu", torch.int64).reshape(-1)
+    if ln.numel() != B:
+        raise ValueError("lens must have one entry per utterance (%d), got %d" % (B, ln.numel()))
+    if B and (int(ln.min()) < 0 or int(ln.max()) > T):
+        raise ValueError("lens must lie in [0, T] (T = %d)" % T)
+    if bool((ln == T).all()):
+        return None
+    full = torch.full((Bp,), T, dtype=torch.int32)
+    full[:B] = ln.to(torch.int32)
+    lens_dev = full.pin_memory().to(dev, non_blocking=True)
+    valid = (torch.arange(T, device=dev)[None, :] < lens_dev[:B, None].long())
+    return lens_dev, valid.unsqueeze(2).float()
+
+
 def _workspace(nbytes, dev):
     """1024-byte aligned scratch for one recurrence launch (counters + exchange tiles)"""
     buf = torch.empty(nbytes + 1024, dtype=torch.uint8, device=dev)
@@ -343,10 +389,17 @@ class GRUStackFunction(torch.autograd.Function):
     forward(x (B,T,In) f32 cuda, ndir, H, train, *weights) -> (B,T,ndir*H) f32
     weights: per layer, per direction: w_ih (3H,In_l), w_hh (3H,H), b_ih (3H), b_hh (3H)
     (the parameter order of nn.GRU: weight_ih_l{k}[_reverse], weight_hh_..., bias_ih_..., bias_hh_...)
+
+    lens (optional, B ints): valid frames per utterance, the semantics of nn.GRU over
+    pack_padded_sequence.  The reverse direction runs on right-aligned operands (time_align), so
+    it starts at each utterance's own last frame; its gates and states stay in those aligned
+    coordinates for the backward pass, and its half of each layer output is left-aligned again.
+    The gradient arriving at output frames >= len_b is ignored (and without the fused projection
+    those output rows are zero), so frames >= len_b of x receive exactly zero gradient.
     """
 
     @staticmethod
-    def forward(ctx, x, ndir, H, dropout, fc_w, fc_b, *weights):
+    def forward(ctx, x, ndir, H, dropout, fc_w, fc_b, lens, *weights):
         """fc_w/fc_b (optional): fuse `LinearND(sum of direction halves)` (reference
         model.py:75-77 + ctc_model.py:29) as ONE contraction on the bf16 top-layer output:
         (h_f + h_b) W^T = [h_f | h_b] [W | W]^T, written batch-first by the GEMM epilogue."""
@@ -360,7 +413,12 @@ class GRUStackFunction(torch.autograd.Function):
             raise _lib.SpeechB200Error("per-GPU batch > 128 not supported by the GRU kernel yet")
         M = T * Bp
         D = ndir * H
+        K3 = 3 * H
         need_grad = any(ctx.needs_input_grad)     # all False under torch.no_grad()
+        lo = _lens_operands(lens, B, T, Bp, dev)
+        al, valid = lo if lo is not None else (None, None)
+        if ndir == 1:
+            al = None                             # the forward direction is causal
 
         # layer-0 operand: time-major, batch padded, K padded to a multiple of 8, bf16
         Inp = _round_up(In, 8)
@@ -398,7 +456,14 @@ class GRUStackFunction(torch.autograd.Function):
                     whh[d].copy_(w_hh[d].detach())
                 bih_cat = torch.cat([b.detach() for b in b_ih]).float().contiguous()
                 bhh = torch.stack([b.detach() for b in b_hh]).float().contiguous()
-            gi = gemm_bf16_tn(X, wih_cat, bias=bih_cat)
+            if al is None:
+                gi = gemm_bf16_tn(X, wih_cat, bias=bih_cat)
+            else:
+                # the reverse projection reads the right-aligned layer input
+                gi = torch.empty(M, 2 * K3, dtype=torch.float32, device=dev)
+                gemm_bf16_tn(X, wih_cat[:K3], out=gi[:, :K3], bias=bih_cat[:K3])
+                gemm_bf16_tn(time_align(X, al, T, Bp, right=True), wih_cat[K3:], out=gi[:, K3:],
+                             bias=bih_cat[K3:])
             y = torch.empty(M, D, dtype=torch.float32, device=dev)
             xn = torch.empty(M, D, dtype=torch.bfloat16, device=dev)
             gates = None
@@ -411,6 +476,11 @@ class GRUStackFunction(torch.autograd.Function):
                                            ws.data_ptr(), nbytes.value, T, Bp, H, ndir, sp))
             mask = None
             hb = xn                                     # bf16 h_t (un-masked): dW_hh operand
+            y_rec = y                                   # as the recurrence wrote it (backward)
+            if al is not None:
+                xn = _align_reverse(xn, al, T, Bp, H, right=False)
+                if (dropout > 0.0 and l + 1 < L) or (l + 1 == L and fc_w is None):
+                    y = _align_reverse(y, al, T, Bp, H, right=False)
             if dropout > 0.0 and l + 1 < L:
                 # inter-layer dropout of nn.GRU(dropout=p): applied to every layer output but the last
                 mask = (torch.rand(M, D, device=dev) >= dropout).float() * (1.0 / (1.0 - dropout))
@@ -418,12 +488,13 @@ class GRUStackFunction(torch.autograd.Function):
                 # fp32 state and round once
                 xn = (y * mask).to(torch.bfloat16)
             if need_grad:
-                saved.append((X, y, gates, mask, wih_cat, whh, hb))
+                saved.append((X, y_rec, gates, mask, wih_cat, whh, hb))
             X = xn
         ctx.saved = saved
         ctx.announce = _announce
         ctx.weights = weights
         ctx.dims = (B, T, In, Bp, H, ndir, L)
+        ctx.lens = (al, valid)
         ctx.fc = None
         if fc_w is not None:
             V = fc_w.shape[0]
@@ -436,6 +507,8 @@ class GRUStackFunction(torch.autograd.Function):
             ctx.fc = (fc_w, X)
             return out
         out = y.view(T, Bp, D)[:, :B].transpose(0, 1).contiguous()
+        if valid is not None:
+            out.mul_(valid)
         return out
 
     @staticmethod
@@ -449,6 +522,9 @@ class GRUStackFunction(torch.autograd.Function):
         M = T * Bp
         D = ndir * H
         K3 = 3 * H
+        al, valid = ctx.lens
+        if valid is not None:
+            dout = dout * valid
         dfc_w = dfc_b = None
         if ctx.fc is not None:
             fc_w, Xtop = ctx.fc
@@ -482,6 +558,8 @@ class GRUStackFunction(torch.autograd.Function):
             X, y, gates, mask, wih_cat, whh, hb = ctx.saved[l]
             if mask is not None:
                 dY = dY * mask
+            if al is not None:
+                dY = _align_reverse(dY, al, T, Bp, H, right=True)
             wl = weights[l * 4 * ndir:(l + 1) * 4 * ndir]
             Kl = X.shape[1]
             In_l = wl[0].shape[1]
@@ -496,6 +574,9 @@ class GRUStackFunction(torch.autograd.Function):
                                                  dbih.data_ptr(), dbhh.data_ptr(), ws.data_ptr(),
                                                  nbytes.value, T, Bp, H, ndir, sp))
             base = l * 4 * ndir
+            # dW_hh pairs dgi with the states in the recurrence's coordinates; dW_ih and dX pair
+            # it with the layer input, where the reverse half is left-aligned
+            dgi_x = dgi if al is None else _align_reverse(dgi, al, T, Bp, K3, right=False)
             # ---- weight gradients: contract the token-major operands over their rows ----
             Ms = M - Bp                      # tokens that have a predecessor in the recurrence
             for d in range(ndir):
@@ -503,7 +584,7 @@ class GRUStackFunction(torch.autograd.Function):
                 sink = _grad_sink(wl[d * 4])
                 dwih = sink if sink is not None else \
                     torch.zeros(K3, In_l, dtype=torch.float32, device=dev)
-                gemm_bf16_tn(dgi[:, d * K3:(d + 1) * K3], X[:, :In_l], out=dwih,
+                gemm_bf16_tn(dgi_x[:, d * K3:(d + 1) * K3], X[:, :In_l], out=dwih,
                              accumulate=True, a_mn=True, b_mn=True)
                 # dW_hh[d] = [dgi_r | dgi_z | dghn]^T h_prev: h_prev of token (t, b) is token
                 # (t-1, b) in the forward direction and (t+1, b) in the reverse one, so the
@@ -540,12 +621,12 @@ class GRUStackFunction(torch.autograd.Function):
             # ---- gradient w.r.t. the layer input ----
             if l > 0 or ctx.needs_input_grad[0]:
                 # dX = dgi W_ih: W_ih (3H x In) is the [K][N] form of the B operand
-                dY = gemm_bf16_tn(dgi, wih_cat, b_mn=True)                # [M][Kl] f32
+                dY = gemm_bf16_tn(dgi_x, wih_cat, b_mn=True)              # [M][Kl] f32
         dx = None
         if ctx.needs_input_grad[0]:
             dx = dY.view(T, Bp, -1)[:, :B, :In].transpose(0, 1).contiguous()
         ctx.saved = None
-        return (dx, None, None, None, dfc_w, dfc_b) + tuple(grads)
+        return (dx, None, None, None, dfc_w, dfc_b, None) + tuple(grads)
 
 
 def _gru_weights(rnn):
@@ -564,33 +645,39 @@ def _gru_weights(rnn):
 GRU_MAX_BATCH = 128   # rows one recurrence launch keeps resident (gru.cu)
 
 
-def _batch_chunks(x, fn):
+def _batch_chunks(x, lens, fn):
     """The recurrence is independent across utterances, so a minibatch larger than one launch
-    holds is run as consecutive chunks of <= GRU_MAX_BATCH rows (exact, autograd sees a cat)."""
+    holds is run as consecutive chunks of <= GRU_MAX_BATCH rows (exact, autograd sees a cat);
+    `lens` (optional) is sliced with the batch."""
     global _announce
     if x.shape[0] <= GRU_MAX_BATCH:
-        return fn(x)
+        return fn(x, lens)
     _announce = False     # several backward passes add into the same .grad: none of them is final
     try:
-        return torch.cat([fn(x[i:i + GRU_MAX_BATCH])
+        return torch.cat([fn(x[i:i + GRU_MAX_BATCH],
+                             None if lens is None else lens[i:i + GRU_MAX_BATCH])
                           for i in range(0, x.shape[0], GRU_MAX_BATCH)], 0)
     finally:
         _announce = True
 
 
-def gru_stack_logits(x, rnn, fc, dropout=0.0):
+def gru_stack_logits(x, rnn, fc, dropout=0.0, lens=None):
     """GRU stack + sum of direction halves + output projection `fc` (an nn.Linear), fused:
-    returns logits (B, T, V) - the encoder tail of CTC.forward_impl (ctc_model.py:25-32)."""
+    returns logits (B, T, V) - the encoder tail of CTC.forward_impl (ctc_model.py:25-32).
+    lens (optional): valid frames per utterance (GRUStackFunction); logits are exact at frames
+    < lens[b]."""
     ndir, weights = _gru_weights(rnn)
-    return _batch_chunks(x, lambda xc: GRUStackFunction.apply(
-        xc, ndir, rnn.hidden_size, float(dropout), fc.weight, fc.bias, *weights))
+    return _batch_chunks(x, lens, lambda xc, lc: GRUStackFunction.apply(
+        xc, ndir, rnn.hidden_size, float(dropout), fc.weight, fc.bias, lc, *weights))
 
 
-def gru_stack(x, rnn, dropout=0.0):
-    """Run the sm_90a GRU stack with the parameters of an nn.GRU module (batch_first, h0 = 0)."""
+def gru_stack(x, rnn, dropout=0.0, lens=None):
+    """Run the sm_90a GRU stack with the parameters of an nn.GRU module (batch_first, h0 = 0).
+    lens (optional): valid frames per utterance, as nn.GRU over pack_padded_sequence followed by
+    pad_packed_sequence (GRUStackFunction)."""
     ndir, weights = _gru_weights(rnn)
-    return _batch_chunks(x, lambda xc: GRUStackFunction.apply(
-        xc, ndir, rnn.hidden_size, float(dropout), None, None, *weights))
+    return _batch_chunks(x, lens, lambda xc, lc: GRUStackFunction.apply(
+        xc, ndir, rnn.hidden_size, float(dropout), None, None, lc, *weights))
 
 
 def _transpose_bf16(src, rows_pad=8, out=None):
@@ -763,9 +850,10 @@ def beam_topk(scores, k):
     return idx.cpu().tolist(), val.cpu().tolist()
 
 
-def attn_step(eh, dhx, ax_prev, conv, lin, log_t):
+def attn_step(eh, dhx, ax_prev, conv, lin, log_t, lens=None):
     """Fused NNAttention forward for the decode path (no autograd).  eh (B,T,H), dhx (B,1,H) or
-    (B,H), ax_prev (B,T) or None; conv = nn.Conv1d(1,H,Kc), lin = nn.Linear(H,1).
+    (B,H), ax_prev (B,T) or None; conv = nn.Conv1d(1,H,Kc), lin = nn.Linear(H,1); lens (optional):
+    frames each utterance attends over (ax is 0 past them).
     Returns (sx (B,1,H), ax (B,T)) like the reference module."""
     _lib.require_cuda(eh, "eh")
     lib = _lib.load()
@@ -781,11 +869,12 @@ def attn_step(eh, dhx, ax_prev, conv, lin, log_t):
     sx = torch.empty(B, H, dtype=torch.float32, device=eh.device)
     ax = torch.empty(B, T, dtype=torch.float32, device=eh.device)
     sp = _lib.stream_ptr()
-    from .functions.s2s import attn_workspace
+    from .functions.s2s import attn_lens, attn_workspace
     ws = attn_workspace(lib, B, T, H, eh.device)
+    ld = attn_lens(lens, B, T, eh.device)
     _launch("attn_step", 0.0,
-            lambda: lib.sb_attn_step(eh.data_ptr(), d.data_ptr(), _lib.ptr(axp), cw.data_ptr(),
-                                     cb.data_ptr(), lw.data_ptr(), lb, 1 if log_t else 0, B, T, H,
-                                     Kc, sx.data_ptr(), ax.data_ptr(), ws.data_ptr(), ws.numel(),
-                                     sp))
+            lambda: lib.sb_attn_step_len(eh.data_ptr(), d.data_ptr(), _lib.ptr(axp), cw.data_ptr(),
+                                         cb.data_ptr(), lw.data_ptr(), lb, 1 if log_t else 0, B, T,
+                                         H, Kc, sx.data_ptr(), ax.data_ptr(), _lib.ptr(ld),
+                                         ws.data_ptr(), ws.numel(), sp))
     return sx.unsqueeze(1), ax

@@ -29,4 +29,12 @@ t2 = Transducer(80, 300, cfg).cuda()       # V+1 = 301: the large-vocabulary joi
 labels2 = [np.random.randint(0, 300, 7 + i).tolist() for i in range(5)]
 l4 = t2.loss((inputs, labels2)); l4.backward()
 print("transducer V+1=301 ok", l4.item(), [len(p) for p in t2.infer((inputs, labels2))])
+cfg_x = dict(cfg, exact_lengths=True)          # per-utterance lengths through every layer
+for cls in (CTC, Transducer):
+    mx = cls(80, 28, cfg_x).cuda()
+    lx = mx.loss((inputs, labels)); lx.backward()
+    print("exact lengths", cls.__name__, lx.item(), [len(p) for p in mx.infer((inputs, labels))])
+sx = Seq2Seq(80, 30, cfg_x).cuda()
+l5 = sx.loss((inputs, lab2)); l5.backward()
+print("exact lengths Seq2Seq", l5.item(), [len(h) for h in sx.infer((inputs, lab2), max_len=12)])
 torch.cuda.synchronize()
