@@ -119,6 +119,13 @@ int sb_gru_bwd(const float* dy, const float* y, const float* gates, const void* 
                void* dgi_bf16, void* dghn_bf16, float* dbih, float* dbhh, void* workspace,
                size_t workspace_bytes, int T, int Bp, int H, int ndir, void* stream);
 
+/* Width Hp >= H at which sb_gru_fwd / sb_gru_bwd run a layer of H hidden units: H rounded up to
+ * a multiple of 16, if both calls accept that width: the constraints above, the shared-memory
+ * ring of each pass and the co-residency of its grid on the current device (SB_ERR_UNSUPPORTED
+ * otherwise; the answer needs a CUDA device).  The caller pads the layer with Hp - H zero units per direction (zero W_ih / W_hh rows, W_hh
+ * columns and biases; zero W_ih columns of the next layer): they stay exactly 0 for all t. */
+int sb_gru_plan(int Bp, int H, int ndir, int* Hp);
+
 /* Per-utterance time alignment of a block of columns of a time-major [T*Bp][ld] matrix (row
  * m = t*Bp + b), for the exact-lengths mode of the GRU stack (csrc/lengths.cu):
  *   right != 0: row (t, b) moves to (t + T - len_b, b)  (each utterance ends at frame T-1)
@@ -334,9 +341,13 @@ int sb_rnnt_fwd_bwd_compact(const float* lat, float* garc, const int* labels,
  *   sb_rnnt_joint_build_slab / _reduce_slab: the hidden activations of Tc <= 8 frames
  *                           (z [B*Tc*U1][H] bf16) for the weight-gradient GEMMs, and the masked
  *                           reduction of dz [B*Tc*U1][H] f32 into dfx (=) and dfy (+=)
- * Constraints: H % 8 == 0, V1 <= 64.  Larger vocabularies (V1 > 64) go through the slab path
- * below: build_slab, sb_gemm_bf16_tn for the logits, and sb_rnnt_joint_vocab_fwd_rows / _bwd_rows.
+ * Constraints: H % 8 == 0, V1 <= 64, and fc2's weight must fit in shared memory next to the
+ * operand ring (H <= 1792 for V1 <= 32, H <= 1024 for V1 <= 64): sb_rnnt_joint_resident(H, V1)
+ * answers 1 exactly for the shapes sb_rnnt_joint_fwd / _dlogits run (pure host arithmetic).  Every
+ * other shape goes through the slab path below: build_slab, sb_gemm_bf16_tn for the logits, and
+ * sb_rnnt_joint_vocab_fwd_rows / _bwd_rows.
  * ------------------------------------------------------------------------------------- */
+int sb_rnnt_joint_resident(int H, int V1);
 int sb_rnnt_joint_fwd(const float* fx, const float* fy, const void* w2_bf16, const float* b2,
                       const int* ymat, float* lat, float* lp_full, int B, int T, int U1, int H,
                       int V1, int blank, void* stream);

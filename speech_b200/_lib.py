@@ -102,6 +102,8 @@ SIGNATURES = {
     "sb_gru_bwd_workspace_size": (_c_int, [_c_int, _c_int, _c_int, ctypes.POINTER(_c_sz)]),
     "sb_gru_bwd": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_sz, _c_int, _c_int,
                             _c_int, _c_int, _vp]),
+    "sb_gru_plan": (_c_int, [_c_int, _c_int, _c_int, ctypes.POINTER(_c_int)]),
+    "sb_rnnt_joint_resident": (_c_int, [_c_int, _c_int]),
 }
 
 _lib = None

@@ -1902,6 +1902,53 @@ static int gru_check(int T, int Bp, int H, int ndir) {
   return SB_OK;
 }
 
+// Shared-memory ring of the plain (every-shape) kernels, forward and backward: -1 if the weight
+// slice leaves no room for one slot.  sb_gru_fwd / sb_gru_bwd launch with exactly these values.
+static int gru_fwd_ring(int Bp, int H, int* gc, size_t* smem) {
+  const int nchunks = (H + 63) / 64;
+  return gru_ring_slots(std::max(nchunks * 48 * 128, 16384 - Bp * 128), Bp, nchunks, 48, gc, smem);
+}
+static int gru_bwd_ring(int Bp, int H, int* gc, size_t* smem) {
+  const int nchunks = (3 * H + 63) / 64;
+  return gru_ring_slots(std::max(nchunks * 16 * 128, 16384 - Bp * 128), Bp, nchunks, 16, gc, smem);
+}
+
+// whether `grid` CTAs of `kernel` with `smem` bytes fit on the device at once (the cluster-size-1
+// launch gru_launch falls back to; the preferred clustered kernels fall back to it in turn)
+static bool gru_coresident(const void* kernel, int grid, size_t smem) {
+  int per_sm = 0;
+  if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) !=
+          cudaSuccess ||
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, GRU_THREADS, smem) !=
+          cudaSuccess) {
+    cudaGetLastError();
+    return false;
+  }
+  return per_sm * sb::device_sm_count() >= grid;
+}
+
+// Width the recurrence kernels run a layer of H hidden units at: H rounded up to whole CTAs of
+// GRU_HC units, provided both passes accept that width: gru_check, the rings of the plain
+// forward and backward kernels (the kernels every shape falls back to) and their co-residency.
+// The caller pads the layer with zero units; such a unit stays exactly 0
+// (h_t = sigmoid(0) * h_{t-1} = 0) and its zero W_hh columns never reach a real unit.
+extern "C" int sb_gru_plan(int Bp, int H, int ndir, int* Hp) {
+  if (!Hp || H <= 0) return SB_ERR_INVALID;
+  const int hp = (H + GRU_HC - 1) / GRU_HC * GRU_HC;
+  const int rc = gru_check(1, Bp, hp, ndir);
+  if (rc != SB_OK) return rc;
+  int gc = 1;
+  size_t fsmem = 0, bsmem = 0;
+  if (gru_fwd_ring(Bp, hp, &gc, &fsmem) < 0 || gru_bwd_ring(Bp, hp, &gc, &bsmem) < 0)
+    return SB_ERR_UNSUPPORTED;
+  const int grid = ndir * (hp / GRU_HC);
+  if (!gru_coresident((const void*)gru_fwd_kernel, grid, fsmem) ||
+      !gru_coresident((const void*)gru_bwd_kernel, grid, bsmem))
+    return SB_ERR_UNSUPPORTED;
+  *Hp = hp;
+  return SB_OK;
+}
+
 // workspace of one recurrence launch: [0,1024) the per-direction grid-barrier words, then the
 // exchange buffers of the backward kernels
 static size_t gru_ws_counters_bytes(int ndir) {
@@ -1927,15 +1974,13 @@ extern "C" int sb_gru_fwd(const float* gi, const void* whh_bf16, const float* bh
   if (workspace_bytes < need) return SB_ERR_WORKSPACE;
   if ((reinterpret_cast<uintptr_t>(workspace) & 1023) != 0) return SB_ERR_INVALID;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  const int nchunks = (H + 63) / 64;
   const int nC = H / GRU_HC;
   if (cudaMemsetAsync(workspace, 0, need, stream) != cudaSuccess) return SB_ERR_CUDA;
   uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
   unsigned int* barrier = reinterpret_cast<unsigned int*>(ws);
   int gc = 1;
   size_t smem = 0;
-  const int ring =
-      gru_ring_slots(std::max(nchunks * 48 * 128, 16384 - Bp * 128), Bp, nchunks, 48, &gc, &smem);
+  const int ring = gru_fwd_ring(Bp, H, &gc, &smem);
   if (ring < 0) return SB_ERR_UNSUPPORTED;
 
   // ---- preferred: K-split over 4-CTA clusters (H % 256 == 0, batch rows <= 64) ----
@@ -2026,7 +2071,6 @@ extern "C" int sb_gru_bwd(const float* dy, const float* y, const float* gates,
   p.dir0 = 0;
   p.ablate = g_gru_ablate & 195;
   const int K3 = 3 * H;
-  const int nchunks = (K3 + 63) / 64;
   size_t smem = 0;
   const int nC_ = H / GRU_HC;
   // counters and barrier words start at zero; the exchange tiles too (columns past 3H of a
@@ -2069,8 +2113,7 @@ extern "C" int sb_gru_bwd(const float* dy, const float* y, const float* gates,
       }
     }
   }
-  p.ring = gru_ring_slots(std::max(nchunks * 16 * 128, 16384 - Bp * 128), Bp, nchunks, 16, &p.gc,
-                          &smem);
+  p.ring = gru_bwd_ring(Bp, H, &p.gc, &smem);
   if (p.ring < 0) return SB_ERR_UNSUPPORTED;
   // per direction: the two parity buffers stacked as [2*Bp rows][3H cols]
   CUtensorMap tm[2];

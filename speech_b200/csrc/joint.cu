@@ -365,17 +365,27 @@ joint_reduce_slab_kernel(const float* __restrict__ dz, const bf16* __restrict__ 
 
 using namespace sb;
 
+// shared memory of the fused kernel for (H, V1): ring | fc2 weight | parked accumulator tile |
+// barriers, bias, bias gradient
+static size_t joint_smem_bytes(int H, int V1) {
+  const int nv = V1 <= 32 ? 32 : 64;
+  const int nkb = (H + 63) / 64;
+  const int stages = nv == 32 ? JtCfg<32>::kStages : JtCfg<64>::kStages;
+  return (size_t)stages * 128 * 128 + (size_t)nkb * nv * 128 + (size_t)128 * (nv + 1) * 4 + 8 +
+         1024 + 16 * stages + 8 * nv;
+}
+
+// 1 if the fused kernel (fc2 resident in shared memory) runs (H, V1), else 0
+extern "C" int sb_rnnt_joint_resident(int H, int V1) {
+  return H > 0 && H % 8 == 0 && V1 > 0 && V1 <= 64 && joint_smem_bytes(H, V1) <= 227 * 1024;
+}
+
 static int joint_launch(JointParams& p, void* stream_) {
-  if (p.H % 8 != 0 || p.V1 > 64 || p.V1 <= 0 || p.blank < 0 || p.blank >= p.V1)
+  if (!sb_rnnt_joint_resident(p.H, p.V1) || p.blank < 0 || p.blank >= p.V1)
     return SB_ERR_UNSUPPORTED;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   const int nv = p.V1 <= 32 ? 32 : 64;
-  const int nkb = (p.H + 63) / 64;
-  const int stages = nv == 32 ? JtCfg<32>::kStages : JtCfg<64>::kStages;
-  // ring | fc2 weight | parked accumulator tile | barriers, bias, bias gradient
-  const size_t smem = (size_t)stages * 128 * 128 + (size_t)nkb * nv * 128 +
-                      (size_t)128 * (nv + 1) * 4 + 8 + 1024 + 16 * stages + 8 * nv;
-  if (smem > 227 * 1024) return SB_ERR_UNSUPPORTED;
+  const size_t smem = joint_smem_bytes(p.H, p.V1);
   const long long ntiles = (p.nodes + 127) / 128;
   int grid = device_sm_count();
   if (grid > ntiles) grid = (int)ntiles;

@@ -92,7 +92,7 @@ class TransducerLoss(torch.nn.Module):
 # (transducer_model.py:71-76) never exist on the training path.
 # ------------------------------------------------------------------------------------------------
 JOINT_SLAB_FRAMES = 8     # frames whose hidden activations are materialised at a time in backward
-JOINT_RESIDENT_MAX_CLASSES = 64   # V+1 up to which fc2's weight stays resident in the fused kernel
+JOINT_RESIDENT_MAX_CLASSES = 64   # V+1 up to which fc2's weight can stay resident in the fused kernel
 # Cap on one slab's fp32 logits in the large-vocabulary path.  Measured on an H100 80GB HBM3 at a
 # 700 W power limit (tools/joint_vocab_bench.py, B=32, T'=247, U+1=100, H=1024), forward + backward:
 #   V+1 = 1024: Tc = 1, 2, 4, 8 -> 40.8, 32.5, 27.0, 24.4 ms (host enqueue 30.5, 16.0, 8.1, 5.9 ms)
@@ -105,6 +105,13 @@ JOINT_VOCAB_SLAB_BYTES = 512 << 20
 
 def _round_up(x, m):
     return (x + m - 1) // m * m
+
+
+def joint_uses_slabs(H, V1):
+    """True if the joint of width H over V1 classes runs a slab of frames at a time: whenever the
+    fused kernel cannot keep fc2's weight in shared memory (V1 > 64, or H too wide for V1, as
+    sb_rnnt_joint_resident decides)."""
+    return V1 > JOINT_RESIDENT_MAX_CLASSES or not _lib.load().sb_rnnt_joint_resident(H, V1)
 
 
 def joint_vocab_slab_frames(B, U1, V1, budget=None):
@@ -214,7 +221,9 @@ def _pack_labels(labels, x_lens, y_lens, B, U1, dev):
 
 def joint_log_probs(fx, fy, fc2, ymat, blank):
     """Full (B, T, U1, V1) log-probabilities of the joint network (what `Transducer.infer` hands
-    to the beam search), from fx = fc1(x) (B,T,H), fy = fc1(pred) (B,U1,H); no autograd."""
+    to the beam search), from fx = fc1(x) (B,T,H), fy = fc1(pred) (B,U1,H); no autograd.
+    fx / fy may carry zero units past fc2's input width (see Transducer.joint_inputs): fc2's
+    weight gets zero columns for them."""
     from .. import ops
     _lib.require_cuda(fx, "fx")
     lib = _lib.load()
@@ -222,10 +231,11 @@ def joint_log_probs(fx, fy, fc2, ymat, blank):
     U1 = fy.shape[1]
     V1 = fc2.weight.shape[0]
     fxc, fyc = fx.detach().float().contiguous(), fy.detach().float().contiguous()
-    w2 = fc2.weight.detach().to(torch.bfloat16).contiguous()
+    w2 = fc2.weight.detach().to(torch.bfloat16)
+    w2 = ops.pad_blocks(w2, 1, 1, w2.shape[1], H).contiguous()
     b2 = fc2.bias.detach().float().contiguous()
     ym = ymat.detach().to(fx.device, torch.int32).contiguous()
-    if V1 > JOINT_RESIDENT_MAX_CLASSES:
+    if joint_uses_slabs(H, V1):
         out = torch.empty(B, T, U1, V1, dtype=torch.float32, device=fx.device)
         joint_vocab_forward(fxc, fyc, w2, b2, ym, blank, lp_full=out)
         return out
@@ -256,7 +266,7 @@ class _JointLossFunction(torch.autograd.Function):
         lab, offs, ylen, xlen = _pack_labels(labels, x_lens, y_lens, B, U1, dev)
         nodes = T * B * U1
         lse = None
-        if V1 > JOINT_RESIDENT_MAX_CLASSES:
+        if joint_uses_slabs(H, V1):
             lat, lse = joint_vocab_forward(fxc, fyc, w2b, b2c, ym, blank)
             sp = _lib.stream_ptr()
         else:
@@ -296,7 +306,7 @@ class _JointLossFunction(torch.autograd.Function):
             return (None,) * 10
         garc = garc * (grad_out.reshape(1, 1).float() * scale)
         nodes = T * B * U1
-        if V1 > JOINT_RESIDENT_MAX_CLASSES:
+        if ctx.lse is not None:                   # the forward ran the slab path
             dfx, dfy, dw2, db2 = joint_vocab_backward(fxc, fyc, w2b, b2c, ym, garc, ctx.lse, blank)
             return dfx, dfy, dw2, db2, None, None, None, None, None, None
         NV = 32 if V1 <= 32 else 64

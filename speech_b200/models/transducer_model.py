@@ -58,18 +58,28 @@ class Transducer(model.Model):
             # the encoder
             fx, fy = self.joint_inputs(self._encode(x, self.exact_lens(x_lens)), y_mat)
             fc2 = self.fc2.fc
+            H = fc2.in_features
             return transducer_fn.JointTransducerLoss(blank=self.blank)(
-                fx, fy, fc2.weight, fc2.bias, y_mat, y, x_lens, y_lens)
+                fx, fy, ops.pad_blocks(fc2.weight, 1, 1, H, fx.shape[2]), fc2.bias, y_mat, y,
+                x_lens, y_lens)
 
     def joint_inputs(self, x, y):
-        """fc1 of both streams (the SAME fc1, :73): x (B,T',H) encoder states -> fx (B,T',H);
-        labels y (B,U) -> embedding, zero start vector, prediction GRU -> fy (B,U+1,H)."""
+        """fc1 of both streams (the SAME fc1, :73): x (B,T',H) encoder states -> fx (B,T',Hj);
+        labels y (B,U) -> embedding, zero start vector, prediction GRU -> fy (B,U+1,Hj).
+        Hj is H rounded up to the joint kernels' multiple of 8: fc1 gets zero output units, which
+        stay 0 through relu(fx + fy), and fc2 zero input columns for them (exact)."""
         emb = self.embedding(y)
         start = torch.zeros((emb.shape[0], 1, emb.shape[2]), device=emb.device, dtype=emb.dtype)
         pred_in = torch.cat([start, emb], dim=1)           # zero vector stands for "no label yet"
         p = self.dec_rnn.dropout if self.training else 0.0
         pred = ops.gru_stack(pred_in, self.dec_rnn, dropout=p)
-        return self.fc1(x), self.fc1(pred)
+        fc1 = self.fc1.fc
+        H = fc1.out_features
+        Hj = (H + 7) // 8 * 8
+        if Hj == H:
+            return self.fc1(x), self.fc1(pred)
+        w1, b1 = ops.pad_blocks(fc1.weight, 0, 1, H, Hj), ops.pad_blocks(fc1.bias, 0, 1, H, Hj)
+        return ops.linear(x, w1, b1), ops.linear(pred, w1, b1)
 
     def decode(self, x, y):
         """x (B, T', H) encoder states, y (B, U) labels -> (B, T', U+1, V+1) log-probs (:54-77),

@@ -20,6 +20,51 @@ def _round_up(x, m):
     return (x + m - 1) // m * m
 
 
+def pad_blocks(t, dim, blocks, n, n_pad):
+    """Dimension `dim` of t as `blocks` consecutive blocks of n entries -> blocks of n_pad, each
+    block's new tail zero (autograd-aware; t itself when n_pad == n).  This is how GRU layers run
+    at the kernels' width: gate blocks (r|z|n) of the weight rows and biases, direction blocks
+    (fwd|rev) of the next layer's input columns, and the conv stack's channels."""
+    if n_pad == n:
+        return t
+    dim %= t.dim()
+    shape = tuple(t.shape)
+    v = t.reshape(shape[:dim] + (blocks, n) + shape[dim + 1:])
+    v = torch.nn.functional.pad(v, [0, 0] * (len(shape) - dim - 1) + [0, n_pad - n])
+    return v.reshape(shape[:dim] + (blocks * n_pad,) + shape[dim + 1:])
+
+
+def unpad_blocks(t, dim, blocks, n, n_pad):
+    """Inverse of pad_blocks: the first n entries of each n_pad-block of dimension `dim`."""
+    if n_pad == n:
+        return t
+    dim %= t.dim()
+    shape = tuple(t.shape)
+    v = t.reshape(shape[:dim] + (blocks, n_pad) + shape[dim + 1:]).narrow(dim + 1, 0, n)
+    return v.reshape(shape[:dim] + (blocks * n,) + shape[dim + 1:])
+
+
+def pad_gru_layer(w_ih, w_hh, b_ih, b_hh, H, Hp, in_dirs):
+    """One direction's nn.GRU parameters of hidden size H as those of a GRU of size Hp whose
+    units H..Hp-1 (per gate) are zero: exact, because a zero unit with h_0 = 0 stays 0
+    (r = z = 1/2, n = tanh(0) = 0, h_t = h_{t-1} / 2) and its zero W_hh column never reaches a
+    real unit.  in_dirs: 0 for the first layer (its input is not padded), else the number of
+    directions of the layer below, whose outputs arrive as in_dirs blocks of Hp columns."""
+    w_ih = pad_blocks(w_ih, 0, 3, H, Hp)
+    if in_dirs:
+        w_ih = pad_blocks(w_ih, 1, in_dirs, H, Hp)
+    return (w_ih, pad_blocks(pad_blocks(w_hh, 0, 3, H, Hp), 1, 1, H, Hp),
+            pad_blocks(b_ih, 0, 3, H, Hp), pad_blocks(b_hh, 0, 3, H, Hp))
+
+
+def gru_padded_width(Bp, H, ndir):
+    """The width the recurrence kernels run a layer of H units at (sb_gru_plan); raises if none."""
+    hp = ctypes.c_int(0)
+    _lib.check(_lib.load().sb_gru_plan(Bp, H, ndir, ctypes.byref(hp)),
+               "sb_gru_plan (H = %d, %d direction(s), %d batch rows)" % (H, ndir, Bp))
+    return hp.value
+
+
 def _apply_env_knobs():
     """Developer knobs (profiling under ncu cannot replay clustered cooperative launches):
     SB_GRU_KSPLIT=0 disables the K-split backward kernel, SB_GRU_CLUSTER=<1|2|4|8> sets the
@@ -396,6 +441,10 @@ class GRUStackFunction(torch.autograd.Function):
     coordinates for the backward pass, and its half of each layer output is left-aligned again.
     The gradient arriving at output frames >= len_b is ignored (and without the fused projection
     those output rows are zero), so frames >= len_b of x receive exactly zero gradient.
+
+    Every layer runs at the kernels' width Hp = gru_padded_width(Bp, H, ndir) >= H: when Hp > H
+    the bf16 operands are built with zero units (pad_gru_layer), all internal activations carry
+    ndir blocks of Hp columns, and the outputs and gradients are sliced back to H.
     """
 
     @staticmethod
@@ -412,8 +461,9 @@ class GRUStackFunction(torch.autograd.Function):
         if Bp > 128:
             raise _lib.SpeechB200Error("per-GPU batch > 128 not supported by the GRU kernel yet")
         M = T * Bp
-        D = ndir * H
-        K3 = 3 * H
+        Hp = gru_padded_width(Bp, H, ndir)
+        D = ndir * Hp
+        K3 = 3 * Hp
         need_grad = any(ctx.needs_input_grad)     # all False under torch.no_grad()
         lo = _lens_operands(lens, B, T, Bp, dev)
         al, valid = lo if lo is not None else (None, None)
@@ -429,33 +479,32 @@ class GRUStackFunction(torch.autograd.Function):
             X[:, :B, :In] = x.transpose(0, 1)
             X = X.view(M, Inp)
         nbytes = ctypes.c_size_t(0)
-        _lib.check(lib.sb_gru_fwd_workspace_size(Bp, H, ndir, ctypes.byref(nbytes)), "ws")
+        _lib.check(lib.sb_gru_fwd_workspace_size(Bp, Hp, ndir, ctypes.byref(nbytes)), "ws")
         ws = _workspace(nbytes.value, dev)
         saved = []
         y = None
         for l in range(L):
             wl = weights[l * 4 * ndir:(l + 1) * 4 * ndir]
-            w_ih = [wl[d * 4 + 0] for d in range(ndir)]
-            w_hh = [wl[d * 4 + 1] for d in range(ndir)]
-            b_ih = [wl[d * 4 + 2] for d in range(ndir)]
-            b_hh = [wl[d * 4 + 3] for d in range(ndir)]
             Kl = X.shape[1]
-            In_l = w_ih[0].shape[1]
-            cached = _cached_gru_operands(w_ih[0], Kl)
+            cached = _cached_gru_operands(wl[0], Kl) if Hp == H else None
             if cached is not None:
                 # views of the optimizer's flat buffers (bf16 shadow written by sgd_clip_step)
                 wih_cat, whh = cached["wih"], cached["whh"]
                 bih_cat, bhh = cached["bih"], cached["bhh"]
             else:
+                # (w_ih, w_hh, b_ih, b_hh) of each direction at the kernels' width
+                lw = [pad_gru_layer(*[q.detach() for q in wl[d * 4:d * 4 + 4]], H, Hp,
+                                    ndir if l > 0 else 0) for d in range(ndir)]
+                In_l = lw[0][0].shape[1]
                 # bf16 operand copies of the master weights: one fused cast+copy per matrix
                 wih_cat = (torch.empty if Kl == In_l else torch.zeros)(
-                    ndir * 3 * H, Kl, dtype=torch.bfloat16, device=dev)
-                whh = torch.empty(ndir, 3 * H, H, dtype=torch.bfloat16, device=dev)
+                    ndir * K3, Kl, dtype=torch.bfloat16, device=dev)
+                whh = torch.empty(ndir, K3, Hp, dtype=torch.bfloat16, device=dev)
                 for d in range(ndir):
-                    wih_cat[d * 3 * H:(d + 1) * 3 * H, :In_l].copy_(w_ih[d].detach())
-                    whh[d].copy_(w_hh[d].detach())
-                bih_cat = torch.cat([b.detach() for b in b_ih]).float().contiguous()
-                bhh = torch.stack([b.detach() for b in b_hh]).float().contiguous()
+                    wih_cat[d * K3:(d + 1) * K3, :In_l].copy_(lw[d][0])
+                    whh[d].copy_(lw[d][1])
+                bih_cat = torch.cat([q[2] for q in lw]).float().contiguous()
+                bhh = torch.stack([q[3] for q in lw]).float().contiguous()
             if al is None:
                 gi = gemm_bf16_tn(X, wih_cat, bias=bih_cat)
             else:
@@ -468,22 +517,25 @@ class GRUStackFunction(torch.autograd.Function):
             xn = torch.empty(M, D, dtype=torch.bfloat16, device=dev)
             gates = None
             if need_grad:
-                gates = torch.empty(M, ndir, 4, H, dtype=torch.float32, device=dev)
+                gates = torch.empty(M, ndir, 4, Hp, dtype=torch.float32, device=dev)
             sp = _lib.stream_ptr()
-            _launch("gru_fwd", 2.0 * M * 3 * H * H * ndir,
+            _launch("gru_fwd", 2.0 * M * 3 * Hp * Hp * ndir,
                     lambda: lib.sb_gru_fwd(gi.data_ptr(), whh.data_ptr(), bhh.data_ptr(),
                                            y.data_ptr(), xn.data_ptr(), _lib.ptr(gates),
-                                           ws.data_ptr(), nbytes.value, T, Bp, H, ndir, sp))
+                                           ws.data_ptr(), nbytes.value, T, Bp, Hp, ndir, sp))
             mask = None
             hb = xn                                     # bf16 h_t (un-masked): dW_hh operand
             y_rec = y                                   # as the recurrence wrote it (backward)
             if al is not None:
-                xn = _align_reverse(xn, al, T, Bp, H, right=False)
+                xn = _align_reverse(xn, al, T, Bp, Hp, right=False)
                 if (dropout > 0.0 and l + 1 < L) or (l + 1 == L and fc_w is None):
-                    y = _align_reverse(y, al, T, Bp, H, right=False)
+                    y = _align_reverse(y, al, T, Bp, Hp, right=False)
             if dropout > 0.0 and l + 1 < L:
-                # inter-layer dropout of nn.GRU(dropout=p): applied to every layer output but the last
-                mask = (torch.rand(M, D, device=dev) >= dropout).float() * (1.0 / (1.0 - dropout))
+                # inter-layer dropout of nn.GRU(dropout=p): applied to every layer output but the
+                # last; drawn over the H real units, so padding does not change the masks
+                mask = (torch.rand(M, ndir * H, device=dev) >= dropout).float() * \
+                    (1.0 / (1.0 - dropout))
+                mask = pad_blocks(mask, 1, ndir, H, Hp)
                 # the next layer's operand stays bf16 (bf16 * f32 would promote to f32): mask the
                 # fp32 state and round once
                 xn = (y * mask).to(torch.bfloat16)
@@ -493,7 +545,7 @@ class GRUStackFunction(torch.autograd.Function):
         ctx.saved = saved
         ctx.announce = _announce
         ctx.weights = weights
-        ctx.dims = (B, T, In, Bp, H, ndir, L)
+        ctx.dims = (B, T, In, Bp, H, Hp, ndir, L)
         ctx.lens = (al, valid)
         ctx.fc = None
         if fc_w is not None:
@@ -501,12 +553,12 @@ class GRUStackFunction(torch.autograd.Function):
             wcat = fc_w.detach().to(torch.bfloat16)
             if ndir == 2:
                 wcat = torch.cat([wcat, wcat], 1)
-            wcat = wcat.contiguous()
+            wcat = pad_blocks(wcat, 1, ndir, H, Hp).contiguous()
             out = gemm_bf16_tn(X, wcat, bias=fc_b.detach().float().contiguous(),
                                remap=(Bp, T, B)).view(B, T, V)
             ctx.fc = (fc_w, X)
             return out
-        out = y.view(T, Bp, D)[:, :B].transpose(0, 1).contiguous()
+        out = unpad_blocks(y.view(T, Bp, D)[:, :B], 2, ndir, H, Hp).transpose(0, 1).contiguous()
         if valid is not None:
             out.mul_(valid)
         return out
@@ -514,14 +566,15 @@ class GRUStackFunction(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dout):
         lib = _lib.load()
-        B, T, In, Bp, H, ndir, L = ctx.dims
+        B, T, In, Bp, H, Hp, ndir, L = ctx.dims
         weights = ctx.weights
         if _grad_ready_hook is not None and ctx.announce and _grad_guard is not None:
             _grad_guard(list(weights))
         dev = dout.device
         M = T * Bp
-        D = ndir * H
-        K3 = 3 * H
+        D = ndir * Hp
+        K3 = 3 * Hp
+        padded = Hp != H
         al, valid = ctx.lens
         if valid is not None:
             dout = dout * valid
@@ -536,22 +589,22 @@ class GRUStackFunction(torch.autograd.Function):
             w = fc_w.detach().to(torch.bfloat16)
             wT = torch.zeros(D, Vp, dtype=torch.bfloat16, device=dev)      # [D][Vp] = [W | W]^T
             for d in range(ndir):
-                wT[d * H:(d + 1) * H, :V] = w.t()
+                wT[d * Hp:d * Hp + H, :V] = w.t()
             dY = gemm_bf16_tn(dl, wT)                                         # [M][D] f32
             dw2 = torch.zeros(Vp, D, dtype=torch.float32, device=dev)
             # dW (Vp x D) = dl^T Xtop, both operands read token-major (MN-major UMMA)
             gemm_bf16_tn(dl, Xtop, out=dw2, accumulate=True, a_mn=True, b_mn=True)
-            dfc_w = dw2[:V, :H] if ndir == 1 else dw2[:V, :H] + dw2[:V, H:]
+            dfc_w = dw2[:V, :H] if ndir == 1 else dw2[:V, :H] + dw2[:V, Hp:Hp + H]
             dfc_b = dout.sum((0, 1))
-        elif B == Bp:
+        elif B == Bp and not padded:
             # (dout may be an expanded stride-0 tensor, e.g. from y.sum(): force a real copy)
             dY = dout.transpose(0, 1).float().contiguous().view(M, D)
         else:
             dY = torch.zeros(T, Bp, D, dtype=torch.float32, device=dev)
-            dY[:, :B] = dout.transpose(0, 1)
+            dY[:, :B] = pad_blocks(dout.transpose(0, 1), 2, ndir, H, Hp)
             dY = dY.view(M, D)
         nbytes = ctypes.c_size_t(0)
-        _lib.check(lib.sb_gru_bwd_workspace_size(Bp, H, ndir, ctypes.byref(nbytes)), "ws")
+        _lib.check(lib.sb_gru_bwd_workspace_size(Bp, Hp, ndir, ctypes.byref(nbytes)), "ws")
         ws = _workspace(nbytes.value, dev)
         grads = [None] * len(weights)
         for l in reversed(range(L)):
@@ -559,20 +612,20 @@ class GRUStackFunction(torch.autograd.Function):
             if mask is not None:
                 dY = dY * mask
             if al is not None:
-                dY = _align_reverse(dY, al, T, Bp, H, right=True)
+                dY = _align_reverse(dY, al, T, Bp, Hp, right=True)
             wl = weights[l * 4 * ndir:(l + 1) * 4 * ndir]
             Kl = X.shape[1]
-            In_l = wl[0].shape[1]
+            In_l = wl[0].shape[1] if l == 0 else D     # input columns at the kernels' width
             dgi = torch.empty(M, ndir * K3, dtype=torch.bfloat16, device=dev)
             dghn = torch.empty(M, D, dtype=torch.bfloat16, device=dev)
             dbih = torch.zeros(ndir * K3, dtype=torch.float32, device=dev)
             dbhh = torch.zeros(ndir * K3, dtype=torch.float32, device=dev)
             sp = _lib.stream_ptr()
-            _launch("gru_bwd", 2.0 * M * 3 * H * H * ndir,
+            _launch("gru_bwd", 2.0 * M * 3 * Hp * Hp * ndir,
                     lambda dY=dY: lib.sb_gru_bwd(dY.data_ptr(), y.data_ptr(), gates.data_ptr(),
                                                  whh.data_ptr(), dgi.data_ptr(), dghn.data_ptr(),
                                                  dbih.data_ptr(), dbhh.data_ptr(), ws.data_ptr(),
-                                                 nbytes.value, T, Bp, H, ndir, sp))
+                                                 nbytes.value, T, Bp, Hp, ndir, sp))
             base = l * 4 * ndir
             # dW_hh pairs dgi with the states in the recurrence's coordinates; dW_ih and dX pair
             # it with the layer input, where the reverse half is left-aligned
@@ -580,8 +633,9 @@ class GRUStackFunction(torch.autograd.Function):
             # ---- weight gradients: contract the token-major operands over their rows ----
             Ms = M - Bp                      # tokens that have a predecessor in the recurrence
             for d in range(ndir):
-                # dW_ih[d] (3H x In_l) = dgi[:, d]^T X
-                sink = _grad_sink(wl[d * 4])
+                # dW_ih[d] (3H x In_l) = dgi[:, d]^T X.  A padded layer computes the padded
+                # gradients into temporaries and hands on (or adds into the sink) the real block.
+                sink = None if padded else _grad_sink(wl[d * 4])
                 dwih = sink if sink is not None else \
                     torch.zeros(K3, In_l, dtype=torch.float32, device=dev)
                 gemm_bf16_tn(dgi_x[:, d * K3:(d + 1) * K3], X[:, :In_l], out=dwih,
@@ -589,20 +643,31 @@ class GRUStackFunction(torch.autograd.Function):
                 # dW_hh[d] = [dgi_r | dgi_z | dghn]^T h_prev: h_prev of token (t, b) is token
                 # (t-1, b) in the forward direction and (t+1, b) in the reverse one, so the
                 # shift is a row offset of Bp on one of the two operands
-                sink_hh = _grad_sink(wl[d * 4 + 1])
+                sink_hh = None if padded else _grad_sink(wl[d * 4 + 1])
                 dwhh = sink_hh if sink_hh is not None else \
-                    torch.zeros(K3, H, dtype=torch.float32, device=dev)
+                    torch.zeros(K3, Hp, dtype=torch.float32, device=dev)
                 if Ms > 0:
                     ga, hp = (slice(Bp, M), slice(0, Ms)) if d == 0 else \
                         (slice(0, Ms), slice(Bp, M))
-                    gemm_bf16_tn(dgi[ga, d * K3:d * K3 + 2 * H], hb[hp, d * H:(d + 1) * H],
-                                 out=dwhh[:2 * H], accumulate=True, a_mn=True, b_mn=True)
-                    gemm_bf16_tn(dghn[ga, d * H:(d + 1) * H], hb[hp, d * H:(d + 1) * H],
-                                 out=dwhh[2 * H:], accumulate=True, a_mn=True, b_mn=True)
+                    gemm_bf16_tn(dgi[ga, d * K3:d * K3 + 2 * Hp], hb[hp, d * Hp:(d + 1) * Hp],
+                                 out=dwhh[:2 * Hp], accumulate=True, a_mn=True, b_mn=True)
+                    gemm_bf16_tn(dghn[ga, d * Hp:(d + 1) * Hp], hb[hp, d * Hp:(d + 1) * Hp],
+                                 out=dwhh[2 * Hp:], accumulate=True, a_mn=True, b_mn=True)
+                dbi, dbh = dbih[d * K3:(d + 1) * K3], dbhh[d * K3:(d + 1) * K3]
+                if padded:
+                    dwih = unpad_blocks(dwih, 0, 3, H, Hp)
+                    if l > 0:
+                        dwih = unpad_blocks(dwih, 1, ndir, H, Hp)
+                    dwhh = unpad_blocks(unpad_blocks(dwhh, 0, 3, H, Hp), 1, 1, H, Hp)
+                    dbi, dbh = unpad_blocks(dbi, 0, 3, H, Hp), unpad_blocks(dbh, 0, 3, H, Hp)
+                    sink, sink_hh = _grad_sink(wl[d * 4]), _grad_sink(wl[d * 4 + 1])
+                    for s, g in ((sink, dwih), (sink_hh, dwhh)):
+                        if s is not None:
+                            s.add_(g)
                 grads[base + d * 4 + 0] = None if sink is not None else dwih
                 grads[base + d * 4 + 1] = None if sink_hh is not None else dwhh
-                grads[base + d * 4 + 2] = dbih[d * K3:(d + 1) * K3]
-                grads[base + d * 4 + 3] = dbhh[d * K3:(d + 1) * K3]
+                grads[base + d * 4 + 2] = dbi
+                grads[base + d * 4 + 3] = dbh
             if _grad_ready_hook is not None and ctx.announce:
                 base = l * 4 * ndir
                 if all(grads[base + d * 4 + k] is None for d in range(ndir) for k in (0, 1)):
@@ -721,10 +786,12 @@ class ConvStackFunction(torch.autograd.Function):
         need_grad = any(ctx.needs_input_grad)
         sp = _lib.stream_ptr()
         for l, (kh, kw, s_) in enumerate(specs):
-            w, b = params[2 * l], params[2 * l + 1]
-            Co = w.shape[0]
-            if Co % 8 != 0:
-                raise _lib.SpeechB200Error("conv out_channels must be a multiple of 8")
+            co_r, ci_r = params[2 * l].shape[:2]
+            # zero filters up to the GEMM's multiple of 8 channels: a padded channel is
+            # ReLU(0) = 0 everywhere, and the next layer's weights for it are zero
+            Co = _round_up(co_r, 8)
+            w = pad_blocks(pad_blocks(params[2 * l].detach(), 0, 1, co_r, Co), 1, 1, ci_r, Ci)
+            b = pad_blocks(params[2 * l + 1].detach(), 0, 1, co_r, Co)
             K = kh * kw * Ci
             Kp = _round_up(K, 8)
             To, Fo = (Ti - kh) // s_ + 1, (Fi - kw) // s_ + 1
@@ -743,7 +810,8 @@ class ConvStackFunction(torch.autograd.Function):
                 mask = (torch.rand(M, Co, device=dev) >= dropout).to(torch.uint8)
             masks.append(mask)
             if need_grad:
-                saved.append((A, cur, C, Wp, (Ti, Fi, Ci, kh, kw, s_, To, Fo, Co, K, Kp)))
+                saved.append((A, cur, C, Wp,
+                              (Ti, Fi, Ci, kh, kw, s_, To, Fo, Co, K, Kp, co_r, ci_r)))
             cur, Ti, Fi, Ci = C, To, Fo, Co
         out = torch.empty(B, Ti, Ci * Fi, dtype=torch.float32, device=dev)
         _launch("conv_relu_to_bct", 0.0,
@@ -755,7 +823,9 @@ class ConvStackFunction(torch.autograd.Function):
         ctx.mscale = mscale
         ctx.B = B
         ctx.nl = len(specs)
-        return out
+        # channel-major features: the real channels 0..co_r-1 are the leading co_r*F' columns
+        ctx.pad_cols = (Ci - co_r) * Fi
+        return out[:, :, :co_r * Fi] if ctx.pad_cols else out
 
     @staticmethod
     def backward(ctx, dY):
@@ -765,9 +835,11 @@ class ConvStackFunction(torch.autograd.Function):
         sp = _lib.stream_ptr()
         grads = [None] * (2 * ctx.nl)
         dY = dY.contiguous().float()
+        if ctx.pad_cols:
+            dY = torch.nn.functional.pad(dY, (0, ctx.pad_cols))
         dC = None
         for l in reversed(range(ctx.nl)):
-            A, Pprev, C, Wp, (Ti, Fi, Ci, kh, kw, s_, To, Fo, Co, K, Kp) = ctx.saved[l]
+            A, Pprev, C, Wp, (Ti, Fi, Ci, kh, kw, s_, To, Fo, Co, K, Kp, co_r, ci_r) = ctx.saved[l]
             M = B * To * Fo
             if dC is None:
                 dC = torch.empty(M, Co, dtype=torch.bfloat16, device=dev)
@@ -778,13 +850,14 @@ class ConvStackFunction(torch.autograd.Function):
                                                  _lib.ptr(ctx.masks[l]), ctx.mscale,
                                                  dCl.data_ptr(),
                                                  db.data_ptr(), B, To, Fo, Co, sp))
-            grads[2 * l + 1] = db
+            grads[2 * l + 1] = db[:co_r]
             # weight gradient: contraction over the M = B*To*Fo patch rows (split-K over all SMs)
             # dWp^T [Kp][Co] = A^T dC with both operands read token-major (MN-major UMMA)
             dWpT = torch.zeros(Kp, Co, dtype=torch.float32, device=dev)
             gemm_bf16_tn(A, dC, out=dWpT, accumulate=True, a_mn=True, b_mn=True)
             dWp = dWpT.t()
-            grads[2 * l] = dWp[:, :K].reshape(Co, kh, kw, Ci).permute(0, 3, 1, 2).contiguous()
+            grads[2 * l] = dWp[:co_r, :K].reshape(co_r, kh, kw, Ci).permute(0, 3, 1, 2)[:, :ci_r] \
+                .contiguous()
             if l > 0:
                 dA = gemm_bf16_tn(dC, Wp, b_mn=True)            # [M][Kp] f32 patch gradient
                 Mp = B * Ti * Fi
@@ -808,12 +881,12 @@ def conv_stack(x, conv, training):
 
     x (B, T, F) -> (B, T', C*F') with the reference's channel-major feature flattening
     (transpose(1,2) of (B,C,T',F') then view, model.py:66-71).  Runs on our im2col + wgmma
-    kernels, including the Dropout after each ReLU when training.  Shapes the kernels do not
-    cover go through the nn modules: grouped / dilated / padded convolutions and out_channels not
-    a multiple of 8 (none of which the reference can express, model.py:21-23), and - only when a
-    gradient is needed - an upper layer whose kernel spans more than 5 x 8 taps per stride phase
-    (the unrolled gather of `col2im_relu_kernel`; the TIMIT recipes' second layer [*, 5, 32, 1]
-    is the one shipped case: its forward / inference still runs on our kernels).
+    kernels, including the Dropout after each ReLU when training, for every stack the reference
+    can express (model.py:21-23: square stride, no padding, dilation or groups, bias, one dropout
+    rate); any other stack raises, there is no library fallback.  Any out_channels runs: a layer
+    whose count is not a multiple of 8 gets zero filters up to the next multiple (exact: such a
+    channel is 0 after the ReLU, and the next layer's weights for it are zero), its dropout mask
+    covers the padded channels too, and the real features are the leading C*F' columns.
     """
     mods = list(conv.children())
     convs = [m for m in mods if isinstance(m, torch.nn.Conv2d)]
@@ -821,13 +894,11 @@ def conv_stack(x, conv, training):
     p_drop = (ps[0] if ps else 0.0) if training else 0.0
     drop = len(set(ps)) > 1
     simple = all(c.stride[0] == c.stride[1] and c.padding == (0, 0) and c.dilation == (1, 1)
-                 and c.groups == 1 and c.bias is not None and c.out_channels % 8 == 0
-                 for c in convs)
+                 and c.groups == 1 and c.bias is not None for c in convs)
     if not (convs and simple and not drop):
         raise _lib.SpeechB200Error(
             "conv_stack: unsupported convolution stack (needs square stride, no padding / "
-            "dilation / groups, bias, out_channels % 8 == 0, one dropout rate); this package has "
-            "no cuDNN fallback")
+            "dilation / groups, bias, one dropout rate); this package has no cuDNN fallback")
     specs = tuple((c.kernel_size[0], c.kernel_size[1], c.stride[0]) for c in convs)
     params = []
     for c in convs:

@@ -37,4 +37,17 @@ for cls in (CTC, Transducer):
 sx = Seq2Seq(80, 30, cfg_x).cuda()
 l5 = sx.loss((inputs, lab2)); l5.backward()
 print("exact lengths Seq2Seq", l5.item(), [len(h) for h in sx.infer((inputs, lab2), max_len=12)])
+# zero-padded shapes: GRU width 1000 (run at 1008), conv channels 4 and 12 (run at 8 and 16),
+# and a Transducer of width 100 (GRUs at 112, joint at 104)
+cfg_p = {"dropout": 0.0, "encoder": {"conv": [[4, 5, 8, 2], [12, 5, 8, 2]],
+                                     "rnn": {"dim": 1000, "bidirectional": True, "layers": 1}},
+         "decoder": {"embedding_dim": 32, "layers": 1}}
+mp = CTC(80, 28, cfg_p).cuda()
+opt_p = FlatSGD(mp, lr=1e-3)
+opt_p.zero_grad(); l6 = mp.loss((inputs, labels)); l6.backward(); opt_p.step()
+print("padded CTC dim 1000 ok", l6.item())
+cfg_p["encoder"]["rnn"]["dim"] = 100
+tp = Transducer(80, 28, cfg_p).cuda()
+l7 = tp.loss((inputs, labels)); l7.backward()
+print("padded Transducer dim 100 ok", l7.item(), [len(p) for p in tp.infer((inputs, labels))])
 torch.cuda.synchronize()
