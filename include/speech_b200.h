@@ -428,12 +428,16 @@ int sb_debug_gru_timeline(void* dev_buffer);
 int sb_debug_umma_mn(int lbo_bytes, int sbo_bytes, int kadv_bytes);
 /* Developer hook, GRU kernel selection / timing knobs (0 = defaults): 8 / 16 = never / always use
  * the transposed-accumulator K-split kernels, 32 = no K-split forward kernel, 64 / 128 = polling
- * mode of the grid barrier; 1 / 2 are timing ablations (results become wrong). */
+ * mode of the grid barrier, 256 / 512 = always (wherever the K-split backward kernel applies) /
+ * never use its L2 reduce-scatter mode (the mode the backward uses when both directions do not
+ * fit as thread-block clusters but do fit without); 1 / 2 are timing ablations (results become
+ * wrong). */
 int sb_debug_gru_flags(int flags);
 /* Developer hook: enable (1, default) / disable (0) the K-split backward GRU kernel. */
 int sb_debug_gru_ksplit(int enable);
 /* Developer hook: set the preferred thread-block-cluster size (1, 2, 4 or 8) of the GRU kernels;
- * returns the cluster size the last GRU launch actually used (0 = query only, -1 = bad value). */
+ * returns the cluster size the last GRU launch actually used (0 = query only, -1 = bad value;
+ * 1 after a launch without clusters, e.g. the L2 reduce-scatter mode). */
 int sb_debug_gru_cluster(int cluster_size);
 
 #ifdef __cplusplus

@@ -76,6 +76,8 @@ struct GruBwdParams {
   int T, Bp, H, ndir, ring, gc;
   int dir0;            // direction of CTA 0 (gru_bwd_ks_kernel launched for one direction: 0 or 1)
   int ablate;          // developer knobs: see sb_debug_gru_flags
+  float* rs;           // L2 reduce-scatter staging [ndir][H/64][2][4][4][Bp][16] (gru_bwd_ks_kernel<true>)
+  unsigned int* rsctr; // its counters, [ndir][H/64] x 32 words (one L2 line each)
 };
 
 SB_DEVINL unsigned long long gtime() {
@@ -685,6 +687,79 @@ SB_DEVINL void bulk_s2peer(uint32_t peer_dst, const void* local_src, uint32_t by
       : "memory");
 }
 
+// ---- reduce-scatter through L2 (gru_bwd_ks_kernel<true>) ---------------------------------------
+// The cluster of the K-split backward kernel serves only the reduce-scatter.  4-CTA clusters cap
+// the resident grid (an H100 holds 30 of them, 120 CTAs), so both directions of H = 1024 (128
+// CTAs) do not fit as one clustered launch; without a cluster they fit as one ordinary cooperative
+// launch of one CTA per SM.  In that mode the "cluster" is a group of 4 consecutive CTAs of a
+// direction (group = cta_in_dir / 4, rank = cta_in_dir % 4) and each step's slices travel
+// through a global staging area [dir][group][parity][dst][src][slice] instead of DSMEM:
+//   * the producer (one epilogue thread) copies its three peer slices from shared memory to the
+//     staging area with bulk copies, waits until those WRITES are complete (wait_group, not
+//     .read), orders them for the generic proxy and arrives on the group's counter (release);
+//   * it then polls the counter (acquire) until all 4 CTAs of the group published the step and
+//     fetches the three slices addressed to it with bulk copies that complete on recvbar, exactly
+//     where the DSMEM copies of the clustered launch complete.
+// Two parities of the staging area are enough: a peer writes parity s & 1 again at step s + 2 at
+// the earliest.  That needs its TMA gather of step s + 2, hence the grid barrier of step s + 1,
+// which counts the owner's arrival after its epilogue of step s + 1; the owner arrives only after
+// recvbar completed for step s + 1, i.e. long after its copies of step s finished reading.
+// (The same mode for gru_fwd_ks_kernel, whose slices are 3x larger, measured 11.22 us per step
+// for both directions at 64 rows against 11.38 for gru_fwd_kernel, and 7.35 against 6.41 at 32
+// rows, H100 80GB HBM3 at 400 W: too little to change the forward's summation order for.)
+SB_DEVINL void bulk_s2g(void* gdst, const void* local_src, uint32_t bytes) {
+  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
+               ::"l"(reinterpret_cast<uint64_t>(gdst)), "r"(smem_u32(local_src)), "r"(bytes)
+               : "memory");
+}
+SB_DEVINL void bulk_g2s(void* dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
+  asm volatile(
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(gsrc)), "r"(bytes), "r"(smem_u32(bar))
+      : "memory");
+}
+
+// One step of the reduce-scatter, issued by one epilogue thread: stage[pr] holds the slice of
+// `slice` floats that belongs to rank pr, recv[crank] already holds the CTA's own.  Arms recvbar
+// for the three incoming slices, which land in recv[src].  L2RS: gslot is this group's staging
+// area of the step's parity, gctr its counter; st (or null) receives two timeline stamps.
+template <bool L2RS>
+SB_DEVINL void ks_exchange(float* recv, const float* stage, uint64_t* recvbar, uint32_t crank,
+                           int slice, float* gslot, unsigned int* gctr, int step,
+                           unsigned long long* st) {
+  const uint32_t bytes = (uint32_t)slice * 4u;
+  mbar_expect_tx(recvbar, (KS - 1) * bytes);
+  if (!L2RS) {
+    for (uint32_t q = 1; q < KS; ++q) {
+      const uint32_t pr = (crank + q) % KS;
+      bulk_s2peer(mapa_shared(smem_u32(recv + (size_t)crank * slice), pr),
+                  stage + (size_t)pr * slice, bytes, mapa_shared(smem_u32(recvbar), pr));
+    }
+    return;
+  }
+  for (uint32_t q = 1; q < KS; ++q) {
+    const uint32_t pr = (crank + q) % KS;
+    bulk_s2g(gslot + ((size_t)pr * KS + crank) * slice, stage + (size_t)pr * slice, bytes);
+  }
+  asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+  asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+  fence_proxy_async_global();   // async-proxy writes -> the release below
+  red_release_gpu_add(gctr, 1u);
+  if (st) st[11] = gtime();
+  unsigned int spins = 0;
+  while (ld_acquire_gpu(gctr) < (unsigned int)(KS * step)) {
+    if (++spins > SB_SPIN_LIMIT) __trap();
+  }
+  if (st) st[12] = gtime();
+  for (uint32_t q = 1; q < KS; ++q) {
+    const uint32_t src = (crank + q) % KS;
+    bulk_g2s(recv + (size_t)src * slice, gslot + ((size_t)crank * KS + src) * slice, bytes,
+             recvbar);
+  }
+}
+
+// L2RS: launched without a cluster, the reduce-scatter goes through L2 (see ks_exchange).
+template <bool L2RS>
 __global__ void __launch_bounds__(GRU_THREADS, 1)
 gru_bwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
                   const __grid_constant__ CUtensorMap tm_d1, const GruBwdParams p) {
@@ -694,8 +769,9 @@ gru_bwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
   const int dir = p.dir0 + blockIdx.x / nC;
   const int cta_in_dir = blockIdx.x % nC;
   const int j0 = cta_in_dir * GRU_HC;                 // own 16 units (elementwise work)
-  const uint32_t crank = cluster_rank();              // == cta_in_dir % 4
+  const uint32_t crank = L2RS ? (uint32_t)(cta_in_dir % KS) : cluster_rank();
   const int k0c = (cta_in_dir / KS) * (KS * GRU_HC);  // first of the cluster's 64 units
+  const int rsg = dir * (nC / KS) + cta_in_dir / KS;  // L2RS: this group's staging area / counter
   const int K3 = 3 * H;
   const int KQ = K3 / KS;                             // this CTA's share of the contraction
   const int nchunks = KQ / 64;
@@ -748,7 +824,7 @@ gru_bwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
   }
   fence_proxy_async_smem();
   __syncthreads();
-  cluster_sync_all();
+  if (!L2RS) cluster_sync_all();
   unsigned int* ctr = p.barrier + dir * 32;   // one L2 line per direction
 
   if (warp == GRU_TMA_WARP) {
@@ -850,17 +926,14 @@ gru_bwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
         if (tid == 0) GRU_STAMP(3);
         // the MMA warpgroup staged the peers' slices: one bulk copy into each peer's receive
         // buffer; the own slice already sits in recv[crank]
-        if (tid == 0) {
-          mbar_expect_tx(recvbar, (uint32_t)((KS - 1) * Bp * 16 * 4));
-          for (uint32_t q = 1; q < KS; ++q) {
-            const uint32_t pr = (crank + q) % KS;
-            bulk_s2peer(mapa_shared(smem_u32(recv + (size_t)crank * Bp * 16), pr),
-                        stage + (size_t)pr * Bp * 16, (uint32_t)(Bp * 16 * 4),
-                        mapa_shared(smem_u32(recvbar), pr));
-          }
-        }
+        if (tid == 0)
+          ks_exchange<L2RS>(recv, stage, recvbar, crank, Bp * 16,
+                            p.rs + ((size_t)rsg * 2 + (step & 1)) * KS * KS * Bp * 16,
+                            p.rsctr + rsg * 32, step,
+                            (p.dbg && blockIdx.x == 0 && step < 64) ? p.dbg + step * 16 : nullptr);
         if (tid == 0) GRU_STAMP(4);
         mbar_wait(recvbar, (step - 1) & 1);
+        if (tid == 0) GRU_STAMP(13);
         if (active) {
 #pragma unroll
           for (int src = 0; src < KS; ++src) {
@@ -933,7 +1006,7 @@ gru_bwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
   }
 
   __syncthreads();
-  cluster_sync_all();
+  if (!L2RS) cluster_sync_all();
 }
 
 // =============================================================================================
@@ -1812,13 +1885,15 @@ static int g_gru_ksplit = 1;   // developer knob: 0 disables the K-split backwar
 // Which K-split flavour: the transposed-accumulator kernels (gru_*_kt_kernel) spend tensor work
 // in proportion to the batch (N = batch) instead of a whole m64 block of batch rows.
 // An H100 holds 30 clusters of 4 one-CTA-per-SM blocks (120 CTAs), so at H = 1024 the two
-// directions (128 CTAs) never fit as one K-split launch: the forward runs gru_fwd_kernel there
-// and the backward gru_bwd_ks_kernel once per direction.  Measured on an H100 80GB HBM3 (400 W
-// power limit), recurrence kernel alone, us per step at T = 247, ONE direction of H = 1024
+// directions (128 CTAs) never fit as one clustered K-split launch: the forward runs
+// gru_fwd_kernel there and the backward gru_bwd_ks_kernel in its L2 reduce-scatter mode, both
+// directions in one launch without a cluster.  Measured on an H100 80GB HBM3 (400 W power
+// limit), recurrence kernel alone, us per step at T = 247, ONE direction of H = 1024
 // (kt | ks): forward 4.12 | 4.17 at 8 rows, 4.59 | 4.34 at 16, 7.73 | 5.46 at 32, 14.68 | 8.38 at
 // 64; backward 3.17 | 4.28 at 8, 4.08 | 4.37 at 16, 6.09 | 5.12 at 32, 8.15 | 7.94 at 64.  Both
-// directions at 64 rows: gru_fwd_kernel 11.7; backward 23.4 with gru_bwd_kernel, 15.5 with the
-// two one-direction gru_bwd_ks_kernel launches.
+// directions: gru_fwd_kernel 6.41 at 32 rows, 11.38 at 64; backward 23.4 at 64 rows with
+// gru_bwd_kernel, and with gru_bwd_ks_kernel 7.29 at 32 rows / 10.25 at 64 in the L2 mode
+// against 10.16 / 15.50 as two one-direction clustered launches (tools/gru_l2rs_bench.py).
 // Developer knob (sb_debug_gru_flags): 16 forces them, 8 disables them.
 static bool gru_use_kt(int Bp, bool backward) {
   if (g_gru_ablate & 8) return false;
@@ -1877,7 +1952,9 @@ extern "C" int sb_debug_gru_timeline(void* dev_buffer) {
 // off-path stores (timing only: results become wrong); 8 / 16: never / always use the
 // transposed-accumulator K-split kernels (default: by batch size, see gru_use_kt); 32: disable
 // the K-split forward kernels;
-// 64 / 128: polling mode of the grid barrier in the K-split kernels (see grid_wait)
+// 64 / 128: polling mode of the grid barrier in the K-split kernels (see grid_wait);
+// 256 / 512: always (wherever the K-split backward kernel applies) / never use its L2
+// reduce-scatter mode (see ks_exchange and sb_gru_bwd)
 extern "C" int sb_debug_gru_flags(int flags) {
   sb::g_gru_ablate = flags;
   return SB_OK;
@@ -1954,6 +2031,18 @@ extern "C" int sb_gru_plan(int Bp, int H, int ndir, int* Hp) {
 static size_t gru_ws_counters_bytes(int ndir) {
   (void)ndir;
   return 1024;
+}
+
+// The L2 reduce-scatter of the K-split backward kernel (ks_exchange), at the END of its
+// workspace: one counter line per direction and group of 4 CTAs, then the staging area, two
+// parities of [dst][src] slices of Bp x 16 floats.  Nothing outside the K-split domain.  Only the
+// counters need zeroing: every slice is written before it is read.
+static size_t gru_rs_groups(int H, int ndir) {
+  return H % (KS * 64) == 0 ? (size_t)ndir * (H / (KS * GRU_HC)) : 0;
+}
+static size_t gru_rs_bytes(int Bp, int H, int ndir, size_t* zeroed) {
+  *zeroed = gru_rs_groups(H, ndir) * 128;
+  return *zeroed + gru_rs_groups(H, ndir) * 2 * KS * KS * (size_t)Bp * GRU_HC * sizeof(float);
 }
 
 extern "C" int sb_gru_fwd_workspace_size(int Bp, int H, int ndir, size_t* bytes) {
@@ -2041,7 +2130,9 @@ extern "C" int sb_gru_bwd_workspace_size(int Bp, int H, int ndir, size_t* bytes)
   // counters + the double-buffered exchange of dgh_t (Bp x 3H bf16 per direction and parity; the
   // tile-major form of the K-split kernel rounds 3H up to whole 64-column chunks)
   const size_t k3p = (size_t)((3 * H + 63) / 64) * 64;
-  *bytes = gru_ws_counters_bytes(ndir) + (size_t)ndir * 2 * Bp * k3p * sizeof(bf16) + 1024;
+  size_t z = 0;
+  *bytes = gru_ws_counters_bytes(ndir) + (size_t)ndir * 2 * Bp * k3p * sizeof(bf16) + 1024 +
+           gru_rs_bytes(Bp, H, ndir, &z);
   return SB_OK;
 }
 
@@ -2073,9 +2164,13 @@ extern "C" int sb_gru_bwd(const float* dy, const float* y, const float* gates,
   const int K3 = 3 * H;
   size_t smem = 0;
   const int nC_ = H / GRU_HC;
+  size_t rs_zeroed = 0;
+  const size_t rs_at = need - gru_rs_bytes(Bp, H, ndir, &rs_zeroed);
+  p.rsctr = reinterpret_cast<unsigned int*>(ws + rs_at);
+  p.rs = reinterpret_cast<float*>(ws + rs_at + rs_zeroed);
   // counters and barrier words start at zero; the exchange tiles too (columns past 3H of a
   // partial chunk are never written and must read as zero)
-  if (cudaMemsetAsync(workspace, 0, need, stream) != cudaSuccess) return SB_ERR_CUDA;
+  if (cudaMemsetAsync(workspace, 0, rs_at + rs_zeroed, stream) != cudaSuccess) return SB_ERR_CUDA;
   // ---- preferred: K-split over 4-CTA clusters ----
   if (g_gru_ksplit && H % 256 == 0 && nC_ % KS == 0 && (K3 / KS / 64) <= 16) {
     const int nq = K3 / KS / 64;
@@ -2092,23 +2187,39 @@ extern "C" int sb_gru_bwd(const float* dy, const float* y, const float* gates,
       void* kargs[] = {(void*)&tq[0], (void*)&tq[1], (void*)&p};
       const size_t kt_smem = (size_t)nq * Bp * 128 + (size_t)nq * 64 * 128 +
                              (size_t)(2 * KS - 1) * GRU_HC * (Bp + 4) * 4 + 1024 + 256;
-      if (gru_use_kt(Bp, true) && Bp <= 64 && kt_smem <= 227 * 1024) {
+      if (gru_use_kt(Bp, true) && !(g_gru_ablate & 256) && Bp <= 64 && kt_smem <= 227 * 1024) {
         const void* kt = Bp > 32   ? (const void*)gru_bwd_kt_kernel<4>
                          : Bp > 16 ? (const void*)gru_bwd_kt_kernel<2>
                                    : (const void*)gru_bwd_kt_kernel<1>;
         rc = gru_launch_exact(kt, ndir * nC_, KS, kt_smem, kargs, stream);
         if (rc == SB_OK) return SB_OK;
       }
-      rc = gru_launch_exact((const void*)gru_bwd_ks_kernel, ndir * nC_, KS, ks_smem, kargs, stream);
-      if (rc == SB_OK) return SB_OK;
-      // Both directions do not fit as 4-CTA clusters (an H100 holds 30 of them, 120 CTAs, against
-      // 128 at H = 1024): run the directions one after the other, each with its own barrier
-      // counter.  Still faster than the plain kernel, whose every CTA gathers all of dgh_t.
+      // 1. both directions as 4-CTA clusters, reduce-scattering through DSMEM
+      const void* ks = (const void*)gru_bwd_ks_kernel<false>;
+      const void* ks_l2 = (const void*)gru_bwd_ks_kernel<true>;
+      rc = SB_ERR_UNSUPPORTED;
+      if (!(g_gru_ablate & 256)) {
+        rc = gru_launch_exact(ks, ndir * nC_, KS, ks_smem, kargs, stream);
+        if (rc == SB_OK) return SB_OK;
+      }
+      // 2. Both directions do not fit as 4-CTA clusters (an H100 holds 30 of them, 120 CTAs,
+      // against 128 at H = 1024), but fit without a cluster, one CTA per SM: the same kernel
+      // reduce-scattering through L2, both directions in one cooperative launch
+      // (sb_debug_gru_cluster(0) then reports 1).  Developer knobs: 256 forces it wherever the
+      // K-split domain holds, 512 disables it.
+      if (rc == SB_ERR_UNSUPPORTED && !(g_gru_ablate & 512) &&
+          gru_coresident(ks_l2, ndir * nC_, ks_smem)) {
+        rc = gru_launch(ks_l2, ndir * nC_, 1, ks_smem, kargs, stream);
+        if (rc == SB_OK) return SB_OK;
+      }
+      // 3. Neither fits (fewer SMs than CTAs, e.g. a 114-SM part): the directions one after the
+      // other as clustered launches, each with its own barrier counter.  Still faster than the
+      // plain kernel, whose every CTA gathers all of dgh_t.
       if (rc == SB_ERR_UNSUPPORTED && ndir == 2) {
-        rc = gru_launch_exact((const void*)gru_bwd_ks_kernel, nC_, KS, ks_smem, kargs, stream);
+        rc = gru_launch_exact(ks, nC_, KS, ks_smem, kargs, stream);
         if (rc == SB_OK) {
           p.dir0 = 1;   // kernel parameters are copied at launch
-          return gru_launch_exact((const void*)gru_bwd_ks_kernel, nC_, KS, ks_smem, kargs, stream);
+          return gru_launch_exact(ks, nC_, KS, ks_smem, kargs, stream);
         }
       }
     }

@@ -68,13 +68,17 @@ def gru_padded_width(Bp, H, ndir):
 def _apply_env_knobs():
     """Developer knobs (profiling under ncu cannot replay clustered cooperative launches):
     SB_GRU_KSPLIT=0 disables the K-split backward kernel, SB_GRU_CLUSTER=<1|2|4|8> sets the
-    preferred cluster size of the other GRU kernels."""
+    preferred cluster size of the other GRU kernels, SB_GRU_FLAGS=<int> sets sb_debug_gru_flags
+    (e.g. 512: no L2 reduce-scatter mode, the backward's two clustered one-direction launches at
+    H = 1024; 256: that mode wherever the K-split backward kernel applies)."""
     import os
     lib = _lib.load()
     if os.environ.get("SB_GRU_KSPLIT") is not None:
         lib.sb_debug_gru_ksplit(int(os.environ["SB_GRU_KSPLIT"]))
     if os.environ.get("SB_GRU_CLUSTER") is not None:
         lib.sb_debug_gru_cluster(int(os.environ["SB_GRU_CLUSTER"]))
+    if os.environ.get("SB_GRU_FLAGS") is not None:
+        lib.sb_debug_gru_flags(int(os.environ["SB_GRU_FLAGS"]))
 
 
 _knobs_applied = False

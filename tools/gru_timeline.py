@@ -39,17 +39,22 @@ print("mode:", MODE)
 raw = dbg.cpu().numpy()
 d = raw[:1024].reshape(64, 16)
 # stamp index -> phase; P: producer warp, M: MMA warpgroup, E: epilogue thread 0.  The K-split
-# kernels stamp 4 after issuing the reduce-scatter bulk copies (the plain kernels: accbuf read).
+# kernels stamp 4 after issuing the reduce-scatter (the plain kernels: accbuf read) and 13 once
+# the backward's peer slices have arrived; in its L2 reduce-scatter mode (flags 256, or the
+# default at H = 1024 on a 132-SM card) 11 when the CTA's own slices are written to L2 and
+# published, 12 when the group's counter shows all four published.
 names = ["P:grid_wait done", "P:tma issued", "M:product staged", "E:accfull",
          "E:reduce-scatter issued", "E:xn stored" if MODE == "fwd" else "E:dgh stored",
-         "E:proxy fence", "E:epi barrier", None, "E:arrived", "E:offpath done"]
+         "E:proxy fence", "E:epi barrier", None, "E:arrived", "E:offpath done",
+         "E:L2 slices published", "E:L2 group complete", "E:slices received"]
+order = [0, 1, 2, 3, 11, 12, 4, 13, 5, 6, 7, 9, 10]
 for step in (11, 40):
     base = d[step - 1][9]   # previous step's arrival by this CTA
     print("step %d (ns since this CTA's previous arrive):" % step)
-    for i, n in enumerate(names):
-        if n is None:
+    for i in order:
+        if d[step][i] == 0:   # not stamped by this kernel
             continue
-        print("   %-22s %7d" % (n, d[step][i] - base))
+        print("   %-22s %7d" % (names[i], d[step][i] - base))
 print("cluster size used:", lib.sb_debug_gru_cluster(0))
 print("mean step period (ns):", (d[60][9] - d[10][9]) / 50.0)
 

@@ -50,4 +50,12 @@ cfg_p["encoder"]["rnn"]["dim"] = 100
 tp = Transducer(80, 28, cfg_p).cuda()
 l7 = tp.loss((inputs, labels)); l7.backward()
 print("padded Transducer dim 100 ok", l7.item(), [len(p) for p in tp.infer((inputs, labels))])
+# the L2 reduce-scatter mode of the K-split backward recurrence kernel, forced
+from speech_b200 import _lib
+_lib.load().sb_debug_gru_flags(256)
+mr = CTC(80, 28, cfg).cuda()
+l8 = mr.loss((inputs, labels)); l8.backward()
+torch.cuda.synchronize()
+_lib.load().sb_debug_gru_flags(0)
+print("L2 reduce-scatter GRU ok", l8.item())
 torch.cuda.synchronize()
