@@ -430,9 +430,13 @@ int sb_debug_umma_mn(int lbo_bytes, int sbo_bytes, int kadv_bytes);
  * the transposed-accumulator K-split kernels, 32 = no K-split forward kernel, 64 / 128 = polling
  * mode of the grid barrier, 256 / 512 = always (wherever the K-split backward kernel applies) /
  * never use its L2 reduce-scatter mode (the mode the backward uses when both directions do not
- * fit as thread-block clusters but do fit without); 1 / 2 are timing ablations (results become
- * wrong). */
+ * fit as thread-block clusters but do fit without), 1024 = the K-split forward over 2-CTA clusters
+ * wherever it applies (H % 128 == 0, at most 64 batch rows; by default only from H = 512 up);
+ * 1 / 2 are timing ablations (results become wrong). */
 int sb_debug_gru_flags(int flags);
+/* Developer hook: which forward recurrence kernel the last sb_gru_fwd launched: "plain", "kt"
+ * (transposed-accumulator K split), "ks4" / "ks2" (K split over 4- / 2-CTA clusters), "none". */
+const char* sb_debug_gru_fwd_kernel(void);
 /* Developer hook: enable (1, default) / disable (0) the K-split backward GRU kernel. */
 int sb_debug_gru_ksplit(int enable);
 /* Developer hook: set the preferred thread-block-cluster size (1, 2, 4 or 8) of the GRU kernels;

@@ -89,6 +89,7 @@ SIGNATURES = {
     "sb_debug_gru_cluster": (_c_int, [_c_int]),
     "sb_debug_gru_ksplit": (_c_int, [_c_int]),
     "sb_debug_gru_flags": (_c_int, [_c_int]),
+    "sb_debug_gru_fwd_kernel": (ctypes.c_char_p, []),
     "sb_debug_umma_mn": (_c_int, [_c_int, _c_int, _c_int]),
     "sb_edit_distance": (_c_ll, [_vp, _c_ll, _vp, _c_ll]),
     "sb_log_specgram": (_c_int, [_vp, _vp, _vp, _c_int, _c_int, _c_int, ctypes.c_double, _fl, _vp,

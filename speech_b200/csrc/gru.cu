@@ -704,7 +704,7 @@ SB_DEVINL void bulk_s2peer(uint32_t peer_dst, const void* local_src, uint32_t by
 // the earliest.  That needs its TMA gather of step s + 2, hence the grid barrier of step s + 1,
 // which counts the owner's arrival after its epilogue of step s + 1; the owner arrives only after
 // recvbar completed for step s + 1, i.e. long after its copies of step s finished reading.
-// (The same mode for gru_fwd_ks_kernel, whose slices are 3x larger, measured 11.22 us per step
+// (The same mode for gru_fwd_ks_kernel<4>, whose slices are 3x larger, measured 11.22 us per step
 // for both directions at 64 rows against 11.38 for gru_fwd_kernel, and 7.35 against 6.41 at 32
 // rows, H100 80GB HBM3 at 400 W: too little to change the forward's summation order for.)
 SB_DEVINL void bulk_s2g(void* gdst, const void* local_src, uint32_t bytes) {
@@ -1010,40 +1010,55 @@ gru_bwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
 }
 
 // =============================================================================================
-// forward, K-split variant: the 4 CTAs of a cluster jointly own 64 hidden units.
+// forward, K-split variant: the KS CTAs of a cluster (KS = 4 or 2) jointly own KS x 16 hidden
+// units.
 //
 // Measured on gru_fwd_kernel (globaltimer timeline, H = 1024, B = 64, 7.4 us/step): 3.5 us pass
 // between "h_{t-1} is complete" and "all MMAs retired", for a gather of 128 KB per CTA - the same
 // ~30 B/ns per SM whether it is fetched as tensor boxes or as contiguous bulk copies, with or
 // without cluster multicast: 128 CTAs x 128 KB = 16 MB of L2->SM traffic per step is the bound,
 // next to 480 KB of shared-memory traffic (TMA writes + MMA operand reads of a 128-row A tile).
-// Here CTA r of a cluster contracts only the r-th QUARTER of K = H for all 64 units of its
-// cluster and all three gates,
-//     D_r[batch x 192] = h_{t-1}[:, quarter r] * W_hh[(r|z|n) x 64 units, quarter r]^T,
-// i.e. it gathers 32 KB instead of 128 KB (the whole quarter stays resident: no ring) and issues
-// 16 MMAs of N = 192 instead of 64 of N = 48; the four partial products are reduce-scattered
-// through distributed shared memory exactly as in gru_bwd_ks_kernel (each CTA receives the
-// 3 x 16 columns of its own units from its three peers: 36 KB per CTA and step).
-// Requires cluster size 4, H % 256 == 0, Bp <= 64.
+// Here CTA r of a cluster contracts only the r-th of KS slices of K = H, for all KS x 16 units of
+// its cluster and all three gates (KS = 4: N = 192, quarters of K),
+//     D_r[batch x 3*KS*16] = h_{t-1}[:, slice r] * W_hh[(r|z|n) x KS*16 units, slice r]^T,
+// i.e. it gathers H/KS columns of h_{t-1} instead of all H (KS = 4: 32 KB instead of 128 KB at
+// H = 1024, Bp = 64; the whole slice stays resident: no ring) and issues 4*H/(KS*64) MMAs of
+// N = 3*KS*16 instead of H/16 of N = 48; the KS partial products are reduce-scattered through
+// distributed shared memory exactly as in gru_bwd_ks_kernel (each CTA receives the 3 x 16 columns
+// of its own units from each of its KS - 1 peers: 12 KB per peer at Bp = 64) and summed in rank
+// order, so the result does not depend on arrival order.
+// KS = 2 exists because an H100 holds at most 30 clusters of 4 such CTAs (120): both directions of
+// H = 1024 (128 CTAs) do not fit with KS = 4, but fit as 64 clusters of 2, and each CTA still
+// gathers half of h_{t-1} (64 KB at Bp = 64) instead of all of it.  Shared memory at Bp = 64,
+// H = 1024 (operand + weights + recv/stage, plus 1.5 KB of barriers and alignment): KS = 4
+// 32 + 96 + 96 KB, KS = 2 64 + 96 + 48 KB.  Measured on an H100 80GB HBM3 at 400 W, both
+// directions of H = 1024, T = 247: 7.50 us per step at 64 rows and 5.10 at 32 with KS = 2,
+// against 11.11 and 6.54 for gru_fwd_kernel.  The globaltimer timeline (tools/gru_timeline.py) of
+// KS = 2 at 64 rows: 2.8 us from the CTA's own arrive until the grid barrier completes, 0.45 us to
+// issue the gather, 1.5 us until the product is staged, 1.5-1.7 us for the exchange and gate math
+// until h_t is stored, 1.0-1.25 us more until the arrive.
+// Requires cluster size KS, H % (KS * 64) == 0, Bp <= 64.
 // =============================================================================================
+template <int KS>
 __global__ void __launch_bounds__(GRU_THREADS, 1)
 gru_fwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
                   const __grid_constant__ CUtensorMap tm_d1, const GruFwdParams p) {
+  static_assert(KS == 2 || KS == 4, "gru_fwd_ks_kernel: K split 2 or 4 ways");
   extern __shared__ uint8_t smem_raw[];
   const int H = p.H, Bp = p.Bp, T = p.T;
   const int nC = H / GRU_HC;
   const int dir = blockIdx.x / nC;
   const int cta_in_dir = blockIdx.x % nC;
   const int j0 = cta_in_dir * GRU_HC;                 // own 16 units (gate math, stores)
-  const uint32_t crank = cluster_rank();              // == cta_in_dir % 4
-  const int k0c = (cta_in_dir / KS) * (KS * GRU_HC);  // first of the cluster's 64 units
+  const uint32_t crank = cluster_rank();              // == cta_in_dir % KS
+  const int k0c = (cta_in_dir / KS) * (KS * GRU_HC);  // first of the cluster's KS*16 units
   const int KQ = H / KS;                              // this CTA's share of the contraction
   const int nchunks = KQ / 64;
-  constexpr int NCOL = 3 * KS * GRU_HC;               // 192 accumulator columns: gate x 64 units
-  constexpr int WCHUNK = NCOL * 128;                  // 192 rows x 64 bf16
+  constexpr int NCOL = 3 * KS * GRU_HC;               // accumulator columns: gate x KS*16 units
+  constexpr int WCHUNK = NCOL * 128;                  // NCOL rows x 64 bf16
   constexpr int RW = 3 * GRU_HC;                      // 48 floats received per row and peer
   const int stride = Bp * 128;
-  const int ring_bytes = nchunks * stride;            // the whole quarter is resident
+  const int ring_bytes = nchunks * stride;            // the whole K slice is resident
   const int wbytes = nchunks * WCHUNK;
   // carve: ring | weights | recv | barriers.  (The 128-row A read of the last chunk runs past the
   // ring into the weights: finite data, rows >= Bp are never used.)
@@ -1066,7 +1081,7 @@ gru_fwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
     reinterpret_cast<uint4*>(base)[k] = make_uint4(0, 0, 0, 0);
   __syncthreads();
   {
-    // resident operand: rows = (gate, unit of the cluster), columns = this CTA's K quarter
+    // resident operand: rows = (gate, unit of the cluster), columns = this CTA's K slice
     const int pieces_per_row = nchunks * 8;
     for (int k = tid; k < NCOL * pieces_per_row; k += GRU_THREADS) {
       const int r = k / pieces_per_row, pc = k % pieces_per_row;
@@ -1094,7 +1109,7 @@ gru_fwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
   unsigned int* ctr = p.barrier + dir * 32;   // one L2 line per direction
 
   if (warp == GRU_TMA_WARP) {
-    // ===================== TMA producer: this CTA's K quarter of h_{t-1} =====================
+    // ===================== TMA producer: this CTA's K slice of h_{t-1} =======================
     if (lane == 0) {
       for (int step = 1; step < T; ++step) {
         const int t = dir == 0 ? step : (T - 1 - step);
@@ -1109,8 +1124,8 @@ gru_fwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
       }
     }
   } else if (warp >= GRU_MMA_WARP) {
-    // ===================== MMA warpgroup: D[Bp x (gate, 64 units)] for this K quarter ========
-    // Column gg*64 + pr*16 + u belongs to unit u of peer pr: it is written straight into
+    // ===================== MMA warpgroup: D[Bp x (gate, KS*16 units)] for this K slice ========
+    // Column gg*KS*16 + pr*16 + u belongs to unit u of peer pr: it is written straight into
     // stage[pr] (row pitch RW = 48, gate-major), the CTA's own columns into recv[crank].
     const int t = tid & 127;
     for (int step = 1; step < T; ++step) {
@@ -1130,9 +1145,9 @@ gru_fwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
       wgmma_fence_regs(d);
 #pragma unroll
       for (int i = 0; i < NCOL / 2; ++i) {
-        const int r = wg_frag_row(t, i), col = wg_frag_col(t, i);
-        const int gg = col >> 6, u = col & 15;
-        const uint32_t pr = (uint32_t)((col >> 4) & 3);
+        const int r = wg_frag_row(t, i), col = wg_frag_col(t, i);   // col >= 0
+        const int gg = (uint32_t)col / (KS * GRU_HC), u = col & 15;
+        const uint32_t pr = (uint32_t)(col >> 4) % KS;
         if (r < Bp)
           (pr == crank ? recv : stage)[((size_t)pr * Bp + r) * RW + gg * GRU_HC + u] = d[i];
       }
@@ -1171,9 +1186,10 @@ gru_fwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
       if (step > 0) {
         mbar_wait(accfull, (step - 1) & 1);
         if (tid == 0) GRU_STAMP(3);
-        // ---- reduce-scatter of the four partial products: the MMA warpgroup staged the three
+        // ---- reduce-scatter of the KS partial products: the MMA warpgroup staged the KS - 1
         // slices that belong to the peers, each leaves as ONE bulk copy into the peer's receive
-        // buffer; the CTA's own slice already sits in recv[crank] ----
+        // buffer; the CTA's own slice already sits in recv[crank].  The slices are summed in
+        // rank order below, whatever order they arrived in ----
         if (tid == 0) {
           mbar_expect_tx(recvbar, (uint32_t)((KS - 1) * Bp * RW * 4));
           for (uint32_t q = 1; q < KS; ++q) {
@@ -1244,7 +1260,7 @@ gru_fwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
 // =============================================================================================
 // forward, K split with the accumulator TRANSPOSED: D^T[(gate, unit) x batch].
 //
-// Same partition as gru_fwd_ks_kernel (cluster of 4 owns 64 units, CTA r contracts K quarter r),
+// Same partition as gru_fwd_ks_kernel<4> (cluster of 4 owns 64 units, CTA r contracts K quarter r),
 // but the resident weight slice is the M-side operand and h_{t-1} the N-side one:
 //     D[192 x NB] = W[(r|z|n) x 64 units, quarter r] * h_{t-1}[:, quarter r]^T
 // issued as three wgmma m64 blocks of weight rows with N = NB (the batch rounded up to 16).  The
@@ -1828,6 +1844,13 @@ static int gru_ring_slots(int wbytes, int Bp, int nchunks, int acc_cols, int* gc
 
 static int g_gru_cluster = 4;   // preferred cluster size (developer knob: sb_debug_gru_cluster)
 static int g_gru_last_cluster = 0;
+// which forward recurrence kernel the last sb_gru_fwd launched (sb_debug_gru_fwd_kernel)
+enum { GRU_FWD_NONE, GRU_FWD_PLAIN, GRU_FWD_KT, GRU_FWD_KS4, GRU_FWD_KS2 };
+static int g_gru_last_fwd = GRU_FWD_NONE;
+static int gru_fwd_launched(int kind) {
+  g_gru_last_fwd = kind;
+  return SB_OK;
+}
 
 static int gru_cluster_size(int nC) {
   int cs = g_gru_cluster;
@@ -1885,13 +1908,14 @@ static int g_gru_ksplit = 1;   // developer knob: 0 disables the K-split backwar
 // Which K-split flavour: the transposed-accumulator kernels (gru_*_kt_kernel) spend tensor work
 // in proportion to the batch (N = batch) instead of a whole m64 block of batch rows.
 // An H100 holds 30 clusters of 4 one-CTA-per-SM blocks (120 CTAs), so at H = 1024 the two
-// directions (128 CTAs) never fit as one clustered K-split launch: the forward runs
-// gru_fwd_kernel there and the backward gru_bwd_ks_kernel in its L2 reduce-scatter mode, both
-// directions in one launch without a cluster.  Measured on an H100 80GB HBM3 (400 W power
-// limit), recurrence kernel alone, us per step at T = 247, ONE direction of H = 1024
+// directions (128 CTAs) never fit as one 4-CTA clustered K-split launch: the forward runs
+// gru_fwd_ks_kernel<2> over 2-CTA clusters there and the backward gru_bwd_ks_kernel in its L2
+// reduce-scatter mode, both directions in one launch each.  Measured on an H100 80GB HBM3 (400 W
+// power limit), recurrence kernel alone, us per step at T = 247, ONE direction of H = 1024
 // (kt | ks): forward 4.12 | 4.17 at 8 rows, 4.59 | 4.34 at 16, 7.73 | 5.46 at 32, 14.68 | 8.38 at
 // 64; backward 3.17 | 4.28 at 8, 4.08 | 4.37 at 16, 6.09 | 5.12 at 32, 8.15 | 7.94 at 64.  Both
-// directions: gru_fwd_kernel 6.41 at 32 rows, 11.38 at 64; backward 23.4 at 64 rows with
+// directions: forward 6.54 at 32 rows / 11.11 at 64 with gru_fwd_kernel against 5.10 / 7.50 with
+// gru_fwd_ks_kernel<2> (tools/gru_fwd_ks2_bench.py, alternated); backward 23.4 at 64 rows with
 // gru_bwd_kernel, and with gru_bwd_ks_kernel 7.29 at 32 rows / 10.25 at 64 in the L2 mode
 // against 10.16 / 15.50 as two one-direction clustered launches (tools/gru_l2rs_bench.py).
 // Developer knob (sb_debug_gru_flags): 16 forces them, 8 disables them.
@@ -1954,7 +1978,8 @@ extern "C" int sb_debug_gru_timeline(void* dev_buffer) {
 // the K-split forward kernels;
 // 64 / 128: polling mode of the grid barrier in the K-split kernels (see grid_wait);
 // 256 / 512: always (wherever the K-split backward kernel applies) / never use its L2
-// reduce-scatter mode (see ks_exchange and sb_gru_bwd)
+// reduce-scatter mode (see ks_exchange and sb_gru_bwd); 1024: the K-split forward over 2-CTA
+// clusters wherever it applies (H % 128 == 0, batch rows <= 64), skipping the 4-CTA ones
 extern "C" int sb_debug_gru_flags(int flags) {
   sb::g_gru_ablate = flags;
   return SB_OK;
@@ -1970,6 +1995,12 @@ extern "C" int sb_debug_gru_cluster(int cluster_size) {
     return -1;
   sb::g_gru_cluster = cluster_size;
   return sb::g_gru_last_cluster;
+}
+// which forward recurrence kernel the last sb_gru_fwd launched: "plain" (gru_fwd_kernel), "kt"
+// (gru_fwd_kt_kernel), "ks4" / "ks2" (gru_fwd_ks_kernel<4> / <2>); "none" before the first
+extern "C" const char* sb_debug_gru_fwd_kernel(void) {
+  static const char* const names[] = {"none", "plain", "kt", "ks4", "ks2"};
+  return names[sb::g_gru_last_fwd];
 }
 
 static int gru_check(int T, int Bp, int H, int ndir) {
@@ -2045,6 +2076,14 @@ static size_t gru_rs_bytes(int Bp, int H, int ndir, size_t* zeroed) {
   return *zeroed + gru_rs_groups(H, ndir) * 2 * KS * KS * (size_t)Bp * GRU_HC * sizeof(float);
 }
 
+// Dynamic shared memory of gru_fwd_ks_kernel<ks>: the K slice of h_{t-1} and of the weights,
+// recv + stage ([ks][Bp][48] fp32 each), barriers and bias, alignment.
+static size_t gru_fwd_ks_smem(int ks, int Bp, int H) {
+  const size_t nq = (size_t)H / ks / 64;
+  return nq * Bp * 128 + nq * (3 * ks * GRU_HC) * 128 + (size_t)2 * ks * Bp * 3 * GRU_HC * 4 +
+         1024 + 512;
+}
+
 extern "C" int sb_gru_fwd_workspace_size(int Bp, int H, int ndir, size_t* bytes) {
   if (!bytes || Bp <= 0 || H <= 0 || (ndir != 1 && ndir != 2)) return SB_ERR_INVALID;
   (void)Bp;
@@ -2072,36 +2111,55 @@ extern "C" int sb_gru_fwd(const float* gi, const void* whh_bf16, const float* bh
   const int ring = gru_fwd_ring(Bp, H, &gc, &smem);
   if (ring < 0) return SB_ERR_UNSUPPORTED;
 
-  // ---- preferred: K-split over 4-CTA clusters (H % 256 == 0, batch rows <= 64) ----
-  if (!(g_gru_ablate & 32) && H % 256 == 0 && nC % KS == 0 && Bp <= 64) {
-    const int nq = H / KS / 64;
-    const size_t ks_smem = (size_t)nq * Bp * 128 + (size_t)nq * 192 * 128 +
-                           (size_t)2 * KS * Bp * 48 * 4 + 1024 + 512;
-    if (ks_smem <= 227 * 1024) {
-      GruFwdParams q;
-      q.gi = gi; q.whh = reinterpret_cast<const bf16*>(whh_bf16); q.bhh = bhh; q.y = y;
-      q.xn = reinterpret_cast<bf16*>(xn_bf16); q.xnT = nullptr; q.gates = gates;
-      q.barrier = barrier; q.T = T; q.Bp = Bp; q.H = H; q.ndir = ndir;
-      q.dbg = g_gru_dbg; q.ablate = g_gru_ablate & 195; q.ring = nq; q.gc = 1;
-      CUtensorMap tq[2];
-      for (int d = 0; d < 2; ++d) {
-        const int dd = d < ndir ? d : 0;
-        rc = make_tmap_bf16_2d(&tq[d], q.xn + (size_t)dd * H, (long long)T * Bp, H,
-                               (long long)ndir * H, Bp);
-        if (rc != SB_OK) return rc;
+  // ---- preferred: K-split over clusters of KS CTAs (H % (KS * 64) == 0, batch rows <= 64) ----
+  // Tried in this order, each where its grid of 1-CTA-per-SM clusters is co-resident: the
+  // transposed-accumulator flavour (small batches, see gru_use_kt) and gru_fwd_ks_kernel<4> over
+  // 4-CTA clusters, then gru_fwd_ks_kernel<2> over 2-CTA clusters from H = 512 up (both
+  // directions of H = 1024 on a 132-SM H100: 128 CTAs fit as 2-CTA clusters, not as 4-CTA ones).
+  // Developer knobs: 32 disables all of them, 1024 skips straight to KS = 2 at any width.
+  if (!(g_gru_ablate & 32) && H % 128 == 0 && Bp <= 64) {
+    GruFwdParams q;
+    q.gi = gi; q.whh = reinterpret_cast<const bf16*>(whh_bf16); q.bhh = bhh; q.y = y;
+    q.xn = reinterpret_cast<bf16*>(xn_bf16); q.xnT = nullptr; q.gates = gates;
+    q.barrier = barrier; q.T = T; q.Bp = Bp; q.H = H; q.ndir = ndir;
+    q.dbg = g_gru_dbg; q.ablate = g_gru_ablate & 195; q.gc = 1;
+    CUtensorMap tq[2];
+    for (int d = 0; d < 2; ++d) {
+      const int dd = d < ndir ? d : 0;
+      rc = make_tmap_bf16_2d(&tq[d], q.xn + (size_t)dd * H, (long long)T * Bp, H,
+                             (long long)ndir * H, Bp);
+      if (rc != SB_OK) return rc;
+    }
+    void* kargs[] = {(void*)&tq[0], (void*)&tq[1], (void*)&q};   // q is copied at launch
+    if (!(g_gru_ablate & 1024) && H % 256 == 0) {
+      const int nq = H / KS / 64;
+      const size_t ks_smem = gru_fwd_ks_smem(KS, Bp, H);   // KS = 4
+      q.ring = nq;
+      if (ks_smem <= 227 * 1024) {
+        const size_t kt_smem = (size_t)nq * Bp * 128 + (size_t)nq * 192 * 128 +
+                               (size_t)(2 * KS - 1) * 48 * (Bp + 4) * 4 + 1024 + 512;
+        if (gru_use_kt(Bp, false) && kt_smem <= 227 * 1024) {
+          const void* kt = Bp > 32   ? (const void*)gru_fwd_kt_kernel<4>
+                           : Bp > 16 ? (const void*)gru_fwd_kt_kernel<2>
+                                     : (const void*)gru_fwd_kt_kernel<1>;
+          rc = gru_launch_exact(kt, ndir * nC, KS, kt_smem, kargs, stream);
+          if (rc == SB_OK) return gru_fwd_launched(GRU_FWD_KT);
+        }
+        rc = gru_launch_exact((const void*)gru_fwd_ks_kernel<KS>, ndir * nC, KS, ks_smem, kargs,
+                              stream);
+        if (rc == SB_OK) return gru_fwd_launched(GRU_FWD_KS4);
       }
-      void* kargs[] = {(void*)&tq[0], (void*)&tq[1], (void*)&q};
-      const size_t kt_smem = (size_t)nq * Bp * 128 + (size_t)nq * 192 * 128 +
-                             (size_t)(2 * KS - 1) * 48 * (Bp + 4) * 4 + 1024 + 512;
-      if (gru_use_kt(Bp, false) && kt_smem <= 227 * 1024) {
-        const void* kt = Bp > 32   ? (const void*)gru_fwd_kt_kernel<4>
-                         : Bp > 16 ? (const void*)gru_fwd_kt_kernel<2>
-                                   : (const void*)gru_fwd_kt_kernel<1>;
-        rc = gru_launch_exact(kt, ndir * nC, KS, kt_smem, kargs, stream);
-        if (rc == SB_OK) return SB_OK;
-      }
-      rc = gru_launch_exact((const void*)gru_fwd_ks_kernel, ndir * nC, KS, ks_smem, kargs, stream);
-      if (rc == SB_OK) return SB_OK;
+    }
+    // KS = 2 by default only from H = 512 up: below, the exchange costs more than halving the
+    // gather saves.  H100 80GB HBM3 at 400 W, T = 247, us per step, gru_fwd_kernel | KS = 2 at 64
+    // rows: H = 128 one direction 3.86 | 4.24, both directions H = 384 4.80 | 5.11, H = 640
+    // 6.44 | 5.74, H = 896 8.90 | 6.88, H = 1024 11.07 | 7.49 (tools/gru_fwd_ks2_bench.py).
+    const size_t ks2_smem = gru_fwd_ks_smem(2, Bp, H);
+    if (ks2_smem <= 227 * 1024 && (H >= 512 || (g_gru_ablate & 1024))) {
+      q.ring = H / 2 / 64;
+      rc = gru_launch_exact((const void*)gru_fwd_ks_kernel<2>, ndir * nC, 2, ks2_smem, kargs,
+                            stream);
+      if (rc == SB_OK) return gru_fwd_launched(GRU_FWD_KS2);
     }
   }
 
@@ -2121,8 +2179,9 @@ extern "C" int sb_gru_fwd(const float* gi, const void* whh_bf16, const float* bh
     if (rc != SB_OK) return rc;
   }
   void* args[] = {(void*)&tm[0], (void*)&tm[1], (void*)&p};
-  return gru_launch((const void*)gru_fwd_kernel, ndir * nC, gru_cluster_size(nC), smem, args,
-                    stream);
+  rc = gru_launch((const void*)gru_fwd_kernel, ndir * nC, gru_cluster_size(nC), smem, args,
+                  stream);
+  return rc == SB_OK ? gru_fwd_launched(GRU_FWD_PLAIN) : rc;
 }
 
 extern "C" int sb_gru_bwd_workspace_size(int Bp, int H, int ndir, size_t* bytes) {

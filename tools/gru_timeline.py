@@ -1,4 +1,8 @@
-"""Developer tool: per-step timeline (ns) of CTA 0 of the GRU forward kernel at north-star width."""
+"""Developer tool: per-step timeline (ns) of CTA 0 of the GRU recurrence kernels at north-star width.
+    python tools/gru_timeline.py [cluster size] [fwd|bwd] [sb_debug_gru_flags]
+Forward flags: 0 = default selection (gru_fwd_ks_kernel<2> over 2-CTA clusters for both directions
+of H = 1024 at <= 64 rows on a 132-SM H100), 32 = the plain gru_fwd_kernel, 1024 = the 2-CTA
+K-split forward forced."""
 import sys
 import numpy as np, torch
 sys.path.insert(0, ".")
@@ -8,7 +12,7 @@ if len(sys.argv) > 1:
     lib.sb_debug_gru_cluster(int(sys.argv[1]))
     print("cluster size preference:", sys.argv[1])
 if len(sys.argv) > 3:
-    lib.sb_debug_gru_flags(int(sys.argv[3]))      # 32: version-1 forward kernel
+    lib.sb_debug_gru_flags(int(sys.argv[3]))      # see the docstring
     print("flags:", sys.argv[3])
 torch.manual_seed(0)
 import os
@@ -39,8 +43,8 @@ print("mode:", MODE)
 raw = dbg.cpu().numpy()
 d = raw[:1024].reshape(64, 16)
 # stamp index -> phase; P: producer warp, M: MMA warpgroup, E: epilogue thread 0.  The K-split
-# kernels stamp 4 after issuing the reduce-scatter (the plain kernels: accbuf read) and 13 once
-# the backward's peer slices have arrived; in its L2 reduce-scatter mode (flags 256, or the
+# kernels (forward: ks4 and ks2 alike) stamp 4 after issuing the reduce-scatter (the plain
+# kernels: accbuf read), and the backward 13 once its peer slices have arrived; in its L2 reduce-scatter mode (flags 256, or the
 # default at H = 1024 on a 132-SM card) 11 when the CTA's own slices are written to L2 and
 # published, 12 when the group's counter shows all four published.
 names = ["P:grid_wait done", "P:tma issued", "M:product staged", "E:accfull",
@@ -56,6 +60,8 @@ for step in (11, 40):
             continue
         print("   %-22s %7d" % (names[i], d[step][i] - base))
 print("cluster size used:", lib.sb_debug_gru_cluster(0))
+if MODE == "fwd":
+    print("forward kernel:", lib.sb_debug_gru_fwd_kernel().decode())
 print("mean step period (ns):", (d[60][9] - d[10][9]) / 50.0)
 
 if MODE == "fwd":

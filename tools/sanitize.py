@@ -58,4 +58,13 @@ l8 = mr.loss((inputs, labels)); l8.backward()
 torch.cuda.synchronize()
 _lib.load().sb_debug_gru_flags(0)
 print("L2 reduce-scatter GRU ok", l8.item())
+# the K-split forward recurrence kernel over 2-CTA clusters, forced
+_lib.load().sb_debug_gru_flags(1024)
+mk = CTC(80, 28, cfg).cuda()
+l9 = mk.loss((inputs, labels)); l9.backward()
+torch.cuda.synchronize()
+fwd_kernel = _lib.load().sb_debug_gru_fwd_kernel().decode()
+_lib.load().sb_debug_gru_flags(0)
+assert fwd_kernel == "ks2", fwd_kernel
+print("2-CTA K-split GRU forward ok", l9.item())
 torch.cuda.synchronize()
