@@ -128,6 +128,56 @@ SB_DEVINL void tma_load_3d(void* smem_dst, const void* tmap, uint64_t* bar, int3
 }
 
 // ----------------------------------------------------------------------------------------------
+// thread-block clusters
+// ----------------------------------------------------------------------------------------------
+SB_DEVINL uint32_t cluster_rank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+SB_DEVINL uint32_t cluster_size() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r));
+  return r;
+}
+SB_DEVINL void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
+  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// TMA box load multicast to every CTA in `mask` (same smem offset + same mbarrier offset in each)
+SB_DEVINL void tma_load_2d_mc(void* smem_dst, const void* tmap, uint64_t* bar, int32_t c0,
+                              int32_t c1, uint16_t mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes"
+      ".multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)),
+        "r"(c0), "r"(c1), "h"(mask)
+      : "memory");
+}
+// arrive on the mbarrier at this offset in each of the first `cs` CTAs of the cluster
+SB_DEVINL void mbar_arrive_all_ctas(uint64_t* bar, uint32_t cs) {
+  for (uint32_t r = 0; r < cs; ++r) {
+    uint32_t ra;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(smem_u32(bar)), "r"(r));
+    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(ra) : "memory");
+  }
+}
+// Arrive on the mbarrier at this offset in CTA `cta` of the cluster, without a memory fence: for
+// releasing a shared-memory slot whose readers are wgmma (already retired by wgmma.wait_group) to a
+// producer whose writes are TMA.  (mbar_arrive_all_ctas's release.cluster costs a MEMBAR.GPU.)
+SB_DEVINL void mbar_arrive_remote(uint64_t* bar, uint32_t cta) {
+  uint32_t ra;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(smem_u32(bar)), "r"(cta));
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(ra) : "memory");
+}
+
+// Register reallocation between the warpgroups of a CTA (every thread of the warpgroup executes it)
+template <int R>
+SB_DEVINL void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+SB_DEVINL void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+
+// ----------------------------------------------------------------------------------------------
 // wgmma (sm_90a warpgroup MMA): D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, both operands in shared
 // memory, fp32 accumulators in the registers of the 128 threads of one warpgroup.
 //   shared-memory matrix descriptor, SWIZZLE_128B:
@@ -223,17 +273,27 @@ SB_DEVINL void wgmma_m64n192k16(float (&d)[96], uint64_t da, uint64_t db, uint32
       : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
 }
 
+template <int TA, int TB>
+SB_DEVINL void wgmma_m64n256k16(float (&d)[128], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, %131, %132;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
+}
+
 template <int N, int TA = 0, int TB = 0>
 SB_DEVINL void wgmma_bf16(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d) {
-  static_assert(N == 16 || N == 32 || N == 48 || N == 64 || N == 96 || N == 128 || N == 192,
-                "wgmma N");
+  static_assert(N == 16 || N == 32 || N == 48 || N == 64 || N == 96 || N == 128 || N == 192 ||
+                N == 256, "wgmma N");
   if constexpr (N == 16) wgmma_m64n16k16<TA, TB>(d, da, db, scale_d);
   else if constexpr (N == 32) wgmma_m64n32k16<TA, TB>(d, da, db, scale_d);
   else if constexpr (N == 48) wgmma_m64n48k16<TA, TB>(d, da, db, scale_d);
   else if constexpr (N == 64) wgmma_m64n64k16<TA, TB>(d, da, db, scale_d);
   else if constexpr (N == 96) wgmma_m64n96k16<TA, TB>(d, da, db, scale_d);
   else if constexpr (N == 128) wgmma_m64n128k16<TA, TB>(d, da, db, scale_d);
-  else wgmma_m64n192k16<TA, TB>(d, da, db, scale_d);
+  else if constexpr (N == 192) wgmma_m64n192k16<TA, TB>(d, da, db, scale_d);
+  else wgmma_m64n256k16<TA, TB>(d, da, db, scale_d);
 }
 
 // Accumulator fragment of m64nN (thread t of the warpgroup, register i): row and column in the

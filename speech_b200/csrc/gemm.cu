@@ -11,6 +11,8 @@
 //     registers; each releases a ring slot as soon as the wgmma group that read it has retired
 //     (one group kept in flight), then stores its rows straight from the registers
 //   * smem ring of kStages {A 128x64, B BNx64} tiles, full/empty mbarriers
+// GEMMs with N > 128 run gemm_bf16_tn_c2_kernel instead: 128 x 256 tiles over 2-CTA clusters that
+// share the B tile by TMA multicast (see there).
 //
 // Roofline: tensor (bf16 dense).  Algorithmic FLOPs = 2*M*N*K per launch.
 #include "common.cuh"
@@ -35,6 +37,7 @@ struct GemmParams {
   int flags;            // SB_GEMM_ACCUMULATE | SB_GEMM_ROW_REMAP
   int remap_B, remap_T, valid_B;
   int m_tiles, n_tiles;
+  int m_pairs;          // gemm_bf16_tn_c2_kernel: ceil(m_tiles / 2)
 };
 
 // MN-major operand tiles: the contraction runs over the ROWS of the global matrix ([K][MN], MN
@@ -214,6 +217,193 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,
 }
 
 // ----------------------------------------------------------------------------------------------
+// gemm_bf16_tn_c2_kernel: 128 x 256 tiles over 2-CTA clusters, for N > 128.
+//
+//   * the two CTAs of a cluster take M tiles 2i and 2i + 1 of the same N tile; each loads its own
+//     A tile (128 x 64) and HALF of the shared B tile (128 of the 256 rows) with a TMA multicast
+//     into both CTAs: 32 KB of L2 -> SM traffic per CTA per k-block for 4.2 MFLOP (7.8 B/kFLOP,
+//     half the 15.6 of the 128 x 128 kernel above)
+//   * register reallocation: the producer warpgroup drops to 40 registers, the two consumer
+//     warpgroups rise to 232, enough for one 64 x 256 fp32 accumulator (128 registers) each
+//   * a ring slot holds data written by both CTAs' TMA, so it is refilled only after the
+//     consumers of BOTH CTAs have released it: each consumer warpgroup arrives on the empty
+//     barrier of both CTAs (count 4)
+//   * an unpaired last M tile runs on rank 0; rank 1 loads a box past M (zero fill) so that the
+//     shared B stays in lockstep, and stores nothing
+// Every output element has the same sum as in gemm_bf16_tn_kernel (one fp32 accumulator,
+// k-blocks ascending, the same k16 wgmma steps), so non-accumulating results are bit-identical.
+// ----------------------------------------------------------------------------------------------
+static constexpr int C2_BN = 256;
+static constexpr int C2_STAGES = 4;
+static constexpr int C2_A_BYTES = BM * BK * 2;                  // 16 KB
+static constexpr int C2_STAGE_BYTES = (BM + C2_BN) * BK * 2;    // 48 KB
+static constexpr int C2_SMEM_BYTES = C2_STAGES * C2_STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+
+template <int TA, int TB>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_bf16_tn_c2_kernel(const __grid_constant__ CUtensorMap tmap_a,
+                       const __grid_constant__ CUtensorMap tmap_b, const GemmParams p,
+                       const MnDesc mn) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* tiles = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
+                                              ~static_cast<uintptr_t>(1023));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(tiles + C2_STAGES * C2_STAGE_BYTES);
+  uint64_t* full_bar = bars;                  // [C2_STAGES]
+  uint64_t* empty_bar = bars + C2_STAGES;     // [C2_STAGES]  one arrive per consumer warpgroup
+                                              //              of each CTA of the cluster
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int rank = (int)cluster_rank();
+
+  if (warp == 0 && lane == 0) {
+    tma_prefetch_desc(&tmap_a);
+    tma_prefetch_desc(&tmap_b);
+    for (int s = 0; s < C2_STAGES; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 4);
+    }
+    mbar_fence_init();
+  }
+  cluster_sync_all();   // the peer's barriers are initialised before anyone signals them
+
+  const int pair_tiles = p.m_pairs * p.n_tiles;
+  const int total_work = pair_tiles * p.split_k;
+  const int kb_per_split = (p.k_blocks_total + p.split_k - 1) / p.split_k;
+  const int cluster_id = blockIdx.x >> 1;
+  const int n_clusters = gridDim.x >> 1;
+
+  if (warp < 4) {
+    // ===================== TMA producer =====================
+    setmaxnreg_dec<40>();
+    if (warp == 0 && lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int w = cluster_id; w < total_work; w += n_clusters) {
+        const int split = w / pair_tiles;
+        const int t = w - split * pair_tiles;
+        const int m_pair = t / p.n_tiles;
+        const int n_blk = t - m_pair * p.n_tiles;
+        const int m_blk = 2 * m_pair + rank;
+        const int kb0 = split * kb_per_split;
+        int kb1 = kb0 + kb_per_split;
+        if (kb1 > p.k_blocks_total) kb1 = p.k_blocks_total;
+        for (int kb = kb0; kb < kb1; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          uint8_t* sa = tiles + stage * C2_STAGE_BYTES;
+          uint8_t* sb_ = sa + C2_A_BYTES;
+          mbar_expect_tx(&full_bar[stage], C2_STAGE_BYTES);   // own A + both halves of B
+          if (TA) {
+#pragma unroll
+            for (int b = 0; b < BM / 64; ++b)
+              tma_load_2d(sa + b * MN_BOX_BYTES, &tmap_a, &full_bar[stage], m_blk * BM + b * 64,
+                          kb * BK);
+          } else {
+            tma_load_2d(sa, &tmap_a, &full_bar[stage], kb * BK, m_blk * BM);
+          }
+          if (TB) {
+#pragma unroll
+            for (int b = 2 * rank; b < 2 * rank + 2; ++b)
+              tma_load_2d_mc(sb_ + b * MN_BOX_BYTES, &tmap_b, &full_bar[stage],
+                             n_blk * C2_BN + b * 64, kb * BK, 0x3);
+          } else {
+            tma_load_2d_mc(sb_ + rank * (C2_BN / 2) * BK * 2, &tmap_b, &full_bar[stage], kb * BK,
+                           n_blk * C2_BN + rank * (C2_BN / 2), 0x3);
+          }
+          if (++stage == C2_STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+    __syncwarp();
+  } else {
+    // ===================== consumers: warpgroup 1 -> rows 0..63, 2 -> rows 64..127 ==========
+    setmaxnreg_inc<232>();
+    const int half = (warp >> 2) - 1;
+    const int t = threadIdx.x & 127;
+    const bool leader = t == 0;
+    const uint64_t a_step = TA ? (uint64_t)(mn.kadv >> 4) : 2u;
+    const uint64_t b_step = TB ? (uint64_t)(mn.kadv >> 4) : 2u;
+    const bool vec_ok = ((p.ldc & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 7) == 0);
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int w = cluster_id; w < total_work; w += n_clusters) {
+      const int split = w / pair_tiles;
+      const int tt = w - split * pair_tiles;
+      const int m_pair = tt / p.n_tiles;
+      const int n_blk = tt - m_pair * p.n_tiles;
+      const int m_blk = 2 * m_pair + rank;
+      const int kb0 = split * kb_per_split;
+      int kb1 = kb0 + kb_per_split;
+      if (kb1 > p.k_blocks_total) kb1 = p.k_blocks_total;
+      float acc[C2_BN / 2];
+#pragma unroll
+      for (int i = 0; i < C2_BN / 2; ++i) acc[i] = 0.f;
+      int prev = -1;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_u32(tiles + stage * C2_STAGE_BYTES);
+        const uint32_t sb_ = sa + C2_A_BYTES;
+        const uint64_t da = TA ? gmma_desc_sw128_mnmajor(sa + half * MN_BOX_BYTES, mn.lbo, mn.sbo)
+                               : gmma_desc_sw128_kmajor(sa + half * 64 * 128);
+        const uint64_t db = TB ? gmma_desc_sw128_mnmajor(sb_, mn.lbo, mn.sbo)
+                               : gmma_desc_sw128_kmajor(sb_);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k)
+          wgmma_bf16<C2_BN, TA, TB>(acc, da + a_step * k, db + b_step * k,
+                                    (kb > kb0 || k > 0) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();                 // the group of the previous k-block has retired
+        if (prev >= 0 && leader) { mbar_arrive_remote(&empty_bar[prev], 0); mbar_arrive_remote(&empty_bar[prev], 1); }
+        prev = stage;
+        if (++stage == C2_STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if (prev >= 0 && leader) { mbar_arrive_remote(&empty_bar[prev], 0); mbar_arrive_remote(&empty_bar[prev], 1); }
+      if (kb1 <= kb0 || m_blk >= p.m_tiles) continue;   // empty K range / unpaired M tile
+
+      // ---- epilogue straight from the registers: rows r, r + 8; column pairs every 8 ----
+      const bool add_bias = (p.bias != nullptr) && (split == 0);
+#pragma unroll
+      for (int rh = 0; rh < 2; ++rh) {
+        const int m = m_blk * BM + half * 64 + ((t >> 5) << 4) + ((t & 31) >> 2) + rh * 8;
+        bool row_ok = m < p.M;
+        long long out_row = m;
+        if (p.flags & SB_GEMM_ROW_REMAP) {
+          const int b = m % p.remap_B;
+          const int tm = m / p.remap_B;
+          row_ok = row_ok && (b < p.valid_B);
+          out_row = (long long)b * p.remap_T + tm;
+        }
+        if (!row_ok) continue;
+        float* crow = p.C + out_row * p.ldc;
+#pragma unroll
+        for (int j = 0; j < C2_BN / 8; ++j) {
+          const int n = n_blk * C2_BN + j * 8 + ((t & 3) << 1);
+          float x0 = acc[4 * j + 2 * rh], x1 = acc[4 * j + 2 * rh + 1];
+          if (n >= p.N) continue;
+          const bool two = n + 1 < p.N;
+          if (add_bias) {
+            x0 += __ldg(p.bias + n);
+            if (two) x1 += __ldg(p.bias + n + 1);
+          }
+          if (p.flags & SB_GEMM_ACCUMULATE) {
+            atomicAdd(crow + n, x0);
+            if (two) atomicAdd(crow + n + 1, x1);
+          } else if (two && vec_ok) {
+            *reinterpret_cast<float2*>(crow + n) = make_float2(x0, x1);
+          } else {
+            crow[n] = x0;
+            if (two) crow[n + 1] = x1;
+          }
+        }
+      }
+    }
+  }
+  cluster_sync_all();   // no CTA leaves while its peer may still multicast into it or signal it
+}
+
+// ----------------------------------------------------------------------------------------------
 // host side
 // ----------------------------------------------------------------------------------------------
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
@@ -299,6 +489,69 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, GemmParams 
   return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
 }
 
+// Clusters of gemm_bf16_tn_c2_kernel resident at once: the size of its persistent grid.  Every
+// instantiation has the same block size, launch bounds and shared memory, so one query serves all.
+static int c2_max_clusters() {
+  static int n = -1;
+  if (n >= 0) return n;
+  auto kernel = gemm_bf16_tn_c2_kernel<0, 0>;
+  n = 0;
+  if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, C2_SMEM_BYTES) !=
+      cudaSuccess) {
+    cudaGetLastError();
+    return n;
+  }
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(2 * (device_sm_count() / 2));
+  cfg.blockDim = dim3(GEMM_THREADS);
+  cfg.dynamicSmemBytes = C2_SMEM_BYTES;
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeClusterDimension;
+  attr.val.clusterDim.x = 2;
+  attr.val.clusterDim.y = 1;
+  attr.val.clusterDim.z = 1;
+  cfg.attrs = &attr;
+  cfg.numAttrs = 1;
+  if (cudaOccupancyMaxActiveClusters(&n, kernel, &cfg) != cudaSuccess) {
+    cudaGetLastError();
+    n = 0;
+  }
+  return n;
+}
+
+template <int TA, int TB>
+static int launch_gemm_c2(const CUtensorMap& ta, const CUtensorMap& tb, GemmParams p,
+                          cudaStream_t stream) {
+  auto kernel = gemm_bf16_tn_c2_kernel<TA, TB>;
+  static bool attr_set = false;
+  if (!attr_set) {
+    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, C2_SMEM_BYTES) !=
+        cudaSuccess)
+      return SB_ERR_CUDA;
+    attr_set = true;
+  }
+  p.n_tiles = (p.N + C2_BN - 1) / C2_BN;
+  p.m_pairs = (p.m_tiles + 1) / 2;
+  const int total = p.m_pairs * p.n_tiles * p.split_k;
+  int clusters = c2_max_clusters();
+  if (clusters <= 0) return SB_ERR_UNSUPPORTED;
+  if (clusters > total) clusters = total;
+  const MnDesc mn = {(uint32_t)g_mn_lbo, (uint32_t)g_mn_sbo, (uint32_t)g_mn_kadv};
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(2 * clusters);
+  cfg.blockDim = dim3(GEMM_THREADS);
+  cfg.dynamicSmemBytes = C2_SMEM_BYTES;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeClusterDimension;
+  attr.val.clusterDim.x = 2;
+  attr.val.clusterDim.y = 1;
+  attr.val.clusterDim.z = 1;
+  cfg.attrs = &attr;
+  cfg.numAttrs = 1;
+  return cudaLaunchKernelEx(&cfg, kernel, ta, tb, p, mn) == cudaSuccess ? SB_OK : SB_ERR_CUDA;
+}
+
 template <int BN>
 static int launch_gemm_bn(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p,
                           bool a_mn, bool b_mn, cudaStream_t stream) {
@@ -306,9 +559,22 @@ static int launch_gemm_bn(const CUtensorMap& ta, const CUtensorMap& tb, const Ge
   return b_mn ? launch_gemm<BN, 0, 1>(ta, tb, p, stream) : launch_gemm<BN, 0, 0>(ta, tb, p, stream);
 }
 
+// developer knob (sb_debug_gemm_flags): 1 = the 128 x BN kernel for every shape
+static int g_gemm_flags = 0;
+// which kernel the last sb_gemm_bf16_tn launched (sb_debug_gemm_kernel)
+static const char* g_gemm_last = "none";
+
 }  // namespace sb
 
 using namespace sb;
+
+extern "C" int sb_debug_gemm_flags(int flags) {
+  sb::g_gemm_flags = flags;
+  return SB_OK;
+}
+// "c2_128x256" (gemm_bf16_tn_c2_kernel), "128x128" / "128x64" / "128x32" (gemm_bf16_tn_kernel at
+// that tile), "none" before the first launch
+extern "C" const char* sb_debug_gemm_kernel(void) { return sb::g_gemm_last; }
 
 // developer hook: override the MN-major descriptor fields (bytes); 0 keeps a field
 extern "C" int sb_debug_umma_mn(int lbo, int sbo, int kadv) {
@@ -337,26 +603,36 @@ extern "C" int sb_gemm_bf16_tn(const void* A, long long lda, const void* B, long
   p.n_tiles = 0;
   const bool a_mn = (flags & SB_GEMM_A_MN) != 0;
   const bool b_mn = (flags & SB_GEMM_B_MN) != 0;
-  // tile-N choice: 128 x 128 tiles keep the 64 accumulator registers per consumer thread below the
-  // register cap of a 3-warpgroup CTA; narrow GEMMs take narrower tiles (an MN-major B tile is
-  // made of 64-wide boxes)
+  // tile-N choice: N > 128 takes the 128 x 256 tiles of the 2-CTA cluster kernel; narrower GEMMs
+  // take 128 x BN tiles of gemm_bf16_tn_kernel (an MN-major B tile is made of 64-wide boxes)
   int bn;
   if (N <= 32 && !b_mn) bn = 32;
   else if (N <= 64) bn = 64;
-  else bn = 128;
-  if (flags & SB_GEMM_ACCUMULATE)
-    p.split_k = pick_wave_filling_split((long long)p.m_tiles * ((N + bn - 1) / bn),
-                                        device_sm_count(), p.k_blocks_total);
+  else if (N <= 128 || (g_gemm_flags & 1)) bn = 128;
+  else bn = C2_BN;
+  if (flags & SB_GEMM_ACCUMULATE) {
+    // the c2 kernel deals tile pairs to clusters
+    const bool c2 = bn == C2_BN;
+    const long long units = c2 ? (long long)((p.m_tiles + 1) / 2) * ((N + bn - 1) / bn)
+                               : (long long)p.m_tiles * ((N + bn - 1) / bn);
+    p.split_k = pick_wave_filling_split(units, c2 ? std::max(c2_max_clusters(), 1) : device_sm_count(),
+                                        p.k_blocks_total);
+  }
   // tensor maps: K-major operands are [rows][K] with box {64 K, rows}; MN-major operands are
-  // [K][rows] with box {64 rows, 64 K}
+  // [K][rows] with box {64 rows, 64 K}.  The c2 kernel loads half of its 256-row B tile per CTA.
   CUtensorMap ta, tb;
   int rc = a_mn ? make_tmap_bf16_2d(&ta, A, K, M, lda, 64) : make_tmap_bf16_2d(&ta, A, M, K, lda, BM);
   if (rc != SB_OK) return rc;
-  rc = b_mn ? make_tmap_bf16_2d(&tb, B, K, N, ldb, 64) : make_tmap_bf16_2d(&tb, B, N, K, ldb, bn);
+  rc = b_mn ? make_tmap_bf16_2d(&tb, B, K, N, ldb, 64)
+            : make_tmap_bf16_2d(&tb, B, N, K, ldb, bn == C2_BN ? C2_BN / 2 : bn);
   if (rc != SB_OK) return rc;
   switch (bn) {
-    case 32: return launch_gemm_bn<32>(ta, tb, p, a_mn, b_mn, stream);
-    case 64: return launch_gemm_bn<64>(ta, tb, p, a_mn, b_mn, stream);
-    default: return launch_gemm_bn<128>(ta, tb, p, a_mn, b_mn, stream);
+    case 32: g_gemm_last = "128x32"; return launch_gemm_bn<32>(ta, tb, p, a_mn, b_mn, stream);
+    case 64: g_gemm_last = "128x64"; return launch_gemm_bn<64>(ta, tb, p, a_mn, b_mn, stream);
+    case 128: g_gemm_last = "128x128"; return launch_gemm_bn<128>(ta, tb, p, a_mn, b_mn, stream);
+    default:
+      g_gemm_last = "c2_128x256";
+      if (a_mn) return b_mn ? launch_gemm_c2<1, 1>(ta, tb, p, stream) : launch_gemm_c2<1, 0>(ta, tb, p, stream);
+      return b_mn ? launch_gemm_c2<0, 1>(ta, tb, p, stream) : launch_gemm_c2<0, 0>(ta, tb, p, stream);
   }
 }

@@ -114,40 +114,6 @@ SB_DEVINL void grid_wait(const unsigned int* ctr, unsigned int target, int mode 
 }
 SB_DEVINL void epi_barrier() { asm volatile("bar.sync 1, %0;" ::"n"(GRU_EPI) : "memory"); }
 
-// ---- cluster helpers ---------------------------------------------------------------------------
-SB_DEVINL uint32_t cluster_rank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-SB_DEVINL uint32_t cluster_size() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r));
-  return r;
-}
-SB_DEVINL void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// TMA box load multicast to every CTA in `mask` (same smem offset + same mbarrier offset in each)
-SB_DEVINL void tma_load_2d_mc(void* smem_dst, const void* tmap, uint64_t* bar, int32_t c0,
-                              int32_t c1, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes"
-      ".multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)),
-        "r"(c0), "r"(c1), "h"(mask)
-      : "memory");
-}
-// arrive on the mbarrier at this offset in each of the first `cs` CTAs of the cluster
-SB_DEVINL void mbar_arrive_all_ctas(uint64_t* bar, uint32_t cs) {
-  for (uint32_t r = 0; r < cs; ++r) {
-    uint32_t ra;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(smem_u32(bar)), "r"(r));
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(ra) : "memory");
-  }
-}
-
 struct GruSmem {
   uint8_t* ring;    // ring slots (stride = Bp*128 bytes), placed BEFORE the weights so that the
                     // 128-row MMA read of the last slot overruns into (finite) weight data

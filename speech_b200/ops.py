@@ -70,7 +70,9 @@ def _apply_env_knobs():
     SB_GRU_KSPLIT=0 disables the K-split backward kernel, SB_GRU_CLUSTER=<1|2|4|8> sets the
     preferred cluster size of the other GRU kernels, SB_GRU_FLAGS=<int> sets sb_debug_gru_flags
     (e.g. 512: no L2 reduce-scatter mode, the backward's two clustered one-direction launches at
-    H = 1024; 256: that mode wherever the K-split backward kernel applies)."""
+    H = 1024; 256: that mode wherever the K-split backward kernel applies), SB_GEMM_FLAGS=<int>
+    sets sb_debug_gemm_flags (1: the 128 x 128 one-CTA GEMM kernel instead of the 128 x 256 one
+    over 2-CTA clusters)."""
     import os
     lib = _lib.load()
     if os.environ.get("SB_GRU_KSPLIT") is not None:
@@ -79,6 +81,8 @@ def _apply_env_knobs():
         lib.sb_debug_gru_cluster(int(os.environ["SB_GRU_CLUSTER"]))
     if os.environ.get("SB_GRU_FLAGS") is not None:
         lib.sb_debug_gru_flags(int(os.environ["SB_GRU_FLAGS"]))
+    if os.environ.get("SB_GEMM_FLAGS") is not None:
+        lib.sb_debug_gemm_flags(int(os.environ["SB_GEMM_FLAGS"]))
 
 
 _knobs_applied = False
@@ -636,14 +640,28 @@ class GRUStackFunction(torch.autograd.Function):
             dgi_x = dgi if al is None else _align_reverse(dgi, al, T, Bp, K3, right=False)
             # ---- weight gradients: contract the token-major operands over their rows ----
             Ms = M - Bp                      # tokens that have a predecessor in the recurrence
+            # When the .grad of both directions' W_ih lie back to back (optim.FlatSGD's flat
+            # gradient buffer), dW_ih of both is one [2*3H][In_l] GEMM into that block: one
+            # wave-filling launch instead of two.
+            both = None
+            if ndir == 2 and not padded and al is None:
+                s0, s1 = _grad_sink(wl[0]), _grad_sink(wl[4])
+                if (s0 is not None and s1 is not None and s0.shape == (K3, In_l)
+                        and s1.shape == s0.shape
+                        and s1.untyped_storage().data_ptr() == s0.untyped_storage().data_ptr()
+                        and s1.data_ptr() == s0.data_ptr() + s0.numel() * s0.element_size()):
+                    both = s0.as_strided((2 * K3, In_l), (In_l, 1))
+                    gemm_bf16_tn(dgi_x, X[:, :In_l], out=both, accumulate=True,
+                                 a_mn=True, b_mn=True)
             for d in range(ndir):
                 # dW_ih[d] (3H x In_l) = dgi[:, d]^T X.  A padded layer computes the padded
                 # gradients into temporaries and hands on (or adds into the sink) the real block.
                 sink = None if padded else _grad_sink(wl[d * 4])
                 dwih = sink if sink is not None else \
                     torch.zeros(K3, In_l, dtype=torch.float32, device=dev)
-                gemm_bf16_tn(dgi_x[:, d * K3:(d + 1) * K3], X[:, :In_l], out=dwih,
-                             accumulate=True, a_mn=True, b_mn=True)
+                if both is None:
+                    gemm_bf16_tn(dgi_x[:, d * K3:(d + 1) * K3], X[:, :In_l], out=dwih,
+                                 accumulate=True, a_mn=True, b_mn=True)
                 # dW_hh[d] = [dgi_r | dgi_z | dghn]^T h_prev: h_prev of token (t, b) is token
                 # (t-1, b) in the forward direction and (t+1, b) in the reverse one, so the
                 # shift is a row offset of Bp on one of the two operands

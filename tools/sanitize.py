@@ -67,4 +67,16 @@ fwd_kernel = _lib.load().sb_debug_gru_fwd_kernel().decode()
 _lib.load().sb_debug_gru_flags(0)
 assert fwd_kernel == "ks2", fwd_kernel
 print("2-CTA K-split GRU forward ok", l9.item())
+# the 128 x 256 GEMM over 2-CTA clusters: odd M-tile count (unpaired last tile), ragged N and K,
+# MN-major operands, accumulating with the library's K split
+from speech_b200 import ops
+A = torch.randn(304, 200, device="cuda").bfloat16()
+Bm = torch.randn(200, 304, device="cuda").bfloat16()
+ops.gemm_bf16_tn(A, Bm.t().contiguous(), bias=torch.randn(304, device="cuda"))
+acc = torch.zeros(304, 304, device="cuda")
+ops.gemm_bf16_tn(A.t().contiguous(), Bm, out=acc, accumulate=True, a_mn=True, b_mn=True)
+torch.cuda.synchronize()
+gemm_kernel = _lib.load().sb_debug_gemm_kernel().decode()
+assert gemm_kernel == "c2_128x256", gemm_kernel
+print("2-CTA GEMM ok")
 torch.cuda.synchronize()
