@@ -426,12 +426,18 @@ int sb_log_specgram(const short* pcm, const long long* offsets, const int* n_sam
  * globaltimer timeline of CTA 0 for the next sb_gru_fwd launches; NULL disables. */
 int sb_debug_gru_timeline(void* dev_buffer);
 int sb_debug_umma_mn(int lbo_bytes, int sbo_bytes, int kadv_bytes);
-/* Developer hook, GEMM kernel selection (0 = default): 1 = run every sb_gemm_bf16_tn with N > 64
- * on the 128 x 128 tiles of the one-CTA kernel instead of the 128 x 256 tiles over 2-CTA clusters. */
+/* Developer hook, GEMM kernel selection (0 = default, bits combine): 1 = run every sb_gemm_bf16_tn
+ * with N > 64 on the 128 x 128 tiles of the one-CTA kernel instead of the 128 x 256 tiles over
+ * 2-CTA clusters; 2 = the 2-CTA kernel stores its output straight from the registers instead of
+ * through shared memory and TMA; 4 = the 2-CTA kernel writes no output at all (timing only). */
 int sb_debug_gemm_flags(int flags);
 /* Developer hook: which kernel the last sb_gemm_bf16_tn launched: "c2_128x256" (2-CTA clusters),
  * "128x128" / "128x64" / "128x32" (one CTA per tile at that tile shape), "none". */
 const char* sb_debug_gemm_kernel(void);
+/* Developer hook: how the last sb_gemm_bf16_tn wrote its output: "tma" / "tma_reduce" (2-CTA
+ * kernel: tiles staged in shared memory, TMA bulk tensor stores / reduce-adds), "regs" (straight
+ * from the registers), "skipped" (flag 4), "none" before the first launch. */
+const char* sb_debug_gemm_epilogue(void);
 /* Developer hook, GRU kernel selection / timing knobs (0 = defaults): 8 / 16 = never / always use
  * the transposed-accumulator K-split kernels, 32 = no K-split forward kernel, 64 / 128 = polling
  * mode of the grid barrier, 256 / 512 = always (wherever the K-split backward kernel applies) /

@@ -93,6 +93,7 @@ SIGNATURES = {
     "sb_debug_umma_mn": (_c_int, [_c_int, _c_int, _c_int]),
     "sb_debug_gemm_flags": (_c_int, [_c_int]),
     "sb_debug_gemm_kernel": (ctypes.c_char_p, []),
+    "sb_debug_gemm_epilogue": (ctypes.c_char_p, []),
     "sb_edit_distance": (_c_ll, [_vp, _c_ll, _vp, _c_ll]),
     "sb_log_specgram": (_c_int, [_vp, _vp, _vp, _c_int, _c_int, _c_int, ctypes.c_double, _fl, _vp,
                                  _vp, _vp, _c_int, _vp]),

@@ -128,6 +128,39 @@ SB_DEVINL void tma_load_3d(void* smem_dst, const void* tmap, uint64_t* bar, int3
 }
 
 // ----------------------------------------------------------------------------------------------
+// TMA: tiled tensor stores and reduce-adds (shared -> global), tracked by bulk async-groups of the
+// issuing thread (smem_src: shared-space address).  The source box must be written and made
+// visible to the async proxy (fence_proxy_async_smem + a barrier) before the issue.
+// ----------------------------------------------------------------------------------------------
+SB_DEVINL void tma_store_2d(const void* tmap, uint32_t smem_src, int32_t c0, int32_t c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_src), "r"(c0), "r"(c1)
+               : "memory");
+}
+SB_DEVINL void tma_reduce_add_2d(const void* tmap, uint32_t smem_src, int32_t c0, int32_t c1) {
+  asm volatile(
+      "cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];"
+      ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_src), "r"(c0), "r"(c1)
+      : "memory");
+}
+SB_DEVINL void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's committed groups may still be reading their shared-memory source
+template <int N>
+SB_DEVINL void bulk_wait_group_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+// at most N of this thread's committed groups may still be incomplete (writes included)
+template <int N>
+SB_DEVINL void bulk_wait_group() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+// barrier `id` (1..15; 0 is __syncthreads) over `n` threads, a multiple of 32
+SB_DEVINL void named_bar_sync(uint32_t id, uint32_t n) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory");
+}
+SB_DEVINL void st_shared_f2(uint32_t addr, float x, float y) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x), "f"(y) : "memory");
+}
+
+// ----------------------------------------------------------------------------------------------
 // thread-block clusters
 // ----------------------------------------------------------------------------------------------
 SB_DEVINL uint32_t cluster_rank() {

@@ -18,6 +18,7 @@
 #include "common.cuh"
 #include <cuda.h>
 #include <stdio.h>
+#include <string.h>
 
 #include "../../include/speech_b200.h"
 
@@ -38,6 +39,15 @@ struct GemmParams {
   int remap_B, remap_T, valid_B;
   int m_tiles, n_tiles;
   int m_pairs;          // gemm_bf16_tn_c2_kernel: ceil(m_tiles / 2)
+  int epi;              // gemm_bf16_tn_c2_kernel: C2Epilogue
+};
+
+// How gemm_bf16_tn_c2_kernel writes its output tiles
+enum C2Epilogue : int {
+  C2_EPI_REGS = 0,        // straight from the registers (st.global / atomicAdd per element pair)
+  C2_EPI_TMA = 1,         // staged through shared memory, TMA bulk tensor stores
+  C2_EPI_TMA_REDUCE = 2,  // staged through shared memory, TMA bulk tensor reduce-add
+  C2_EPI_NONE = 3,        // timing only: no output at all
 };
 
 // MN-major operand tiles: the contraction runs over the ROWS of the global matrix ([K][MN], MN
@@ -230,6 +240,14 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,
 //     barrier of both CTAs (count 4)
 //   * an unpaired last M tile runs on rank 0; rank 1 loads a box past M (zero fill) so that the
 //     shared B stays in lockstep, and stores nothing
+//   * epilogue (C2_EPI_TMA / C2_EPI_TMA_REDUCE): each consumer warpgroup writes its 64 x 256 fp32
+//     rows, bias added, into a shared-memory box of 64 rows x 32 columns (128 B rows, SWIZZLE_128B
+//     so the st.shared are free of bank conflicts), and one thread hands the box to the TMA unit as
+//     a bulk tensor store (reduce-add for accumulating launches).  C2_EPI_BUFS boxes per
+//     warpgroup take turns; a box is rewritten only after the TMA has read it, so the global
+//     writes of a tile drain while the warpgroup fills the next boxes and runs the next tile's
+//     MMAs.  The tensor map of C clips rows >= M and columns >= N.  C2_EPI_REGS stores straight
+//     from the registers (row remap, C not 16-byte aligned, split-K accumulation).
 // Every output element has the same sum as in gemm_bf16_tn_kernel (one fp32 accumulator,
 // k-blocks ascending, the same k16 wgmma steps), so non-accumulating results are bit-identical.
 // ----------------------------------------------------------------------------------------------
@@ -237,17 +255,24 @@ static constexpr int C2_BN = 256;
 static constexpr int C2_STAGES = 4;
 static constexpr int C2_A_BYTES = BM * BK * 2;                  // 16 KB
 static constexpr int C2_STAGE_BYTES = (BM + C2_BN) * BK * 2;    // 48 KB
-static constexpr int C2_SMEM_BYTES = C2_STAGES * C2_STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+static constexpr int C2_EPI_COLS = 32;                          // fp32 columns of a staging box
+static constexpr int C2_EPI_BOX_BYTES = 64 * C2_EPI_COLS * 4;   // 8 KB: 64 rows of 128 B
+static constexpr int C2_EPI_BUFS = 2;                           // staging boxes per warpgroup
+static constexpr int C2_EPI_BYTES = 2 /*warpgroups*/ * C2_EPI_BUFS * C2_EPI_BOX_BYTES;
+static constexpr int C2_SMEM_BYTES = C2_STAGES * C2_STAGE_BYTES + C2_EPI_BYTES + 1024 /*align*/ +
+                                     256 /*barriers*/;
 
 template <int TA, int TB>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_tn_c2_kernel(const __grid_constant__ CUtensorMap tmap_a,
-                       const __grid_constant__ CUtensorMap tmap_b, const GemmParams p,
+                       const __grid_constant__ CUtensorMap tmap_b,
+                       const __grid_constant__ CUtensorMap tmap_c, const GemmParams p,
                        const MnDesc mn) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* tiles = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                               ~static_cast<uintptr_t>(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(tiles + C2_STAGES * C2_STAGE_BYTES);
+  uint8_t* epi_boxes = tiles + C2_STAGES * C2_STAGE_BYTES;     // [warpgroup][C2_EPI_BUFS] boxes
+  uint64_t* bars = reinterpret_cast<uint64_t*>(epi_boxes + C2_EPI_BYTES);
   uint64_t* full_bar = bars;                  // [C2_STAGES]
   uint64_t* empty_bar = bars + C2_STAGES;     // [C2_STAGES]  one arrive per consumer warpgroup
                                               //              of each CTA of the cluster
@@ -258,6 +283,7 @@ gemm_bf16_tn_c2_kernel(const __grid_constant__ CUtensorMap tmap_a,
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
+    if (p.epi == C2_EPI_TMA || p.epi == C2_EPI_TMA_REDUCE) tma_prefetch_desc(&tmap_c);
     for (int s = 0; s < C2_STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 4);
@@ -323,6 +349,8 @@ gemm_bf16_tn_c2_kernel(const __grid_constant__ CUtensorMap tmap_a,
     const uint64_t a_step = TA ? (uint64_t)(mn.kadv >> 4) : 2u;
     const uint64_t b_step = TB ? (uint64_t)(mn.kadv >> 4) : 2u;
     const bool vec_ok = ((p.ldc & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 7) == 0);
+    const uint32_t my_boxes = smem_u32(epi_boxes + half * C2_EPI_BUFS * C2_EPI_BOX_BYTES);
+    uint32_t n_boxes = 0;                // boxes this warpgroup has staged (the next buffer follows)
     int stage = 0;
     uint32_t phase = 0;
     for (int w = cluster_id; w < total_work; w += n_clusters) {
@@ -361,9 +389,57 @@ gemm_bf16_tn_c2_kernel(const __grid_constant__ CUtensorMap tmap_a,
       wgmma_fence_regs(acc);
       if (prev >= 0 && leader) { mbar_arrive_remote(&empty_bar[prev], 0); mbar_arrive_remote(&empty_bar[prev], 1); }
       if (kb1 <= kb0 || m_blk >= p.m_tiles) continue;   // empty K range / unpaired M tile
+      if (p.epi == C2_EPI_NONE) continue;
+      const bool add_bias = (p.bias != nullptr) && (split == 0);
+
+      if (p.epi != C2_EPI_REGS) {
+        // ---- staged epilogue: eight 64 x 32 boxes, TMA bulk store / reduce-add of each ----
+        // Thread t holds rows r, r + 8 (r = 16 * warp + lane / 4) and, in box b, the column pairs
+        // 8 jj + 2 (t & 3) (jj < 4): registers acc[4 (4b + jj) + 2 rh + {0, 1}].  Pair jj of row
+        // r lies in 16-byte chunk 2 jj + (t & 3) / 2 of the 128-byte row, stored at chunk
+        // position chunk ^ (r & 7) (SWIZZLE_128B; r & 7 = lane / 4).
+        const int r0 = ((t >> 5) << 4) + ((t & 31) >> 2);
+        const uint32_t sw = (uint32_t)((t & 31) >> 2);
+        const int row0 = m_blk * BM + half * 64;
+#pragma unroll
+        for (int b = 0; b < C2_BN / C2_EPI_COLS; ++b) {
+          const int col0 = n_blk * C2_BN + b * C2_EPI_COLS;
+          if (col0 >= p.N) break;          // the rest of the tile lies past N (same for all)
+          float bv[8];
+          if (add_bias) {
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+              const int n = col0 + (i >> 1) * 8 + ((t & 3) << 1) + (i & 1);
+              bv[i] = n < p.N ? __ldg(p.bias + n) : 0.f;
+            }
+          }
+          const uint32_t box = my_boxes + (n_boxes % C2_EPI_BUFS) * C2_EPI_BOX_BYTES;
+          if (leader) bulk_wait_group_read<C2_EPI_BUFS - 1>();   // the TMA has read this buffer
+          named_bar_sync(1 + half, 128);
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj) {
+            const uint32_t chunk = (uint32_t)(2 * jj + ((t & 3) >> 1));
+            const uint32_t off = ((chunk ^ sw) << 4) + ((t & 1) << 3);
+#pragma unroll
+            for (int rh = 0; rh < 2; ++rh) {
+              float x0 = acc[4 * (4 * b + jj) + 2 * rh], x1 = acc[4 * (4 * b + jj) + 2 * rh + 1];
+              if (add_bias) { x0 += bv[2 * jj]; x1 += bv[2 * jj + 1]; }
+              st_shared_f2(box + (uint32_t)(r0 + 8 * rh) * 128u + off, x0, x1);
+            }
+          }
+          fence_proxy_async_smem();
+          named_bar_sync(1 + half, 128);
+          if (leader) {
+            if (p.epi == C2_EPI_TMA_REDUCE) tma_reduce_add_2d(&tmap_c, box, col0, row0);
+            else tma_store_2d(&tmap_c, box, col0, row0);
+            bulk_commit_group();
+          }
+          ++n_boxes;
+        }
+        continue;
+      }
 
       // ---- epilogue straight from the registers: rows r, r + 8; column pairs every 8 ----
-      const bool add_bias = (p.bias != nullptr) && (split == 0);
 #pragma unroll
       for (int rh = 0; rh < 2; ++rh) {
         const int m = m_blk * BM + half * 64 + ((t >> 5) << 4) + ((t & 31) >> 2) + rh * 8;
@@ -399,6 +475,7 @@ gemm_bf16_tn_c2_kernel(const __grid_constant__ CUtensorMap tmap_a,
         }
       }
     }
+    if (leader) bulk_wait_group<0>();    // the last boxes are written before the CTA exits
   }
   cluster_sync_all();   // no CTA leaves while its peer may still multicast into it or signal it
 }
@@ -436,6 +513,23 @@ int make_tmap_bf16_2d(CUtensorMap* map, const void* base, long long rows, long l
   CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), gdim, gstride,
                    box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? SB_OK : SB_ERR_CUDA;
+}
+
+// 2-D fp32 tensor map over the row-major [rows, cols] output C (leading dimension ld elements) for
+// the staged epilogue of gemm_bf16_tn_c2_kernel: box = C2_EPI_COLS columns (128 B) x 64 rows,
+// SWIZZLE_128B; stores and reduce-adds outside [rows, cols] are dropped.
+static int make_tmap_f32_c(CUtensorMap* map, const float* base, long long rows, long long cols,
+                           long long ld) {
+  PFN_encodeTiled enc = get_encode_fn();
+  if (!enc) return SB_ERR_CUDA;
+  cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  cuuint64_t gstride[1] = {(cuuint64_t)ld * 4};
+  cuuint32_t box[2] = {(cuuint32_t)C2_EPI_COLS, 64};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), gdim, gstride,
+                   box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                   CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? SB_OK : SB_ERR_CUDA;
 }
 
@@ -520,8 +614,8 @@ static int c2_max_clusters() {
 }
 
 template <int TA, int TB>
-static int launch_gemm_c2(const CUtensorMap& ta, const CUtensorMap& tb, GemmParams p,
-                          cudaStream_t stream) {
+static int launch_gemm_c2(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc,
+                          GemmParams p, cudaStream_t stream) {
   auto kernel = gemm_bf16_tn_c2_kernel<TA, TB>;
   static bool attr_set = false;
   if (!attr_set) {
@@ -549,7 +643,7 @@ static int launch_gemm_c2(const CUtensorMap& ta, const CUtensorMap& tb, GemmPara
   attr.val.clusterDim.z = 1;
   cfg.attrs = &attr;
   cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, kernel, ta, tb, p, mn) == cudaSuccess ? SB_OK : SB_ERR_CUDA;
+  return cudaLaunchKernelEx(&cfg, kernel, ta, tb, tc, p, mn) == cudaSuccess ? SB_OK : SB_ERR_CUDA;
 }
 
 template <int BN>
@@ -559,10 +653,12 @@ static int launch_gemm_bn(const CUtensorMap& ta, const CUtensorMap& tb, const Ge
   return b_mn ? launch_gemm<BN, 0, 1>(ta, tb, p, stream) : launch_gemm<BN, 0, 0>(ta, tb, p, stream);
 }
 
-// developer knob (sb_debug_gemm_flags): 1 = the 128 x BN kernel for every shape
+// developer knob (sb_debug_gemm_flags): 1 = the 128 x BN kernel for every shape, 2 = the c2
+// kernel stores from the registers, 4 = the c2 kernel stores nothing (timing only)
 static int g_gemm_flags = 0;
-// which kernel the last sb_gemm_bf16_tn launched (sb_debug_gemm_kernel)
+// which kernel and which epilogue the last sb_gemm_bf16_tn launched (sb_debug_gemm_kernel / _epilogue)
 static const char* g_gemm_last = "none";
+static const char* g_gemm_epi_last = "none";
 
 }  // namespace sb
 
@@ -575,6 +671,10 @@ extern "C" int sb_debug_gemm_flags(int flags) {
 // "c2_128x256" (gemm_bf16_tn_c2_kernel), "128x128" / "128x64" / "128x32" (gemm_bf16_tn_kernel at
 // that tile), "none" before the first launch
 extern "C" const char* sb_debug_gemm_kernel(void) { return sb::g_gemm_last; }
+// "tma" / "tma_reduce" (c2 kernel, tiles staged through shared memory and written by TMA bulk
+// stores / reduce-adds), "regs" (stored straight from the registers: every other kernel, and the
+// c2 kernel's fall-back), "skipped" (flag 4), "none" before the first launch
+extern "C" const char* sb_debug_gemm_epilogue(void) { return sb::g_gemm_epi_last; }
 
 // developer hook: override the MN-major descriptor fields (bytes); 0 keeps a field
 extern "C" int sb_debug_umma_mn(int lbo, int sbo, int kadv) {
@@ -601,6 +701,8 @@ extern "C" int sb_gemm_bf16_tn(const void* A, long long lda, const void* B, long
   p.remap_B = remap_B; p.remap_T = remap_T; p.valid_B = valid_B;
   p.m_tiles = (M + BM - 1) / BM;
   p.n_tiles = 0;
+  p.m_pairs = 0;
+  p.epi = C2_EPI_REGS;
   const bool a_mn = (flags & SB_GEMM_A_MN) != 0;
   const bool b_mn = (flags & SB_GEMM_B_MN) != 0;
   // tile-N choice: N > 128 takes the 128 x 256 tiles of the 2-CTA cluster kernel; narrower GEMMs
@@ -626,13 +728,31 @@ extern "C" int sb_gemm_bf16_tn(const void* A, long long lda, const void* B, long
   rc = b_mn ? make_tmap_bf16_2d(&tb, B, K, N, ldb, 64)
             : make_tmap_bf16_2d(&tb, B, N, K, ldb, bn == C2_BN ? C2_BN / 2 : bn);
   if (rc != SB_OK) return rc;
+  // output of the c2 kernel: staged through shared memory and written by TMA, except for a row
+  // remap, a C the tensor map cannot describe (base or row pitch not a multiple of 16 bytes) and
+  // split-K accumulation (several CTAs add into the same tile), which store from the registers
+  CUtensorMap tc;
+  memset(&tc, 0, sizeof(tc));
+  if (bn == C2_BN) {
+    const bool tma_ok = !(flags & SB_GEMM_ROW_REMAP) && (reinterpret_cast<uintptr_t>(C) & 15) == 0 &&
+                        ((ldc * 4) & 15) == 0 && !(g_gemm_flags & 2);
+    if (g_gemm_flags & 4) p.epi = C2_EPI_NONE;
+    else if (tma_ok && !(flags & SB_GEMM_ACCUMULATE)) p.epi = C2_EPI_TMA;
+    else if (tma_ok && p.split_k == 1) p.epi = C2_EPI_TMA_REDUCE;
+    if (p.epi == C2_EPI_TMA || p.epi == C2_EPI_TMA_REDUCE) {
+      rc = make_tmap_f32_c(&tc, C, M, N, ldc);
+      if (rc != SB_OK) return rc;
+    }
+  }
   switch (bn) {
-    case 32: g_gemm_last = "128x32"; return launch_gemm_bn<32>(ta, tb, p, a_mn, b_mn, stream);
-    case 64: g_gemm_last = "128x64"; return launch_gemm_bn<64>(ta, tb, p, a_mn, b_mn, stream);
-    case 128: g_gemm_last = "128x128"; return launch_gemm_bn<128>(ta, tb, p, a_mn, b_mn, stream);
+    case 32: g_gemm_last = "128x32"; g_gemm_epi_last = "regs"; return launch_gemm_bn<32>(ta, tb, p, a_mn, b_mn, stream);
+    case 64: g_gemm_last = "128x64"; g_gemm_epi_last = "regs"; return launch_gemm_bn<64>(ta, tb, p, a_mn, b_mn, stream);
+    case 128: g_gemm_last = "128x128"; g_gemm_epi_last = "regs"; return launch_gemm_bn<128>(ta, tb, p, a_mn, b_mn, stream);
     default:
       g_gemm_last = "c2_128x256";
-      if (a_mn) return b_mn ? launch_gemm_c2<1, 1>(ta, tb, p, stream) : launch_gemm_c2<1, 0>(ta, tb, p, stream);
-      return b_mn ? launch_gemm_c2<0, 1>(ta, tb, p, stream) : launch_gemm_c2<0, 0>(ta, tb, p, stream);
+      g_gemm_epi_last = p.epi == C2_EPI_TMA ? "tma" : p.epi == C2_EPI_TMA_REDUCE ? "tma_reduce"
+                      : p.epi == C2_EPI_NONE ? "skipped" : "regs";
+      if (a_mn) return b_mn ? launch_gemm_c2<1, 1>(ta, tb, tc, p, stream) : launch_gemm_c2<1, 0>(ta, tb, tc, p, stream);
+      return b_mn ? launch_gemm_c2<0, 1>(ta, tb, tc, p, stream) : launch_gemm_c2<0, 0>(ta, tb, tc, p, stream);
   }
 }

@@ -71,8 +71,9 @@ def _apply_env_knobs():
     preferred cluster size of the other GRU kernels, SB_GRU_FLAGS=<int> sets sb_debug_gru_flags
     (e.g. 512: no L2 reduce-scatter mode, the backward's two clustered one-direction launches at
     H = 1024; 256: that mode wherever the K-split backward kernel applies), SB_GEMM_FLAGS=<int>
-    sets sb_debug_gemm_flags (1: the 128 x 128 one-CTA GEMM kernel instead of the 128 x 256 one
-    over 2-CTA clusters)."""
+    sets sb_debug_gemm_flags (bits: 1 = the 128 x 128 one-CTA GEMM kernel instead of the 128 x 256
+    one over 2-CTA clusters; 2 = that kernel stores its output straight from the registers instead
+    of through shared memory and TMA; 4 = it stores no output at all, for timing only)."""
     import os
     lib = _lib.load()
     if os.environ.get("SB_GRU_KSPLIT") is not None:

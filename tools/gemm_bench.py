@@ -1,10 +1,13 @@
 """Developer tool: time sb_gemm_bf16_tn at the GEMM shapes of one north-star training step
-(B = 64, T' = 247, M = 247 * 64 = 15808 tokens, 5 x biGRU-1024), with the call sites' operand
-layouts (MN-major views, bias, accumulate, the library's K split), under three kernels:
-    c2      the default selection (gemm_bf16_tn_c2_kernel for N > 128)
+(B = 64, T' = 247, M = 247 * 64 = 15808 tokens, 5 x biGRU-1024, conv2 of the front-end), with
+the call sites' operand layouts (MN-major views, bias, accumulate, the library's K split), under:
+    c2      the default selection (gemm_bf16_tn_c2_kernel for N > 128, TMA-store epilogue)
+    regs    sb_debug_gemm_flags(2): the same kernel, output stored straight from the registers
     legacy  sb_debug_gemm_flags(1): gemm_bf16_tn_kernel at 128 x 128 for every N > 64
     cublas  torch.matmul on the same bf16 operands (bf16 output), as a yardstick
-    python tools/gemm_bench.py [--reps 20] [--rounds 3]"""
+    nostore sb_debug_gemm_flags(4), with --nostore: the c2 kernel with no output at all (timing
+            only: the mainloop alone)
+    python tools/gemm_bench.py [--reps 20] [--rounds 3] [--nostore] [--only SUBSTRING]"""
 import argparse
 import subprocess
 import sys
@@ -88,6 +91,19 @@ def shapes():
         lambda: ops.gemm_bf16_tn(dghn[BP:, :H], hb[:Ms, :H], out=dwhh[2 * H:],
                                  accumulate=True, a_mn=True, b_mn=True),
         lambda: torch.matmul(dghn[BP:, :H].t(), hb[:Ms, :H]), 2.0 * H * H * Ms)
+    dl = rnd(M, 32)                    # fc output gradient (vocabulary padded to 32)
+    wT = rnd(D, 32)
+    dy = torch.empty(M, D, device="cuda")
+    add("fc dY 15808x2048x32", 1,
+        lambda: ops.gemm_bf16_tn(dl, wT, out=dy),
+        lambda: torch.matmul(dl, wT.t()), 2.0 * M * D * 32)
+    MC = BP * 247 * 15                 # conv2 patch rows: B x T' x F'
+    dC = rnd(MC, 32)
+    Wp = rnd(32, 1280)                 # [Co][Kp] = [K][N]
+    dA = torch.empty(MC, 1280, device="cuda")
+    add("conv2 dA 237120x1280x32 bT", 1,
+        lambda: ops.gemm_bf16_tn(dC, Wp, out=dA, b_mn=True),
+        lambda: torch.matmul(dC, Wp), 2.0 * MC * 1280 * 32)
     return out
 
 
@@ -107,41 +123,49 @@ def run_ours(fn, flags, reps):
     lib.sb_debug_gemm_flags(flags)
     try:
         ms = timed(fn, reps)
-        return ms, lib.sb_debug_gemm_kernel().decode()
+        return ms, (lib.sb_debug_gemm_kernel().decode(), lib.sb_debug_gemm_epilogue().decode())
     finally:
         lib.sb_debug_gemm_flags(0)
 
 
-def main(reps, rounds):
+def main(reps, rounds, nostore, only):
     print("device:", card())
     print("ms per launch (median of %d rounds of %d launches); TFLOP/s = 2MNK / time" % (rounds, reps))
-    step = {"c2": 0.0, "legacy": 0.0, "cublas": 0.0}
+    flags = {"c2": 0, "regs": 2, "legacy": 1}
+    if nostore:
+        flags["nostore"] = 4
+    cols = list(flags) + ["cublas"]
+    step = {k: 0.0 for k in cols}
     for name, n, ours, cub, flops in shapes():
-        res = {"c2": [], "legacy": [], "cublas": []}
+        if only and not any(o in name for o in only):
+            continue
+        res = {k: [] for k in cols}
         kern = {}
         for _ in range(rounds):
-            ms, kern["c2"] = run_ours(ours, 0, reps)
-            res["c2"].append(ms)
-            ms, kern["legacy"] = run_ours(ours, 1, reps)
-            res["legacy"].append(ms)
+            for k, f in flags.items():
+                ms, kern[k] = run_ours(ours, f, reps)
+                res[k].append(ms)
             res["cublas"].append(timed(cub, reps))
         med = {k: sorted(v)[len(v) // 2] for k, v in res.items()}
-        print("%-52s x%-2d  c2 %7.3f ms %5.0f TF/s (%s) | legacy %7.3f ms %5.0f TF/s (%s) | "
-              "cublas %7.3f ms %5.0f TF/s | c2/legacy %.3f"
-              % (name, n, med["c2"], flops / med["c2"] / 1e9, kern["c2"], med["legacy"],
-                 flops / med["legacy"] / 1e9, kern["legacy"], med["cublas"],
-                 flops / med["cublas"] / 1e9, med["c2"] / med["legacy"]))
+        print("%-52s x%-2d " % (name, n) + " | ".join(
+            "%s %7.3f ms %5.0f TF/s%s" % (k, med[k], flops / med[k] / 1e9,
+                                          " (%s %s)" % kern[k] if k in kern else "")
+            for k in cols) + " | c2/regs %.3f" % (med["c2"] / med["regs"]))
         if "both directions" in name:
             continue              # an alternative to the per-direction launches, not extra work
-        for k in step:
+        for k in cols:
             step[k] += n * med[k]
-    print("per-step GEMM time of these shapes (per-direction dW_ih): c2 %.2f ms, legacy %.2f ms, "
-          "cublas %.2f ms" % (step["c2"], step["legacy"], step["cublas"]))
+    print("per-step GEMM time of these shapes (per-direction dW_ih): " +
+          ", ".join("%s %.2f ms" % (k, step[k]) for k in cols))
 
 
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--nostore", action="store_true",
+                    help="add a column with the c2 kernel's output stores skipped (flag 4)")
+    ap.add_argument("--only", action="append", default=[],
+                    help="time only the shapes whose name contains this (repeatable)")
     a = ap.parse_args()
-    main(a.reps, a.rounds)
+    main(a.reps, a.rounds, a.nostore, a.only)

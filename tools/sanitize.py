@@ -68,15 +68,28 @@ _lib.load().sb_debug_gru_flags(0)
 assert fwd_kernel == "ks2", fwd_kernel
 print("2-CTA K-split GRU forward ok", l9.item())
 # the 128 x 256 GEMM over 2-CTA clusters: odd M-tile count (unpaired last tile), ragged N and K,
-# MN-major operands, accumulating with the library's K split
+# MN-major operands, accumulating with and without the library's K split; under both epilogues
+# (flag 2: stores straight from the registers instead of through shared memory and TMA)
 from speech_b200 import ops
 A = torch.randn(304, 200, device="cuda").bfloat16()
-Bm = torch.randn(200, 304, device="cuda").bfloat16()
-ops.gemm_bf16_tn(A, Bm.t().contiguous(), bias=torch.randn(304, device="cuda"))
-acc = torch.zeros(304, 304, device="cuda")
-ops.gemm_bf16_tn(A.t().contiguous(), Bm, out=acc, accumulate=True, a_mn=True, b_mn=True)
-torch.cuda.synchronize()
-gemm_kernel = _lib.load().sb_debug_gemm_kernel().decode()
-assert gemm_kernel == "c2_128x256", gemm_kernel
+Bm = torch.randn(200, 304, device="cuda").bfloat16()[:, :303]       # N = 303, row pitch 304
+Ak = torch.randn(5000, 304, device="cuda").bfloat16()
+Bk = torch.randn(5000, 304, device="cuda").bfloat16()[:, :303]
+for gemm_flags, want in ((0, ("tma", "tma_reduce", "regs")), (2, ("regs", "regs", "regs"))):
+    _lib.load().sb_debug_gemm_flags(gemm_flags)
+    got = []
+    out = torch.zeros(304, 304, device="cuda")[:, :303]              # ragged N, padded row pitch
+    ops.gemm_bf16_tn(A, Bm.t().contiguous(), out=out, bias=torch.randn(303, device="cuda"))
+    got.append(_lib.load().sb_debug_gemm_epilogue().decode())
+    acc = torch.zeros(304, 304, device="cuda")[:, :303]
+    ops.gemm_bf16_tn(A.t().contiguous(), Bm, out=acc, accumulate=True, a_mn=True, b_mn=True)
+    got.append(_lib.load().sb_debug_gemm_epilogue().decode())
+    ops.gemm_bf16_tn(Ak, Bk, out=acc, accumulate=True, a_mn=True, b_mn=True)    # split K
+    got.append(_lib.load().sb_debug_gemm_epilogue().decode())
+    torch.cuda.synchronize()
+    _lib.load().sb_debug_gemm_flags(0)
+    gemm_kernel = _lib.load().sb_debug_gemm_kernel().decode()
+    assert gemm_kernel == "c2_128x256", gemm_kernel
+    assert tuple(got) == want, (gemm_flags, got)
 print("2-CTA GEMM ok")
 torch.cuda.synchronize()
