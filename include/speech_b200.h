@@ -88,7 +88,11 @@ int sb_gemm_bf16_tn(const void* A, long long lda, const void* B, long long ldb, 
  *   gates  [T*Bp][ndir][4][H] f32 saved r,z,n,(W_hn h + b_hn) for backward (out; may be NULL)
  *   workspace  >= sb_gru_fwd_workspace_size bytes, 1024-byte aligned: per-chunk ready counters
  *          and the double-buffered exchange tiles of h_t (zeroed by the call itself)
- * Constraints: H % 16 == 0, Bp % 8 == 0, Bp <= 128, ndir*H/16 <= number of SMs.
+ * Constraints: H % 16 == 0, Bp % 8 == 0, Bp <= 128, and either ndir*H/16 <= number of SMs
+ *   (W_hh slices resident in shared memory) or, for wider layers, H % U == 0 and
+ *   ndir*H/U <= number of SMs for U = 16 or 32 (the wide kernel: U units per CTA, W_hh partly streamed
+ *   from L2 every step).  Ceiling: ndir*H <= 32 * SMs (2112 bidirectional, 4224 unidirectional
+ *   on a 132-SM H100 SXM).
  * ------------------------------------------------------------------------------------- */
 int sb_gru_fwd_workspace_size(int Bp, int H, int ndir, size_t* bytes);
 int sb_gru_fwd(const float* gi, const void* whh_bf16, const float* bhh, float* y, void* xn_bf16,
@@ -112,7 +116,9 @@ int sb_gru_fwd_f32(const float* gi, const float* whh_f32, const float* bhh, floa
  *          (the weight gradients contract these token-major operands directly with
  *           SB_GEMM_A_MN | SB_GEMM_B_MN; no transposed copies exist)
  *   dbih, dbhh [ndir*3H] f32 accumulated (+=)
- *   workspace  >= sb_gru_bwd_workspace_size bytes, 1024-byte aligned (zeroed by the call itself)
+ *   workspace  >= sb_gru_bwd_workspace_size bytes, 1024-byte aligned (zeroed by the call itself;
+ *          at widths that run the wide kernel it also holds W_hh^T, ndir*3H*H bf16)
+ * Constraints: those of sb_gru_fwd.
  */
 int sb_gru_bwd_workspace_size(int Bp, int H, int ndir, size_t* bytes);
 int sb_gru_bwd(const float* dy, const float* y, const float* gates, const void* whh_bf16,
@@ -120,9 +126,12 @@ int sb_gru_bwd(const float* dy, const float* y, const float* gates, const void* 
                size_t workspace_bytes, int T, int Bp, int H, int ndir, void* stream);
 
 /* Width Hp >= H at which sb_gru_fwd / sb_gru_bwd run a layer of H hidden units: H rounded up to
- * a multiple of 16, if both calls accept that width: the constraints above, the shared-memory
- * ring of each pass and the co-residency of its grid on the current device (SB_ERR_UNSUPPORTED
- * otherwise; the answer needs a CUDA device).  The caller pads the layer with Hp - H zero units per direction (zero W_ih / W_hh rows, W_hh
+ * a multiple of 16, if both calls accept that width with the resident kernels: the constraints
+ * above, the shared-memory ring of each pass and the co-residency of its grid on the current
+ * device.  Otherwise the width of the wide kernels: H rounded up to a multiple of U, U = 16 or 32
+ * the smallest whose grid of ndir*Hp/U CTAs fits on the SMs, so Hp - H < U, provided both wide
+ * passes fit in shared memory and are co-resident.  SB_ERR_UNSUPPORTED past the ceiling above
+ * (the answer needs a CUDA device).  The caller pads the layer with Hp - H zero units per direction (zero W_ih / W_hh rows, W_hh
  * columns and biases; zero W_ih columns of the next layer): they stay exactly 0 for all t. */
 int sb_gru_plan(int Bp, int H, int ndir, int* Hp);
 
@@ -443,12 +452,26 @@ const char* sb_debug_gemm_epilogue(void);
  * mode of the grid barrier, 256 / 512 = always (wherever the K-split backward kernel applies) /
  * never use its L2 reduce-scatter mode (the mode the backward uses when both directions do not
  * fit as thread-block clusters but do fit without), 1024 = the K-split forward over 2-CTA clusters
- * wherever it applies (H % 128 == 0, at most 64 batch rows; by default only from H = 512 up);
- * 1 / 2 are timing ablations (results become wrong). */
+ * wherever it applies (H % 128 == 0, at most 64 batch rows; by default only from H = 512 up),
+ * 2048 = the wide kernels with no resident W_hh chunks wherever they apply (every width they
+ * take, so that the weight stream is tested at small widths); 1 / 2 are timing ablations
+ * (results become wrong). */
 int sb_debug_gru_flags(int flags);
 /* Developer hook: which forward recurrence kernel the last sb_gru_fwd launched: "plain", "kt"
- * (transposed-accumulator K split), "ks4" / "ks2" (K split over 4- / 2-CTA clusters), "none". */
+ * (transposed-accumulator K split), "ks4" / "ks2" (K split over 4- / 2-CTA clusters), "wide"
+ * (U units per CTA, W_hh partly streamed), "none". */
 const char* sb_debug_gru_fwd_kernel(void);
+/* Developer hook: which backward recurrence kernel the last sb_gru_bwd launched: "plain", "kt",
+ * "ks4" (K split over 4-CTA clusters), "ks_l2" (its L2 reduce-scatter mode), "ks4_x2" (one
+ * clustered launch per direction), "wide", "none". */
+const char* sb_debug_gru_bwd_kernel(void);
+/* Developer hook: plan of the last wide launch of a pass (backward = 0: sb_gru_fwd, 1: sb_gru_bwd):
+ * out[0] = units per CTA, out[1] = resident and out[2] = streamed 64-wide K chunks of W_hh per
+ * CTA; all three 0 when that launch ran another kernel. */
+int sb_debug_gru_plan(int backward, int* out);
+/* Developer hook: gather-ring size in KB of the wide recurrence kernels (kb > 0 sets it; returns the
+ * size in use).  Changes the shared memory of the next wide plans and launches. */
+int sb_debug_gru_wide_ring(int kb);
 /* Developer hook: enable (1, default) / disable (0) the K-split backward GRU kernel. */
 int sb_debug_gru_ksplit(int enable);
 /* Developer hook: set the preferred thread-block-cluster size (1, 2, 4 or 8) of the GRU kernels;

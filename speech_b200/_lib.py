@@ -90,6 +90,9 @@ SIGNATURES = {
     "sb_debug_gru_ksplit": (_c_int, [_c_int]),
     "sb_debug_gru_flags": (_c_int, [_c_int]),
     "sb_debug_gru_fwd_kernel": (ctypes.c_char_p, []),
+    "sb_debug_gru_bwd_kernel": (ctypes.c_char_p, []),
+    "sb_debug_gru_plan": (_c_int, [_c_int, ctypes.POINTER(_c_int)]),
+    "sb_debug_gru_wide_ring": (_c_int, [_c_int]),
     "sb_debug_umma_mn": (_c_int, [_c_int, _c_int, _c_int]),
     "sb_debug_gemm_flags": (_c_int, [_c_int]),
     "sb_debug_gemm_kernel": (ctypes.c_char_p, []),

@@ -59,6 +59,7 @@ struct GruFwdParams {
   unsigned long long* dbg;  // optional timeline (CTA 0): [step][16] globaltimer stamps, or null
   int T, Bp, H, ndir, ring, gc;   // ring: slots (groups of gc chunks) in shared memory
   int ablate;          // developer knobs: see sb_debug_gru_flags
+  int rg, wr;          // wide kernels: resident weight groups, weight-ring slots
 };
 
 struct GruBwdParams {
@@ -78,6 +79,8 @@ struct GruBwdParams {
   int ablate;          // developer knobs: see sb_debug_gru_flags
   float* rs;           // L2 reduce-scatter staging [ndir][H/64][2][4][4][Bp][16] (gru_bwd_ks_kernel<true>)
   unsigned int* rsctr; // its counters, [ndir][H/64] x 32 words (one L2 line each)
+  int rg, wr;          // gru_bwd_wide_kernel: resident weight groups, weight-ring slots
+  bf16* whhT;          // gru_bwd_wide_kernel: [ndir][H][3H] W_hh transposed (each CTA its rows)
 };
 
 SB_DEVINL unsigned long long gtime() {
@@ -1773,6 +1776,563 @@ gru_bwd_kt_kernel(const __grid_constant__ CUtensorMap tm_d0,
   cluster_sync_all();
 }
 
+// =============================================================================================
+// wide layers: W_hh no longer fits in the shared memory of one CTA per 16 units per SM.
+//
+// CTA c of direction d owns U = 16 or 32 hidden units (ndir * H / U <= SM count).  Its weight
+// slice is NW = 3U rows of W_hh (forward) or U rows of W_hh^T (backward), cut into 64-wide K
+// chunks handled in groups of gc chunks.  The first rg groups stay resident in shared memory; the
+// remaining ones are streamed from L2 every step through a ring of wr slots of their own (TMA with
+// an evict_last hint: the weights are the only operand every step re-reads).  The producer issues
+// the first min(streamed, wr) weight groups of a step BEFORE it waits on the grid barrier, so that
+// they travel during the wait; the rest follow the gather group they pair with.  Producer order
+// never waits on something not yet issued: the gather slot of group g is released by group
+// g - ring, the weight slot of streamed group g by streamed group g - wr, both issued earlier.
+// The all-gather of h_{t-1} / dgh_t, the grid barrier, the .cs stores and the GRU_STAMP points are
+// those of gru_fwd_kernel / gru_bwd_kernel.  The epilogue maps thread = (batch row, 8 units) with
+// 2048 / U rows per pass of the 256 threads, so NQ = 2 passes at U = 32 above 64 rows.
+// The backward reads its weight tiles K-major from a transposed copy W_hh^T in the workspace
+// that each CTA writes for its own U rows in its prologue, so both passes share one tile format.
+// Shared memory: gather ring | resident groups | weight ring (at least 16 KB - Bp*128 after the
+// gather ring: the 64/128-row A read of the last slot runs past it) | barriers | bias | product.
+// =============================================================================================
+static constexpr int GRU_WIDE_MAX_WR = 8;
+static constexpr int GRU_WIDE_GATHER_KB = 64;   // default gather-ring bytes / 1024 (see below)
+static constexpr int GRU_FORCE_STREAM = 2048;   // sb_debug_gru_flags bit: wide kernels, rg = 0
+
+SB_DEVINL uint64_t l2_evict_last_policy() {
+  uint64_t pol;
+  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+  return pol;
+}
+SB_DEVINL void tma_load_2d_hint(void* smem_dst, const void* tmap, uint64_t* bar, int32_t c0,
+                                int32_t c1, uint64_t pol) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes"
+      ".L2::cache_hint [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)),
+        "r"(c0), "r"(c1), "l"(pol)
+      : "memory");
+}
+
+struct WideSmem {
+  uint8_t* ring;     // gather ring
+  uint8_t* wres;     // resident weight groups
+  uint8_t* wring;    // streamed weight groups
+  uint64_t *full, *empty, *wfull, *wempty, *accfull, *wresbar;
+  float* scratch;    // [4 * U]: bias (forward) / bias-gradient reduction (backward)
+  float* accbuf;     // [Bp][NW + 4]
+};
+
+__host__ __device__ inline int gru_wide_wbytes(int rg, int wr, int wgroup, int Bp) {
+  const int w = (rg + wr) * wgroup;
+  return w > 16384 - Bp * 128 ? w : 16384 - Bp * 128;
+}
+
+SB_DEVINL WideSmem wide_carve(uint8_t* raw, int ring_bytes, int rg, int wgroup, int wbytes, int U) {
+  WideSmem s;
+  s.ring = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(raw) + 1023) &
+                                      ~static_cast<uintptr_t>(1023));
+  s.wres = s.ring + ring_bytes;
+  s.wring = s.wres + rg * wgroup;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s.wres + wbytes);
+  s.full = bars;
+  s.empty = bars + GRU_MAX_RING;
+  s.wfull = bars + 2 * GRU_MAX_RING;
+  s.wempty = s.wfull + GRU_WIDE_MAX_WR;
+  s.accfull = s.wempty + GRU_WIDE_MAX_WR;
+  s.wresbar = s.accfull + 1;
+  s.scratch = reinterpret_cast<float*>(s.wresbar + 1);
+  s.accbuf = s.scratch + 4 * U;
+  return s;
+}
+
+// Weight group g into `dst` (gc chunks of NW rows = nbox boxes of U rows each; box b of chunk c
+// comes from rows wrow0 + b * wstep, columns c * 64 of the weight tensor map).
+SB_DEVINL void wide_load_wgroup(uint8_t* dst, const CUtensorMap* tw, uint64_t* bar, int g, int gc,
+                                int U, int nbox, int wrow0, int wstep, uint64_t pol) {
+  for (int i = 0; i < gc; ++i) {
+    const int c = g * gc + i;
+    for (int b = 0; b < nbox; ++b)
+      tma_load_2d_hint(dst + (i * nbox + b) * U * 128, tw, bar, c * 64, wrow0 + b * wstep, pol);
+  }
+}
+
+// streamed weight group g (rg <= g < ngroups) into weight-ring slot wn % wr; wn counts the
+// streamed groups issued since the launch
+SB_DEVINL void wide_issue_wgroup(const WideSmem& s, const CUtensorMap* tw, int g, int gc, int U,
+                                 int nbox, int wr, unsigned int& wn, int wrow0, int wstep,
+                                 uint64_t pol) {
+  const int slot = (int)(wn % (unsigned int)wr);
+  const unsigned int use = wn / (unsigned int)wr;
+  if (use > 0) mbar_wait(&s.wempty[slot], (use - 1u) & 1u);
+  mbar_expect_tx(&s.wfull[slot], (uint32_t)(gc * nbox * U * 128));
+  wide_load_wgroup(s.wring + slot * gc * nbox * U * 128, tw, &s.wfull[slot], g, gc, U, nbox, wrow0,
+                   wstep, pol);
+  ++wn;
+}
+
+// TMA producer of one product: wide_prefetch_weights ahead of the grid barrier, wide_gather after
+// it (the gather interleaved with the streamed weight groups the prefetch left out)
+SB_DEVINL void wide_prefetch_weights(const WideSmem& s, const CUtensorMap* tw, int ngroups, int gc,
+                                     int rg, int wr, int U, int nbox, int wrow0, int wstep,
+                                     unsigned int& wn, uint64_t pol) {
+  const int sg = ngroups - rg;
+  const int pre = sg < wr ? sg : wr;
+  for (int g = rg; g < rg + pre; ++g)
+    wide_issue_wgroup(s, tw, g, gc, U, nbox, wr, wn, wrow0, wstep, pol);
+}
+// The gather ring of the wide kernels counts its uses across steps (gn), so any ring of >= 2
+// slots works: every reuse waits for the slot's release, whatever the group count.
+SB_DEVINL void wide_gather(const WideSmem& s, const CUtensorMap* tm, const CUtensorMap* tw,
+                           int row0, int Bp, int ngroups, int ring, int gc, int rg, int wr, int U,
+                           int nbox, int wrow0, int wstep, unsigned int& gn, unsigned int& wn,
+                           uint64_t pol, uint32_t rank, uint32_t cs) {
+  const int sg = ngroups - rg;
+  const int pre = sg < wr ? sg : wr;
+  const int stride = Bp * 128;
+  const uint16_t mask = (uint16_t)((1u << cs) - 1u);
+  for (int g = 0; g < ngroups; ++g, ++gn) {
+    const int slot = (int)(gn % (unsigned int)ring);
+    const unsigned int use = gn / (unsigned int)ring;
+    if (use > 0) mbar_wait(&s.empty[slot], (use - 1u) & 1u);   // released by ALL CTAs of the cluster
+    mbar_expect_tx(&s.full[slot], (uint32_t)(stride * gc));
+    for (int i = 0; i < gc; ++i) {
+      const int c = g * gc + i;
+      if ((uint32_t)c % cs != rank) continue;
+      uint8_t* dst = s.ring + (slot * gc + i) * stride;
+      if (cs > 1) tma_load_2d_mc(dst, tm, &s.full[slot], c * 64, row0, mask);
+      else tma_load_2d(dst, tm, &s.full[slot], c * 64, row0);
+    }
+    if (g >= rg + pre) wide_issue_wgroup(s, tw, g, gc, U, nbox, wr, wn, wrow0, wstep, pol);
+  }
+}
+
+// MMA warpgroup, product k: D[Bp x NW] over all groups, resident or streamed; parks D in accbuf
+// (pitch NW + 4) and arrives on accfull (count 128).  wn counts the streamed groups consumed.  One
+// group's MMAs stay in flight while the next group's operands are awaited: a group's gather and
+// weight slots are released once the following group has been issued and it has retired.
+template <int NW, bool TWO>
+SB_DEVINL void wide_mma(const WideSmem& s, int Bp, int ngroups, int ring, int gc, int rg, int wr,
+                        unsigned int& gn, unsigned int& wn, uint32_t cs) {
+  constexpr int WCHUNK = NW * 128;
+  const int stride = Bp * 128;
+  const bool leader = (threadIdx.x & 127) == 0;
+  float d0[NW / 2], d1[NW / 2];
+  int prev_slot = -1, prev_wslot = -1;
+  auto release = [&](int slot, int wslot) {
+    if (!leader || slot < 0) return;
+    if (cs > 1) mbar_arrive_all_ctas(&s.empty[slot], cs);
+    else mbar_arrive(&s.empty[slot]);
+    if (wslot >= 0) mbar_arrive(&s.wempty[wslot]);
+  };
+  for (int g = 0; g < ngroups; ++g, ++gn) {
+    const int slot = (int)(gn % (unsigned int)ring);
+    mbar_wait(&s.full[slot], (gn / (unsigned int)ring) & 1u);
+    int wslot = -1;
+    const uint8_t* wsrc = s.wres + g * gc * WCHUNK;
+    if (g >= rg) {
+      wslot = (int)(wn % (unsigned int)wr);
+      mbar_wait(&s.wfull[wslot], (wn / (unsigned int)wr) & 1u);
+      wsrc = s.wring + wslot * gc * WCHUNK;
+      ++wn;
+    }
+    wgmma_fence();
+    for (int i = 0; i < gc; ++i) {
+      const int c = g * gc + i;
+      const uint32_t sa = smem_u32(s.ring + (slot * gc + i) * stride);
+      const uint64_t da0 = gmma_desc_sw128_kmajor(sa);
+      const uint64_t da1 = gmma_desc_sw128_kmajor(sa + 64 * 128);
+      const uint64_t db = gmma_desc_sw128_kmajor(smem_u32(wsrc + i * WCHUNK));
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
+        const uint32_t acc = (c > 0 || kk > 0) ? 1u : 0u;
+        wgmma_bf16<NW>(d0, da0 + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), acc);
+        if constexpr (TWO) wgmma_bf16<NW>(d1, da1 + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), acc);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<1>();          // the previous group's MMAs have retired
+    release(prev_slot, prev_wslot);
+    prev_slot = slot;
+    prev_wslot = wslot;
+  }
+  wgmma_wait<0>();
+  release(prev_slot, prev_wslot);
+  wgmma_fence_regs(d0);
+  wg_store_rows<NW>(d0, s.accbuf, NW + 4, 0, Bp);
+  if constexpr (TWO) {
+    wgmma_fence_regs(d1);
+    wg_store_rows<NW>(d1, s.accbuf, NW + 4, 64, Bp);
+  }
+  mbar_arrive(s.accfull);
+}
+
+// one-time setup shared by both wide kernels: zero the operand regions, barriers, resident groups
+SB_DEVINL void wide_setup(const WideSmem& s, int ring_bytes, int wbytes, uint32_t csize,
+                          const CUtensorMap* tm, const CUtensorMap* tw) {
+  const int tid = threadIdx.x;
+  for (int k = tid; k < (ring_bytes + wbytes) / 16; k += GRU_THREADS)
+    reinterpret_cast<uint4*>(s.ring)[k] = make_uint4(0, 0, 0, 0);
+  if (tid == 0) {
+    for (int i = 0; i < GRU_MAX_RING; ++i) {
+      mbar_init(&s.full[i], 1);
+      mbar_init(&s.empty[i], csize);
+    }
+    for (int i = 0; i < GRU_WIDE_MAX_WR; ++i) {
+      mbar_init(&s.wfull[i], 1);
+      mbar_init(&s.wempty[i], 1);
+    }
+    mbar_init(s.accfull, 128);
+    mbar_init(s.wresbar, 1);
+    mbar_fence_init();
+    tma_prefetch_desc(tm);
+    tma_prefetch_desc(tw);
+  }
+  fence_proxy_async_smem();
+}
+
+template <int U, int NQ>
+__global__ void __launch_bounds__(GRU_THREADS, 1)
+gru_fwd_wide_kernel(const __grid_constant__ CUtensorMap tm_d0,
+                    const __grid_constant__ CUtensorMap tm_d1,
+                    const __grid_constant__ CUtensorMap tm_w, const GruFwdParams p) {
+  constexpr int NW = 3 * U;
+  constexpr int WCHUNK = NW * 128;
+  constexpr int RPT = 2048 / U;      // batch rows per pass of the 256 epilogue threads
+  extern __shared__ uint8_t smem_raw[];
+  const int H = p.H, Bp = p.Bp, T = p.T;
+  const int nC = H / U;
+  const int dir = blockIdx.x / nC;
+  const int j0 = (blockIdx.x % nC) * U;
+  const int nchunks = (H + 63) / 64;
+  const int gc = p.gc, ngroups = nchunks / gc, rg = p.rg, wr = p.wr;
+  const int ring_bytes = p.ring * gc * Bp * 128;
+  const int wbytes = gru_wide_wbytes(rg, wr, gc * WCHUNK, Bp);
+  const WideSmem s = wide_carve(smem_raw, ring_bytes, rg, gc * WCHUNK, wbytes, U);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int D = p.ndir * H;
+  const CUtensorMap* tm = dir == 0 ? &tm_d0 : &tm_d1;
+  const uint32_t crank = cluster_rank(), csize = cluster_size();
+  const int wrow0 = dir * 3 * H + j0;   // gate b of the slice: rows wrow0 + b * H of W_hh
+
+  wide_setup(s, ring_bytes, wbytes, csize, tm, &tm_w);
+  if (tid < NW) s.scratch[tid] = p.bhh[dir * 3 * H + (tid / U) * H + j0 + tid % U];
+  __syncthreads();
+  cluster_sync_all();
+  unsigned int* ctr = p.barrier + dir * 32;
+
+  if (warp == GRU_TMA_WARP) {
+    if (lane == 0) {
+      const uint64_t pol = l2_evict_last_policy();
+      if (rg > 0) {
+        mbar_expect_tx(s.wresbar, (uint32_t)(rg * gc * WCHUNK));
+        for (int g = 0; g < rg; ++g)
+          wide_load_wgroup(s.wres + g * gc * WCHUNK, &tm_w, s.wresbar, g, gc, U, 3, wrow0, H, pol);
+      }
+      unsigned int gn = 0, wn = 0;
+      for (int step = 1; step < T; ++step) {
+        const int t = dir == 0 ? step : (T - 1 - step);
+        const int tp = dir == 0 ? t - 1 : t + 1;
+        wide_prefetch_weights(s, &tm_w, ngroups, gc, rg, wr, U, 3, wrow0, H, wn, pol);
+        grid_wait(ctr, (unsigned int)nC * step);   // all CTAs published h_{tp}
+        GRU_STAMP(0);
+        wide_gather(s, tm, &tm_w, tp * Bp, Bp, ngroups, p.ring, gc, rg, wr, U, 3, wrow0, H, gn,
+                    wn, pol, crank, csize);
+        GRU_STAMP(1);
+      }
+    }
+  } else if (warp >= GRU_MMA_WARP) {
+    if (rg > 0) mbar_wait(s.wresbar, 0);
+    unsigned int gn = 0, wn = 0;
+    for (int step = 1; step < T; ++step) {
+      if (Bp > 64) wide_mma<NW, true>(s, Bp, ngroups, p.ring, gc, rg, wr, gn, wn, csize);
+      else wide_mma<NW, false>(s, Bp, ngroups, p.ring, gc, rg, wr, gn, wn, csize);
+      if (tid == GRU_MMA_WARP * 32) GRU_STAMP(2);
+    }
+  } else {
+    // ===================== epilogue: thread = (batch row, 8 of the CTA's U units) per pass =====
+    const int rsub = tid % RPT;
+    const int uo = (tid / RPT) * GRU_UPT;
+    const int ju = j0 + uo;
+    float hprev[NQ][GRU_UPT];
+    float bias[3][GRU_UPT];
+#pragma unroll
+    for (int g = 0; g < 3; ++g)
+#pragma unroll
+      for (int jj = 0; jj < GRU_UPT; ++jj) bias[g][jj] = s.scratch[g * U + uo + jj];
+#pragma unroll
+    for (int q = 0; q < NQ; ++q)
+#pragma unroll
+      for (int jj = 0; jj < GRU_UPT; ++jj) hprev[q][jj] = 0.f;
+    for (int step = 0; step < T; ++step) {
+      const int t = dir == 0 ? step : (T - 1 - step);
+      float gi[NQ][3][GRU_UPT];
+#pragma unroll
+      for (int q = 0; q < NQ; ++q) {
+        const int row = rsub + q * RPT;
+        if (row < Bp) {
+          const float* g = p.gi + ((long long)t * Bp + row) * (p.ndir * 3 * H) + dir * 3 * H + ju;
+#pragma unroll
+          for (int gg = 0; gg < 3; ++gg) ld8(g + gg * H, gi[q][gg]);
+        }
+      }
+      if (step > 0) {
+        mbar_wait(s.accfull, (step - 1) & 1);
+        if (tid == 0) GRU_STAMP(3);
+      }
+      float rr[NQ][GRU_UPT], zz[NQ][GRU_UPT], nn[NQ][GRU_UPT], hn[NQ][GRU_UPT];
+      bool any = false;
+#pragma unroll
+      for (int q = 0; q < NQ; ++q) {
+        const int row = rsub + q * RPT;
+        if (row >= Bp) continue;
+        any = true;
+        const float* ar = s.accbuf + row * (NW + 4) + uo;
+#pragma unroll
+        for (int jj = 0; jj < GRU_UPT; ++jj) {
+          const float a0 = step > 0 ? ar[jj] : 0.f;
+          const float a1 = step > 0 ? ar[U + jj] : 0.f;
+          const float a2 = step > 0 ? ar[2 * U + jj] : 0.f;
+          rr[q][jj] = fast_sigmoid(gi[q][0][jj] + a0 + bias[0][jj]);
+          zz[q][jj] = fast_sigmoid(gi[q][1][jj] + a1 + bias[1][jj]);
+          hn[q][jj] = a2 + bias[2][jj];
+          nn[q][jj] = fast_tanh(gi[q][2][jj] + rr[q][jj] * hn[q][jj]);
+          hprev[q][jj] = (1.f - zz[q][jj]) * nn[q][jj] + zz[q][jj] * hprev[q][jj];
+        }
+        const long long m = (long long)t * Bp + row;
+        *reinterpret_cast<uint4*>(p.xn + m * D + dir * H + ju) = pack8(hprev[q]);
+      }
+      if (tid == 0) GRU_STAMP(5);
+      if (any) fence_proxy_async_global();   // generic writes -> other CTAs' TMA reads
+      if (tid == 0) GRU_STAMP(6);
+      epi_barrier();
+      if (tid == 0) {
+        GRU_STAMP(7);
+        grid_arrive(ctr);
+        GRU_STAMP(9);
+      }
+#pragma unroll
+      for (int q = 0; q < NQ; ++q) {
+        const int row = rsub + q * RPT;
+        if (row >= Bp) continue;
+        const long long m = (long long)t * Bp + row;
+        st8(p.y + m * D + dir * H + ju, hprev[q]);
+        if (p.gates) {
+          float* go = p.gates + ((m * p.ndir + dir) * 4) * H + ju;
+          st8(go, rr[q]);
+          st8(go + H, zz[q]);
+          st8(go + 2 * H, nn[q]);
+          st8(go + 3 * H, hn[q]);
+        }
+      }
+      if (tid == 0) GRU_STAMP(10);
+    }
+  }
+
+  __syncthreads();
+  cluster_sync_all();
+}
+
+template <int U, int NQ>
+__global__ void __launch_bounds__(GRU_THREADS, 1)
+gru_bwd_wide_kernel(const __grid_constant__ CUtensorMap tm_d0,
+                    const __grid_constant__ CUtensorMap tm_d1,
+                    const __grid_constant__ CUtensorMap tm_w, const GruBwdParams p) {
+  constexpr int WCHUNK = U * 128;
+  constexpr int RPT = 2048 / U;
+  extern __shared__ uint8_t smem_raw[];
+  const int H = p.H, Bp = p.Bp, T = p.T;
+  const int nC = H / U;
+  const int dir = blockIdx.x / nC;
+  const int j0 = (blockIdx.x % nC) * U;
+  const int K3 = 3 * H;
+  const int nchunks = (K3 + 63) / 64;
+  const int gc = p.gc, ngroups = nchunks / gc, rg = p.rg, wr = p.wr;
+  const int ring_bytes = p.ring * gc * Bp * 128;
+  const int wbytes = gru_wide_wbytes(rg, wr, gc * WCHUNK, Bp);
+  const WideSmem s = wide_carve(smem_raw, ring_bytes, rg, gc * WCHUNK, wbytes, U);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int D = p.ndir * H;
+  const CUtensorMap* tm = dir == 0 ? &tm_d0 : &tm_d1;
+  const uint32_t crank = cluster_rank(), csize = cluster_size();
+  const int wrow0 = dir * H + j0;       // rows of W_hh^T: the CTA's units
+
+  // this CTA's U rows of W_hh^T (read back by its own TMA only): thread = (k, 8 units)
+  for (int k = tid; k < K3 * (U / 8); k += GRU_THREADS) {
+    const int kk = k % K3, piece = k / K3;
+    const uint4 v = *reinterpret_cast<const uint4*>(
+        p.whh + ((long long)dir * K3 + kk) * H + j0 + piece * 8);
+    const bf16* e = reinterpret_cast<const bf16*>(&v);
+#pragma unroll
+    for (int q = 0; q < 8; ++q) p.whhT[(long long)(wrow0 + piece * 8 + q) * K3 + kk] = e[q];
+  }
+  fence_proxy_async_global();   // generic writes -> this CTA's TMA reads
+  wide_setup(s, ring_bytes, wbytes, csize, tm, &tm_w);
+  __syncthreads();
+  cluster_sync_all();
+  unsigned int* ctr = p.barrier + dir * 32;
+
+  if (warp == GRU_TMA_WARP) {
+    if (lane == 0) {
+      const uint64_t pol = l2_evict_last_policy();
+      if (rg > 0) {
+        mbar_expect_tx(s.wresbar, (uint32_t)(rg * gc * WCHUNK));
+        for (int g = 0; g < rg; ++g)
+          wide_load_wgroup(s.wres + g * gc * WCHUNK, &tm_w, s.wresbar, g, gc, U, 1, wrow0, 0, pol);
+      }
+      unsigned int gn = 0, wn = 0;
+      for (int step = 0; step + 1 < T; ++step) {
+        wide_prefetch_weights(s, &tm_w, ngroups, gc, rg, wr, U, 1, wrow0, 0, wn, pol);
+        grid_wait(ctr, (unsigned int)nC * (step + 1));   // dgh of this step is complete
+        GRU_STAMP(0);
+        wide_gather(s, tm, &tm_w, (step & 1) * Bp, Bp, ngroups, p.ring, gc, rg, wr, U, 1, wrow0, 0,
+                    gn, wn, pol, crank, csize);
+        GRU_STAMP(1);
+      }
+    }
+  } else if (warp >= GRU_MMA_WARP) {
+    if (rg > 0) mbar_wait(s.wresbar, 0);
+    unsigned int gn = 0, wn = 0;
+    for (int step = 0; step + 1 < T; ++step) {
+      if (Bp > 64) wide_mma<U, true>(s, Bp, ngroups, p.ring, gc, rg, wr, gn, wn, csize);
+      else wide_mma<U, false>(s, Bp, ngroups, p.ring, gc, rg, wr, gn, wn, csize);
+      if (tid == GRU_MMA_WARP * 32) GRU_STAMP(2);
+    }
+  } else {
+    const int rsub = tid % RPT;
+    const int uo = (tid / RPT) * GRU_UPT;
+    const int ju = j0 + uo;
+    float dh_rec[NQ][GRU_UPT];
+    float db_r[NQ][GRU_UPT], db_z[NQ][GRU_UPT], db_n[NQ][GRU_UPT], db_hn[NQ][GRU_UPT];
+#pragma unroll
+    for (int q = 0; q < NQ; ++q)
+#pragma unroll
+      for (int jj = 0; jj < GRU_UPT; ++jj) {
+        dh_rec[q][jj] = 0.f; db_r[q][jj] = 0.f; db_z[q][jj] = 0.f; db_n[q][jj] = 0.f;
+        db_hn[q][jj] = 0.f;
+      }
+
+    for (int step = 0; step < T; ++step) {
+      const int t = dir == 0 ? (T - 1 - step) : step;
+      const int tp = dir == 0 ? t - 1 : t + 1;
+      const bool has_prev = dir == 0 ? (t > 0) : (t < T - 1);
+      bf16* xb = p.xchg + ((long long)(dir * 2 + (step & 1)) * Bp) * K3;
+      // saved activations of this step: independent of the recurrence, fetched first
+      float rr[NQ][GRU_UPT], zz[NQ][GRU_UPT], nn[NQ][GRU_UPT], hn[NQ][GRU_UPT];
+      float dh[NQ][GRU_UPT], hp[NQ][GRU_UPT];
+#pragma unroll
+      for (int q = 0; q < NQ; ++q) {
+        const int row = rsub + q * RPT;
+        if (row >= Bp) continue;
+        const long long m = (long long)t * Bp + row;
+        const float* go = p.gates + ((m * p.ndir + dir) * 4) * H + ju;
+        ld8(go, rr[q]);
+        ld8(go + H, zz[q]);
+        ld8(go + 2 * H, nn[q]);
+        ld8(go + 3 * H, hn[q]);
+        ld8(p.dy + m * D + dir * H + ju, dh[q]);
+        if (has_prev) {
+          ld8(p.y + ((long long)tp * Bp + row) * D + dir * H + ju, hp[q]);
+        } else {
+#pragma unroll
+          for (int jj = 0; jj < GRU_UPT; ++jj) hp[q][jj] = 0.f;
+        }
+      }
+      if (step > 0) {
+        mbar_wait(s.accfull, (step - 1) & 1);
+        if (tid == 0) GRU_STAMP(3);
+      }
+      uint4 o_r[NQ], o_z[NQ], o_n[NQ], o_nr[NQ];   // this step's dgi / dghn rows, bf16
+      bool any = false;
+#pragma unroll
+      for (int q = 0; q < NQ; ++q) {
+        const int row = rsub + q * RPT;
+        if (row >= Bp) continue;
+        any = true;
+        const float* ar = s.accbuf + row * (U + 4) + uo;
+        float dr[GRU_UPT], dz[GRU_UPT], dn[GRU_UPT], dnr[GRU_UPT];
+#pragma unroll
+        for (int jj = 0; jj < GRU_UPT; ++jj) {
+          if (step > 0) dh_rec[q][jj] += ar[jj];
+          const float g = dh[q][jj] + dh_rec[q][jj];
+          dn[jj] = g * (1.f - zz[q][jj]) * (1.f - nn[q][jj] * nn[q][jj]);
+          dz[jj] = g * (hp[q][jj] - nn[q][jj]) * zz[q][jj] * (1.f - zz[q][jj]);
+          dr[jj] = dn[jj] * hn[q][jj] * rr[q][jj] * (1.f - rr[q][jj]);
+          dnr[jj] = dn[jj] * rr[q][jj];
+          dh_rec[q][jj] = g * zz[q][jj];
+          db_r[q][jj] += dr[jj];
+          db_z[q][jj] += dz[jj];
+          db_n[q][jj] += dn[jj];
+          db_hn[q][jj] += dnr[jj];
+        }
+        o_r[q] = pack8(dr); o_z[q] = pack8(dz); o_n[q] = pack8(dn); o_nr[q] = pack8(dnr);
+        if (step + 1 < T) {
+          bf16* x = xb + (long long)row * K3 + ju;
+          *reinterpret_cast<uint4*>(x) = o_r[q];
+          *reinterpret_cast<uint4*>(x + H) = o_z[q];
+          *reinterpret_cast<uint4*>(x + 2 * H) = o_nr[q];
+        }
+      }
+      if (step + 1 < T) {
+        if (tid == 0) GRU_STAMP(5);
+        if (any) fence_proxy_async_global();
+        if (tid == 0) GRU_STAMP(6);
+        epi_barrier();
+        if (tid == 0) {
+          GRU_STAMP(7);
+          grid_arrive(ctr);
+          GRU_STAMP(9);
+        }
+      }
+#pragma unroll
+      for (int q = 0; q < NQ; ++q) {
+        const int row = rsub + q * RPT;
+        if (row >= Bp) continue;
+        const long long m = (long long)t * Bp + row;
+        bf16* o = p.dgi + m * (p.ndir * K3) + dir * K3 + ju;
+        st_stream_u4(o, o_r[q]);
+        st_stream_u4(o + H, o_z[q]);
+        st_stream_u4(o + 2 * H, o_n[q]);
+        st_stream_u4(p.dghn + m * D + dir * H + ju, o_nr[q]);
+      }
+      if (tid == 0) GRU_STAMP(10);
+    }
+    // ---- bias gradients: the warp's rows share its 8 units; reduce over the CTA ----
+    epi_barrier();
+    float* red = s.scratch;   // [4][U]: r z n hn
+    for (int i = tid; i < 4 * U; i += GRU_EPI) red[i] = 0.f;
+    epi_barrier();
+#pragma unroll
+    for (int q = 0; q < NQ; ++q) {
+      const bool active = rsub + q * RPT < Bp;
+#pragma unroll
+      for (int jj = 0; jj < GRU_UPT; ++jj) {
+        const float a = warp_sum(active ? db_r[q][jj] : 0.f);
+        const float b = warp_sum(active ? db_z[q][jj] : 0.f);
+        const float c = warp_sum(active ? db_n[q][jj] : 0.f);
+        const float d = warp_sum(active ? db_hn[q][jj] : 0.f);
+        if (lane == 0) {
+          atomicAdd(&red[uo + jj], a);
+          atomicAdd(&red[U + uo + jj], b);
+          atomicAdd(&red[2 * U + uo + jj], c);
+          atomicAdd(&red[3 * U + uo + jj], d);
+        }
+      }
+    }
+    epi_barrier();
+    if (tid < 3 * U) {
+      const int g = tid / U, jj = tid % U;
+      const int idx = dir * K3 + g * H + j0 + jj;
+      atomicAdd(p.dbih + idx, red[tid]);
+      atomicAdd(p.dbhh + idx, g < 2 ? red[tid] : red[3 * U + jj]);
+    }
+  }
+
+  __syncthreads();
+  cluster_sync_all();
+}
+
 int make_tmap_bf16_2d(CUtensorMap* map, const void* base, long long rows, long long cols,
                       long long ld, int box_rows);
 
@@ -1811,7 +2371,7 @@ static int gru_ring_slots(int wbytes, int Bp, int nchunks, int acc_cols, int* gc
 static int g_gru_cluster = 4;   // preferred cluster size (developer knob: sb_debug_gru_cluster)
 static int g_gru_last_cluster = 0;
 // which forward recurrence kernel the last sb_gru_fwd launched (sb_debug_gru_fwd_kernel)
-enum { GRU_FWD_NONE, GRU_FWD_PLAIN, GRU_FWD_KT, GRU_FWD_KS4, GRU_FWD_KS2 };
+enum { GRU_FWD_NONE, GRU_FWD_PLAIN, GRU_FWD_KT, GRU_FWD_KS4, GRU_FWD_KS2, GRU_FWD_WIDE };
 static int g_gru_last_fwd = GRU_FWD_NONE;
 static int gru_fwd_launched(int kind) {
   g_gru_last_fwd = kind;
@@ -1929,6 +2489,83 @@ static int gru_launch_exact(const void* kernel, int grid, int cs, size_t smem, v
   return SB_OK;
 }
 
+// ---- wide kernels: plan, selection, launch -----------------------------------------------------
+enum { GRU_BWD_NONE, GRU_BWD_PLAIN, GRU_BWD_KT, GRU_BWD_KS4, GRU_BWD_KS_L2, GRU_BWD_KS4_X2,
+       GRU_BWD_WIDE };
+static int g_gru_last_bwd = GRU_BWD_NONE;
+static int gru_bwd_launched(int kind) {
+  g_gru_last_bwd = kind;
+  return SB_OK;
+}
+// [pass][units per CTA, resident K chunks, streamed K chunks] of the last launch; zeros unless it
+// ran a wide kernel
+static int g_gru_last_plan[2][3];
+
+struct GruWidePlan {
+  int U, gc, ngroups, ring, rg, wr;
+  size_t smem;
+};
+
+// Bytes of the wide kernels' gather ring (developer knob sb_debug_gru_wide_ring; the default was
+// chosen by tools/gru_wide_bench.py --ring-sweep, see the comment of gru_fwd_wide_kernel).
+static int g_gru_wide_gather_kb = GRU_WIDE_GATHER_KB;
+
+// Shared memory of one wide pass over nchunks K chunks of nw weight rows.  Groups of gc = 2
+// chunks where 2 divides nchunks; the gather ring holds g_gru_wide_gather_kb, at least 2 and at
+// most GRU_MAX_RING slots (the MMA warpgroup holds two while one group is in flight); the rest
+// holds as many resident groups as fit next to a weight ring of 2 slots, or every group.
+// no_resident (GRU_FORCE_STREAM): rg = 0.
+static bool gru_wide_layout(int Bp, int U, int nchunks, int nw, bool no_resident, GruWidePlan* w) {
+  const int budget = 227 * 1024;
+  w->U = U;
+  w->gc = nchunks % 2 == 0 ? 2 : 1;
+  w->ngroups = nchunks / w->gc;
+  const int gslot = w->gc * Bp * 128, wslot = w->gc * nw * 128;
+  const int fixed = 1024 /*align*/ + (2 * GRU_MAX_RING + 2 * GRU_WIDE_MAX_WR + 2) * 8 +
+                    4 * U * 4 + Bp * (nw + 4) * 4;
+  w->ring = std::min(std::max(g_gru_wide_gather_kb * 1024 / gslot, 2), GRU_MAX_RING);
+  const int avail = budget - fixed - w->ring * gslot;
+  if (!no_resident && avail >= w->ngroups * wslot) {
+    w->rg = w->ngroups;
+    w->wr = 0;
+  } else {
+    w->rg = no_resident ? 0 : std::min(w->ngroups - 1, std::max(0, avail / wslot - 2));
+    w->wr = std::min(std::min(w->ngroups - w->rg, GRU_WIDE_MAX_WR), (avail - w->rg * wslot) / wslot);
+    if (w->wr < std::min(w->ngroups - w->rg, 2)) return false;
+  }
+  w->smem = (size_t)fixed + (size_t)w->ring * gslot + gru_wide_wbytes(w->rg, w->wr, wslot, Bp);
+  return w->smem <= (size_t)budget;
+}
+
+// Wide plan of one pass at width H: U = the smallest of 16, 32 that divides H, puts the grid of
+// ndir * H / U CTAs on the SMs and whose shared memory fits.  Arithmetic only (workspace queries).
+static bool gru_wide_plan(int Bp, int H, int ndir, bool backward, bool no_resident,
+                          GruWidePlan* w) {
+  if (Bp <= 0 || Bp % 8 != 0 || Bp > 128 || H <= 0 || (ndir != 1 && ndir != 2)) return false;
+  for (int U = 16; U <= 32; U += 16) {
+    if (H % U != 0 || ndir * (H / U) > sb::device_sm_count()) continue;
+    const int nchunks = backward ? (3 * H + 63) / 64 : (H + 63) / 64;
+    if (gru_wide_layout(Bp, U, nchunks, backward ? U : 3 * U, no_resident, w)) return true;
+  }
+  return false;
+}
+
+static const void* gru_wide_kernel_fn(const GruWidePlan& w, int Bp, bool backward) {
+  if (backward)
+    return w.U == 16 ? (const void*)gru_bwd_wide_kernel<16, 1>
+           : Bp > 64 ? (const void*)gru_bwd_wide_kernel<32, 2>
+                     : (const void*)gru_bwd_wide_kernel<32, 1>;
+  return w.U == 16 ? (const void*)gru_fwd_wide_kernel<16, 1>
+         : Bp > 64 ? (const void*)gru_fwd_wide_kernel<32, 2>
+                   : (const void*)gru_fwd_wide_kernel<32, 1>;
+}
+
+static void gru_record_plan(int pass, const GruWidePlan* w) {
+  g_gru_last_plan[pass][0] = w ? w->U : 0;
+  g_gru_last_plan[pass][1] = w ? w->rg * w->gc : 0;
+  g_gru_last_plan[pass][2] = w ? (w->ngroups - w->rg) * w->gc : 0;
+}
+
 }  // namespace sb
 
 using namespace sb;
@@ -1945,7 +2582,8 @@ extern "C" int sb_debug_gru_timeline(void* dev_buffer) {
 // 64 / 128: polling mode of the grid barrier in the K-split kernels (see grid_wait);
 // 256 / 512: always (wherever the K-split backward kernel applies) / never use its L2
 // reduce-scatter mode (see ks_exchange and sb_gru_bwd); 1024: the K-split forward over 2-CTA
-// clusters wherever it applies (H % 128 == 0, batch rows <= 64), skipping the 4-CTA ones
+// clusters wherever it applies (H % 128 == 0, batch rows <= 64), skipping the 4-CTA ones;
+// 2048: the wide kernels with no resident weight chunks wherever they apply (tests the stream)
 extern "C" int sb_debug_gru_flags(int flags) {
   sb::g_gru_ablate = flags;
   return SB_OK;
@@ -1963,15 +2601,43 @@ extern "C" int sb_debug_gru_cluster(int cluster_size) {
   return sb::g_gru_last_cluster;
 }
 // which forward recurrence kernel the last sb_gru_fwd launched: "plain" (gru_fwd_kernel), "kt"
-// (gru_fwd_kt_kernel), "ks4" / "ks2" (gru_fwd_ks_kernel<4> / <2>); "none" before the first
+// (gru_fwd_kt_kernel), "ks4" / "ks2" (gru_fwd_ks_kernel<4> / <2>), "wide" (gru_fwd_wide_kernel);
+// "none" before the first
 extern "C" const char* sb_debug_gru_fwd_kernel(void) {
-  static const char* const names[] = {"none", "plain", "kt", "ks4", "ks2"};
+  static const char* const names[] = {"none", "plain", "kt", "ks4", "ks2", "wide"};
   return names[sb::g_gru_last_fwd];
 }
+// which backward recurrence kernel the last sb_gru_bwd launched: "plain" (gru_bwd_kernel), "kt"
+// (gru_bwd_kt_kernel), "ks4" (gru_bwd_ks_kernel over 4-CTA clusters), "ks_l2" (its L2
+// reduce-scatter mode), "ks4_x2" (one clustered launch per direction), "wide"
+// (gru_bwd_wide_kernel); "none" before the first
+extern "C" const char* sb_debug_gru_bwd_kernel(void) {
+  static const char* const names[] = {"none", "plain", "kt", "ks4", "ks_l2", "ks4_x2", "wide"};
+  return names[sb::g_gru_last_bwd];
+}
+// plan of the last sb_gru_fwd (backward = 0) / sb_gru_bwd (1) launch: out[0] units per CTA,
+// out[1] resident and out[2] streamed W_hh chunks of 64 per CTA; all 0 unless it was "wide"
+extern "C" int sb_debug_gru_plan(int backward, int* out) {
+  if (!out || (backward != 0 && backward != 1)) return SB_ERR_INVALID;
+  for (int i = 0; i < 3; ++i) out[i] = sb::g_gru_last_plan[backward][i];
+  return SB_OK;
+}
 
-static int gru_check(int T, int Bp, int H, int ndir) {
+// developer knob: gather-ring bytes / 1024 of the wide kernels (> 0 sets; returns the value in use)
+extern "C" int sb_debug_gru_wide_ring(int kb) {
+  if (kb > 0) sb::g_gru_wide_gather_kb = kb;
+  return sb::g_gru_wide_gather_kb;
+}
+
+static int gru_check_shape(int T, int Bp, int H, int ndir) {
   if (T <= 0 || Bp <= 0 || H <= 0 || (ndir != 1 && ndir != 2)) return SB_ERR_INVALID;
   if (H % GRU_HC != 0 || Bp % 8 != 0 || Bp > 128) return SB_ERR_UNSUPPORTED;
+  return SB_OK;
+}
+// the resident kernels: one CTA of 16 units per SM
+static int gru_check(int T, int Bp, int H, int ndir) {
+  const int rc = gru_check_shape(T, Bp, H, ndir);
+  if (rc != SB_OK) return rc;
   if (ndir * (H / GRU_HC) > sb::device_sm_count()) return SB_ERR_UNSUPPORTED;
   return SB_OK;
 }
@@ -2001,26 +2667,63 @@ static bool gru_coresident(const void* kernel, int grid, size_t smem) {
   return per_sm * sb::device_sm_count() >= grid;
 }
 
-// Width the recurrence kernels run a layer of H hidden units at: H rounded up to whole CTAs of
-// GRU_HC units, provided both passes accept that width: gru_check, the rings of the plain
-// forward and backward kernels (the kernels every shape falls back to) and their co-residency.
-// The caller pads the layer with zero units; such a unit stays exactly 0
-// (h_t = sigmoid(0) * h_{t-1} = 0) and its zero W_hh columns never reach a real unit.
+// Whether a pass runs the wide kernel at width H (and its plan): where the resident kernels do
+// not take the width (more CTAs of 16 units than SMs, or no ring next to the weight slice), or
+// everywhere the wide kernel applies under the developer flag GRU_FORCE_STREAM.  Arithmetic only.
+static bool gru_selects_wide(int Bp, int H, int ndir, bool backward, GruWidePlan* w) {
+  const bool force = (g_gru_ablate & GRU_FORCE_STREAM) != 0;
+  int gc = 1;
+  size_t smem = 0;
+  const bool resident = ndir * (H / GRU_HC) <= sb::device_sm_count() &&
+                        (backward ? gru_bwd_ring(Bp, H, &gc, &smem) : gru_fwd_ring(Bp, H, &gc, &smem)) >= 0;
+  return (force || !resident) && gru_wide_plan(Bp, H, ndir, backward, force, w);
+}
+
+// Width the recurrence kernels run a layer of H hidden units at.  First H rounded up to whole CTAs
+// of GRU_HC units, provided both passes accept that width with the resident kernels: gru_check,
+// the rings of the plain forward and backward kernels (the kernels every such shape falls back
+// to) and their co-residency.  Otherwise the wide kernels' width: H rounded up to whole CTAs of
+// U = 16 or 32 units (the smallest whose grid fits on the SMs), provided both wide passes fit in
+// shared memory and are co-resident.  The caller pads the layer with zero units; such a unit stays
+// exactly 0 (h_t = sigmoid(0) * h_{t-1} = 0) and its zero W_hh columns never reach a real unit.
 extern "C" int sb_gru_plan(int Bp, int H, int ndir, int* Hp) {
   if (!Hp || H <= 0) return SB_ERR_INVALID;
   const int hp = (H + GRU_HC - 1) / GRU_HC * GRU_HC;
-  const int rc = gru_check(1, Bp, hp, ndir);
+  const int rc = gru_check_shape(1, Bp, hp, ndir);
   if (rc != SB_OK) return rc;
-  int gc = 1;
-  size_t fsmem = 0, bsmem = 0;
-  if (gru_fwd_ring(Bp, hp, &gc, &fsmem) < 0 || gru_bwd_ring(Bp, hp, &gc, &bsmem) < 0)
-    return SB_ERR_UNSUPPORTED;
-  const int grid = ndir * (hp / GRU_HC);
-  if (!gru_coresident((const void*)gru_fwd_kernel, grid, fsmem) ||
-      !gru_coresident((const void*)gru_bwd_kernel, grid, bsmem))
-    return SB_ERR_UNSUPPORTED;
-  *Hp = hp;
-  return SB_OK;
+  if (gru_check(1, Bp, hp, ndir) == SB_OK) {
+    int gc = 1;
+    size_t fsmem = 0, bsmem = 0;
+    const int grid = ndir * (hp / GRU_HC);
+    if (gru_fwd_ring(Bp, hp, &gc, &fsmem) >= 0 && gru_bwd_ring(Bp, hp, &gc, &bsmem) >= 0 &&
+        gru_coresident((const void*)gru_fwd_kernel, grid, fsmem) &&
+        gru_coresident((const void*)gru_bwd_kernel, grid, bsmem)) {
+      *Hp = hp;
+      return SB_OK;
+    }
+  }
+  // each pass at hw: the kernel it will launch (wide, or resident where that pass still fits)
+  // must be co-resident with its exact grid and shared memory
+  auto pass_fits = [&](int hw, bool backward, int U) {
+    GruWidePlan w;
+    if (gru_selects_wide(Bp, hw, ndir, backward, &w))
+      return w.U == U && gru_coresident(gru_wide_kernel_fn(w, Bp, backward), ndir * (hw / U), w.smem);
+    int gc = 1;
+    size_t smem = 0;
+    if ((backward ? gru_bwd_ring(Bp, hw, &gc, &smem) : gru_fwd_ring(Bp, hw, &gc, &smem)) < 0 ||
+        ndir * (hw / GRU_HC) > sb::device_sm_count())
+      return false;
+    return gru_coresident(backward ? (const void*)gru_bwd_kernel : (const void*)gru_fwd_kernel,
+                          ndir * (hw / GRU_HC), smem);
+  };
+  for (int U = 16; U <= 32; U += 16) {
+    const int hw = (H + U - 1) / U * U;
+    if (pass_fits(hw, false, U) && pass_fits(hw, true, U)) {
+      *Hp = hw;
+      return SB_OK;
+    }
+  }
+  return SB_ERR_UNSUPPORTED;
 }
 
 // workspace of one recurrence launch: [0,1024) the per-direction grid-barrier words, then the
@@ -2060,7 +2763,10 @@ extern "C" int sb_gru_fwd_workspace_size(int Bp, int H, int ndir, size_t* bytes)
 extern "C" int sb_gru_fwd(const float* gi, const void* whh_bf16, const float* bhh, float* y,
                           void* xn_bf16, float* gates, void* workspace, size_t workspace_bytes,
                           int T, int Bp, int H, int ndir, void* stream_) {
-  int rc = gru_check(T, Bp, H, ndir);
+  GruWidePlan w;
+  const bool wide = gru_check_shape(T, Bp, H, ndir) == SB_OK &&
+                    gru_selects_wide(Bp, H, ndir, false, &w);
+  int rc = wide ? SB_OK : gru_check(T, Bp, H, ndir);
   if (rc != SB_OK) return rc;
   if (!gi || !whh_bf16 || !bhh || !y || !xn_bf16 || !workspace) return SB_ERR_INVALID;
   size_t need = 0;
@@ -2072,6 +2778,34 @@ extern "C" int sb_gru_fwd(const float* gi, const void* whh_bf16, const float* bh
   if (cudaMemsetAsync(workspace, 0, need, stream) != cudaSuccess) return SB_ERR_CUDA;
   uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
   unsigned int* barrier = reinterpret_cast<unsigned int*>(ws);
+  gru_record_plan(0, nullptr);
+
+  // ---- wide layers: U units per CTA, W_hh partly streamed from L2 (gru_fwd_wide_kernel) ----
+  if (wide) {
+    GruFwdParams p;
+    memset(&p, 0, sizeof(p));
+    p.gi = gi; p.whh = reinterpret_cast<const bf16*>(whh_bf16); p.bhh = bhh; p.y = y;
+    p.xn = reinterpret_cast<bf16*>(xn_bf16); p.gates = gates; p.barrier = barrier;
+    p.T = T; p.Bp = Bp; p.H = H; p.ndir = ndir; p.dbg = g_gru_dbg;
+    p.ring = w.ring; p.gc = w.gc; p.rg = w.rg; p.wr = w.wr;
+    CUtensorMap tm[3];
+    for (int d = 0; d < 2; ++d) {
+      const int dd = d < ndir ? d : 0;
+      rc = make_tmap_bf16_2d(&tm[d], p.xn + (size_t)dd * H, (long long)T * Bp, H,
+                             (long long)ndir * H, Bp);
+      if (rc != SB_OK) return rc;
+    }
+    rc = make_tmap_bf16_2d(&tm[2], p.whh, (long long)ndir * 3 * H, H, H, w.U);
+    if (rc != SB_OK) return rc;
+    void* args[] = {(void*)&tm[0], (void*)&tm[1], (void*)&tm[2], (void*)&p};
+    const int nCw = H / w.U;
+    rc = gru_launch(gru_wide_kernel_fn(w, Bp, false), ndir * nCw, gru_cluster_size(nCw), w.smem,
+                    args, stream);
+    if (rc != SB_OK) return rc;
+    gru_record_plan(0, &w);
+    return gru_fwd_launched(GRU_FWD_WIDE);
+  }
+
   int gc = 1;
   size_t smem = 0;
   const int ring = gru_fwd_ring(Bp, H, &gc, &smem);
@@ -2150,14 +2884,22 @@ extern "C" int sb_gru_fwd(const float* gi, const void* whh_bf16, const float* bh
   return rc == SB_OK ? gru_fwd_launched(GRU_FWD_PLAIN) : rc;
 }
 
-extern "C" int sb_gru_bwd_workspace_size(int Bp, int H, int ndir, size_t* bytes) {
-  if (!bytes || Bp <= 0 || H <= 0 || (ndir != 1 && ndir != 2)) return SB_ERR_INVALID;
-  // counters + the double-buffered exchange of dgh_t (Bp x 3H bf16 per direction and parity; the
-  // tile-major form of the K-split kernel rounds 3H up to whole 64-column chunks)
+// counters + the double-buffered exchange of dgh_t (Bp x 3H bf16 per direction and parity; the
+// tile-major form of the K-split kernel rounds 3H up to whole 64-column chunks) + the L2
+// reduce-scatter area; the wide kernel's W_hh^T ([ndir][H][3H] bf16) follows at this offset
+static size_t gru_bwd_ws_base(int Bp, int H, int ndir) {
   const size_t k3p = (size_t)((3 * H + 63) / 64) * 64;
   size_t z = 0;
-  *bytes = gru_ws_counters_bytes(ndir) + (size_t)ndir * 2 * Bp * k3p * sizeof(bf16) + 1024 +
-           gru_rs_bytes(Bp, H, ndir, &z);
+  return gru_ws_counters_bytes(ndir) + (size_t)ndir * 2 * Bp * k3p * sizeof(bf16) + 1024 +
+         gru_rs_bytes(Bp, H, ndir, &z);
+}
+
+extern "C" int sb_gru_bwd_workspace_size(int Bp, int H, int ndir, size_t* bytes) {
+  if (!bytes || Bp <= 0 || H <= 0 || (ndir != 1 && ndir != 2)) return SB_ERR_INVALID;
+  *bytes = gru_bwd_ws_base(Bp, H, ndir);
+  GruWidePlan w;
+  if (gru_check_shape(1, Bp, H, ndir) == SB_OK && gru_selects_wide(Bp, H, ndir, true, &w))
+    *bytes = (*bytes + 1023) / 1024 * 1024 + (size_t)ndir * 3 * H * H * sizeof(bf16);
   return SB_OK;
 }
 
@@ -2165,7 +2907,10 @@ extern "C" int sb_gru_bwd(const float* dy, const float* y, const float* gates,
                           const void* whh_bf16, void* dgi_bf16, void* dghn_bf16, float* dbih,
                           float* dbhh, void* workspace, size_t workspace_bytes, int T, int Bp,
                           int H, int ndir, void* stream_) {
-  int rc = gru_check(T, Bp, H, ndir);
+  GruWidePlan w;
+  const bool wide = gru_check_shape(T, Bp, H, ndir) == SB_OK &&
+                    gru_selects_wide(Bp, H, ndir, true, &w);
+  int rc = wide ? SB_OK : gru_check(T, Bp, H, ndir);
   if (rc != SB_OK) return rc;
   if (!dy || !y || !gates || !whh_bf16 || !dgi_bf16 || !dghn_bf16 || !dbih || !dbhh ||
       !workspace)
@@ -2190,12 +2935,34 @@ extern "C" int sb_gru_bwd(const float* dy, const float* y, const float* gates,
   size_t smem = 0;
   const int nC_ = H / GRU_HC;
   size_t rs_zeroed = 0;
-  const size_t rs_at = need - gru_rs_bytes(Bp, H, ndir, &rs_zeroed);
+  const size_t rs_at = gru_bwd_ws_base(Bp, H, ndir) - gru_rs_bytes(Bp, H, ndir, &rs_zeroed);
   p.rsctr = reinterpret_cast<unsigned int*>(ws + rs_at);
   p.rs = reinterpret_cast<float*>(ws + rs_at + rs_zeroed);
   // counters and barrier words start at zero; the exchange tiles too (columns past 3H of a
   // partial chunk are never written and must read as zero)
   if (cudaMemsetAsync(workspace, 0, rs_at + rs_zeroed, stream) != cudaSuccess) return SB_ERR_CUDA;
+  gru_record_plan(1, nullptr);
+
+  // ---- wide layers: U units per CTA, W_hh^T partly streamed from L2 (gru_bwd_wide_kernel) ----
+  if (wide) {
+    p.whhT = reinterpret_cast<bf16*>(ws + (gru_bwd_ws_base(Bp, H, ndir) + 1023) / 1024 * 1024);
+    p.ring = w.ring; p.gc = w.gc; p.rg = w.rg; p.wr = w.wr;
+    CUtensorMap tm[3];
+    for (int d = 0; d < 2; ++d) {
+      const int dd = d < ndir ? d : 0;
+      rc = make_tmap_bf16_2d(&tm[d], p.xchg + (size_t)dd * 2 * Bp * K3, 2LL * Bp, K3, K3, Bp);
+      if (rc != SB_OK) return rc;
+    }
+    rc = make_tmap_bf16_2d(&tm[2], p.whhT, (long long)ndir * H, K3, K3, w.U);
+    if (rc != SB_OK) return rc;
+    void* args[] = {(void*)&tm[0], (void*)&tm[1], (void*)&tm[2], (void*)&p};
+    const int nCw = H / w.U;
+    rc = gru_launch(gru_wide_kernel_fn(w, Bp, true), ndir * nCw, gru_cluster_size(nCw), w.smem,
+                    args, stream);
+    if (rc != SB_OK) return rc;
+    gru_record_plan(1, &w);
+    return gru_bwd_launched(GRU_BWD_WIDE);
+  }
   // ---- preferred: K-split over 4-CTA clusters ----
   if (g_gru_ksplit && H % 256 == 0 && nC_ % KS == 0 && (K3 / KS / 64) <= 16) {
     const int nq = K3 / KS / 64;
@@ -2217,7 +2984,7 @@ extern "C" int sb_gru_bwd(const float* dy, const float* y, const float* gates,
                          : Bp > 16 ? (const void*)gru_bwd_kt_kernel<2>
                                    : (const void*)gru_bwd_kt_kernel<1>;
         rc = gru_launch_exact(kt, ndir * nC_, KS, kt_smem, kargs, stream);
-        if (rc == SB_OK) return SB_OK;
+        if (rc == SB_OK) return gru_bwd_launched(GRU_BWD_KT);
       }
       // 1. both directions as 4-CTA clusters, reduce-scattering through DSMEM
       const void* ks = (const void*)gru_bwd_ks_kernel<false>;
@@ -2225,7 +2992,7 @@ extern "C" int sb_gru_bwd(const float* dy, const float* y, const float* gates,
       rc = SB_ERR_UNSUPPORTED;
       if (!(g_gru_ablate & 256)) {
         rc = gru_launch_exact(ks, ndir * nC_, KS, ks_smem, kargs, stream);
-        if (rc == SB_OK) return SB_OK;
+        if (rc == SB_OK) return gru_bwd_launched(GRU_BWD_KS4);
       }
       // 2. Both directions do not fit as 4-CTA clusters (an H100 holds 30 of them, 120 CTAs,
       // against 128 at H = 1024), but fit without a cluster, one CTA per SM: the same kernel
@@ -2235,7 +3002,7 @@ extern "C" int sb_gru_bwd(const float* dy, const float* y, const float* gates,
       if (rc == SB_ERR_UNSUPPORTED && !(g_gru_ablate & 512) &&
           gru_coresident(ks_l2, ndir * nC_, ks_smem)) {
         rc = gru_launch(ks_l2, ndir * nC_, 1, ks_smem, kargs, stream);
-        if (rc == SB_OK) return SB_OK;
+        if (rc == SB_OK) return gru_bwd_launched(GRU_BWD_KS_L2);
       }
       // 3. Neither fits (fewer SMs than CTAs, e.g. a 114-SM part): the directions one after the
       // other as clustered launches, each with its own barrier counter.  Still faster than the
@@ -2244,7 +3011,8 @@ extern "C" int sb_gru_bwd(const float* dy, const float* y, const float* gates,
         rc = gru_launch_exact(ks, nC_, KS, ks_smem, kargs, stream);
         if (rc == SB_OK) {
           p.dir0 = 1;   // kernel parameters are copied at launch
-          return gru_launch_exact(ks, nC_, KS, ks_smem, kargs, stream);
+          rc = gru_launch_exact(ks, nC_, KS, ks_smem, kargs, stream);
+          return rc == SB_OK ? gru_bwd_launched(GRU_BWD_KS4_X2) : rc;
         }
       }
     }
@@ -2260,6 +3028,7 @@ extern "C" int sb_gru_bwd(const float* dy, const float* y, const float* gates,
   }
   void* args[] = {(void*)&tm[0], (void*)&tm[1], (void*)&p};
   const int nC = H / GRU_HC;
-  return gru_launch((const void*)gru_bwd_kernel, ndir * nC, gru_cluster_size(nC), smem, args,
-                    stream);
+  rc = gru_launch((const void*)gru_bwd_kernel, ndir * nC, gru_cluster_size(nC), smem, args,
+                  stream);
+  return rc == SB_OK ? gru_bwd_launched(GRU_BWD_PLAIN) : rc;
 }

@@ -1,5 +1,6 @@
 """Developer tool: per-step timeline (ns) of CTA 0 of the GRU recurrence kernels at north-star width.
     python tools/gru_timeline.py [cluster size] [fwd|bwd] [sb_debug_gru_flags]
+(environment: TL_B batch rows, default 64; TL_H width, default 1024, e.g. 1280 for the wide kernels)
 Forward flags: 0 = default selection (gru_fwd_ks_kernel<2> over 2-CTA clusters for both directions
 of H = 1024 at <= 64 rows on a 132-SM H100), 32 = the plain gru_fwd_kernel, 1024 = the 2-CTA
 K-split forward forced."""
@@ -16,7 +17,7 @@ if len(sys.argv) > 3:
     print("flags:", sys.argv[3])
 torch.manual_seed(0)
 import os
-B, T, In, H = int(os.environ.get('TL_B', '64')), 64, 2048, 1024
+B, T, In, H = int(os.environ.get('TL_B', '64')), 64, 2048, int(os.environ.get('TL_H', '1024'))
 rnn = torch.nn.GRU(In, H, 1, batch_first=True, bidirectional=True).cuda()
 x = torch.randn(B, T, In, device="cuda")
 dbg = torch.zeros(64 * 16 + 512, dtype=torch.int64, device="cuda")
@@ -62,6 +63,8 @@ for step in (11, 40):
 print("cluster size used:", lib.sb_debug_gru_cluster(0))
 if MODE == "fwd":
     print("forward kernel:", lib.sb_debug_gru_fwd_kernel().decode())
+else:
+    print("backward kernel:", lib.sb_debug_gru_bwd_kernel().decode())
 print("mean step period (ns):", (d[60][9] - d[10][9]) / 50.0)
 
 if MODE == "fwd":

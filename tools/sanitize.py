@@ -67,6 +67,16 @@ fwd_kernel = _lib.load().sb_debug_gru_fwd_kernel().decode()
 _lib.load().sb_debug_gru_flags(0)
 assert fwd_kernel == "ks2", fwd_kernel
 print("2-CTA K-split GRU forward ok", l9.item())
+# the wide recurrence kernels with every W_hh chunk streamed (flag 2048) at a small width
+_lib.load().sb_debug_gru_flags(2048)
+mw = CTC(80, 28, cfg).cuda()
+l10 = mw.loss((inputs, labels)); l10.backward()
+torch.cuda.synchronize()
+kernels = (_lib.load().sb_debug_gru_fwd_kernel().decode(),
+           _lib.load().sb_debug_gru_bwd_kernel().decode())
+_lib.load().sb_debug_gru_flags(0)
+assert kernels == ("wide", "wide"), kernels
+print("streamed wide GRU ok", l10.item())
 # the 128 x 256 GEMM over 2-CTA clusters: odd M-tile count (unpaired last tile), ragged N and K,
 # MN-major operands, accumulating with and without the library's K split; under both epilogues
 # (flag 2: stores straight from the registers instead of through shared memory and TMA)
