@@ -304,6 +304,45 @@ int sb_s2s_beam_gather(const float* hx_in, const float* sx_in, const float* ax_i
                        float* sx_out, float* ax_out, const int* parent_row, const void* state,
                        int K, int H, int T, void* stream);
 
+/* Large vocabularies (csrc/s2s_vocab.cu, csrc/s2s.cu).  sb_s2s_attn_fwd runs the output projection
+ * in the utterance's last CTA, which holds every logit in shared memory: it takes fc_w only where
+ * sb_s2s_fc_fused(H, C) is 1 (C <= 7 H; pure host arithmetic).  Other shapes run the attention
+ * without fc_w, then:
+ *   sb_s2s_fc_rows    logits of R rows over many CTAs: o = hx + sx (sx may be NULL), row r written
+ *                     at logits + (r % row_group) * ld0 + (r / row_group) * ld1 (logits may be
+ *                     NULL); each logit is summed in an order that depends on H only, so a row
+ *                     projects to the same bits alone or among any number of rows.  The same launch
+ *                     reduces every row (deterministic, in-kernel tickets): optional arg-max (first
+ *                     maximum), greedy history[r * hist_stride + hist_col], end_count += 1 where
+ *                     the arg-max is end_tok, and the row's log-sum-exp, kept in the workspace
+ *   sb_s2s_fc_logp    logp (R, C) = logits - log-sum-exp of the last sb_s2s_fc_rows on the same
+ *                     workspace and shape (logp may alias a dense logits buffer)
+ *   workspace: >= sb_s2s_fc_workspace_size(R, C) bytes, ZERO before the first call; one workspace
+ *   serves every call with the same (R, C) on one stream.  H % 4 == 0, H <= 3200.
+ * The single-CTA sb_s2s_beam_select holds all K*C float64 candidates in shared memory:
+ * sb_s2s_beam_select_fits(K, C) is 1 where it runs (K <= 32, K*C*8 <= 200 KB).  Otherwise
+ *   sb_s2s_beam_select_split  the same selection and bookkeeping (same state, outputs and tie
+ *                     order) in two stages: per-tile top 2K candidates over many CTAs, then one
+ *                     CTA merges the tiles' lists; workspace >= sb_s2s_beam_split_workspace_size.
+ * Backward of the projection where sb_s2s_dout does not run (C > 8192): d_o = dlogits W_fc as a
+ * 3-pass split-bf16 sb_gemm_bf16_tn with SB_GEMM_B_MN (the host mirror, functions/s2s.py). */
+int sb_s2s_fc_fused(int H, int C);
+int sb_s2s_fc_workspace_size(long long R, int C, size_t* bytes);
+int sb_s2s_fc_rows(const float* hx, const float* sx, const float* fc_w, const float* fc_b,
+                   long long R, int H, int C, float* logits, int row_group, long long ld0,
+                   long long ld1, int* argmax, int* history, int hist_stride, int hist_col,
+                   int* end_count, int end_tok, const int* done, void* workspace,
+                   size_t workspace_bytes, void* stream);
+int sb_s2s_fc_logp(const float* logits, int row_group, long long ld0, long long ld1, float* logp,
+                   long long R, int C, const int* done, const void* workspace,
+                   size_t workspace_bytes, void* stream);
+int sb_s2s_beam_select_fits(int K, int C);
+int sb_s2s_beam_split_workspace_size(int K, int C, size_t* bytes);
+int sb_s2s_beam_select_split(const float* logp, void* state, double* c_scores, int* nodes,
+                             int* parent_row, int* tok_next, int* out_tokens, int K, int C,
+                             int end_tok, int step, int max_len, int node_cap, int c_cap,
+                             void* workspace, size_t workspace_bytes, void* stream);
+
 /* Beam expand/prune of Seq2Seq.beam_search (speech/models/seq2seq.py:200-212): indices and values
  * of the k best of n float64 scores, ordered by (score descending, index ascending) - the order of
  * the reference's stable sort over (beam, vocab) candidates. */

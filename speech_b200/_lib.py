@@ -63,6 +63,18 @@ SIGNATURES = {
                                     _c_int, _c_int, _c_int, _c_int, _vp]),
     "sb_s2s_beam_gather": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_int, _c_int, _c_int,
                                     _vp]),
+    "sb_s2s_fc_fused": (_c_int, [_c_int, _c_int]),
+    "sb_s2s_fc_workspace_size": (_c_int, [_c_ll, _c_int, ctypes.POINTER(_c_sz)]),
+    "sb_s2s_fc_rows": (_c_int, [_vp, _vp, _vp, _vp, _c_ll, _c_int, _c_int, _vp, _c_int, _c_ll,
+                                _c_ll, _vp, _vp, _c_int, _c_int, _vp, _c_int, _vp, _vp, _c_sz,
+                                _vp]),
+    "sb_s2s_fc_logp": (_c_int, [_vp, _c_int, _c_ll, _c_ll, _vp, _c_ll, _c_int, _vp, _vp, _c_sz,
+                                _vp]),
+    "sb_s2s_beam_select_fits": (_c_int, [_c_int, _c_int]),
+    "sb_s2s_beam_split_workspace_size": (_c_int, [_c_int, _c_int, ctypes.POINTER(_c_sz)]),
+    "sb_s2s_beam_select_split": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_int, _c_int,
+                                          _c_int, _c_int, _c_int, _c_int, _c_int, _vp, _c_sz,
+                                          _vp]),
     "sb_beam_topk": (_c_int, [_vp, _c_int, _c_int, _vp, _vp, _vp]),
     "sb_rnnt_workspace_size": (_c_int, [_c_int, _c_int, _c_int, ctypes.POINTER(_c_sz)]),
     "sb_rnnt_fwd_bwd": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int,

@@ -877,6 +877,9 @@ struct BeamParams {
   int K, C, end_tok, step, max_len, node_cap, c_cap;
 };
 
+SB_DEVINL void beam_bookkeep(const BeamParams& p, const int* sel_idx, const double* sel_sc,
+                             int want);
+
 __global__ void __launch_bounds__(256) s2s_beam_select_kernel(const BeamParams p) {
   extern __shared__ unsigned char bm_smem[];
   double* sc = reinterpret_cast<double*>(bm_smem);       // [K * C]
@@ -920,7 +923,121 @@ __global__ void __launch_bounds__(256) s2s_beam_select_kernel(const BeamParams p
     __syncthreads();
   }
   if (tid != 0) return;
-  // ---- the reference's bookkeeping, sequential (a handful of entries) ----
+  beam_bookkeep(p, sel_idx, sel_sc, want);
+}
+
+// ------------------------------------------------------------------------------------------------
+// split beam selection, for K*C candidates that do not fit one CTA's shared memory:
+//   stage 1 (s2s_beam_tiles): CTA per tile of BM_TILE flat indices i*C + c of the live rows; each
+//           keeps its own top min(2K, n) candidates by (score desc, index asc), in that order.
+//   stage 2 (s2s_beam_merge): one CTA merges the tiles' sorted lists (a head per tile) into the
+//           global first min(2K, nl*C) and runs the same bookkeeping.
+// The union of the top K and the first K non-ended candidates lies in the global top 2K (at most
+// K of the top K end in end_tok), so the 2K per tile lose nothing.
+// ------------------------------------------------------------------------------------------------
+static constexpr int BM_PER_THREAD = 16;
+static constexpr int BM_TILE = 256 * BM_PER_THREAD;
+
+// (score desc, index asc): does (s1, i1) come before (s2, i2)?  i < 0 = no candidate
+SB_DEVINL bool bm_before(double s1, int i1, double s2, int i2) {
+  return i1 >= 0 && (i2 < 0 || s1 > s2 || (s1 == s2 && i1 < i2));
+}
+
+// CTA-wide first of the 256 threads' (bs, bi); every thread gets it
+SB_DEVINL void bm_block_best(double& bs, int& bi, double* rs, int* ri) {
+  const int tid = threadIdx.x;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const double os = __shfl_xor_sync(0xffffffffu, bs, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+    if (bm_before(os, oi, bs, bi)) { bs = os; bi = oi; }
+  }
+  __syncthreads();                                   // rs / ri of the previous round are read
+  if ((tid & 31) == 0) { rs[tid >> 5] = bs; ri[tid >> 5] = bi; }
+  __syncthreads();
+  bs = rs[0]; bi = ri[0];
+  for (int w = 1; w < 8; ++w)
+    if (bm_before(rs[w], ri[w], bs, bi)) { bs = rs[w]; bi = ri[w]; }
+}
+
+__global__ void __launch_bounds__(256) s2s_beam_tiles_kernel(const BeamParams p, double* t_sc,
+                                                             int* t_idx, int* t_cnt) {
+  __shared__ double rs[8];
+  __shared__ int ri[8];
+  const BeamState* st = p.st;
+  if (st->done) return;
+  const int tid = threadIdx.x, tile = blockIdx.x, K2 = 2 * p.K, C = p.C;
+  const int n = st->nlive * C;
+  double v[BM_PER_THREAD];
+#pragma unroll
+  for (int j = 0; j < BM_PER_THREAD; ++j) {
+    const int i = tile * BM_TILE + j * 256 + tid;
+    v[j] = nan("");
+    if (i < n) {
+      const int r = i / C, c = i - r * C;
+      v[j] = st->score[r] + (double)p.logp[(size_t)r * C + c];
+    }
+  }
+  int q = 0;
+  for (; q < K2; ++q) {
+    double bs = 0.0;
+    int bi = -1;
+#pragma unroll
+    for (int j = 0; j < BM_PER_THREAD; ++j)      // ascending index: strict > keeps the first
+      if (!isnan(v[j]) && (bi < 0 || v[j] > bs)) { bs = v[j]; bi = tile * BM_TILE + j * 256 + tid; }
+    bm_block_best(bs, bi, rs, ri);
+    if (bi < 0) break;
+    if (tid == 0) { t_sc[(size_t)tile * K2 + q] = bs; t_idx[(size_t)tile * K2 + q] = bi; }
+#pragma unroll
+    for (int j = 0; j < BM_PER_THREAD; ++j)
+      if (tile * BM_TILE + j * 256 + tid == bi) v[j] = nan("");
+  }
+  if (tid == 0) t_cnt[tile] = q;
+}
+
+__global__ void __launch_bounds__(256) s2s_beam_merge_kernel(const BeamParams p, const double* t_sc,
+                                                             const int* t_idx, const int* t_cnt,
+                                                             int ntiles) {
+  extern __shared__ int bmm_head[];                  // [ntiles] next entry of each tile's list
+  __shared__ double rs[8];
+  __shared__ int ri[8];
+  __shared__ int sel_idx[2 * BM_MAXK];
+  __shared__ double sel_sc[2 * BM_MAXK];
+  BeamState* st = p.st;
+  if (st->done) return;
+  const int tid = threadIdx.x, K2 = 2 * p.K;
+  const int want = min(K2, st->nlive * p.C);
+  for (int t = tid; t < ntiles; t += 256) bmm_head[t] = 0;
+  __syncthreads();
+  for (int q = 0; q < want; ++q) {
+    double bs = 0.0;
+    int bi = -1;
+    for (int t = tid; t < ntiles; t += 256) {
+      const int h = bmm_head[t];
+      if (h < t_cnt[t]) {
+        const double s = t_sc[(size_t)t * K2 + h];
+        const int i = t_idx[(size_t)t * K2 + h];
+        if (bm_before(s, i, bs, bi)) { bs = s; bi = i; }
+      }
+    }
+    bm_block_best(bs, bi, rs, ri);
+    if (tid == 0) {
+      sel_idx[q] = bi;
+      sel_sc[q] = bs;
+      if (bi >= 0) bmm_head[bi / BM_TILE] += 1;
+    }
+    __syncthreads();
+  }
+  if (tid != 0) return;
+  beam_bookkeep(p, sel_idx, sel_sc, want);
+}
+
+// ---- the reference's bookkeeping, sequential (a handful of entries): the first `want` candidates
+// in (score desc, index asc) order -> complete / next beam / stop rule / back-track ----
+SB_DEVINL void beam_bookkeep(const BeamParams& p, const int* sel_idx, const double* sel_sc,
+                             int want) {
+  BeamState* st = p.st;
+  const int K = p.K, C = p.C, nl = st->nlive;
   int old_node[BM_MAXK];
   for (int r = 0; r < nl; ++r) old_node[r] = st->node[r];
   int nb = 0;
@@ -1242,6 +1359,55 @@ extern "C" int sb_s2s_beam_select(const float* logp, void* state, double* c_scor
   p.K = K; p.C = C; p.end_tok = end_tok; p.step = step; p.max_len = max_len;
   p.node_cap = node_cap; p.c_cap = c_cap;
   sb::s2s_beam_select_kernel<<<1, 256, smem, stream>>>(p);
+  return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
+}
+
+extern "C" int sb_s2s_beam_select_fits(int K, int C) {
+  return (K > 0 && K <= sb::BM_MAXK && C > 0 && (long long)K * C * 8 <= 200 * 1024) ? 1 : 0;
+}
+
+static int beam_split_tiles(int K, int C) {
+  return (int)(((long long)K * C + sb::BM_TILE - 1) / sb::BM_TILE);
+}
+
+extern "C" int sb_s2s_beam_split_workspace_size(int K, int C, size_t* bytes) {
+  if (!bytes || K <= 0 || C <= 0) return SB_ERR_INVALID;
+  const size_t nt = (size_t)beam_split_tiles(K, C);
+  *bytes = nt * 2 * K * (sizeof(double) + sizeof(int)) + nt * sizeof(int) + 64;
+  return SB_OK;
+}
+
+extern "C" int sb_s2s_beam_select_split(const float* logp, void* state, double* c_scores,
+                                        int* nodes, int* parent_row, int* tok_next,
+                                        int* out_tokens, int K, int C, int end_tok, int step,
+                                        int max_len, int node_cap, int c_cap, void* workspace,
+                                        size_t workspace_bytes, void* stream_) {
+  if (!logp || !state || !c_scores || !nodes || !parent_row || !tok_next || !out_tokens ||
+      !workspace)
+    return SB_ERR_INVALID;
+  if (K <= 0 || K > sb::BM_MAXK || C <= 0 || (long long)K * C > 0x7fffffffLL)
+    return SB_ERR_UNSUPPORTED;
+  size_t need = 0;
+  sb_s2s_beam_split_workspace_size(K, C, &need);
+  if (workspace_bytes < need) return SB_ERR_WORKSPACE;
+  const int nt = beam_split_tiles(K, C);
+  const size_t smem = (size_t)nt * sizeof(int);
+  if (smem > 200 * 1024) return SB_ERR_UNSUPPORTED;
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (smem > 40 * 1024 &&
+      cudaFuncSetAttribute(sb::s2s_beam_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           (int)smem) != cudaSuccess)
+    return SB_ERR_CUDA;
+  double* t_sc = reinterpret_cast<double*>(workspace);
+  int* t_idx = reinterpret_cast<int*>(t_sc + (size_t)nt * 2 * K);
+  int* t_cnt = t_idx + (size_t)nt * 2 * K;
+  sb::BeamParams p;
+  p.logp = logp; p.st = reinterpret_cast<sb::BeamState*>(state); p.c_scores = c_scores;
+  p.nodes = nodes; p.parent_row = parent_row; p.tok_next = tok_next; p.out_tokens = out_tokens;
+  p.K = K; p.C = C; p.end_tok = end_tok; p.step = step; p.max_len = max_len;
+  p.node_cap = node_cap; p.c_cap = c_cap;
+  sb::s2s_beam_tiles_kernel<<<nt, 256, 0, stream>>>(p, t_sc, t_idx, t_cnt);
+  sb::s2s_beam_merge_kernel<<<1, 256, smem, stream>>>(p, t_sc, t_idx, t_cnt, nt);
   return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
 }
 

@@ -17,8 +17,35 @@ def _f(t):
     return t.detach().float().contiguous()
 
 
+# Routes by shape.  The attention kernel runs the output projection in one CTA per utterance,
+# which holds all C logits next to its 8 H-float tiles: C <= 7 H (sb_s2s_fc_fused).  Larger
+# vocabularies project over many CTAs (sb_s2s_fc_rows, csrc/s2s_vocab.cu).  sb_s2s_dout holds one
+# row of dlogits in shared memory (C <= 8192); past that d_o runs on the GEMM.  The single-CTA beam
+# selection holds all K*C float64 candidates (<= 200 KB); past that it runs split over many CTAs.
+FC_FUSED_MAX_RATIO = 7
+DOUT_MAX_CLASSES = 8192
+BEAM_SELECT_MAX_BYTES = 200 * 1024
+BEAM_MAX = 32
+
+
+def fc_fused(H, C):
+    """True where the attention kernel computes the logits itself (= sb_s2s_fc_fused(H, C))."""
+    return H > 0 and 0 < C <= FC_FUSED_MAX_RATIO * H
+
+
+def dout_fits(C):
+    """True where sb_s2s_dout runs the backward of the projection; else it runs on the GEMM."""
+    return 0 < C <= DOUT_MAX_CLASSES
+
+
+def beam_select_fits(K, C):
+    """True where the single-CTA beam selection runs (= sb_s2s_beam_select_fits(K, C))."""
+    return 0 < K <= BEAM_MAX and C > 0 and K * C * 8 <= BEAM_SELECT_MAX_BYTES
+
+
 class DecoderWeights:
-    """fp32 contiguous views of the decoder parameters, in the layout the kernels take."""
+    """fp32 contiguous views of the decoder parameters, in the layout the kernels take.  `fused`:
+    the attention kernel runs the output projection (fc_fused), else sb_s2s_fc_rows does."""
 
     def __init__(self, m):
         self.emb = _f(m.embedding.weight)
@@ -36,6 +63,7 @@ class DecoderWeights:
         self.C = self.fc_w.shape[0]
         if self.emb.shape[1] != self.H:
             raise _lib.SpeechB200Error("Seq2Seq: embedding_dim must equal the encoder dim (ix + sx)")
+        self.fused = fc_fused(self.H, self.C)
         # device addresses, looked up once: the per-token loops only do integer arithmetic
         for n in ("emb", "w_ih", "w_hh", "b_ih", "b_hh", "conv_wT", "conv_b", "lin_w", "fc_w",
                   "fc_b"):
@@ -76,6 +104,55 @@ def _attn_fwd(lib, w, ws, eh, bcast, hx, ax_prev, sx, ax, B, T, sp, logits=None,
                                                 logits, logit_stride, _a(logp), _a(argmax),
                                                 history, hist_stride, hist_col, end_count,
                                                 end_tok, done, _a(lens), _a(ws), ws.numel(), sp))
+
+
+def fc_workspace(lib, R, C, dev):
+    """zeroed scratch of sb_s2s_fc_rows / _logp for R rows (tile partials, log-sum-exp, tickets)"""
+    n = ctypes.c_size_t(0)
+    _lib.check(lib.sb_s2s_fc_workspace_size(R, C, ctypes.byref(n)), "s2s fc workspace")
+    return torch.zeros(n.value, dtype=torch.uint8, device=dev)
+
+
+def _fc_rows(lib, w, ws, hx, sx, R, sp, logits=None, group=0, ld0=0, ld1=0, argmax=None,
+             history=None, hist_stride=0, hist_col=0, end_count=None, end_tok=-1, done=None):
+    """logits of R rows o = hx + sx over many CTAs; row r at logits + (r % group) * ld0 +
+    (r / group) * ld1 (default: dense (R, C)), with the row reductions of the same launch."""
+    from .. import ops
+    group = group or R
+    ld0 = ld0 or w.C
+    ops._launch("s2s_fc_rows", 2.0 * R * w.C * w.H,
+                lambda: lib.sb_s2s_fc_rows(_a(hx), _a(sx), w.p_fc_w, w.p_fc_b, R, w.H, w.C,
+                                           _a(logits), group, ld0, ld1, _a(argmax), _a(history),
+                                           hist_stride, hist_col, _a(end_count), end_tok, _a(done),
+                                           _a(ws), ws.numel(), sp))
+
+
+def _fc_logp(lib, w, ws, logits, logp, R, sp, done=None):
+    """logp (R, C) = logits (dense (R, C)) - the log-sum-exp the last _fc_rows left in ws"""
+    from .. import ops
+    ops._launch("s2s_fc_logp", 0.0,
+                lambda: lib.sb_s2s_fc_logp(_a(logits), R, w.C, 0, _a(logp), R, w.C, _a(done),
+                                           _a(ws), ws.numel(), sp))
+
+
+def _dout_gemm(dl, fc_w, d_o):
+    """d_o (R, H) = dl (R, C) @ fc_w (C, H) for C past sb_s2s_dout: 3-pass split-bf16 on the wgmma
+    GEMM (hi*hi + hi*lo + lo*hi, relative error ~2^-16, as ops.gemm_split), fc_w read as [K][N]."""
+    from .. import ops
+    R, C = dl.shape
+    H = fc_w.shape[1]
+    Cp, Hp = (C + 7) // 8 * 8, (H + 7) // 8 * 8
+    a_hi, a_lo = ops._split_bf16(dl, Cp)
+    wp = fc_w
+    if Cp != C:
+        wp = torch.zeros(Cp, H, dtype=torch.float32, device=dl.device)
+        wp[:C] = fc_w
+    b_hi, b_lo = ops._split_bf16(wp, Hp)
+    out = torch.empty(R, Hp, dtype=torch.float32, device=dl.device)
+    ops.gemm_bf16_tn(a_hi, b_hi, out=out, b_mn=True)
+    ops.gemm_bf16_tn(a_hi, b_lo, out=out, accumulate=True, b_mn=True)
+    ops.gemm_bf16_tn(a_lo, b_hi, out=out, accumulate=True, b_mn=True)
+    d_o.copy_(out[:, :H])
 
 
 def attn_lens(lens, B, T, dev):
@@ -129,6 +206,11 @@ class DecodeFunction(torch.autograd.Function):
         p_gt = gates_all.data_ptr() if need else None
         p_tok, p_logits = tok.data_ptr(), logits.data_ptr()
         p_amax = amax.data_ptr() if sampling else None
+        # large vocabularies: the attention without fc, the logits over many CTAs - per step when
+        # the arg-max feeds the next step, else once over all steps*B rows after the loop
+        fc_ws = None
+        if not w.fused and steps > 0:
+            fc_ws = fc_workspace(lib, B if sampling else steps * B, w.C, dev)
         for u in range(steps):
             if u > 0 and sample_flags[u]:
                 if need:
@@ -139,9 +221,22 @@ class DecodeFunction(torch.autograd.Function):
             _cell_fwd(lib, w, tk, ts, p_sx + (u - 1) * BH if u > 0 else None, p_hx + u * BH,
                       p_hx + (u + 1) * BH, p_ix + u * BH if need else None,
                       p_gt + 4 * u * BH if need else None, None, B, sp)
-            _attn_fwd(lib, w, ws, ehc, 0, p_hx + (u + 1) * BH, p_ax + (u - 1) * BT if u > 0 else None,
-                      p_sx + u * BH, p_ax + u * BT, B, T, sp, logits=p_logits + 4 * u * w.C,
-                      logit_stride=steps * w.C, argmax=p_amax, lens=lens)
+            if w.fused:
+                _attn_fwd(lib, w, ws, ehc, 0, p_hx + (u + 1) * BH,
+                          p_ax + (u - 1) * BT if u > 0 else None, p_sx + u * BH, p_ax + u * BT, B,
+                          T, sp, logits=p_logits + 4 * u * w.C, logit_stride=steps * w.C,
+                          argmax=p_amax, lens=lens)
+                continue
+            _attn_fwd(lib, w, ws, ehc, 0, p_hx + (u + 1) * BH,
+                      p_ax + (u - 1) * BT if u > 0 else None, p_sx + u * BH, p_ax + u * BT, B, T,
+                      sp, with_fc=False, lens=lens)
+            if sampling:
+                _fc_rows(lib, w, fc_ws, p_hx + (u + 1) * BH, p_sx + u * BH, B, sp,
+                         logits=p_logits + 4 * u * w.C, ld0=steps * w.C, argmax=p_amax)
+        if not w.fused and not sampling and steps > 0:
+            # row r = u*B + b of (hx_all[1:], sx_all) -> logits[b, u]
+            _fc_rows(lib, w, fc_ws, p_hx + BH, p_sx, steps * B, sp, logits=p_logits, group=B,
+                     ld0=steps * w.C, ld1=w.C)
         ctx.w = w
         ctx.lens = lens
         ctx.saved = (ehc, hx_all, sx_all, ax_all, ix_all, gates_all, used)
@@ -182,9 +277,13 @@ class DecodeFunction(torch.autograd.Function):
         sp = _lib.stream_ptr()
         ws = attn_workspace(lib, B, T, H, dev)
         w_ihT, w_hhT = w.w_ih.t().contiguous(), w.w_hh.t().contiguous()
-        ops._launch("s2s_dout", 0.0, lambda: lib.sb_s2s_dout(
-            dl.data_ptr(), w.fc_w.data_ptr(), hx_all[1:].data_ptr(), sx_all.data_ptr(),
-            d_o.data_ptr(), o_all.data_ptr(), steps * B, C, H, sp))
+        if dout_fits(C):
+            ops._launch("s2s_dout", 0.0, lambda: lib.sb_s2s_dout(
+                dl.data_ptr(), w.fc_w.data_ptr(), hx_all[1:].data_ptr(), sx_all.data_ptr(),
+                d_o.data_ptr(), o_all.data_ptr(), steps * B, C, H, sp))
+        else:
+            torch.add(hx_all[1:], sx_all, out=o_all)
+            _dout_gemm(dl.view(steps * B, C), w.fc_w, d_o.view(steps * B, H))
         BH, BT = 4 * B * H, 4 * B * T
         p_eh, p_hx, p_ax = ehc.data_ptr(), hx_all.data_ptr(), ax_all.data_ptr()
         p_gt, p_do, p_dix = gates_all.data_ptr(), d_o.data_ptr(), d_ix.data_ptr()
@@ -280,8 +379,15 @@ def decode_step(m, eh, y, state, softmax, lens=None):
     ws = attn_workspace(lib, B, T, H, dev)
     ld = attn_lens(lens, B, T, dev)
     _cell_fwd(lib, w, tok.data_ptr(), 1, sx_prev, hx_prev, hx, None, None, None, B, sp)
-    _attn_fwd(lib, w, ws, ehc, 0, hx, ax_prev, sx, ax, B, T, sp, logits=out.data_ptr(),
-              logit_stride=w.C, logp=logp, lens=ld)
+    if w.fused:
+        _attn_fwd(lib, w, ws, ehc, 0, hx, ax_prev, sx, ax, B, T, sp, logits=out.data_ptr(),
+                  logit_stride=w.C, logp=logp, lens=ld)
+    else:
+        _attn_fwd(lib, w, ws, ehc, 0, hx, ax_prev, sx, ax, B, T, sp, with_fc=False, lens=ld)
+        fc_ws = fc_workspace(lib, B, w.C, dev)
+        _fc_rows(lib, w, fc_ws, hx, sx, B, sp, logits=out)
+        if softmax:
+            _fc_logp(lib, w, fc_ws, out, logp, B, sp)
     return (logp if softmax else out), (hx, ax, sx.unsqueeze(1))
 
 
@@ -306,14 +412,22 @@ def greedy(m, eh, start, end_tok, max_len, lens=None):
     ws = attn_workspace(lib, B, T, H, dev)
     ld = attn_lens(lens, B, T, dev)
     from .. import ops
+    fc_ws = None if w.fused else fc_workspace(lib, B, w.C, dev)
     for e in range(max_len):
         cur, prv = e & 1, (e & 1) ^ 1
         _cell_fwd(lib, w, hist.data_ptr() + 4 * e, max_len + 1, sx[prv] if e > 0 else None,
                   hx[prv], hx[cur], None, None, done.data_ptr(), B, sp)
-        _attn_fwd(lib, w, ws, ehc, 0, hx[cur], ax[prv] if e > 0 else None, sx[cur], ax[cur], B, T, sp,
-                  history=hist.data_ptr(), hist_stride=max_len + 1, hist_col=e + 1,
-                  end_count=ctl.data_ptr() + 4 * e, end_tok=int(end_tok), done=done.data_ptr(),
-                  lens=ld)
+        if w.fused:
+            _attn_fwd(lib, w, ws, ehc, 0, hx[cur], ax[prv] if e > 0 else None, sx[cur], ax[cur], B,
+                      T, sp, history=hist.data_ptr(), hist_stride=max_len + 1, hist_col=e + 1,
+                      end_count=ctl.data_ptr() + 4 * e, end_tok=int(end_tok),
+                      done=done.data_ptr(), lens=ld)
+        else:
+            _attn_fwd(lib, w, ws, ehc, 0, hx[cur], ax[prv] if e > 0 else None, sx[cur], ax[cur], B,
+                      T, sp, done=done.data_ptr(), with_fc=False, lens=ld)
+            _fc_rows(lib, w, fc_ws, hx[cur], sx[cur], B, sp, history=hist.data_ptr(),
+                     hist_stride=max_len + 1, hist_col=e + 1, end_count=ctl.data_ptr() + 4 * e,
+                     end_tok=int(end_tok), done=done.data_ptr())
         ops._launch("s2s_check_done", 0.0,
                     lambda: lib.sb_s2s_check_done(ctl.data_ptr() + 4 * e, B, done.data_ptr(),
                                                   nsteps.data_ptr(), e + 1, sp))
@@ -352,16 +466,34 @@ def beam_search(m, eh, start_tok, end_tok, beam_size, max_len):
                                     int(start_tok), sp), "beam init")
     # the `done` word of the state struct doubles as the no-op flag of the step kernels
     done_ptr = state.data_ptr() + _beam_done_offset()
+    fc_ws = None if w.fused else fc_workspace(lib, K, C, dev)
+    split = not beam_select_fits(K, C)
+    if split:
+        _lib.check(lib.sb_s2s_beam_split_workspace_size(K, C, ctypes.byref(nbytes)),
+                   "beam split workspace")
+        sel_ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
     # buffers: [0] = state entering the step (gathered), [1] = state produced by the step
     for e in range(max_len):
         _cell_fwd(lib, w, tok.data_ptr(), 1, sx[0] if e > 0 else None, hx[0], hx[1], None, None,
                   done_ptr, K, sp)
-        _attn_fwd(lib, w, ws, ehc, 1, hx[1], ax[0] if e > 0 else None, sx[1], ax[1], K, T, sp,
-                  logp=logp, done=done_ptr)
-        ops._launch("s2s_beam_select", 0.0, lambda: lib.sb_s2s_beam_select(
-            logp.data_ptr(), state.data_ptr(), c_scores.data_ptr(), nodes.data_ptr(),
-            parent.data_ptr(), tok.data_ptr(), out_tokens.data_ptr(), K, C, int(end_tok), e,
-            max_len, node_cap, c_cap, sp))
+        if w.fused:
+            _attn_fwd(lib, w, ws, ehc, 1, hx[1], ax[0] if e > 0 else None, sx[1], ax[1], K, T, sp,
+                      logp=logp, done=done_ptr)
+        else:
+            _attn_fwd(lib, w, ws, ehc, 1, hx[1], ax[0] if e > 0 else None, sx[1], ax[1], K, T, sp,
+                      done=done_ptr, with_fc=False)
+            _fc_rows(lib, w, fc_ws, hx[1], sx[1], K, sp, logits=logp, done=done_ptr)
+            _fc_logp(lib, w, fc_ws, logp, logp, K, sp, done=done_ptr)
+        if split:
+            ops._launch("s2s_beam_select_split", 0.0, lambda: lib.sb_s2s_beam_select_split(
+                logp.data_ptr(), state.data_ptr(), c_scores.data_ptr(), nodes.data_ptr(),
+                parent.data_ptr(), tok.data_ptr(), out_tokens.data_ptr(), K, C, int(end_tok), e,
+                max_len, node_cap, c_cap, sel_ws.data_ptr(), sel_ws.numel(), sp))
+        else:
+            ops._launch("s2s_beam_select", 0.0, lambda: lib.sb_s2s_beam_select(
+                logp.data_ptr(), state.data_ptr(), c_scores.data_ptr(), nodes.data_ptr(),
+                parent.data_ptr(), tok.data_ptr(), out_tokens.data_ptr(), K, C, int(end_tok), e,
+                max_len, node_cap, c_cap, sp))
         ops._launch("s2s_beam_gather", 0.0, lambda: lib.sb_s2s_beam_gather(
             hx[1].data_ptr(), sx[1].data_ptr(), ax[1].data_ptr(), hx[0].data_ptr(),
             sx[0].data_ptr(), ax[0].data_ptr(), parent.data_ptr(), state.data_ptr(), K, H, T, sp))

@@ -102,4 +102,19 @@ for gemm_flags, want in ((0, ("tma", "tma_reduce", "regs")), (2, ("regs", "regs"
     assert gemm_kernel == "c2_128x256", gemm_kernel
     assert tuple(got) == want, (gemm_flags, got)
 print("2-CTA GEMM ok")
+# the attention model at a large vocabulary (C = 9000 > 7 H): the many-CTA projection over
+# several class tiles and row blocks, its log-softmax, the GEMM backward of the projection, and the
+# split beam selection (beam 8 x 9000 candidates: several tiles)
+cfg_v = {"dropout": 0.0, "encoder": {"conv": [[8, 5, 8, 2]],
+                                     "rnn": {"dim": 64, "bidirectional": True, "layers": 1}},
+         "decoder": {"embedding_dim": 64, "layers": 1, "sample_prob": 0.5}}
+sv = Seq2Seq(80, 9001, cfg_v).cuda()
+lab3 = [[9000] + np.random.randint(0, 8999, 7 + i).tolist() + [8999] for i in range(5)]
+l11 = sv.loss((inputs, lab3)); l11.backward()              # scheduled sampling: per-step projection
+sv.scheduled_sampling = False
+l12 = sv.loss((inputs, lab3)); l12.backward()              # one projection over all rows
+sv.set_eval()
+print("seq2seq C=9000 ok", l11.item(), l12.item(),
+      [len(h) for h in sv.infer((inputs, lab3), max_len=6)],
+      sv.beam_search(([inputs[0]], [lab3[0]]), beam_size=8, max_len=5))
 torch.cuda.synchronize()
