@@ -53,7 +53,6 @@ struct GruFwdParams {
   const float* bhh;    // [ndir][3H]
   float* y;            // [T*Bp][ndir*H]   h_t fp32
   bf16* xn;            // [T*Bp][ndir*H]   h_t bf16 (operand of the next projection)
-  bf16* xnT;           // [ndir*H][(T+2)*Bp] h_t bf16 transposed, column (t+1)*Bp+b ; may be null
   float* gates;        // [T*Bp][ndir][4][H] saved r,z,n,hn for backward ; may be null
   unsigned int* barrier;  // [ndir] zero-initialised counters
   unsigned long long* dbg;  // optional timeline (CTA 0): [step][16] globaltimer stamps, or null
@@ -222,28 +221,295 @@ SB_DEVINL float fast_tanh(float x) {
   return 1.0f - __fdividef(2.0f, __expf(2.0f * xc) + 1.0f);
 }
 
+// ---- vectors of UPT = 1, 2, 4 or 8 consecutive hidden units of one thread ----------------------
 // One-touch data (gi, saved gates, dy, fp32 state, GEMM operands written for later kernels) uses
 // the streaming cache policy (.cs) so that it does not evict the latency-critical bf16 exchange
 // buffers, which every CTA re-reads from L2 each step.
-SB_DEVINL void ld8(const float* p, float (&v)[8]) {
-  const float4 a = __ldcs(reinterpret_cast<const float4*>(p));
-  const float4 b = __ldcs(reinterpret_cast<const float4*>(p) + 1);
-  v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+template <int UPT>
+SB_DEVINL void ld_stream(const float* p, float (&v)[UPT]) {
+  if constexpr (UPT >= 4) {
+#pragma unroll
+    for (int i = 0; i < UPT; i += 4) {
+      const float4 a = __ldcs(reinterpret_cast<const float4*>(p + i));
+      v[i] = a.x; v[i + 1] = a.y; v[i + 2] = a.z; v[i + 3] = a.w;
+    }
+  } else if constexpr (UPT == 2) {
+    const float2 a = __ldcs(reinterpret_cast<const float2*>(p));
+    v[0] = a.x; v[1] = a.y;
+  } else {
+    v[0] = __ldcs(p);
+  }
 }
-SB_DEVINL void st8(float* p, const float (&v)[8]) {
-  __stcs(reinterpret_cast<float4*>(p), make_float4(v[0], v[1], v[2], v[3]));
-  __stcs(reinterpret_cast<float4*>(p) + 1, make_float4(v[4], v[5], v[6], v[7]));
+template <int UPT>
+SB_DEVINL void st_stream(float* p, const float (&v)[UPT]) {
+  if constexpr (UPT >= 4) {
+#pragma unroll
+    for (int i = 0; i < UPT; i += 4)
+      __stcs(reinterpret_cast<float4*>(p + i), make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]));
+  } else if constexpr (UPT == 2) {
+    __stcs(reinterpret_cast<float2*>(p), make_float2(v[0], v[1]));
+  } else {
+    __stcs(p, v[0]);
+  }
 }
-SB_DEVINL void st_stream_u4(void* p, uint4 v) { __stcs(reinterpret_cast<uint4*>(p), v); }
-SB_DEVINL void st_stream_bf16(bf16* p, float v) {
-  const unsigned short u = __bfloat16_as_ushort(__float2bfloat16_rn(v));
-  asm volatile("st.global.cs.u16 [%0], %1;" ::"l"(p), "h"(u) : "memory");
+// bf16 vectors are rounded once (to_bf16) and kept packed in pairs until stored: the backward
+// stores each of its gradients twice, once on each side of the grid barrier, and packed halves
+// the registers they hold across it.  UPT = 1 uses the low half of w[0].
+template <int UPT>
+struct Bf16Vec {
+  uint32_t w[(UPT + 1) / 2];
+};
+template <int UPT>
+SB_DEVINL Bf16Vec<UPT> to_bf16(const float (&v)[UPT]) {
+  Bf16Vec<UPT> b;
+  if constexpr (UPT == 1) {
+    b.w[0] = __bfloat16_as_ushort(__float2bfloat16_rn(v[0]));
+  } else {
+#pragma unroll
+    for (int i = 0; i < UPT / 2; ++i) b.w[i] = pack_bf16x2(v[2 * i], v[2 * i + 1]);
+  }
+  return b;
 }
-SB_DEVINL uint4 pack8(const float (&v)[8]) {
-  uint4 r;
-  r.x = pack_bf16x2(v[0], v[1]); r.y = pack_bf16x2(v[2], v[3]);
-  r.z = pack_bf16x2(v[4], v[5]); r.w = pack_bf16x2(v[6], v[7]);
-  return r;
+// the default policy (the exchange rows other CTAs read next) and the streaming one
+template <int UPT>
+SB_DEVINL void st_bf16(bf16* p, const Bf16Vec<UPT>& b) {
+  if constexpr (UPT == 8) *reinterpret_cast<uint4*>(p) = make_uint4(b.w[0], b.w[1], b.w[2], b.w[3]);
+  else if constexpr (UPT == 4) *reinterpret_cast<uint2*>(p) = make_uint2(b.w[0], b.w[1]);
+  else if constexpr (UPT == 2) *reinterpret_cast<uint32_t*>(p) = b.w[0];
+  else *reinterpret_cast<unsigned short*>(p) = (unsigned short)b.w[0];
+}
+template <int UPT>
+SB_DEVINL void st_stream_bf16(bf16* p, const Bf16Vec<UPT>& b) {
+  if constexpr (UPT == 8) {
+    __stcs(reinterpret_cast<uint4*>(p), make_uint4(b.w[0], b.w[1], b.w[2], b.w[3]));
+  } else if constexpr (UPT == 4) {
+    __stcs(reinterpret_cast<uint2*>(p), make_uint2(b.w[0], b.w[1]));
+  } else if constexpr (UPT == 2) {
+    __stcs(reinterpret_cast<unsigned int*>(p), b.w[0]);
+  } else {
+    asm volatile("st.global.cs.u16 [%0], %1;" ::"l"(p), "h"((unsigned short)b.w[0]) : "memory");
+  }
+}
+
+// ---- the GRU cell, shared by every recurrence kernel ------------------------------------------
+// Four per-gate values of UPT units: the saved activations r, z, n, hn (= W_hn h_{t-1} + b_hn),
+// their gradients dr, dz, dn, dn*r (the pre-activation gradients of the r, z and n gates, and of
+// hn), or the bias partial sums of those.
+template <int UPT>
+struct GruGates {
+  float r[UPT], z[UPT], n[UPT], hn[UPT];
+};
+template <int UPT>
+struct GruGatesBf16 {
+  Bf16Vec<UPT> r, z, n, hn;
+};
+
+// Forward step of one batch row: gi = the input projections (b_ih included), acc = the finished
+// recurrent product W_hh h_{t-1}, bias = b_hh; h holds h_{t-1} and receives h_t.
+template <int UPT>
+SB_DEVINL void gru_cell_fwd(const float (&gi)[3][UPT], const float (&acc)[3][UPT],
+                            const float (&bias)[3][UPT], float (&h)[UPT], GruGates<UPT>& g) {
+#pragma unroll
+  for (int jj = 0; jj < UPT; ++jj) {
+    g.r[jj] = fast_sigmoid(gi[0][jj] + acc[0][jj] + bias[0][jj]);
+    g.z[jj] = fast_sigmoid(gi[1][jj] + acc[1][jj] + bias[1][jj]);
+    g.hn[jj] = acc[2][jj] + bias[2][jj];
+    g.n[jj] = fast_tanh(gi[2][jj] + g.r[jj] * g.hn[jj]);
+    h[jj] = (1.f - g.z[jj]) * g.n[jj] + g.z[jj] * h[jj];
+  }
+}
+
+// Backward step of one batch row: dh = dL/dh_t from the layer output, dh_rec = its recurrent part
+// (on return: the direct path h_{t-1} -> h_t; the W_hh path is added next step), s = the saved
+// gates, hp = h_{t-1}.  Adds the pre-activation gradients to the bias sums db and returns them in
+// bf16, the form every kernel stores.
+template <int UPT>
+SB_DEVINL GruGatesBf16<UPT> gru_cell_bwd(const float (&dh)[UPT], float (&dh_rec)[UPT],
+                                         const GruGates<UPT>& s, const float (&hp)[UPT],
+                                         GruGates<UPT>& db) {
+  GruGates<UPT> d;
+#pragma unroll
+  for (int jj = 0; jj < UPT; ++jj) {
+    const float g = dh[jj] + dh_rec[jj];
+    d.n[jj] = g * (1.f - s.z[jj]) * (1.f - s.n[jj] * s.n[jj]);
+    d.z[jj] = g * (hp[jj] - s.n[jj]) * s.z[jj] * (1.f - s.z[jj]);
+    d.r[jj] = d.n[jj] * s.hn[jj] * s.r[jj] * (1.f - s.r[jj]);
+    d.hn[jj] = d.n[jj] * s.r[jj];
+    dh_rec[jj] = g * s.z[jj];
+    db.r[jj] += d.r[jj];
+    db.z[jj] += d.z[jj];
+    db.n[jj] += d.n[jj];
+    db.hn[jj] += d.hn[jj];
+  }
+  return {to_bf16(d.r), to_bf16(d.z), to_bf16(d.n), to_bf16(d.hn)};
+}
+
+// ---- per-step epilogue pieces -----------------------------------------------------------------
+// This step's input projections of UPT units from ju of batch row `row`: they do not depend on
+// the recurrence, so every kernel fetches them before it waits for the product.
+template <int UPT>
+SB_DEVINL void gru_load_gi(const GruFwdParams& p, int t, int row, int dir, int ju,
+                           float (&gi)[3][UPT]) {
+  const int H = p.H;
+  const float* g = p.gi + ((long long)t * p.Bp + row) * (p.ndir * 3 * H) + dir * 3 * H + ju;
+#pragma unroll
+  for (int gg = 0; gg < 3; ++gg) ld_stream<UPT>(g + gg * H, gi[gg]);
+}
+
+// b_hh of the thread's units from shared memory (`pitch` floats per gate)
+template <int UPT>
+SB_DEVINL void gru_load_bias(const float* src, int pitch, float (&bias)[3][UPT]) {
+#pragma unroll
+  for (int g = 0; g < 3; ++g)
+#pragma unroll
+    for (int jj = 0; jj < UPT; ++jj) bias[g][jj] = src[g * pitch + jj];
+}
+
+// The saved activations of backward step t (forward time index): gates, dy and h_{t-1} (zero where
+// the direction's sequence starts).  Independent of the recurrence: fetched first.
+template <int UPT>
+SB_DEVINL void gru_load_saved(const GruBwdParams& p, int t, int row, int dir, int ju,
+                              GruGates<UPT>& s, float (&dh)[UPT], float (&hp)[UPT]) {
+  const int H = p.H, Bp = p.Bp, D = p.ndir * H;
+  const long long m = (long long)t * Bp + row;
+  const float* go = p.gates + ((m * p.ndir + dir) * 4) * H + ju;
+  ld_stream<UPT>(go, s.r);
+  ld_stream<UPT>(go + H, s.z);
+  ld_stream<UPT>(go + 2 * H, s.n);
+  ld_stream<UPT>(go + 3 * H, s.hn);
+  ld_stream<UPT>(p.dy + m * D + dir * H + ju, dh);
+  const int tp = dir == 0 ? t - 1 : t + 1;
+  if (dir == 0 ? (t > 0) : (t < p.T - 1)) {
+    ld_stream<UPT>(p.y + ((long long)tp * Bp + row) * D + dir * H + ju, hp);
+  } else {
+#pragma unroll
+    for (int jj = 0; jj < UPT; ++jj) hp[jj] = 0.f;
+  }
+}
+
+// Critical path of the backward: the exchange row [dr | dz | dn*r] every CTA gathers next step
+template <int UPT>
+SB_DEVINL void gru_store_xchg(const GruBwdParams& p, int step, int row, int dir, int ju,
+                              const GruGatesBf16<UPT>& d) {
+  const int H = p.H;
+  bf16* x = p.xchg + ((long long)(dir * 2 + (step & 1)) * p.Bp + row) * (3 * H) + ju;
+  st_bf16<UPT>(x, d.r);
+  st_bf16<UPT>(x + H, d.z);
+  st_bf16<UPT>(x + 2 * H, d.hn);
+}
+
+// After the CTA's bf16 rows of the step are stored (wrote: by this thread): order them before the
+// other CTAs' TMA reads (generic -> async proxy), then one release arrive per CTA on the
+// direction's grid barrier once every epilogue thread is done.  skew_probe: the K-split forward
+// kernels record the arrive of step 20 per CTA (tools/gru_timeline.py).
+// Developer knob (sb_debug_gru_flags) 1 drops the fence: timing only, results become wrong.
+template <class Params>
+SB_DEVINL void gru_publish(const Params& p, unsigned int* ctr, int step, bool wrote,
+                           bool skew_probe) {
+  const bool lead = threadIdx.x == 0;
+  if (lead) GRU_STAMP(5);
+  if (wrote && !(p.ablate & 1)) fence_proxy_async_global();
+  if (lead) GRU_STAMP(6);
+  epi_barrier();
+  if (lead) {
+    GRU_STAMP(7);
+    if (skew_probe && p.dbg && step == 20) p.dbg[1024 + blockIdx.x] = gtime();
+    grid_arrive(ctr);   // release: cumulative over the CTA's writes ordered by bar.sync
+    GRU_STAMP(9);
+  }
+}
+
+// Off the critical path: the forward's fp32 h_t and saved gates, the backward's operands of the
+// dX / dW GEMMs.  Developer knob 2 skips them (timing only).
+template <int UPT>
+SB_DEVINL void gru_store_fwd(const GruFwdParams& p, long long m, int dir, int ju,
+                             const float (&h)[UPT], const GruGates<UPT>& g) {
+  if (p.ablate & 2) return;
+  const int H = p.H;
+  st_stream<UPT>(p.y + m * (p.ndir * H) + dir * H + ju, h);
+  if (p.gates) {
+    float* go = p.gates + ((m * p.ndir + dir) * 4) * H + ju;
+    st_stream<UPT>(go, g.r);
+    st_stream<UPT>(go + H, g.z);
+    st_stream<UPT>(go + 2 * H, g.n);
+    st_stream<UPT>(go + 3 * H, g.hn);
+  }
+}
+template <int UPT>
+SB_DEVINL void gru_store_bwd(const GruBwdParams& p, long long m, int dir, int ju,
+                             const GruGatesBf16<UPT>& d) {
+  if (p.ablate & 2) return;
+  const int H = p.H, K3 = 3 * H;
+  bf16* o = p.dgi + m * (p.ndir * K3) + dir * K3 + ju;
+  st_stream_bf16<UPT>(o, d.r);
+  st_stream_bf16<UPT>(o + H, d.z);
+  st_stream_bf16<UPT>(o + 2 * H, d.n);
+  st_stream_bf16<UPT>(p.dghn + m * (p.ndir * H) + dir * H + ju, d.hn);
+}
+
+// ---- prologue pieces --------------------------------------------------------------------------
+SB_DEVINL void smem_zero(uint8_t* base, int bytes) {
+  for (int k = threadIdx.x; k < bytes / 16; k += GRU_THREADS)
+    reinterpret_cast<uint4*>(base)[k] = make_uint4(0, 0, 0, 0);
+}
+
+// Forward weight layout: shared-memory row r <- row row_of(r) of one direction's W_hh ([3H][H],
+// the row of gate g and unit u is g * H + u), columns k0 .. k0 + ncols, into K-major SWIZZLE_128B
+// chunks of 64 columns (wchunk bytes each).  Pieces past ncols keep the zeroed contents.
+template <class RowOf>
+SB_DEVINL void stage_w_rows(uint8_t* wtile, int wchunk, const bf16* w, int H, int nrows, int k0,
+                            int ncols, RowOf row_of) {
+  const int pieces_per_row = (ncols + 63) / 64 * 8;
+  for (int k = threadIdx.x; k < nrows * pieces_per_row; k += GRU_THREADS) {
+    const int r = k / pieces_per_row, pc = k % pieces_per_row;
+    if (pc * 8 < ncols) {
+      const uint4 v =
+          *reinterpret_cast<const uint4*>(w + (long long)row_of(r) * H + k0 + pc * 8);
+      *reinterpret_cast<uint4*>(wtile + (pc >> 3) * wchunk + sw128_offset(r, pc & 7)) = v;
+    }
+  }
+}
+
+// Backward weight layout: rows = the NU units u0.. of one direction's W_hh^T, K = rows k0 .. k0 + nk
+// of W_hh.  W_hh is read as stored (2 * NU contiguous bytes per k) and transposed on the way into
+// K-major SWIZZLE_128B chunks of NU rows x 64.
+template <int NU>
+SB_DEVINL void stage_w_cols(uint8_t* wtile, const bf16* w, int H, int k0, int nk, int u0) {
+  constexpr int PIECES = NU / 8;
+  for (int k = threadIdx.x; k < nk * PIECES; k += GRU_THREADS) {
+    const int kl = k / PIECES, piece = k % PIECES;
+    const uint4 v = *reinterpret_cast<const uint4*>(w + (long long)(k0 + kl) * H + u0 + piece * 8);
+    const unsigned short* e = reinterpret_cast<const unsigned short*>(&v);
+    uint8_t* chunk = wtile + (kl >> 6) * (NU * 128) + (kl & 7) * 2;
+#pragma unroll
+    for (int q = 0; q < 8; ++q)
+      *reinterpret_cast<unsigned short*>(
+          chunk + sw128_offset((uint32_t)(piece * 8 + q), (uint32_t)((kl & 63) >> 3))) = e[q];
+  }
+}
+
+// Thread 0 initialises the kernel's mbarriers (init) and prefetches the tensor-map descriptors
+// (tw may be null); then the CTA syncs, and with `cluster` the cluster too, so that no peer
+// multicasts into or signals a barrier before it is initialised.
+template <class Init>
+SB_DEVINL void gru_init_barriers(const CUtensorMap* tm, const CUtensorMap* tw, bool cluster,
+                                 Init init) {
+  if (threadIdx.x == 0) {
+    init();
+    mbar_fence_init();
+    tma_prefetch_desc(tm);
+    if (tw) tma_prefetch_desc(tw);
+  }
+  fence_proxy_async_smem();
+  __syncthreads();
+  if (cluster) cluster_sync_all();
+}
+// the full / empty pairs of a gather ring whose slots every CTA of the cluster releases
+SB_DEVINL void init_ring_bars(uint64_t* full, uint64_t* empty, uint32_t csize) {
+  for (int i = 0; i < GRU_MAX_RING; ++i) {
+    mbar_init(&full[i], 1);
+    mbar_init(&empty[i], csize);
+  }
 }
 
 // =============================================================================================
@@ -265,43 +531,19 @@ gru_fwd_kernel(const __grid_constant__ CUtensorMap tm_d0, const __grid_constant_
   const GruSmem s = carve(smem_raw, ring_bytes, wbytes);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int D = p.ndir * H;
-  const long long ldT = (long long)(T + 2) * Bp;
   const CUtensorMap* tm = dir == 0 ? &tm_d0 : &tm_d1;
   const uint32_t crank = cluster_rank(), csize = cluster_size();
 
   // ---- one-time setup: zero ring + weight region, stage the 48 weight rows, barriers ----
-  for (int k = tid; k < (ring_bytes + wbytes) / 16; k += GRU_THREADS)
-    reinterpret_cast<uint4*>(s.ring)[k] = make_uint4(0, 0, 0, 0);
+  smem_zero(s.ring, ring_bytes + wbytes);
   __syncthreads();
-  {
-    const int pieces_per_row = nchunks * 8;
-    for (int k = tid; k < 48 * pieces_per_row; k += GRU_THREADS) {
-      const int r = k / pieces_per_row, pc = k % pieces_per_row;
-      const int g = r / GRU_HC, jj = r % GRU_HC;
-      const int col = pc * 8;
-      if (col < H) {
-        const uint4 v = *reinterpret_cast<const uint4*>(
-            p.whh + ((long long)dir * 3 * H + g * H + j0 + jj) * H + col);
-        *reinterpret_cast<uint4*>(s.wtile + (pc >> 3) * WCHUNK + sw128_offset(r, pc & 7)) = v;
-      }
-    }
-    if (tid < 48) {
-      const int g = tid / GRU_HC, jj = tid % GRU_HC;
-      s.scratch[tid] = p.bhh[dir * 3 * H + g * H + j0 + jj];
-    }
-  }
-  if (tid == 0) {
-    for (int i = 0; i < GRU_MAX_RING; ++i) {
-      mbar_init(&s.full[i], 1);
-      mbar_init(&s.empty[i], csize);
-    }
+  stage_w_rows(s.wtile, WCHUNK, p.whh + (long long)dir * 3 * H * H, H, 48, 0, H,
+               [=](int r) { return (r / GRU_HC) * H + j0 + r % GRU_HC; });
+  if (tid < 48) s.scratch[tid] = p.bhh[dir * 3 * H + (tid / GRU_HC) * H + j0 + tid % GRU_HC];
+  gru_init_barriers(tm, nullptr, true, [=] {
+    init_ring_bars(s.full, s.empty, csize);
     mbar_init(s.accfull, 128);
-    mbar_fence_init();
-    tma_prefetch_desc(tm);
-  }
-  fence_proxy_async_smem();
-  __syncthreads();
-  cluster_sync_all();   // peers' barriers are initialised before anyone multicasts into them
+  });
   unsigned int* ctr = p.barrier + dir * 32;   // one L2 line per direction
 
   if (warp == GRU_TMA_WARP) {
@@ -319,9 +561,16 @@ gru_fwd_kernel(const __grid_constant__ CUtensorMap tm_d0, const __grid_constant_
     }
   } else if (warp >= GRU_MMA_WARP) {
     // ===================== MMA warpgroup =====================
+    // accbuf is made opaque to the compiler, which otherwise recomputes it from the carve before
+    // each store of the parked product, on the critical path of every step.  Measured with and
+    // without this line, same source otherwise (H100 80GB HBM3 at 700 W, both directions, us
+    // per step): H = 1024 at 64 rows 11.2 with, 11.6 without; at 8 rows 3.3 with, 3.7 without;
+    // H = 384 at 32 rows 4.0 with, 4.4 without.
+    GruSmem sm = s;
+    asm volatile("" : "+l"(sm.accbuf));
     for (int step = 1; step < T; ++step) {
-      if (Bp > 64) mma_consume<48, true>(s, nchunks, WCHUNK, Bp, p.ring, p.gc, step - 1, csize);
-      else mma_consume<48, false>(s, nchunks, WCHUNK, Bp, p.ring, p.gc, step - 1, csize);
+      if (Bp > 64) mma_consume<48, true>(sm, nchunks, WCHUNK, Bp, p.ring, p.gc, step - 1, csize);
+      else mma_consume<48, false>(sm, nchunks, WCHUNK, Bp, p.ring, p.gc, step - 1, csize);
       if (tid == GRU_MMA_WARP * 32) GRU_STAMP(2);
     }
   } else {
@@ -329,24 +578,14 @@ gru_fwd_kernel(const __grid_constant__ CUtensorMap tm_d0, const __grid_constant_
     const int row = (warp & 3) * 32 + lane;      // batch row
     const int uh = warp >> 2;                    // which 8 of the CTA's 16 units
     const int ju = j0 + uh * GRU_UPT;
-    float hprev[GRU_UPT];
-#pragma unroll
-    for (int jj = 0; jj < GRU_UPT; ++jj) hprev[jj] = 0.f;
+    float hprev[GRU_UPT] = {};
     float bias[3][GRU_UPT];
-#pragma unroll
-    for (int g = 0; g < 3; ++g)
-#pragma unroll
-      for (int jj = 0; jj < GRU_UPT; ++jj) bias[g][jj] = s.scratch[g * 16 + uh * GRU_UPT + jj];
+    gru_load_bias(s.scratch + uh * GRU_UPT, GRU_HC, bias);
     const bool active = row < Bp;
     for (int step = 0; step < T; ++step) {
       const int t = dir == 0 ? step : (T - 1 - step);
-      // this step's input projections do not depend on the recurrence: fetch them first
       float gi[3][GRU_UPT];
-      if (active) {
-        const float* g = p.gi + ((long long)t * Bp + row) * (p.ndir * 3 * H) + dir * 3 * H + ju;
-#pragma unroll
-        for (int gg = 0; gg < 3; ++gg) ld8(g + gg * H, gi[gg]);
-      }
+      if (active) gru_load_gi(p, t, row, dir, ju, gi);
       float acc[3][GRU_UPT];
       if (step > 0) {
         mbar_wait(s.accfull, (step - 1) & 1);
@@ -364,44 +603,14 @@ gru_fwd_kernel(const __grid_constant__ CUtensorMap tm_d0, const __grid_constant_
           for (int jj = 0; jj < GRU_UPT; ++jj) acc[gg][jj] = 0.f;
       }
       const long long m = (long long)t * Bp + row;
-      float hn[GRU_UPT], rr[GRU_UPT], zz[GRU_UPT], nn[GRU_UPT];
+      GruGates<GRU_UPT> gt;
       if (active) {
-#pragma unroll
-        for (int jj = 0; jj < GRU_UPT; ++jj) {
-          rr[jj] = fast_sigmoid(gi[0][jj] + acc[0][jj] + bias[0][jj]);
-          zz[jj] = fast_sigmoid(gi[1][jj] + acc[1][jj] + bias[1][jj]);
-          hn[jj] = acc[2][jj] + bias[2][jj];
-          nn[jj] = fast_tanh(gi[2][jj] + rr[jj] * hn[jj]);
-          hprev[jj] = (1.f - zz[jj]) * nn[jj] + zz[jj] * hprev[jj];
-        }
+        gru_cell_fwd(gi, acc, bias, hprev, gt);
         // critical path: only the bf16 h_t that the other CTAs gather next step
-        *reinterpret_cast<uint4*>(p.xn + m * D + dir * H + ju) = pack8(hprev);
-        if (tid == 0) GRU_STAMP(5);
-        if (!(p.ablate & 1)) fence_proxy_async_global();   // generic writes -> other CTAs' TMA reads
-        if (tid == 0) GRU_STAMP(6);
+        st_bf16(p.xn + m * D + dir * H + ju, to_bf16(hprev));
       }
-      epi_barrier();
-      if (tid == 0) {
-        GRU_STAMP(7);
-        grid_arrive(ctr);          // release: cumulative over the CTA's writes ordered by bar.sync
-        GRU_STAMP(9);
-      }
-      // off the critical path: fp32 state, transposed copy, saved gates
-      if (active && !(p.ablate & 2)) {
-        st8(p.y + m * D + dir * H + ju, hprev);
-        if (p.xnT) {
-          bf16* xt = p.xnT + (long long)(dir * H + ju) * ldT + (long long)(t + 1) * Bp + row;
-#pragma unroll
-          for (int jj = 0; jj < GRU_UPT; ++jj) st_stream_bf16(xt + jj * ldT, hprev[jj]);
-        }
-        if (p.gates) {
-          float* go = p.gates + ((m * p.ndir + dir) * 4) * H + ju;
-          st8(go, rr);
-          st8(go + H, zz);
-          st8(go + 2 * H, nn);
-          st8(go + 3 * H, hn);
-        }
-      }
+      gru_publish(p, ctr, step, active, false);
+      if (active) gru_store_fwd(p, m, dir, ju, hprev, gt);
       if (tid == 0) GRU_STAMP(10);
     }
   }
@@ -428,40 +637,17 @@ gru_bwd_kernel(const __grid_constant__ CUtensorMap tm_d0, const __grid_constant_
   const int wbytes = max(nchunks * WCHUNK, 16384 - Bp * 128);
   const GruSmem s = carve(smem_raw, ring_bytes, wbytes);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int D = p.ndir * H;
   const CUtensorMap* tm = dir == 0 ? &tm_d0 : &tm_d1;
   const uint32_t crank = cluster_rank(), csize = cluster_size();
 
-  for (int k = tid; k < (ring_bytes + wbytes) / 16; k += GRU_THREADS)
-    reinterpret_cast<uint4*>(s.ring)[k] = make_uint4(0, 0, 0, 0);
+  smem_zero(s.ring, ring_bytes + wbytes);
   __syncthreads();
-  {
-    // resident operand: rows = the 16 hidden units j0..j0+15 of W_hh^T, K = 3H.  W_hh is read as
-    // stored ([3H][H]: 32 contiguous bytes per k) and transposed on the way into shared memory
-    for (int k = tid; k < K3 * 2; k += GRU_THREADS) {
-      const int kk = k >> 1, half = k & 1;
-      const uint4 v = *reinterpret_cast<const uint4*>(
-          p.whh + ((long long)dir * K3 + kk) * H + j0 + half * 8);
-      const unsigned short* e = reinterpret_cast<const unsigned short*>(&v);
-      uint8_t* chunk = s.wtile + (kk >> 6) * WCHUNK + (kk & 7) * 2;
-#pragma unroll
-      for (int q = 0; q < 8; ++q)
-        *reinterpret_cast<unsigned short*>(
-            chunk + sw128_offset((uint32_t)(half * 8 + q), (uint32_t)((kk & 63) >> 3))) = e[q];
-    }
-  }
-  if (tid == 0) {
-    for (int i = 0; i < GRU_MAX_RING; ++i) {
-      mbar_init(&s.full[i], 1);
-      mbar_init(&s.empty[i], csize);
-    }
+  // resident operand: rows = the 16 hidden units j0..j0+15 of W_hh^T, K = 3H
+  stage_w_cols<GRU_HC>(s.wtile, p.whh + (long long)dir * K3 * H, H, 0, K3, j0);
+  gru_init_barriers(tm, nullptr, true, [=] {
+    init_ring_bars(s.full, s.empty, csize);
     mbar_init(s.accfull, 128);
-    mbar_fence_init();
-    tma_prefetch_desc(tm);
-  }
-  fence_proxy_async_smem();
-  __syncthreads();
-  cluster_sync_all();
+  });
   unsigned int* ctr = p.barrier + dir * 32;   // one L2 line per direction
 
   if (warp == GRU_TMA_WARP) {
@@ -485,36 +671,16 @@ gru_bwd_kernel(const __grid_constant__ CUtensorMap tm_d0, const __grid_constant_
     const int uh = warp >> 2;
     const int ju = j0 + uh * GRU_UPT;
     const bool active = row < Bp;
-    float dh_rec[GRU_UPT];   // dL/dh_t arriving through the recurrence (own units)
-    float db_r[GRU_UPT], db_z[GRU_UPT], db_n[GRU_UPT], db_hn[GRU_UPT];
-#pragma unroll
-    for (int jj = 0; jj < GRU_UPT; ++jj) {
-      dh_rec[jj] = 0.f; db_r[jj] = 0.f; db_z[jj] = 0.f; db_n[jj] = 0.f; db_hn[jj] = 0.f;
-    }
+    float dh_rec[GRU_UPT] = {};   // dL/dh_t arriving through the recurrence (own units)
+    GruGates<GRU_UPT> db = {};
 
     for (int step = 0; step < T; ++step) {
       // forward order of dir 0 is t=0..T-1, so its backward order is T-1..0; dir 1 mirrored
       const int t = dir == 0 ? (T - 1 - step) : step;
-      const int tp = dir == 0 ? t - 1 : t + 1;       // time index of h_{prev} in forward order
-      const bool has_prev = dir == 0 ? (t > 0) : (t < T - 1);
-      bf16* xb = p.xchg + ((long long)(dir * 2 + (step & 1)) * Bp) * K3;
       const long long m = (long long)t * Bp + row;
-      // ---- saved activations of this step: independent of the recurrence, fetched first ----
-      float rr[GRU_UPT], zz[GRU_UPT], nn[GRU_UPT], hn[GRU_UPT], dh[GRU_UPT], hp[GRU_UPT];
-      if (active) {
-        const float* go = p.gates + ((m * p.ndir + dir) * 4) * H + ju;
-        ld8(go, rr);
-        ld8(go + H, zz);
-        ld8(go + 2 * H, nn);
-        ld8(go + 3 * H, hn);
-        ld8(p.dy + m * D + dir * H + ju, dh);
-        if (has_prev) {
-          ld8(p.y + ((long long)tp * Bp + row) * D + dir * H + ju, hp);
-        } else {
-#pragma unroll
-          for (int jj = 0; jj < GRU_UPT; ++jj) hp[jj] = 0.f;
-        }
-      }
+      GruGates<GRU_UPT> sv;
+      float dh[GRU_UPT], hp[GRU_UPT];
+      if (active) gru_load_saved(p, t, row, dir, ju, sv, dh, hp);
       // ---- recurrent part of dL/dh_t: product issued in the previous step ----
       if (step > 0) {
         mbar_wait(s.accfull, (step - 1) & 1);
@@ -524,48 +690,13 @@ gru_bwd_kernel(const __grid_constant__ CUtensorMap tm_d0, const __grid_constant_
 #pragma unroll
         for (int jj = 0; jj < GRU_UPT; ++jj) dh_rec[jj] += active ? ar[jj] : 0.f;
       }
-      float dr[GRU_UPT], dz[GRU_UPT], dn[GRU_UPT], dnr[GRU_UPT];
+      GruGatesBf16<GRU_UPT> d;
       if (active) {
-#pragma unroll
-        for (int jj = 0; jj < GRU_UPT; ++jj) {
-          const float g = dh[jj] + dh_rec[jj];
-          dn[jj] = g * (1.f - zz[jj]) * (1.f - nn[jj] * nn[jj]);
-          dz[jj] = g * (hp[jj] - nn[jj]) * zz[jj] * (1.f - zz[jj]);
-          dr[jj] = dn[jj] * hn[jj] * rr[jj] * (1.f - rr[jj]);
-          dnr[jj] = dn[jj] * rr[jj];
-          dh_rec[jj] = g * zz[jj];      // direct path h_{t-1} -> h_t; the W_hh path is added next step
-          db_r[jj] += dr[jj];
-          db_z[jj] += dz[jj];
-          db_n[jj] += dn[jj];
-          db_hn[jj] += dnr[jj];
-        }
-        // critical path: the exchange rows [dr | dz | dn*r] every CTA gathers for the product
-        if (step + 1 < T) {
-          bf16* x = xb + (long long)row * K3 + ju;
-          *reinterpret_cast<uint4*>(x) = pack8(dr);
-          *reinterpret_cast<uint4*>(x + H) = pack8(dz);
-          *reinterpret_cast<uint4*>(x + 2 * H) = pack8(dnr);
-          if (tid == 0) GRU_STAMP(5);
-          fence_proxy_async_global();
-          if (tid == 0) GRU_STAMP(6);
-        }
+        d = gru_cell_bwd(dh, dh_rec, sv, hp, db);
+        if (step + 1 < T) gru_store_xchg(p, step, row, dir, ju, d);
       }
-      if (step + 1 < T) {
-        epi_barrier();
-        if (tid == 0) {
-          GRU_STAMP(7);
-          grid_arrive(ctr);
-          GRU_STAMP(9);
-        }
-      }
-      // ---- off the critical path: operands of the dX / dW GEMMs ----
-      if (active) {
-        bf16* o = p.dgi + m * (p.ndir * K3) + dir * K3 + ju;
-        st_stream_u4(o, pack8(dr));
-        st_stream_u4(o + H, pack8(dz));
-        st_stream_u4(o + 2 * H, pack8(dn));
-        st_stream_u4(p.dghn + m * D + dir * H + ju, pack8(dnr));
-      }
+      if (step + 1 < T) gru_publish(p, ctr, step, active, false);
+      if (active) gru_store_bwd(p, m, dir, ju, d);
       if (tid == 0) GRU_STAMP(10);
     }
     // ---- bias gradients: reduce the per-batch-row partial sums over the CTA ----
@@ -575,10 +706,10 @@ gru_bwd_kernel(const __grid_constant__ CUtensorMap tm_d0, const __grid_constant_
     epi_barrier();
 #pragma unroll
     for (int jj = 0; jj < GRU_UPT; ++jj) {
-      const float a = warp_sum(active ? db_r[jj] : 0.f);
-      const float b = warp_sum(active ? db_z[jj] : 0.f);
-      const float c = warp_sum(active ? db_n[jj] : 0.f);
-      const float d = warp_sum(active ? db_hn[jj] : 0.f);
+      const float a = warp_sum(active ? db.r[jj] : 0.f);
+      const float b = warp_sum(active ? db.z[jj] : 0.f);
+      const float c = warp_sum(active ? db.n[jj] : 0.f);
+      const float d = warp_sum(active ? db.hn[jj] : 0.f);
       if (lane == 0) {
         atomicAdd(&red[uh * GRU_UPT + jj], a);
         atomicAdd(&red[16 + uh * GRU_UPT + jj], b);
@@ -760,40 +891,19 @@ gru_bwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
   uint64_t* accfull = bars + 4;
   uint64_t* recvbar = bars + 5;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int D = p.ndir * H;
   const CUtensorMap* tm = dir == 0 ? &tm_d0 : &tm_d1;
   const int gc = (nchunks % 4 == 0) ? 4 : ((nchunks % 3 == 0) ? 3 : ((nchunks % 2 == 0) ? 2 : 1));
   const int ngroups = nchunks / gc;                   // <= 4 for H <= 1024 ... checked on host
 
-  for (int k = tid; k < (ring_bytes + wbytes + 2 * KS * Bp * 64) / 16; k += GRU_THREADS)
-    reinterpret_cast<uint4*>(base)[k] = make_uint4(0, 0, 0, 0);
+  smem_zero(base, ring_bytes + wbytes + 2 * KS * Bp * 64);
   __syncthreads();
-  {
-    // resident operand: rows = the cluster's 64 units of W_hh^T, columns = this CTA's K quarter.
-    // W_hh is read as stored ([3H][H]: the cluster's 64 units are 128 contiguous bytes of row k)
-    // and transposed on the way into shared memory (once per launch)
-    for (int k = tid; k < KQ * 8; k += GRU_THREADS) {
-      const int kl = k >> 3, piece = k & 7;       // local k, 8-unit piece of the 64 units
-      const uint4 v = *reinterpret_cast<const uint4*>(
-          p.whh + ((long long)dir * K3 + (long long)crank * KQ + kl) * H + k0c + piece * 8);
-      const unsigned short* e = reinterpret_cast<const unsigned short*>(&v);
-      uint8_t* chunk = wtile + (kl >> 6) * WCHUNK + (kl & 7) * 2;
-#pragma unroll
-      for (int q = 0; q < 8; ++q)
-        *reinterpret_cast<unsigned short*>(
-            chunk + sw128_offset((uint32_t)(piece * 8 + q), (uint32_t)((kl & 63) >> 3))) = e[q];
-    }
-  }
-  if (tid == 0) {
+  // resident operand: rows = the cluster's 64 units of W_hh^T, columns = this CTA's K quarter
+  stage_w_cols<KS * GRU_HC>(wtile, p.whh + (long long)dir * K3 * H, H, (int)crank * KQ, KQ, k0c);
+  gru_init_barriers(tm, nullptr, !L2RS, [=] {
     for (int i = 0; i < 4; ++i) mbar_init(&full[i], 1);
     mbar_init(accfull, 128);
     mbar_init(recvbar, 1);   // one local arrive.expect_tx per step; the peers' copies complete_tx
-    mbar_fence_init();
-    tma_prefetch_desc(tm);
-  }
-  fence_proxy_async_smem();
-  __syncthreads();
-  if (!L2RS) cluster_sync_all();
+  });
   unsigned int* ctr = p.barrier + dir * 32;   // one L2 line per direction
 
   if (warp == GRU_TMA_WARP) {
@@ -861,34 +971,15 @@ gru_bwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
     const int uh = warp >> 2;
     const int ju = j0 + uh * GRU_UPT;
     const bool active = row < Bp;
-    float dh_rec[GRU_UPT];
-    float db_r[GRU_UPT], db_z[GRU_UPT], db_n[GRU_UPT], db_hn[GRU_UPT];
-#pragma unroll
-    for (int jj = 0; jj < GRU_UPT; ++jj) {
-      dh_rec[jj] = 0.f; db_r[jj] = 0.f; db_z[jj] = 0.f; db_n[jj] = 0.f; db_hn[jj] = 0.f;
-    }
+    float dh_rec[GRU_UPT] = {};
+    GruGates<GRU_UPT> db = {};
 
     for (int step = 0; step < T; ++step) {
       const int t = dir == 0 ? (T - 1 - step) : step;
-      const int tp = dir == 0 ? t - 1 : t + 1;
-      const bool has_prev = dir == 0 ? (t > 0) : (t < T - 1);
-      bf16* xb = p.xchg + ((long long)(dir * 2 + (step & 1)) * Bp) * K3;
       const long long m = (long long)t * Bp + row;
-      float rr[GRU_UPT], zz[GRU_UPT], nn[GRU_UPT], hn[GRU_UPT], dh[GRU_UPT], hp[GRU_UPT];
-      if (active) {
-        const float* go = p.gates + ((m * p.ndir + dir) * 4) * H + ju;
-        ld8(go, rr);
-        ld8(go + H, zz);
-        ld8(go + 2 * H, nn);
-        ld8(go + 3 * H, hn);
-        ld8(p.dy + m * D + dir * H + ju, dh);
-        if (has_prev) {
-          ld8(p.y + ((long long)tp * Bp + row) * D + dir * H + ju, hp);
-        } else {
-#pragma unroll
-          for (int jj = 0; jj < GRU_UPT; ++jj) hp[jj] = 0.f;
-        }
-      }
+      GruGates<GRU_UPT> sv;
+      float dh[GRU_UPT], hp[GRU_UPT];
+      if (active) gru_load_saved(p, t, row, dir, ju, sv, dh, hp);
       // ---- recurrent part of dL/dh_t: reduce-scatter of the four partial products ----
       if (step > 0) {
         mbar_wait(accfull, (step - 1) & 1);
@@ -914,54 +1005,21 @@ gru_bwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
           }
         }
       }
-      float dr[GRU_UPT], dz[GRU_UPT], dn[GRU_UPT], dnr[GRU_UPT];
+      GruGatesBf16<GRU_UPT> d;
       if (active) {
-#pragma unroll
-        for (int jj = 0; jj < GRU_UPT; ++jj) {
-          const float g = dh[jj] + dh_rec[jj];
-          dn[jj] = g * (1.f - zz[jj]) * (1.f - nn[jj] * nn[jj]);
-          dz[jj] = g * (hp[jj] - nn[jj]) * zz[jj] * (1.f - zz[jj]);
-          dr[jj] = dn[jj] * hn[jj] * rr[jj] * (1.f - rr[jj]);
-          dnr[jj] = dn[jj] * rr[jj];
-          dh_rec[jj] = g * zz[jj];
-          db_r[jj] += dr[jj];
-          db_z[jj] += dz[jj];
-          db_n[jj] += dn[jj];
-          db_hn[jj] += dnr[jj];
-        }
-        if (step + 1 < T) {
-          bf16* x = xb + (long long)row * K3 + ju;
-          *reinterpret_cast<uint4*>(x) = pack8(dr);
-          *reinterpret_cast<uint4*>(x + H) = pack8(dz);
-          *reinterpret_cast<uint4*>(x + 2 * H) = pack8(dnr);
-          if (tid == 0) GRU_STAMP(5);
-          if (!(p.ablate & 1)) fence_proxy_async_global();
-          if (tid == 0) GRU_STAMP(6);
-        }
+        d = gru_cell_bwd(dh, dh_rec, sv, hp, db);
+        if (step + 1 < T) gru_store_xchg(p, step, row, dir, ju, d);
       }
-      if (step + 1 < T) {
-        epi_barrier();
-        if (tid == 0) {
-          GRU_STAMP(7);
-          grid_arrive(ctr);
-          GRU_STAMP(9);
-        }
-      }
-      if (active && !(p.ablate & 2)) {
-        bf16* o = p.dgi + m * (p.ndir * K3) + dir * K3 + ju;
-        st_stream_u4(o, pack8(dr));
-        st_stream_u4(o + H, pack8(dz));
-        st_stream_u4(o + 2 * H, pack8(dn));
-        st_stream_u4(p.dghn + m * D + dir * H + ju, pack8(dnr));
-      }
+      if (step + 1 < T) gru_publish(p, ctr, step, active, false);
+      if (active) gru_store_bwd(p, m, dir, ju, d);
       if (tid == 0) GRU_STAMP(10);
     }
 #pragma unroll
     for (int jj = 0; jj < GRU_UPT; ++jj) {
-      const float a = warp_sum(active ? db_r[jj] : 0.f);
-      const float b = warp_sum(active ? db_z[jj] : 0.f);
-      const float c = warp_sum(active ? db_n[jj] : 0.f);
-      const float d = warp_sum(active ? db_hn[jj] : 0.f);
+      const float a = warp_sum(active ? db.r[jj] : 0.f);
+      const float b = warp_sum(active ? db.z[jj] : 0.f);
+      const float c = warp_sum(active ? db.n[jj] : 0.f);
+      const float d = warp_sum(active ? db.hn[jj] : 0.f);
       if (lane == 0) {
         const int bi = dir * K3 + ju + jj;
         atomicAdd(p.dbih + bi, a);
@@ -1046,35 +1104,17 @@ gru_fwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
   const int D = p.ndir * H;
   const CUtensorMap* tm = dir == 0 ? &tm_d0 : &tm_d1;
 
-  for (int k = tid; k < (ring_bytes + wbytes + 2 * KS * Bp * RW * 4) / 16; k += GRU_THREADS)
-    reinterpret_cast<uint4*>(base)[k] = make_uint4(0, 0, 0, 0);
+  smem_zero(base, ring_bytes + wbytes + 2 * KS * Bp * RW * 4);
   __syncthreads();
-  {
-    // resident operand: rows = (gate, unit of the cluster), columns = this CTA's K slice
-    const int pieces_per_row = nchunks * 8;
-    for (int k = tid; k < NCOL * pieces_per_row; k += GRU_THREADS) {
-      const int r = k / pieces_per_row, pc = k % pieces_per_row;
-      const int g = r / (KS * GRU_HC), u = r % (KS * GRU_HC);
-      const uint4 v = *reinterpret_cast<const uint4*>(
-          p.whh + ((long long)dir * 3 * H + (long long)g * H + k0c + u) * H + (long long)crank * KQ +
-          pc * 8);
-      *reinterpret_cast<uint4*>(wtile + (pc >> 3) * WCHUNK + sw128_offset(r, pc & 7)) = v;
-    }
-    if (tid < RW) {
-      const int g = tid / GRU_HC, jj = tid % GRU_HC;
-      bias_s[tid] = p.bhh[dir * 3 * H + g * H + j0 + jj];
-    }
-  }
-  if (tid == 0) {
+  // resident operand: rows = (gate, unit of the cluster), columns = this CTA's K slice
+  stage_w_rows(wtile, WCHUNK, p.whh + (long long)dir * 3 * H * H, H, NCOL, (int)crank * KQ, KQ,
+               [=](int r) { return (r / (KS * GRU_HC)) * H + k0c + r % (KS * GRU_HC); });
+  if (tid < RW) bias_s[tid] = p.bhh[dir * 3 * H + (tid / GRU_HC) * H + j0 + tid % GRU_HC];
+  gru_init_barriers(tm, nullptr, true, [=] {
     mbar_init(full, 1);
     mbar_init(accfull, 128);
     mbar_init(recvbar, 1);   // one local arrive.expect_tx per step; the peers' copies complete_tx
-    mbar_fence_init();
-    tma_prefetch_desc(tm);
-  }
-  fence_proxy_async_smem();
-  __syncthreads();
-  cluster_sync_all();
+  });
   unsigned int* ctr = p.barrier + dir * 32;   // one L2 line per direction
 
   if (warp == GRU_TMA_WARP) {
@@ -1130,28 +1170,15 @@ gru_fwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
     const int uh = warp >> 2;
     const int ju = j0 + uh * GRU_UPT;
     const bool active = row < Bp;
-    float hprev[GRU_UPT];
-#pragma unroll
-    for (int jj = 0; jj < GRU_UPT; ++jj) hprev[jj] = 0.f;
+    float hprev[GRU_UPT] = {};
     float bias[3][GRU_UPT];
-#pragma unroll
-    for (int g = 0; g < 3; ++g)
-#pragma unroll
-      for (int jj = 0; jj < GRU_UPT; ++jj) bias[g][jj] = bias_s[g * GRU_HC + uh * GRU_UPT + jj];
+    gru_load_bias(bias_s + uh * GRU_UPT, GRU_HC, bias);
 
     for (int step = 0; step < T; ++step) {
       const int t = dir == 0 ? step : (T - 1 - step);
       float gi[3][GRU_UPT];
-      if (active) {
-        const float* g = p.gi + ((long long)t * Bp + row) * (p.ndir * 3 * H) + dir * 3 * H + ju;
-#pragma unroll
-        for (int gg = 0; gg < 3; ++gg) ld8(g + gg * H, gi[gg]);
-      }
-      float acc[3][GRU_UPT];
-#pragma unroll
-      for (int gg = 0; gg < 3; ++gg)
-#pragma unroll
-        for (int jj = 0; jj < GRU_UPT; ++jj) acc[gg][jj] = 0.f;
+      if (active) gru_load_gi(p, t, row, dir, ju, gi);
+      float acc[3][GRU_UPT] = {};
       if (step > 0) {
         mbar_wait(accfull, (step - 1) & 1);
         if (tid == 0) GRU_STAMP(3);
@@ -1185,39 +1212,13 @@ gru_fwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
         }
       }
       const long long m = (long long)t * Bp + row;
-      float hn[GRU_UPT], rr[GRU_UPT], zz[GRU_UPT], nn[GRU_UPT];
+      GruGates<GRU_UPT> gt;
       if (active) {
-#pragma unroll
-        for (int jj = 0; jj < GRU_UPT; ++jj) {
-          rr[jj] = fast_sigmoid(gi[0][jj] + acc[0][jj] + bias[0][jj]);
-          zz[jj] = fast_sigmoid(gi[1][jj] + acc[1][jj] + bias[1][jj]);
-          hn[jj] = acc[2][jj] + bias[2][jj];
-          nn[jj] = fast_tanh(gi[2][jj] + rr[jj] * hn[jj]);
-          hprev[jj] = (1.f - zz[jj]) * nn[jj] + zz[jj] * hprev[jj];
-        }
-        // critical path: only the bf16 h_t that the other CTAs gather next step
-        *reinterpret_cast<uint4*>(p.xn + m * D + dir * H + ju) = pack8(hprev);
-        if (tid == 0) GRU_STAMP(5);
-        if (!(p.ablate & 1)) fence_proxy_async_global();   // generic writes -> other CTAs' TMA reads
-        if (tid == 0) GRU_STAMP(6);
+        gru_cell_fwd(gi, acc, bias, hprev, gt);
+        st_bf16(p.xn + m * D + dir * H + ju, to_bf16(hprev));
       }
-      epi_barrier();
-      if (tid == 0) {
-        GRU_STAMP(7);
-        if (p.dbg && step == 20) p.dbg[1024 + blockIdx.x] = gtime();         // skew probe
-        grid_arrive(ctr);
-        GRU_STAMP(9);
-      }
-      if (active && !(p.ablate & 2)) {
-        st8(p.y + m * D + dir * H + ju, hprev);
-        if (p.gates) {
-          float* go = p.gates + ((m * p.ndir + dir) * 4) * H + ju;
-          st8(go, rr);
-          st8(go + H, zz);
-          st8(go + 2 * H, nn);
-          st8(go + 3 * H, hn);
-        }
-      }
+      gru_publish(p, ctr, step, active, true);
+      if (active) gru_store_fwd(p, m, dir, ju, hprev, gt);
       if (tid == 0) GRU_STAMP(10);
     }
   }
@@ -1242,40 +1243,26 @@ gru_fwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
 // epilogue threads (thread = batch row x UPT units) from the four received slices.
 // Requires cluster size 4, H % 256 == 0, Bp <= 64 (Bp % 8 == 0 as everywhere).
 // =============================================================================================
-template <int UPT>
-SB_DEVINL void ldu(const float* p, float (&v)[UPT]) {
-  if constexpr (UPT == 4) {
-    const float4 a = __ldcs(reinterpret_cast<const float4*>(p));
-    v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w;
-  } else if constexpr (UPT == 2) {
-    const float2 a = __ldcs(reinterpret_cast<const float2*>(p));
-    v[0] = a.x; v[1] = a.y;
-  } else {
-    v[0] = __ldcs(p);
-  }
-}
-template <int UPT>
-SB_DEVINL void stu(float* p, const float (&v)[UPT]) {
-  if constexpr (UPT == 4) __stcs(reinterpret_cast<float4*>(p), make_float4(v[0], v[1], v[2], v[3]));
-  else if constexpr (UPT == 2) __stcs(reinterpret_cast<float2*>(p), make_float2(v[0], v[1]));
-  else __stcs(p, v[0]);
-}
-template <int UPT>
-SB_DEVINL void st_bf16u(bf16* p, const float (&v)[UPT]) {
-  if constexpr (UPT == 4) {
-    *reinterpret_cast<uint2*>(p) = make_uint2(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]));
-  } else if constexpr (UPT == 2) {
-    *reinterpret_cast<uint32_t*>(p) = pack_bf16x2(v[0], v[1]);
-  } else {
-    *p = __float2bfloat16_rn(v[0]);
-  }
-}
-
 // Owner-major staging of the transposed accumulators: slice of peer q (the own slice lives in
 // recv[crank], the others in stage[(q - crank) mod KS - 1]), row srow, column = batch row.
 SB_DEVINL float* kt_slice(float* recv, float* stage, int slice, uint32_t q, uint32_t crank) {
   const uint32_t q0 = (q + KS - crank) % KS;
   return q0 == 0 ? recv + (size_t)crank * slice : stage + (size_t)(q0 - 1) * slice;
+}
+
+// Reduce-scatter of one step once the MMA warpgroup staged the three outgoing slices (and the own
+// one in recv[crank]): thread 0 arms recvbar for the incoming ones, lane 0 of warp w = 1..3 sends
+// the slice of peer crank + w as one bulk copy into its recv[crank].
+SB_DEVINL void kt_exchange(float* recv, const float* stage, uint64_t* recvbar, uint32_t crank,
+                           int slice) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) mbar_expect_tx(recvbar, (uint32_t)((KS - 1) * slice * 4));
+  if (lane == 0 && warp >= 1 && warp <= KS - 1) {
+    const uint32_t pr = (crank + (uint32_t)warp) % KS;
+    bulk_s2peer(mapa_shared(smem_u32(recv + (size_t)crank * slice), pr),
+                stage + (size_t)(warp - 1) * slice, (uint32_t)(slice * 4),
+                mapa_shared(smem_u32(recvbar), pr));
+  }
 }
 
 // MMA warpgroup of gru_fwd_kt_kernel, one step per iteration: three m64 blocks of weight rows
@@ -1398,37 +1385,20 @@ gru_fwd_kt_kernel(const __grid_constant__ CUtensorMap tm_d0,
   const int D = p.ndir * H;
   const CUtensorMap* tm = dir == 0 ? &tm_d0 : &tm_d1;
 
-  for (int k = tid; k < (ring_bytes + wbytes + (2 * KS - 1) * slice * 4) / 16; k += GRU_THREADS)
-    reinterpret_cast<uint4*>(base)[k] = make_uint4(0, 0, 0, 0);
+  smem_zero(base, ring_bytes + wbytes + (2 * KS - 1) * slice * 4);
   __syncthreads();
-  {
-    // resident operand: rows ordered by owner (see above), columns = this CTA's K quarter
-    const int pieces_per_row = nchunks * 8;
-    for (int k = tid; k < WROWS * pieces_per_row; k += GRU_THREADS) {
-      const int r = k / pieces_per_row, pc = k % pieces_per_row;
-      int g, u;
-      if (r < 128) { g = (r & 31) >> 4; u = (r >> 5) * GRU_HC + (r & 15); }
-      else { g = 2; u = r - 128; }
-      const uint4 v = *reinterpret_cast<const uint4*>(
-          p.whh + ((long long)dir * 3 * H + (long long)g * H + k0c + u) * H + (long long)crank * KQ +
-          pc * 8);
-      *reinterpret_cast<uint4*>(wtile + (pc >> 3) * WCHUNK + sw128_offset(r, pc & 7)) = v;
-    }
-    if (tid < RW) {
-      const int g = tid / GRU_HC, jj = tid % GRU_HC;
-      bias_s[tid] = p.bhh[dir * 3 * H + g * H + j0 + jj];
-    }
-  }
-  if (tid == 0) {
+  // resident operand: rows ordered by owner (see above), columns = this CTA's K quarter
+  stage_w_rows(wtile, WCHUNK, p.whh + (long long)dir * 3 * H * H, H, WROWS, (int)crank * KQ, KQ,
+               [=](int r) {
+                 return r < 128 ? ((r & 31) >> 4) * H + k0c + (r >> 5) * GRU_HC + (r & 15)
+                                : 2 * H + k0c + r - 128;
+               });
+  if (tid < RW) bias_s[tid] = p.bhh[dir * 3 * H + (tid / GRU_HC) * H + j0 + tid % GRU_HC];
+  gru_init_barriers(tm, nullptr, true, [=] {
     mbar_init(full, 1);
     mbar_init(accfull, 128);
     mbar_init(recvbar, 1);   // one local arrive.expect_tx per step; the peers' copies complete_tx
-    mbar_fence_init();
-    tma_prefetch_desc(tm);
-  }
-  fence_proxy_async_smem();
-  __syncthreads();
-  cluster_sync_all();
+  });
   unsigned int* ctr = p.barrier + dir * 32;   // one L2 line per direction
 
   if (warp == GRU_TMA_WARP) {
@@ -1461,39 +1431,19 @@ gru_fwd_kt_kernel(const __grid_constant__ CUtensorMap tm_d0,
     const bool active = ug * UPT < GRU_HC;
     const int u0 = ug * UPT;
     const int ju = j0 + u0;
-    float hprev[UPT];
-#pragma unroll
-    for (int jj = 0; jj < UPT; ++jj) hprev[jj] = 0.f;
-    float bias[3][UPT];
-#pragma unroll
-    for (int g = 0; g < 3; ++g)
-#pragma unroll
-      for (int jj = 0; jj < UPT; ++jj) bias[g][jj] = active ? bias_s[g * GRU_HC + u0 + jj] : 0.f;
+    float hprev[UPT] = {};
+    float bias[3][UPT] = {};
+    if (active) gru_load_bias(bias_s + u0, GRU_HC, bias);
 
     for (int step = 0; step < T; ++step) {
       const int t = dir == 0 ? step : (T - 1 - step);
       float gi[3][UPT];
-      if (active) {
-        const float* g = p.gi + ((long long)t * Bp + b) * (p.ndir * 3 * H) + dir * 3 * H + ju;
-#pragma unroll
-        for (int gg = 0; gg < 3; ++gg) ldu<UPT>(g + gg * H, gi[gg]);
-      }
-      float acc[3][UPT];
-#pragma unroll
-      for (int gg = 0; gg < 3; ++gg)
-#pragma unroll
-        for (int jj = 0; jj < UPT; ++jj) acc[gg][jj] = 0.f;
+      if (active) gru_load_gi(p, t, b, dir, ju, gi);
+      float acc[3][UPT] = {};
       if (step > 0) {
         mbar_wait(accfull, (step - 1) & 1);
         if (tid == 0) GRU_STAMP(3);
-        // the MMA warpgroup staged the three outgoing slices (and the own one in recv[crank])
-        if (tid == 0) mbar_expect_tx(recvbar, (uint32_t)((KS - 1) * slice * 4));
-        if (lane == 0 && warp >= 1 && warp <= KS - 1) {
-          const uint32_t pr = (crank + (uint32_t)warp) % KS;
-          bulk_s2peer(mapa_shared(smem_u32(recv + (size_t)crank * slice), pr),
-                      stage + (size_t)(warp - 1) * slice, (uint32_t)(slice * 4),
-                      mapa_shared(smem_u32(recvbar), pr));
-        }
+        kt_exchange(recv, stage, recvbar, crank, slice);
         if (tid == 0) GRU_STAMP(4);
         mbar_wait(recvbar, (step - 1) & 1);
         if (active) {
@@ -1508,39 +1458,13 @@ gru_fwd_kt_kernel(const __grid_constant__ CUtensorMap tm_d0,
         }
       }
       const long long m = (long long)t * Bp + b;
-      float hn[UPT], rr[UPT], zz[UPT], nn[UPT];
+      GruGates<UPT> gt;
       if (active) {
-#pragma unroll
-        for (int jj = 0; jj < UPT; ++jj) {
-          rr[jj] = fast_sigmoid(gi[0][jj] + acc[0][jj] + bias[0][jj]);
-          zz[jj] = fast_sigmoid(gi[1][jj] + acc[1][jj] + bias[1][jj]);
-          hn[jj] = acc[2][jj] + bias[2][jj];
-          nn[jj] = fast_tanh(gi[2][jj] + rr[jj] * hn[jj]);
-          hprev[jj] = (1.f - zz[jj]) * nn[jj] + zz[jj] * hprev[jj];
-        }
-        // critical path: only the bf16 h_t that the other CTAs gather next step
-        st_bf16u<UPT>(p.xn + m * D + dir * H + ju, hprev);
-        if (tid == 0) GRU_STAMP(5);
-        fence_proxy_async_global();   // generic writes -> other CTAs' TMA reads
-        if (tid == 0) GRU_STAMP(6);
+        gru_cell_fwd(gi, acc, bias, hprev, gt);
+        st_bf16(p.xn + m * D + dir * H + ju, to_bf16(hprev));
       }
-      epi_barrier();
-      if (tid == 0) {
-        GRU_STAMP(7);
-        if (p.dbg && step == 20) p.dbg[1024 + blockIdx.x] = gtime();         // skew probe
-        grid_arrive(ctr);
-        GRU_STAMP(9);
-      }
-      if (active) {
-        stu<UPT>(p.y + m * D + dir * H + ju, hprev);
-        if (p.gates) {
-          float* go = p.gates + ((m * p.ndir + dir) * 4) * H + ju;
-          stu<UPT>(go, rr);
-          stu<UPT>(go + H, zz);
-          stu<UPT>(go + 2 * H, nn);
-          stu<UPT>(go + 3 * H, hn);
-        }
-      }
+      gru_publish(p, ctr, step, active, true);
+      if (active) gru_store_fwd(p, m, dir, ju, hprev, gt);
       if (tid == 0) GRU_STAMP(10);
     }
   }
@@ -1557,17 +1481,6 @@ gru_fwd_kt_kernel(const __grid_constant__ CUtensorMap tm_d0,
 // of the cluster); an accumulator row is a unit, so its Bp partial sums go to exactly one peer, and the elementwise work runs on all 256
 // epilogue threads (thread = batch row x UPT units).
 // =============================================================================================
-template <int UPT>
-SB_DEVINL void st_stream_bf16u(bf16* p, const float (&v)[UPT]) {
-  if constexpr (UPT == 4) {
-    __stcs(reinterpret_cast<uint2*>(p), make_uint2(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3])));
-  } else if constexpr (UPT == 2) {
-    __stcs(reinterpret_cast<unsigned int*>(p), pack_bf16x2(v[0], v[1]));
-  } else {
-    st_stream_bf16(p, v[0]);
-  }
-}
-
 template <int UPT>
 __global__ void __launch_bounds__(GRU_THREADS, 1)
 gru_bwd_kt_kernel(const __grid_constant__ CUtensorMap tm_d0,
@@ -1602,39 +1515,19 @@ gru_bwd_kt_kernel(const __grid_constant__ CUtensorMap tm_d0,
   uint64_t* accfull = bars + 4;
   uint64_t* recvbar = bars + 5;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int D = p.ndir * H;
   const CUtensorMap* tm = dir == 0 ? &tm_d0 : &tm_d1;
   const int gc = (nchunks % 4 == 0) ? 4 : ((nchunks % 3 == 0) ? 3 : ((nchunks % 2 == 0) ? 2 : 1));
   const int ngroups = nchunks / gc;                   // <= 4 for H <= 1024 ... checked on host
 
-  for (int k = tid; k < (ring_bytes + wbytes + (2 * KS - 1) * slice * 4) / 16;
-       k += GRU_THREADS)
-    reinterpret_cast<uint4*>(base)[k] = make_uint4(0, 0, 0, 0);
+  smem_zero(base, ring_bytes + wbytes + (2 * KS - 1) * slice * 4);
   __syncthreads();
-  {
-    // resident operand: see gru_bwd_ks_kernel
-    for (int k = tid; k < KQ * 8; k += GRU_THREADS) {
-      const int kl = k >> 3, piece = k & 7;       // local k, 8-unit piece of the 64 units
-      const uint4 v = *reinterpret_cast<const uint4*>(
-          p.whh + ((long long)dir * K3 + (long long)crank * KQ + kl) * H + k0c + piece * 8);
-      const unsigned short* e = reinterpret_cast<const unsigned short*>(&v);
-      uint8_t* chunk = wtile + (kl >> 6) * WCHUNK + (kl & 7) * 2;
-#pragma unroll
-      for (int q = 0; q < 8; ++q)
-        *reinterpret_cast<unsigned short*>(
-            chunk + sw128_offset((uint32_t)(piece * 8 + q), (uint32_t)((kl & 63) >> 3))) = e[q];
-    }
-  }
-  if (tid == 0) {
+  // resident operand: see gru_bwd_ks_kernel
+  stage_w_cols<KS * GRU_HC>(wtile, p.whh + (long long)dir * K3 * H, H, (int)crank * KQ, KQ, k0c);
+  gru_init_barriers(tm, nullptr, true, [=] {
     for (int i = 0; i < 4; ++i) mbar_init(&full[i], 1);
     mbar_init(accfull, 128);
     mbar_init(recvbar, 1);
-    mbar_fence_init();
-    tma_prefetch_desc(tm);
-  }
-  fence_proxy_async_smem();
-  __syncthreads();
-  cluster_sync_all();
+  });
   unsigned int* ctr = p.barrier + dir * 32;   // one L2 line per direction
 
   if (warp == GRU_TMA_WARP) {
@@ -1666,45 +1559,19 @@ gru_bwd_kt_kernel(const __grid_constant__ CUtensorMap tm_d0,
     const bool active = ug * UPT < GRU_HC;
     const int u0 = ug * UPT;
     const int ju = j0 + u0;
-    float dh_rec[UPT];
-    float db_r[UPT], db_z[UPT], db_n[UPT], db_hn[UPT];
-#pragma unroll
-    for (int jj = 0; jj < UPT; ++jj) {
-      dh_rec[jj] = 0.f; db_r[jj] = 0.f; db_z[jj] = 0.f; db_n[jj] = 0.f; db_hn[jj] = 0.f;
-    }
+    float dh_rec[UPT] = {};
+    GruGates<UPT> db = {};
 
     for (int step = 0; step < T; ++step) {
       const int t = dir == 0 ? (T - 1 - step) : step;
-      const int tp = dir == 0 ? t - 1 : t + 1;
-      const bool has_prev = dir == 0 ? (t > 0) : (t < T - 1);
-      bf16* xb = p.xchg + ((long long)(dir * 2 + (step & 1)) * Bp) * K3;
       const long long m = (long long)t * Bp + b;
-      float rr[UPT], zz[UPT], nn[UPT], hn[UPT], dh[UPT], hp[UPT];
-      if (active) {
-        const float* go = p.gates + ((m * p.ndir + dir) * 4) * H + ju;
-        ldu<UPT>(go, rr);
-        ldu<UPT>(go + H, zz);
-        ldu<UPT>(go + 2 * H, nn);
-        ldu<UPT>(go + 3 * H, hn);
-        ldu<UPT>(p.dy + m * D + dir * H + ju, dh);
-        if (has_prev) {
-          ldu<UPT>(p.y + ((long long)tp * Bp + b) * D + dir * H + ju, hp);
-        } else {
-#pragma unroll
-          for (int jj = 0; jj < UPT; ++jj) hp[jj] = 0.f;
-        }
-      }
+      GruGates<UPT> sv;
+      float dh[UPT], hp[UPT];
+      if (active) gru_load_saved(p, t, b, dir, ju, sv, dh, hp);
       if (step > 0) {
         mbar_wait(accfull, (step - 1) & 1);
         if (tid == 0) GRU_STAMP(3);
-        // the MMA warpgroup staged the three outgoing slices (and the own one in recv[crank])
-        if (tid == 0) mbar_expect_tx(recvbar, (uint32_t)((KS - 1) * slice * 4));
-        if (lane == 0 && warp >= 1 && warp <= KS - 1) {
-          const uint32_t pr = (crank + (uint32_t)warp) % KS;
-          bulk_s2peer(mapa_shared(smem_u32(recv + (size_t)crank * slice), pr),
-                      stage + (size_t)(warp - 1) * slice, (uint32_t)(slice * 4),
-                      mapa_shared(smem_u32(recvbar), pr));
-        }
+        kt_exchange(recv, stage, recvbar, crank, slice);
         if (tid == 0) GRU_STAMP(4);
         mbar_wait(recvbar, (step - 1) & 1);
         if (active) {
@@ -1716,58 +1583,25 @@ gru_bwd_kt_kernel(const __grid_constant__ CUtensorMap tm_d0,
           }
         }
       }
-      float dr[UPT], dz[UPT], dn[UPT], dnr[UPT];
+      GruGatesBf16<UPT> d;
       if (active) {
-#pragma unroll
-        for (int jj = 0; jj < UPT; ++jj) {
-          const float g = dh[jj] + dh_rec[jj];
-          dn[jj] = g * (1.f - zz[jj]) * (1.f - nn[jj] * nn[jj]);
-          dz[jj] = g * (hp[jj] - nn[jj]) * zz[jj] * (1.f - zz[jj]);
-          dr[jj] = dn[jj] * hn[jj] * rr[jj] * (1.f - rr[jj]);
-          dnr[jj] = dn[jj] * rr[jj];
-          dh_rec[jj] = g * zz[jj];
-          db_r[jj] += dr[jj];
-          db_z[jj] += dz[jj];
-          db_n[jj] += dn[jj];
-          db_hn[jj] += dnr[jj];
-        }
-        if (step + 1 < T) {
-          bf16* x = xb + (long long)b * K3 + ju;
-          st_bf16u<UPT>(x, dr);
-          st_bf16u<UPT>(x + H, dz);
-          st_bf16u<UPT>(x + 2 * H, dnr);
-          if (tid == 0) GRU_STAMP(5);
-          fence_proxy_async_global();
-          if (tid == 0) GRU_STAMP(6);
-        }
+        d = gru_cell_bwd(dh, dh_rec, sv, hp, db);
+        if (step + 1 < T) gru_store_xchg(p, step, b, dir, ju, d);
       }
-      if (step + 1 < T) {
-        epi_barrier();
-        if (tid == 0) {
-          GRU_STAMP(7);
-          grid_arrive(ctr);
-          GRU_STAMP(9);
-        }
-      }
-      if (active) {
-        bf16* o = p.dgi + m * (p.ndir * K3) + dir * K3 + ju;
-        st_stream_bf16u<UPT>(o, dr);
-        st_stream_bf16u<UPT>(o + H, dz);
-        st_stream_bf16u<UPT>(o + 2 * H, dn);
-        st_stream_bf16u<UPT>(p.dghn + m * D + dir * H + ju, dnr);
-      }
+      if (step + 1 < T) gru_publish(p, ctr, step, active, false);
+      if (active) gru_store_bwd(p, m, dir, ju, d);
       if (tid == 0) GRU_STAMP(10);
     }
     if (active) {
 #pragma unroll
       for (int jj = 0; jj < UPT; ++jj) {
         const int bi = dir * K3 + ju + jj;
-        atomicAdd(p.dbih + bi, db_r[jj]);
-        atomicAdd(p.dbih + bi + H, db_z[jj]);
-        atomicAdd(p.dbih + bi + 2 * H, db_n[jj]);
-        atomicAdd(p.dbhh + bi, db_r[jj]);
-        atomicAdd(p.dbhh + bi + H, db_z[jj]);
-        atomicAdd(p.dbhh + bi + 2 * H, db_hn[jj]);
+        atomicAdd(p.dbih + bi, db.r[jj]);
+        atomicAdd(p.dbih + bi + H, db.z[jj]);
+        atomicAdd(p.dbih + bi + 2 * H, db.n[jj]);
+        atomicAdd(p.dbhh + bi, db.r[jj]);
+        atomicAdd(p.dbhh + bi + H, db.z[jj]);
+        atomicAdd(p.dbhh + bi + 2 * H, db.hn[jj]);
       }
     }
   }
@@ -1968,28 +1802,19 @@ SB_DEVINL void wide_mma(const WideSmem& s, int Bp, int ngroups, int ring, int gc
   mbar_arrive(s.accfull);
 }
 
-// one-time setup shared by both wide kernels: zero the operand regions, barriers, resident groups
+// one-time setup shared by both wide kernels: zero the operand regions, barriers, cluster sync
 SB_DEVINL void wide_setup(const WideSmem& s, int ring_bytes, int wbytes, uint32_t csize,
                           const CUtensorMap* tm, const CUtensorMap* tw) {
-  const int tid = threadIdx.x;
-  for (int k = tid; k < (ring_bytes + wbytes) / 16; k += GRU_THREADS)
-    reinterpret_cast<uint4*>(s.ring)[k] = make_uint4(0, 0, 0, 0);
-  if (tid == 0) {
-    for (int i = 0; i < GRU_MAX_RING; ++i) {
-      mbar_init(&s.full[i], 1);
-      mbar_init(&s.empty[i], csize);
-    }
+  smem_zero(s.ring, ring_bytes + wbytes);
+  gru_init_barriers(tm, tw, true, [=] {
+    init_ring_bars(s.full, s.empty, csize);
     for (int i = 0; i < GRU_WIDE_MAX_WR; ++i) {
       mbar_init(&s.wfull[i], 1);
       mbar_init(&s.wempty[i], 1);
     }
     mbar_init(s.accfull, 128);
     mbar_init(s.wresbar, 1);
-    mbar_fence_init();
-    tma_prefetch_desc(tm);
-    tma_prefetch_desc(tw);
-  }
-  fence_proxy_async_smem();
+  });
 }
 
 template <int U, int NQ>
@@ -2016,10 +1841,8 @@ gru_fwd_wide_kernel(const __grid_constant__ CUtensorMap tm_d0,
   const uint32_t crank = cluster_rank(), csize = cluster_size();
   const int wrow0 = dir * 3 * H + j0;   // gate b of the slice: rows wrow0 + b * H of W_hh
 
-  wide_setup(s, ring_bytes, wbytes, csize, tm, &tm_w);
   if (tid < NW) s.scratch[tid] = p.bhh[dir * 3 * H + (tid / U) * H + j0 + tid % U];
-  __syncthreads();
-  cluster_sync_all();
+  wide_setup(s, ring_bytes, wbytes, csize, tm, &tm_w);
   unsigned int* ctr = p.barrier + dir * 32;
 
   if (warp == GRU_TMA_WARP) {
@@ -2055,33 +1878,20 @@ gru_fwd_wide_kernel(const __grid_constant__ CUtensorMap tm_d0,
     const int rsub = tid % RPT;
     const int uo = (tid / RPT) * GRU_UPT;
     const int ju = j0 + uo;
-    float hprev[NQ][GRU_UPT];
+    float hprev[NQ][GRU_UPT] = {};
     float bias[3][GRU_UPT];
-#pragma unroll
-    for (int g = 0; g < 3; ++g)
-#pragma unroll
-      for (int jj = 0; jj < GRU_UPT; ++jj) bias[g][jj] = s.scratch[g * U + uo + jj];
-#pragma unroll
-    for (int q = 0; q < NQ; ++q)
-#pragma unroll
-      for (int jj = 0; jj < GRU_UPT; ++jj) hprev[q][jj] = 0.f;
+    gru_load_bias(s.scratch + uo, U, bias);
     for (int step = 0; step < T; ++step) {
       const int t = dir == 0 ? step : (T - 1 - step);
       float gi[NQ][3][GRU_UPT];
 #pragma unroll
-      for (int q = 0; q < NQ; ++q) {
-        const int row = rsub + q * RPT;
-        if (row < Bp) {
-          const float* g = p.gi + ((long long)t * Bp + row) * (p.ndir * 3 * H) + dir * 3 * H + ju;
-#pragma unroll
-          for (int gg = 0; gg < 3; ++gg) ld8(g + gg * H, gi[q][gg]);
-        }
-      }
+      for (int q = 0; q < NQ; ++q)
+        if (rsub + q * RPT < Bp) gru_load_gi(p, t, rsub + q * RPT, dir, ju, gi[q]);
       if (step > 0) {
         mbar_wait(s.accfull, (step - 1) & 1);
         if (tid == 0) GRU_STAMP(3);
       }
-      float rr[NQ][GRU_UPT], zz[NQ][GRU_UPT], nn[NQ][GRU_UPT], hn[NQ][GRU_UPT];
+      GruGates<GRU_UPT> gt[NQ];
       bool any = false;
 #pragma unroll
       for (int q = 0; q < NQ; ++q) {
@@ -2089,42 +1899,19 @@ gru_fwd_wide_kernel(const __grid_constant__ CUtensorMap tm_d0,
         if (row >= Bp) continue;
         any = true;
         const float* ar = s.accbuf + row * (NW + 4) + uo;
+        float acc[3][GRU_UPT];
 #pragma unroll
-        for (int jj = 0; jj < GRU_UPT; ++jj) {
-          const float a0 = step > 0 ? ar[jj] : 0.f;
-          const float a1 = step > 0 ? ar[U + jj] : 0.f;
-          const float a2 = step > 0 ? ar[2 * U + jj] : 0.f;
-          rr[q][jj] = fast_sigmoid(gi[q][0][jj] + a0 + bias[0][jj]);
-          zz[q][jj] = fast_sigmoid(gi[q][1][jj] + a1 + bias[1][jj]);
-          hn[q][jj] = a2 + bias[2][jj];
-          nn[q][jj] = fast_tanh(gi[q][2][jj] + rr[q][jj] * hn[q][jj]);
-          hprev[q][jj] = (1.f - zz[q][jj]) * nn[q][jj] + zz[q][jj] * hprev[q][jj];
-        }
-        const long long m = (long long)t * Bp + row;
-        *reinterpret_cast<uint4*>(p.xn + m * D + dir * H + ju) = pack8(hprev[q]);
+        for (int gg = 0; gg < 3; ++gg)
+#pragma unroll
+          for (int jj = 0; jj < GRU_UPT; ++jj) acc[gg][jj] = step > 0 ? ar[gg * U + jj] : 0.f;
+        gru_cell_fwd(gi[q], acc, bias, hprev[q], gt[q]);
+        st_bf16(p.xn + ((long long)t * Bp + row) * D + dir * H + ju, to_bf16(hprev[q]));
       }
-      if (tid == 0) GRU_STAMP(5);
-      if (any) fence_proxy_async_global();   // generic writes -> other CTAs' TMA reads
-      if (tid == 0) GRU_STAMP(6);
-      epi_barrier();
-      if (tid == 0) {
-        GRU_STAMP(7);
-        grid_arrive(ctr);
-        GRU_STAMP(9);
-      }
+      gru_publish(p, ctr, step, any, false);
 #pragma unroll
       for (int q = 0; q < NQ; ++q) {
         const int row = rsub + q * RPT;
-        if (row >= Bp) continue;
-        const long long m = (long long)t * Bp + row;
-        st8(p.y + m * D + dir * H + ju, hprev[q]);
-        if (p.gates) {
-          float* go = p.gates + ((m * p.ndir + dir) * 4) * H + ju;
-          st8(go, rr[q]);
-          st8(go + H, zz[q]);
-          st8(go + 2 * H, nn[q]);
-          st8(go + 3 * H, hn[q]);
-        }
+        if (row < Bp) gru_store_fwd(p, (long long)t * Bp + row, dir, ju, hprev[q], gt[q]);
       }
       if (tid == 0) GRU_STAMP(10);
     }
@@ -2153,7 +1940,6 @@ gru_bwd_wide_kernel(const __grid_constant__ CUtensorMap tm_d0,
   const int wbytes = gru_wide_wbytes(rg, wr, gc * WCHUNK, Bp);
   const WideSmem s = wide_carve(smem_raw, ring_bytes, rg, gc * WCHUNK, wbytes, U);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int D = p.ndir * H;
   const CUtensorMap* tm = dir == 0 ? &tm_d0 : &tm_d1;
   const uint32_t crank = cluster_rank(), csize = cluster_size();
   const int wrow0 = dir * H + j0;       // rows of W_hh^T: the CTA's units
@@ -2169,8 +1955,6 @@ gru_bwd_wide_kernel(const __grid_constant__ CUtensorMap tm_d0,
   }
   fence_proxy_async_global();   // generic writes -> this CTA's TMA reads
   wide_setup(s, ring_bytes, wbytes, csize, tm, &tm_w);
-  __syncthreads();
-  cluster_sync_all();
   unsigned int* ctr = p.barrier + dir * 32;
 
   if (warp == GRU_TMA_WARP) {
@@ -2203,47 +1987,21 @@ gru_bwd_wide_kernel(const __grid_constant__ CUtensorMap tm_d0,
     const int rsub = tid % RPT;
     const int uo = (tid / RPT) * GRU_UPT;
     const int ju = j0 + uo;
-    float dh_rec[NQ][GRU_UPT];
-    float db_r[NQ][GRU_UPT], db_z[NQ][GRU_UPT], db_n[NQ][GRU_UPT], db_hn[NQ][GRU_UPT];
-#pragma unroll
-    for (int q = 0; q < NQ; ++q)
-#pragma unroll
-      for (int jj = 0; jj < GRU_UPT; ++jj) {
-        dh_rec[q][jj] = 0.f; db_r[q][jj] = 0.f; db_z[q][jj] = 0.f; db_n[q][jj] = 0.f;
-        db_hn[q][jj] = 0.f;
-      }
+    float dh_rec[NQ][GRU_UPT] = {};
+    GruGates<GRU_UPT> db[NQ] = {};
 
     for (int step = 0; step < T; ++step) {
       const int t = dir == 0 ? (T - 1 - step) : step;
-      const int tp = dir == 0 ? t - 1 : t + 1;
-      const bool has_prev = dir == 0 ? (t > 0) : (t < T - 1);
-      bf16* xb = p.xchg + ((long long)(dir * 2 + (step & 1)) * Bp) * K3;
-      // saved activations of this step: independent of the recurrence, fetched first
-      float rr[NQ][GRU_UPT], zz[NQ][GRU_UPT], nn[NQ][GRU_UPT], hn[NQ][GRU_UPT];
+      GruGates<GRU_UPT> sv[NQ];
       float dh[NQ][GRU_UPT], hp[NQ][GRU_UPT];
 #pragma unroll
-      for (int q = 0; q < NQ; ++q) {
-        const int row = rsub + q * RPT;
-        if (row >= Bp) continue;
-        const long long m = (long long)t * Bp + row;
-        const float* go = p.gates + ((m * p.ndir + dir) * 4) * H + ju;
-        ld8(go, rr[q]);
-        ld8(go + H, zz[q]);
-        ld8(go + 2 * H, nn[q]);
-        ld8(go + 3 * H, hn[q]);
-        ld8(p.dy + m * D + dir * H + ju, dh[q]);
-        if (has_prev) {
-          ld8(p.y + ((long long)tp * Bp + row) * D + dir * H + ju, hp[q]);
-        } else {
-#pragma unroll
-          for (int jj = 0; jj < GRU_UPT; ++jj) hp[q][jj] = 0.f;
-        }
-      }
+      for (int q = 0; q < NQ; ++q)
+        if (rsub + q * RPT < Bp) gru_load_saved(p, t, rsub + q * RPT, dir, ju, sv[q], dh[q], hp[q]);
       if (step > 0) {
         mbar_wait(s.accfull, (step - 1) & 1);
         if (tid == 0) GRU_STAMP(3);
       }
-      uint4 o_r[NQ], o_z[NQ], o_n[NQ], o_nr[NQ];   // this step's dgi / dghn rows, bf16
+      GruGatesBf16<GRU_UPT> d[NQ];
       bool any = false;
 #pragma unroll
       for (int q = 0; q < NQ; ++q) {
@@ -2251,50 +2009,18 @@ gru_bwd_wide_kernel(const __grid_constant__ CUtensorMap tm_d0,
         if (row >= Bp) continue;
         any = true;
         const float* ar = s.accbuf + row * (U + 4) + uo;
-        float dr[GRU_UPT], dz[GRU_UPT], dn[GRU_UPT], dnr[GRU_UPT];
+        if (step > 0) {
 #pragma unroll
-        for (int jj = 0; jj < GRU_UPT; ++jj) {
-          if (step > 0) dh_rec[q][jj] += ar[jj];
-          const float g = dh[q][jj] + dh_rec[q][jj];
-          dn[jj] = g * (1.f - zz[q][jj]) * (1.f - nn[q][jj] * nn[q][jj]);
-          dz[jj] = g * (hp[q][jj] - nn[q][jj]) * zz[q][jj] * (1.f - zz[q][jj]);
-          dr[jj] = dn[jj] * hn[q][jj] * rr[q][jj] * (1.f - rr[q][jj]);
-          dnr[jj] = dn[jj] * rr[q][jj];
-          dh_rec[q][jj] = g * zz[q][jj];
-          db_r[q][jj] += dr[jj];
-          db_z[q][jj] += dz[jj];
-          db_n[q][jj] += dn[jj];
-          db_hn[q][jj] += dnr[jj];
+          for (int jj = 0; jj < GRU_UPT; ++jj) dh_rec[q][jj] += ar[jj];
         }
-        o_r[q] = pack8(dr); o_z[q] = pack8(dz); o_n[q] = pack8(dn); o_nr[q] = pack8(dnr);
-        if (step + 1 < T) {
-          bf16* x = xb + (long long)row * K3 + ju;
-          *reinterpret_cast<uint4*>(x) = o_r[q];
-          *reinterpret_cast<uint4*>(x + H) = o_z[q];
-          *reinterpret_cast<uint4*>(x + 2 * H) = o_nr[q];
-        }
+        d[q] = gru_cell_bwd(dh[q], dh_rec[q], sv[q], hp[q], db[q]);
+        if (step + 1 < T) gru_store_xchg(p, step, row, dir, ju, d[q]);
       }
-      if (step + 1 < T) {
-        if (tid == 0) GRU_STAMP(5);
-        if (any) fence_proxy_async_global();
-        if (tid == 0) GRU_STAMP(6);
-        epi_barrier();
-        if (tid == 0) {
-          GRU_STAMP(7);
-          grid_arrive(ctr);
-          GRU_STAMP(9);
-        }
-      }
+      if (step + 1 < T) gru_publish(p, ctr, step, any, false);
 #pragma unroll
       for (int q = 0; q < NQ; ++q) {
         const int row = rsub + q * RPT;
-        if (row >= Bp) continue;
-        const long long m = (long long)t * Bp + row;
-        bf16* o = p.dgi + m * (p.ndir * K3) + dir * K3 + ju;
-        st_stream_u4(o, o_r[q]);
-        st_stream_u4(o + H, o_z[q]);
-        st_stream_u4(o + 2 * H, o_n[q]);
-        st_stream_u4(p.dghn + m * D + dir * H + ju, o_nr[q]);
+        if (row < Bp) gru_store_bwd(p, (long long)t * Bp + row, dir, ju, d[q]);
       }
       if (tid == 0) GRU_STAMP(10);
     }
@@ -2308,10 +2034,10 @@ gru_bwd_wide_kernel(const __grid_constant__ CUtensorMap tm_d0,
       const bool active = rsub + q * RPT < Bp;
 #pragma unroll
       for (int jj = 0; jj < GRU_UPT; ++jj) {
-        const float a = warp_sum(active ? db_r[q][jj] : 0.f);
-        const float b = warp_sum(active ? db_z[q][jj] : 0.f);
-        const float c = warp_sum(active ? db_n[q][jj] : 0.f);
-        const float d = warp_sum(active ? db_hn[q][jj] : 0.f);
+        const float a = warp_sum(active ? db[q].r[jj] : 0.f);
+        const float b = warp_sum(active ? db[q].z[jj] : 0.f);
+        const float c = warp_sum(active ? db[q].n[jj] : 0.f);
+        const float d = warp_sum(active ? db[q].hn[jj] : 0.f);
         if (lane == 0) {
           atomicAdd(&red[uo + jj], a);
           atomicAdd(&red[U + uo + jj], b);
@@ -2384,26 +2110,38 @@ static int gru_cluster_size(int nC) {
   return cs < 1 ? 1 : cs;
 }
 
-static int gru_launch(const void* kernel, int grid, int cs, size_t smem, void** args,
-                      cudaStream_t stream) {
-  if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) !=
-      cudaSuccess)
-    return SB_ERR_CUDA;
+// Launch configuration of a recurrence kernel: `grid` CTAs in clusters of cs.  Cooperative:
+// attrs = {cooperative, cluster}; otherwise attrs = {cluster}.
+static cudaLaunchConfig_t gru_launch_config(int grid, int cs, bool cooperative, size_t smem,
+                                            cudaStream_t stream, cudaLaunchAttribute (&attrs)[2]) {
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3(grid);
   cfg.blockDim = dim3(GRU_THREADS);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
-  cudaLaunchAttribute attrs[2];
-  attrs[0].id = cudaLaunchAttributeCooperative;
-  attrs[0].val.cooperative = 1;
-  attrs[1].id = cudaLaunchAttributeClusterDimension;
-  attrs[1].val.clusterDim.x = cs;
-  attrs[1].val.clusterDim.y = 1;
-  attrs[1].val.clusterDim.z = 1;
+  int n = 0;
+  if (cooperative) {
+    attrs[n].id = cudaLaunchAttributeCooperative;
+    attrs[n++].val.cooperative = 1;
+  }
+  attrs[n].id = cudaLaunchAttributeClusterDimension;
+  attrs[n].val.clusterDim.x = cs;
+  attrs[n].val.clusterDim.y = 1;
+  attrs[n].val.clusterDim.z = 1;
   cfg.attrs = attrs;
-  cfg.numAttrs = 2;
+  cfg.numAttrs = n + 1;
+  return cfg;
+}
+
+// cooperative launch over clusters of at most cs CTAs
+static int gru_launch(const void* kernel, int grid, int cs, size_t smem, void** args,
+                      cudaStream_t stream) {
+  if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) !=
+      cudaSuccess)
+    return SB_ERR_CUDA;
+  cudaLaunchAttribute attrs[2];
+  cudaLaunchConfig_t cfg = gru_launch_config(grid, cs, true, smem, stream, attrs);
   // all CTAs must be co-resident (grid barrier): shrink the cluster until the grid fits
   if (cs > 1 &&
       cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 0) != cudaSuccess)
@@ -2459,22 +2197,11 @@ static int gru_launch_exact(const void* kernel, int grid, int cs, size_t smem, v
     cudaGetLastError();
     return SB_ERR_CUDA;
   }
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(GRU_THREADS);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
   // Clustered launches are NOT flagged cooperative: co-residency of the whole grid is established
   // by the occupancy query below (1 CTA per SM, grid <= resident capacity), every spin-wait in
   // the kernels is bounded, and Nsight Compute cannot replay cooperative+cluster launches.
-  cudaLaunchAttribute attrs[1];
-  attrs[0].id = cudaLaunchAttributeClusterDimension;
-  attrs[0].val.clusterDim.x = cs;
-  attrs[0].val.clusterDim.y = 1;
-  attrs[0].val.clusterDim.z = 1;
-  cfg.attrs = attrs;
-  cfg.numAttrs = 1;
+  cudaLaunchAttribute attrs[2];
+  const cudaLaunchConfig_t cfg = gru_launch_config(grid, cs, false, smem, stream, attrs);
   int nclusters = 0;
   if (cudaOccupancyMaxActiveClusters(&nclusters, kernel, &cfg) != cudaSuccess ||
       nclusters * cs < grid) {
@@ -2575,10 +2302,10 @@ extern "C" int sb_debug_gru_timeline(void* dev_buffer) {
   sb::g_gru_dbg = reinterpret_cast<unsigned long long*>(dev_buffer);
   return SB_OK;
 }
-// developer knobs: 1 / 2: gru_fwd_kernel and the gru_*_ks_kernel without the proxy fence / the
-// off-path stores (timing only: results become wrong); 8 / 16: never / always use the
-// transposed-accumulator K-split kernels (default: by batch size, see gru_use_kt); 32: disable
-// the K-split forward kernels;
+// developer knobs: 1 / 2: the recurrence kernels without the proxy fence / the off-path stores
+// (timing only: results become wrong; see gru_publish, gru_store_fwd); 8 / 16: never / always
+// use the transposed-accumulator K-split kernels (default: by batch size, see gru_use_kt); 32:
+// disable the K-split forward kernels;
 // 64 / 128: polling mode of the grid barrier in the K-split kernels (see grid_wait);
 // 256 / 512: always (wherever the K-split backward kernel applies) / never use its L2
 // reduce-scatter mode (see ks_exchange and sb_gru_bwd); 1024: the K-split forward over 2-CTA
@@ -2726,12 +2453,9 @@ extern "C" int sb_gru_plan(int Bp, int H, int ndir, int* Hp) {
   return SB_ERR_UNSUPPORTED;
 }
 
-// workspace of one recurrence launch: [0,1024) the per-direction grid-barrier words, then the
-// exchange buffers of the backward kernels
-static size_t gru_ws_counters_bytes(int ndir) {
-  (void)ndir;
-  return 1024;
-}
+// workspace of one recurrence launch: [0,1024) the per-direction grid-barrier words (one L2 line
+// each), then the exchange buffers of the backward kernels
+static constexpr size_t GRU_WS_COUNTERS = 1024;
 
 // The L2 reduce-scatter of the K-split backward kernel (ks_exchange), at the END of its
 // workspace: one counter line per direction and group of 4 CTAs, then the staging area, two
@@ -2752,11 +2476,42 @@ static size_t gru_fwd_ks_smem(int ks, int Bp, int H) {
   return nq * Bp * 128 + nq * (3 * ks * GRU_HC) * 128 + (size_t)2 * ks * Bp * 3 * GRU_HC * 4 +
          1024 + 512;
 }
+// gru_fwd_kt_kernel: the K quarter of h_{t-1} and of the 192 weight rows, recv + stage
+// ([4 + 3][48][Bp + 4] fp32), barriers and bias, alignment.
+static size_t gru_fwd_kt_smem(int Bp, int H) {
+  const size_t nq = (size_t)H / KS / 64;
+  return nq * Bp * 128 + nq * (3 * KS * GRU_HC) * 128 +
+         (size_t)(2 * KS - 1) * 3 * GRU_HC * (Bp + 4) * 4 + 1024 + 512;
+}
+// gru_bwd_ks_kernel: the K quarter of dgh_t (3H / 4 columns) and of the 64 weight rows, recv +
+// stage ([4][Bp][16] fp32 each), barriers, alignment.
+static size_t gru_bwd_ks_smem(int Bp, int H) {
+  const size_t nq = (size_t)3 * H / KS / 64;
+  return nq * Bp * 128 + nq * (KS * GRU_HC) * 128 + (size_t)2 * KS * Bp * GRU_HC * 4 + 1024 + 256;
+}
+// gru_bwd_kt_kernel: as gru_bwd_ks_kernel, with recv + stage [4 + 3][16][Bp + 4] fp32.
+static size_t gru_bwd_kt_smem(int Bp, int H) {
+  const size_t nq = (size_t)3 * H / KS / 64;
+  return nq * Bp * 128 + nq * (KS * GRU_HC) * 128 + (size_t)(2 * KS - 1) * GRU_HC * (Bp + 4) * 4 +
+         1024 + 256;
+}
+
+// The two per-direction tensor maps of a gathered operand (boxes of Bp rows): direction d's
+// [rows x cols] matrix (pitch ld) starts d * dir_stride elements after `base`; a one-direction
+// layer maps direction 0 twice.
+static int gru_dir_tmaps(CUtensorMap* tm, const bf16* base, size_t dir_stride, long long rows,
+                         long long cols, long long ld, int ndir, int Bp) {
+  for (int d = 0; d < 2; ++d) {
+    const int rc = make_tmap_bf16_2d(&tm[d], base + (d < ndir ? d : 0) * dir_stride, rows, cols,
+                                     ld, Bp);
+    if (rc != SB_OK) return rc;
+  }
+  return SB_OK;
+}
 
 extern "C" int sb_gru_fwd_workspace_size(int Bp, int H, int ndir, size_t* bytes) {
   if (!bytes || Bp <= 0 || H <= 0 || (ndir != 1 && ndir != 2)) return SB_ERR_INVALID;
-  (void)Bp;
-  *bytes = gru_ws_counters_bytes(ndir);      // the forward kernels exchange h_t through xn itself
+  *bytes = GRU_WS_COUNTERS;      // the forward kernels exchange h_t through xn itself
   return SB_OK;
 }
 
@@ -2786,15 +2541,11 @@ extern "C" int sb_gru_fwd(const float* gi, const void* whh_bf16, const float* bh
     memset(&p, 0, sizeof(p));
     p.gi = gi; p.whh = reinterpret_cast<const bf16*>(whh_bf16); p.bhh = bhh; p.y = y;
     p.xn = reinterpret_cast<bf16*>(xn_bf16); p.gates = gates; p.barrier = barrier;
-    p.T = T; p.Bp = Bp; p.H = H; p.ndir = ndir; p.dbg = g_gru_dbg;
+    p.T = T; p.Bp = Bp; p.H = H; p.ndir = ndir; p.dbg = g_gru_dbg; p.ablate = g_gru_ablate & 3;
     p.ring = w.ring; p.gc = w.gc; p.rg = w.rg; p.wr = w.wr;
     CUtensorMap tm[3];
-    for (int d = 0; d < 2; ++d) {
-      const int dd = d < ndir ? d : 0;
-      rc = make_tmap_bf16_2d(&tm[d], p.xn + (size_t)dd * H, (long long)T * Bp, H,
-                             (long long)ndir * H, Bp);
-      if (rc != SB_OK) return rc;
-    }
+    rc = gru_dir_tmaps(tm, p.xn, H, (long long)T * Bp, H, (long long)ndir * H, ndir, Bp);
+    if (rc != SB_OK) return rc;
     rc = make_tmap_bf16_2d(&tm[2], p.whh, (long long)ndir * 3 * H, H, H, w.U);
     if (rc != SB_OK) return rc;
     void* args[] = {(void*)&tm[0], (void*)&tm[1], (void*)&tm[2], (void*)&p};
@@ -2820,24 +2571,18 @@ extern "C" int sb_gru_fwd(const float* gi, const void* whh_bf16, const float* bh
   if (!(g_gru_ablate & 32) && H % 128 == 0 && Bp <= 64) {
     GruFwdParams q;
     q.gi = gi; q.whh = reinterpret_cast<const bf16*>(whh_bf16); q.bhh = bhh; q.y = y;
-    q.xn = reinterpret_cast<bf16*>(xn_bf16); q.xnT = nullptr; q.gates = gates;
+    q.xn = reinterpret_cast<bf16*>(xn_bf16); q.gates = gates;
     q.barrier = barrier; q.T = T; q.Bp = Bp; q.H = H; q.ndir = ndir;
     q.dbg = g_gru_dbg; q.ablate = g_gru_ablate & 195; q.gc = 1;
     CUtensorMap tq[2];
-    for (int d = 0; d < 2; ++d) {
-      const int dd = d < ndir ? d : 0;
-      rc = make_tmap_bf16_2d(&tq[d], q.xn + (size_t)dd * H, (long long)T * Bp, H,
-                             (long long)ndir * H, Bp);
-      if (rc != SB_OK) return rc;
-    }
+    rc = gru_dir_tmaps(tq, q.xn, H, (long long)T * Bp, H, (long long)ndir * H, ndir, Bp);
+    if (rc != SB_OK) return rc;
     void* kargs[] = {(void*)&tq[0], (void*)&tq[1], (void*)&q};   // q is copied at launch
     if (!(g_gru_ablate & 1024) && H % 256 == 0) {
-      const int nq = H / KS / 64;
       const size_t ks_smem = gru_fwd_ks_smem(KS, Bp, H);   // KS = 4
-      q.ring = nq;
+      q.ring = H / KS / 64;
       if (ks_smem <= 227 * 1024) {
-        const size_t kt_smem = (size_t)nq * Bp * 128 + (size_t)nq * 192 * 128 +
-                               (size_t)(2 * KS - 1) * 48 * (Bp + 4) * 4 + 1024 + 512;
+        const size_t kt_smem = gru_fwd_kt_smem(Bp, H);
         if (gru_use_kt(Bp, false) && kt_smem <= 227 * 1024) {
           const void* kt = Bp > 32   ? (const void*)gru_fwd_kt_kernel<4>
                            : Bp > 16 ? (const void*)gru_fwd_kt_kernel<2>
@@ -2866,18 +2611,14 @@ extern "C" int sb_gru_fwd(const float* gi, const void* whh_bf16, const float* bh
   // ---- every other shape: each CTA gathers all of h_{t-1} (tensor-map TMA, cluster multicast) ----
   GruFwdParams p;
   p.gi = gi; p.whh = reinterpret_cast<const bf16*>(whh_bf16); p.bhh = bhh; p.y = y;
-  p.xn = reinterpret_cast<bf16*>(xn_bf16); p.xnT = nullptr;
+  p.xn = reinterpret_cast<bf16*>(xn_bf16);
   p.gates = gates; p.barrier = barrier; p.T = T; p.Bp = Bp; p.H = H; p.ndir = ndir;
   p.dbg = g_gru_dbg;
   p.ablate = g_gru_ablate & 31;
   p.ring = ring; p.gc = gc;
   CUtensorMap tm[2];
-  for (int d = 0; d < 2; ++d) {
-    const int dd = d < ndir ? d : 0;
-    rc = make_tmap_bf16_2d(&tm[d], p.xn + (size_t)dd * H, (long long)T * Bp, H,
-                           (long long)ndir * H, Bp);
-    if (rc != SB_OK) return rc;
-  }
+  rc = gru_dir_tmaps(tm, p.xn, H, (long long)T * Bp, H, (long long)ndir * H, ndir, Bp);
+  if (rc != SB_OK) return rc;
   void* args[] = {(void*)&tm[0], (void*)&tm[1], (void*)&p};
   rc = gru_launch((const void*)gru_fwd_kernel, ndir * nC, gru_cluster_size(nC), smem, args,
                   stream);
@@ -2890,7 +2631,7 @@ extern "C" int sb_gru_fwd(const float* gi, const void* whh_bf16, const float* bh
 static size_t gru_bwd_ws_base(int Bp, int H, int ndir) {
   const size_t k3p = (size_t)((3 * H + 63) / 64) * 64;
   size_t z = 0;
-  return gru_ws_counters_bytes(ndir) + (size_t)ndir * 2 * Bp * k3p * sizeof(bf16) + 1024 +
+  return GRU_WS_COUNTERS + (size_t)ndir * 2 * Bp * k3p * sizeof(bf16) + 1024 +
          gru_rs_bytes(Bp, H, ndir, &z);
 }
 
@@ -2926,7 +2667,7 @@ extern "C" int sb_gru_bwd(const float* dy, const float* y, const float* gates,
   p.dgi = reinterpret_cast<bf16*>(dgi_bf16);
   p.dghn = reinterpret_cast<bf16*>(dghn_bf16);
   p.barrier = reinterpret_cast<unsigned int*>(ws);
-  p.xchg = reinterpret_cast<bf16*>(ws + gru_ws_counters_bytes(ndir));
+  p.xchg = reinterpret_cast<bf16*>(ws + GRU_WS_COUNTERS);
   p.dbih = dbih; p.dbhh = dbhh; p.T = T; p.Bp = Bp; p.H = H; p.ndir = ndir;
   p.dbg = g_gru_dbg;
   p.dir0 = 0;
@@ -2948,11 +2689,8 @@ extern "C" int sb_gru_bwd(const float* dy, const float* y, const float* gates,
     p.whhT = reinterpret_cast<bf16*>(ws + (gru_bwd_ws_base(Bp, H, ndir) + 1023) / 1024 * 1024);
     p.ring = w.ring; p.gc = w.gc; p.rg = w.rg; p.wr = w.wr;
     CUtensorMap tm[3];
-    for (int d = 0; d < 2; ++d) {
-      const int dd = d < ndir ? d : 0;
-      rc = make_tmap_bf16_2d(&tm[d], p.xchg + (size_t)dd * 2 * Bp * K3, 2LL * Bp, K3, K3, Bp);
-      if (rc != SB_OK) return rc;
-    }
+    rc = gru_dir_tmaps(tm, p.xchg, (size_t)2 * Bp * K3, 2LL * Bp, K3, K3, ndir, Bp);
+    if (rc != SB_OK) return rc;
     rc = make_tmap_bf16_2d(&tm[2], p.whhT, (long long)ndir * H, K3, K3, w.U);
     if (rc != SB_OK) return rc;
     void* args[] = {(void*)&tm[0], (void*)&tm[1], (void*)&tm[2], (void*)&p};
@@ -2965,20 +2703,14 @@ extern "C" int sb_gru_bwd(const float* dy, const float* y, const float* gates,
   }
   // ---- preferred: K-split over 4-CTA clusters ----
   if (g_gru_ksplit && H % 256 == 0 && nC_ % KS == 0 && (K3 / KS / 64) <= 16) {
-    const int nq = K3 / KS / 64;
-    const size_t ks_smem = (size_t)nq * Bp * 128 + (size_t)nq * 64 * 128 +
-                           (size_t)2 * KS * Bp * 64 + 1024 + 256;
+    const size_t ks_smem = gru_bwd_ks_smem(Bp, H);
     if (ks_smem <= 227 * 1024) {
       CUtensorMap tq[2];
-      for (int d = 0; d < 2; ++d) {
-        const int dd = d < ndir ? d : 0;
-        rc = make_tmap_bf16_2d(&tq[d], p.xchg + (size_t)dd * 2 * Bp * K3, 2LL * Bp, K3, K3, Bp);
-        if (rc != SB_OK) return rc;
-      }
-      p.ring = nq; p.gc = 1;
+      rc = gru_dir_tmaps(tq, p.xchg, (size_t)2 * Bp * K3, 2LL * Bp, K3, K3, ndir, Bp);
+      if (rc != SB_OK) return rc;
+      p.ring = K3 / KS / 64; p.gc = 1;
       void* kargs[] = {(void*)&tq[0], (void*)&tq[1], (void*)&p};
-      const size_t kt_smem = (size_t)nq * Bp * 128 + (size_t)nq * 64 * 128 +
-                             (size_t)(2 * KS - 1) * GRU_HC * (Bp + 4) * 4 + 1024 + 256;
+      const size_t kt_smem = gru_bwd_kt_smem(Bp, H);
       if (gru_use_kt(Bp, true) && !(g_gru_ablate & 256) && Bp <= 64 && kt_smem <= 227 * 1024) {
         const void* kt = Bp > 32   ? (const void*)gru_bwd_kt_kernel<4>
                          : Bp > 16 ? (const void*)gru_bwd_kt_kernel<2>
@@ -3021,11 +2753,8 @@ extern "C" int sb_gru_bwd(const float* dy, const float* y, const float* gates,
   if (p.ring < 0) return SB_ERR_UNSUPPORTED;
   // per direction: the two parity buffers stacked as [2*Bp rows][3H cols]
   CUtensorMap tm[2];
-  for (int d = 0; d < 2; ++d) {
-    const int dd = d < ndir ? d : 0;
-    rc = make_tmap_bf16_2d(&tm[d], p.xchg + (size_t)dd * 2 * Bp * K3, 2LL * Bp, K3, K3, Bp);
-    if (rc != SB_OK) return rc;
-  }
+  rc = gru_dir_tmaps(tm, p.xchg, (size_t)2 * Bp * K3, 2LL * Bp, K3, K3, ndir, Bp);
+  if (rc != SB_OK) return rc;
   void* args[] = {(void*)&tm[0], (void*)&tm[1], (void*)&p};
   const int nC = H / GRU_HC;
   rc = gru_launch((const void*)gru_bwd_kernel, ndir * nC, gru_cluster_size(nC), smem, args,
