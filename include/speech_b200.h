@@ -53,6 +53,23 @@ int sb_ctc_fwd_bwd(const float* acts, float* grads, const int* labels, const int
                    int max_label_len, float* costs, void* workspace, size_t workspace_bytes,
                    void* stream);
 
+/* Any vocabulary size (csrc/ctc.cu).  The fused kernel above keeps per-class occupancies [4][V] in
+ * shared memory next to the lattice rows; shapes where it does not fit (both its staged and its
+ * unstaged layouts over 220 KB: V above about 13,000 at T = 247, about 9,900 with 512 to 1023
+ * labels) take a compact path inside sb_ctc_fwd_bwd, and every other shape keeps the fused kernel.
+ * The compact path reduces each frame, over many CTAs, to Vc = max_label_len + 2 columns (blank,
+ * the utterance's distinct label classes, and the log-sum-exp of every other class), runs the same
+ * fused kernel on them, and expands the gradient (softmax for the classes left out).  Same costs and
+ * gradients up to float32 rounding; max_label_len <= 1023 as above.
+ *   sb_ctc_fwd_bwd_compact         the compact path at any shape (same arguments as sb_ctc_fwd_bwd)
+ *   sb_ctc_compact_workspace_size  its workspace; sb_ctc_workspace_size returns this size exactly
+ *                                  for the shapes where sb_ctc_fwd_bwd takes the compact path */
+int sb_ctc_compact_workspace_size(int B, int T, int V, int max_label_len, size_t* bytes);
+int sb_ctc_fwd_bwd_compact(const float* acts, float* grads, const int* labels,
+                           const int* label_offsets, const int* label_lens, const int* act_lens,
+                           int B, int T, int V, int blank, int max_label_len, float* costs,
+                           void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---------------------------------------------------------------------------------------
  * Dense contraction on wgmma tensor cores:
  *     C[M,N] (f32)  (+)=  A[M,K] (bf16, row-major) * B[N,K]^T (bf16, row-major)  (+ bias[N])
@@ -161,11 +178,23 @@ int sb_time_align(const void* src, long long ld_src, void* dst, long long ld_dst
  *   out_scores  (B) float64: negative log-likelihood of that prefix (ctc_decoder.py:112-113)
  * beam_size <= 32.  Lattice arithmetic is float64, ties are broken like the reference's
  * stable sort over dict insertion order.
+ * Any S: where the K*S + K candidates of a frame do not fit in shared memory (K*(S+1)*13 bytes over
+ * 200 KB), sb_ctc_prefix_beam runs the shortlist search; every other shape keeps the full scan.
+ *   sb_ctc_prefix_beam_shortlist  the shortlist search at any shape (same arguments): a pre-pass
+ *       writes each frame's 2K+1 most probable non-blank symbols, and each entry scores only those,
+ *       its own last symbol and its stay candidate; a per-frame bound check (csrc/decode.cu) falls
+ *       back to a full scan of the frame where it cannot prove the selection complete.  Hypotheses,
+ *       lengths and float64 scores are bit-identical to the full scan.
+ * The workspace size has no S argument, so it always includes the shortlists, B*T*(2K+1) ints.
  * ------------------------------------------------------------------------------------- */
 int sb_ctc_prefix_beam_workspace_size(int B, int T, int beam_size, size_t* bytes);
 int sb_ctc_prefix_beam(const float* logp, const int* lens, int B, int T, int S, int beam_size,
                        int blank, int* out_labels, int* out_lens, double* out_scores,
                        void* workspace, size_t workspace_bytes, void* stream);
+int sb_ctc_prefix_beam_shortlist(const float* logp, const int* lens, int B, int T, int S,
+                                 int beam_size, int blank, int* out_labels, int* out_lens,
+                                 double* out_scores, void* workspace, size_t workspace_bytes,
+                                 void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Conv2d(+ReLU) front-end as im2col + sb_gemm_bf16_tn.

@@ -23,11 +23,17 @@ SIGNATURES = {
     "sb_ctc_workspace_size": (_c_int, [_c_int, _c_int, _c_int, _c_int, ctypes.POINTER(_c_sz)]),
     "sb_ctc_fwd_bwd": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _c_int, _c_int, _c_int, _c_int,
                                 _c_int, _vp, _vp, _c_sz, _vp]),
+    "sb_ctc_compact_workspace_size": (_c_int, [_c_int, _c_int, _c_int, _c_int,
+                                               ctypes.POINTER(_c_sz)]),
+    "sb_ctc_fwd_bwd_compact": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _c_int, _c_int, _c_int,
+                                        _c_int, _c_int, _vp, _vp, _c_sz, _vp]),
     "sb_gemm_bf16_tn": (_c_int, [_vp, _c_ll, _vp, _c_ll, _vp, _c_ll, _vp, _c_int, _c_int, _c_int,
                                  _c_int, _c_int, _c_int, _c_int, _c_int, _vp]),
     "sb_ctc_prefix_beam_workspace_size": (_c_int, [_c_int, _c_int, _c_int, ctypes.POINTER(_c_sz)]),
     "sb_ctc_prefix_beam": (_c_int, [_vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int, _vp, _vp, _vp,
                                     _vp, _c_sz, _vp]),
+    "sb_ctc_prefix_beam_shortlist": (_c_int, [_vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int,
+                                              _vp, _vp, _vp, _vp, _c_sz, _vp]),
     "sb_conv_im2col": (_c_int, [_vp, _vp, _fl, _vp, _c_int, _c_int, _c_int, _c_int, _c_int, _c_int,
                                 _c_int, _c_int, _c_int, _vp]),
     "sb_conv_relu_to_bct": (_c_int, [_vp, _vp, _fl, _vp, _c_int, _c_int, _c_int, _c_int, _vp]),

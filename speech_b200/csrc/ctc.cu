@@ -375,50 +375,34 @@ static int ctc_ns_for(int max_label_len) {
   return -1;
 }
 
-}  // namespace sb
-
-using namespace sb;
-
-extern "C" int sb_ctc_workspace_size(int B, int T, int V, int max_label_len, size_t* bytes) {
-  if (!bytes || B <= 0 || T < 0 || V <= 0 || max_label_len < 0) return SB_ERR_INVALID;
-  const int ns = ctc_ns_for(max_label_len);
-  if (ns < 0) return SB_ERR_UNSUPPORTED;
-  const size_t Tn = (size_t)(T > 0 ? T : 1);
-  *bytes = (size_t)B * Tn * (size_t)(ns * CTC_SIDE) * sizeof(float) + (size_t)B * Tn * sizeof(double) + 512;
-  return SB_OK;
+// Shared memory of the fused kernel: lattice rows, occupancies occ[4][V], reduction scratch, and
+// either the staged (T x V) log-softmax or the per-frame log-sum-exp.
+static constexpr size_t CTC_SMEM_LIMIT = 220 * 1024;
+static size_t ctc_fixed_smem(int ns, int V) {
+  return (size_t)(4 * (ns * CTC_SIDE + 4)) * sizeof(double) + (size_t)(4 * V + 64) * sizeof(float) + 8;
+}
+static bool ctc_staged(int ns, int T, int V) {
+  return ctc_fixed_smem(ns, V) + (size_t)T * V * sizeof(float) <= CTC_SMEM_LIMIT;
+}
+// true where the fused kernel holds the shape (staged or not); every other shape takes the compact path
+static bool ctc_fused_fits(int ns, int T, int V) {
+  return ctc_staged(ns, T, V) || ctc_fixed_smem(ns, V) + (size_t)T * sizeof(float) <= CTC_SMEM_LIMIT;
 }
 
-extern "C" int sb_ctc_fwd_bwd(const float* acts, float* grads, const int* labels_dev,
-                              const int* label_offsets_dev, const int* label_lens_dev,
-                              const int* act_lens_dev, int B, int T, int V, int blank,
-                              int max_label_len, float* costs, void* workspace,
-                              size_t workspace_bytes, void* stream_) {
-  if (!acts || !labels_dev || !label_offsets_dev || !label_lens_dev || !act_lens_dev || !costs ||
-      !workspace)
-    return SB_ERR_INVALID;
-  if (B <= 0 || T <= 0 || V <= 0 || blank < 0 || blank >= V) return SB_ERR_INVALID;
-  size_t need = 0;
-  int rc = sb_ctc_workspace_size(B, T, V, max_label_len, &need);
-  if (rc != SB_OK) return rc;
-  if (workspace_bytes < need) return SB_ERR_WORKSPACE;
-  const int ns = ctc_ns_for(max_label_len);
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+static size_t ctc_fused_ws_bytes(int B, int T, int ns) {
+  const size_t Tn = (size_t)(T > 0 ? T : 1);
+  return (size_t)B * Tn * (size_t)(ns * CTC_SIDE) * sizeof(float) + (size_t)B * Tn * sizeof(double) + 512;
+}
 
-  CtcParams p;
-  p.acts = acts; p.grads = grads; p.labels = labels_dev; p.label_off = label_offsets_dev;
-  p.label_lens = label_lens_dev; p.act_lens = act_lens_dev; p.costs = costs;
+// the fused kernel at (B, T, p.V); p.offs / p.ws are carved from `workspace`
+static int ctc_run_fused(CtcParams p, int ns, void* workspace, cudaStream_t stream) {
+  const int B = p.B, T = p.T, V = p.V;
   p.offs = reinterpret_cast<double*>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
   p.ws = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(p.offs + (size_t)B * T) + 255) & ~(uintptr_t)255);
-  p.B = B; p.T = T; p.V = V; p.blank = blank; p.S_stride = ns * CTC_SIDE;
-
-  const size_t fixed = (size_t)(4 * (ns * CTC_SIDE + 4)) * sizeof(double) +
-                       (size_t)(4 * V + 64) * sizeof(float) + 8;
-  const size_t staged_bytes = fixed + (size_t)T * V * sizeof(float);
-  const size_t unstaged_bytes = fixed + (size_t)T * sizeof(float);
-  const size_t limit = 220 * 1024;
-  const bool staged = staged_bytes <= limit;
-  if (!staged && unstaged_bytes > limit) return SB_ERR_UNSUPPORTED;
-  const size_t smem = staged ? staged_bytes : unstaged_bytes;
+  p.S_stride = ns * CTC_SIDE;
+  if (!ctc_fused_fits(ns, T, V)) return SB_ERR_UNSUPPORTED;
+  const bool staged = ctc_staged(ns, T, V);
+  const size_t smem = ctc_fixed_smem(ns, V) + (size_t)T * (staged ? V : 1) * sizeof(float);
 
 #define SB_CTC_CASE(NSV)                                                      \
   case NSV:                                                                   \
@@ -432,4 +416,297 @@ extern "C" int sb_ctc_fwd_bwd(const float* acts, float* grads, const int* labels
   }
 #undef SB_CTC_CASE
   return SB_ERR_UNSUPPORTED;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Compact path (any V).  The lattice of utterance b reads only the blank, its own label classes and
+// each frame's log-sum-exp.  So each frame is reduced to Vc = max_label_len + 2 columns
+//   0 = blank, 1..D_b = the D_b distinct non-blank label classes (order of first occurrence),
+//   D_b + 1 = rest = log-sum-exp of the logits of every class outside that set (-inf if none),
+//   D_b + 2 .. Vc - 1 = -inf (padding: no mass, zero gradient),
+// whose log-softmax equals the full row's at the kept classes; the unchanged fused kernel then runs
+// on the compact rows with blank = 0 and the labels remapped to columns.  The gradient of a class
+// outside the set is its softmax (its occupancy is 0), that of a kept class the compact gradient of
+// its column.  Labels equal to the blank class map to column 0, as the fused kernel treats them.
+// ------------------------------------------------------------------------------------------------
+static constexpr int CTC_CMP_THREADS = 256;
+static constexpr int CTC_CMP_ROWS = 32;   // frames per CTA of the row kernels (one warp per frame)
+
+struct CtcCompact {
+  const float* acts;     // (B, T, V)
+  float* grads;          // (B, T, V) or nullptr
+  const int* labels;
+  const int* label_off;
+  const int* label_lens;
+  const int* act_lens;
+  const float* costs;    // (B) written by the fused kernel (read by the gradient expansion)
+  float* acts_c;         // (B, T, Vc)
+  const float* grads_c;  // (B, T, Vc)
+  float* lse;            // (B, T) full-row log-sum-exp
+  int* lab_c;            // (B, Lmax) labels as columns, utterance b at b * Lmax
+  int* off_c;            // (B) = b * Lmax
+  int* col_cls;          // (B, Vc) class of each column: >= 0 class, -1 rest, -2 padding
+  int* ncols;            // (B) D_b
+  int B, T, V, Vc, blank, Lmax;
+};
+
+// one CTA per utterance: dedupe the labels into columns (L <= 1023)
+__global__ void __launch_bounds__(CTC_CMP_THREADS) ctc_colmap_kernel(const CtcCompact p) {
+  __shared__ int first[1024];   // position of the first occurrence of label j's class
+  __shared__ int colid[1024];   // column of a first occurrence
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int L = min(p.label_lens[b], p.Lmax);
+  const int* lab = p.labels + p.label_off[b];
+  for (int j = tid; j < L; j += CTC_CMP_THREADS) {
+    const int c = lab[j];
+    int f = j;
+    for (int i = 0; i < j; ++i)
+      if (lab[i] == c) { f = i; break; }
+    first[j] = f;
+  }
+  __syncthreads();
+  int* cls = p.col_cls + (size_t)b * p.Vc;
+  if (tid == 0) {
+    int d = 0;
+    cls[0] = p.blank;
+    for (int j = 0; j < L; ++j) {
+      if (first[j] == j && lab[j] != p.blank) { colid[j] = ++d; cls[d] = lab[j]; }
+    }
+    for (int c = d + 1; c < p.Vc; ++c) cls[c] = (c == d + 1) ? -1 : -2;
+    p.ncols[b] = d;
+    p.off_c[b] = b * p.Lmax;
+  }
+  __syncthreads();
+  int* out = p.lab_c + (size_t)b * p.Lmax;
+  for (int j = tid; j < L; j += CTC_CMP_THREADS)
+    out[j] = lab[j] == p.blank ? 0 : colid[first[j]];
+}
+
+// V-bit membership bitmap of {blank} + labels of utterance b in shared memory
+SB_DEVINL void ctc_build_bitmap(const CtcCompact& p, int b, unsigned* bits) {
+  const int words = (p.V + 31) >> 5;
+  for (int w = threadIdx.x; w < words; w += blockDim.x) bits[w] = 0u;
+  __syncthreads();
+  const int L = min(p.label_lens[b], p.Lmax);
+  const int* lab = p.labels + p.label_off[b];
+  for (int j = threadIdx.x; j <= L; j += blockDim.x) {
+    const int c = j < L ? lab[j] : p.blank;
+    atomicOr(&bits[c >> 5], 1u << (c & 31));
+  }
+  __syncthreads();
+}
+
+// running (max, sum of exp(x - max)) of a stream of logits
+SB_DEVINL void lse_push(float x, float& m, float& s) {
+  if (x > m) {
+    s = (m == CTC_NEG_INF ? 0.f : s * __expf(m - x)) + 1.f;
+    m = x;
+  } else if (x != CTC_NEG_INF) {
+    s += __expf(x - m);
+  }
+}
+SB_DEVINL float lse_warp(float m, float s) {
+  const float M = warp_max(m);
+  s = (M == CTC_NEG_INF || m == CTC_NEG_INF) ? 0.f : s * __expf(m - M);
+  s = warp_sum(s);
+  return s > 0.f ? M + __logf(s) : CTC_NEG_INF;
+}
+
+// grid (ceil(T / CTC_CMP_ROWS), B): compact rows and full-row log-sum-exp of the frames t < act_lens[b]
+__global__ void __launch_bounds__(CTC_CMP_THREADS) ctc_compact_rows_kernel(const CtcCompact p) {
+  extern __shared__ unsigned ctc_bits[];
+  const int b = blockIdx.y;
+  const int Tb = min(p.act_lens[b], p.T);
+  const int t0 = blockIdx.x * CTC_CMP_ROWS;
+  if (t0 >= Tb) return;
+  ctc_build_bitmap(p, b, ctc_bits);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int V = p.V, Vc = p.Vc;
+  const int* cls = p.col_cls + (size_t)b * Vc;
+  for (int t = t0 + warp; t < min(t0 + CTC_CMP_ROWS, Tb); t += CTC_CMP_THREADS / 32) {
+    const size_t row = (size_t)b * p.T + t;
+    const float* a = p.acts + row * V;
+    float mf = CTC_NEG_INF, sf = 0.f, mr = CTC_NEG_INF, sr = 0.f;
+    for (int k = lane; k < V; k += 32) {
+      const float x = __ldg(a + k);
+      lse_push(x, mf, sf);
+      if (!((ctc_bits[k >> 5] >> (k & 31)) & 1u)) lse_push(x, mr, sr);
+    }
+    const float lse_full = lse_warp(mf, sf);
+    const float rest = lse_warp(mr, sr);
+    if (lane == 0) p.lse[row] = lse_full;
+    float* ac = p.acts_c + row * Vc;
+    for (int c = lane; c < Vc; c += 32) {
+      const int k = cls[c];
+      ac[c] = k >= 0 ? __ldg(a + k) : (k == -1 ? rest : CTC_NEG_INF);
+    }
+  }
+}
+
+// grid (ceil(T / CTC_CMP_ROWS), B): every grads[b, t, k]
+__global__ void __launch_bounds__(CTC_CMP_THREADS) ctc_expand_grads_kernel(const CtcCompact p) {
+  extern __shared__ unsigned ctc_bits[];
+  const int b = blockIdx.y;
+  const int t0 = blockIdx.x * CTC_CMP_ROWS;
+  if (t0 >= p.T) return;
+  const int Tb = p.costs[b] == INFINITY ? 0 : min(p.act_lens[b], p.T);
+  const bool any = t0 < Tb;
+  if (any) ctc_build_bitmap(p, b, ctc_bits);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int V = p.V, Vc = p.Vc;
+  const int* cls = p.col_cls + (size_t)b * Vc;
+  const int D = p.ncols[b];
+  for (int t = t0 + warp; t < min(t0 + CTC_CMP_ROWS, p.T); t += CTC_CMP_THREADS / 32) {
+    const size_t row = (size_t)b * p.T + t;
+    float* g = p.grads + row * V;
+    if (t >= Tb) {
+      for (int k = lane; k < V; k += 32) g[k] = 0.f;
+      continue;
+    }
+    const float* a = p.acts + row * V;
+    const float lz = p.lse[row];
+    for (int k = lane; k < V; k += 32)
+      if (!((ctc_bits[k >> 5] >> (k & 31)) & 1u)) g[k] = __expf(__ldg(a + k) - lz);
+    const float* gc = p.grads_c + row * Vc;
+    for (int c = lane; c <= D; c += 32) g[cls[c]] = gc[c];
+  }
+}
+
+static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+struct CtcCompactLayout {
+  size_t fused, acts_c, grads_c, lse, lab_c, off_c, col_cls, ncols, total;
+};
+static CtcCompactLayout ctc_compact_layout(int B, int T, int max_label_len, int ns) {
+  const int Vc = max_label_len + 2;
+  const size_t rows = (size_t)B * T;
+  CtcCompactLayout l;
+  size_t o = 256;   // slack for aligning the base pointer
+  l.fused = o;   o += align256(ctc_fused_ws_bytes(B, T, ns));
+  l.acts_c = o;  o += align256(rows * Vc * sizeof(float));
+  l.grads_c = o; o += align256(rows * Vc * sizeof(float));
+  l.lse = o;     o += align256(rows * sizeof(float));
+  l.lab_c = o;   o += align256((size_t)B * (max_label_len > 0 ? max_label_len : 1) * sizeof(int));
+  l.off_c = o;   o += align256((size_t)B * sizeof(int));
+  l.col_cls = o; o += align256((size_t)B * Vc * sizeof(int));
+  l.ncols = o;   o += align256((size_t)B * sizeof(int));
+  l.total = o;
+  return l;
+}
+
+template <typename K>
+static int ctc_bitmap_kernel_attr(K kernel, size_t smem) {
+  if (smem <= 48 * 1024) return SB_OK;
+  return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) ==
+                 cudaSuccess ? SB_OK : SB_ERR_CUDA;
+}
+
+static int ctc_run_compact(const CtcParams& full, int max_label_len, int ns, void* workspace,
+                           cudaStream_t stream) {
+  const int B = full.B, T = full.T, V = full.V;
+  const CtcCompactLayout l = ctc_compact_layout(B, T, max_label_len, ns);
+  unsigned char* base = reinterpret_cast<unsigned char*>(
+      (reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255) - 256;
+  CtcCompact c;
+  c.acts = full.acts; c.grads = full.grads; c.labels = full.labels; c.label_off = full.label_off;
+  c.label_lens = full.label_lens; c.act_lens = full.act_lens; c.costs = full.costs;
+  c.acts_c = reinterpret_cast<float*>(base + l.acts_c);
+  c.grads_c = reinterpret_cast<float*>(base + l.grads_c);
+  c.lse = reinterpret_cast<float*>(base + l.lse);
+  c.lab_c = reinterpret_cast<int*>(base + l.lab_c);
+  c.off_c = reinterpret_cast<int*>(base + l.off_c);
+  c.col_cls = reinterpret_cast<int*>(base + l.col_cls);
+  c.ncols = reinterpret_cast<int*>(base + l.ncols);
+  c.B = B; c.T = T; c.V = V; c.Vc = max_label_len + 2; c.blank = full.blank;
+  c.Lmax = max_label_len > 0 ? max_label_len : 1;
+
+  const size_t bits_smem = (size_t)((V + 31) / 32) * sizeof(unsigned);
+  const dim3 rgrid((T + CTC_CMP_ROWS - 1) / CTC_CMP_ROWS, B);
+  if (ctc_bitmap_kernel_attr(ctc_compact_rows_kernel, bits_smem) != SB_OK ||
+      ctc_bitmap_kernel_attr(ctc_expand_grads_kernel, bits_smem) != SB_OK)
+    return SB_ERR_CUDA;
+  ctc_colmap_kernel<<<B, CTC_CMP_THREADS, 0, stream>>>(c);
+  ctc_compact_rows_kernel<<<rgrid, CTC_CMP_THREADS, bits_smem, stream>>>(c);
+  if (cudaGetLastError() != cudaSuccess) return SB_ERR_CUDA;
+
+  CtcParams p = full;
+  p.acts = c.acts_c;
+  p.grads = full.grads ? const_cast<float*>(c.grads_c) : nullptr;
+  p.labels = c.lab_c;
+  p.label_off = c.off_c;
+  p.V = c.Vc;
+  p.blank = 0;
+  const int rc = ctc_run_fused(p, ns, base + l.fused, stream);
+  if (rc != SB_OK || !full.grads) return rc;
+  ctc_expand_grads_kernel<<<rgrid, CTC_CMP_THREADS, bits_smem, stream>>>(c);
+  return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
+}
+
+}  // namespace sb
+
+using namespace sb;
+
+extern "C" int sb_ctc_compact_workspace_size(int B, int T, int V, int max_label_len,
+                                             size_t* bytes) {
+  if (!bytes || B <= 0 || T < 0 || V <= 0 || max_label_len < 0) return SB_ERR_INVALID;
+  const int ns = ctc_ns_for(max_label_len);
+  if (ns < 0) return SB_ERR_UNSUPPORTED;
+  *bytes = ctc_compact_layout(B, T > 0 ? T : 1, max_label_len, ns).total;
+  return SB_OK;
+}
+
+extern "C" int sb_ctc_workspace_size(int B, int T, int V, int max_label_len, size_t* bytes) {
+  if (!bytes || B <= 0 || T < 0 || V <= 0 || max_label_len < 0) return SB_ERR_INVALID;
+  const int ns = ctc_ns_for(max_label_len);
+  if (ns < 0) return SB_ERR_UNSUPPORTED;
+  if (!ctc_fused_fits(ns, T, V)) return sb_ctc_compact_workspace_size(B, T, V, max_label_len, bytes);
+  *bytes = ctc_fused_ws_bytes(B, T, ns);
+  return SB_OK;
+}
+
+static int ctc_entry(const float* acts, float* grads, const int* labels_dev,
+                     const int* label_offsets_dev, const int* label_lens_dev,
+                     const int* act_lens_dev, int B, int T, int V, int blank, int max_label_len,
+                     float* costs, void* workspace, size_t workspace_bytes, void* stream_,
+                     bool compact) {
+  if (!acts || !labels_dev || !label_offsets_dev || !label_lens_dev || !act_lens_dev || !costs ||
+      !workspace)
+    return SB_ERR_INVALID;
+  if (B <= 0 || T <= 0 || V <= 0 || blank < 0 || blank >= V || max_label_len < 0)
+    return SB_ERR_INVALID;
+  const int ns = ctc_ns_for(max_label_len);
+  if (ns < 0) return SB_ERR_UNSUPPORTED;
+  compact = compact || !ctc_fused_fits(ns, T, V);
+  size_t need = 0;
+  int rc = compact ? sb_ctc_compact_workspace_size(B, T, V, max_label_len, &need)
+                   : sb_ctc_workspace_size(B, T, V, max_label_len, &need);
+  if (rc != SB_OK) return rc;
+  if (workspace_bytes < need) return SB_ERR_WORKSPACE;
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+
+  CtcParams p;
+  p.acts = acts; p.grads = grads; p.labels = labels_dev; p.label_off = label_offsets_dev;
+  p.label_lens = label_lens_dev; p.act_lens = act_lens_dev; p.costs = costs;
+  p.offs = nullptr; p.ws = nullptr;
+  p.B = B; p.T = T; p.V = V; p.blank = blank; p.S_stride = ns * CTC_SIDE;
+  return compact ? ctc_run_compact(p, max_label_len, ns, workspace, stream)
+                 : ctc_run_fused(p, ns, workspace, stream);
+}
+
+extern "C" int sb_ctc_fwd_bwd(const float* acts, float* grads, const int* labels_dev,
+                              const int* label_offsets_dev, const int* label_lens_dev,
+                              const int* act_lens_dev, int B, int T, int V, int blank,
+                              int max_label_len, float* costs, void* workspace,
+                              size_t workspace_bytes, void* stream) {
+  return ctc_entry(acts, grads, labels_dev, label_offsets_dev, label_lens_dev, act_lens_dev, B, T,
+                   V, blank, max_label_len, costs, workspace, workspace_bytes, stream, false);
+}
+
+extern "C" int sb_ctc_fwd_bwd_compact(const float* acts, float* grads, const int* labels_dev,
+                                      const int* label_offsets_dev, const int* label_lens_dev,
+                                      const int* act_lens_dev, int B, int T, int V, int blank,
+                                      int max_label_len, float* costs, void* workspace,
+                                      size_t workspace_bytes, void* stream) {
+  return ctc_entry(acts, grads, labels_dev, label_offsets_dev, label_lens_dev, act_lens_dev, B, T,
+                   V, blank, max_label_len, costs, workspace, workspace_bytes, stream, true);
 }

@@ -118,3 +118,37 @@ print("seq2seq C=9000 ok", l11.item(), l12.item(),
       [len(h) for h in sv.infer((inputs, lab3), max_len=6)],
       sv.beam_search(([inputs[0]], [lab3[0]]), beam_size=8, max_len=5))
 torch.cuda.synchronize()
+# the CTC model at a subword-sized vocabulary (V = 20001): the compact loss path (column map, row
+# compaction, fused lattice at the compact width, gradient expansion) and the shortlist beam search
+cv = CTC(80, 20000, cfg).cuda()
+labels4 = [np.random.randint(0, 20000, 7 + i).tolist() for i in range(5)]
+l13 = cv.loss((inputs, labels4)); l13.backward()
+print("ctc V=20001 ok", l13.item(), [len(p) for p in cv.infer((inputs, labels4), beam_size=8)])
+lp = torch.log_softmax(torch.randn(2, 30, 29, device="cuda"), 2).contiguous()
+lens = torch.tensor([30, 21], dtype=torch.int32, device="cuda")
+import ctypes
+lib = _lib.load()
+nb = ctypes.c_size_t(0)
+lib.sb_ctc_prefix_beam_workspace_size(2, 30, 4, ctypes.byref(nb))
+ws = torch.empty(nb.value, dtype=torch.uint8, device="cuda")
+o_lab = torch.empty(2, 30, dtype=torch.int32, device="cuda")
+o_len = torch.empty(2, dtype=torch.int32, device="cuda")
+o_sc = torch.empty(2, dtype=torch.float64, device="cuda")
+_lib.check(lib.sb_ctc_prefix_beam_shortlist(lp.data_ptr(), lens.data_ptr(), 2, 30, 29, 4, 28,
+                                            o_lab.data_ptr(), o_len.data_ptr(), o_sc.data_ptr(),
+                                            ws.data_ptr(), nb.value, _lib.stream_ptr()),
+           "sb_ctc_prefix_beam_shortlist")
+acts = torch.randn(2, 30, 29, device="cuda")
+nc = ctypes.c_size_t(0)
+lib.sb_ctc_compact_workspace_size(2, 30, 29, 3, ctypes.byref(nc))
+wc = torch.empty(nc.value, dtype=torch.uint8, device="cuda")
+# [labels | offsets | label_lens | act_lens]
+dl = torch.tensor([1, 2, 2, 3, 4, 5, 0, 3, 3, 3, 30, 21], dtype=torch.int32, device="cuda")
+g = torch.empty_like(acts)
+c = torch.empty(2, device="cuda")
+_lib.check(lib.sb_ctc_fwd_bwd_compact(acts.data_ptr(), g.data_ptr(), dl.data_ptr(),
+                                      dl[6:].data_ptr(), dl[8:].data_ptr(), dl[10:].data_ptr(), 2,
+                                      30, 29, 28, 3, c.data_ptr(), wc.data_ptr(), nc.value,
+                                      _lib.stream_ptr()), "sb_ctc_fwd_bwd_compact")
+torch.cuda.synchronize()
+print("ctc compact / shortlist entries ok", c.tolist(), o_len.tolist())
