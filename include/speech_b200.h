@@ -459,6 +459,20 @@ int sb_rnnt_joint_vocab_bwd_rows(const float* logits, long long ld, const float*
                                  const float* garc, const int* ymat, void* dlogits_bf16,
                                  long long ldd, float* db2, int B, int T, int U1, int V1, int blank,
                                  int t0, int Tc, void* stream);
+/* Shortlists of the lattice for sb_rnnt_decode_static_shortlist, one per node, batch-first:
+ *   sl_val  (B, T, U1, kp) f32  the kp best non-blank lp by (lp desc, class asc), -inf padded
+ *   sl_idx  (B, T, U1, kp) i32  their classes, -1 past the V1 - 1 non-blank classes
+ *   sl_meta (B, T, U1, 2)  f32  {lp of the blank, lp of the (kp+1)-th non-blank class or -inf}
+ * lp_k = v_k - lse[n] in the fp32 arithmetic of sb_rnnt_joint_vocab_fwd_rows' lp_full (bit-
+ * identical values), or v_k itself when lse is NULL.  Rows of v (leading dimension ld >= V1, any
+ * alignment) are either
+ *   time_major = 1: a slab of the joint, as sb_rnnt_joint_vocab_fwd_rows reads it (row r is node
+ *                   n = t0*B*U1 + r; lse indexed by n), or
+ *   time_major = 0: the whole batch-first (B, T, U1) lattice (t0 = 0, Tc = T).
+ * 1 <= kp <= 64 (SB_ERR_UNSUPPORTED above). */
+int sb_rnnt_shortlist_rows(const float* v, long long ld, const float* lse, int B, int T, int U1,
+                           int V1, int blank, int kp, int t0, int Tc, int time_major,
+                           float* sl_val, int* sl_idx, float* sl_meta, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Transducer beam search over a precomputed (teacher-forced) lattice, one CTA per utterance.
@@ -469,12 +483,27 @@ int sb_rnnt_joint_vocab_bwd_rows(const float* logits, long long ld, const float*
  *   tlens    (B) frames searched per utterance, ulens (B) lattice rows (labels + 1)
  *   out_labels (B, U1) int32, out_lens (B), out_scores (B) f64 log-probability of the best
  *   workspace >= sb_rnnt_decode_static_workspace_size bytes;  beam_size <= 32
+ * sb_rnnt_decode_static keeps every candidate in shared memory: it runs where
+ * beam_size * V * 8 + 16 <= 200 KB, which sb_rnnt_decode_static_fits(beam_size, V) answers (1 / 0,
+ * host arithmetic); SB_ERR_UNSUPPORTED elsewhere.
+ * sb_rnnt_decode_static_shortlist runs the same search, at any V, from the shortlists of
+ * sb_rnnt_shortlist_rows (kp per node, beam_size <= kp <= 64): a K-way merge of the frontier's
+ * lists replaces the scan of beam_size * V candidates.  Labels, lengths and scores are bit-
+ * identical to sb_rnnt_decode_static unless out_flags (B, int32) counts, for an utterance, a
+ * selection the lists cannot prove (two distinct float32 lp rounding to one float64 score at the
+ * end of a list, csrc/tdecode.cu); rerun such utterances with longer lists.
  * ------------------------------------------------------------------------------------- */
 int sb_rnnt_decode_static_workspace_size(int B, int T, int U1, int beam_size, size_t* bytes);
+int sb_rnnt_decode_static_fits(int beam_size, int V);
 int sb_rnnt_decode_static(const float* lp, const int* tlens, const int* ulens, int B, int T, int U1,
                           int V, int beam_size, int blank, int* out_labels, int* out_lens,
                           double* out_scores, void* workspace, size_t workspace_bytes,
                           void* stream);
+int sb_rnnt_decode_static_shortlist(const float* sl_val, const int* sl_idx, const float* sl_meta,
+                                    int kp, const int* tlens, const int* ulens, int B, int T,
+                                    int U1, int V, int beam_size, int blank, int* out_labels,
+                                    int* out_lens, double* out_scores, int* out_flags,
+                                    void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Scoring (SURVEY.md section 8f rank 4), HOST function: Levenshtein distance of two int32 token

@@ -103,6 +103,12 @@ SIGNATURES = {
                                                       ctypes.POINTER(_c_sz)]),
     "sb_rnnt_decode_static": (_c_int, [_vp, _vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int, _c_int,
                                        _vp, _vp, _vp, _vp, _c_sz, _vp]),
+    "sb_rnnt_decode_static_fits": (_c_int, [_c_int, _c_int]),
+    "sb_rnnt_shortlist_rows": (_c_int, [_vp, _c_ll, _vp, _c_int, _c_int, _c_int, _c_int, _c_int,
+                                        _c_int, _c_int, _c_int, _c_int, _vp, _vp, _vp, _vp]),
+    "sb_rnnt_decode_static_shortlist": (_c_int, [_vp, _vp, _vp, _c_int, _vp, _vp, _c_int, _c_int,
+                                                 _c_int, _c_int, _c_int, _c_int, _vp, _vp, _vp, _vp,
+                                                 _vp, _c_sz, _vp]),
     "sb_debug_gru_timeline": (_c_int, [_vp]),
     "sb_debug_gru_cluster": (_c_int, [_c_int]),
     "sb_debug_gru_ksplit": (_c_int, [_c_int]),

@@ -9,6 +9,9 @@
 //      backward: sb_rnnt_joint_vocab_bwd_rows   dlogits = g_b [k = blank] + g_l [k = label]
 //                                                          - (g_b + g_l) exp(v_k - lse)  (bf16)
 //                                                db2 += column sums of dlogits
+//   4. decoding: sb_rnnt_shortlist_rows   per node the blank's log-prob, the kp best non-blank
+//                                          classes and the next value, for the beam search of
+//                                          csrc/tdecode.cu (also run on a given lp tensor)
 // Neither the (nodes x V1) logits nor their gradient ever exist in full, only one slab of each.
 // Roofline of the row kernels: memory bandwidth (one fp32 read per logit, plus one bf16 write per
 // logit in the backward pass); the slab is read back from L2 when it fits there.
@@ -130,6 +133,116 @@ joint_vocab_bwd_rows_kernel(const float* __restrict__ logits, long long ld,
   }
 }
 
+// ---- shortlist rows: one warp per row.  lp_k = v_k - lse is formed with the same fp32 expression
+// as the lp_full rows of joint_vocab_fwd_rows_kernel (or read as is when lse is NULL), so every
+// shortlisted value is bit-identical to the full tensor's entry.  The row streams through a
+// per-warp buffer of SL_CAP candidates: a class enters it when it ranks above the current
+// threshold by (lp desc, k asc) - ranking on the ROUNDED lp, since v - lse can map distinct logits
+// to equal log-probs - and a full buffer is sorted (bitonic) and cut to its P = kp + 1 best, whose
+// last entry becomes the threshold.  On a random row only O(P log(V1 / P)) classes ever enter.
+// -inf entries are ranked like any other value (the beam search treats them as live). ----
+static constexpr int SL_CAP = 256;     // >= SL_MAX_KP + 1 + 32: one cut leaves room for a warp's row
+static constexpr int SL_MAX_KP = 64;
+
+SB_DEVINL bool sl_better(float a, int ka, float b, int kb) { return a > b || (a == b && ka < kb); }
+
+// sorts bv / bi [0, SL_CAP) best first (entries past `cnt` are padded with the worst key first)
+SB_DEVINL void sl_sort(float* bv, int* bi, int cnt, int lane) {
+  for (int i = cnt + lane; i < SL_CAP; i += 32) { bv[i] = -INFINITY; bi[i] = 0x7fffffff; }
+  __syncwarp();
+  for (int k = 2; k <= SL_CAP; k <<= 1)
+    for (int j = k >> 1; j > 0; j >>= 1) {
+      for (int i = lane; i < SL_CAP; i += 32) {
+        const int l = i ^ j;
+        if (l > i) {
+          const float a = bv[i], c = bv[l];
+          const int ka = bi[i], kc = bi[l];
+          if ((i & k) == 0 ? sl_better(c, kc, a, ka) : sl_better(a, ka, c, kc)) {
+            bv[i] = c; bi[i] = kc; bv[l] = a; bi[l] = ka;
+          }
+        }
+      }
+      __syncwarp();
+    }
+}
+
+__global__ void __launch_bounds__(256)
+rnnt_shortlist_rows_kernel(const float* __restrict__ v, long long ld, const float* __restrict__ lse,
+                           int B, int T, int U1, int V1, int blank, int kp, long long n0,
+                           long long rows, int time_major, float* __restrict__ sl_val,
+                           int* __restrict__ sl_idx, float* __restrict__ sl_meta) {
+  __shared__ float buf_v[8][SL_CAP];
+  __shared__ int buf_i[8][SL_CAP];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const long long r = blockIdx.x * 8LL + w;
+  if (r >= rows) return;                   // whole warps: only __syncwarp below
+  float* bv = buf_v[w];
+  int* bi = buf_i[w];
+  const long long n = n0 + r;
+  const float* row = v + r * ld;
+  const float l = lse ? lse[n] : 0.f;
+  long long o = n;                         // batch-first output node
+  if (time_major) {
+    const long long tb = n / U1;
+    const int u = (int)(n - tb * U1);
+    o = ((tb % B) * T + tb / B) * U1 + u;
+  }
+  const int P = kp + 1;
+  int cnt = 0;
+  bool thr = false;
+  float tv = 0.f;
+  int tk = 0;
+  for (int base = 0; base < V1; base += 128) {
+    float x[4];
+    bool q[4];
+    bool anyq = false;
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int j = base + e * 32 + lane;
+      q[e] = j < V1 && j != blank;
+      x[e] = 0.f;
+      if (q[e]) {
+        x[e] = lse ? row[j] - l : row[j];
+        q[e] = !thr || sl_better(x[e], j, tv, tk);
+      }
+      anyq |= q[e];
+    }
+    if (!__any_sync(0xffffffffu, anyq)) continue;
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int j = base + e * 32 + lane;
+      unsigned m = __ballot_sync(0xffffffffu, q[e]);
+      if (!m) continue;
+      if (cnt + __popc(m) > SL_CAP) {      // cut the buffer to its P best, raise the threshold
+        sl_sort(bv, bi, cnt, lane);
+        cnt = P;
+        thr = true;
+        tv = bv[P - 1];
+        tk = bi[P - 1];
+        __syncwarp();
+        q[e] = q[e] && sl_better(x[e], j, tv, tk);
+        m = __ballot_sync(0xffffffffu, q[e]);
+      }
+      if (q[e]) {
+        const int pos = cnt + __popc(m & ((1u << lane) - 1u));
+        bv[pos] = x[e];
+        bi[pos] = j;
+      }
+      cnt += __popc(m);
+      __syncwarp();
+    }
+  }
+  sl_sort(bv, bi, cnt, lane);
+  for (int e = lane; e < kp; e += 32) {
+    sl_val[o * kp + e] = e < cnt ? bv[e] : -INFINITY;
+    sl_idx[o * kp + e] = e < cnt ? bi[e] : -1;
+  }
+  if (lane == 0) {
+    const float bl = lse ? row[blank] - l : row[blank];
+    *reinterpret_cast<float2*>(sl_meta + o * 2) = make_float2(bl, cnt > kp ? bv[kp] : -INFINITY);
+  }
+}
+
 // argument checks shared by both entry points: the leading dimension of a row is a multiple of 8
 // elements (16-byte aligned float4 / bf16x4 accesses), the slab lies within [0, T)
 static int vocab_check(long long ld, int B, int T, int U1, int V1, int blank, int t0, int Tc) {
@@ -159,6 +272,26 @@ extern "C" int sb_rnnt_joint_vocab_fwd_rows(const float* logits, long long ld, c
   if (grid > 0x7fffffffLL) return SB_ERR_UNSUPPORTED;
   joint_vocab_fwd_rows_kernel<<<(unsigned)grid, 256, 0, stream>>>(logits, ld, ymat, lat, lse, lp_full,
                                                                   B, T, U1, V1, blank, n0, rows);
+  return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
+}
+
+extern "C" int sb_rnnt_shortlist_rows(const float* v, long long ld, const float* lse, int B, int T,
+                                      int U1, int V1, int blank, int kp, int t0, int Tc,
+                                      int time_major, float* sl_val, int* sl_idx, float* sl_meta,
+                                      void* stream_) {
+  if (!v || !sl_val || !sl_idx || !sl_meta || ld < V1) return SB_ERR_INVALID;
+  if (B <= 0 || T <= 0 || U1 <= 0 || V1 <= 0 || Tc <= 0 || t0 < 0 || t0 + Tc > T)
+    return SB_ERR_INVALID;
+  if (blank < 0 || blank >= V1 || kp < 1 || (!time_major && (t0 != 0 || Tc != T)))
+    return SB_ERR_INVALID;
+  if (kp > SL_MAX_KP) return SB_ERR_UNSUPPORTED;
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  const long long rows = (long long)Tc * B * U1;
+  const long long n0 = (long long)t0 * B * U1;
+  const long long grid = (rows + 7) / 8;
+  if (grid > 0x7fffffffLL) return SB_ERR_UNSUPPORTED;
+  rnnt_shortlist_rows_kernel<<<(unsigned)grid, 256, 0, stream>>>(
+      v, ld, lse, B, T, U1, V1, blank, kp, n0, rows, time_major, sl_val, sl_idx, sl_meta);
   return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
 }
 

@@ -20,6 +20,33 @@
 // Hypotheses are nodes (parent, label) of a per-utterance trie made canonical by a hash map, so
 // "the same label sequence" is an integer comparison.  Scores are float64, as Python floats.
 // Roofline: HBM-nominal (the lattice is read once); latency-bound by the T x U serial expansion.
+//
+// sb_rnnt_decode_static_shortlist: the same search from per-node shortlists instead of the full
+// lattice (sb_rnnt_shortlist_rows, csrc/joint_vocab.cu): for node (t, u) the blank's lp, the kp
+// best non-blank classes as (lp, k) sorted by (lp desc, k asc), and beta = the (kp+1)-th lp in
+// that order (-inf when there is none).  Everything but the label expansion is the kernel above.
+// The expansion is a K-way merge: K rounds of an arg-max over the heads of the frontier's lists,
+// with the full search's order (score desc, i asc, k asc).
+//   Scores are s_q = fr_s + (double)lp_q.  Double addition is monotone, so s_q is non-increasing
+//   along a list; but distinct float32 lp can round to the same s, and the full search takes such
+//   equal-score entries in class order.  So the head of list i is the smallest unconsumed class in
+//   the run of equal s that holds its first unconsumed position (a 64-bit mask per hypothesis
+//   records what was taken); the rank between lists only needs (s, i).
+//   A hypothesis with fr_s = -inf scores -inf on every class: its candidates are the non-blank
+//   classes in index order, and it reads no list.
+// Exactness.  A selection (s, k) from list i is what the full search takes unless a class left
+// out of the list ties with it on s and has a smaller k.  Left-out classes have lp <= beta <= every
+// listed lp, so by monotonicity one ties only if fr_s + beta == s.  Given that:
+//   - left-out classes with lp == beta have larger k than every listed entry with lp == beta (the
+//     list is the head of the (lp desc, k asc) order), so they are safe when the selected lp ==
+//     beta, and may precede it when the selected lp > beta;
+//   - left-out classes with lp < beta have lp <= nextafterf(beta, -inf) and any k; they tie only
+//     if fr_s + nextafterf(beta, -inf) == s as well (never when beta = -inf: nothing lies below).
+// The kernel counts every selection that fails either test in out_flags[b]; the caller re-runs
+// flagged utterances from longer lists.  Both tests need two distinct float32 values to round to
+// one float64 sum, i.e. |fr_s| of roughly 2^29 times their gap, so real lattices never raise it.
+// A hypothesis takes at most K of its entries, so kp >= K lists are never exhausted while a
+// left-out class could still follow.
 #include "common.cuh"
 #include <math.h>
 
@@ -29,9 +56,14 @@ namespace sb {
 
 static constexpr int TD_THREADS = 128;
 static constexpr int TD_MAX_BEAM = 32;
+static constexpr int TD_MAX_KP = 64;
+static constexpr size_t TD_SMEM_MAX = 200 * 1024;
 
 struct TdParams {
-  const float* lp;      // (B, T, U1, V) log-probabilities
+  const float* lp;      // (B, T, U1, V) log-probabilities (full lattice)
+  const float* sl_val;  // (B, T, U1, kp) shortlisted log-probabilities (shortlist search)
+  const int* sl_idx;    // (B, T, U1, kp) their classes, -1 past V-1 entries
+  const float* sl_meta; // (B, T, U1, 2) {blank lp, beta}
   const int* tlens;     // (B) frames to search (<= T)
   const int* ulens;     // (B) lattice rows U = labels + 1 (<= U1)
   int* nodes;           // (B, 2*node_cap) trie arena: parent, label
@@ -43,7 +75,8 @@ struct TdParams {
   int* out_labels;      // (B, U1)
   int* out_lens;        // (B)
   double* out_scores;   // (B) log-probability of the best hypothesis
-  int B, T, U1, V, K, blank, hcap, node_cap, done_cap;
+  int* out_flags;       // (B) unproven shortlist selections (shortlist search)
+  int B, T, U1, V, K, kp, blank, hcap, node_cap, done_cap;
 };
 
 SB_DEVINL double td_lse(double a, double b) {
@@ -80,19 +113,53 @@ SB_DEVINL int td_argmax(const double* sc, int n, double* red_s, int* red_i, int 
   return bi;
 }
 
-__global__ void __launch_bounds__(TD_THREADS) rnnt_decode_static_kernel(const TdParams p) {
+// nextafterf(x, -inf) for finite x
+SB_DEVINL float td_next_down(float x) {
+  const int i = __float_as_int(x);
+  if (x == 0.f) return -__int_as_float(1);                 // -(smallest subnormal)
+  return __int_as_float(x > 0.f ? i - 1 : i + 1);
+}
+
+// canonical trie node of hypothesis node `parent` extended by label k (one thread); a new node
+// gets id 1 + round_id * K + nsel, -1 when the arena is full
+SB_DEVINL int td_extend(const TdParams& p, int* nodes, unsigned long long* hkeys, int* hvals,
+                        int parent, int k, int round_id, int nsel) {
+  const unsigned long long key =
+      ((unsigned long long)(unsigned int)parent << 32) | (unsigned int)(k + 1);
+  unsigned int h = (unsigned int)((key * 0x9E3779B97F4A7C15ull) >> 32) & (p.hcap - 1);
+  int id = -1;
+  for (int probe = 0; probe < p.hcap; ++probe) {
+    const unsigned long long kk = hkeys[h];
+    if (kk == key) { id = hvals[h]; break; }
+    if (kk == 0ull) {
+      id = 1 + round_id * p.K + nsel;
+      if (id >= p.node_cap) { id = -1; break; }
+      hkeys[h] = key;
+      hvals[h] = id;
+      nodes[2 * id] = parent;
+      nodes[2 * id + 1] = k;
+      break;
+    }
+    h = (h + 1) & (p.hcap - 1);
+  }
+  return id;
+}
+
+// the search of one utterance (blockIdx.x); SHORT: candidates from the shortlists
+template <bool SHORT>
+SB_DEVINL void td_search(const TdParams& p) {
   extern __shared__ unsigned char td_smem[];
   const int b = blockIdx.x, tid = threadIdx.x;
   const int K = p.K, V = p.V;
   const int T = min(p.tlens[b], p.T), U = min(p.ulens[b], p.U1);
-  double* cand = reinterpret_cast<double*>(td_smem);       // [K * V]
+  double* cand = reinterpret_cast<double*>(td_smem);       // [K * V] (full lattice only)
   __shared__ double beam_s[TD_MAX_BEAM], fr_s[TD_MAX_BEAM], new_s[TD_MAX_BEAM];
   __shared__ int beam_n[TD_MAX_BEAM], beam_l[TD_MAX_BEAM];
   __shared__ int fr_n[TD_MAX_BEAM], fr_l[TD_MAX_BEAM];
   __shared__ int new_n[TD_MAX_BEAM], new_l[TD_MAX_BEAM];
   __shared__ double red_s[TD_THREADS / 32];
   __shared__ int red_i[TD_THREADS / 32];
-  __shared__ int nbeam, nfr, ndone, found, round_id;
+  __shared__ int nbeam, nfr, ndone, found, round_id, nsel_s, nflag;
 
   int* nodes = p.nodes + (size_t)b * 2 * p.node_cap;
   unsigned long long* hkeys = p.hkeys + (size_t)b * p.hcap;
@@ -100,13 +167,15 @@ __global__ void __launch_bounds__(TD_THREADS) rnnt_decode_static_kernel(const Td
   double* dscore = p.done_score + (size_t)b * p.done_cap;
   int* dnode = p.done_node + (size_t)b * p.done_cap;
   int* dlen = p.done_len + (size_t)b * p.done_cap;
-  const float* lp = p.lp + (size_t)b * p.T * p.U1 * V;
+  const float* lp = SHORT ? nullptr : p.lp + (size_t)b * p.T * p.U1 * V;
+  const size_t node0 = (size_t)b * p.T * p.U1;             // batch-first node of (b, 0, 0)
 
   for (int k = tid; k < p.hcap; k += TD_THREADS) hkeys[k] = 0ull;
   if (tid == 0) {
     nbeam = 1; beam_s[0] = 0.0; beam_n[0] = 0; beam_l[0] = 0;
     nodes[0] = -1; nodes[1] = -1;
     round_id = 0;
+    nflag = 0;
   }
   __syncthreads();
 
@@ -127,57 +196,116 @@ __global__ void __launch_bounds__(TD_THREADS) rnnt_decode_static_kernel(const Td
           if (dnode[j] == me) found = j;            // at most one entry holds this hypothesis
         __syncthreads();
         if (tid == 0) {
-          const double bsc = fr_s[i] + (double)lp[((size_t)t * p.U1 + u) * V + p.blank];
+          const size_t node = (size_t)t * p.U1 + u;
+          const float blp = SHORT ? p.sl_meta[2 * (node0 + node)] : lp[node * V + p.blank];
+          const double bsc = fr_s[i] + (double)blp;
           if (found >= 0) dscore[found] = td_lse(dscore[found], bsc);
           else if (nd < p.done_cap) { dscore[nd] = bsc; dnode[nd] = me; dlen[nd] = u; ndone = nd + 1; }
         }
         __syncthreads();
       }
       // ---- 2. label expansions: candidates (i, k), the K best form the next frontier ----
-      bool any = false;
-      for (int c = tid; c < K * V; c += TD_THREADS) {
-        const int i = c / V, k = c - i * V;
-        double sc = nan("");
-        if (i < nf && k != p.blank && fr_l[i] + 1 < U) {
-          sc = fr_s[i] + (double)lp[((size_t)t * p.U1 + fr_l[i]) * V + k];
-          any = true;
-        }
-        cand[c] = sc;
-      }
-      const int have = __syncthreads_or(any ? 1 : 0);
-      if (!have) break;
       int nsel = 0;
-      for (int r = 0; r < K; ++r) {
-        const int c = td_argmax(cand, K * V, red_s, red_i, tid);
-        if (c < 0) break;
-        if (tid == 0) {
+      if (!SHORT) {
+        bool any = false;
+        for (int c = tid; c < K * V; c += TD_THREADS) {
           const int i = c / V, k = c - i * V;
-          // canonical node of hypothesis i extended by label k
-          const unsigned long long key =
-              ((unsigned long long)(unsigned int)fr_n[i] << 32) | (unsigned int)(k + 1);
-          unsigned int h = (unsigned int)((key * 0x9E3779B97F4A7C15ull) >> 32) & (p.hcap - 1);
-          int id = -1;
-          for (int probe = 0; probe < p.hcap; ++probe) {
-            const unsigned long long kk = hkeys[h];
-            if (kk == key) { id = hvals[h]; break; }
-            if (kk == 0ull) {
-              id = 1 + round_id * K + nsel;
-              if (id >= p.node_cap) { id = -1; break; }
-              hkeys[h] = key;
-              hvals[h] = id;
-              nodes[2 * id] = fr_n[i];
-              nodes[2 * id + 1] = k;
-              break;
-            }
-            h = (h + 1) & (p.hcap - 1);
+          double sc = nan("");
+          if (i < nf && k != p.blank && fr_l[i] + 1 < U) {
+            sc = fr_s[i] + (double)lp[((size_t)t * p.U1 + fr_l[i]) * V + k];
+            any = true;
           }
-          new_s[nsel] = cand[c];
-          new_n[nsel] = id;
-          new_l[nsel] = fr_l[i] + 1;
-          cand[c] = nan("");
+          cand[c] = sc;
         }
-        ++nsel;
-        __syncthreads();
+        const int have = __syncthreads_or(any ? 1 : 0);
+        if (!have) break;
+        for (int r = 0; r < K; ++r) {
+          const int c = td_argmax(cand, K * V, red_s, red_i, tid);
+          if (c < 0) break;
+          if (tid == 0) {
+            const int i = c / V, k = c - i * V;
+            new_s[nsel] = cand[c];
+            new_n[nsel] = td_extend(p, nodes, hkeys, hvals, fr_n[i], k, round_id, nsel);
+            new_l[nsel] = fr_l[i] + 1;
+            cand[c] = nan("");
+          }
+          ++nsel;
+          __syncthreads();
+        }
+      } else {
+        // K-way merge of the frontier's shortlists, one lane per hypothesis (warp 0)
+        bool live = false;
+        if (tid < 32) {
+          const int i = tid;
+          live = i < nf && fr_l[i] + 1 < U && V > 1;
+          const double fs = live ? fr_s[i] : 0.0;
+          const bool all_tie = live && fs == -INFINITY;
+          const int n = min(p.kp, V - 1);
+          const float* lv = nullptr;
+          const int* li = nullptr;
+          float beta = -INFINITY;
+          if (live && !all_tie) {
+            const size_t node = node0 + (size_t)t * p.U1 + fr_l[i];
+            lv = p.sl_val + node * p.kp;
+            li = p.sl_idx + node * p.kp;
+            beta = p.sl_meta[2 * node + 1];
+          }
+          const unsigned long long inlist = n >= 64 ? ~0ull : (1ull << n) - 1ull;
+          unsigned long long used = 0ull;
+          int taken = 0, nfl = 0, ns = 0;
+          const bool have = __any_sync(0xffffffffu, live);
+          for (int r = 0; r < K && have; ++r) {
+            bool hv = false;
+            double hs = 0.0;
+            int hk = -1, hq = -1;
+            if (all_tie) {
+              if (taken < V - 1) { hv = true; hs = -INFINITY; hk = taken < p.blank ? taken : taken + 1; }
+            } else if (live) {
+              const unsigned long long fr = ~used & inlist;
+              if (fr) {
+                hq = __ffsll((long long)fr) - 1;
+                hk = li[hq];
+                hs = fs + (double)lv[hq];
+                hv = true;
+                for (int q = hq + 1; q < n && fs + (double)lv[q] == hs; ++q)
+                  if (!((used >> q) & 1ull) && li[q] < hk) { hk = li[q]; hq = q; }
+              }
+            }
+            double bs = hs;
+            int bi = hv ? i : -1;
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) {
+              const double os = __shfl_xor_sync(0xffffffffu, bs, o);
+              const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+              if (oi >= 0 && (bi < 0 || os > bs || (os == bs && oi < bi))) { bs = os; bi = oi; }
+            }
+            if (bi < 0) break;
+            const int k = __shfl_sync(0xffffffffu, hk, bi);
+            if (i == bi) {
+              if (all_tie) {
+                ++taken;
+              } else {
+                used |= 1ull << hq;
+                const float x = lv[hq];
+                if (fs + (double)beta == hs &&
+                    (x != beta ||
+                     (beta != -INFINITY && fs + (double)td_next_down(beta) == hs)))
+                  ++nfl;
+              }
+            }
+            if (i == 0) {
+              new_s[ns] = bs;
+              new_n[ns] = td_extend(p, nodes, hkeys, hvals, fr_n[bi], k, round_id, ns);
+              new_l[ns] = fr_l[bi] + 1;
+            }
+            ++ns;
+            __syncwarp();
+          }
+          nfl = __reduce_add_sync(0xffffffffu, nfl);
+          if (i == 0) { nsel_s = ns; nflag += nfl; }
+        }
+        if (!__syncthreads_or(live ? 1 : 0)) break;
+        nsel = nsel_s;
       }
       if (tid < nsel) { fr_s[tid] = new_s[tid]; fr_n[tid] = new_n[tid]; fr_l[tid] = new_l[tid]; }
       if (tid == 0) { nfr = nsel; ++round_id; }
@@ -209,7 +337,19 @@ __global__ void __launch_bounds__(TD_THREADS) rnnt_decode_static_kernel(const Td
     for (int q = n; q > 0; q = nodes[2 * q]) out[--k] = nodes[2 * q + 1];
     p.out_lens[b] = len;
     p.out_scores[b] = nbeam > 0 ? beam_s[0] : -INFINITY;
+    if (SHORT) p.out_flags[b] = nflag;
   }
+}
+
+__global__ void __launch_bounds__(TD_THREADS) rnnt_decode_static_kernel(const TdParams p) {
+  td_search<false>(p);
+}
+
+// (one CTA per SM is all a batch of utterances asks for; the bound lets ptxas keep every value of
+// the merge in registers)
+__global__ void __launch_bounds__(TD_THREADS, 1) rnnt_decode_static_shortlist_kernel(
+    const TdParams p) {
+  td_search<true>(p);
 }
 
 static int td_pow2(size_t need) {
@@ -229,6 +369,40 @@ static TdSizes td_sizes(int B, int T, int U1, int K) {
   return s;
 }
 
+static size_t td_full_smem(int beam_size, int V) { return (size_t)beam_size * V * sizeof(double) + 16; }
+
+// checks shared by both searches; fills the workspace carve-up, shapes and outputs of p
+static int td_setup(TdParams* p, const int* tlens, const int* ulens, int B, int T, int U1, int V,
+                    int beam_size, int blank, int* out_labels, int* out_lens, double* out_scores,
+                    void* workspace, size_t workspace_bytes) {
+  if (!tlens || !ulens || !out_labels || !out_lens || !out_scores || !workspace)
+    return SB_ERR_INVALID;
+  if (B <= 0 || T <= 0 || U1 <= 0 || V <= 0 || blank < 0 || blank >= V || beam_size <= 0)
+    return SB_ERR_INVALID;
+  if (beam_size > TD_MAX_BEAM) return SB_ERR_UNSUPPORTED;
+  const TdSizes sz = td_sizes(B, T, U1, beam_size);
+  if (workspace_bytes < sz.total) return SB_ERR_WORKSPACE;
+  uintptr_t w = (reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255;
+  p->hkeys = reinterpret_cast<unsigned long long*>(w);
+  w += (size_t)B * sz.hcap * sizeof(unsigned long long);
+  p->done_score = reinterpret_cast<double*>(w);
+  w += (size_t)B * sz.done_cap * sizeof(double);
+  p->hvals = reinterpret_cast<int*>(w);
+  w += (size_t)B * sz.hcap * sizeof(int);
+  p->nodes = reinterpret_cast<int*>(w);
+  w += (size_t)B * 2 * sz.node_cap * sizeof(int);
+  p->done_node = reinterpret_cast<int*>(w);
+  w += (size_t)B * sz.done_cap * sizeof(int);
+  p->done_len = reinterpret_cast<int*>(w);
+  p->lp = nullptr; p->sl_val = nullptr; p->sl_idx = nullptr; p->sl_meta = nullptr;
+  p->out_flags = nullptr;
+  p->tlens = tlens; p->ulens = ulens;
+  p->out_labels = out_labels; p->out_lens = out_lens; p->out_scores = out_scores;
+  p->B = B; p->T = T; p->U1 = U1; p->V = V; p->K = beam_size; p->kp = 0; p->blank = blank;
+  p->hcap = (int)sz.hcap; p->node_cap = (int)sz.node_cap; p->done_cap = (int)sz.done_cap;
+  return SB_OK;
+}
+
 }  // namespace sb
 
 using namespace sb;
@@ -240,41 +414,48 @@ extern "C" int sb_rnnt_decode_static_workspace_size(int B, int T, int U1, int be
   return SB_OK;
 }
 
+extern "C" int sb_rnnt_decode_static_fits(int beam_size, int V) {
+  return beam_size > 0 && beam_size <= TD_MAX_BEAM && V > 0 &&
+         td_full_smem(beam_size, V) <= TD_SMEM_MAX;
+}
+
 extern "C" int sb_rnnt_decode_static(const float* lp, const int* tlens, const int* ulens, int B,
                                      int T, int U1, int V, int beam_size, int blank,
                                      int* out_labels, int* out_lens, double* out_scores,
                                      void* workspace, size_t workspace_bytes, void* stream_) {
-  if (!lp || !tlens || !ulens || !out_labels || !out_lens || !out_scores || !workspace)
-    return SB_ERR_INVALID;
-  if (B <= 0 || T <= 0 || U1 <= 0 || V <= 0 || blank < 0 || blank >= V || beam_size <= 0)
-    return SB_ERR_INVALID;
-  if (beam_size > TD_MAX_BEAM) return SB_ERR_UNSUPPORTED;
-  const TdSizes sz = td_sizes(B, T, U1, beam_size);
-  if (workspace_bytes < sz.total) return SB_ERR_WORKSPACE;
-  const size_t smem = (size_t)beam_size * V * sizeof(double) + 16;
-  if (smem > 200 * 1024) return SB_ERR_UNSUPPORTED;
+  if (!lp) return SB_ERR_INVALID;
+  TdParams p;
+  const int rc = td_setup(&p, tlens, ulens, B, T, U1, V, beam_size, blank, out_labels, out_lens,
+                          out_scores, workspace, workspace_bytes);
+  if (rc != SB_OK) return rc;
+  const size_t smem = td_full_smem(beam_size, V);
+  if (smem > TD_SMEM_MAX) return SB_ERR_UNSUPPORTED;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (smem > 40 * 1024 &&
-      cudaFuncSetAttribute(rnnt_decode_static_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                           (int)smem) != cudaSuccess)
+      cudaFuncSetAttribute(rnnt_decode_static_kernel,
+                           cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
     return SB_ERR_CUDA;
-  TdParams p;
-  uintptr_t w = (reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255;
-  p.hkeys = reinterpret_cast<unsigned long long*>(w);
-  w += (size_t)B * sz.hcap * sizeof(unsigned long long);
-  p.done_score = reinterpret_cast<double*>(w);
-  w += (size_t)B * sz.done_cap * sizeof(double);
-  p.hvals = reinterpret_cast<int*>(w);
-  w += (size_t)B * sz.hcap * sizeof(int);
-  p.nodes = reinterpret_cast<int*>(w);
-  w += (size_t)B * 2 * sz.node_cap * sizeof(int);
-  p.done_node = reinterpret_cast<int*>(w);
-  w += (size_t)B * sz.done_cap * sizeof(int);
-  p.done_len = reinterpret_cast<int*>(w);
-  p.lp = lp; p.tlens = tlens; p.ulens = ulens;
-  p.out_labels = out_labels; p.out_lens = out_lens; p.out_scores = out_scores;
-  p.B = B; p.T = T; p.U1 = U1; p.V = V; p.K = beam_size; p.blank = blank;
-  p.hcap = (int)sz.hcap; p.node_cap = (int)sz.node_cap; p.done_cap = (int)sz.done_cap;
+  p.lp = lp;
   rnnt_decode_static_kernel<<<B, TD_THREADS, smem, stream>>>(p);
+  return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
+}
+
+extern "C" int sb_rnnt_decode_static_shortlist(const float* sl_val, const int* sl_idx,
+                                               const float* sl_meta, int kp, const int* tlens,
+                                               const int* ulens, int B, int T, int U1, int V,
+                                               int beam_size, int blank, int* out_labels,
+                                               int* out_lens, double* out_scores, int* out_flags,
+                                               void* workspace, size_t workspace_bytes,
+                                               void* stream_) {
+  if (!sl_val || !sl_idx || !sl_meta || !out_flags) return SB_ERR_INVALID;
+  TdParams p;
+  const int rc = td_setup(&p, tlens, ulens, B, T, U1, V, beam_size, blank, out_labels, out_lens,
+                          out_scores, workspace, workspace_bytes);
+  if (rc != SB_OK) return rc;
+  if (kp < beam_size) return SB_ERR_INVALID;
+  if (kp > TD_MAX_KP) return SB_ERR_UNSUPPORTED;
+  p.sl_val = sl_val; p.sl_idx = sl_idx; p.sl_meta = sl_meta; p.kp = kp; p.out_flags = out_flags;
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  rnnt_decode_static_shortlist_kernel<<<B, TD_THREADS, 0, stream>>>(p);
   return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
 }

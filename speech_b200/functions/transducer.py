@@ -123,11 +123,12 @@ def joint_vocab_slab_frames(B, U1, V1, budget=None):
     return max(1, min(JOINT_SLAB_FRAMES, budget // frame))
 
 
-def joint_vocab_forward(fxc, fyc, w2b, b2c, ym, blank, lp_full=None):
+def joint_vocab_forward(fxc, fyc, w2b, b2c, ym, blank, lp_full=None, shortlists=None):
     """Joint + log-softmax for any V1 (used for V1 > 64), a slab of frames at a time:
     z = relu(fx + fy) (bf16) -> logits = z W2^T + b2 (f32, GEMM) -> per-row log-sum-exp.
     fxc (B,T,H) f32, fyc (B,U1,H) f32, w2b (V1,H) bf16, b2c (V1,) f32, ym (B,U1-1) int32, all
-    contiguous on the device.  Fills lp_full (B,T,U1,V1) f32 if given.
+    contiguous on the device.  Fills lp_full (B,T,U1,V1) f32 if given, and the batch-first
+    shortlists (val, idx, meta) of sb_rnnt_shortlist_rows if given (kp = val.shape[3]).
     -> lat (nodes, 2) {log p(blank), log p(label)}, lse (nodes,) log-sum-exp of every node."""
     from .. import ops
     lib = _lib.load()
@@ -153,6 +154,13 @@ def joint_vocab_forward(fxc, fyc, w2b, b2c, ym, blank, lp_full=None):
                                                              lat.data_ptr(), lse.data_ptr(),
                                                              _lib.ptr(lp_full), B, T, U1, V1,
                                                              int(blank), t0, tc, sp))
+        if shortlists is not None:
+            val, idx, meta = shortlists
+            ops._launch("rnnt_shortlist_rows", 0.0,
+                        lambda: lib.sb_rnnt_shortlist_rows(logits.data_ptr(), ld, lse.data_ptr(), B,
+                                                           T, U1, V1, int(blank), val.shape[3], t0,
+                                                           tc, 1, val.data_ptr(), idx.data_ptr(),
+                                                           meta.data_ptr(), sp))
     return lat, lse
 
 
@@ -219,6 +227,19 @@ def _pack_labels(labels, x_lens, y_lens, B, U1, dev):
     return packed[:n], packed[n:n + B], packed[n + B:n + 2 * B], packed[n + 2 * B:]
 
 
+def _joint_operands(fx, fy, fc2, ymat):
+    """fx, fy (f32), fc2's weight (bf16, zero columns up to fx's width), bias (f32) and the label
+    matrix (int32), contiguous on fx's device, as the joint kernels take them."""
+    from .. import ops
+    H = fx.shape[2]
+    fxc, fyc = fx.detach().float().contiguous(), fy.detach().float().contiguous()
+    w2 = fc2.weight.detach().to(torch.bfloat16)
+    w2 = ops.pad_blocks(w2, 1, 1, w2.shape[1], H).contiguous()
+    b2 = fc2.bias.detach().float().contiguous()
+    ym = ymat.detach().to(fx.device, torch.int32).contiguous()
+    return fxc, fyc, w2, b2, ym
+
+
 def joint_log_probs(fx, fy, fc2, ymat, blank):
     """Full (B, T, U1, V1) log-probabilities of the joint network (what `Transducer.infer` hands
     to the beam search), from fx = fc1(x) (B,T,H), fy = fc1(pred) (B,U1,H); no autograd.
@@ -230,11 +251,7 @@ def joint_log_probs(fx, fy, fc2, ymat, blank):
     B, T, H = fx.shape
     U1 = fy.shape[1]
     V1 = fc2.weight.shape[0]
-    fxc, fyc = fx.detach().float().contiguous(), fy.detach().float().contiguous()
-    w2 = fc2.weight.detach().to(torch.bfloat16)
-    w2 = ops.pad_blocks(w2, 1, 1, w2.shape[1], H).contiguous()
-    b2 = fc2.bias.detach().float().contiguous()
-    ym = ymat.detach().to(fx.device, torch.int32).contiguous()
+    fxc, fyc, w2, b2, ym = _joint_operands(fx, fy, fc2, ymat)
     if joint_uses_slabs(H, V1):
         out = torch.empty(B, T, U1, V1, dtype=torch.float32, device=fx.device)
         joint_vocab_forward(fxc, fyc, w2, b2, ym, blank, lp_full=out)
@@ -247,6 +264,24 @@ def joint_log_probs(fx, fy, fc2, ymat, blank):
                                               b2.data_ptr(), ym.data_ptr(), lat.data_ptr(),
                                               out.data_ptr(), B, T, U1, H, V1, int(blank), sp))
     return out
+
+
+def joint_shortlists(fx, fy, fc2, ymat, blank, kp):
+    """Shortlists of the joint's log-probabilities (transducer_decoders.alloc_shortlists' layout,
+    kp entries per node) for the beam search where the full lattice is too large to hold: the
+    slabs of joint_vocab_forward, so the values are joint_log_probs' entries bit for bit, without
+    ever materialising the (B, T, U1, V1) tensor.  Arguments as joint_log_probs."""
+    from ..transducer_decoders import alloc_shortlists, shortlists_of_lp
+    _lib.require_cuda(fx, "fx")
+    B, T, H = fx.shape
+    U1 = fy.shape[1]
+    V1 = fc2.weight.shape[0]
+    if not joint_uses_slabs(H, V1):     # fc2 resident: a lattice small enough to write in full
+        return shortlists_of_lp(joint_log_probs(fx, fy, fc2, ymat, blank), kp, blank)
+    fxc, fyc, w2, b2, ym = _joint_operands(fx, fy, fc2, ymat)
+    sl = alloc_shortlists(B, T, U1, kp, fx.device)
+    joint_vocab_forward(fxc, fyc, w2, b2, ym, blank, shortlists=sl)
+    return sl
 
 
 class _JointLossFunction(torch.autograd.Function):

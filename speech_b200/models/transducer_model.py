@@ -7,7 +7,8 @@ Encoder and prediction network run on the sm_90a GRU kernels (ops.gru_stack); th
 return the reference's full log-probability tensor, written by the same fused kernel.
 The fused kernel keeps fc2's weight in shared memory, which holds up to V+1 = 64 classes; larger
 vocabularies run the same computation a slab of frames at a time (GEMM logits + row kernels of
-csrc/joint_vocab.cu), so only one slab's logits ever exist.
+csrc/joint_vocab.cu), so only one slab's logits ever exist.  Where the full lattice is too large
+for the beam search, `infer` decodes from per-node shortlists that the slab path writes instead.
 """
 import torch
 import torch.nn as nn
@@ -15,7 +16,7 @@ import torch.nn as nn
 from . import model
 from .. import ops
 from ..functions import transducer as transducer_fn
-from ..transducer_decoders import decode_static_batch
+from ..transducer_decoders import decode_static_batch, decode_static_fits, decode_static_shortlist
 
 
 class Transducer(model.Model):
@@ -94,17 +95,52 @@ class Transducer(model.Model):
     def infer(self, batch, beam_size=4):
         """Beam search on the TEACHER-FORCED lattice, as the reference does (:92-101), including
         its use of the un-subsampled input length as the time bound (clamped by slicing); in the
-        exact-lengths mode the bound is each utterance's own conv_out_size(T_b) frames."""
+        exact-lengths mode the bound is each utterance's own conv_out_size(T_b) frames.
+        Where the full-lattice search does not fit (beam_size * (V+1) * 8 bytes over 200 KB) the
+        joint writes per-node shortlists instead of the (B, T', U+1, V+1) tensor, and the search
+        runs on those, with the same predictions."""
+        if not decode_static_fits(beam_size, self.fc2.fc.out_features):
+            return self._infer_shortlists(batch, beam_size)
         with torch.no_grad():
             out = self(batch)                                  # (B, T', U+1, V+1) on the device
         # the reference slices lp[:T, :U] per utterance with the UN-subsampled T (clamped by
         # numpy slicing to T') and U = labels + 1; the search itself runs batched on the GPU
+        tlens, ulens = self._search_lens(batch, out.shape[1])
+        preds, _ = decode_static_batch(out, tlens, ulens, beam_size, self.blank)
+        return preds
+
+    def _search_lens(self, batch, frames):
         if self.exact_lengths:
             tlens = [max(0, self.conv_out_size(i.shape[0], 0)) for i in batch[0]]
         else:
-            tlens = [min(i.shape[0], out.shape[1]) for i in batch[0]]
-        ulens = [len(l) + 1 for l in batch[1]]
-        preds, _ = decode_static_batch(out, tlens, ulens, beam_size, self.blank)
+            tlens = [min(i.shape[0], frames) for i in batch[0]]
+        return tlens, [len(l) + 1 for l in batch[1]]
+
+    def _infer_shortlists(self, batch, beam_size):
+        # the joint inputs exactly as `forward` computes them
+        with torch.no_grad():
+            x, y, x_lens, y_lens = self.collate(*batch)
+            y_mat = self.label_collate(batch[1])
+            with self._grad_ctx():
+                lens = self.exact_lens(x_lens)
+                if self.is_cuda:
+                    x = x.cuda(non_blocking=True)
+                    y_mat = y_mat.cuda(non_blocking=True)
+                fx, fy = self.joint_inputs(self._encode(x, lens), y_mat)
+        T, U1 = fx.shape[1], fy.shape[1]
+        tlens, ulens = self._search_lens(batch, T)
+        tlens = [min(t, T) for t in tlens]
+        ulens = [min(u, U1) for u in ulens]
+        V1 = self.fc2.fc.out_features
+
+        # a rerun of flagged utterances (rows) recomputes the slab joint of the whole batch and
+        # keeps their rows: the joint's GEMM may sum a row differently in a smaller batch, and the
+        # rerun's lists must hold the same values as the first pass (and as `forward`) bit for bit
+        def produce(kp, rows):
+            with torch.no_grad():
+                sl = transducer_fn.joint_shortlists(fx, fy, self.fc2.fc, y_mat, self.blank, kp)
+            return sl if rows is None else tuple(a[rows].contiguous() for a in sl)
+        preds, _ = decode_static_shortlist(produce, tlens, ulens, V1, beam_size, self.blank)
         return preds
 
     def label_collate(self, labels):

@@ -8,12 +8,104 @@ a whole minibatch of lattices with one launch and one device->host copy (what
 `Transducer.infer` uses).  The dependency is un-vendored (Makefile:10-12), so the algorithm is the
 standard transducer beam search on a static lattice; its CPU restatement and how it is pinned are
 in oracle/decode_static_ref.py (test infrastructure - not imported here).  There is no CPU path.
+
+The search keeps every candidate in shared memory where beam_size * V * 8 bytes fit in 200 KB
+(`decode_static_fits`).  Larger vocabularies search per-node shortlists instead (the kp = beam_size
+best non-blank classes, csrc/tdecode.cu), with the same results bit for bit: the kernel flags any
+selection the lists cannot prove, and flagged utterances are searched again from lists of
+SHORTLIST_RERUN entries.
 """
 import ctypes
 
 import torch
 
 from . import _lib
+
+SHORTLIST_RERUN = 64      # list length of the second search of flagged utterances (the maximum)
+
+
+def decode_static_fits(beam_size, V):
+    """True where sb_rnnt_decode_static holds the beam_size * V candidates in shared memory
+    (beam_size * V * 8 + 16 <= 200 KB, beam_size <= 32); elsewhere the shortlist search runs."""
+    return bool(_lib.load().sb_rnnt_decode_static_fits(int(beam_size), int(V)))
+
+
+def alloc_shortlists(B, T, U1, kp, device):
+    """Empty batch-first shortlists: values (B,T,U1,kp) f32, classes (B,T,U1,kp) int32 and
+    {blank lp, next lp} (B,T,U1,2) f32, as sb_rnnt_shortlist_rows writes them."""
+    return (torch.empty(B, T, U1, kp, dtype=torch.float32, device=device),
+            torch.empty(B, T, U1, kp, dtype=torch.int32, device=device),
+            torch.empty(B, T, U1, 2, dtype=torch.float32, device=device))
+
+
+def shortlists_of_lp(lp, kp, blank):
+    """Shortlists of a given (B, T, U1, V) float32 CUDA log-probability tensor."""
+    from . import ops
+    lib = _lib.load()
+    B, T, U1, V = lp.shape
+    val, idx, meta = alloc_shortlists(B, T, U1, kp, lp.device)
+    with torch.cuda.device(lp.device):
+        sp = _lib.stream_ptr()
+        ops._launch("rnnt_shortlist_rows", 0.0,
+                    lambda: lib.sb_rnnt_shortlist_rows(lp.data_ptr(), V, None, B, T, U1, V,
+                                                       int(blank), int(kp), 0, T, 0,
+                                                       val.data_ptr(), idx.data_ptr(),
+                                                       meta.data_ptr(), sp))
+    return val, idx, meta
+
+
+def _shortlist_search(sl, tl, ul, V, beam_size, blank):
+    """One sb_rnnt_decode_static_shortlist launch over the shortlists sl of len(tl) utterances ->
+    (label lists, log-probabilities, flag counts) on the host."""
+    from . import ops
+    lib = _lib.load()
+    val, idx, meta = sl
+    B, T, U1, kp = val.shape
+    dev = val.device
+    lens = torch.tensor(list(tl) + list(ul), dtype=torch.int32).pin_memory().to(dev,
+                                                                                non_blocking=True)
+    nbytes = ctypes.c_size_t(0)
+    _lib.check(lib.sb_rnnt_decode_static_workspace_size(B, T, U1, int(beam_size),
+                                                        ctypes.byref(nbytes)), "ws")
+    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+    labels = torch.empty(B, U1, dtype=torch.int32, device=dev)
+    counts = torch.empty(2, B, dtype=torch.int32, device=dev)      # lengths, flags
+    scores = torch.empty(B, dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        sp = _lib.stream_ptr()
+        ops._launch("rnnt_decode_static", 0.0,
+                    lambda: lib.sb_rnnt_decode_static_shortlist(
+                        val.data_ptr(), idx.data_ptr(), meta.data_ptr(), kp, lens[:B].data_ptr(),
+                        lens[B:].data_ptr(), B, T, U1, V, int(beam_size), int(blank),
+                        labels.data_ptr(), counts[0].data_ptr(), scores.data_ptr(),
+                        counts[1].data_ptr(), ws.data_ptr(), nbytes.value, sp))
+    lab = labels.cpu()
+    n, flags = counts.cpu().tolist()
+    return [lab[b, :n[b]].tolist() for b in range(B)], scores.cpu().tolist(), flags
+
+
+def decode_static_shortlist(produce, tlens, ulens, V, beam_size, blank):
+    """Beam search over shortlists: produce(kp, rows) returns the shortlists (alloc_shortlists'
+    layout) of the utterances `rows` (None: all of them) at kp entries per node.  Searches from
+    kp = beam_size lists, then searches again every utterance the kernel flagged from
+    SHORTLIST_RERUN-entry lists; an utterance flagged there too raises rather than return an
+    unproven hypothesis.  tlens / ulens are already clamped to the lattice.
+    Returns (list of label lists, list of log-probabilities)."""
+    labels, scores, flags = _shortlist_search(produce(int(beam_size), None), tlens, ulens, V,
+                                              beam_size, blank)
+    rerun = [b for b, f in enumerate(flags) if f]
+    if rerun:
+        sl = produce(SHORTLIST_RERUN, rerun)
+        lab2, sc2, fl2 = _shortlist_search(sl, [tlens[b] for b in rerun],
+                                           [ulens[b] for b in rerun], V, beam_size, blank)
+        if any(fl2):
+            raise _lib.SpeechB200Error(
+                "speech_b200: the shortlist beam search cannot order tied candidates of "
+                "utterance(s) %s even from %d-entry lists" %
+                ([b for b, f in zip(rerun, fl2) if f], SHORTLIST_RERUN))
+        for j, b in enumerate(rerun):
+            labels[b], scores[b] = lab2[j], sc2[j]
+    return labels, scores
 
 
 def decode_static_batch(lp, tlens, ulens, beam_size, blank):
@@ -25,8 +117,13 @@ def decode_static_batch(lp, tlens, ulens, beam_size, blank):
     lp = lp.detach().float().contiguous()
     B, T, U1, V = lp.shape
     dev = lp.device
-    lens = torch.tensor([min(int(t), T) for t in tlens] + [min(int(u), U1) for u in ulens],
-                        dtype=torch.int32).pin_memory().to(dev, non_blocking=True)
+    tl = [min(int(t), T) for t in tlens]
+    ul = [min(int(u), U1) for u in ulens]
+    if not decode_static_fits(beam_size, V):
+        def produce(kp, rows):
+            return shortlists_of_lp(lp if rows is None else lp[rows].contiguous(), kp, blank)
+        return decode_static_shortlist(produce, tl, ul, V, beam_size, blank)
+    lens = torch.tensor(tl + ul, dtype=torch.int32).pin_memory().to(dev, non_blocking=True)
     nbytes = ctypes.c_size_t(0)
     _lib.check(lib.sb_rnnt_decode_static_workspace_size(B, T, U1, int(beam_size),
                                                         ctypes.byref(nbytes)), "ws")

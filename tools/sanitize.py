@@ -152,3 +152,15 @@ _lib.check(lib.sb_ctc_fwd_bwd_compact(acts.data_ptr(), g.data_ptr(), dl.data_ptr
                                       _lib.stream_ptr()), "sb_ctc_fwd_bwd_compact")
 torch.cuda.synchronize()
 print("ctc compact / shortlist entries ok", c.tolist(), o_len.tolist())
+# the Transducer at a subword-sized vocabulary (V+1 = 20001): infer's shortlist route (slab joint
+# with the shortlist producer, then the shortlist beam search), the producer on a given lattice and
+# the search's flag rerun at 64-entry lists
+tv = Transducer(80, 20000, cfg).cuda()
+l14 = tv.loss((inputs, labels4)); l14.backward()
+print("transducer V+1=20001 ok", l14.item(), [len(p) for p in tv.infer((inputs, labels4), beam_size=4)])
+from speech_b200.transducer_decoders import decode_static
+sys.path.insert(0, "tests")
+from test_rnnt_shortlist_host import tie_lattice          # the lattice the tests flag
+tie, blank = tie_lattice()
+print("rnnt shortlist rerun ok", decode_static(tie, 2, blank))
+torch.cuda.synchronize()
