@@ -5,16 +5,17 @@
 // so that hypotheses come out IDENTICAL to the reference, including its tie-breaks:
 //   * beam entries carry (p_blank, p_non_blank) in float64 log space, as the reference's Python
 //     floats; log-sum-exp is evaluated in the reference's argument order;
-//   * prefixes are nodes (parent, symbol) of a per-utterance trie, so "prefix + s is already in
-//     the beam" (the merge case, ctc_decoder.py:84-103) is an integer comparison;
-//   * pruning = repeated arg-max over (score desc, first-touch rank asc): the reference sorts
-//     a dict's items with a stable sort, so ties keep dict insertion order, which is the order
-//     of first touch in its `for s in vocab: for prefix in beam:` loops (ctc_decoder.py:65-103).
+//   * prefixes are nodes of a per-utterance trie (beam.cuh), so "prefix + s is already in the
+//     beam" (the merge case, ctc_decoder.py:84-103) is an integer comparison;
+//   * pruning = K rounds of the selection of beam.cuh with the first-touch rank as the key: the
+//     reference sorts a dict's items with a stable sort, so ties keep dict insertion order, which
+//     is the order of first touch in its `for s in vocab: for prefix in beam:` loops
+//     (ctc_decoder.py:65-103).
 // Input is log-probabilities (the host wrapper applies the same float32 log as the reference).
 //
 // Roofline: HBM-nominal (reads T*S floats per utterance), in practice latency-bound by the
 // T-serial beam update; decode is not on the training path.
-#include "common.cuh"
+#include "beam.cuh"
 #include <math.h>
 
 #include "../../include/speech_b200.h"
@@ -27,10 +28,7 @@ static constexpr int DEC_MAX_BEAM = 32;
 struct DecParams {
   const float* logp;   // (B, T, S)
   const int* lens;     // (B) frames per utterance (<= T)
-  int* nodes;          // (B, 2*(T*K+1)) trie arena: parent, symbol
-  unsigned long long* hkeys;  // (B, hcap) (parent, symbol) -> node id map: keys (0 = empty)
-  int* hvals;                 // (B, hcap)
-  int hcap;                   // power of two >= 2*(T*K+1)
+  BeamTrie trie;       // utterance 0 of B; T*K + 1 nodes each
   int* out_labels;     // (B, T)
   int* out_lens;       // (B)
   double* out_scores;  // (B)  negative log-likelihood of the best prefix
@@ -132,98 +130,50 @@ __device__ __forceinline__ bool cand_value(const Beam& cur, int c, const float* 
   return true;
 }
 
-// (score desc, rank asc): the order of the reference's stable sort
-__device__ __forceinline__ bool dec_better(double s, int r, double bs, int br) {
-  return s > bs || (s == bs && r < br);
-}
-
-// Block arg-max of the threads' (bs, br, bc) (bc < 0: none); the winner ends up in thread 0.
-__device__ __forceinline__ void dec_block_argmax(double& bs, int& br, int& bc, double* red_s,
-                                                 int* red_r, int* red_c) {
+// One selection round over the scored candidates of a frame: the first live one by (score desc,
+// rank asc) is struck off and returned to every thread, with its score and rank (-1: none left).
+// live[c] is read and written by thread c % DEC_THREADS only, so striking needs no barrier.
+__device__ __forceinline__ int dec_take_first(const double* score, const int* rank,
+                                              unsigned char* live, int ncand, double& bs, int& br) {
   const int tid = threadIdx.x;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const double os = __shfl_xor_sync(0xffffffffu, bs, o);
-    const int orr = __shfl_xor_sync(0xffffffffu, br, o);
-    const int oc = __shfl_xor_sync(0xffffffffu, bc, o);
-    if (oc >= 0 && (bc < 0 || os > bs || (os == bs && orr < br))) { bs = os; br = orr; bc = oc; }
+  bs = d_neg_inf();
+  br = -1;
+  int bc = -1;
+  for (int c = tid; c < ncand; c += DEC_THREADS) {
+    if (!live[c]) continue;
+    if (beam_before(score[c], rank[c], bs, br)) { bs = score[c]; br = rank[c]; bc = c; }
   }
-  if ((tid & 31) == 0) { red_s[tid >> 5] = bs; red_r[tid >> 5] = br; red_c[tid >> 5] = bc; }
-  __syncthreads();
-  if (tid == 0) {
-    for (int w = 1; w < DEC_THREADS / 32; ++w) {
-      if (red_c[w] >= 0 && (bc < 0 || red_s[w] > bs || (red_s[w] == bs && red_r[w] < br))) {
-        bs = red_s[w]; br = red_r[w]; bc = red_c[w];
-      }
-    }
-  }
+  beam_block_first<DEC_THREADS>(bs, br, bc);
+  if (bc >= 0 && (bc & (DEC_THREADS - 1)) == tid) live[bc] = 0;
+  return bc;
 }
 
-// Per-utterance search state in global memory: trie arena and (parent, symbol) -> node map.
-struct DecUtt {
-  int* nodes;
-  unsigned long long* hkeys;
-  int* hvals;
-};
-
-__device__ __forceinline__ DecUtt dec_begin(const DecParams& p, Beam* beams) {
-  const int b = blockIdx.x, tid = threadIdx.x;
-  DecUtt u;
-  u.nodes = p.nodes + (size_t)b * 2 * ((size_t)p.T * p.K + 1);
-  u.hkeys = p.hkeys + (size_t)b * p.hcap;
-  u.hvals = p.hvals + (size_t)b * p.hcap;
-  // Node ids must be CANONICAL over the whole utterance: a prefix that is pruned and later
-  // re-created has to get its old id back, because surviving descendants still name it as parent.
-  for (int k = tid; k < p.hcap; k += DEC_THREADS) u.hkeys[k] = 0ull;
-
-  if (tid == 0) {
+__device__ __forceinline__ void dec_begin(const DecParams& p, Beam* beams) {
+  if (threadIdx.x == 0) {
     beams[0].size = 1;
     beams[0].pb[0] = 0.0;
     beams[0].pnb[0] = d_neg_inf();
     beams[0].node[0] = 0;
     beams[0].last[0] = -1;
     beams[0].parent[0] = -1;
-    u.nodes[0] = -1;
-    u.nodes[1] = -1;
   }
-  __syncthreads();
-  return u;
+  p.trie.of(blockIdx.x).clear<DEC_THREADS>();
 }
 
-// Materialise the pruned beam of frame t from the ns selected candidates (full-scan numbering).
-__device__ __forceinline__ void dec_commit(const DecParams& p, const DecUtt& u, const Beam& cur, Beam& nxt,
-                           const int* sel, int ns, const float* lp, int t) {
+// Materialise the pruned beam of frame t: thread r < ns holds the r-th selected candidate in `mine`
+// (full-scan numbering).
+__device__ __forceinline__ void dec_commit(const DecParams& p, const Beam& cur, Beam& nxt, int mine,
+                                           int ns, const float* lp, int t) {
   const int tid = threadIdx.x, K = p.K, S = p.S;
   if (tid < ns) {
-    const int c = sel[tid];
+    const int c = mine;
     if (c < K * S) {
       const int i = c / S, s = c - i * S;
       double x; int rk;
       ext_value(cur, i, s, lp, K, x, rk);
-      // find-or-insert (parent node, symbol) in the utterance's hash map
-      const unsigned long long key =
-          ((unsigned long long)(unsigned int)cur.node[i] << 32) | (unsigned int)(s + 1);
-      unsigned int h = (unsigned int)((key * 0x9E3779B97F4A7C15ull) >> 32) & (p.hcap - 1);
-      int id = -1;
-      for (int probe = 0; probe < p.hcap; ++probe) {
-        const unsigned long long k = u.hkeys[h];
-        if (k == key) { id = u.hvals[h]; break; }
-        if (k == 0ull) {
-          const unsigned long long old = atomicCAS(&u.hkeys[h], 0ull, key);
-          if (old == 0ull) {
-            id = 1 + t * K + tid;
-            u.hvals[h] = id;
-            u.nodes[2 * id] = cur.node[i];
-            u.nodes[2 * id + 1] = s;
-            break;
-          }
-          if (old == key) { id = u.hvals[h]; break; }
-        }
-        h = (h + 1) & (p.hcap - 1);
-      }
       nxt.pb[tid] = d_neg_inf();
       nxt.pnb[tid] = x;
-      nxt.node[tid] = id;
+      nxt.node[tid] = p.trie.of(blockIdx.x).find_or_insert<true>(cur.node[i], s, 1 + t * K + tid);
       nxt.last[tid] = s;
       nxt.parent[tid] = cur.node[i];
     } else {
@@ -242,16 +192,10 @@ __device__ __forceinline__ void dec_commit(const DecParams& p, const DecUtt& u, 
 }
 
 // Best hypothesis of the final beam: back-track the trie.
-__device__ __forceinline__ void dec_finish(const DecParams& p, const DecUtt& u, const Beam& fin) {
+__device__ __forceinline__ void dec_finish(const DecParams& p, const Beam& fin) {
   if (threadIdx.x == 0) {
     const int b = blockIdx.x;
-    int n = fin.node[0];
-    int len = 0;
-    for (int q = n; q > 0; q = u.nodes[2 * q]) ++len;
-    int* out = p.out_labels + (size_t)b * p.T;
-    int k = len;
-    for (int q = n; q > 0; q = u.nodes[2 * q]) out[--k] = u.nodes[2 * q + 1];
-    p.out_lens[b] = len;
+    p.out_lens[b] = p.trie.of(b).backtrack(fin.node[0], p.out_labels + (size_t)b * p.T);
     p.out_scores[b] = -lse2d(fin.pb[0], fin.pnb[0]);
   }
 }
@@ -265,154 +209,37 @@ __global__ void __launch_bounds__(DEC_THREADS) ctc_prefix_beam_kernel(const DecP
   int* rank = reinterpret_cast<int*>(score + ncand);               // [ncand]
   unsigned char* live = reinterpret_cast<unsigned char*>(rank + ncand);  // [ncand]
   __shared__ Beam beams[2];
-  __shared__ double red_s[DEC_THREADS / 32];
-  __shared__ int red_r[DEC_THREADS / 32];
-  __shared__ int red_c[DEC_THREADS / 32];
-  __shared__ int sel[DEC_MAX_BEAM];
-  __shared__ int nsel;
 
-  int* nodes = p.nodes + (size_t)b * 2 * ((size_t)p.T * K + 1);
-  unsigned long long* hkeys = p.hkeys + (size_t)b * p.hcap;
-  int* hvals = p.hvals + (size_t)b * p.hcap;
+  dec_begin(p, beams);
   const float* logp = p.logp + (size_t)b * p.T * S;
-  // Node ids must be CANONICAL over the whole utterance: a prefix that is pruned and later
-  // re-created has to get its old id back, because surviving descendants still name it as parent.
-  for (int k = tid; k < p.hcap; k += DEC_THREADS) hkeys[k] = 0ull;
-
-  if (tid == 0) {
-    beams[0].size = 1;
-    beams[0].pb[0] = 0.0;
-    beams[0].pnb[0] = d_neg_inf();
-    beams[0].node[0] = 0;
-    beams[0].last[0] = -1;
-    beams[0].parent[0] = -1;
-    nodes[0] = -1;
-    nodes[1] = -1;
-  }
-  __syncthreads();
 
   for (int t = 0; t < T; ++t) {
     const Beam& cur = beams[t & 1];
     Beam& nxt = beams[(t & 1) ^ 1];
     const float* lp = logp + (size_t)t * S;
-    const int nb = cur.size;
     // ---- 1. score every candidate ----
     for (int c = tid; c < ncand; c += DEC_THREADS) {
-      double sc = d_neg_inf();
-      int rk = 0x7fffffff;
-      bool ok = false;
-      if (c < K * S) {
-        const int i = c / S, s = c - i * S;
-        if (i < nb && s != p.blank) {
-          double x;
-          ok = ext_value(cur, i, s, lp, K, x, rk);
-          if (ok) sc = x;  // logsumexp(-inf, x) == x exactly
-        }
-      } else {
-        const int j = c - K * S;
-        if (j < nb) {
-          double npb, npnb;
-          stay_value(cur, j, lp, p.blank, K, npb, npnb, rk);
-          sc = lse2d(npb, npnb);
-          ok = true;
-        }
-      }
+      double sc;
+      int rk;
+      live[c] = cand_value(cur, c, lp, K, S, p.blank, sc, rk) ? 1 : 0;
       score[c] = sc;
       rank[c] = rk;
-      live[c] = ok ? 1 : 0;
     }
     __syncthreads();
-    // ---- 2. K rounds of arg-max by (score desc, rank asc) ----
-    if (tid == 0) nsel = 0;
+    // ---- 2. the K first by (score desc, rank asc); thread r keeps the r-th ----
+    int ns = 0, mine = -1;
     for (int r = 0; r < K; ++r) {
-      double bs = d_neg_inf();
-      int br = 0x7fffffff, bc = -1;
-      for (int c = tid; c < ncand; c += DEC_THREADS) {
-        if (!live[c]) continue;
-        const double sc = score[c];
-        const int rk = rank[c];
-        if (bc < 0 || sc > bs || (sc == bs && rk < br)) { bs = sc; br = rk; bc = c; }
-      }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        const double os = __shfl_xor_sync(0xffffffffu, bs, o);
-        const int orr = __shfl_xor_sync(0xffffffffu, br, o);
-        const int oc = __shfl_xor_sync(0xffffffffu, bc, o);
-        if (oc >= 0 && (bc < 0 || os > bs || (os == bs && orr < br))) { bs = os; br = orr; bc = oc; }
-      }
-      if ((tid & 31) == 0) { red_s[tid >> 5] = bs; red_r[tid >> 5] = br; red_c[tid >> 5] = bc; }
-      __syncthreads();
-      if (tid == 0) {
-        for (int w = 1; w < DEC_THREADS / 32; ++w) {
-          if (red_c[w] >= 0 && (bc < 0 || red_s[w] > bs || (red_s[w] == bs && red_r[w] < br))) {
-            bs = red_s[w]; br = red_r[w]; bc = red_c[w];
-          }
-        }
-        if (bc >= 0) { sel[nsel++] = bc; live[bc] = 0; }
-      }
-      __syncthreads();
+      double bs;
+      int br;
+      const int bc = dec_take_first(score, rank, live, ncand, bs, br);
+      if (bc < 0) break;
+      if (tid == ns) mine = bc;
+      ++ns;
     }
     // ---- 3. materialise the pruned beam ----
-    const int ns = nsel;
-    if (tid < ns) {
-      const int c = sel[tid];
-      if (c < K * S) {
-        const int i = c / S, s = c - i * S;
-        double x; int rk;
-        ext_value(cur, i, s, lp, K, x, rk);
-        // find-or-insert (parent node, symbol) in the utterance's hash map
-        const unsigned long long key =
-            ((unsigned long long)(unsigned int)cur.node[i] << 32) | (unsigned int)(s + 1);
-        unsigned int h = (unsigned int)((key * 0x9E3779B97F4A7C15ull) >> 32) & (p.hcap - 1);
-        int id = -1;
-        for (int probe = 0; probe < p.hcap; ++probe) {
-          const unsigned long long k = hkeys[h];
-          if (k == key) { id = hvals[h]; break; }
-          if (k == 0ull) {
-            const unsigned long long old = atomicCAS(&hkeys[h], 0ull, key);
-            if (old == 0ull) {
-              id = 1 + t * K + tid;
-              hvals[h] = id;
-              nodes[2 * id] = cur.node[i];
-              nodes[2 * id + 1] = s;
-              break;
-            }
-            if (old == key) { id = hvals[h]; break; }
-          }
-          h = (h + 1) & (p.hcap - 1);
-        }
-        nxt.pb[tid] = d_neg_inf();
-        nxt.pnb[tid] = x;
-        nxt.node[tid] = id;
-        nxt.last[tid] = s;
-        nxt.parent[tid] = cur.node[i];
-      } else {
-        const int j = c - K * S;
-        double npb, npnb; int rk;
-        stay_value(cur, j, lp, p.blank, K, npb, npnb, rk);
-        nxt.pb[tid] = npb;
-        nxt.pnb[tid] = npnb;
-        nxt.node[tid] = cur.node[j];
-        nxt.last[tid] = cur.last[j];
-        nxt.parent[tid] = cur.parent[j];
-      }
-    }
-    if (tid == 0) nxt.size = ns;
-    __syncthreads();
+    dec_commit(p, cur, nxt, mine, ns, lp, t);
   }
-
-  // ---- best hypothesis: back-track the trie ----
-  if (tid == 0) {
-    const Beam& fin = beams[T & 1];
-    int n = fin.node[0];
-    int len = 0;
-    for (int q = n; q > 0; q = nodes[2 * q]) ++len;
-    int* out = p.out_labels + (size_t)b * p.T;
-    int k = len;
-    for (int q = n; q > 0; q = nodes[2 * q]) out[--k] = nodes[2 * q + 1];
-    p.out_lens[b] = len;
-    p.out_scores[b] = -lse2d(fin.pb[0], fin.pnb[0]);
-  }
+  dec_finish(p, beams[T & 1]);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -445,52 +272,29 @@ __global__ void __launch_bounds__(DEC_THREADS) ctc_prefix_beam_kernel(const DecP
 // ------------------------------------------------------------------------------------------------
 static constexpr int DEC_SL_THREADS = 256;
 
-// (p desc, s asc) order of the shortlist: true if (x, s) comes strictly after (px, ps)
-__device__ __forceinline__ bool sl_after(float x, int s, float px, int ps) {
-  return x < px || (x == px && s > ps);
-}
-
 // grid (T, B): shortlist[(b*T + t)*LS + j], j < L, for the frames t < lens[b]
 __global__ void __launch_bounds__(DEC_SL_THREADS) ctc_shortlist_kernel(
     const float* __restrict__ logp, const int* __restrict__ lens, int* __restrict__ shortlist,
     int T, int S, int blank, int L, int LS) {
   const int t = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
   if (t >= min(lens[b], T)) return;
-  __shared__ float red_x[DEC_SL_THREADS / 32];
-  __shared__ int red_s[DEC_SL_THREADS / 32];
-  __shared__ float prev_x;
-  __shared__ int prev_s;
   const float* lp = logp + ((size_t)b * T + t) * S;
   int* out = shortlist + ((size_t)b * T + t) * LS;
+  float px = 0.f;                          // the previous round's symbol: (p desc, s asc) order
+  int ps = -1;
   for (int j = 0; j < L; ++j) {
-    const float px = j ? prev_x : 0.f;
-    const int ps = j ? prev_s : -1;
     float bx = 0.f;
     int bsym = -1;
     for (int s = tid; s < S; s += DEC_SL_THREADS) {
       if (s == blank) continue;
       const float x = __ldg(lp + s);
-      if (j && !sl_after(x, s, px, ps)) continue;
-      if (bsym < 0 || !sl_after(x, s, bx, bsym)) { bx = x; bsym = s; }
+      if (j && !beam_order(px, ps, x, s)) continue;     // listed in an earlier round
+      if (beam_before(x, s, bx, bsym)) { bx = x; bsym = s; }
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float ox = __shfl_xor_sync(0xffffffffu, bx, o);
-      const int os = __shfl_xor_sync(0xffffffffu, bsym, o);
-      if (os >= 0 && (bsym < 0 || !sl_after(ox, os, bx, bsym))) { bx = ox; bsym = os; }
-    }
-    if ((tid & 31) == 0) { red_x[tid >> 5] = bx; red_s[tid >> 5] = bsym; }
-    __syncthreads();
-    if (tid == 0) {
-      for (int w = 1; w < DEC_SL_THREADS / 32; ++w)
-        if (red_s[w] >= 0 && (bsym < 0 || !sl_after(red_x[w], red_s[w], bx, bsym))) {
-          bx = red_x[w]; bsym = red_s[w];
-        }
-      out[j] = bsym;
-      prev_x = bx;
-      prev_s = bsym;
-    }
-    __syncthreads();
+    beam_block_first<DEC_SL_THREADS>(bx, bsym);
+    if (tid == 0) out[j] = bsym;
+    px = bx;
+    ps = bsym;
   }
 }
 
@@ -506,17 +310,10 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) ctc_prefix_beam_shortlist_kern
   int* full = rank + ncand;                                        // [ncand] full-scan number
   unsigned char* live = reinterpret_cast<unsigned char*>(full + ncand);  // [ncand]
   __shared__ Beam beams[2];
-  __shared__ double red_s[DEC_THREADS / 32];
-  __shared__ int red_r[DEC_THREADS / 32];
-  __shared__ int red_c[DEC_THREADS / 32];
-  __shared__ int sel[DEC_MAX_BEAM];
-  __shared__ int nsel;
-  __shared__ double last_s;
-  __shared__ int last_r;
   __shared__ int rescan;
   const bool complete = L >= S - 1;        // every non-blank symbol is on the list
 
-  const DecUtt u = dec_begin(p, beams);
+  dec_begin(p, beams);
   const float* logp = p.logp + (size_t)b * p.T * S;
 
   for (int t = 0; t < T; ++t) {
@@ -553,25 +350,19 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) ctc_prefix_beam_shortlist_kern
       live[c] = ok ? 1 : 0;
     }
     __syncthreads();
-    // ---- 2. K rounds of arg-max by (score desc, rank asc), as the full scan ----
-    if (tid == 0) nsel = 0;
+    // ---- 2. the K first by (score desc, rank asc), as the full scan; thread r keeps the r-th,
+    //         every thread the score and rank of the last ----
+    int ns = 0, mine = -1, last_r = -1;
+    double last_s = d_neg_inf();
     for (int r = 0; r < K; ++r) {
-      double bs = d_neg_inf();
-      int br = 0x7fffffff, bc = -1;
-      for (int c = tid; c < ncand; c += DEC_THREADS) {
-        if (!live[c]) continue;
-        const double sc = score[c];
-        const int rk = rank[c];
-        if (bc < 0 || sc > bs || (sc == bs && rk < br)) { bs = sc; br = rk; bc = c; }
-      }
-      dec_block_argmax(bs, br, bc, red_s, red_r, red_c);
-      if (tid == 0 && bc >= 0) {
-        sel[nsel++] = full[bc];
-        live[bc] = 0;
-        last_s = bs;
-        last_r = br;
-      }
-      __syncthreads();
+      double bs;
+      int br;
+      const int bc = dec_take_first(score, rank, live, ncand, bs, br);
+      if (bc < 0) break;
+      if (tid == ns) mine = full[bc];
+      ++ns;
+      last_s = bs;
+      last_r = br;
     }
     // ---- 3. check that no left-out candidate can reach the selection ----
     if (!complete && tid < 32) {
@@ -581,7 +372,7 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) ctc_prefix_beam_shortlist_kern
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) U = fmax(U, __shfl_xor_sync(0xffffffffu, U, o));
       if (tid == 0) {
-        bool ok = nsel == K && last_s != d_neg_inf();
+        bool ok = ns == K && last_s != d_neg_inf();
         if (ok && U != d_neg_inf()) ok = last_s > U + 1e-12 * (1.0 + fabs(U));
         rescan = ok ? 0 : 1;
       }
@@ -589,45 +380,40 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) ctc_prefix_beam_shortlist_kern
     __syncthreads();
     // ---- 3b. otherwise: full streamed scan of this frame ----
     if (!complete && rescan) {
-      if (tid == 0) nsel = 0;
+      ns = 0;
       for (int r = 0; r < K; ++r) {
-        const double ps = last_s;
-        const int pr = last_r;
         double bs = d_neg_inf();
-        int br = 0x7fffffff, bc = -1;
+        int br = -1, bc = -1;
         for (int c = tid; c < K * S + K; c += DEC_THREADS) {
           double sc;
           int rk;
           if (!cand_value(cur, c, lp, K, S, p.blank, sc, rk)) continue;
-          if (r > 0 && !dec_better(ps, pr, sc, rk)) continue;   // selected in an earlier round
-          if (bc < 0 || dec_better(sc, rk, bs, br)) { bs = sc; br = rk; bc = c; }
+          if (r > 0 && !beam_order(last_s, last_r, sc, rk)) continue;   // selected earlier
+          if (beam_before(sc, rk, bs, br)) { bs = sc; br = rk; bc = c; }
         }
-        dec_block_argmax(bs, br, bc, red_s, red_r, red_c);
-        if (tid == 0 && bc >= 0) { sel[nsel++] = bc; last_s = bs; last_r = br; }
-        __syncthreads();
-        if (nsel <= r) break;
+        beam_block_first<DEC_THREADS>(bs, br, bc);
+        if (bc < 0) break;
+        if (tid == ns) mine = bc;
+        ++ns;
+        last_s = bs;
+        last_r = br;
       }
     }
     // ---- 4. materialise the pruned beam ----
-    dec_commit(p, u, cur, nxt, sel, nsel, lp, t);
+    dec_commit(p, cur, nxt, mine, ns, lp, t);
   }
-  dec_finish(p, u, beams[T & 1]);
+  dec_finish(p, beams[T & 1]);
 }
 
 }  // namespace sb
 
 using namespace sb;
 
-static int dec_hash_cap(int T, int K) {
-  size_t need = 2 * ((size_t)T * K + 1);
-  size_t cap = 64;
-  while (cap < need) cap <<= 1;
-  return (int)cap;
-}
+static size_t dec_node_cap(int T, int K) { return (size_t)T * K + 1; }
 
 static size_t dec_shortlist_offset(int B, int T, int K) {
-  const size_t cap = (size_t)dec_hash_cap(T, K);
-  return (size_t)B * 2 * ((size_t)T * K + 1) * sizeof(int) + 256 +
+  const size_t cap = (size_t)beam_pow2_cap(2 * dec_node_cap(T, K));
+  return (size_t)B * 2 * dec_node_cap(T, K) * sizeof(int) + 256 +
          (size_t)B * cap * (sizeof(unsigned long long) + sizeof(int)) + 512;
 }
 
@@ -653,12 +439,15 @@ static int dec_entry(const float* logp, const int* lens, int B, int T, int S, in
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   DecParams p;
   p.logp = logp; p.lens = lens;
-  p.nodes = reinterpret_cast<int*>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
-  p.hcap = dec_hash_cap(T, beam_size);
-  p.hkeys = reinterpret_cast<unsigned long long*>(
-      (reinterpret_cast<uintptr_t>(p.nodes + (size_t)B * 2 * ((size_t)T * beam_size + 1)) + 255) &
+  BeamTrie& tr = p.trie;
+  tr.node_cap = (int)dec_node_cap(T, beam_size);
+  tr.cap = beam_pow2_cap(2 * dec_node_cap(T, beam_size));
+  tr.nodes =
+      reinterpret_cast<int*>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
+  tr.keys = reinterpret_cast<unsigned long long*>(
+      (reinterpret_cast<uintptr_t>(tr.nodes + (size_t)B * 2 * tr.node_cap) + 255) &
       ~(uintptr_t)255);
-  p.hvals = reinterpret_cast<int*>(p.hkeys + (size_t)B * p.hcap);
+  tr.vals = reinterpret_cast<int*>(tr.keys + (size_t)B * tr.cap);
   p.out_labels = out_labels; p.out_lens = out_lens; p.out_scores = out_scores;
   p.B = B; p.T = T; p.S = S; p.K = beam_size; p.blank = blank;
 
@@ -711,44 +500,20 @@ extern "C" int sb_ctc_prefix_beam_shortlist(const float* logp, const int* lens, 
 // sb_beam_topk: the expand/prune step of Seq2Seq.beam_search (speech/models/seq2seq.py:200-212):
 // the reference sorts ALL beam x vocab candidates with a stable descending sort and keeps a
 // prefix, so ties keep (beam index, vocab index) order = ascending flat index.  One CTA selects
-// the top k of n float64 scores by k rounds of block arg-max on (score desc, index asc).
+// the top k of n float64 scores by k rounds of beam_take_first.
 // ------------------------------------------------------------------------------------------------
 namespace sb {
 __global__ void __launch_bounds__(256) beam_topk_kernel(const double* __restrict__ scores, int n,
                                                         int k, int* out_idx, double* out_val) {
   extern __shared__ unsigned char topk_smem[];
   double* sc = reinterpret_cast<double*>(topk_smem);
-  __shared__ double rs[8];
-  __shared__ int ri[8];
   const int tid = threadIdx.x;
   for (int i = tid; i < n; i += 256) sc[i] = scores[i];
   __syncthreads();
   for (int r = 0; r < k; ++r) {
-    double bs = 0.0;
-    int bi = -1;
-    for (int i = tid; i < n; i += 256) {
-      const double v = sc[i];
-      if (isnan(v)) continue;                      // NaN marks "already taken"
-      if (bi < 0 || v > bs) { bs = v; bi = i; }    // ascending i: first index wins ties
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const double os = __shfl_xor_sync(0xffffffffu, bs, o);
-      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-      if (oi >= 0 && (bi < 0 || os > bs || (os == bs && oi < bi))) { bs = os; bi = oi; }
-    }
-    if ((tid & 31) == 0) { rs[tid >> 5] = bs; ri[tid >> 5] = bi; }
-    __syncthreads();
-    if (tid == 0) {
-      for (int w = 1; w < 8; ++w)
-        if (ri[w] >= 0 && (bi < 0 || rs[w] > bs || (rs[w] == bs && ri[w] < bi))) {
-          bs = rs[w]; bi = ri[w];
-        }
-      out_idx[r] = bi;
-      out_val[r] = bs;
-      if (bi >= 0) sc[bi] = nan("");
-    }
-    __syncthreads();
+    double bs;
+    const int bi = beam_take_first<256>(sc, n, bs);
+    if (tid == 0) { out_idx[r] = bi; out_val[r] = bs; }
   }
 }
 }  // namespace sb

@@ -30,7 +30,7 @@
 // over all (u, b) rows and run once per sequence on the wgmma GEMM (SB_GEMM_A_MN | SB_GEMM_B_MN).
 // Everything is fp32 (the reference's arithmetic); roofline: L2 bandwidth on eh and the cell
 // weights per token (B*T*H*4 bytes forward, 3x that backward, + 24 H^2), in practice launch-bound.
-#include "common.cuh"
+#include "beam.cuh"
 #include <math.h>
 #include <string.h>
 
@@ -848,8 +848,10 @@ __global__ void __launch_bounds__(32 * CELL_WARPS) s2s_cell_bwd_kernel(const Cel
 //   end in end_tok join `complete` (:207-209); the first K non-ended ones are the next beam
 //   (:211-212, with the py3 list() fix); stop when the beam is empty (:214) or K completed
 //   hypotheses beat the best live one (:217-221).
-// Hypotheses are nodes (parent node, token); the best complete (else best live) hypothesis is
-// back-tracked on the device when the search stops.
+// The "sort" is the selection of beam.cuh, a round per candidate wanted.  Hypotheses are nodes
+// (parent node, token) in a plain list: nothing merges prefixes here, so ids need not be canonical,
+// and the root is a real token (the start token).  The best complete (else best live) hypothesis
+// is back-tracked on the device when the search stops.
 // ------------------------------------------------------------------------------------------------
 static constexpr int BM_MAXK = 32;
 struct BeamState {
@@ -883,8 +885,6 @@ SB_DEVINL void beam_bookkeep(const BeamParams& p, const int* sel_idx, const doub
 __global__ void __launch_bounds__(256) s2s_beam_select_kernel(const BeamParams p) {
   extern __shared__ unsigned char bm_smem[];
   double* sc = reinterpret_cast<double*>(bm_smem);       // [K * C]
-  __shared__ double rs[8];
-  __shared__ int ri[8];
   __shared__ int sel_idx[2 * BM_MAXK];
   __shared__ double sel_sc[2 * BM_MAXK];
   const int tid = threadIdx.x;
@@ -898,29 +898,9 @@ __global__ void __launch_bounds__(256) s2s_beam_select_kernel(const BeamParams p
   __syncthreads();
   const int want = min(2 * K, nl * C);
   for (int q = 0; q < want; ++q) {
-    double bs = 0.0;
-    int bi = -1;
-    for (int i = tid; i < K * C; i += 256) {
-      const double v = sc[i];
-      if (isnan(v)) continue;
-      if (bi < 0 || v > bs) { bs = v; bi = i; }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const double os = __shfl_xor_sync(0xffffffffu, bs, o);
-      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-      if (oi >= 0 && (bi < 0 || os > bs || (os == bs && oi < bi))) { bs = os; bi = oi; }
-    }
-    if ((tid & 31) == 0) { rs[tid >> 5] = bs; ri[tid >> 5] = bi; }
-    __syncthreads();
-    if (tid == 0) {
-      for (int w = 1; w < 8; ++w)
-        if (ri[w] >= 0 && (bi < 0 || rs[w] > bs || (rs[w] == bs && ri[w] < bi))) { bs = rs[w]; bi = ri[w]; }
-      sel_idx[q] = bi;
-      sel_sc[q] = bs;
-      if (bi >= 0) sc[bi] = nan("");
-    }
-    __syncthreads();
+    double bs;
+    const int bi = beam_take_first<256>(sc, K * C, bs);
+    if (tid == 0) { sel_idx[q] = bi; sel_sc[q] = bs; }
   }
   if (tid != 0) return;
   beam_bookkeep(p, sel_idx, sel_sc, want);
@@ -938,32 +918,8 @@ __global__ void __launch_bounds__(256) s2s_beam_select_kernel(const BeamParams p
 static constexpr int BM_PER_THREAD = 16;
 static constexpr int BM_TILE = 256 * BM_PER_THREAD;
 
-// (score desc, index asc): does (s1, i1) come before (s2, i2)?  i < 0 = no candidate
-SB_DEVINL bool bm_before(double s1, int i1, double s2, int i2) {
-  return i1 >= 0 && (i2 < 0 || s1 > s2 || (s1 == s2 && i1 < i2));
-}
-
-// CTA-wide first of the 256 threads' (bs, bi); every thread gets it
-SB_DEVINL void bm_block_best(double& bs, int& bi, double* rs, int* ri) {
-  const int tid = threadIdx.x;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const double os = __shfl_xor_sync(0xffffffffu, bs, o);
-    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-    if (bm_before(os, oi, bs, bi)) { bs = os; bi = oi; }
-  }
-  __syncthreads();                                   // rs / ri of the previous round are read
-  if ((tid & 31) == 0) { rs[tid >> 5] = bs; ri[tid >> 5] = bi; }
-  __syncthreads();
-  bs = rs[0]; bi = ri[0];
-  for (int w = 1; w < 8; ++w)
-    if (bm_before(rs[w], ri[w], bs, bi)) { bs = rs[w]; bi = ri[w]; }
-}
-
 __global__ void __launch_bounds__(256) s2s_beam_tiles_kernel(const BeamParams p, double* t_sc,
                                                              int* t_idx, int* t_cnt) {
-  __shared__ double rs[8];
-  __shared__ int ri[8];
   const BeamState* st = p.st;
   if (st->done) return;
   const int tid = threadIdx.x, tile = blockIdx.x, K2 = 2 * p.K, C = p.C;
@@ -983,9 +939,9 @@ __global__ void __launch_bounds__(256) s2s_beam_tiles_kernel(const BeamParams p,
     double bs = 0.0;
     int bi = -1;
 #pragma unroll
-    for (int j = 0; j < BM_PER_THREAD; ++j)      // ascending index: strict > keeps the first
-      if (!isnan(v[j]) && (bi < 0 || v[j] > bs)) { bs = v[j]; bi = tile * BM_TILE + j * 256 + tid; }
-    bm_block_best(bs, bi, rs, ri);
+    for (int j = 0; j < BM_PER_THREAD; ++j)
+      beam_scan_step(v[j], tile * BM_TILE + j * 256 + tid, bs, bi);
+    beam_block_first<256>(bs, bi);
     if (bi < 0) break;
     if (tid == 0) { t_sc[(size_t)tile * K2 + q] = bs; t_idx[(size_t)tile * K2 + q] = bi; }
 #pragma unroll
@@ -999,8 +955,6 @@ __global__ void __launch_bounds__(256) s2s_beam_merge_kernel(const BeamParams p,
                                                              const int* t_idx, const int* t_cnt,
                                                              int ntiles) {
   extern __shared__ int bmm_head[];                  // [ntiles] next entry of each tile's list
-  __shared__ double rs[8];
-  __shared__ int ri[8];
   __shared__ int sel_idx[2 * BM_MAXK];
   __shared__ double sel_sc[2 * BM_MAXK];
   BeamState* st = p.st;
@@ -1017,10 +971,10 @@ __global__ void __launch_bounds__(256) s2s_beam_merge_kernel(const BeamParams p,
       if (h < t_cnt[t]) {
         const double s = t_sc[(size_t)t * K2 + h];
         const int i = t_idx[(size_t)t * K2 + h];
-        if (bm_before(s, i, bs, bi)) { bs = s; bi = i; }
+        if (beam_before(s, i, bs, bi)) { bs = s; bi = i; }
       }
     }
-    bm_block_best(bs, bi, rs, ri);
+    beam_block_first<256>(bs, bi);
     if (tid == 0) {
       sel_idx[q] = bi;
       sel_sc[q] = bs;
@@ -1339,13 +1293,28 @@ extern "C" int sb_s2s_beam_init(void* state, int* nodes, int* tok_next, int star
   return SB_OK;
 }
 
+// checks and fill-in shared by the single-CTA and the split selection
+static int beam_params(sb::BeamParams* p, const float* logp, void* state, double* c_scores,
+                       int* nodes, int* parent_row, int* tok_next, int* out_tokens, int K, int C,
+                       int end_tok, int step, int max_len, int node_cap, int c_cap) {
+  if (!logp || !state || !c_scores || !nodes || !parent_row || !tok_next || !out_tokens)
+    return SB_ERR_INVALID;
+  if (K <= 0 || K > sb::BM_MAXK || C <= 0) return SB_ERR_UNSUPPORTED;
+  p->logp = logp; p->st = reinterpret_cast<sb::BeamState*>(state); p->c_scores = c_scores;
+  p->nodes = nodes; p->parent_row = parent_row; p->tok_next = tok_next; p->out_tokens = out_tokens;
+  p->K = K; p->C = C; p->end_tok = end_tok; p->step = step; p->max_len = max_len;
+  p->node_cap = node_cap; p->c_cap = c_cap;
+  return SB_OK;
+}
+
 extern "C" int sb_s2s_beam_select(const float* logp, void* state, double* c_scores, int* nodes,
                                   int* parent_row, int* tok_next, int* out_tokens, int K, int C,
                                   int end_tok, int step, int max_len, int node_cap, int c_cap,
                                   void* stream_) {
-  if (!logp || !state || !c_scores || !nodes || !parent_row || !tok_next || !out_tokens)
-    return SB_ERR_INVALID;
-  if (K <= 0 || K > sb::BM_MAXK || C <= 0) return SB_ERR_UNSUPPORTED;
+  sb::BeamParams p;
+  const int rc = beam_params(&p, logp, state, c_scores, nodes, parent_row, tok_next, out_tokens, K,
+                             C, end_tok, step, max_len, node_cap, c_cap);
+  if (rc != SB_OK) return rc;
   const size_t smem = (size_t)K * C * sizeof(double);
   if (smem > 200 * 1024) return SB_ERR_UNSUPPORTED;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
@@ -1353,11 +1322,6 @@ extern "C" int sb_s2s_beam_select(const float* logp, void* state, double* c_scor
       cudaFuncSetAttribute(sb::s2s_beam_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                            (int)smem) != cudaSuccess)
     return SB_ERR_CUDA;
-  sb::BeamParams p;
-  p.logp = logp; p.st = reinterpret_cast<sb::BeamState*>(state); p.c_scores = c_scores;
-  p.nodes = nodes; p.parent_row = parent_row; p.tok_next = tok_next; p.out_tokens = out_tokens;
-  p.K = K; p.C = C; p.end_tok = end_tok; p.step = step; p.max_len = max_len;
-  p.node_cap = node_cap; p.c_cap = c_cap;
   sb::s2s_beam_select_kernel<<<1, 256, smem, stream>>>(p);
   return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
 }
@@ -1382,11 +1346,12 @@ extern "C" int sb_s2s_beam_select_split(const float* logp, void* state, double* 
                                         int* out_tokens, int K, int C, int end_tok, int step,
                                         int max_len, int node_cap, int c_cap, void* workspace,
                                         size_t workspace_bytes, void* stream_) {
-  if (!logp || !state || !c_scores || !nodes || !parent_row || !tok_next || !out_tokens ||
-      !workspace)
-    return SB_ERR_INVALID;
-  if (K <= 0 || K > sb::BM_MAXK || C <= 0 || (long long)K * C > 0x7fffffffLL)
-    return SB_ERR_UNSUPPORTED;
+  if (!workspace) return SB_ERR_INVALID;
+  sb::BeamParams p;
+  const int rc = beam_params(&p, logp, state, c_scores, nodes, parent_row, tok_next, out_tokens, K,
+                             C, end_tok, step, max_len, node_cap, c_cap);
+  if (rc != SB_OK) return rc;
+  if ((long long)K * C > 0x7fffffffLL) return SB_ERR_UNSUPPORTED;
   size_t need = 0;
   sb_s2s_beam_split_workspace_size(K, C, &need);
   if (workspace_bytes < need) return SB_ERR_WORKSPACE;
@@ -1401,11 +1366,6 @@ extern "C" int sb_s2s_beam_select_split(const float* logp, void* state, double* 
   double* t_sc = reinterpret_cast<double*>(workspace);
   int* t_idx = reinterpret_cast<int*>(t_sc + (size_t)nt * 2 * K);
   int* t_cnt = t_idx + (size_t)nt * 2 * K;
-  sb::BeamParams p;
-  p.logp = logp; p.st = reinterpret_cast<sb::BeamState*>(state); p.c_scores = c_scores;
-  p.nodes = nodes; p.parent_row = parent_row; p.tok_next = tok_next; p.out_tokens = out_tokens;
-  p.K = K; p.C = C; p.end_tok = end_tok; p.step = step; p.max_len = max_len;
-  p.node_cap = node_cap; p.c_cap = c_cap;
   sb::s2s_beam_tiles_kernel<<<nt, 256, 0, stream>>>(p, t_sc, t_idx, t_cnt);
   sb::s2s_beam_merge_kernel<<<1, 256, smem, stream>>>(p, t_sc, t_idx, t_cnt, nt);
   return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;

@@ -17,8 +17,8 @@
 //             (score desc, i*V + k asc) = a stable descending sort of the candidate list
 //     beam = the beam_size best of done by (score desc, insertion order asc)
 //   result = beam[0] after the last frame.
-// Hypotheses are nodes (parent, label) of a per-utterance trie made canonical by a hash map, so
-// "the same label sequence" is an integer comparison.  Scores are float64, as Python floats.
+// Both selections and the trie of hypotheses (prefix merging compares node ids) are those of
+// beam.cuh.  Scores are float64, as Python floats.
 // Roofline: HBM-nominal (the lattice is read once); latency-bound by the T x U serial expansion.
 //
 // sb_rnnt_decode_static_shortlist: the same search from per-node shortlists instead of the full
@@ -47,7 +47,7 @@
 // one float64 sum, i.e. |fr_s| of roughly 2^29 times their gap, so real lattices never raise it.
 // A hypothesis takes at most K of its entries, so kp >= K lists are never exhausted while a
 // left-out class could still follow.
-#include "common.cuh"
+#include "beam.cuh"
 #include <math.h>
 
 #include "../../include/speech_b200.h"
@@ -66,9 +66,7 @@ struct TdParams {
   const float* sl_meta; // (B, T, U1, 2) {blank lp, beta}
   const int* tlens;     // (B) frames to search (<= T)
   const int* ulens;     // (B) lattice rows U = labels + 1 (<= U1)
-  int* nodes;           // (B, 2*node_cap) trie arena: parent, label
-  unsigned long long* hkeys;   // (B, hcap)
-  int* hvals;                  // (B, hcap)
+  BeamTrie trie;        // utterance 0 of B
   double* done_score;   // (B, done_cap)
   int* done_node;       // (B, done_cap)
   int* done_len;        // (B, done_cap)
@@ -76,7 +74,7 @@ struct TdParams {
   int* out_lens;        // (B)
   double* out_scores;   // (B) log-probability of the best hypothesis
   int* out_flags;       // (B) unproven shortlist selections (shortlist search)
-  int B, T, U1, V, K, kp, blank, hcap, node_cap, done_cap;
+  int B, T, U1, V, K, kp, blank, done_cap;
 };
 
 SB_DEVINL double td_lse(double a, double b) {
@@ -84,65 +82,11 @@ SB_DEVINL double td_lse(double a, double b) {
   return m + log(exp(a - m) + exp(b - m));
 }
 
-// block arg-max over (score desc, index asc) of the live entries of sc[0..n); returns the index
-// (or -1) to every thread.  `taken` entries carry NaN.
-SB_DEVINL int td_argmax(const double* sc, int n, double* red_s, int* red_i, int tid) {
-  double bs = 0.0;
-  int bi = -1;
-  for (int i = tid; i < n; i += TD_THREADS) {
-    const double v = sc[i];
-    if (isnan(v)) continue;
-    if (bi < 0 || v > bs) { bs = v; bi = i; }
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const double os = __shfl_xor_sync(0xffffffffu, bs, o);
-    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-    if (oi >= 0 && (bi < 0 || os > bs || (os == bs && oi < bi))) { bs = os; bi = oi; }
-  }
-  if ((tid & 31) == 0) { red_s[tid >> 5] = bs; red_i[tid >> 5] = bi; }
-  __syncthreads();
-  bs = red_s[0];
-  bi = red_i[0];
-  for (int w = 1; w < TD_THREADS / 32; ++w)
-    if (red_i[w] >= 0 && (bi < 0 || red_s[w] > bs || (red_s[w] == bs && red_i[w] < bi))) {
-      bs = red_s[w];
-      bi = red_i[w];
-    }
-  __syncthreads();
-  return bi;
-}
-
 // nextafterf(x, -inf) for finite x
 SB_DEVINL float td_next_down(float x) {
   const int i = __float_as_int(x);
   if (x == 0.f) return -__int_as_float(1);                 // -(smallest subnormal)
   return __int_as_float(x > 0.f ? i - 1 : i + 1);
-}
-
-// canonical trie node of hypothesis node `parent` extended by label k (one thread); a new node
-// gets id 1 + round_id * K + nsel, -1 when the arena is full
-SB_DEVINL int td_extend(const TdParams& p, int* nodes, unsigned long long* hkeys, int* hvals,
-                        int parent, int k, int round_id, int nsel) {
-  const unsigned long long key =
-      ((unsigned long long)(unsigned int)parent << 32) | (unsigned int)(k + 1);
-  unsigned int h = (unsigned int)((key * 0x9E3779B97F4A7C15ull) >> 32) & (p.hcap - 1);
-  int id = -1;
-  for (int probe = 0; probe < p.hcap; ++probe) {
-    const unsigned long long kk = hkeys[h];
-    if (kk == key) { id = hvals[h]; break; }
-    if (kk == 0ull) {
-      id = 1 + round_id * p.K + nsel;
-      if (id >= p.node_cap) { id = -1; break; }
-      hkeys[h] = key;
-      hvals[h] = id;
-      nodes[2 * id] = parent;
-      nodes[2 * id + 1] = k;
-      break;
-    }
-    h = (h + 1) & (p.hcap - 1);
-  }
-  return id;
 }
 
 // the search of one utterance (blockIdx.x); SHORT: candidates from the shortlists
@@ -157,27 +101,21 @@ SB_DEVINL void td_search(const TdParams& p) {
   __shared__ int beam_n[TD_MAX_BEAM], beam_l[TD_MAX_BEAM];
   __shared__ int fr_n[TD_MAX_BEAM], fr_l[TD_MAX_BEAM];
   __shared__ int new_n[TD_MAX_BEAM], new_l[TD_MAX_BEAM];
-  __shared__ double red_s[TD_THREADS / 32];
-  __shared__ int red_i[TD_THREADS / 32];
   __shared__ int nbeam, nfr, ndone, found, round_id, nsel_s, nflag;
 
-  int* nodes = p.nodes + (size_t)b * 2 * p.node_cap;
-  unsigned long long* hkeys = p.hkeys + (size_t)b * p.hcap;
-  int* hvals = p.hvals + (size_t)b * p.hcap;
+  const BeamTrie trie = p.trie.of(b);
   double* dscore = p.done_score + (size_t)b * p.done_cap;
   int* dnode = p.done_node + (size_t)b * p.done_cap;
   int* dlen = p.done_len + (size_t)b * p.done_cap;
   const float* lp = SHORT ? nullptr : p.lp + (size_t)b * p.T * p.U1 * V;
   const size_t node0 = (size_t)b * p.T * p.U1;             // batch-first node of (b, 0, 0)
 
-  for (int k = tid; k < p.hcap; k += TD_THREADS) hkeys[k] = 0ull;
   if (tid == 0) {
     nbeam = 1; beam_s[0] = 0.0; beam_n[0] = 0; beam_l[0] = 0;
-    nodes[0] = -1; nodes[1] = -1;
     round_id = 0;
     nflag = 0;
   }
-  __syncthreads();
+  trie.clear<TD_THREADS>();
 
   for (int t = 0; t < T; ++t) {
     if (tid < nbeam) { fr_s[tid] = beam_s[tid]; fr_n[tid] = beam_n[tid]; fr_l[tid] = beam_l[tid]; }
@@ -220,18 +158,18 @@ SB_DEVINL void td_search(const TdParams& p) {
         const int have = __syncthreads_or(any ? 1 : 0);
         if (!have) break;
         for (int r = 0; r < K; ++r) {
-          const int c = td_argmax(cand, K * V, red_s, red_i, tid);
+          double sc;
+          const int c = beam_take_first<TD_THREADS>(cand, K * V, sc);
           if (c < 0) break;
           if (tid == 0) {
             const int i = c / V, k = c - i * V;
-            new_s[nsel] = cand[c];
-            new_n[nsel] = td_extend(p, nodes, hkeys, hvals, fr_n[i], k, round_id, nsel);
+            new_s[nsel] = sc;
+            new_n[nsel] = trie.find_or_insert<false>(fr_n[i], k, 1 + round_id * K + nsel);
             new_l[nsel] = fr_l[i] + 1;
-            cand[c] = nan("");
           }
           ++nsel;
-          __syncthreads();
         }
+        __syncthreads();                            // thread 0 has read fr_* and written new_*
       } else {
         // K-way merge of the frontier's shortlists, one lane per hypothesis (warp 0)
         bool live = false;
@@ -273,12 +211,7 @@ SB_DEVINL void td_search(const TdParams& p) {
             }
             double bs = hs;
             int bi = hv ? i : -1;
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-              const double os = __shfl_xor_sync(0xffffffffu, bs, o);
-              const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-              if (oi >= 0 && (bi < 0 || os > bs || (os == bs && oi < bi))) { bs = os; bi = oi; }
-            }
+            beam_warp_first(bs, bi);
             if (bi < 0) break;
             const int k = __shfl_sync(0xffffffffu, hk, bi);
             if (i == bi) {
@@ -295,7 +228,7 @@ SB_DEVINL void td_search(const TdParams& p) {
             }
             if (i == 0) {
               new_s[ns] = bs;
-              new_n[ns] = td_extend(p, nodes, hkeys, hvals, fr_n[bi], k, round_id, ns);
+              new_n[ns] = trie.find_or_insert<false>(fr_n[bi], k, 1 + round_id * K + ns);
               new_l[ns] = fr_l[bi] + 1;
             }
             ++ns;
@@ -315,27 +248,18 @@ SB_DEVINL void td_search(const TdParams& p) {
     const int nd = ndone;
     int nb = 0;
     for (int r = 0; r < K; ++r) {
-      const int j = td_argmax(dscore, nd, red_s, red_i, tid);
+      double sc;
+      const int j = beam_take_first<TD_THREADS>(dscore, nd, sc);
       if (j < 0) break;
-      if (tid == 0) {
-        beam_s[nb] = dscore[j]; beam_n[nb] = dnode[j]; beam_l[nb] = dlen[j];
-        dscore[j] = nan("");
-      }
+      if (tid == 0) { beam_s[nb] = sc; beam_n[nb] = dnode[j]; beam_l[nb] = dlen[j]; }
       ++nb;
-      __syncthreads();
     }
     if (tid == 0) nbeam = nb;
     __syncthreads();
   }
 
   if (tid == 0) {
-    int len = 0;
-    const int n = nbeam > 0 ? beam_n[0] : 0;
-    for (int q = n; q > 0; q = nodes[2 * q]) ++len;
-    int* out = p.out_labels + (size_t)b * p.U1;
-    int k = len;
-    for (int q = n; q > 0; q = nodes[2 * q]) out[--k] = nodes[2 * q + 1];
-    p.out_lens[b] = len;
+    p.out_lens[b] = trie.backtrack(nbeam > 0 ? beam_n[0] : 0, p.out_labels + (size_t)b * p.U1);
     p.out_scores[b] = nbeam > 0 ? beam_s[0] : -INFINITY;
     if (SHORT) p.out_flags[b] = nflag;
   }
@@ -352,16 +276,11 @@ __global__ void __launch_bounds__(TD_THREADS, 1) rnnt_decode_static_shortlist_ke
   td_search<true>(p);
 }
 
-static int td_pow2(size_t need) {
-  size_t cap = 64;
-  while (cap < need) cap <<= 1;
-  return (int)cap;
-}
 struct TdSizes { size_t node_cap, hcap, done_cap, total; };
 static TdSizes td_sizes(int B, int T, int U1, int K) {
   TdSizes s;
   s.node_cap = (size_t)T * U1 * K + 2;
-  s.hcap = (size_t)td_pow2(2 * s.node_cap);
+  s.hcap = (size_t)beam_pow2_cap(2 * s.node_cap);
   s.done_cap = (size_t)K * (U1 + 1) + 1;
   s.total = 1024 + (size_t)B * (2 * s.node_cap * sizeof(int) +
                                 s.hcap * (sizeof(unsigned long long) + sizeof(int)) +
@@ -383,13 +302,13 @@ static int td_setup(TdParams* p, const int* tlens, const int* ulens, int B, int 
   const TdSizes sz = td_sizes(B, T, U1, beam_size);
   if (workspace_bytes < sz.total) return SB_ERR_WORKSPACE;
   uintptr_t w = (reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255;
-  p->hkeys = reinterpret_cast<unsigned long long*>(w);
+  p->trie.keys = reinterpret_cast<unsigned long long*>(w);
   w += (size_t)B * sz.hcap * sizeof(unsigned long long);
   p->done_score = reinterpret_cast<double*>(w);
   w += (size_t)B * sz.done_cap * sizeof(double);
-  p->hvals = reinterpret_cast<int*>(w);
+  p->trie.vals = reinterpret_cast<int*>(w);
   w += (size_t)B * sz.hcap * sizeof(int);
-  p->nodes = reinterpret_cast<int*>(w);
+  p->trie.nodes = reinterpret_cast<int*>(w);
   w += (size_t)B * 2 * sz.node_cap * sizeof(int);
   p->done_node = reinterpret_cast<int*>(w);
   w += (size_t)B * sz.done_cap * sizeof(int);
@@ -399,7 +318,7 @@ static int td_setup(TdParams* p, const int* tlens, const int* ulens, int B, int 
   p->tlens = tlens; p->ulens = ulens;
   p->out_labels = out_labels; p->out_lens = out_lens; p->out_scores = out_scores;
   p->B = B; p->T = T; p->U1 = U1; p->V = V; p->K = beam_size; p->kp = 0; p->blank = blank;
-  p->hcap = (int)sz.hcap; p->node_cap = (int)sz.node_cap; p->done_cap = (int)sz.done_cap;
+  p->trie.cap = (int)sz.hcap; p->trie.node_cap = (int)sz.node_cap; p->done_cap = (int)sz.done_cap;
   return SB_OK;
 }
 
