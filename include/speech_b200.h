@@ -206,7 +206,6 @@ int sb_ctc_prefix_beam_shortlist(const float* logp, const int* lens, int B, int 
  *   sb_conv_relu_to_bct  C of the last layer -> (B, To, Co*Fo) f32 with ReLU (model.py:66-71)
  *   sb_conv_dtop         dY (B,To,Co*Fo) * (C>0) -> dC bf16 [M][Co]; db[c] += column sums
  *   sb_conv_col2im_relu  dA f32 [M][ldA] -> dC of the layer below (gather, masked by Pprev>0)
- *   sb_transpose_bf16    [R][C] -> [C][R] (weight-gradient operands)
  * ------------------------------------------------------------------------------------- */
 /* `mask_u8` (may be NULL): dropout keep-bytes (1 keep, 0 drop) of the activations involved, same
  * pixel-major channels-last layout as those activations; kept values are multiplied by `mscale`
@@ -221,8 +220,6 @@ int sb_conv_dtop(const float* dY, const float* C, const void* mask_u8, float msc
 int sb_conv_col2im_relu(const float* dA, long long ldA, const float* Pprev,
                         const void* maskprev_u8, float mscale, void* dCprev_bf16, float* db, int B,
                         int Ti, int Fi, int Ci, int kh, int kw, int stride, void* stream);
-int sb_transpose_bf16(const void* src, void* dst, long long R, int C, long long ld_src,
-                      long long ld_dst, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Tail of the training step over flat fp32 buffers.
@@ -253,8 +250,8 @@ int sb_sgd_clip_step(float* params, const float* grads, float* momentum_buf, voi
  *   sb_s2s_attn_fwd   attention of every row over eh (eh_bcast: all rows attend over utterance
  *                     0 - beam search), sx (B,H) / ax (B,T); with fc_w: logits = fc(hx + sx) written
  *                     at logits[b*logit_stride + c], optional log-softmax, arg-max, greedy history
- *                     and end-token count; `done` (device int, may be NULL): != 0 -> no-op
- *   sb_attn_step      the attention alone (NNAttention.forward on the decode path)
+ *                     and end-token count; `done` (device int, may be NULL): != 0 -> no-op.
+ *                     Without fc_w: the attention alone (NNAttention.forward on the decode path)
  *   sb_s2s_dout       backward of the output projection for all (step, utterance) rows at once:
  *                     d_o = dlogits W_fc, o = hx + sx (operand of the time-batched d W_fc)
  *   sb_s2s_attn_bwd / sb_s2s_cell_bwd   gradients of one step (see csrc/s2s.cu)
@@ -268,12 +265,12 @@ int sb_sgd_clip_step(float* params, const float* grads, float* momentum_buf, voi
  * call (ticket counters; the kernels leave them zero); one workspace serves all steps.
  * Constraints: H % 4 == 0 (attention backward: H <= 1664, its shared-memory tile is 33 H floats),
  * conv kernel width odd and <= 15, T <= 6144, beam <= 32.
+ * Exact lengths: `lens` (B) int32 on the device gives the frames row b attends over (clamped to
+ * [1, T]; NULL = all T).  Frames t >= lens[b] are left out of the softmax, so a_t = 0 exactly
+ * there, and out of the location conv's input; log_t scales by log(lens[b]); d eh stays untouched
+ * (zero) there.  CTAs whose frame tile lies wholly past lens[b] exit at once.
  * ------------------------------------------------------------------------------------- */
 int sb_s2s_workspace_size(int B, int T, int H, size_t* bytes);
-int sb_attn_step(const float* eh, const float* dhx, const float* ax_prev, const float* conv_wT,
-                 const float* conv_b, const float* lin_w, float lin_b, int log_t, int B, int T,
-                 int H, int Kc, float* sx, float* ax, void* workspace, size_t workspace_bytes,
-                 void* stream);
 int sb_s2s_cell_fwd(const float* emb, const int* tok, int tok_stride, const float* sx_prev,
                     const float* hx_prev, const float* w_ih, const float* w_hh, const float* b_ih,
                     const float* b_hh, float* hx, float* ix_save, float* gates_save,
@@ -284,7 +281,7 @@ int sb_s2s_attn_fwd(const float* eh, int eh_bcast, const float* hx, const float*
                     const float* fc_w, const float* fc_b, int C, float* logits,
                     long long logit_stride, float* logp, int* argmax, int* history,
                     int hist_stride, int hist_col, int* end_count, int end_tok, const int* done,
-                    void* workspace, size_t workspace_bytes, void* stream);
+                    const int* lens, void* workspace, size_t workspace_bytes, void* stream);
 int sb_s2s_dout(const float* dlogits, const float* fc_w, const float* hx, const float* sx,
                 float* d_o, float* o_all, long long rows, int C, int H, void* stream);
 int sb_s2s_attn_bwd(const float* eh, const float* hx, const float* hx_prev, const float* ax_prev,
@@ -293,37 +290,15 @@ int sb_s2s_attn_bwd(const float* eh, const float* hx, const float* hx_prev, cons
                     const float* d_ax_next, const float* d_hx_next, const float* gates,
                     float* d_eh, float* d_ax_prev, float* d_gi, float* d_gh, float* d_hx_direct,
                     float* g_conv_wT, float* g_conv_b, float* g_lin_w, float* g_lin_b, int log_t,
-                    int B, int T, int H, int Kc, void* workspace, size_t workspace_bytes,
-                    void* stream);
-/* Length-masked variants (exact-lengths mode): `lens` (B) int32 on the device gives the frames
- * row b attends over (clamped to [1, T]; NULL = all T, which is what the entry points above pass).
- * Frames t >= lens[b] are left out of the softmax, so a_t = 0 exactly there, and out of the
- * location conv's input; log_t scales by log(lens[b]); d eh stays untouched (zero) there.  CTAs
- * whose frame tile lies wholly past lens[b] exit at once. */
-int sb_attn_step_len(const float* eh, const float* dhx, const float* ax_prev, const float* conv_wT,
-                     const float* conv_b, const float* lin_w, float lin_b, int log_t, int B, int T,
-                     int H, int Kc, float* sx, float* ax, const int* lens, void* workspace,
-                     size_t workspace_bytes, void* stream);
-int sb_s2s_attn_fwd_len(const float* eh, int eh_bcast, const float* hx, const float* ax_prev,
-                        const float* conv_wT, const float* conv_b, const float* lin_w, float lin_b,
-                        int log_t, int B, int T, int H, int Kc, float* sx, float* ax,
-                        const float* fc_w, const float* fc_b, int C, float* logits,
-                        long long logit_stride, float* logp, int* argmax, int* history,
-                        int hist_stride, int hist_col, int* end_count, int end_tok,
-                        const int* done, const int* lens, void* workspace,
-                        size_t workspace_bytes, void* stream);
-int sb_s2s_attn_bwd_len(const float* eh, const float* hx, const float* hx_prev,
-                        const float* ax_prev, const float* ax, const float* conv_wT,
-                        const float* conv_b, const float* lin_w, const float* d_o,
-                        const float* d_ix_next, const float* d_ax_next, const float* d_hx_next,
-                        const float* gates, float* d_eh, float* d_ax_prev, float* d_gi,
-                        float* d_gh, float* d_hx_direct, float* g_conv_wT, float* g_conv_b,
-                        float* g_lin_w, float* g_lin_b, int log_t, int B, int T, int H, int Kc,
-                        const int* lens, void* workspace, size_t workspace_bytes, void* stream);
+                    int B, int T, int H, int Kc, const int* lens, void* workspace,
+                    size_t workspace_bytes, void* stream);
 int sb_s2s_cell_bwd(const float* d_gi, const float* d_gh, const float* d_hx_direct,
                     const float* w_ihT, const float* w_hhT, float* d_ix, float* d_hx_prev, int B,
                     int H, void* stream);
 int sb_s2s_check_done(const int* end_count, int B, int* done, int* nsteps, int step1, void* stream);
+/* The beam state is opaque but for two int32 fields the host reads in place: `done` at byte 0
+ * (nonzero once the search has stopped; it doubles as the `done` flag of the step kernels) and
+ * the length of the final hypothesis in out_tokens at byte 4. */
 int sb_s2s_beam_state_size(size_t* bytes);
 int sb_s2s_beam_init(void* state, int* nodes, int* tok_next, int start_tok, void* stream);
 int sb_s2s_beam_select(const float* logp, void* state, double* c_scores, int* nodes,
@@ -371,11 +346,6 @@ int sb_s2s_beam_select_split(const float* logp, void* state, double* c_scores, i
                              int* parent_row, int* tok_next, int* out_tokens, int K, int C,
                              int end_tok, int step, int max_len, int node_cap, int c_cap,
                              void* workspace, size_t workspace_bytes, void* stream);
-
-/* Beam expand/prune of Seq2Seq.beam_search (speech/models/seq2seq.py:200-212): indices and values
- * of the k best of n float64 scores, ordered by (score descending, index ascending) - the order of
- * the reference's stable sort over (beam, vocab) candidates. */
-int sb_beam_topk(const double* scores, int n, int k, int* out_idx, double* out_val, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * RNN-Transducer loss + gradient w.r.t. the log-probabilities.
@@ -531,7 +501,6 @@ int sb_log_specgram(const short* pcm, const long long* offsets, const int* n_sam
 /* Developer hook (not part of the drop-in surface): device buffer of >= 64*16 uint64 receiving a
  * globaltimer timeline of CTA 0 for the next sb_gru_fwd launches; NULL disables. */
 int sb_debug_gru_timeline(void* dev_buffer);
-int sb_debug_umma_mn(int lbo_bytes, int sbo_bytes, int kadv_bytes);
 /* Developer hook, GEMM kernel selection (0 = default, bits combine): 1 = run every sb_gemm_bf16_tn
  * with N > 64 on the 128 x 128 tiles of the one-CTA kernel instead of the 128 x 256 tiles over
  * 2-CTA clusters; 2 = the 2-CTA kernel stores its output straight from the registers instead of

@@ -40,27 +40,17 @@ SIGNATURES = {
     "sb_conv_dtop": (_c_int, [_vp, _vp, _vp, _fl, _vp, _vp, _c_int, _c_int, _c_int, _c_int, _vp]),
     "sb_conv_col2im_relu": (_c_int, [_vp, _c_ll, _vp, _vp, _fl, _vp, _vp, _c_int, _c_int, _c_int,
                                      _c_int, _c_int, _c_int, _c_int, _vp]),
-    "sb_transpose_bf16": (_c_int, [_vp, _vp, _c_ll, _c_int, _c_ll, _c_ll, _vp]),
     "sb_sumsq_workspace_size": (_c_int, [ctypes.POINTER(_c_sz)]),
     "sb_sumsq": (_c_int, [_vp, _c_ll, _vp, _vp, _vp]),
     "sb_sgd_clip_step": (_c_int, [_vp, _vp, _vp, _vp, _c_ll, _vp, _fl, _fl, _fl, _vp]),
     "sb_s2s_workspace_size": (_c_int, [_c_int, _c_int, _c_int, ctypes.POINTER(_c_sz)]),
-    "sb_attn_step": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _fl, _c_int, _c_int, _c_int, _c_int,
-                              _c_int, _vp, _vp, _vp, _c_sz, _vp]),
     "sb_s2s_cell_fwd": (_c_int, [_vp, _vp, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                  _c_int, _c_int, _vp]),
     "sb_s2s_attn_fwd": (_c_int, [_vp, _c_int, _vp, _vp, _vp, _vp, _vp, _fl, _c_int, _c_int, _c_int,
                                  _c_int, _c_int, _vp, _vp, _vp, _vp, _c_int, _vp, _c_ll, _vp, _vp,
-                                 _vp, _c_int, _c_int, _vp, _c_int, _vp, _vp, _c_sz, _vp]),
-    "sb_attn_step_len": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _fl, _c_int, _c_int, _c_int, _c_int,
-                                  _c_int, _vp, _vp, _vp, _vp, _c_sz, _vp]),
-    "sb_s2s_attn_fwd_len": (_c_int, [_vp, _c_int, _vp, _vp, _vp, _vp, _vp, _fl, _c_int, _c_int,
-                                     _c_int, _c_int, _c_int, _vp, _vp, _vp, _vp, _c_int, _vp, _c_ll,
-                                     _vp, _vp, _vp, _c_int, _c_int, _vp, _c_int, _vp, _vp, _vp,
-                                     _c_sz, _vp]),
-    "sb_s2s_attn_bwd_len": (_c_int, [_vp] * 22 + [_c_int] * 5 + [_vp, _vp, _c_sz, _vp]),
+                                 _vp, _c_int, _c_int, _vp, _c_int, _vp, _vp, _vp, _c_sz, _vp]),
     "sb_s2s_dout": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _c_ll, _c_int, _c_int, _vp]),
-    "sb_s2s_attn_bwd": (_c_int, [_vp] * 22 + [_c_int] * 5 + [_vp, _c_sz, _vp]),
+    "sb_s2s_attn_bwd": (_c_int, [_vp] * 22 + [_c_int] * 5 + [_vp, _vp, _c_sz, _vp]),
     "sb_s2s_cell_bwd": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_int, _c_int, _vp]),
     "sb_s2s_check_done": (_c_int, [_vp, _c_int, _vp, _vp, _c_int, _vp]),
     "sb_s2s_beam_state_size": (_c_int, [ctypes.POINTER(_c_sz)]),
@@ -81,7 +71,6 @@ SIGNATURES = {
     "sb_s2s_beam_select_split": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_int, _c_int,
                                           _c_int, _c_int, _c_int, _c_int, _c_int, _vp, _c_sz,
                                           _vp]),
-    "sb_beam_topk": (_c_int, [_vp, _c_int, _c_int, _vp, _vp, _vp]),
     "sb_rnnt_workspace_size": (_c_int, [_c_int, _c_int, _c_int, ctypes.POINTER(_c_sz)]),
     "sb_rnnt_fwd_bwd": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int,
                                  _vp, _vp, _c_sz, _vp]),
@@ -117,7 +106,6 @@ SIGNATURES = {
     "sb_debug_gru_bwd_kernel": (ctypes.c_char_p, []),
     "sb_debug_gru_plan": (_c_int, [_c_int, ctypes.POINTER(_c_int)]),
     "sb_debug_gru_wide_ring": (_c_int, [_c_int]),
-    "sb_debug_umma_mn": (_c_int, [_c_int, _c_int, _c_int]),
     "sb_debug_gemm_flags": (_c_int, [_c_int]),
     "sb_debug_gemm_kernel": (ctypes.c_char_p, []),
     "sb_debug_gemm_epilogue": (ctypes.c_char_p, []),
@@ -167,6 +155,44 @@ def check(status, what):
     if status != 0:
         msg = load().sb_status_string(status).decode()
         raise SpeechB200Error("speech_b200: %s failed: %s (status %d)" % (what, msg, status))
+
+
+def workspace_size(query, *args):
+    """Bytes a `sb_*_workspace_size` / `sb_s2s_beam_state_size` query asks for: query(*args,
+    &bytes); raises through check."""
+    n = _c_sz(0)
+    check(query(*args, ctypes.byref(n)), query.__name__)
+    return n.value
+
+
+def pack_labels(labels, label_lens, act_lens, B, dev, num_classes=None, lattice_rows=None):
+    """The flat label format sb_ctc_fwd_bwd and sb_rnnt_fwd_bwd(_compact) share, moved to `dev` in
+    one pinned host->device copy of [labels | offsets | label_lens | act_lens] (int32).
+    Raises ValueError unless label_lens / act_lens hold one entry per utterance and label_lens sums
+    to the number of labels; num_classes (CTC): every label lies in [0, num_classes);
+    lattice_rows (Transducer, U+1): no label sequence is longer than lattice_rows - 1.
+    -> (labels, offsets, label_lens, act_lens) device views, longest label sequence (0 if B = 0)."""
+    import torch
+    lab = labels.detach().to("cpu", torch.int32).reshape(-1)
+    llen = label_lens.detach().to("cpu", torch.int32).reshape(-1)
+    alen = act_lens.detach().to("cpu", torch.int32).reshape(-1)
+    if llen.numel() != B or alen.numel() != B:
+        raise ValueError("act_lens / label_lens must have one entry per utterance")
+    n = lab.numel()
+    if int(llen.sum()) != n:
+        if lattice_rows is not None:
+            raise ValueError("labels / y_lens mismatch")
+        raise ValueError("labels has %d entries but label_lens sums to %d" % (n, int(llen.sum())))
+    if num_classes is not None and n and (int(lab.min()) < 0 or int(lab.max()) >= num_classes):
+        raise ValueError("label out of range")
+    max_len = int(llen.max()) if B else 0
+    if lattice_rows is not None and max_len > lattice_rows - 1:
+        raise ValueError("a label sequence is longer than the lattice (U+1 = %d)" % lattice_rows)
+    offs = torch.zeros(B, dtype=torch.int32)
+    if B > 1:
+        offs[1:] = torch.cumsum(llen[:-1], 0)
+    packed = torch.cat([lab, offs, llen, alen]).pin_memory().to(dev, non_blocking=True)
+    return (packed[:n], packed[n:n + B], packed[n + B:n + 2 * B], packed[n + 2 * B:]), max_len
 
 
 def ptr(t):

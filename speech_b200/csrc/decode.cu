@@ -495,39 +495,3 @@ extern "C" int sb_ctc_prefix_beam_shortlist(const float* logp, const int* lens, 
   return dec_entry(logp, lens, B, T, S, beam_size, blank, out_labels, out_lens, out_scores,
                    workspace, workspace_bytes, stream, true);
 }
-
-// ------------------------------------------------------------------------------------------------
-// sb_beam_topk: the expand/prune step of Seq2Seq.beam_search (speech/models/seq2seq.py:200-212):
-// the reference sorts ALL beam x vocab candidates with a stable descending sort and keeps a
-// prefix, so ties keep (beam index, vocab index) order = ascending flat index.  One CTA selects
-// the top k of n float64 scores by k rounds of beam_take_first.
-// ------------------------------------------------------------------------------------------------
-namespace sb {
-__global__ void __launch_bounds__(256) beam_topk_kernel(const double* __restrict__ scores, int n,
-                                                        int k, int* out_idx, double* out_val) {
-  extern __shared__ unsigned char topk_smem[];
-  double* sc = reinterpret_cast<double*>(topk_smem);
-  const int tid = threadIdx.x;
-  for (int i = tid; i < n; i += 256) sc[i] = scores[i];
-  __syncthreads();
-  for (int r = 0; r < k; ++r) {
-    double bs;
-    const int bi = beam_take_first<256>(sc, n, bs);
-    if (tid == 0) { out_idx[r] = bi; out_val[r] = bs; }
-  }
-}
-}  // namespace sb
-
-extern "C" int sb_beam_topk(const double* scores, int n, int k, int* out_idx, double* out_val,
-                            void* stream_) {
-  if (!scores || !out_idx || !out_val || n <= 0 || k <= 0 || k > n) return SB_ERR_INVALID;
-  const size_t smem = (size_t)n * sizeof(double);
-  if (smem > 200 * 1024) return SB_ERR_UNSUPPORTED;
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (smem > 40 * 1024 &&
-      cudaFuncSetAttribute(sb::beam_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                           (int)smem) != cudaSuccess)
-    return SB_ERR_CUDA;
-  sb::beam_topk_kernel<<<1, 256, smem, stream>>>(scores, n, k, out_idx, out_val);
-  return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
-}

@@ -57,9 +57,7 @@ enum C2Epilogue : int {
 // 8 K-rows of 128 B per swizzle atom (SBO = 1024 B between atoms), the next 64 MN at
 // LBO = 8192 B (the next box).  One MMA (K = 16) spans two atoms; the next MMA starts 2048 B on.
 static constexpr int MN_BOX_BYTES = 64 * 64 * 2;
-static int g_mn_lbo = MN_BOX_BYTES, g_mn_sbo = 1024, g_mn_kadv = 2048;   // developer knobs
-
-struct MnDesc { uint32_t lbo, sbo, kadv; };
+static constexpr uint32_t MN_LBO = MN_BOX_BYTES, MN_SBO = 1024, MN_KADV = 2048;
 
 template <int BN>
 struct GemmCfg {
@@ -72,8 +70,7 @@ struct GemmCfg {
 template <int BN, int TA, int TB>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,
-                    const __grid_constant__ CUtensorMap tmap_b, const GemmParams p,
-                    const MnDesc mn) {
+                    const __grid_constant__ CUtensorMap tmap_b, const GemmParams p) {
   using Cfg = GemmCfg<BN>;
   constexpr int kStages = Cfg::kStages;
   extern __shared__ uint8_t smem_raw[];
@@ -145,8 +142,8 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,
     const int half = (warp >> 2) - 1;
     const int t = threadIdx.x & 127;
     const bool leader = t == 0;
-    const uint64_t a_step = TA ? (uint64_t)(mn.kadv >> 4) : 2u;
-    const uint64_t b_step = TB ? (uint64_t)(mn.kadv >> 4) : 2u;
+    const uint64_t a_step = TA ? (uint64_t)(MN_KADV >> 4) : 2u;
+    const uint64_t b_step = TB ? (uint64_t)(MN_KADV >> 4) : 2u;
     const bool vec_ok = ((p.ldc & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 7) == 0);
     int stage = 0;
     uint32_t phase = 0;
@@ -167,9 +164,9 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,
         const uint32_t sa = smem_u32(tiles + stage * Cfg::kStageBytes);
         const uint32_t sb_ = sa + BM * BK * 2;
         // K-major A: rows 64*half.. start 8 KB on; MN-major A: the half-th 64-wide box
-        const uint64_t da = TA ? gmma_desc_sw128_mnmajor(sa + half * MN_BOX_BYTES, mn.lbo, mn.sbo)
+        const uint64_t da = TA ? gmma_desc_sw128_mnmajor(sa + half * MN_BOX_BYTES, MN_LBO, MN_SBO)
                                : gmma_desc_sw128_kmajor(sa + half * 64 * 128);
-        const uint64_t db = TB ? gmma_desc_sw128_mnmajor(sb_, mn.lbo, mn.sbo)
+        const uint64_t db = TB ? gmma_desc_sw128_mnmajor(sb_, MN_LBO, MN_SBO)
                                : gmma_desc_sw128_kmajor(sb_);
         wgmma_fence();
 #pragma unroll
@@ -266,8 +263,7 @@ template <int TA, int TB>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_tn_c2_kernel(const __grid_constant__ CUtensorMap tmap_a,
                        const __grid_constant__ CUtensorMap tmap_b,
-                       const __grid_constant__ CUtensorMap tmap_c, const GemmParams p,
-                       const MnDesc mn) {
+                       const __grid_constant__ CUtensorMap tmap_c, const GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* tiles = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                               ~static_cast<uintptr_t>(1023));
@@ -346,8 +342,8 @@ gemm_bf16_tn_c2_kernel(const __grid_constant__ CUtensorMap tmap_a,
     const int half = (warp >> 2) - 1;
     const int t = threadIdx.x & 127;
     const bool leader = t == 0;
-    const uint64_t a_step = TA ? (uint64_t)(mn.kadv >> 4) : 2u;
-    const uint64_t b_step = TB ? (uint64_t)(mn.kadv >> 4) : 2u;
+    const uint64_t a_step = TA ? (uint64_t)(MN_KADV >> 4) : 2u;
+    const uint64_t b_step = TB ? (uint64_t)(MN_KADV >> 4) : 2u;
     const bool vec_ok = ((p.ldc & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 7) == 0);
     const uint32_t my_boxes = smem_u32(epi_boxes + half * C2_EPI_BUFS * C2_EPI_BOX_BYTES);
     uint32_t n_boxes = 0;                // boxes this warpgroup has staged (the next buffer follows)
@@ -370,9 +366,9 @@ gemm_bf16_tn_c2_kernel(const __grid_constant__ CUtensorMap tmap_a,
         mbar_wait(&full_bar[stage], phase);
         const uint32_t sa = smem_u32(tiles + stage * C2_STAGE_BYTES);
         const uint32_t sb_ = sa + C2_A_BYTES;
-        const uint64_t da = TA ? gmma_desc_sw128_mnmajor(sa + half * MN_BOX_BYTES, mn.lbo, mn.sbo)
+        const uint64_t da = TA ? gmma_desc_sw128_mnmajor(sa + half * MN_BOX_BYTES, MN_LBO, MN_SBO)
                                : gmma_desc_sw128_kmajor(sa + half * 64 * 128);
-        const uint64_t db = TB ? gmma_desc_sw128_mnmajor(sb_, mn.lbo, mn.sbo)
+        const uint64_t db = TB ? gmma_desc_sw128_mnmajor(sb_, MN_LBO, MN_SBO)
                                : gmma_desc_sw128_kmajor(sb_);
         wgmma_fence();
 #pragma unroll
@@ -578,8 +574,7 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, GemmParams 
   const int total = p.m_tiles * p.n_tiles * p.split_k;
   int grid = device_sm_count();
   if (grid > total) grid = total;
-  const MnDesc mn = {(uint32_t)g_mn_lbo, (uint32_t)g_mn_sbo, (uint32_t)g_mn_kadv};
-  gemm_bf16_tn_kernel<BN, TA, TB><<<grid, GEMM_THREADS, Cfg::kSmemBytes, stream>>>(ta, tb, p, mn);
+  gemm_bf16_tn_kernel<BN, TA, TB><<<grid, GEMM_THREADS, Cfg::kSmemBytes, stream>>>(ta, tb, p);
   return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
 }
 
@@ -630,7 +625,6 @@ static int launch_gemm_c2(const CUtensorMap& ta, const CUtensorMap& tb, const CU
   int clusters = c2_max_clusters();
   if (clusters <= 0) return SB_ERR_UNSUPPORTED;
   if (clusters > total) clusters = total;
-  const MnDesc mn = {(uint32_t)g_mn_lbo, (uint32_t)g_mn_sbo, (uint32_t)g_mn_kadv};
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(2 * clusters);
   cfg.blockDim = dim3(GEMM_THREADS);
@@ -643,7 +637,7 @@ static int launch_gemm_c2(const CUtensorMap& ta, const CUtensorMap& tb, const CU
   attr.val.clusterDim.z = 1;
   cfg.attrs = &attr;
   cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, kernel, ta, tb, tc, p, mn) == cudaSuccess ? SB_OK : SB_ERR_CUDA;
+  return cudaLaunchKernelEx(&cfg, kernel, ta, tb, tc, p) == cudaSuccess ? SB_OK : SB_ERR_CUDA;
 }
 
 template <int BN>
@@ -675,14 +669,6 @@ extern "C" const char* sb_debug_gemm_kernel(void) { return sb::g_gemm_last; }
 // stores / reduce-adds), "regs" (stored straight from the registers: every other kernel, and the
 // c2 kernel's fall-back), "skipped" (flag 4), "none" before the first launch
 extern "C" const char* sb_debug_gemm_epilogue(void) { return sb::g_gemm_epi_last; }
-
-// developer hook: override the MN-major descriptor fields (bytes); 0 keeps a field
-extern "C" int sb_debug_umma_mn(int lbo, int sbo, int kadv) {
-  if (lbo > 0) sb::g_mn_lbo = lbo;
-  if (sbo > 0) sb::g_mn_sbo = sbo;
-  if (kadv > 0) sb::g_mn_kadv = kadv;
-  return SB_OK;
-}
 
 extern "C" int sb_gemm_bf16_tn(const void* A, long long lda, const void* B, long long ldb, float* C,
                                long long ldc, const float* bias, int M, int N, int K, int flags,

@@ -32,6 +32,7 @@
 // weights per token (B*T*H*4 bytes forward, 3x that backward, + 24 H^2), in practice launch-bound.
 #include "beam.cuh"
 #include <math.h>
+#include <stddef.h>
 #include <string.h>
 
 #include "../../include/speech_b200.h"
@@ -854,7 +855,10 @@ __global__ void __launch_bounds__(32 * CELL_WARPS) s2s_cell_bwd_kernel(const Cel
 // is back-tracked on the device when the search stops.
 // ------------------------------------------------------------------------------------------------
 static constexpr int BM_MAXK = 32;
+// done and out_len lead, at the byte offsets the header promises (the host reads them in place)
 struct BeamState {
+  int done;
+  int out_len;
   double score[BM_MAXK];     // live beam scores
   int node[BM_MAXK];         // node id of each live entry
   int token[BM_MAXK];        // last token of each live entry (input of the next step)
@@ -863,10 +867,10 @@ struct BeamState {
   double best_c_score;       // best complete hypothesis (first inserted among equals)
   int best_c_node;
   int have_complete;
-  int done;
   int nodes_used;
-  int out_len;
 };
+static_assert(offsetof(BeamState, done) == 0 && offsetof(BeamState, out_len) == 4,
+              "sb_s2s_beam_state_size: done / out_len offsets");
 
 struct BeamParams {
   const float* logp;         // (K, C) log-softmax of this step's logits
@@ -1103,15 +1107,14 @@ static int attn_dims_ok(int B, int T, int H, int Kc) {
   return SB_OK;
 }
 
-extern "C" int sb_s2s_attn_fwd_len(const float* eh, int eh_bcast, const float* hx,
-                                   const float* ax_prev, const float* conv_wT, const float* conv_b,
-                                   const float* lin_w, float lin_b, int log_t, int B, int T, int H,
-                                   int Kc, float* sx, float* ax, const float* fc_w,
-                                   const float* fc_b, int C, float* logits,
-                                   long long logit_stride, float* logp, int* argmax, int* history,
-                                   int hist_stride, int hist_col, int* end_count, int end_tok,
-                                   const int* done, const int* lens, void* workspace,
-                                   size_t workspace_bytes, void* stream_) {
+extern "C" int sb_s2s_attn_fwd(const float* eh, int eh_bcast, const float* hx, const float* ax_prev,
+                               const float* conv_wT, const float* conv_b, const float* lin_w,
+                               float lin_b, int log_t, int B, int T, int H, int Kc, float* sx,
+                               float* ax, const float* fc_w, const float* fc_b, int C,
+                               float* logits, long long logit_stride, float* logp, int* argmax,
+                               int* history, int hist_stride, int hist_col, int* end_count,
+                               int end_tok, const int* done, const int* lens, void* workspace,
+                               size_t workspace_bytes, void* stream_) {
   if (!eh || !hx || !conv_wT || !conv_b || !lin_w || !sx || !ax || !workspace) return SB_ERR_INVALID;
   int rc = attn_dims_ok(B, T, H, Kc);
   if (rc != SB_OK) return rc;
@@ -1136,40 +1139,6 @@ extern "C" int sb_s2s_attn_fwd_len(const float* eh, int eh_bcast, const float* h
   return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
 }
 
-extern "C" int sb_s2s_attn_fwd(const float* eh, int eh_bcast, const float* hx, const float* ax_prev,
-                               const float* conv_wT, const float* conv_b, const float* lin_w,
-                               float lin_b, int log_t, int B, int T, int H, int Kc, float* sx,
-                               float* ax, const float* fc_w, const float* fc_b, int C,
-                               float* logits, long long logit_stride, float* logp, int* argmax,
-                               int* history, int hist_stride, int hist_col, int* end_count,
-                               int end_tok, const int* done, void* workspace,
-                               size_t workspace_bytes, void* stream_) {
-  return sb_s2s_attn_fwd_len(eh, eh_bcast, hx, ax_prev, conv_wT, conv_b, lin_w, lin_b, log_t, B,
-                             T, H, Kc, sx, ax, fc_w, fc_b, C, logits, logit_stride, logp, argmax,
-                             history, hist_stride, hist_col, end_count, end_tok, done, nullptr,
-                             workspace, workspace_bytes, stream_);
-}
-
-// the standalone attention step (no output projection): NNAttention.forward on the decode path
-extern "C" int sb_attn_step_len(const float* eh, const float* dhx, const float* ax_prev,
-                                const float* conv_wT, const float* conv_b, const float* lin_w,
-                                float lin_b, int log_t, int B, int T, int H, int Kc, float* sx,
-                                float* ax, const int* lens, void* workspace,
-                                size_t workspace_bytes, void* stream_) {
-  return sb_s2s_attn_fwd_len(eh, 0, dhx, ax_prev, conv_wT, conv_b, lin_w, lin_b, log_t, B, T, H,
-                             Kc, sx, ax, nullptr, nullptr, 0, nullptr, 0, nullptr, nullptr,
-                             nullptr, 0, 0, nullptr, 0, nullptr, lens, workspace, workspace_bytes,
-                             stream_);
-}
-
-extern "C" int sb_attn_step(const float* eh, const float* dhx, const float* ax_prev,
-                            const float* conv_wT, const float* conv_b, const float* lin_w,
-                            float lin_b, int log_t, int B, int T, int H, int Kc, float* sx,
-                            float* ax, void* workspace, size_t workspace_bytes, void* stream_) {
-  return sb_attn_step_len(eh, dhx, ax_prev, conv_wT, conv_b, lin_w, lin_b, log_t, B, T, H, Kc, sx,
-                          ax, nullptr, workspace, workspace_bytes, stream_);
-}
-
 extern "C" int sb_s2s_dout(const float* dlogits, const float* fc_w, const float* hx, const float* sx,
                            float* d_o, float* o_all, long long rows, int C, int H, void* stream_) {
   if (!dlogits || !fc_w || !hx || !sx || !d_o || !o_all || rows <= 0 || C <= 0 || H <= 0)
@@ -1180,16 +1149,15 @@ extern "C" int sb_s2s_dout(const float* dlogits, const float* fc_w, const float*
   return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
 }
 
-extern "C" int sb_s2s_attn_bwd_len(const float* eh, const float* hx, const float* hx_prev,
-                                   const float* ax_prev, const float* ax, const float* conv_wT,
-                                   const float* conv_b, const float* lin_w, const float* d_o,
-                                   const float* d_ix_next, const float* d_ax_next,
-                                   const float* d_hx_next, const float* gates, float* d_eh,
-                                   float* d_ax_prev, float* d_gi, float* d_gh, float* d_hx_direct,
-                                   float* g_conv_wT, float* g_conv_b, float* g_lin_w,
-                                   float* g_lin_b, int log_t, int B, int T, int H, int Kc,
-                                   const int* lens, void* workspace, size_t workspace_bytes,
-                                   void* stream_) {
+extern "C" int sb_s2s_attn_bwd(const float* eh, const float* hx, const float* hx_prev,
+                               const float* ax_prev, const float* ax, const float* conv_wT,
+                               const float* conv_b, const float* lin_w, const float* d_o,
+                               const float* d_ix_next, const float* d_ax_next,
+                               const float* d_hx_next, const float* gates, float* d_eh,
+                               float* d_ax_prev, float* d_gi, float* d_gh, float* d_hx_direct,
+                               float* g_conv_wT, float* g_conv_b, float* g_lin_w, float* g_lin_b,
+                               int log_t, int B, int T, int H, int Kc, const int* lens,
+                               void* workspace, size_t workspace_bytes, void* stream_) {
   if (!eh || !hx || !hx_prev || !ax || !conv_wT || !conv_b || !lin_w || !d_o || !gates || !d_eh ||
       !d_ax_prev || !d_gi || !d_gh || !d_hx_direct || !g_conv_wT || !g_conv_b || !g_lin_w ||
       !g_lin_b || !workspace)
@@ -1219,21 +1187,6 @@ extern "C" int sb_s2s_attn_bwd_len(const float* eh, const float* hx, const float
   s2s_attn_bwd_a_kernel<<<grid, ATT_THREADS, smem_a, stream>>>(p);
   s2s_attn_bwd_b_kernel<<<grid, ATT_THREADS, smem_b, stream>>>(p);
   return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
-}
-
-extern "C" int sb_s2s_attn_bwd(const float* eh, const float* hx, const float* hx_prev,
-                               const float* ax_prev, const float* ax, const float* conv_wT,
-                               const float* conv_b, const float* lin_w, const float* d_o,
-                               const float* d_ix_next, const float* d_ax_next,
-                               const float* d_hx_next, const float* gates, float* d_eh,
-                               float* d_ax_prev, float* d_gi, float* d_gh, float* d_hx_direct,
-                               float* g_conv_wT, float* g_conv_b, float* g_lin_w, float* g_lin_b,
-                               int log_t, int B, int T, int H, int Kc, void* workspace,
-                               size_t workspace_bytes, void* stream_) {
-  return sb_s2s_attn_bwd_len(eh, hx, hx_prev, ax_prev, ax, conv_wT, conv_b, lin_w, d_o, d_ix_next,
-                             d_ax_next, d_hx_next, gates, d_eh, d_ax_prev, d_gi, d_gh, d_hx_direct,
-                             g_conv_wT, g_conv_b, g_lin_w, g_lin_b, log_t, B, T, H, Kc, nullptr,
-                             workspace, workspace_bytes, stream_);
 }
 
 extern "C" int sb_s2s_cell_bwd(const float* d_gi, const float* d_gh, const float* d_hx_direct,

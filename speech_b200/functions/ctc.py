@@ -16,7 +16,7 @@ could not be inspected (SURVEY.md §8b).
 """
 import torch
 
-from .. import _lib
+from .. import _lib, ops
 
 
 def ctc_costs_and_grads(acts, labels, act_lens, label_lens, blank=None, need_grad=True):
@@ -30,44 +30,19 @@ def ctc_costs_and_grads(acts, labels, act_lens, label_lens, blank=None, need_gra
     if blank is None:
         blank = V - 1
     dev = acts.device
-
-    lab = labels.detach().to("cpu", torch.int32).reshape(-1)
-    llen = label_lens.detach().to("cpu", torch.int32).reshape(-1)
-    alen = act_lens.detach().to("cpu", torch.int32).reshape(-1)
-    if llen.numel() != B or alen.numel() != B:
-        raise ValueError("act_lens / label_lens must have one entry per utterance")
-    if int(llen.sum()) != lab.numel():
-        raise ValueError("labels has %d entries but label_lens sums to %d"
-                         % (lab.numel(), int(llen.sum())))
-    if lab.numel() and (int(lab.min()) < 0 or int(lab.max()) >= V):
-        raise ValueError("label out of range")
-    max_l = int(llen.max()) if B else 0
-    offs = torch.zeros(B, dtype=torch.int32)
-    if B > 1:
-        offs[1:] = torch.cumsum(llen[:-1], 0)
-    # one packed host->device copy: [labels | offsets | label_lens | act_lens]
-    n_lab = lab.numel()
-    packed = torch.cat([lab, offs, llen, alen]).pin_memory().to(dev, non_blocking=True)
-    d_lab = packed[:n_lab]
-    d_off = packed[n_lab:n_lab + B]
-    d_llen = packed[n_lab + B:n_lab + 2 * B]
-    d_alen = packed[n_lab + 2 * B:]
-
-    import ctypes
-    nbytes = ctypes.c_size_t(0)
-    _lib.check(lib.sb_ctc_workspace_size(B, T, V, max_l, ctypes.byref(nbytes)),
-               "sb_ctc_workspace_size")
-    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+    (d_lab, d_off, d_llen, d_alen), max_l = _lib.pack_labels(labels, label_lens, act_lens, B, dev,
+                                                            num_classes=V)
+    nbytes = _lib.workspace_size(lib.sb_ctc_workspace_size, B, T, V, max_l)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     costs = torch.empty(B, dtype=torch.float32, device=dev)
     grads = torch.empty_like(acts) if need_grad else None
-    from .. import ops
     with torch.cuda.device(dev):
         sp = _lib.stream_ptr()
         ops._launch("ctc_fwd_bwd", 0.0,
                     lambda: lib.sb_ctc_fwd_bwd(acts.data_ptr(), _lib.ptr(grads), d_lab.data_ptr(),
                                                d_off.data_ptr(), d_llen.data_ptr(),
                                                d_alen.data_ptr(), B, T, V, int(blank), max_l,
-                                               costs.data_ptr(), ws.data_ptr(), nbytes.value, sp))
+                                               costs.data_ptr(), ws.data_ptr(), nbytes, sp))
     return costs, grads
 
 

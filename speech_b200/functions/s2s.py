@@ -6,11 +6,9 @@ steps in one launch, the weight gradients time-batched on the wgmma GEMM), a gre
 beam search that never leave the device: the host only enqueues kernels and reads the final
 hypothesis back once.
 """
-import ctypes
-
 import torch
 
-from .. import _lib
+from .. import _lib, ops
 
 
 def _f(t):
@@ -21,16 +19,17 @@ def _f(t):
 # which holds all C logits next to its 8 H-float tiles: C <= 7 H (sb_s2s_fc_fused).  Larger
 # vocabularies project over many CTAs (sb_s2s_fc_rows, csrc/s2s_vocab.cu).  sb_s2s_dout holds one
 # row of dlogits in shared memory (C <= 8192); past that d_o runs on the GEMM.  The single-CTA beam
-# selection holds all K*C float64 candidates (<= 200 KB); past that it runs split over many CTAs.
-FC_FUSED_MAX_RATIO = 7
+# selection holds all K*C float64 candidates (<= 200 KB, sb_s2s_beam_select_fits); past that it
+# runs split over many CTAs.
 DOUT_MAX_CLASSES = 8192
-BEAM_SELECT_MAX_BYTES = 200 * 1024
-BEAM_MAX = 32
+# byte offsets of `done` and of the final hypothesis' length in the beam state (speech_b200.h)
+BEAM_DONE_OFFSET = 0
+BEAM_OUT_LEN_OFFSET = 4
 
 
 def fc_fused(H, C):
-    """True where the attention kernel computes the logits itself (= sb_s2s_fc_fused(H, C))."""
-    return H > 0 and 0 < C <= FC_FUSED_MAX_RATIO * H
+    """True where the attention kernel computes the logits itself (sb_s2s_fc_fused(H, C))."""
+    return bool(_lib.load().sb_s2s_fc_fused(int(H), int(C)))
 
 
 def dout_fits(C):
@@ -39,43 +38,52 @@ def dout_fits(C):
 
 
 def beam_select_fits(K, C):
-    """True where the single-CTA beam selection runs (= sb_s2s_beam_select_fits(K, C))."""
-    return 0 < K <= BEAM_MAX and C > 0 and K * C * 8 <= BEAM_SELECT_MAX_BYTES
+    """True where the single-CTA beam selection runs (sb_s2s_beam_select_fits(K, C))."""
+    return bool(_lib.load().sb_s2s_beam_select_fits(int(K), int(C)))
 
 
-class DecoderWeights:
-    """fp32 contiguous views of the decoder parameters, in the layout the kernels take.  `fused`:
-    the attention kernel runs the output projection (fc_fused), else sb_s2s_fc_rows does."""
+class AttentionWeights:
+    """fp32 contiguous views of NNAttention's parameters, in the layout the attention kernel takes,
+    and their device addresses (looked up once: the per-token loops only do integer arithmetic)."""
 
-    def __init__(self, m):
-        self.emb = _f(m.embedding.weight)
-        self.w_ih, self.w_hh = _f(m.dec_rnn.weight_ih), _f(m.dec_rnn.weight_hh)
-        self.b_ih, self.b_hh = _f(m.dec_rnn.bias_ih), _f(m.dec_rnn.bias_hh)
-        conv, lin = m.attend.conv, m.attend.nn[1].fc
+    def __init__(self, attend):
+        conv, lin = attend.conv, attend.nn[1].fc
         self.conv_wT = _f(conv.weight).reshape(conv.weight.shape[0], -1).t().contiguous()  # (Kc, H)
         self.conv_b = _f(conv.bias)
         self.lin_w = _f(lin.weight).reshape(-1)
         self.lin_b = float(lin.bias.detach().float().item()) if lin.bias is not None else 0.0
+        self.log_t = 1 if attend.log_t else 0
+        self.Kc, self.H = self.conv_wT.shape
+        self._addresses("conv_wT", "conv_b", "lin_w")
+
+    def _addresses(self, *names):
+        for n in names:
+            setattr(self, "p_" + n, getattr(self, n).data_ptr())
+
+
+class DecoderWeights(AttentionWeights):
+    """fp32 contiguous views of the decoder parameters, in the layout the kernels take.  `fused`:
+    the attention kernel runs the output projection (fc_fused), else sb_s2s_fc_rows does."""
+
+    def __init__(self, m):
+        super().__init__(m.attend)
+        self.emb = _f(m.embedding.weight)
+        self.w_ih, self.w_hh = _f(m.dec_rnn.weight_ih), _f(m.dec_rnn.weight_hh)
+        self.b_ih, self.b_hh = _f(m.dec_rnn.bias_ih), _f(m.dec_rnn.bias_hh)
         self.fc_w, self.fc_b = _f(m.fc.fc.weight), _f(m.fc.fc.bias)
-        self.log_t = 1 if m.attend.log_t else 0
         self.H = self.w_hh.shape[1]
-        self.Kc = self.conv_wT.shape[0]
         self.C = self.fc_w.shape[0]
         if self.emb.shape[1] != self.H:
             raise _lib.SpeechB200Error("Seq2Seq: embedding_dim must equal the encoder dim (ix + sx)")
         self.fused = fc_fused(self.H, self.C)
-        # device addresses, looked up once: the per-token loops only do integer arithmetic
-        for n in ("emb", "w_ih", "w_hh", "b_ih", "b_hh", "conv_wT", "conv_b", "lin_w", "fc_w",
-                  "fc_b"):
-            setattr(self, "p_" + n, getattr(self, n).data_ptr())
+        self._addresses("emb", "w_ih", "w_hh", "b_ih", "b_hh", "fc_w", "fc_b")
 
 
 def attn_workspace(lib, B, T, H, dev):
     """zeroed scratch of the attention kernels (per-CTA softmax partials + ticket counters); one
     buffer serves every step of a decode on the same stream"""
-    n = ctypes.c_size_t(0)
-    _lib.check(lib.sb_s2s_workspace_size(B, T, H, ctypes.byref(n)), "s2s workspace")
-    return torch.zeros(n.value, dtype=torch.uint8, device=dev)
+    n = _lib.workspace_size(lib.sb_s2s_workspace_size, B, T, H)
+    return torch.zeros(n, dtype=torch.uint8, device=dev)
 
 
 def _a(x):
@@ -84,7 +92,6 @@ def _a(x):
 
 
 def _cell_fwd(lib, w, tok, tok_stride, sx_prev, hx_prev, hx, ix_save, gates_save, done, B, sp):
-    from .. import ops
     ops._launch("s2s_cell_fwd", 0.0,
                 lambda: lib.sb_s2s_cell_fwd(w.p_emb, tok, tok_stride, _a(sx_prev), _a(hx_prev),
                                             w.p_w_ih, w.p_w_hh, w.p_b_ih, w.p_b_hh, _a(hx),
@@ -94,30 +101,28 @@ def _cell_fwd(lib, w, tok, tok_stride, sx_prev, hx_prev, hx, ix_save, gates_save
 def _attn_fwd(lib, w, ws, eh, bcast, hx, ax_prev, sx, ax, B, T, sp, logits=None, logit_stride=0,
               logp=None, argmax=None, history=None, hist_stride=0, hist_col=0, end_count=None,
               end_tok=-1, done=None, with_fc=True, lens=None):
-    from .. import ops
+    """the attention step of B rows; with_fc: also the output projection (w: DecoderWeights),
+    else the attention alone (w may be AttentionWeights)"""
+    fc_w, fc_b, C = (w.p_fc_w, w.p_fc_b, w.C) if with_fc else (None, None, 0)
     ops._launch("s2s_attn_fwd", 0.0,
-                lambda: lib.sb_s2s_attn_fwd_len(_a(eh), bcast, _a(hx), _a(ax_prev), w.p_conv_wT,
-                                                w.p_conv_b, w.p_lin_w, w.lin_b, w.log_t, B, T, w.H,
-                                                w.Kc, _a(sx), _a(ax),
-                                                w.p_fc_w if with_fc else None,
-                                                w.p_fc_b if with_fc else None, w.C,
-                                                logits, logit_stride, _a(logp), _a(argmax),
-                                                history, hist_stride, hist_col, end_count,
-                                                end_tok, done, _a(lens), _a(ws), ws.numel(), sp))
+                lambda: lib.sb_s2s_attn_fwd(_a(eh), bcast, _a(hx), _a(ax_prev), w.p_conv_wT,
+                                            w.p_conv_b, w.p_lin_w, w.lin_b, w.log_t, B, T, w.H,
+                                            w.Kc, _a(sx), _a(ax), fc_w, fc_b, C, logits,
+                                            logit_stride, _a(logp), _a(argmax), history,
+                                            hist_stride, hist_col, end_count, end_tok, done,
+                                            _a(lens), _a(ws), ws.numel(), sp))
 
 
 def fc_workspace(lib, R, C, dev):
     """zeroed scratch of sb_s2s_fc_rows / _logp for R rows (tile partials, log-sum-exp, tickets)"""
-    n = ctypes.c_size_t(0)
-    _lib.check(lib.sb_s2s_fc_workspace_size(R, C, ctypes.byref(n)), "s2s fc workspace")
-    return torch.zeros(n.value, dtype=torch.uint8, device=dev)
+    n = _lib.workspace_size(lib.sb_s2s_fc_workspace_size, R, C)
+    return torch.zeros(n, dtype=torch.uint8, device=dev)
 
 
 def _fc_rows(lib, w, ws, hx, sx, R, sp, logits=None, group=0, ld0=0, ld1=0, argmax=None,
              history=None, hist_stride=0, hist_col=0, end_count=None, end_tok=-1, done=None):
     """logits of R rows o = hx + sx over many CTAs; row r at logits + (r % group) * ld0 +
     (r / group) * ld1 (default: dense (R, C)), with the row reductions of the same launch."""
-    from .. import ops
     group = group or R
     ld0 = ld0 or w.C
     ops._launch("s2s_fc_rows", 2.0 * R * w.C * w.H,
@@ -129,7 +134,6 @@ def _fc_rows(lib, w, ws, hx, sx, R, sp, logits=None, group=0, ld0=0, ld1=0, argm
 
 def _fc_logp(lib, w, ws, logits, logp, R, sp, done=None):
     """logp (R, C) = logits (dense (R, C)) - the log-sum-exp the last _fc_rows left in ws"""
-    from .. import ops
     ops._launch("s2s_fc_logp", 0.0,
                 lambda: lib.sb_s2s_fc_logp(_a(logits), R, w.C, 0, _a(logp), R, w.C, _a(done),
                                            _a(ws), ws.numel(), sp))
@@ -138,7 +142,6 @@ def _fc_logp(lib, w, ws, logits, logp, R, sp, done=None):
 def _dout_gemm(dl, fc_w, d_o):
     """d_o (R, H) = dl (R, C) @ fc_w (C, H) for C past sb_s2s_dout: 3-pass split-bf16 on the wgmma
     GEMM (hi*hi + hi*lo + lo*hi, relative error ~2^-16, as ops.gemm_split), fc_w read as [K][N]."""
-    from .. import ops
     R, C = dl.shape
     H = fc_w.shape[1]
     Cp, Hp = (C + 7) // 8 * 8, (H + 7) // 8 * 8
@@ -168,6 +171,25 @@ def attn_lens(lens, B, T, dev):
     if bool((ln == T).all()):
         return None
     return ln.to(torch.int32).to(dev)
+
+
+def attn_step(attend, eh, dhx, ax_prev, lens=None):
+    """NNAttention.forward on the decode path (no autograd): eh (B,T,H), dhx (B,1,H) or (B,H),
+    ax_prev (B,T) or None; lens (optional): frames each utterance attends over (ax is 0 past
+    them).  Returns (sx (B,1,H), ax (B,T)) like the reference module."""
+    _lib.require_cuda(eh, "eh")
+    lib = _lib.load()
+    w = AttentionWeights(attend)
+    eh = _f(eh)
+    B, T, H = eh.shape
+    d = dhx.detach().float().reshape(B, H).contiguous()
+    axp = None if ax_prev is None else _f(ax_prev)
+    sx = torch.empty(B, H, dtype=torch.float32, device=eh.device)
+    ax = torch.empty(B, T, dtype=torch.float32, device=eh.device)
+    ws = attn_workspace(lib, B, T, H, eh.device)
+    ld = attn_lens(lens, B, T, eh.device)
+    _attn_fwd(lib, w, ws, eh, 0, d, axp, sx, ax, B, T, _lib.stream_ptr(), with_fc=False, lens=ld)
+    return sx.unsqueeze(1), ax
 
 
 class DecodeFunction(torch.autograd.Function):
@@ -249,7 +271,6 @@ class DecodeFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dlogits, daligns):
-        from .. import ops
         lib = _lib.load()
         w = ctx.w
         ehc, hx_all, sx_all, ax_all, ix_all, gates_all, used = ctx.saved
@@ -302,7 +323,7 @@ class DecodeFunction(torch.autograd.Function):
                     d_ax_next = da_ext[u].data_ptr()
                 else:
                     d_ax[(u + 1) & 1].add_(da_ext[u])
-            ops._launch("s2s_attn_bwd", 0.0, lambda: lib.sb_s2s_attn_bwd_len(
+            ops._launch("s2s_attn_bwd", 0.0, lambda: lib.sb_s2s_attn_bwd(
                 p_eh, p_hx + (u + 1) * BH, p_hx + u * BH, p_ax + (u - 1) * BT if u > 0 else None,
                 p_ax + u * BT, w.p_conv_wT, w.p_conv_b, w.p_lin_w, p_do + u * BH,
                 None if last else p_dix + (u + 1) * BH, d_ax_next, None if last else p_dhp,
@@ -411,7 +432,6 @@ def greedy(m, eh, start, end_tok, max_len, lens=None):
     sp = _lib.stream_ptr()
     ws = attn_workspace(lib, B, T, H, dev)
     ld = attn_lens(lens, B, T, dev)
-    from .. import ops
     fc_ws = None if w.fused else fc_workspace(lib, B, w.C, dev)
     for e in range(max_len):
         cur, prv = e & 1, (e & 1) ^ 1
@@ -439,16 +459,14 @@ def beam_search(m, eh, start_tok, end_tok, beam_size, max_len):
     """Seq2Seq.beam_search for one utterance (seq2seq.py:180-227), device-resident: the beam
     entries are the rows of the step kernels, expand/prune/complete/stop run in one bookkeeping
     kernel per step (csrc/s2s.cu), the hypothesis is back-tracked on the device."""
-    from .. import ops
     lib = _lib.load()
     w = DecoderWeights(m)
     ehc = _f(eh)[:1].contiguous()
     _, T, H = ehc.shape
     K, C = int(beam_size), w.C
     dev = ehc.device
-    nbytes = ctypes.c_size_t(0)
-    _lib.check(lib.sb_s2s_beam_state_size(ctypes.byref(nbytes)), "beam state")
-    state = torch.zeros(nbytes.value + 64, dtype=torch.uint8, device=dev)
+    state = torch.zeros(_lib.workspace_size(lib.sb_s2s_beam_state_size) + 64, dtype=torch.uint8,
+                        device=dev)
     node_cap = 2 * K * (max_len + 1) + 2
     nodes = torch.zeros(node_cap, 2, dtype=torch.int32, device=dev)
     c_cap = K * (max_len + 1)
@@ -465,13 +483,12 @@ def beam_search(m, eh, start_tok, end_tok, beam_size, max_len):
     _lib.check(lib.sb_s2s_beam_init(state.data_ptr(), nodes.data_ptr(), tok.data_ptr(),
                                     int(start_tok), sp), "beam init")
     # the `done` word of the state struct doubles as the no-op flag of the step kernels
-    done_ptr = state.data_ptr() + _beam_done_offset()
+    done_ptr = state.data_ptr() + BEAM_DONE_OFFSET
     fc_ws = None if w.fused else fc_workspace(lib, K, C, dev)
     split = not beam_select_fits(K, C)
     if split:
-        _lib.check(lib.sb_s2s_beam_split_workspace_size(K, C, ctypes.byref(nbytes)),
-                   "beam split workspace")
-        sel_ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+        sel_ws = torch.empty(_lib.workspace_size(lib.sb_s2s_beam_split_workspace_size, K, C),
+                             dtype=torch.uint8, device=dev)
     # buffers: [0] = state entering the step (gathered), [1] = state produced by the step
     for e in range(max_len):
         _cell_fwd(lib, w, tok.data_ptr(), 1, sx[0] if e > 0 else None, hx[0], hx[1], None, None,
@@ -497,15 +514,5 @@ def beam_search(m, eh, start_tok, end_tok, beam_size, max_len):
         ops._launch("s2s_beam_gather", 0.0, lambda: lib.sb_s2s_beam_gather(
             hx[1].data_ptr(), sx[1].data_ptr(), ax[1].data_ptr(), hx[0].data_ptr(),
             sx[0].data_ptr(), ax[0].data_ptr(), parent.data_ptr(), state.data_ptr(), K, H, T, sp))
-    n = int(state[_beam_outlen_offset():_beam_outlen_offset() + 4].view(torch.int32).item())
+    n = int(state[BEAM_OUT_LEN_OFFSET:BEAM_OUT_LEN_OFFSET + 4].view(torch.int32).item())
     return tuple(out_tokens[:n].cpu().tolist())
-
-
-def _beam_done_offset():
-    # struct BeamState { double score[32]; int node[32]; int token[32]; int nlive; int ncomplete;
-    #                    double best_c_score; int best_c_node; int have_complete; int done; ... }
-    return 32 * 8 + 32 * 4 + 32 * 4 + 4 + 4 + 8 + 4 + 4
-
-
-def _beam_outlen_offset():
-    return _beam_done_offset() + 4 + 4

@@ -9,11 +9,9 @@ speech/models/transducer_model.py:11 (call site :46-52; dependency cloned by Mak
 Blank = last class (transducer_model.py:28); reduction = sum over the minibatch.  Both are
 constructor keywords because the un-vendored dependency could not be inspected.
 """
-import ctypes
-
 import torch
 
-from .. import _lib
+from .. import _lib, ops
 
 
 def rnnt_costs_and_grads(log_probs, labels, x_lens, y_lens, blank=None, need_grad=True):
@@ -24,34 +22,18 @@ def rnnt_costs_and_grads(log_probs, labels, x_lens, y_lens, blank=None, need_gra
     if blank is None:
         blank = V - 1
     dev = lp.device
-    lab = labels.detach().to("cpu", torch.int32).reshape(-1)
-    ylen = y_lens.detach().to("cpu", torch.int32).reshape(-1)
-    xlen = x_lens.detach().to("cpu", torch.int32).reshape(-1)
-    if int(ylen.sum()) != lab.numel():
-        raise ValueError("labels / y_lens mismatch")
-    if B and int(ylen.max()) > U1 - 1:
-        raise ValueError("a label sequence is longer than the lattice (U+1 = %d)" % U1)
-    offs = torch.zeros(B, dtype=torch.int32)
-    if B > 1:
-        offs[1:] = torch.cumsum(ylen[:-1], 0)
-    n = lab.numel()
-    packed = torch.cat([lab, offs, ylen, xlen]).pin_memory().to(dev, non_blocking=True)
-    nbytes = ctypes.c_size_t(0)
-    _lib.check(lib.sb_rnnt_workspace_size(B, T, U1, ctypes.byref(nbytes)), "sb_rnnt_workspace_size")
-    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+    (lab, offs, ylen, xlen), _ = _lib.pack_labels(labels, y_lens, x_lens, B, dev, lattice_rows=U1)
+    nbytes = _lib.workspace_size(lib.sb_rnnt_workspace_size, B, T, U1)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     costs = torch.empty(B, dtype=torch.float32, device=dev)
     grads = torch.empty_like(lp) if need_grad else None
-    from .. import ops
     with torch.cuda.device(dev):
         sp = _lib.stream_ptr()
         ops._launch("rnnt_fwd_bwd", 0.0,
-                    lambda: lib.sb_rnnt_fwd_bwd(lp.data_ptr(), _lib.ptr(grads),
-                                                packed[:n].data_ptr(),
-                                                packed[n:n + B].data_ptr(),
-                                                packed[n + B:n + 2 * B].data_ptr(),
-                                                packed[n + 2 * B:].data_ptr(), B, T, U1, V,
-                                                int(blank), costs.data_ptr(), ws.data_ptr(),
-                                                nbytes.value, sp))
+                    lambda: lib.sb_rnnt_fwd_bwd(lp.data_ptr(), _lib.ptr(grads), lab.data_ptr(),
+                                                offs.data_ptr(), ylen.data_ptr(), xlen.data_ptr(),
+                                                B, T, U1, V, int(blank), costs.data_ptr(),
+                                                ws.data_ptr(), nbytes, sp))
     return costs, grads
 
 
@@ -130,7 +112,6 @@ def joint_vocab_forward(fxc, fyc, w2b, b2c, ym, blank, lp_full=None, shortlists=
     contiguous on the device.  Fills lp_full (B,T,U1,V1) f32 if given, and the batch-first
     shortlists (val, idx, meta) of sb_rnnt_shortlist_rows if given (kp = val.shape[3]).
     -> lat (nodes, 2) {log p(blank), log p(label)}, lse (nodes,) log-sum-exp of every node."""
-    from .. import ops
     lib = _lib.load()
     B, T, H = fxc.shape
     U1 = fyc.shape[1]
@@ -169,7 +150,6 @@ def joint_vocab_backward(fxc, fyc, w2b, b2c, ym, garc, lse, blank):
     forward's lse.  Per slab: z, the logits again (same GEMM), dlogits (bf16) and db2 from the row
     kernel, dW2 += dlogits^T z, dz = dlogits W2, then dz is reduced into dfx / dfy.
     -> dfx (B,T,H), dfy (B,U1,H), dw2 (V1,H), db2 (V1,), all f32."""
-    from .. import ops
     lib = _lib.load()
     B, T, H = fxc.shape
     U1 = fyc.shape[1]
@@ -211,26 +191,9 @@ def joint_vocab_backward(fxc, fyc, w2b, b2c, ym, garc, lse, blank):
     return dfx, dfy, dw2, db2
 
 
-def _pack_labels(labels, x_lens, y_lens, B, U1, dev):
-    lab = labels.detach().to("cpu", torch.int32).reshape(-1)
-    ylen = y_lens.detach().to("cpu", torch.int32).reshape(-1)
-    xlen = x_lens.detach().to("cpu", torch.int32).reshape(-1)
-    if int(ylen.sum()) != lab.numel():
-        raise ValueError("labels / y_lens mismatch")
-    if B and int(ylen.max()) > U1 - 1:
-        raise ValueError("a label sequence is longer than the lattice (U+1 = %d)" % U1)
-    offs = torch.zeros(B, dtype=torch.int32)
-    if B > 1:
-        offs[1:] = torch.cumsum(ylen[:-1], 0)
-    n = lab.numel()
-    packed = torch.cat([lab, offs, ylen, xlen]).pin_memory().to(dev, non_blocking=True)
-    return packed[:n], packed[n:n + B], packed[n + B:n + 2 * B], packed[n + 2 * B:]
-
-
 def _joint_operands(fx, fy, fc2, ymat):
     """fx, fy (f32), fc2's weight (bf16, zero columns up to fx's width), bias (f32) and the label
     matrix (int32), contiguous on fx's device, as the joint kernels take them."""
-    from .. import ops
     H = fx.shape[2]
     fxc, fyc = fx.detach().float().contiguous(), fy.detach().float().contiguous()
     w2 = fc2.weight.detach().to(torch.bfloat16)
@@ -245,7 +208,6 @@ def joint_log_probs(fx, fy, fc2, ymat, blank):
     to the beam search), from fx = fc1(x) (B,T,H), fy = fc1(pred) (B,U1,H); no autograd.
     fx / fy may carry zero units past fc2's input width (see Transducer.joint_inputs): fc2's
     weight gets zero columns for them."""
-    from .. import ops
     _lib.require_cuda(fx, "fx")
     lib = _lib.load()
     B, T, H = fx.shape
@@ -287,7 +249,6 @@ def joint_shortlists(fx, fy, fc2, ymat, blank, kp):
 class _JointLossFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, fx, fy, w2, b2, ymat, labels, x_lens, y_lens, blank, size_average):
-        from .. import ops
         _lib.require_cuda(fx, "fx")
         lib = _lib.load()
         B, T, H = fx.shape
@@ -298,7 +259,8 @@ class _JointLossFunction(torch.autograd.Function):
         w2b = w2.detach().to(torch.bfloat16).contiguous()
         b2c = b2.detach().float().contiguous()
         ym = ymat.detach().to(dev, torch.int32).contiguous()
-        lab, offs, ylen, xlen = _pack_labels(labels, x_lens, y_lens, B, U1, dev)
+        (lab, offs, ylen, xlen), _ = _lib.pack_labels(labels, y_lens, x_lens, B, dev,
+                                                      lattice_rows=U1)
         nodes = T * B * U1
         lse = None
         if joint_uses_slabs(H, V1):
@@ -312,9 +274,8 @@ class _JointLossFunction(torch.autograd.Function):
                                                       b2c.data_ptr(), ym.data_ptr(), lat.data_ptr(),
                                                       None, B, T, U1, H, V1, int(blank), sp))
         need = any(ctx.needs_input_grad[:4])
-        nbytes = ctypes.c_size_t(0)
-        _lib.check(lib.sb_rnnt_workspace_size(B, T, U1, ctypes.byref(nbytes)), "ws")
-        ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+        nbytes = _lib.workspace_size(lib.sb_rnnt_workspace_size, B, T, U1)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         costs = torch.empty(B, dtype=torch.float32, device=dev)
         garc = torch.empty(nodes, 2, dtype=torch.float32, device=dev) if need else None
         ops._launch("rnnt_fwd_bwd", 0.0,
@@ -322,7 +283,7 @@ class _JointLossFunction(torch.autograd.Function):
                                                         lab.data_ptr(), offs.data_ptr(),
                                                         ylen.data_ptr(), xlen.data_ptr(), B, T, U1,
                                                         int(blank), costs.data_ptr(), ws.data_ptr(),
-                                                        nbytes.value, sp))
+                                                        nbytes, sp))
         loss = costs.sum().reshape(1)
         scale = 1.0 / B if size_average else 1.0
         ctx.saved = (fxc, fyc, w2b, b2c, ym, garc)
@@ -332,7 +293,6 @@ class _JointLossFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_out):
-        from .. import ops
         lib = _lib.load()
         fxc, fyc, w2b, b2c, ym, garc = ctx.saved
         B, T, U1, H, V1, blank, scale = ctx.dims

@@ -5,8 +5,6 @@
 sb_ctc_prefix_beam (csrc/decode.cu), one CTA per utterance.  `decode_batch` is the batched
 entry CTC.infer uses (the reference loops over utterances in Python, ctc_model.py:59-60).
 """
-import ctypes
-
 import numpy as np
 import torch
 
@@ -17,10 +15,8 @@ def _run(logp, lens, beam_size, blank):
     lib = _lib.load()
     B, T, S = logp.shape
     dev = logp.device
-    nbytes = ctypes.c_size_t(0)
-    _lib.check(lib.sb_ctc_prefix_beam_workspace_size(B, T, beam_size, ctypes.byref(nbytes)),
-               "sb_ctc_prefix_beam_workspace_size")
-    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+    nbytes = _lib.workspace_size(lib.sb_ctc_prefix_beam_workspace_size, B, T, beam_size)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     out_labels = torch.empty(B, T, dtype=torch.int32, device=dev)
     out_lens = torch.empty(B, dtype=torch.int32, device=dev)
     out_scores = torch.empty(B, dtype=torch.float64, device=dev)
@@ -28,7 +24,7 @@ def _run(logp, lens, beam_size, blank):
         _lib.check(lib.sb_ctc_prefix_beam(logp.data_ptr(), lens.data_ptr(), B, T, S,
                                           int(beam_size), int(blank), out_labels.data_ptr(),
                                           out_lens.data_ptr(), out_scores.data_ptr(),
-                                          ws.data_ptr(), nbytes.value, _lib.stream_ptr()),
+                                          ws.data_ptr(), nbytes, _lib.stream_ptr()),
                    "sb_ctc_prefix_beam")
     labels = out_labels.cpu().numpy()
     n = out_lens.cpu().numpy()

@@ -161,8 +161,8 @@ class NNAttention(nn.Module):
         """(sx (B,1,H), ax (B,T)) of one attention step on the fused kernel (csrc/s2s.cu).  The
         module is a parameter container for the decoder: training differentiates the whole
         decode through functions/s2s.py, so this stand-alone call carries no autograd."""
-        from .. import ops
+        from ..functions import s2s
         if torch.is_grad_enabled() and (eh.requires_grad or dhx.requires_grad):
             raise RuntimeError("NNAttention.forward is inference-only; gradients flow through "
                                "Seq2Seq.decode (speech_b200.functions.s2s)")
-        return ops.attn_step(eh, dhx, ax, self.conv, self.nn[1].fc, self.log_t, lens)
+        return s2s.attn_step(self, eh, dhx, ax, lens)

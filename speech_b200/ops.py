@@ -487,9 +487,8 @@ class GRUStackFunction(torch.autograd.Function):
             X = torch.zeros(T, Bp, Inp, dtype=torch.bfloat16, device=dev)
             X[:, :B, :In] = x.transpose(0, 1)
             X = X.view(M, Inp)
-        nbytes = ctypes.c_size_t(0)
-        _lib.check(lib.sb_gru_fwd_workspace_size(Bp, Hp, ndir, ctypes.byref(nbytes)), "ws")
-        ws = _workspace(nbytes.value, dev)
+        nbytes = _lib.workspace_size(lib.sb_gru_fwd_workspace_size, Bp, Hp, ndir)
+        ws = _workspace(nbytes, dev)
         saved = []
         y = None
         for l in range(L):
@@ -531,7 +530,7 @@ class GRUStackFunction(torch.autograd.Function):
             _launch("gru_fwd", 2.0 * M * 3 * Hp * Hp * ndir,
                     lambda: lib.sb_gru_fwd(gi.data_ptr(), whh.data_ptr(), bhh.data_ptr(),
                                            y.data_ptr(), xn.data_ptr(), _lib.ptr(gates),
-                                           ws.data_ptr(), nbytes.value, T, Bp, Hp, ndir, sp))
+                                           ws.data_ptr(), nbytes, T, Bp, Hp, ndir, sp))
             mask = None
             hb = xn                                     # bf16 h_t (un-masked): dW_hh operand
             y_rec = y                                   # as the recurrence wrote it (backward)
@@ -612,9 +611,8 @@ class GRUStackFunction(torch.autograd.Function):
             dY = torch.zeros(T, Bp, D, dtype=torch.float32, device=dev)
             dY[:, :B] = pad_blocks(dout.transpose(0, 1), 2, ndir, H, Hp)
             dY = dY.view(M, D)
-        nbytes = ctypes.c_size_t(0)
-        _lib.check(lib.sb_gru_bwd_workspace_size(Bp, Hp, ndir, ctypes.byref(nbytes)), "ws")
-        ws = _workspace(nbytes.value, dev)
+        nbytes = _lib.workspace_size(lib.sb_gru_bwd_workspace_size, Bp, Hp, ndir)
+        ws = _workspace(nbytes, dev)
         grads = [None] * len(weights)
         for l in reversed(range(L)):
             X, y, gates, mask, wih_cat, whh, hb = ctx.saved[l]
@@ -634,7 +632,7 @@ class GRUStackFunction(torch.autograd.Function):
                     lambda dY=dY: lib.sb_gru_bwd(dY.data_ptr(), y.data_ptr(), gates.data_ptr(),
                                                  whh.data_ptr(), dgi.data_ptr(), dghn.data_ptr(),
                                                  dbih.data_ptr(), dbhh.data_ptr(), ws.data_ptr(),
-                                                 nbytes.value, T, Bp, Hp, ndir, sp))
+                                                 nbytes, T, Bp, Hp, ndir, sp))
             base = l * 4 * ndir
             # dW_hh pairs dgi with the states in the recurrence's coordinates; dW_ih and dX pair
             # it with the layer input, where the reverse half is left-aligned
@@ -766,25 +764,6 @@ def gru_stack(x, rnn, dropout=0.0, lens=None):
     ndir, weights = _gru_weights(rnn)
     return _batch_chunks(x, lens, lambda xc, lc: GRUStackFunction.apply(
         xc, ndir, rnn.hidden_size, float(dropout), None, None, lc, *weights))
-
-
-def _transpose_bf16(src, rows_pad=8, out=None):
-    """[R][C] bf16 -> [C][Rp] bf16 (Rp = R rounded up so that rows stay 16-byte aligned);
-    `out` (optional): a [C][>=R] bf16 destination with contiguous rows."""
-    lib = _lib.load()
-    R, C = src.shape
-    Rp = _round_up(R, rows_pad)
-    if out is not None:
-        dst = out
-    elif Rp != R:
-        dst = torch.zeros(C, Rp, dtype=torch.bfloat16, device=src.device)
-    else:
-        dst = torch.empty(C, Rp, dtype=torch.bfloat16, device=src.device)
-    sp = _lib.stream_ptr()
-    _launch("transpose_bf16", 0.0,
-            lambda: lib.sb_transpose_bf16(src.data_ptr(), dst.data_ptr(), R, C, src.stride(0),
-                                          dst.stride(0), sp))
-    return dst[:, :R]
 
 
 class ConvStackFunction(torch.autograd.Function):
@@ -927,48 +906,3 @@ def conv_stack(x, conv, training):
     for c in convs:
         params += [c.weight, c.bias]
     return ConvStackFunction.apply(x, specs, float(p_drop), *params)
-
-
-def beam_topk(scores, k):
-    """Top-k of a float64 CUDA score matrix in the reference's stable-sort order (score
-    descending, flat index ascending).  Returns (list of flat indices, list of scores)."""
-    _lib.require_cuda(scores, "scores")
-    lib = _lib.load()
-    sc = scores.detach().double().contiguous().reshape(-1)
-    n = sc.numel()
-    idx = torch.empty(k, dtype=torch.int32, device=sc.device)
-    val = torch.empty(k, dtype=torch.float64, device=sc.device)
-    sp = _lib.stream_ptr()
-    _launch("beam_topk", 0.0,
-            lambda: lib.sb_beam_topk(sc.data_ptr(), n, k, idx.data_ptr(), val.data_ptr(), sp))
-    return idx.cpu().tolist(), val.cpu().tolist()
-
-
-def attn_step(eh, dhx, ax_prev, conv, lin, log_t, lens=None):
-    """Fused NNAttention forward for the decode path (no autograd).  eh (B,T,H), dhx (B,1,H) or
-    (B,H), ax_prev (B,T) or None; conv = nn.Conv1d(1,H,Kc), lin = nn.Linear(H,1); lens (optional):
-    frames each utterance attends over (ax is 0 past them).
-    Returns (sx (B,1,H), ax (B,T)) like the reference module."""
-    _lib.require_cuda(eh, "eh")
-    lib = _lib.load()
-    eh = eh.detach().float().contiguous()
-    B, T, H = eh.shape
-    d = dhx.detach().float().reshape(B, H).contiguous()
-    axp = None if ax_prev is None else ax_prev.detach().float().contiguous()
-    cw = conv.weight.detach().float().reshape(H, -1).t().contiguous()     # (Kc, H)
-    Kc = cw.shape[0]
-    cb = conv.bias.detach().float().contiguous()
-    lw = lin.weight.detach().float().reshape(-1).contiguous()
-    lb = float(lin.bias.detach().float().item()) if lin.bias is not None else 0.0
-    sx = torch.empty(B, H, dtype=torch.float32, device=eh.device)
-    ax = torch.empty(B, T, dtype=torch.float32, device=eh.device)
-    sp = _lib.stream_ptr()
-    from .functions.s2s import attn_lens, attn_workspace
-    ws = attn_workspace(lib, B, T, H, eh.device)
-    ld = attn_lens(lens, B, T, eh.device)
-    _launch("attn_step", 0.0,
-            lambda: lib.sb_attn_step_len(eh.data_ptr(), d.data_ptr(), _lib.ptr(axp), cw.data_ptr(),
-                                         cb.data_ptr(), lw.data_ptr(), lb, 1 if log_t else 0, B, T,
-                                         H, Kc, sx.data_ptr(), ax.data_ptr(), _lib.ptr(ld),
-                                         ws.data_ptr(), ws.numel(), sp))
-    return sx.unsqueeze(1), ax

@@ -62,10 +62,8 @@ class FlatSGD:
         self.flat_g = torch.zeros(n, dtype=torch.float32, device=dev)
         self.mom = torch.zeros(n, dtype=torch.float32, device=dev) if self.momentum != 0 else None
         self.sumsq = torch.zeros(1, dtype=torch.float32, device=dev)
-        import ctypes
-        nb = ctypes.c_size_t(0)
-        _lib.check(_lib.load().sb_sumsq_workspace_size(ctypes.byref(nb)), "sumsq ws")
-        self.sumsq_ws = torch.zeros(nb.value, dtype=torch.uint8, device=dev)
+        nb = _lib.workspace_size(_lib.load().sb_sumsq_workspace_size)
+        self.sumsq_ws = torch.zeros(nb, dtype=torch.uint8, device=dev)
         self.spans = {}
         self.offs = {}
         for p, o in zip(self.params, offs):

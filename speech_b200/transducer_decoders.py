@@ -15,11 +15,9 @@ best non-blank classes, csrc/tdecode.cu), with the same results bit for bit: the
 selection the lists cannot prove, and flagged utterances are searched again from lists of
 SHORTLIST_RERUN entries.
 """
-import ctypes
-
 import torch
 
-from . import _lib
+from . import _lib, ops
 
 SHORTLIST_RERUN = 64      # list length of the second search of flagged utterances (the maximum)
 
@@ -40,7 +38,6 @@ def alloc_shortlists(B, T, U1, kp, device):
 
 def shortlists_of_lp(lp, kp, blank):
     """Shortlists of a given (B, T, U1, V) float32 CUDA log-probability tensor."""
-    from . import ops
     lib = _lib.load()
     B, T, U1, V = lp.shape
     val, idx, meta = alloc_shortlists(B, T, U1, kp, lp.device)
@@ -57,17 +54,15 @@ def shortlists_of_lp(lp, kp, blank):
 def _shortlist_search(sl, tl, ul, V, beam_size, blank):
     """One sb_rnnt_decode_static_shortlist launch over the shortlists sl of len(tl) utterances ->
     (label lists, log-probabilities, flag counts) on the host."""
-    from . import ops
     lib = _lib.load()
     val, idx, meta = sl
     B, T, U1, kp = val.shape
     dev = val.device
     lens = torch.tensor(list(tl) + list(ul), dtype=torch.int32).pin_memory().to(dev,
                                                                                 non_blocking=True)
-    nbytes = ctypes.c_size_t(0)
-    _lib.check(lib.sb_rnnt_decode_static_workspace_size(B, T, U1, int(beam_size),
-                                                        ctypes.byref(nbytes)), "ws")
-    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+    nbytes = _lib.workspace_size(lib.sb_rnnt_decode_static_workspace_size, B, T, U1,
+                                 int(beam_size))
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     labels = torch.empty(B, U1, dtype=torch.int32, device=dev)
     counts = torch.empty(2, B, dtype=torch.int32, device=dev)      # lengths, flags
     scores = torch.empty(B, dtype=torch.float64, device=dev)
@@ -78,7 +73,7 @@ def _shortlist_search(sl, tl, ul, V, beam_size, blank):
                         val.data_ptr(), idx.data_ptr(), meta.data_ptr(), kp, lens[:B].data_ptr(),
                         lens[B:].data_ptr(), B, T, U1, V, int(beam_size), int(blank),
                         labels.data_ptr(), counts[0].data_ptr(), scores.data_ptr(),
-                        counts[1].data_ptr(), ws.data_ptr(), nbytes.value, sp))
+                        counts[1].data_ptr(), ws.data_ptr(), nbytes, sp))
     lab = labels.cpu()
     n, flags = counts.cpu().tolist()
     return [lab[b, :n[b]].tolist() for b in range(B)], scores.cpu().tolist(), flags
@@ -111,7 +106,6 @@ def decode_static_shortlist(produce, tlens, ulens, V, beam_size, blank):
 def decode_static_batch(lp, tlens, ulens, beam_size, blank):
     """lp (B, T, U1, V) float32 CUDA log-probabilities; tlens / ulens: frames and lattice rows
     (labels + 1) of every utterance.  Returns (list of label lists, list of log-probabilities)."""
-    from . import ops
     _lib.require_cuda(lp, "lp")
     lib = _lib.load()
     lp = lp.detach().float().contiguous()
@@ -124,10 +118,9 @@ def decode_static_batch(lp, tlens, ulens, beam_size, blank):
             return shortlists_of_lp(lp if rows is None else lp[rows].contiguous(), kp, blank)
         return decode_static_shortlist(produce, tl, ul, V, beam_size, blank)
     lens = torch.tensor(tl + ul, dtype=torch.int32).pin_memory().to(dev, non_blocking=True)
-    nbytes = ctypes.c_size_t(0)
-    _lib.check(lib.sb_rnnt_decode_static_workspace_size(B, T, U1, int(beam_size),
-                                                        ctypes.byref(nbytes)), "ws")
-    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+    nbytes = _lib.workspace_size(lib.sb_rnnt_decode_static_workspace_size, B, T, U1,
+                                 int(beam_size))
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     labels = torch.empty(B, U1, dtype=torch.int32, device=dev)
     olens = torch.empty(B, dtype=torch.int32, device=dev)
     scores = torch.empty(B, dtype=torch.float64, device=dev)
@@ -139,7 +132,7 @@ def decode_static_batch(lp, tlens, ulens, beam_size, blank):
                                                       int(beam_size), int(blank),
                                                       labels.data_ptr(), olens.data_ptr(),
                                                       scores.data_ptr(), ws.data_ptr(),
-                                                      nbytes.value, sp))
+                                                      nbytes, sp))
     lab = labels.cpu()
     n = olens.cpu().tolist()
     sc = scores.cpu().tolist()

@@ -261,7 +261,7 @@ def test_transducer_infer_decodes_each_utterance_over_its_frames(cuda_lib):
 # ---- 6. masked attention ----------------------------------------------------------------------
 @pytest.mark.parametrize("log_t", [False, True])
 def test_masked_attention_decode_matches_oracle(cuda_lib, log_t):
-    """s2s.decode with lens (sb_s2s_attn_fwd_len / _bwd_len) on a padded batch against the masked
+    """s2s.decode with lens (sb_s2s_attn_fwd / _bwd) on a padded batch against the masked
     float64 restatement, which equals each utterance run alone (test_exact_lengths_host); bounds
     of test_teacher_forced_decode_forward_and_backward.  Padded frames get exactly zero
     alignment and zero gradient."""
@@ -305,7 +305,7 @@ def test_masked_attention_decode_matches_oracle(cuda_lib, log_t):
 
 @pytest.mark.parametrize("log_t", [False, True])
 def test_masked_attn_step_matches_each_utterance_alone(cuda_lib, log_t):
-    """NNAttention.forward with lens (sb_attn_step_len), first and later steps, against the
+    """NNAttention.forward with lens (sb_s2s_attn_fwd), first and later steps, against the
     unmasked kernel on each utterance alone; bound of test_attn_step_kernel_matches_reference_
     formulation."""
     from speech_b200.models.seq2seq import NNAttention

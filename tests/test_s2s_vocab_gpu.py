@@ -310,6 +310,42 @@ def test_split_selection_equals_single_cta_selection(cuda_lib, K, C, ties):
             assert torch.equal(a[key], b[key]), (step, key)
 
 
+@pytest.mark.parametrize("split", [False, True])
+def test_selection_breaks_ties_by_flat_index(cuda_lib, split):
+    """The reference's stable descending sort over (beam row, class) candidates: equal float64
+    scores keep ascending flat index r * C + c.  Integer logp make nearly every score a tie; no
+    end token is ever selected, so every step keeps the K best candidates."""
+    from speech_b200 import _lib
+    lib = _lib.load()
+    dev = torch.device("cuda")
+    K, C, max_len = 4, 6, 5
+    g = torch.Generator().manual_seed(7)
+    buf = _beam_buffers(lib, K, C, max_len, dev)
+    sp = _lib.stream_ptr()
+    _lib.check(lib.sb_s2s_beam_init(buf["state"].data_ptr(), buf["nodes"].data_ptr(),
+                                    buf["tok"].data_ptr(), 0, sp), "beam init")
+    n = ctypes.c_size_t(0)
+    lib.sb_s2s_beam_split_workspace_size(K, C, ctypes.byref(n))
+    ws = torch.empty(n.value, dtype=torch.uint8, device=dev)
+    scores = [0.0]
+    for step in range(max_len - 1):
+        lp = torch.randint(-2, 1, (K, C), generator=g).float()
+        lpd = lp.to(dev)
+        args = (lpd.data_ptr(), buf["state"].data_ptr(), buf["c_scores"].data_ptr(),
+                buf["nodes"].data_ptr(), buf["parent"].data_ptr(), buf["tok"].data_ptr(),
+                buf["out"].data_ptr(), K, C, C, step, max_len, buf["node_cap"], buf["c_cap"])
+        if split:
+            _lib.check(lib.sb_s2s_beam_select_split(*args, ws.data_ptr(), ws.numel(), sp), "split")
+        else:
+            _lib.check(lib.sb_s2s_beam_select(*args, sp), "select")
+        torch.cuda.synchronize()
+        cand = sorted(((scores[r] + float(lp[r, c]), r * C + c) for r in range(len(scores))
+                       for c in range(C)), key=lambda e: (-e[0], e[1]))[:K]
+        assert buf["parent"].tolist() == [i // C for _, i in cand], step
+        assert buf["tok"].tolist() == [i % C for _, i in cand], step
+        scores = [s for s, _ in cand]
+
+
 def test_public_class_end_to_end_at_4001_pieces(cuda_lib):
     from speech_b200.models import Seq2Seq
     torch.manual_seed(5)
