@@ -475,6 +475,54 @@ int sb_rnnt_decode_static_shortlist(const float* sl_val, const int* sl_idx, cons
                                     int* out_lens, double* out_scores, int* out_flags,
                                     void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * Label-free transducer beam search (csrc/rnnt_search.cu): the search above with the row of
+ * hypothesis h at frame t computed from h itself (prediction network run on h's labels) instead of
+ * read at lat[t, len(h)].  The caller's loop, per frame t and level l = 0 .. S
+ * (S = max_symbols_per_frame): rows of the level-l frontier, sb_rnnt_search_round, and for l < S
+ * the prediction states of the new frontier; then sb_rnnt_search_frame_end.  Once before:
+ * sb_rnnt_search_init; once after: sb_rnnt_search_final.  Each call is one launch, one CTA per
+ * utterance; utterances with t >= tlens[b] (or no live frontier) return at once.
+ *   workspace  >= sb_rnnt_search_workspace_size(B, T, S, beam_size) bytes =
+ *              1024 + 4096 + B * (1184 + 8 n + 12 c + 20 d) with n = T*S*K + 2 trie nodes,
+ *              c = the least power of two >= max(64, 2 n) map slots, d = K*(S+1) + 1 `done` entries
+ *   slot_lens  (B, K) int32: labels of the hypothesis in each slot of the frontier whose rows are
+ *              asked for next (what a static lattice needs to supply rows)
+ *   sb_rnnt_search_round: rows of the level's K frontier slots, either lp (B, K, V) f32 (needs
+ *              beam_size * V * 8 + 16 <= 200 KB, sb_rnnt_decode_static_fits) or, with lp NULL, the
+ *              shortlists (B, K, kp) / (B, K, 2) of sb_rnnt_shortlist_rows; writes par (B, K) the
+ *              parent slot of each new frontier slot (-2: none), sym (B, K) its symbol, slot_lens
+ *   sb_rnnt_search_frame_end: the K best of `done` become the beam; when hid / fy are not NULL it
+ *              gathers their prediction states into block `next` of the arenas hid [S+2][layers]
+ *              [B*K][H] and fy [S+2][B*K][Hj] (block l = level l's frontier, blocks cur / next =
+ *              0 / S+1 in turn = the beam)
+ *   sb_rnnt_search_final: out_labels (B, max_len), out_lens, out_scores (f64), out_flags (may be
+ *              NULL; shortlist selections the lists could not prove, as in
+ *              sb_rnnt_decode_static_shortlist)
+ * sb_rnnt_pred_step: one GRU layer (gates r, z, n; fp32 on CUDA cores) over R = B*K rows: input row
+ *   emb[sym[r]] (Kin = embedding width; sym[r] = -1 or sym NULL: zeros) or x[r] (Kin = H), hidden
+ *   state h_prev[(r / K) * K + par[r]] (par[r] = -1 or par NULL: zeros; -2: row skipped) -> h[r],
+ *   and bf16(h[r]) at y[r * ldy] if y is not NULL.  beam_size <= 32, kp <= 64.
+ * ------------------------------------------------------------------------------------- */
+int sb_rnnt_search_workspace_size(int B, int T, int S, int beam_size, size_t* bytes);
+int sb_rnnt_search_init(int* slot_lens, int B, int T, int S, int beam_size, void* workspace,
+                        size_t workspace_bytes, void* stream);
+int sb_rnnt_search_round(const float* lp, const float* sl_val, const int* sl_idx,
+                         const float* sl_meta, int kp, const int* tlens, int t, int level,
+                         int max_len, int* par, int* sym, int* slot_lens, int B, int T, int S,
+                         int V, int beam_size, int blank, void* workspace, size_t workspace_bytes,
+                         void* stream);
+int sb_rnnt_search_frame_end(const int* tlens, int t, int* slot_lens, float* hid, int layers,
+                             int H, float* fy, int Hj, int cur, int next, int B, int T, int S,
+                             int beam_size, void* workspace, size_t workspace_bytes, void* stream);
+int sb_rnnt_search_final(int* out_labels, int max_len, int* out_lens, double* out_scores,
+                         int* out_flags, int B, int T, int S, int beam_size, void* workspace,
+                         size_t workspace_bytes, void* stream);
+int sb_rnnt_pred_step(const float* emb, const int* sym, const float* x, const float* h_prev,
+                      const int* par, const float* w_ih, const float* w_hh, const float* b_ih,
+                      const float* b_hh, float* h, void* y_bf16, int ldy, int R, int K, int Kin,
+                      int H, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Scoring (SURVEY.md section 8f rank 4), HOST function: Levenshtein distance of two int32 token
  * sequences; replaces `editdistance.eval` in speech/utils/score.py:15-16.  Returns -1 on invalid

@@ -98,6 +98,19 @@ SIGNATURES = {
     "sb_rnnt_decode_static_shortlist": (_c_int, [_vp, _vp, _vp, _c_int, _vp, _vp, _c_int, _c_int,
                                                  _c_int, _c_int, _c_int, _c_int, _vp, _vp, _vp, _vp,
                                                  _vp, _c_sz, _vp]),
+    "sb_rnnt_search_workspace_size": (_c_int, [_c_int, _c_int, _c_int, _c_int,
+                                               ctypes.POINTER(_c_sz)]),
+    "sb_rnnt_search_init": (_c_int, [_vp, _c_int, _c_int, _c_int, _c_int, _vp, _c_sz, _vp]),
+    "sb_rnnt_search_round": (_c_int, [_vp, _vp, _vp, _vp, _c_int, _vp, _c_int, _c_int, _c_int, _vp,
+                                      _vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int, _c_int,
+                                      _vp, _c_sz, _vp]),
+    "sb_rnnt_search_frame_end": (_c_int, [_vp, _c_int, _vp, _vp, _c_int, _c_int, _vp, _c_int,
+                                          _c_int, _c_int, _c_int, _c_int, _c_int, _c_int, _vp,
+                                          _c_sz, _vp]),
+    "sb_rnnt_search_final": (_c_int, [_vp, _c_int, _vp, _vp, _vp, _c_int, _c_int, _c_int, _c_int,
+                                      _vp, _c_sz, _vp]),
+    "sb_rnnt_pred_step": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_int,
+                                   _c_int, _c_int, _c_int, _c_int, _vp]),
     "sb_debug_gru_timeline": (_c_int, [_vp]),
     "sb_debug_gru_cluster": (_c_int, [_c_int]),
     "sb_debug_gru_ksplit": (_c_int, [_c_int]),

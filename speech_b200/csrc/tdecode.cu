@@ -18,7 +18,8 @@
 //     beam = the beam_size best of done by (score desc, insertion order asc)
 //   result = beam[0] after the last frame.
 // Both selections and the trie of hypotheses (prefix merging compares node ids) are those of
-// beam.cuh.  Scores are float64, as Python floats.
+// beam.cuh; the rounds themselves are tsearch.cuh's, shared with the label-free search
+// (rnnt_search.cu).  Scores are float64, as Python floats.
 // Roofline: HBM-nominal (the lattice is read once); latency-bound by the T x U serial expansion.
 //
 // sb_rnnt_decode_static_shortlist: the same search from per-node shortlists instead of the full
@@ -47,7 +48,7 @@
 // one float64 sum, i.e. |fr_s| of roughly 2^29 times their gap, so real lattices never raise it.
 // A hypothesis takes at most K of its entries, so kp >= K lists are never exhausted while a
 // left-out class could still follow.
-#include "beam.cuh"
+#include "tsearch.cuh"
 #include <math.h>
 
 #include "../../include/speech_b200.h"
@@ -77,18 +78,6 @@ struct TdParams {
   int B, T, U1, V, K, kp, blank, done_cap;
 };
 
-SB_DEVINL double td_lse(double a, double b) {
-  const double m = fmax(a, b);
-  return m + log(exp(a - m) + exp(b - m));
-}
-
-// nextafterf(x, -inf) for finite x
-SB_DEVINL float td_next_down(float x) {
-  const int i = __float_as_int(x);
-  if (x == 0.f) return -__int_as_float(1);                 // -(smallest subnormal)
-  return __int_as_float(x > 0.f ? i - 1 : i + 1);
-}
-
 // the search of one utterance (blockIdx.x); SHORT: candidates from the shortlists
 template <bool SHORT>
 SB_DEVINL void td_search(const TdParams& p) {
@@ -100,8 +89,8 @@ SB_DEVINL void td_search(const TdParams& p) {
   __shared__ double beam_s[TD_MAX_BEAM], fr_s[TD_MAX_BEAM], new_s[TD_MAX_BEAM];
   __shared__ int beam_n[TD_MAX_BEAM], beam_l[TD_MAX_BEAM];
   __shared__ int fr_n[TD_MAX_BEAM], fr_l[TD_MAX_BEAM];
-  __shared__ int new_n[TD_MAX_BEAM], new_l[TD_MAX_BEAM];
-  __shared__ int nbeam, nfr, ndone, found, round_id, nsel_s, nflag;
+  __shared__ int new_n[TD_MAX_BEAM], new_l[TD_MAX_BEAM], new_p[TD_MAX_BEAM], new_k[TD_MAX_BEAM];
+  __shared__ int nbeam, nfr, ndone, round_id, nflag;
 
   const BeamTrie trie = p.trie.of(b);
   double* dscore = p.done_score + (size_t)b * p.done_cap;
@@ -109,6 +98,7 @@ SB_DEVINL void td_search(const TdParams& p) {
   int* dlen = p.done_len + (size_t)b * p.done_cap;
   const float* lp = SHORT ? nullptr : p.lp + (size_t)b * p.T * p.U1 * V;
   const size_t node0 = (size_t)b * p.T * p.U1;             // batch-first node of (b, 0, 0)
+  const TsNew nw{new_s, new_n, new_l, new_p, new_k};
 
   if (tid == 0) {
     nbeam = 1; beam_s[0] = 0.0; beam_n[0] = 0; beam_l[0] = 0;
@@ -124,136 +114,40 @@ SB_DEVINL void td_search(const TdParams& p) {
     for (int level = 0; level < U; ++level) {
       // ---- 1. blank emissions into `done`, hypothesis by hypothesis (merging order matters) ----
       const int nf = nfr;
-      for (int i = 0; i < nf; ++i) {
-        const int u = fr_l[i];
-        if (u >= U) continue;                       // (uniform: shared data)
-        if (tid == 0) found = -1;
-        __syncthreads();
-        const int nd = ndone, me = fr_n[i];
-        for (int j = tid; j < nd; j += TD_THREADS)
-          if (dnode[j] == me) found = j;            // at most one entry holds this hypothesis
-        __syncthreads();
-        if (tid == 0) {
-          const size_t node = (size_t)t * p.U1 + u;
-          const float blp = SHORT ? p.sl_meta[2 * (node0 + node)] : lp[node * V + p.blank];
-          const double bsc = fr_s[i] + (double)blp;
-          if (found >= 0) dscore[found] = td_lse(dscore[found], bsc);
-          else if (nd < p.done_cap) { dscore[nd] = bsc; dnode[nd] = me; dlen[nd] = u; ndone = nd + 1; }
-        }
-        __syncthreads();
-      }
+      ts_merge_blanks<TD_THREADS>(
+          nf, fr_s, fr_n, fr_l, U,
+          [&](int, int u) {
+            const size_t node = (size_t)t * p.U1 + u;
+            return SHORT ? p.sl_meta[2 * (node0 + node)] : lp[node * V + p.blank];
+          },
+          dscore, dnode, dlen, nullptr, 0, &ndone, p.done_cap);
       // ---- 2. label expansions: candidates (i, k), the K best form the next frontier ----
-      int nsel = 0;
+      const auto can_extend = [&](int i) { return fr_l[i] + 1 < U; };
+      int nsel;
       if (!SHORT) {
-        bool any = false;
-        for (int c = tid; c < K * V; c += TD_THREADS) {
-          const int i = c / V, k = c - i * V;
-          double sc = nan("");
-          if (i < nf && k != p.blank && fr_l[i] + 1 < U) {
-            sc = fr_s[i] + (double)lp[((size_t)t * p.U1 + fr_l[i]) * V + k];
-            any = true;
-          }
-          cand[c] = sc;
-        }
-        const int have = __syncthreads_or(any ? 1 : 0);
-        if (!have) break;
-        for (int r = 0; r < K; ++r) {
-          double sc;
-          const int c = beam_take_first<TD_THREADS>(cand, K * V, sc);
-          if (c < 0) break;
-          if (tid == 0) {
-            const int i = c / V, k = c - i * V;
-            new_s[nsel] = sc;
-            new_n[nsel] = trie.find_or_insert<false>(fr_n[i], k, 1 + round_id * K + nsel);
-            new_l[nsel] = fr_l[i] + 1;
-          }
-          ++nsel;
-        }
-        __syncthreads();                            // thread 0 has read fr_* and written new_*
+        nsel = ts_expand_full<TD_THREADS>(
+            cand, K, V, p.blank, nf, fr_s, fr_n, fr_l, can_extend,
+            [&](int i, int k) { return lp[((size_t)t * p.U1 + fr_l[i]) * V + k]; }, trie,
+            round_id, nw);
       } else {
-        // K-way merge of the frontier's shortlists, one lane per hypothesis (warp 0)
-        bool live = false;
-        if (tid < 32) {
-          const int i = tid;
-          live = i < nf && fr_l[i] + 1 < U && V > 1;
-          const double fs = live ? fr_s[i] : 0.0;
-          const bool all_tie = live && fs == -INFINITY;
-          const int n = min(p.kp, V - 1);
-          const float* lv = nullptr;
-          const int* li = nullptr;
-          float beta = -INFINITY;
-          if (live && !all_tie) {
-            const size_t node = node0 + (size_t)t * p.U1 + fr_l[i];
-            lv = p.sl_val + node * p.kp;
-            li = p.sl_idx + node * p.kp;
-            beta = p.sl_meta[2 * node + 1];
-          }
-          const unsigned long long inlist = n >= 64 ? ~0ull : (1ull << n) - 1ull;
-          unsigned long long used = 0ull;
-          int taken = 0, nfl = 0, ns = 0;
-          const bool have = __any_sync(0xffffffffu, live);
-          for (int r = 0; r < K && have; ++r) {
-            bool hv = false;
-            double hs = 0.0;
-            int hk = -1, hq = -1;
-            if (all_tie) {
-              if (taken < V - 1) { hv = true; hs = -INFINITY; hk = taken < p.blank ? taken : taken + 1; }
-            } else if (live) {
-              const unsigned long long fr = ~used & inlist;
-              if (fr) {
-                hq = __ffsll((long long)fr) - 1;
-                hk = li[hq];
-                hs = fs + (double)lv[hq];
-                hv = true;
-                for (int q = hq + 1; q < n && fs + (double)lv[q] == hs; ++q)
-                  if (!((used >> q) & 1ull) && li[q] < hk) { hk = li[q]; hq = q; }
-              }
-            }
-            double bs = hs;
-            int bi = hv ? i : -1;
-            beam_warp_first(bs, bi);
-            if (bi < 0) break;
-            const int k = __shfl_sync(0xffffffffu, hk, bi);
-            if (i == bi) {
-              if (all_tie) {
-                ++taken;
-              } else {
-                used |= 1ull << hq;
-                const float x = lv[hq];
-                if (fs + (double)beta == hs &&
-                    (x != beta ||
-                     (beta != -INFINITY && fs + (double)td_next_down(beta) == hs)))
-                  ++nfl;
-              }
-            }
-            if (i == 0) {
-              new_s[ns] = bs;
-              new_n[ns] = trie.find_or_insert<false>(fr_n[bi], k, 1 + round_id * K + ns);
-              new_l[ns] = fr_l[bi] + 1;
-            }
-            ++ns;
-            __syncwarp();
-          }
-          nfl = __reduce_add_sync(0xffffffffu, nfl);
-          if (i == 0) { nsel_s = ns; nflag += nfl; }
-        }
-        if (!__syncthreads_or(live ? 1 : 0)) break;
-        nsel = nsel_s;
+        nsel = ts_expand_shortlist(
+            K, V, p.kp, p.blank, nf, fr_s, fr_n, fr_l, can_extend,
+            [&](int i, const float** lv, const int** li, float* beta) {
+              const size_t node = node0 + (size_t)t * p.U1 + fr_l[i];
+              *lv = p.sl_val + node * p.kp;
+              *li = p.sl_idx + node * p.kp;
+              *beta = p.sl_meta[2 * node + 1];
+            },
+            trie, round_id, nw, &nflag);
       }
+      if (nsel < 0) break;
       if (tid < nsel) { fr_s[tid] = new_s[tid]; fr_n[tid] = new_n[tid]; fr_l[tid] = new_l[tid]; }
       if (tid == 0) { nfr = nsel; ++round_id; }
       __syncthreads();
     }
     // ---- 3. beam = the K best of `done` ----
-    const int nd = ndone;
-    int nb = 0;
-    for (int r = 0; r < K; ++r) {
-      double sc;
-      const int j = beam_take_first<TD_THREADS>(dscore, nd, sc);
-      if (j < 0) break;
-      if (tid == 0) { beam_s[nb] = sc; beam_n[nb] = dnode[j]; beam_l[nb] = dlen[j]; }
-      ++nb;
-    }
+    const int nb = ts_select_done<TD_THREADS>(dscore, dnode, dlen, nullptr, ndone, K, beam_s,
+                                              beam_n, beam_l, nullptr);
     if (tid == 0) nbeam = nb;
     __syncthreads();
   }

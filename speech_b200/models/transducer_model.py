@@ -16,7 +16,9 @@ import torch.nn as nn
 from . import model
 from .. import ops
 from ..functions import transducer as transducer_fn
-from ..transducer_decoders import decode_static_batch, decode_static_fits, decode_static_shortlist
+from .. import _lib
+from ..transducer_decoders import (decode_static_batch, decode_static_fits, decode_static_shortlist,
+                                   search_batch)
 
 
 class Transducer(model.Model):
@@ -143,5 +145,134 @@ class Transducer(model.Model):
         preds, _ = decode_static_shortlist(produce, tlens, ulens, V1, beam_size, self.blank)
         return preds
 
+    def recognize(self, inputs, beam_size=4, max_symbols_per_frame=4, max_len=None,
+                  return_scores=False):
+        """Beam search from the audio alone: `infer`'s search with the row of each hypothesis
+        computed by the prediction network reading the hypothesis's own labels (dropout off),
+        instead of the reference transcript.  inputs: the (T_i, F) arrays of batch[0].  A frame
+        emits at most max_symbols_per_frame labels; a hypothesis with max_len labels (default: no
+        cap beyond frames * max_symbols_per_frame) is not extended.  Frames searched: the padded T'
+        for every utterance, or its own conv_out_size(T_b) in the exact-lengths mode.
+        Returns the label lists (and their float64 log-probabilities with return_scores)."""
+        rows = PredictionRows(self, inputs)
+        labels, scores = search_batch(rows, rows.tlens, beam_size, self.blank,
+                                      max_symbols_per_frame, max_len)
+        return (labels, scores) if return_scores else labels
+
     def label_collate(self, labels):
         return torch.from_numpy(model.end_pad_labels(labels))
+
+
+class PredictionRows:
+    """Row provider of transducer_decoders.search_batch for a Transducer on a batch of inputs: the
+    encoder's fc1 outputs once (time-major, frame t = a contiguous (B, Hj) block), then per level
+    one sb_rnnt_pred_step per prediction-network layer and fc1 of the new states (the wgmma GEMM,
+    bf16 operands: the arithmetic of ops.linear with joint_inputs' padded weights) into an arena of
+    per-slot states, and the joint rows at frame t with `forward`'s kernels (fused at T = 1,
+    U1 = K where fc2 is resident, else one slab of the large-vocabulary joint)."""
+
+    def __init__(self, model, inputs):
+        with torch.no_grad():
+            x = model.stage_inputs(inputs)
+            if model.exact_lengths:
+                tl = [max(0, model.conv_out_size(i.shape[0], 0)) for i in inputs]
+                enc = model._encode(x, torch.tensor(tl, dtype=torch.int32))
+            else:
+                enc = model._encode(x, None)
+            fc1 = model.fc1.fc
+            H = fc1.out_features
+            Hj = (H + 7) // 8 * 8
+            w1 = ops.pad_blocks(fc1.weight.detach(), 0, 1, H, Hj)
+            b1 = ops.pad_blocks(fc1.bias.detach(), 0, 1, H, Hj).float().contiguous()
+            fx = model.fc1(enc) if Hj == H else ops.linear(enc, w1, b1)
+        self.model = model
+        self.B, self.T = fx.shape[0], fx.shape[1]
+        self.tlens = tl if model.exact_lengths else [self.T] * self.B
+        self.device = fx.device
+        self.fxT = fx.detach().float().transpose(0, 1).contiguous()        # (T', B, Hj)
+        self.H, self.Hj, self.Hp = H, Hj, (H + 7) // 8 * 8
+        self.w1 = torch.nn.functional.pad(w1.to(torch.bfloat16), (0, self.Hp - H)).contiguous()
+        self.b1 = b1
+        fc2 = model.fc2.fc
+        self.V1 = fc2.out_features
+        self.w2 = ops.pad_blocks(fc2.weight.detach().to(torch.bfloat16), 1, 1, H, Hj).contiguous()
+        self.b2 = fc2.bias.detach().float().contiguous()
+        self.slabs = transducer_fn.joint_uses_slabs(Hj, self.V1)
+        rnn = model.dec_rnn
+        self.layers = rnn.num_layers
+        self.emb = model.embedding.weight.detach().float().contiguous()
+        self.gru = [tuple(getattr(rnn, "%s_l%d" % (n, l)).detach().float().contiguous()
+                          for n in ("weight_ih", "weight_hh", "bias_ih", "bias_hh"))
+                    for l in range(self.layers)]
+
+    def begin(self, slots):
+        B, K, S, dev = self.B, slots.K, slots.S, self.device
+        R = B * K
+        self.K = K
+        self.hid = torch.zeros(S + 2, self.layers, R, self.H, dtype=torch.float32, device=dev)
+        self.fy = torch.zeros(S + 2, R, self.Hj, dtype=torch.float32, device=dev)
+        self.ybf = torch.zeros(R, self.Hp, dtype=torch.bfloat16, device=dev)
+        self.ym = torch.zeros(R + 1, dtype=torch.int32, device=dev)
+        self.lat = torch.empty(R, 2, dtype=torch.float32, device=dev)
+        if self.slabs:
+            self.ld = (self.V1 + 7) // 8 * 8
+            self.z = torch.empty(R, self.Hj, dtype=torch.bfloat16, device=dev)
+            self.logits = torch.empty(R, self.ld, dtype=torch.float32, device=dev)
+            self.lse = torch.empty(R, dtype=torch.float32, device=dev)
+        self._step(None, 0, None, None)                  # the empty hypothesis, into block 0
+
+    def _step(self, src, dst, par, sym):
+        """states of block dst's rows: GRU layers from block src's states at slots par, inputs
+        emb[sym] (None: the zero start vector / zero state), then fc1"""
+        lib = _lib.load()
+        R, H = self.B * self.K, self.H
+        sp = _lib.stream_ptr()
+        E = self.emb.shape[1]
+        for l, (w_ih, w_hh, b_ih, b_hh) in enumerate(self.gru):
+            x = None if l == 0 else self.hid[dst, l - 1]
+            h_prev = None if src is None else self.hid[src, l]
+            y = self.ybf if l == self.layers - 1 else None
+            ops._launch("rnnt_pred_step", 6.0 * R * H * (H + (E if l == 0 else H)),
+                        lambda: lib.sb_rnnt_pred_step(
+                            self.emb.data_ptr() if l == 0 else None,
+                            _lib.ptr(sym) if l == 0 else None, _lib.ptr(x), _lib.ptr(h_prev),
+                            _lib.ptr(par), w_ih.data_ptr(), w_hh.data_ptr(), b_ih.data_ptr(),
+                            b_hh.data_ptr(), self.hid[dst, l].data_ptr(), _lib.ptr(y), self.Hp,
+                            R, self.K, E if l == 0 else H, H, sp))
+        ops.gemm_bf16_tn(self.ybf, self.w1, out=self.fy[dst], bias=self.b1)
+
+    def extend(self, src, dst, slots):
+        self._step(src, dst, slots.par, slots.sym)
+
+    def rows(self, t, block, slots):
+        lib = _lib.load()
+        B, K, Hj, V1 = self.B, self.K, self.Hj, self.V1
+        blank = self.model.blank
+        fx, fy = self.fxT[t], self.fy[block]
+        sp = _lib.stream_ptr()
+        if not self.slabs:
+            ops._launch("rnnt_joint", 2.0 * B * K * Hj * V1,
+                        lambda: lib.sb_rnnt_joint_fwd(fx.data_ptr(), fy.data_ptr(),
+                                                      self.w2.data_ptr(), self.b2.data_ptr(),
+                                                      self.ym.data_ptr(), self.lat.data_ptr(),
+                                                      slots.lp.data_ptr(), B, 1, K, Hj, V1,
+                                                      blank, sp))
+            return
+        ops._launch("rnnt_joint_slab", 0.0,
+                    lambda: lib.sb_rnnt_joint_build_slab(fx.data_ptr(), fy.data_ptr(),
+                                                         self.z.data_ptr(), B, 1, K, Hj, 0, 1, sp))
+        ops.gemm_bf16_tn(self.z, self.w2, out=self.logits, bias=self.b2)
+        ops._launch("rnnt_joint_rows", 0.0,
+                    lambda: lib.sb_rnnt_joint_vocab_fwd_rows(
+                        self.logits.data_ptr(), self.ld, self.ym.data_ptr(), self.lat.data_ptr(),
+                        self.lse.data_ptr(), _lib.ptr(slots.lp), B, 1, K, V1, blank, 0, 1, sp))
+        if slots.sl is not None:
+            val, idx, meta = slots.sl
+            ops._launch("rnnt_shortlist_rows", 0.0,
+                        lambda: lib.sb_rnnt_shortlist_rows(
+                            self.logits.data_ptr(), self.ld, self.lse.data_ptr(), B, 1, K, V1,
+                            blank, slots.kp, 0, 1, 1, val.data_ptr(), idx.data_ptr(),
+                            meta.data_ptr(), sp))
+
+    def arenas(self):
+        return self.hid, self.layers, self.H, self.fy, self.Hj

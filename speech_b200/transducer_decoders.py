@@ -148,3 +148,107 @@ def decode_static(lp, beam_size, blank=0):
     T, U, V = lp.shape
     labels, scores = decode_static_batch(lp.unsqueeze(0), [T], [U], beam_size, blank)
     return labels[0], scores[0]
+
+
+# ------------------------------------------------------------------------------------------------
+# Label-free search (csrc/rnnt_search.cu): decode_static's search with the row of hypothesis h at
+# frame t computed from h itself.  A row provider supplies the rows; Transducer.recognize passes the
+# prediction and joint networks (models/transducer_model.PredictionRows), tests pass a static
+# lattice.  Its CPU restatement is oracle/rnnt_search_ref.py.
+# ------------------------------------------------------------------------------------------------
+class SearchSlots:
+    """Device tensors of one search that a row provider reads: B, K, S, T, kp (None: full rows);
+    par / sym / slot_lens (B, K) int32 (csrc/rnnt_search.cu), lp (B, K, V1) f32 or sl (the
+    shortlists, alloc_shortlists(B, 1, K, kp)) that rows() fills."""
+
+    def __init__(self, B, K, S, T, V1, kp, dev):
+        self.B, self.K, self.S, self.T, self.kp = B, K, S, T, kp
+        self.par, self.sym, self.slot_lens = torch.zeros(3, B, K, dtype=torch.int32, device=dev)
+        self.lp = torch.empty(B, K, V1, dtype=torch.float32, device=dev) if kp is None else None
+        self.sl = None if kp is None else alloc_shortlists(B, 1, K, kp, dev)
+
+
+def _search_once(provider, tl, T, K, S, max_len, L, blank, kp):
+    lib = _lib.load()
+    B, V1, dev = provider.B, provider.V1, provider.device
+    slots = SearchSlots(B, K, S, T, V1, kp, dev)
+    nbytes = _lib.workspace_size(lib.sb_rnnt_search_workspace_size, B, T, S, K)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    tl_dev = torch.tensor(tl, dtype=torch.int32).pin_memory().to(dev, non_blocking=True)
+    # results: labels (B, L) | lengths (B) | flags (B) | scores (B) f64, one device->host copy
+    n_int = B * (L + 2)
+    n_int += n_int % 2
+    out = torch.zeros(n_int + 2 * B, dtype=torch.int32, device=dev)
+    labels, lens, flags = out[:B * L], out[B * L:B * L + B], out[B * L + B:B * L + 2 * B]
+    scores = out[n_int:].view(torch.float64)
+    sl = slots.sl
+    with torch.cuda.device(dev):
+        sp = _lib.stream_ptr()
+        provider.begin(slots)
+        ops._launch("rnnt_search", 0.0, lambda: lib.sb_rnnt_search_init(
+            slots.slot_lens.data_ptr(), B, T, S, K, ws.data_ptr(), nbytes, sp))
+        cur = 0
+        for t in range(T):
+            for level in range(S + 1):
+                block = cur if level == 0 else level
+                provider.rows(t, block, slots)
+                ops._launch("rnnt_search", 0.0, lambda: lib.sb_rnnt_search_round(
+                    _lib.ptr(slots.lp), *(_lib.ptr(a) for a in (sl or (None,) * 3)), kp or 0,
+                    tl_dev.data_ptr(), t, level, max_len, slots.par.data_ptr(),
+                    slots.sym.data_ptr(), slots.slot_lens.data_ptr(), B, T, S, V1, K, blank,
+                    ws.data_ptr(), nbytes, sp))
+                if level < S:
+                    provider.extend(block, level + 1, slots)
+            hid, layers, H, fy, Hj = provider.arenas()
+            ops._launch("rnnt_search", 0.0, lambda: lib.sb_rnnt_search_frame_end(
+                tl_dev.data_ptr(), t, slots.slot_lens.data_ptr(), _lib.ptr(hid), layers, H,
+                _lib.ptr(fy), Hj, cur, S + 1 - cur, B, T, S, K, ws.data_ptr(), nbytes, sp))
+            cur = S + 1 - cur
+        ops._launch("rnnt_search", 0.0, lambda: lib.sb_rnnt_search_final(
+            labels.data_ptr(), L, lens.data_ptr(), scores.data_ptr(), flags.data_ptr(), B, T, S,
+            K, ws.data_ptr(), nbytes, sp))
+    host = out.cpu()
+    lab = host[:B * L].view(B, L)
+    n = host[B * L:B * L + B].tolist()
+    fl = host[B * L + B:B * L + 2 * B].tolist()
+    sc = host[n_int:].view(torch.float64).tolist()
+    return [lab[b, :n[b]].tolist() for b in range(B)], sc, fl
+
+
+def search_batch(provider, tlens, beam_size, blank, max_symbols_per_frame, max_len=None):
+    """Label-free beam search of a batch.  provider: B, T (frames available), V1, device, and
+    begin(slots) (states of the empty hypothesis in block 0), rows(t, block, slots) (rows of the K
+    frontier slots of `block` at frame t into slots.lp or slots.sl), extend(src, dst, slots) (states
+    of the new frontier, slots.par / slots.sym, in block dst from block src), arenas() -> (hid,
+    layers, H, fy, Hj) (None, 0, 0, None, 0 without states).  tlens: frames searched per utterance
+    (clamped to T).  A frame emits at most max_symbols_per_frame labels; a hypothesis with max_len
+    labels (default: frames * max_symbols_per_frame) is not extended.  Rows through shortlists
+    where the full candidate list does not fit (decode_static_fits), with decode_static_shortlist's
+    rerun of flagged utterances from SHORTLIST_RERUN-entry lists (the whole batch, so that every row
+    is computed as in the first pass).  Returns (list of label lists, list of float64 scores)."""
+    B, T, V1 = provider.B, provider.T, provider.V1
+    K, S = int(beam_size), int(max_symbols_per_frame)
+    if K <= 0 or S <= 0:
+        raise ValueError("beam_size and max_symbols_per_frame must be positive")
+    tl = [max(0, min(int(t), T)) for t in tlens]
+    if len(tl) != B:
+        raise ValueError("tlens must have one entry per utterance")
+    if T == 0:
+        return [[] for _ in range(B)], [0.0] * B
+    cap = T * S if max_len is None else min(int(max_len), T * S)
+    L = max(1, cap)
+    if decode_static_fits(K, V1):
+        labels, scores, _ = _search_once(provider, tl, T, K, S, cap, L, blank, None)
+        return labels, scores
+    labels, scores, flags = _search_once(provider, tl, T, K, S, cap, L, blank, K)
+    rerun = [b for b, f in enumerate(flags) if f]
+    if rerun:
+        lab2, sc2, fl2 = _search_once(provider, tl, T, K, S, cap, L, blank, SHORTLIST_RERUN)
+        bad = [b for b in rerun if fl2[b]]
+        if bad:
+            raise _lib.SpeechB200Error(
+                "speech_b200: the shortlist beam search cannot order tied candidates of "
+                "utterance(s) %s even from %d-entry lists" % (bad, SHORTLIST_RERUN))
+        for b in rerun:
+            labels[b], scores[b] = lab2[b], sc2[b]
+    return labels, scores

@@ -164,3 +164,9 @@ from test_rnnt_shortlist_host import tie_lattice          # the lattice the test
 tie, blank = tie_lattice()
 print("rnnt shortlist rerun ok", decode_static(tie, 2, blank))
 torch.cuda.synchronize()
+# label-free search (csrc/rnnt_search.cu): prediction step, rounds, frame ends, final backtrack;
+# full candidate lists at V+1 = 29, shortlists at V+1 = 301 (beam 32) and 20001
+for tm, V1, beam in ((t, 29, 4), (t2, 301, 32), (tv, 20001, 4)):
+    tm.set_eval()
+    print("recognize V+1=%d beam %d" % (V1, beam),
+          [len(p) for p in tm.recognize(inputs[:3], beam_size=beam, max_symbols_per_frame=2)])
