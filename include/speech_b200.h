@@ -247,8 +247,9 @@ int sb_sgd_clip_step(float* params, const float* grads, float* momentum_buf, voi
  *           beam_search (:180-227).
  *   sb_s2s_cell_fwd   ix = emb[tok[b*tok_stride]] + sx_prev (NULL at the first step);
  *                     hx = GRUCell(ix, hx_prev); optionally saves ix and the gates (r, z, n, hn)
- *   sb_s2s_attn_fwd   attention of every row over eh (eh_bcast: all rows attend over utterance
- *                     0 - beam search), sx (B,H) / ax (B,T); with fc_w: logits = fc(hx + sx) written
+ *   sb_s2s_attn_fwd   attention of every row over eh: row b attends over utterance b / eh_group
+ *                     (1: its own; the beam search passes K, its rows per utterance), sx (B,H) /
+ *                     ax (B,T); with fc_w: logits = fc(hx + sx) written
  *                     at logits[b*logit_stride + c], optional log-softmax, arg-max, greedy history
  *                     and end-token count; `done` (device int, may be NULL): != 0 -> no-op.
  *                     Without fc_w: the attention alone (NNAttention.forward on the decode path)
@@ -264,7 +265,7 @@ int sb_sgd_clip_step(float* params, const float* grads, float* momentum_buf, voi
  * workspace: >= sb_s2s_workspace_size(B, T, H) bytes, its first 4*B bytes ZERO before the first
  * call (ticket counters; the kernels leave them zero); one workspace serves all steps.
  * Constraints: H % 4 == 0 (attention backward: H <= 1664, its shared-memory tile is 33 H floats),
- * conv kernel width odd and <= 15, T <= 6144, beam <= 32.
+ * conv kernel width odd and <= 15, T <= 6144, beam <= 32, beam batch B <= 65535.
  * Exact lengths: `lens` (B) int32 on the device gives the frames row b attends over (clamped to
  * [1, T]; NULL = all T).  Frames t >= lens[b] are left out of the softmax, so a_t = 0 exactly
  * there, and out of the location conv's input; log_t scales by log(lens[b]); d eh stays untouched
@@ -275,7 +276,7 @@ int sb_s2s_cell_fwd(const float* emb, const int* tok, int tok_stride, const floa
                     const float* hx_prev, const float* w_ih, const float* w_hh, const float* b_ih,
                     const float* b_hh, float* hx, float* ix_save, float* gates_save,
                     const int* done, int B, int H, void* stream);
-int sb_s2s_attn_fwd(const float* eh, int eh_bcast, const float* hx, const float* ax_prev,
+int sb_s2s_attn_fwd(const float* eh, int eh_group, const float* hx, const float* ax_prev,
                     const float* conv_wT, const float* conv_b, const float* lin_w, float lin_b,
                     int log_t, int B, int T, int H, int Kc, float* sx, float* ax,
                     const float* fc_w, const float* fc_b, int C, float* logits,
@@ -296,9 +297,18 @@ int sb_s2s_cell_bwd(const float* d_gi, const float* d_gh, const float* d_hx_dire
                     const float* w_ihT, const float* w_hhT, float* d_ix, float* d_hx_prev, int B,
                     int H, void* stream);
 int sb_s2s_check_done(const int* end_count, int B, int* done, int* nsteps, int step1, void* stream);
-/* The beam state is opaque but for two int32 fields the host reads in place: `done` at byte 0
- * (nonzero once the search has stopped; it doubles as the `done` flag of the step kernels) and
- * the length of the final hypothesis in out_tokens at byte 4. */
+/* The beam state is opaque but for the fields the host reads in place: `done` (int32) at byte 0
+ * (0 while the search runs, then the number of steps it ran; for one utterance it doubles as the
+ * `done` flag of the step kernels), the length of the final hypothesis in out_tokens (int32) at byte 4, and its
+ * float64 score in the last 8 bytes of the state.
+ * Batched forms (*_batch): B utterances searched at once, each exactly as it would be alone.
+ * States [B], nodes [B][node_cap][2], c_scores [B][c_cap], out_tokens [B][max_len + 2] sit back
+ * to back; logp, parent_row and tok_next have B*K rows, utterance b's are b*K .. b*K+K-1, and
+ * parent_row holds rows within the utterance.  `stop` (device int32[2], zeroed by the init):
+ * stop[0] counts the utterances that have stopped, stop[1] becomes 1 when the last one does - the
+ * `done` flag of the batch's step kernels.  Rows of stopped utterances are still computed by the
+ * step kernels until then; the select and gather of a stopped utterance do nothing.  The
+ * single-utterance entry points are the batched ones at B = 1 without `stop`. */
 int sb_s2s_beam_state_size(size_t* bytes);
 int sb_s2s_beam_init(void* state, int* nodes, int* tok_next, int start_tok, void* stream);
 int sb_s2s_beam_select(const float* logp, void* state, double* c_scores, int* nodes,
@@ -307,6 +317,15 @@ int sb_s2s_beam_select(const float* logp, void* state, double* c_scores, int* no
 int sb_s2s_beam_gather(const float* hx_in, const float* sx_in, const float* ax_in, float* hx_out,
                        float* sx_out, float* ax_out, const int* parent_row, const void* state,
                        int K, int H, int T, void* stream);
+int sb_s2s_beam_init_batch(void* state, int* nodes, int node_cap, int* tok_next, int K,
+                           int start_tok, int* stop, int B, void* stream);
+int sb_s2s_beam_select_batch(const float* logp, void* state, double* c_scores, int* nodes,
+                             int* parent_row, int* tok_next, int* out_tokens, int K, int C,
+                             int end_tok, int step, int max_len, int node_cap, int c_cap,
+                             int* stop, int B, void* stream);
+int sb_s2s_beam_gather_batch(const float* hx_in, const float* sx_in, const float* ax_in,
+                             float* hx_out, float* sx_out, float* ax_out, const int* parent_row,
+                             const void* state, int K, int H, int T, int B, void* stream);
 
 /* Large vocabularies (csrc/s2s_vocab.cu, csrc/s2s.cu).  sb_s2s_attn_fwd runs the output projection
  * in the utterance's last CTA, which holds every logit in shared memory: it takes fc_w only where
@@ -327,7 +346,8 @@ int sb_s2s_beam_gather(const float* hx_in, const float* sx_in, const float* ax_i
  * sb_s2s_beam_select_fits(K, C) is 1 where it runs (K <= 32, K*C*8 <= 200 KB).  Otherwise
  *   sb_s2s_beam_select_split  the same selection and bookkeeping (same state, outputs and tie
  *                     order) in two stages: per-tile top 2K candidates over many CTAs, then one
- *                     CTA merges the tiles' lists; workspace >= sb_s2s_beam_split_workspace_size.
+ *                     CTA merges the tiles' lists; workspace >= sb_s2s_beam_split_workspace_size
+ *                     (batched: sb_s2s_beam_split_workspace_size_batch, B times as many bytes).
  * Backward of the projection where sb_s2s_dout does not run (C > 8192): d_o = dlogits W_fc as a
  * 3-pass split-bf16 sb_gemm_bf16_tn with SB_GEMM_B_MN (the host mirror, functions/s2s.py). */
 int sb_s2s_fc_fused(int H, int C);
@@ -346,6 +366,12 @@ int sb_s2s_beam_select_split(const float* logp, void* state, double* c_scores, i
                              int* parent_row, int* tok_next, int* out_tokens, int K, int C,
                              int end_tok, int step, int max_len, int node_cap, int c_cap,
                              void* workspace, size_t workspace_bytes, void* stream);
+int sb_s2s_beam_split_workspace_size_batch(int K, int C, int B, size_t* bytes);
+int sb_s2s_beam_select_split_batch(const float* logp, void* state, double* c_scores, int* nodes,
+                                   int* parent_row, int* tok_next, int* out_tokens, int K, int C,
+                                   int end_tok, int step, int max_len, int node_cap, int c_cap,
+                                   int* stop, int B, void* workspace, size_t workspace_bytes,
+                                   void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * RNN-Transducer loss + gradient w.r.t. the log-probabilities.

@@ -59,6 +59,12 @@ SIGNATURES = {
                                     _c_int, _c_int, _c_int, _c_int, _vp]),
     "sb_s2s_beam_gather": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_int, _c_int, _c_int,
                                     _vp]),
+    "sb_s2s_beam_init_batch": (_c_int, [_vp, _vp, _c_int, _vp, _c_int, _c_int, _vp, _c_int, _vp]),
+    "sb_s2s_beam_select_batch": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_int, _c_int,
+                                          _c_int, _c_int, _c_int, _c_int, _c_int, _vp, _c_int,
+                                          _vp]),
+    "sb_s2s_beam_gather_batch": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_int, _c_int,
+                                          _c_int, _c_int, _vp]),
     "sb_s2s_fc_fused": (_c_int, [_c_int, _c_int]),
     "sb_s2s_fc_workspace_size": (_c_int, [_c_ll, _c_int, ctypes.POINTER(_c_sz)]),
     "sb_s2s_fc_rows": (_c_int, [_vp, _vp, _vp, _vp, _c_ll, _c_int, _c_int, _vp, _c_int, _c_ll,
@@ -71,6 +77,11 @@ SIGNATURES = {
     "sb_s2s_beam_select_split": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_int, _c_int,
                                           _c_int, _c_int, _c_int, _c_int, _c_int, _vp, _c_sz,
                                           _vp]),
+    "sb_s2s_beam_split_workspace_size_batch": (_c_int, [_c_int, _c_int, _c_int,
+                                                        ctypes.POINTER(_c_sz)]),
+    "sb_s2s_beam_select_split_batch": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_int, _c_int,
+                                                _c_int, _c_int, _c_int, _c_int, _c_int, _vp,
+                                                _c_int, _vp, _c_sz, _vp]),
     "sb_rnnt_workspace_size": (_c_int, [_c_int, _c_int, _c_int, ctypes.POINTER(_c_sz)]),
     "sb_rnnt_fwd_bwd": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int,
                                  _vp, _vp, _c_sz, _vp]),

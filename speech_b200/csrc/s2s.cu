@@ -225,8 +225,8 @@ static AttnWs attn_ws_carve(void* ws, int B, int T, int H) {
 }
 
 struct AttnFwdParams {
-  const float* eh;        // (Beh, T, H) encoder states
-  int eh_bcast;           // 1: every row attends over utterance 0 (beam search of one utterance)
+  const float* eh;        // (B / eh_group, T, H) encoder states
+  int eh_group;           // row b attends over utterance b / eh_group (1: its own; K: K beam rows each)
   const float* hx;        // (B, H) decoder state of this step
   const float* ax_prev;   // (B, T) or null
   const float* conv_wT;   // (Kc, H)  transposed location-conv weights
@@ -283,7 +283,7 @@ __global__ void __launch_bounds__(ATT_THREADS) s2s_attn_fwd_kernel(const AttnFwd
   float* sct = wst + 2 * ATT_NW;               // [TS] scale of each CTA partial (final combine)
   const bool has_prev = p.ax_prev != nullptr;
   const float tscale = p.log_t ? logf((float)Tb) : 1.0f;
-  const float* eh = p.eh + (p.eh_bcast ? 0 : (size_t)b * T * H);
+  const float* eh = p.eh + (size_t)(b / p.eh_group) * T * H;
   const int tw = ts * ATT_TT + warp * ATT_FG;
   const int nf = max(0, min(ATT_FG, Tb - tw));
 
@@ -841,8 +841,9 @@ __global__ void __launch_bounds__(32 * CELL_WARPS) s2s_cell_bwd_kernel(const Cel
 }
 
 // ------------------------------------------------------------------------------------------------
-// beam search bookkeeping on the device (Seq2Seq.beam_search, seq2seq.py:180-227; one utterance,
-// the beam entries are the rows of the step kernels).  Per step, ONE CTA:
+// beam search bookkeeping on the device (Seq2Seq.beam_search, seq2seq.py:180-227, run for each of
+// B utterances on its own; the K beam entries of utterance b are rows b*K .. b*K+K-1 of the step
+// kernels).  Per step, ONE CTA per utterance:
 //   candidates (i, c): score_i + logp[i][c] for every live row i (float64, like the reference's
 //   Python floats), "sorted" by (score desc, i*C + c asc) = the reference's stable descending sort
 //   over its (beam-outer, vocabulary-inner) candidate list (:200-204); the first K of them that
@@ -853,9 +854,15 @@ __global__ void __launch_bounds__(32 * CELL_WARPS) s2s_cell_bwd_kernel(const Cel
 // (parent node, token) in a plain list: nothing merges prefixes here, so ids need not be canonical,
 // and the root is a real token (the start token).  The best complete (else best live) hypothesis
 // is back-tracked on the device when the search stops.
+// A batch keeps B states and B arenas (nodes, complete scores, final hypothesis) back to back.
+// Each utterance's CTA counts itself into stop[0] once, when its search stops; the CTA that makes
+// the count B sets stop[1], the no-op flag of the batch's step kernels (B = 1: the same step at
+// which the utterance's own `done` is set).  Utterances that stopped keep their rows in the step
+// kernels until then; their select and gather CTAs do nothing.
 // ------------------------------------------------------------------------------------------------
 static constexpr int BM_MAXK = 32;
-// done and out_len lead, at the byte offsets the header promises (the host reads them in place)
+// done and out_len lead, at the byte offsets the header promises (the host reads them in place);
+// final_score is the last 8 bytes
 struct BeamState {
   int done;
   int out_len;
@@ -868,26 +875,44 @@ struct BeamState {
   int best_c_node;
   int have_complete;
   int nodes_used;
+  double final_score;        // float64 score of the final hypothesis (written when it stops)
 };
-static_assert(offsetof(BeamState, done) == 0 && offsetof(BeamState, out_len) == 4,
-              "sb_s2s_beam_state_size: done / out_len offsets");
+static_assert(offsetof(BeamState, done) == 0 && offsetof(BeamState, out_len) == 4 &&
+                  offsetof(BeamState, final_score) == sizeof(BeamState) - 8,
+              "sb_s2s_beam_state_size: done / out_len / final_score offsets");
 
+// Pointers are those of utterance 0; of(b) gives utterance b's.
 struct BeamParams {
-  const float* logp;         // (K, C) log-softmax of this step's logits
-  BeamState* st;
-  double* c_scores;          // [max complete] scores of complete hypotheses (for the stop rule)
-  int* nodes;                // [node_cap][2] parent, token
-  int* parent_row;           // (K) out: row of the previous beam each new entry continues
-  int* tok_next;             // (K) out: token fed to the next step
-  int* out_tokens;           // [max_len + 2] final hypothesis (written when the search stops)
-  int K, C, end_tok, step, max_len, node_cap, c_cap;
+  const float* logp;         // [B][K][C] log-softmax of this step's logits
+  BeamState* st;             // [B]
+  double* c_scores;          // [B][c_cap] scores of complete hypotheses (for the stop rule)
+  int* nodes;                // [B][node_cap][2] parent, token
+  int* parent_row;           // [B][K] out: row of the previous beam each new entry continues
+  int* tok_next;             // [B][K] out: token fed to the next step
+  int* out_tokens;           // [B][max_len + 2] final hypothesis (written when the search stops)
+  int* stop;                 // [2] stopped utterances, batch done flag (or null)
+  int K, C, end_tok, step, max_len, node_cap, c_cap, B;
+
+  SB_DEVINL BeamParams of(int b) const {
+    BeamParams q = *this;
+    q.logp += (size_t)b * K * C;
+    q.st += b;
+    q.c_scores += (size_t)b * c_cap;
+    q.nodes += (size_t)b * 2 * node_cap;
+    q.parent_row += (size_t)b * K;
+    q.tok_next += (size_t)b * K;
+    q.out_tokens += (size_t)b * (max_len + 2);
+    return q;
+  }
 };
 
 SB_DEVINL void beam_bookkeep(const BeamParams& p, const int* sel_idx, const double* sel_sc,
                              int want);
 
-__global__ void __launch_bounds__(256) s2s_beam_select_kernel(const BeamParams p) {
+// grid B: CTA b selects for utterance b
+__global__ void __launch_bounds__(256) s2s_beam_select_kernel(const BeamParams pb) {
   extern __shared__ unsigned char bm_smem[];
+  const BeamParams p = pb.of(blockIdx.x);
   double* sc = reinterpret_cast<double*>(bm_smem);       // [K * C]
   __shared__ int sel_idx[2 * BM_MAXK];
   __shared__ double sel_sc[2 * BM_MAXK];
@@ -912,21 +937,28 @@ __global__ void __launch_bounds__(256) s2s_beam_select_kernel(const BeamParams p
 
 // ------------------------------------------------------------------------------------------------
 // split beam selection, for K*C candidates that do not fit one CTA's shared memory:
-//   stage 1 (s2s_beam_tiles): CTA per tile of BM_TILE flat indices i*C + c of the live rows; each
-//           keeps its own top min(2K, n) candidates by (score desc, index asc), in that order.
-//   stage 2 (s2s_beam_merge): one CTA merges the tiles' sorted lists (a head per tile) into the
-//           global first min(2K, nl*C) and runs the same bookkeeping.
+//   stage 1 (s2s_beam_tiles): grid (tiles, B), CTA per tile of BM_TILE flat indices i*C + c of the
+//           utterance's live rows; each keeps its own top min(2K, n) candidates by (score desc,
+//           index asc), in that order.
+//   stage 2 (s2s_beam_merge): grid B, a CTA per utterance merges its tiles' sorted lists (a head
+//           per tile) into the first min(2K, nl*C) and runs the same bookkeeping.
 // The union of the top K and the first K non-ended candidates lies in the global top 2K (at most
 // K of the top K end in end_tok), so the 2K per tile lose nothing.
 // ------------------------------------------------------------------------------------------------
 static constexpr int BM_PER_THREAD = 16;
 static constexpr int BM_TILE = 256 * BM_PER_THREAD;
 
-__global__ void __launch_bounds__(256) s2s_beam_tiles_kernel(const BeamParams p, double* t_sc,
+// t_sc / t_idx [B][tiles][2K], t_cnt [B][tiles]
+__global__ void __launch_bounds__(256) s2s_beam_tiles_kernel(const BeamParams pb, double* t_sc,
                                                              int* t_idx, int* t_cnt) {
+  const BeamParams p = pb.of(blockIdx.y);
   const BeamState* st = p.st;
   if (st->done) return;
   const int tid = threadIdx.x, tile = blockIdx.x, K2 = 2 * p.K, C = p.C;
+  const size_t u0 = (size_t)blockIdx.y * gridDim.x;      // the utterance's first tile slot
+  t_sc += u0 * K2;
+  t_idx += u0 * K2;
+  t_cnt += u0;
   const int n = st->nlive * C;
   double v[BM_PER_THREAD];
 #pragma unroll
@@ -955,15 +987,20 @@ __global__ void __launch_bounds__(256) s2s_beam_tiles_kernel(const BeamParams p,
   if (tid == 0) t_cnt[tile] = q;
 }
 
-__global__ void __launch_bounds__(256) s2s_beam_merge_kernel(const BeamParams p, const double* t_sc,
-                                                             const int* t_idx, const int* t_cnt,
-                                                             int ntiles) {
+__global__ void __launch_bounds__(256) s2s_beam_merge_kernel(const BeamParams pb,
+                                                             const double* t_sc, const int* t_idx,
+                                                             const int* t_cnt, int ntiles) {
   extern __shared__ int bmm_head[];                  // [ntiles] next entry of each tile's list
   __shared__ int sel_idx[2 * BM_MAXK];
   __shared__ double sel_sc[2 * BM_MAXK];
+  const BeamParams p = pb.of(blockIdx.x);
   BeamState* st = p.st;
   if (st->done) return;
   const int tid = threadIdx.x, K2 = 2 * p.K;
+  const size_t u0 = (size_t)blockIdx.x * ntiles;
+  t_sc += u0 * K2;
+  t_idx += u0 * K2;
+  t_cnt += u0;
   const int want = min(K2, st->nlive * p.C);
   for (int t = tid; t < ntiles; t += 256) bmm_head[t] = 0;
   __syncthreads();
@@ -990,8 +1027,9 @@ __global__ void __launch_bounds__(256) s2s_beam_merge_kernel(const BeamParams p,
   beam_bookkeep(p, sel_idx, sel_sc, want);
 }
 
-// ---- the reference's bookkeeping, sequential (a handful of entries): the first `want` candidates
-// in (score desc, index asc) order -> complete / next beam / stop rule / back-track ----
+// ---- the reference's bookkeeping of one utterance (p = BeamParams::of(b)), sequential (a handful
+// of entries): the first `want` candidates in (score desc, index asc) order -> complete / next
+// beam / stop rule / back-track; parent_row holds rows within the utterance ----
 SB_DEVINL void beam_bookkeep(const BeamParams& p, const int* sel_idx, const double* sel_sc,
                              int want) {
   BeamState* st = p.st;
@@ -1007,7 +1045,7 @@ SB_DEVINL void beam_bookkeep(const BeamParams& p, const int* sel_idx, const doub
     if (ended && q >= K) continue;                 // only the first K candidates may complete
     if (!ended && nb >= K) continue;
     int id = st->nodes_used;
-    if (id >= p.node_cap) { st->done = 1; break; }
+    if (id >= p.node_cap) { st->done = p.step + 1; break; }
     st->nodes_used = id + 1;
     p.nodes[2 * id] = old_node[r];
     p.nodes[2 * id + 1] = c;
@@ -1037,7 +1075,7 @@ SB_DEVINL void beam_bookkeep(const BeamParams& p, const int* sel_idx, const doub
     stop = better >= K;
   }
   if (stop) {
-    st->done = 1;
+    st->done = p.step + 1;                         // nonzero: the steps the search ran
     // best complete hypothesis, else the best live one (seq2seq.py:223-227)
     int n = st->have_complete ? st->best_c_node : (nb > 0 ? st->node[0] : -1);
     int len = 0;
@@ -1045,24 +1083,44 @@ SB_DEVINL void beam_bookkeep(const BeamParams& p, const int* sel_idx, const doub
     int k = len;
     for (int q = n; q >= 0; q = p.nodes[2 * q]) p.out_tokens[--k] = p.nodes[2 * q + 1];
     st->out_len = len;
+    st->final_score = st->have_complete ? st->best_c_score : (nb > 0 ? st->score[0] : -INFINITY);
   }
+  // stopped in this call (here or at the node cap): count it; the last of the batch sets the flag
+  if (st->done && p.stop && atomicAdd(p.stop, 1) == p.B - 1) p.stop[1] = 1;
 }
 
-// rows of the next beam continue rows parent_row[] of the previous one: gather hx / sx / ax
+// rows of the next beam continue rows parent_row[] of the previous one: gather hx / sx / ax.
+// Grid B*K: CTA b*K + r fills row r of utterance b from row parent_row[b*K + r] of the same one.
 __global__ void __launch_bounds__(256)
 s2s_beam_gather_kernel(const float* __restrict__ hx_in, const float* __restrict__ sx_in,
                        const float* __restrict__ ax_in, float* __restrict__ hx_out,
                        float* __restrict__ sx_out, float* __restrict__ ax_out,
-                       const int* __restrict__ parent_row, const BeamState* st, int H, int T) {
-  if (st->done) return;
-  const int r = blockIdx.x;
-  if (r >= st->nlive) return;
-  const int src = parent_row[r];
+                       const int* __restrict__ parent_row, const BeamState* st, int K, int H,
+                       int T) {
+  const int b = blockIdx.x / K, r = blockIdx.x - b * K;
+  if (st[b].done || r >= st[b].nlive) return;
+  const size_t dst = blockIdx.x, src = (size_t)b * K + parent_row[dst];
   for (int h = threadIdx.x; h < H; h += 256) {
-    hx_out[(size_t)r * H + h] = hx_in[(size_t)src * H + h];
-    sx_out[(size_t)r * H + h] = sx_in[(size_t)src * H + h];
+    hx_out[dst * H + h] = hx_in[src * H + h];
+    sx_out[dst * H + h] = sx_in[src * H + h];
   }
-  for (int t = threadIdx.x; t < T; t += 256) ax_out[(size_t)r * T + t] = ax_in[(size_t)src * T + t];
+  for (int t = threadIdx.x; t < T; t += 256) ax_out[dst * T + t] = ax_in[src * T + t];
+}
+
+// grid B: utterance b's state (the root alone), its root node and the token of its first row
+__global__ void s2s_beam_init_kernel(BeamState* st, int* nodes, int node_cap, int* tok_next, int K,
+                                     int start_tok, int* stop) {
+  const int b = blockIdx.x;
+  int* w = reinterpret_cast<int*>(st + b);
+  for (int i = threadIdx.x; i < (int)(sizeof(BeamState) / sizeof(int)); i += blockDim.x) w[i] = 0;
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  BeamState* s = st + b;
+  s->score[0] = 0.0; s->node[0] = 0; s->token[0] = start_tok; s->nlive = 1; s->nodes_used = 1;
+  nodes[(size_t)b * 2 * node_cap] = -1;
+  nodes[(size_t)b * 2 * node_cap + 1] = start_tok;
+  tok_next[(size_t)b * K] = start_tok;
+  if (stop && b == 0) { stop[0] = 0; stop[1] = 0; }
 }
 
 // greedy decode: stop when EVERY row emitted end_tok at this step (seq2seq.py:162-178, :155-156)
@@ -1107,7 +1165,7 @@ static int attn_dims_ok(int B, int T, int H, int Kc) {
   return SB_OK;
 }
 
-extern "C" int sb_s2s_attn_fwd(const float* eh, int eh_bcast, const float* hx, const float* ax_prev,
+extern "C" int sb_s2s_attn_fwd(const float* eh, int eh_group, const float* hx, const float* ax_prev,
                                const float* conv_wT, const float* conv_b, const float* lin_w,
                                float lin_b, int log_t, int B, int T, int H, int Kc, float* sx,
                                float* ax, const float* fc_w, const float* fc_b, int C,
@@ -1115,7 +1173,8 @@ extern "C" int sb_s2s_attn_fwd(const float* eh, int eh_bcast, const float* hx, c
                                int* history, int hist_stride, int hist_col, int* end_count,
                                int end_tok, const int* done, const int* lens, void* workspace,
                                size_t workspace_bytes, void* stream_) {
-  if (!eh || !hx || !conv_wT || !conv_b || !lin_w || !sx || !ax || !workspace) return SB_ERR_INVALID;
+  if (!eh || eh_group < 1 || !hx || !conv_wT || !conv_b || !lin_w || !sx || !ax || !workspace)
+    return SB_ERR_INVALID;
   int rc = attn_dims_ok(B, T, H, Kc);
   if (rc != SB_OK) return rc;
   if (workspace_bytes < attn_ws_bytes(B, T, H)) return SB_ERR_WORKSPACE;
@@ -1128,7 +1187,7 @@ extern "C" int sb_s2s_attn_fwd(const float* eh, int eh_bcast, const float* hx, c
                            (int)smem) != cudaSuccess)
     return SB_ERR_CUDA;
   AttnFwdParams p;
-  p.eh = eh; p.eh_bcast = eh_bcast; p.hx = hx; p.ax_prev = ax_prev; p.conv_wT = conv_wT;
+  p.eh = eh; p.eh_group = eh_group; p.hx = hx; p.ax_prev = ax_prev; p.conv_wT = conv_wT;
   p.conv_b = conv_b; p.lin_w = lin_w; p.lin_b = lin_b; p.sx = sx; p.ax = ax; p.fc_w = fc_w;
   p.fc_b = fc_b; p.logits = logits; p.logit_stride = logit_stride; p.logp = logp;
   p.argmax = argmax; p.history = history; p.hist_stride = hist_stride; p.hist_col = hist_col;
@@ -1227,46 +1286,60 @@ extern "C" int sb_s2s_beam_state_size(size_t* bytes) {
   return SB_OK;
 }
 
-// state must be zero-filled except: score[0] = 0, node[0] = root node id 0 (nodes[0] = {-1, start
-// token}), token[0] = start token, nlive = 1, nodes_used = 1 -- sb_s2s_beam_init does that.
+// The single-utterance entry points below are the batched ones at B = 1 without a stop counter:
+// the utterance's own `done` is then the no-op flag of the step kernels.
+static int beam_batch_ok(int B) {
+  return B <= 0 ? SB_ERR_INVALID : (B > 65535 ? SB_ERR_UNSUPPORTED : SB_OK);
+}
+
+// utterance b: state zero but score[0] = 0, node[0] = root node id 0 (its nodes[0] = {-1, start
+// token}), token[0] = start token, nlive = 1, nodes_used = 1; tok_next[b*K] = start token
+static int beam_init(void* state, int* nodes, int node_cap, int* tok_next, int K, int start_tok,
+                     int* stop, int B, void* stream_) {
+  if (!state || !nodes || !tok_next || K <= 0 || node_cap <= 0) return SB_ERR_INVALID;
+  const int rc = beam_batch_ok(B);
+  if (rc != SB_OK) return rc;
+  sb::s2s_beam_init_kernel<<<B, 32, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
+      reinterpret_cast<sb::BeamState*>(state), nodes, node_cap, tok_next, K, start_tok, stop);
+  return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
+}
+
 extern "C" int sb_s2s_beam_init(void* state, int* nodes, int* tok_next, int start_tok,
                                 void* stream_) {
-  if (!state || !nodes || !tok_next) return SB_ERR_INVALID;
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  sb::BeamState h;
-  memset(&h, 0, sizeof(h));
-  h.score[0] = 0.0; h.node[0] = 0; h.token[0] = start_tok; h.nlive = 1; h.nodes_used = 1;
-  const int root[2] = {-1, start_tok};
-  if (cudaMemcpyAsync(state, &h, sizeof(h), cudaMemcpyHostToDevice, stream) != cudaSuccess ||
-      cudaMemcpyAsync(nodes, root, sizeof(root), cudaMemcpyHostToDevice, stream) != cudaSuccess ||
-      cudaMemcpyAsync(tok_next, &start_tok, sizeof(int), cudaMemcpyHostToDevice, stream) !=
-          cudaSuccess)
-    return SB_ERR_CUDA;
-  // (pageable host sources: the copies are staged before the call returns)
-  return SB_OK;
+  return beam_init(state, nodes, 1, tok_next, 1, start_tok, nullptr, 1, stream_);
+}
+
+extern "C" int sb_s2s_beam_init_batch(void* state, int* nodes, int node_cap, int* tok_next, int K,
+                                      int start_tok, int* stop, int B, void* stream_) {
+  if (!stop) return SB_ERR_INVALID;
+  return beam_init(state, nodes, node_cap, tok_next, K, start_tok, stop, B, stream_);
 }
 
 // checks and fill-in shared by the single-CTA and the split selection
 static int beam_params(sb::BeamParams* p, const float* logp, void* state, double* c_scores,
                        int* nodes, int* parent_row, int* tok_next, int* out_tokens, int K, int C,
-                       int end_tok, int step, int max_len, int node_cap, int c_cap) {
+                       int end_tok, int step, int max_len, int node_cap, int c_cap, int* stop,
+                       int B) {
   if (!logp || !state || !c_scores || !nodes || !parent_row || !tok_next || !out_tokens)
     return SB_ERR_INVALID;
+  const int rc = beam_batch_ok(B);
+  if (rc != SB_OK) return rc;
   if (K <= 0 || K > sb::BM_MAXK || C <= 0) return SB_ERR_UNSUPPORTED;
   p->logp = logp; p->st = reinterpret_cast<sb::BeamState*>(state); p->c_scores = c_scores;
   p->nodes = nodes; p->parent_row = parent_row; p->tok_next = tok_next; p->out_tokens = out_tokens;
+  p->stop = stop;
   p->K = K; p->C = C; p->end_tok = end_tok; p->step = step; p->max_len = max_len;
-  p->node_cap = node_cap; p->c_cap = c_cap;
+  p->node_cap = node_cap; p->c_cap = c_cap; p->B = B;
   return SB_OK;
 }
 
-extern "C" int sb_s2s_beam_select(const float* logp, void* state, double* c_scores, int* nodes,
-                                  int* parent_row, int* tok_next, int* out_tokens, int K, int C,
-                                  int end_tok, int step, int max_len, int node_cap, int c_cap,
-                                  void* stream_) {
+static int beam_select(const float* logp, void* state, double* c_scores, int* nodes,
+                       int* parent_row, int* tok_next, int* out_tokens, int K, int C, int end_tok,
+                       int step, int max_len, int node_cap, int c_cap, int* stop, int B,
+                       void* stream_) {
   sb::BeamParams p;
   const int rc = beam_params(&p, logp, state, c_scores, nodes, parent_row, tok_next, out_tokens, K,
-                             C, end_tok, step, max_len, node_cap, c_cap);
+                             C, end_tok, step, max_len, node_cap, c_cap, stop, B);
   if (rc != SB_OK) return rc;
   const size_t smem = (size_t)K * C * sizeof(double);
   if (smem > 200 * 1024) return SB_ERR_UNSUPPORTED;
@@ -1275,8 +1348,26 @@ extern "C" int sb_s2s_beam_select(const float* logp, void* state, double* c_scor
       cudaFuncSetAttribute(sb::s2s_beam_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                            (int)smem) != cudaSuccess)
     return SB_ERR_CUDA;
-  sb::s2s_beam_select_kernel<<<1, 256, smem, stream>>>(p);
+  sb::s2s_beam_select_kernel<<<B, 256, smem, stream>>>(p);
   return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
+}
+
+extern "C" int sb_s2s_beam_select(const float* logp, void* state, double* c_scores, int* nodes,
+                                  int* parent_row, int* tok_next, int* out_tokens, int K, int C,
+                                  int end_tok, int step, int max_len, int node_cap, int c_cap,
+                                  void* stream_) {
+  return beam_select(logp, state, c_scores, nodes, parent_row, tok_next, out_tokens, K, C, end_tok,
+                     step, max_len, node_cap, c_cap, nullptr, 1, stream_);
+}
+
+extern "C" int sb_s2s_beam_select_batch(const float* logp, void* state, double* c_scores,
+                                        int* nodes, int* parent_row, int* tok_next,
+                                        int* out_tokens, int K, int C, int end_tok, int step,
+                                        int max_len, int node_cap, int c_cap, int* stop, int B,
+                                        void* stream_) {
+  if (!stop) return SB_ERR_INVALID;
+  return beam_select(logp, state, c_scores, nodes, parent_row, tok_next, out_tokens, K, C, end_tok,
+                     step, max_len, node_cap, c_cap, stop, B, stream_);
 }
 
 extern "C" int sb_s2s_beam_select_fits(int K, int C) {
@@ -1287,26 +1378,32 @@ static int beam_split_tiles(int K, int C) {
   return (int)(((long long)K * C + sb::BM_TILE - 1) / sb::BM_TILE);
 }
 
-extern "C" int sb_s2s_beam_split_workspace_size(int K, int C, size_t* bytes) {
-  if (!bytes || K <= 0 || C <= 0) return SB_ERR_INVALID;
+// B utterances: B times the bytes of one; carved as [B][tiles][2K] scores | [B][tiles][2K]
+// indices | [B][tiles] counts, which needs less than that
+extern "C" int sb_s2s_beam_split_workspace_size_batch(int K, int C, int B, size_t* bytes) {
+  if (!bytes || K <= 0 || C <= 0 || B <= 0) return SB_ERR_INVALID;
   const size_t nt = (size_t)beam_split_tiles(K, C);
-  *bytes = nt * 2 * K * (sizeof(double) + sizeof(int)) + nt * sizeof(int) + 64;
+  *bytes = (size_t)B * (nt * 2 * K * (sizeof(double) + sizeof(int)) + nt * sizeof(int) + 64);
   return SB_OK;
 }
 
-extern "C" int sb_s2s_beam_select_split(const float* logp, void* state, double* c_scores,
-                                        int* nodes, int* parent_row, int* tok_next,
-                                        int* out_tokens, int K, int C, int end_tok, int step,
-                                        int max_len, int node_cap, int c_cap, void* workspace,
-                                        size_t workspace_bytes, void* stream_) {
+extern "C" int sb_s2s_beam_split_workspace_size(int K, int C, size_t* bytes) {
+  return sb_s2s_beam_split_workspace_size_batch(K, C, 1, bytes);
+}
+
+static int beam_select_split(const float* logp, void* state, double* c_scores, int* nodes,
+                             int* parent_row, int* tok_next, int* out_tokens, int K, int C,
+                             int end_tok, int step, int max_len, int node_cap, int c_cap,
+                             int* stop, int B, void* workspace, size_t workspace_bytes,
+                             void* stream_) {
   if (!workspace) return SB_ERR_INVALID;
   sb::BeamParams p;
   const int rc = beam_params(&p, logp, state, c_scores, nodes, parent_row, tok_next, out_tokens, K,
-                             C, end_tok, step, max_len, node_cap, c_cap);
+                             C, end_tok, step, max_len, node_cap, c_cap, stop, B);
   if (rc != SB_OK) return rc;
   if ((long long)K * C > 0x7fffffffLL) return SB_ERR_UNSUPPORTED;
   size_t need = 0;
-  sb_s2s_beam_split_workspace_size(K, C, &need);
+  sb_s2s_beam_split_workspace_size_batch(K, C, B, &need);
   if (workspace_bytes < need) return SB_ERR_WORKSPACE;
   const int nt = beam_split_tiles(K, C);
   const size_t smem = (size_t)nt * sizeof(int);
@@ -1316,11 +1413,49 @@ extern "C" int sb_s2s_beam_select_split(const float* logp, void* state, double* 
       cudaFuncSetAttribute(sb::s2s_beam_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                            (int)smem) != cudaSuccess)
     return SB_ERR_CUDA;
+  const size_t slots = (size_t)B * nt * 2 * K;
   double* t_sc = reinterpret_cast<double*>(workspace);
-  int* t_idx = reinterpret_cast<int*>(t_sc + (size_t)nt * 2 * K);
-  int* t_cnt = t_idx + (size_t)nt * 2 * K;
-  sb::s2s_beam_tiles_kernel<<<nt, 256, 0, stream>>>(p, t_sc, t_idx, t_cnt);
-  sb::s2s_beam_merge_kernel<<<1, 256, smem, stream>>>(p, t_sc, t_idx, t_cnt, nt);
+  int* t_idx = reinterpret_cast<int*>(t_sc + slots);
+  int* t_cnt = t_idx + slots;
+  sb::s2s_beam_tiles_kernel<<<dim3(nt, B), 256, 0, stream>>>(p, t_sc, t_idx, t_cnt);
+  sb::s2s_beam_merge_kernel<<<B, 256, smem, stream>>>(p, t_sc, t_idx, t_cnt, nt);
+  return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
+}
+
+extern "C" int sb_s2s_beam_select_split(const float* logp, void* state, double* c_scores,
+                                        int* nodes, int* parent_row, int* tok_next,
+                                        int* out_tokens, int K, int C, int end_tok, int step,
+                                        int max_len, int node_cap, int c_cap, void* workspace,
+                                        size_t workspace_bytes, void* stream_) {
+  return beam_select_split(logp, state, c_scores, nodes, parent_row, tok_next, out_tokens, K, C,
+                           end_tok, step, max_len, node_cap, c_cap, nullptr, 1, workspace,
+                           workspace_bytes, stream_);
+}
+
+extern "C" int sb_s2s_beam_select_split_batch(const float* logp, void* state, double* c_scores,
+                                              int* nodes, int* parent_row, int* tok_next,
+                                              int* out_tokens, int K, int C, int end_tok,
+                                              int step, int max_len, int node_cap, int c_cap,
+                                              int* stop, int B, void* workspace,
+                                              size_t workspace_bytes, void* stream_) {
+  if (!stop) return SB_ERR_INVALID;
+  return beam_select_split(logp, state, c_scores, nodes, parent_row, tok_next, out_tokens, K, C,
+                           end_tok, step, max_len, node_cap, c_cap, stop, B, workspace,
+                           workspace_bytes, stream_);
+}
+
+extern "C" int sb_s2s_beam_gather_batch(const float* hx_in, const float* sx_in,
+                                        const float* ax_in, float* hx_out, float* sx_out,
+                                        float* ax_out, const int* parent_row, const void* state,
+                                        int K, int H, int T, int B, void* stream_) {
+  if (!hx_in || !sx_in || !ax_in || !hx_out || !sx_out || !ax_out || !parent_row || !state ||
+      K <= 0)
+    return SB_ERR_INVALID;
+  const int rc = beam_batch_ok(B);
+  if (rc != SB_OK) return rc;
+  sb::s2s_beam_gather_kernel<<<B * K, 256, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
+      hx_in, sx_in, ax_in, hx_out, sx_out, ax_out, parent_row,
+      reinterpret_cast<const sb::BeamState*>(state), K, H, T);
   return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
 }
 
@@ -1328,10 +1463,6 @@ extern "C" int sb_s2s_beam_gather(const float* hx_in, const float* sx_in, const 
                                   float* hx_out, float* sx_out, float* ax_out,
                                   const int* parent_row, const void* state, int K, int H, int T,
                                   void* stream_) {
-  if (!hx_in || !sx_in || !ax_in || !hx_out || !sx_out || !ax_out || !parent_row || !state)
-    return SB_ERR_INVALID;
-  sb::s2s_beam_gather_kernel<<<K, 256, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
-      hx_in, sx_in, ax_in, hx_out, sx_out, ax_out, parent_row,
-      reinterpret_cast<const sb::BeamState*>(state), H, T);
-  return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
+  return sb_s2s_beam_gather_batch(hx_in, sx_in, ax_in, hx_out, sx_out, ax_out, parent_row, state,
+                                  K, H, T, 1, stream_);
 }

@@ -3,8 +3,8 @@ Seq2Seq.decode / decode_step / infer / beam_search (speech/models/seq2seq.py:78-
 NNAttention.forward (:344-360) as two kernels per token (GRU cell; attention + output projection),
 with a hand-written backward (three kernels per token, the output-projection backward of all
 steps in one launch, the weight gradients time-batched on the wgmma GEMM), a greedy loop and a
-beam search that never leave the device: the host only enqueues kernels and reads the final
-hypothesis back once.
+beam search over a whole batch that never leave the device: the host only enqueues kernels and
+reads the final hypotheses back once.
 """
 import torch
 
@@ -22,9 +22,11 @@ def _f(t):
 # selection holds all K*C float64 candidates (<= 200 KB, sb_s2s_beam_select_fits); past that it
 # runs split over many CTAs.
 DOUT_MAX_CLASSES = 8192
-# byte offsets of `done` and of the final hypothesis' length in the beam state (speech_b200.h)
+# byte offsets of `done` and of the final hypothesis' length in the beam state (speech_b200.h); the
+# hypothesis' float64 score is the state's last 8 bytes
 BEAM_DONE_OFFSET = 0
 BEAM_OUT_LEN_OFFSET = 4
+BEAM_MAX_WIDTH = 32
 
 
 def fc_fused(H, C):
@@ -98,14 +100,14 @@ def _cell_fwd(lib, w, tok, tok_stride, sx_prev, hx_prev, hx, ix_save, gates_save
                                             _a(ix_save), _a(gates_save), done, B, w.H, sp))
 
 
-def _attn_fwd(lib, w, ws, eh, bcast, hx, ax_prev, sx, ax, B, T, sp, logits=None, logit_stride=0,
+def _attn_fwd(lib, w, ws, eh, group, hx, ax_prev, sx, ax, B, T, sp, logits=None, logit_stride=0,
               logp=None, argmax=None, history=None, hist_stride=0, hist_col=0, end_count=None,
               end_tok=-1, done=None, with_fc=True, lens=None):
-    """the attention step of B rows; with_fc: also the output projection (w: DecoderWeights),
-    else the attention alone (w may be AttentionWeights)"""
+    """the attention step of B rows, row b over utterance b // group of eh; with_fc: also the
+    output projection (w: DecoderWeights), else the attention alone (w may be AttentionWeights)"""
     fc_w, fc_b, C = (w.p_fc_w, w.p_fc_b, w.C) if with_fc else (None, None, 0)
     ops._launch("s2s_attn_fwd", 0.0,
-                lambda: lib.sb_s2s_attn_fwd(_a(eh), bcast, _a(hx), _a(ax_prev), w.p_conv_wT,
+                lambda: lib.sb_s2s_attn_fwd(_a(eh), group, _a(hx), _a(ax_prev), w.p_conv_wT,
                                             w.p_conv_b, w.p_lin_w, w.lin_b, w.log_t, B, T, w.H,
                                             w.Kc, _a(sx), _a(ax), fc_w, fc_b, C, logits,
                                             logit_stride, _a(logp), _a(argmax), history,
@@ -188,7 +190,7 @@ def attn_step(attend, eh, dhx, ax_prev, lens=None):
     ax = torch.empty(B, T, dtype=torch.float32, device=eh.device)
     ws = attn_workspace(lib, B, T, H, eh.device)
     ld = attn_lens(lens, B, T, eh.device)
-    _attn_fwd(lib, w, ws, eh, 0, d, axp, sx, ax, B, T, _lib.stream_ptr(), with_fc=False, lens=ld)
+    _attn_fwd(lib, w, ws, eh, 1, d, axp, sx, ax, B, T, _lib.stream_ptr(), with_fc=False, lens=ld)
     return sx.unsqueeze(1), ax
 
 
@@ -244,12 +246,12 @@ class DecodeFunction(torch.autograd.Function):
                       p_hx + (u + 1) * BH, p_ix + u * BH if need else None,
                       p_gt + 4 * u * BH if need else None, None, B, sp)
             if w.fused:
-                _attn_fwd(lib, w, ws, ehc, 0, p_hx + (u + 1) * BH,
+                _attn_fwd(lib, w, ws, ehc, 1, p_hx + (u + 1) * BH,
                           p_ax + (u - 1) * BT if u > 0 else None, p_sx + u * BH, p_ax + u * BT, B,
                           T, sp, logits=p_logits + 4 * u * w.C, logit_stride=steps * w.C,
                           argmax=p_amax, lens=lens)
                 continue
-            _attn_fwd(lib, w, ws, ehc, 0, p_hx + (u + 1) * BH,
+            _attn_fwd(lib, w, ws, ehc, 1, p_hx + (u + 1) * BH,
                       p_ax + (u - 1) * BT if u > 0 else None, p_sx + u * BH, p_ax + u * BT, B, T,
                       sp, with_fc=False, lens=lens)
             if sampling:
@@ -401,10 +403,10 @@ def decode_step(m, eh, y, state, softmax, lens=None):
     ld = attn_lens(lens, B, T, dev)
     _cell_fwd(lib, w, tok.data_ptr(), 1, sx_prev, hx_prev, hx, None, None, None, B, sp)
     if w.fused:
-        _attn_fwd(lib, w, ws, ehc, 0, hx, ax_prev, sx, ax, B, T, sp, logits=out.data_ptr(),
+        _attn_fwd(lib, w, ws, ehc, 1, hx, ax_prev, sx, ax, B, T, sp, logits=out.data_ptr(),
                   logit_stride=w.C, logp=logp, lens=ld)
     else:
-        _attn_fwd(lib, w, ws, ehc, 0, hx, ax_prev, sx, ax, B, T, sp, with_fc=False, lens=ld)
+        _attn_fwd(lib, w, ws, ehc, 1, hx, ax_prev, sx, ax, B, T, sp, with_fc=False, lens=ld)
         fc_ws = fc_workspace(lib, B, w.C, dev)
         _fc_rows(lib, w, fc_ws, hx, sx, B, sp, logits=out)
         if softmax:
@@ -438,12 +440,12 @@ def greedy(m, eh, start, end_tok, max_len, lens=None):
         _cell_fwd(lib, w, hist.data_ptr() + 4 * e, max_len + 1, sx[prv] if e > 0 else None,
                   hx[prv], hx[cur], None, None, done.data_ptr(), B, sp)
         if w.fused:
-            _attn_fwd(lib, w, ws, ehc, 0, hx[cur], ax[prv] if e > 0 else None, sx[cur], ax[cur], B,
+            _attn_fwd(lib, w, ws, ehc, 1, hx[cur], ax[prv] if e > 0 else None, sx[cur], ax[cur], B,
                       T, sp, history=hist.data_ptr(), hist_stride=max_len + 1, hist_col=e + 1,
                       end_count=ctl.data_ptr() + 4 * e, end_tok=int(end_tok),
                       done=done.data_ptr(), lens=ld)
         else:
-            _attn_fwd(lib, w, ws, ehc, 0, hx[cur], ax[prv] if e > 0 else None, sx[cur], ax[cur], B,
+            _attn_fwd(lib, w, ws, ehc, 1, hx[cur], ax[prv] if e > 0 else None, sx[cur], ax[cur], B,
                       T, sp, done=done.data_ptr(), with_fc=False, lens=ld)
             _fc_rows(lib, w, fc_ws, hx[cur], sx[cur], B, sp, history=hist.data_ptr(),
                      hist_stride=max_len + 1, hist_col=e + 1, end_count=ctl.data_ptr() + 4 * e,
@@ -456,63 +458,88 @@ def greedy(m, eh, start, end_tok, max_len, lens=None):
 
 
 def beam_search(m, eh, start_tok, end_tok, beam_size, max_len):
-    """Seq2Seq.beam_search for one utterance (seq2seq.py:180-227), device-resident: the beam
-    entries are the rows of the step kernels, expand/prune/complete/stop run in one bookkeeping
-    kernel per step (csrc/s2s.cu), the hypothesis is back-tracked on the device."""
+    """Seq2Seq.beam_search for one utterance (seq2seq.py:180-227): beam_search_batch on the first
+    utterance of eh.  -> token tuple."""
+    return beam_search_batch(m, _f(eh)[:1], start_tok, end_tok, beam_size, max_len)[0][0]
+
+
+def beam_search_batch(m, eh, start_tok, end_tok, beam_size, max_len, lens=None):
+    """Seq2Seq.beam_search (seq2seq.py:180-227) for each of the B utterances of eh (B, T, H) at
+    once, device-resident.  Utterance b's K beam entries are rows b*K .. b*K+K-1 of the step
+    kernels, which run over all B*K rows until every utterance has stopped; expand / prune /
+    complete / stop run in one bookkeeping CTA per utterance and step (csrc/s2s.cu), and the
+    hypotheses are back-tracked on the device.  Each utterance's search is the one it gets alone,
+    bit for bit.  The host enqueues every step up front and reads all B results back in ONE copy.
+    lens (optional): frames each utterance attends over.  -> list of B (token tuple, float64
+    score of that hypothesis, steps that utterance's search ran)."""
     lib = _lib.load()
     w = DecoderWeights(m)
-    ehc = _f(eh)[:1].contiguous()
-    _, T, H = ehc.shape
+    ehc = _f(eh)
+    B, T, H = ehc.shape
     K, C = int(beam_size), w.C
+    R = B * K
     dev = ehc.device
-    state = torch.zeros(_lib.workspace_size(lib.sb_s2s_beam_state_size) + 64, dtype=torch.uint8,
-                        device=dev)
+    ld = attn_lens(lens, B, T, dev)
+    if ld is not None:
+        ld = ld.repeat_interleave(K)
+    S = _lib.workspace_size(lib.sb_s2s_beam_state_size)
+    out_cap = max_len + 2
+    # the B states, then the B final hypotheses: the buffer the one device->host copy reads
+    res = torch.zeros(B * S + 4 * B * out_cap, dtype=torch.uint8, device=dev)
+    state, out_tokens = res[:B * S], res[B * S:].view(torch.int32)
     node_cap = 2 * K * (max_len + 1) + 2
-    nodes = torch.zeros(node_cap, 2, dtype=torch.int32, device=dev)
+    nodes = torch.zeros(B, node_cap, 2, dtype=torch.int32, device=dev)
     c_cap = K * (max_len + 1)
-    c_scores = torch.zeros(c_cap, dtype=torch.float64, device=dev)
-    parent = torch.zeros(K, dtype=torch.int32, device=dev)
-    tok = torch.zeros(K, dtype=torch.int32, device=dev)
-    out_tokens = torch.zeros(max_len + 2, dtype=torch.int32, device=dev)
-    hx = [torch.zeros(K, H, dtype=torch.float32, device=dev) for _ in range(3)]
-    sx = [torch.zeros(K, H, dtype=torch.float32, device=dev) for _ in range(3)]
-    ax = [torch.zeros(K, T, dtype=torch.float32, device=dev) for _ in range(3)]
-    logp = torch.empty(K, C, dtype=torch.float32, device=dev)
+    c_scores = torch.zeros(B, c_cap, dtype=torch.float64, device=dev)
+    parent = torch.zeros(R, dtype=torch.int32, device=dev)
+    tok = torch.zeros(R, dtype=torch.int32, device=dev)
+    stop = torch.zeros(2, dtype=torch.int32, device=dev)        # stopped utterances | batch done
+    hx = [torch.zeros(R, H, dtype=torch.float32, device=dev) for _ in range(2)]
+    sx = [torch.zeros(R, H, dtype=torch.float32, device=dev) for _ in range(2)]
+    ax = [torch.zeros(R, T, dtype=torch.float32, device=dev) for _ in range(2)]
+    logp = torch.empty(R, C, dtype=torch.float32, device=dev)
     sp = _lib.stream_ptr()
-    ws = attn_workspace(lib, K, T, H, dev)
-    _lib.check(lib.sb_s2s_beam_init(state.data_ptr(), nodes.data_ptr(), tok.data_ptr(),
-                                    int(start_tok), sp), "beam init")
-    # the `done` word of the state struct doubles as the no-op flag of the step kernels
-    done_ptr = state.data_ptr() + BEAM_DONE_OFFSET
-    fc_ws = None if w.fused else fc_workspace(lib, K, C, dev)
+    ws = attn_workspace(lib, R, T, H, dev)
+    _lib.check(lib.sb_s2s_beam_init_batch(state.data_ptr(), nodes.data_ptr(), node_cap,
+                                          tok.data_ptr(), K, int(start_tok), stop.data_ptr(), B,
+                                          sp), "beam init")
+    done_ptr = stop.data_ptr() + 4              # the no-op flag of the step kernels
+    fc_ws = None if w.fused else fc_workspace(lib, R, C, dev)
     split = not beam_select_fits(K, C)
     if split:
-        sel_ws = torch.empty(_lib.workspace_size(lib.sb_s2s_beam_split_workspace_size, K, C),
-                             dtype=torch.uint8, device=dev)
+        sel_ws = torch.empty(_lib.workspace_size(lib.sb_s2s_beam_split_workspace_size_batch, K, C,
+                                                 B), dtype=torch.uint8, device=dev)
+    p_state, p_c, p_nodes = state.data_ptr(), c_scores.data_ptr(), nodes.data_ptr()
+    p_par, p_tok, p_out = parent.data_ptr(), tok.data_ptr(), out_tokens.data_ptr()
+    p_stop = stop.data_ptr()
     # buffers: [0] = state entering the step (gathered), [1] = state produced by the step
     for e in range(max_len):
-        _cell_fwd(lib, w, tok.data_ptr(), 1, sx[0] if e > 0 else None, hx[0], hx[1], None, None,
-                  done_ptr, K, sp)
+        _cell_fwd(lib, w, p_tok, 1, sx[0] if e > 0 else None, hx[0], hx[1], None, None, done_ptr,
+                  R, sp)
         if w.fused:
-            _attn_fwd(lib, w, ws, ehc, 1, hx[1], ax[0] if e > 0 else None, sx[1], ax[1], K, T, sp,
-                      logp=logp, done=done_ptr)
+            _attn_fwd(lib, w, ws, ehc, K, hx[1], ax[0] if e > 0 else None, sx[1], ax[1], R, T, sp,
+                      logp=logp, done=done_ptr, lens=ld)
         else:
-            _attn_fwd(lib, w, ws, ehc, 1, hx[1], ax[0] if e > 0 else None, sx[1], ax[1], K, T, sp,
-                      done=done_ptr, with_fc=False)
-            _fc_rows(lib, w, fc_ws, hx[1], sx[1], K, sp, logits=logp, done=done_ptr)
-            _fc_logp(lib, w, fc_ws, logp, logp, K, sp, done=done_ptr)
+            _attn_fwd(lib, w, ws, ehc, K, hx[1], ax[0] if e > 0 else None, sx[1], ax[1], R, T, sp,
+                      done=done_ptr, with_fc=False, lens=ld)
+            _fc_rows(lib, w, fc_ws, hx[1], sx[1], R, sp, logits=logp, done=done_ptr)
+            _fc_logp(lib, w, fc_ws, logp, logp, R, sp, done=done_ptr)
         if split:
-            ops._launch("s2s_beam_select_split", 0.0, lambda: lib.sb_s2s_beam_select_split(
-                logp.data_ptr(), state.data_ptr(), c_scores.data_ptr(), nodes.data_ptr(),
-                parent.data_ptr(), tok.data_ptr(), out_tokens.data_ptr(), K, C, int(end_tok), e,
-                max_len, node_cap, c_cap, sel_ws.data_ptr(), sel_ws.numel(), sp))
+            ops._launch("s2s_beam_select_split", 0.0, lambda: lib.sb_s2s_beam_select_split_batch(
+                logp.data_ptr(), p_state, p_c, p_nodes, p_par, p_tok, p_out, K, C, int(end_tok), e,
+                max_len, node_cap, c_cap, p_stop, B, sel_ws.data_ptr(), sel_ws.numel(), sp))
         else:
-            ops._launch("s2s_beam_select", 0.0, lambda: lib.sb_s2s_beam_select(
-                logp.data_ptr(), state.data_ptr(), c_scores.data_ptr(), nodes.data_ptr(),
-                parent.data_ptr(), tok.data_ptr(), out_tokens.data_ptr(), K, C, int(end_tok), e,
-                max_len, node_cap, c_cap, sp))
-        ops._launch("s2s_beam_gather", 0.0, lambda: lib.sb_s2s_beam_gather(
+            ops._launch("s2s_beam_select", 0.0, lambda: lib.sb_s2s_beam_select_batch(
+                logp.data_ptr(), p_state, p_c, p_nodes, p_par, p_tok, p_out, K, C, int(end_tok), e,
+                max_len, node_cap, c_cap, p_stop, B, sp))
+        ops._launch("s2s_beam_gather", 0.0, lambda: lib.sb_s2s_beam_gather_batch(
             hx[1].data_ptr(), sx[1].data_ptr(), ax[1].data_ptr(), hx[0].data_ptr(),
-            sx[0].data_ptr(), ax[0].data_ptr(), parent.data_ptr(), state.data_ptr(), K, H, T, sp))
-    n = int(state[BEAM_OUT_LEN_OFFSET:BEAM_OUT_LEN_OFFSET + 4].view(torch.int32).item())
-    return tuple(out_tokens[:n].cpu().tolist())
+            sx[0].data_ptr(), ax[0].data_ptr(), p_par, p_state, K, H, T, B, sp))
+    host = res.cpu()                            # the one synchronisation of the whole search
+    st = host[:B * S].view(B, S)
+    steps = st[:, BEAM_DONE_OFFSET:BEAM_DONE_OFFSET + 4].contiguous().view(torch.int32).reshape(B)
+    n = st[:, BEAM_OUT_LEN_OFFSET:BEAM_OUT_LEN_OFFSET + 4].contiguous().view(torch.int32).reshape(B)
+    score = st[:, S - 8:].contiguous().view(torch.float64).reshape(B)
+    toks = host[B * S:].view(torch.int32).view(B, out_cap)
+    return [(tuple(toks[b, :int(n[b])].tolist()), float(score[b]), int(steps[b]))
+            for b in range(B)]

@@ -138,6 +138,41 @@ class Seq2Seq(model.Model):
             x = self.encode(x)
             return [s2s.beam_search(self, x, start_tok, end_tok, beam_size, max_len)]
 
+    def recognize(self, inputs, beam_size=10, max_len=200, start_tok=None, end_tok=None,
+                  return_scores=False):
+        """Beam search of every utterance of a batch at once, from the audio alone.  inputs: the
+        (T_i, F) arrays of batch[0].  Each utterance gets `beam_search`'s search on its own (float64
+        scores, stable-descending tie order, the same completion and stop rules), bit for bit, and
+        one stopping never changes another's search.  start_tok / end_tok default to the
+        Preprocessor's convention: START = vocab_size - 1, END = vocab_size - 2.  Frames attended:
+        the padded T' for every utterance, or its own conv_out_size(T_b) in the exact-lengths mode.
+        Returns B token lists (START first; END last where a hypothesis completed, else the best
+        live one), and their float64 scores with return_scores.  Device-resident
+        (functions/s2s.py: beam_search_batch)."""
+        from ..functions import s2s
+        V = self.embedding.num_embeddings
+        start_tok = V - 1 if start_tok is None else int(start_tok)
+        end_tok = V - 2 if end_tok is None else int(end_tok)
+        if not 1 <= int(beam_size) <= s2s.BEAM_MAX_WIDTH:
+            raise ValueError("beam_size must lie in [1, %d], got %r"
+                             % (s2s.BEAM_MAX_WIDTH, beam_size))
+        if int(max_len) < 1:
+            raise ValueError("max_len must be >= 1, got %r" % (max_len,))
+        if not 0 <= start_tok < V:
+            raise ValueError("start_tok %d is not a token of the vocabulary (%d)" % (start_tok, V))
+        if not 0 <= end_tok < V - 1:
+            raise ValueError("end_tok %d is not a class the model predicts (%d)" % (end_tok, V - 1))
+        if len(inputs) == 0:
+            raise ValueError("recognize needs at least one utterance")
+        lens = self.input_lens(inputs)
+        x = self.stage_inputs(inputs)
+        with torch.no_grad():
+            x = self._encode(x, lens)
+            res = s2s.beam_search_batch(self, x, start_tok, end_tok, int(beam_size), int(max_len),
+                                        lens)
+        labels = [list(r[0]) for r in res]
+        return (labels, [r[1] for r in res]) if return_scores else labels
+
     def collate(self, inputs, labels):
         return self.stage_inputs(inputs), torch.from_numpy(end_pad_concat(labels))
 

@@ -22,6 +22,7 @@ lab2 = [[29] + l + [28] for l in labels]
 l2 = s.loss((inputs, lab2)); l2.backward()
 print("seq2seq ok", l2.item(), [len(h) for h in s.infer((inputs, lab2), max_len=12)],
       s.beam_search(([inputs[0]], [lab2[0]]), beam_size=3, max_len=8))
+print("seq2seq recognize", [len(h) for h in s.recognize(inputs, beam_size=3, max_len=8)])
 t = Transducer(80, 28, cfg).cuda()
 l3 = t.loss((inputs, labels)); l3.backward()
 print("transducer ok", l3.item())
