@@ -197,6 +197,69 @@ int sb_ctc_prefix_beam_shortlist(const float* logp, const int* lens, int B, int 
                                  void* stream);
 
 /* ---------------------------------------------------------------------------------------
+ * CTC prefix beam search with shallow fusion of a token-level backoff n-gram LM.
+ * The LM is over the model's own output classes (the blank is never an LM token), orders 1..10.
+ * Its device tables (built by speech_b200.lm.NGramLM) are one open-addressed map, linear probing,
+ * slot h = ((key * 0x9E3779B97F4A7C15) mod 2^64 >> 32) & (cap - 1), with two kinds of key:
+ *   (c << 32) | ((t + 1) << 1) | 0  -> context node of "context c preceded by token t"
+ *   (c << 32) | ((t + 1) << 1) | 1  -> index into logp of the n-gram "context c, then token t"
+ * Context nodes form a trie over contexts read most recent token first; node 0 is the empty
+ * context.  Every context of a stored n-gram has a node, so a walk that stops at depth m proves
+ * that no longer context of that entry holds an n-gram.
+ * lm(s | h), h the last order-1 symbols of the prefix preceded by <s> where it is shorter, is the
+ * ARPA backoff value in natural log: acc = 0, then acc += bow[h'] for each context h' of h from
+ * the longest down while (h', s) is not stored, then acc += logp[(h', s)].
+ * Fusion: extending beam entry i by symbol s uses q = p_s + (lm_weight * lm(s | ctx_i) +
+ * insertion_bonus) for p_s in every term of that extension (float64, in that order).  Blank terms
+ * and the repeated symbol that keeps the prefix use p_s.  The returned score is
+ * -lse(p_b, p_nb) of the best prefix: acoustic + lm_weight * LM + insertion_bonus * length.
+ * With lm_weight = insertion_bonus = 0 the results equal sb_ctc_prefix_beam's bit for bit.
+ * ------------------------------------------------------------------------------------- */
+#define SB_LM_MAX_ORDER 10
+typedef struct SbNgramLm {
+  const unsigned long long* keys;  /* [cap] map keys, 0 = empty slot (device) */
+  const int* vals;                 /* [cap] context node or logp index (device) */
+  const double* logp;              /* [n-grams] natural-log probability (device) */
+  const double* bow;               /* [context nodes] natural-log backoff weight, 0 where the
+                                      ARPA model stores none (device) */
+  const int* tok;                  /* [num_classes] LM token of each class; a class the LM does
+                                      not know maps to the token of <unk>; every class but the
+                                      blank maps to a token with a unigram (device) */
+  int cap;                         /* power of two, at least twice the number of keys */
+  int order;                       /* 1 .. SB_LM_MAX_ORDER */
+  int num_classes;                 /* classes tok covers; must be >= S */
+  int bos;                         /* token of <s> */
+  int blank;                       /* the class that is not an LM token; must equal the search's */
+  double lm_upper;                 /* >= every lm(s | h): the largest logp plus, per order, the
+                                      largest positive bow of that order */
+  double lm_abs;                   /* >= |every partial sum of a lookup|: the largest |logp| plus,
+                                      per order, the largest |bow| of that order */
+} SbNgramLm;
+
+/*   sb_ctc_prefix_beam_lm_workspace_size  bytes for (B, T, beam_size, order)
+ *   sb_ctc_prefix_beam_lm                 sb_ctc_prefix_beam's arguments and route choice, plus
+ *                                         the LM (host struct of device pointers) and the weights
+ *   sb_ctc_prefix_beam_lm_shortlist       the shortlist search at any shape (same arguments);
+ *                                         bit-identical to the full scan with the same LM
+ * SB_ERR_INVALID for lm_weight < 0, a non-finite weight or bound, lm->num_classes < S, or
+ * lm->blank != blank;
+ * SB_ERR_UNSUPPORTED for order > SB_LM_MAX_ORDER or beam_size > 32. */
+int sb_ctc_prefix_beam_lm_workspace_size(int B, int T, int beam_size, int order, size_t* bytes);
+int sb_ctc_prefix_beam_lm(const float* logp, const int* lens, int B, int T, int S, int beam_size,
+                          int blank, const SbNgramLm* lm, double lm_weight,
+                          double insertion_bonus, int* out_labels, int* out_lens,
+                          double* out_scores, void* workspace, size_t workspace_bytes,
+                          void* stream);
+int sb_ctc_prefix_beam_lm_shortlist(const float* logp, const int* lens, int B, int T, int S,
+                                    int beam_size, int blank, const SbNgramLm* lm,
+                                    double lm_weight, double insertion_bonus, int* out_labels,
+                                    int* out_lens, double* out_scores, void* workspace,
+                                    size_t workspace_bytes, void* stream);
+/* Developer counter: frames the LM-fused shortlist search rescanned in full, over every call
+ * since the last query (synchronous: waits for the device); resets it. */
+int sb_debug_ctc_lm_rescans(unsigned long long* frames);
+
+/* ---------------------------------------------------------------------------------------
  * Conv2d(+ReLU) front-end as im2col + sb_gemm_bf16_tn.
  * Replaces: the cuDNN convolutions behind nn.Conv2d in Model.encode
  *           (speech/models/model.py:19-29,60-71; valid conv, kernel (kh,kw), stride s both dims).

@@ -15,6 +15,18 @@ _c_sz = ctypes.c_size_t
 _vp = ctypes.c_void_p
 _fl = ctypes.c_float
 
+
+class SbNgramLm(ctypes.Structure):
+    """struct SbNgramLm of include/speech_b200.h: device tables of an n-gram LM"""
+    _fields_ = [("keys", _vp), ("vals", _vp), ("logp", _vp), ("bow", _vp), ("tok", _vp),
+                ("cap", _c_int), ("order", _c_int), ("num_classes", _c_int), ("bos", _c_int),
+                ("blank", _c_int),
+                ("lm_upper", ctypes.c_double), ("lm_abs", ctypes.c_double)]
+
+
+_lmp = ctypes.POINTER(SbNgramLm)
+_db = ctypes.c_double
+
 # name -> (restype, argtypes): every symbol include/speech_b200.h declares
 SIGNATURES = {
     "sb_version": (_c_int, []),
@@ -34,6 +46,13 @@ SIGNATURES = {
                                     _vp, _c_sz, _vp]),
     "sb_ctc_prefix_beam_shortlist": (_c_int, [_vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int,
                                               _vp, _vp, _vp, _vp, _c_sz, _vp]),
+    "sb_ctc_prefix_beam_lm_workspace_size": (_c_int, [_c_int, _c_int, _c_int, _c_int,
+                                                      ctypes.POINTER(_c_sz)]),
+    "sb_ctc_prefix_beam_lm": (_c_int, [_vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int, _lmp, _db,
+                                       _db, _vp, _vp, _vp, _vp, _c_sz, _vp]),
+    "sb_ctc_prefix_beam_lm_shortlist": (_c_int, [_vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int,
+                                                 _lmp, _db, _db, _vp, _vp, _vp, _vp, _c_sz, _vp]),
+    "sb_debug_ctc_lm_rescans": (_c_int, [ctypes.POINTER(ctypes.c_ulonglong)]),
     "sb_conv_im2col": (_c_int, [_vp, _vp, _fl, _vp, _c_int, _c_int, _c_int, _c_int, _c_int, _c_int,
                                 _c_int, _c_int, _c_int, _vp]),
     "sb_conv_relu_to_bct": (_c_int, [_vp, _vp, _fl, _vp, _c_int, _c_int, _c_int, _c_int, _vp]),

@@ -58,9 +58,91 @@ struct Beam {
   int size;
 };
 
+// ------------------------------------------------------------------------------------------------
+// Shallow fusion.  The search is written once over a policy that gives the value q an extension
+// of beam entry i by symbol s scores with, from the acoustic log-probability p = p_s:
+//   NoFuse  q = p (the LM-less search, its arithmetic untouched);
+//   LmFuse  q = p + (alpha * lm(s | ctx_i) + beta), lm the backoff lookup of SbNgramLm.
+// Entry i's context is its last order-1 symbols, kept most recent first in LmShared::hist (-1
+// stands for <s>, before which there is nothing).  Once per frame each entry walks the context
+// trie along them (lm_resolve); a candidate's lookup is then at most `order` probes.
+// ------------------------------------------------------------------------------------------------
+struct NoFuse {
+  static constexpr bool kLm = false;
+  static constexpr int kMinBlocks = 0;
+  __device__ __forceinline__ double q(int, int, double p) const { return p; }
+};
+
+struct LmShared {
+  int hist[2][DEC_MAX_BEAM][SB_LM_MAX_ORDER - 1];  // per beam buffer (t & 1) and entry
+  int ctx[DEC_MAX_BEAM][SB_LM_MAX_ORDER];          // context nodes, [0] = root .. [depth]
+  int depth[DEC_MAX_BEAM];
+};
+__device__ __forceinline__ LmShared& lm_shared() {
+  __shared__ LmShared sh;
+  return sh;
+}
+
+__device__ __forceinline__ int lm_find(const SbNgramLm& lm, int node, int tok, int kind) {
+  const unsigned long long key = ((unsigned long long)(unsigned int)node << 32) |
+                                 ((unsigned long long)(unsigned int)(tok + 1) << 1) |
+                                 (unsigned long long)kind;
+  unsigned int h = (unsigned int)((key * 0x9E3779B97F4A7C15ull) >> 32) & (lm.cap - 1);
+  for (int probe = 0; probe < lm.cap; ++probe) {
+    const unsigned long long k = __ldg(lm.keys + h);
+    if (k == key) return __ldg(lm.vals + h);
+    if (k == 0ull) return -1;
+    h = (h + 1) & (lm.cap - 1);
+  }
+  return -1;
+}
+
+struct LmFuse {
+  static constexpr bool kLm = true;
+  static constexpr int kMinBlocks = 1;
+  SbNgramLm lm;
+  double alpha, beta;
+
+  // lm(s | ctx_i): the longest stored context first, adding the backoff of each that misses
+  __device__ __forceinline__ double lm_logp(int i, int s) const {
+    const LmShared& sh = lm_shared();
+    const int t = __ldg(lm.tok + s);
+    double acc = 0.0;
+    for (int d = sh.depth[i]; d >= 0; --d) {
+      const int c = sh.ctx[i][d];
+      const int g = lm_find(lm, c, t, 1);
+      if (g >= 0) return acc + __ldg(lm.logp + g);
+      acc += __ldg(lm.bow + c);
+    }
+    return acc;   // not reached: every non-blank class maps to a token with a unigram
+  }
+  __device__ __forceinline__ double q(int i, int s, double p) const {
+    return p + (alpha * lm_logp(i, s) + beta);
+  }
+};
+
+// entry i of the beam in buffer par: its context nodes, thread i for i < nb; the caller syncs
+__device__ __forceinline__ void lm_resolve(const LmFuse& fu, int par, int nb) {
+  LmShared& sh = lm_shared();
+  const int i = threadIdx.x;
+  if (i >= nb) return;
+  int c = 0, d = 0;
+  sh.ctx[i][0] = 0;
+  for (int k = 0; k < fu.lm.order - 1; ++k) {
+    const int h = sh.hist[par][i][k];
+    const int nc = lm_find(fu.lm, c, h < 0 ? fu.lm.bos : __ldg(fu.lm.tok + h), 0);
+    if (nc < 0) break;
+    c = nc;
+    sh.ctx[i][++d] = c;
+    if (h < 0) break;
+  }
+  sh.depth[i] = d;
+}
+
 // value of the candidate "beam entry j keeps its prefix" at this frame
+template <class Fuse>
 __device__ void stay_value(const Beam& bm, int j, const float* lp, int blank, int K, double& npb,
-                           double& npnb, int& rank) {
+                           double& npnb, int& rank, const Fuse& fu) {
   const double pblank = (double)lp[blank];
   npb = lse3d(d_neg_inf(), bm.pb[j] + pblank, bm.pnb[j] + pblank);
   npnb = d_neg_inf();
@@ -76,12 +158,13 @@ __device__ void stay_value(const Beam& bm, int j, const float* lp, int blank, in
     if (pi >= 0) {
       const int par_rank = s * 2 * K + 2 * pi;
       const bool rep = (bm.last[pi] == s);
+      const double q = fu.q(pi, s, p);     // the parent's extension by s
       if (pi < j) {
-        npnb = rep ? lse2d(npnb, bm.pb[pi] + p) : lse3d(npnb, bm.pb[pi] + p, bm.pnb[pi] + p);
+        npnb = rep ? lse2d(npnb, bm.pb[pi] + q) : lse3d(npnb, bm.pb[pi] + q, bm.pnb[pi] + q);
         npnb = lse2d(npnb, bm.pnb[j] + p);
       } else {
         npnb = lse2d(npnb, bm.pnb[j] + p);
-        npnb = rep ? lse2d(npnb, bm.pb[pi] + p) : lse3d(npnb, bm.pb[pi] + p, bm.pnb[pi] + p);
+        npnb = rep ? lse2d(npnb, bm.pb[pi] + q) : lse3d(npnb, bm.pb[pi] + q, bm.pnb[pi] + q);
       }
       rank = min(rank, min(self_rank, par_rank));
     } else {
@@ -93,13 +176,14 @@ __device__ void stay_value(const Beam& bm, int j, const float* lp, int blank, in
 
 // value of the candidate "beam entry i extended by symbol s" (s != blank); returns false when the
 // extended prefix is already a beam entry (then it is accounted for by that entry's stay_value)
+template <class Fuse>
 __device__ bool ext_value(const Beam& bm, int i, int s, const float* lp, int K, double& npnb,
-                          int& rank) {
+                          int& rank, const Fuse& fu) {
   for (int j = 0; j < bm.size; ++j)
     if (bm.last[j] == s && bm.parent[j] == bm.node[i] && bm.node[j] != 0) return false;
-  const double p = (double)lp[s];
-  if (s != bm.last[i]) npnb = lse3d(d_neg_inf(), bm.pb[i] + p, bm.pnb[i] + p);
-  else npnb = lse2d(d_neg_inf(), bm.pb[i] + p);
+  const double q = fu.q(i, s, (double)lp[s]);
+  if (s != bm.last[i]) npnb = lse3d(d_neg_inf(), bm.pb[i] + q, bm.pnb[i] + q);
+  else npnb = lse2d(d_neg_inf(), bm.pb[i] + q);
   rank = s * 2 * K + 2 * i;
   return true;
 }
@@ -107,8 +191,9 @@ __device__ bool ext_value(const Beam& bm, int i, int s, const float* lp, int K, 
 // Candidate c of a frame, numbered as the full scan numbers them: c < K*S is "entry c / S extended
 // by symbol c % S", c = K*S + j is "entry j keeps its prefix".  Returns false for a candidate that
 // does not exist (no such entry, the blank as an extension, or an extension that is a beam entry).
+template <class Fuse>
 __device__ __forceinline__ bool cand_value(const Beam& cur, int c, const float* lp, int K, int S,
-                                           int blank, double& sc, int& rk) {
+                                           int blank, double& sc, int& rk, const Fuse& fu) {
   sc = d_neg_inf();
   rk = 0x7fffffff;
   const int nb = cur.size;
@@ -116,7 +201,7 @@ __device__ __forceinline__ bool cand_value(const Beam& cur, int c, const float* 
     const int i = c / S, s = c - i * S;
     if (i < nb && s != blank) {
       double x;
-      const bool ok = ext_value(cur, i, s, lp, K, x, rk);
+      const bool ok = ext_value(cur, i, s, lp, K, x, rk, fu);
       if (ok) sc = x;  // logsumexp(-inf, x) == x exactly
       return ok;
     }
@@ -125,7 +210,7 @@ __device__ __forceinline__ bool cand_value(const Beam& cur, int c, const float* 
   const int j = c - K * S;
   if (j >= nb) return false;
   double npb, npnb;
-  stay_value(cur, j, lp, blank, K, npb, npnb, rk);
+  stay_value(cur, j, lp, blank, K, npb, npnb, rk, fu);
   sc = lse2d(npb, npnb);
   return true;
 }
@@ -148,6 +233,7 @@ __device__ __forceinline__ int dec_take_first(const double* score, const int* ra
   return bc;
 }
 
+template <class Fuse>
 __device__ __forceinline__ void dec_begin(const DecParams& p, Beam* beams) {
   if (threadIdx.x == 0) {
     beams[0].size = 1;
@@ -156,35 +242,58 @@ __device__ __forceinline__ void dec_begin(const DecParams& p, Beam* beams) {
     beams[0].node[0] = 0;
     beams[0].last[0] = -1;
     beams[0].parent[0] = -1;
+    if constexpr (Fuse::kLm) lm_shared().hist[0][0][0] = -1;   // the empty prefix: <s>
   }
   p.trie.of(blockIdx.x).clear<DEC_THREADS>();
 }
 
+// Start of frame t over the beam cur: with an LM, every entry's context nodes.
+template <class Fuse>
+__device__ __forceinline__ void dec_frame(const Fuse& fu, const Beam& cur, int t) {
+  if constexpr (Fuse::kLm) {
+    lm_resolve(fu, t & 1, cur.size);
+    __syncthreads();
+  }
+}
+
 // Materialise the pruned beam of frame t: thread r < ns holds the r-th selected candidate in `mine`
-// (full-scan numbering).
+// (full-scan numbering).  With an LM, an extension's context is its parent's shifted by one symbol
+// and an entry that stays copies its own.
+template <class Fuse>
 __device__ __forceinline__ void dec_commit(const DecParams& p, const Beam& cur, Beam& nxt, int mine,
-                                           int ns, const float* lp, int t) {
+                                           int ns, const float* lp, int t, const Fuse& fu) {
   const int tid = threadIdx.x, K = p.K, S = p.S;
   if (tid < ns) {
     const int c = mine;
     if (c < K * S) {
       const int i = c / S, s = c - i * S;
       double x; int rk;
-      ext_value(cur, i, s, lp, K, x, rk);
+      ext_value(cur, i, s, lp, K, x, rk, fu);
       nxt.pb[tid] = d_neg_inf();
       nxt.pnb[tid] = x;
       nxt.node[tid] = p.trie.of(blockIdx.x).find_or_insert<true>(cur.node[i], s, 1 + t * K + tid);
       nxt.last[tid] = s;
       nxt.parent[tid] = cur.node[i];
+      if constexpr (Fuse::kLm) {
+        LmShared& sh = lm_shared();
+        const int par = t & 1;
+        for (int k = fu.lm.order - 2; k > 0; --k) sh.hist[par ^ 1][tid][k] = sh.hist[par][i][k - 1];
+        if (fu.lm.order > 1) sh.hist[par ^ 1][tid][0] = s;
+      }
     } else {
       const int j = c - K * S;
       double npb, npnb; int rk;
-      stay_value(cur, j, lp, p.blank, K, npb, npnb, rk);
+      stay_value(cur, j, lp, p.blank, K, npb, npnb, rk, fu);
       nxt.pb[tid] = npb;
       nxt.pnb[tid] = npnb;
       nxt.node[tid] = cur.node[j];
       nxt.last[tid] = cur.last[j];
       nxt.parent[tid] = cur.parent[j];
+      if constexpr (Fuse::kLm) {
+        LmShared& sh = lm_shared();
+        const int par = t & 1;
+        for (int k = 0; k < fu.lm.order - 1; ++k) sh.hist[par ^ 1][tid][k] = sh.hist[par][j][k];
+      }
     }
   }
   if (tid == 0) nxt.size = ns;
@@ -200,7 +309,11 @@ __device__ __forceinline__ void dec_finish(const DecParams& p, const Beam& fin) 
   }
 }
 
-__global__ void __launch_bounds__(DEC_THREADS) ctc_prefix_beam_kernel(const DecParams p) {
+// kMinBlocks: 0 leaves the LM-less kernel's register allocation as it was; 1 lets the LM kernel
+// use 70 registers instead of 56 and an 8-byte spill (one CTA per utterance either way).
+template <class Fuse>
+__global__ void __launch_bounds__(DEC_THREADS, Fuse::kMinBlocks) ctc_prefix_beam_kernel(
+    const DecParams p, const Fuse fu) {
   extern __shared__ unsigned char dec_smem[];
   const int b = blockIdx.x, tid = threadIdx.x;
   const int K = p.K, S = p.S, T = min(p.lens[b], p.T);
@@ -210,18 +323,19 @@ __global__ void __launch_bounds__(DEC_THREADS) ctc_prefix_beam_kernel(const DecP
   unsigned char* live = reinterpret_cast<unsigned char*>(rank + ncand);  // [ncand]
   __shared__ Beam beams[2];
 
-  dec_begin(p, beams);
+  dec_begin<Fuse>(p, beams);
   const float* logp = p.logp + (size_t)b * p.T * S;
 
   for (int t = 0; t < T; ++t) {
     const Beam& cur = beams[t & 1];
     Beam& nxt = beams[(t & 1) ^ 1];
     const float* lp = logp + (size_t)t * S;
+    dec_frame(fu, cur, t);
     // ---- 1. score every candidate ----
     for (int c = tid; c < ncand; c += DEC_THREADS) {
       double sc;
       int rk;
-      live[c] = cand_value(cur, c, lp, K, S, p.blank, sc, rk) ? 1 : 0;
+      live[c] = cand_value(cur, c, lp, K, S, p.blank, sc, rk, fu) ? 1 : 0;
       score[c] = sc;
       rank[c] = rk;
     }
@@ -237,7 +351,7 @@ __global__ void __launch_bounds__(DEC_THREADS) ctc_prefix_beam_kernel(const DecP
       ++ns;
     }
     // ---- 3. materialise the pruned beam ----
-    dec_commit(p, cur, nxt, mine, ns, lp, t);
+    dec_commit(p, cur, nxt, mine, ns, lp, t, fu);
   }
   dec_finish(p, beams[T & 1]);
 }
@@ -267,10 +381,25 @@ __global__ void __launch_bounds__(DEC_THREADS) ctc_prefix_beam_kernel(const DecP
 // candidates, each round taking the best candidate after the previous one.  Both ways select the
 // full scan's K candidates in its order, with the same ext_value / stay_value arithmetic.
 //
+// With an LM the extension of i by s scores f_i(q_s), q_s = p_s + (alpha * lm(s | ctx_i) + beta),
+// and the order of the p_s no longer orders the q_s, so the short list is only a guess; the check
+// is what keeps the search exact.  For a left-out symbol, alpha >= 0 and lm(s | ctx_i) <= lm_upper
+// give q_s <= q_max = p_min + (alpha * lm_upper + beta) in exact arithmetic, and U = max_i f_i(q_max)
+// as computed.  Rounding now enters through every term of q as well (a lookup sums at most
+// order + 1 values, each of magnitude <= lm_abs; then one product and two sums), so the margin is
+//     1e-12 * (1 + |U| + |p_min| + alpha * lm_abs + |beta|),
+// which bounds the magnitude of every operand on the way to f and U; the rounding error of the
+// twenty-odd operations in between is below 1e-14 times it.  When p_min = -inf every left-out q_s
+// is -inf exactly (the LM terms are finite), so U = -inf keeps its meaning.  A frame the check
+// cannot prove is rescanned as above, with the same fused arithmetic.
+//
 // The shortlist of every frame (2K + 1 ints, or S - 1 if fewer) comes from a pre-pass over the
 // B*T rows (ctc_shortlist_kernel, one CTA per frame).
 // ------------------------------------------------------------------------------------------------
 static constexpr int DEC_SL_THREADS = 256;
+
+// frames the LM-fused shortlist search rescanned (sb_debug_ctc_lm_rescans)
+__device__ unsigned long long dec_lm_rescans;
 
 // grid (T, B): shortlist[(b*T + t)*LS + j], j < L, for the frames t < lens[b]
 __global__ void __launch_bounds__(DEC_SL_THREADS) ctc_shortlist_kernel(
@@ -298,8 +427,9 @@ __global__ void __launch_bounds__(DEC_SL_THREADS) ctc_shortlist_kernel(
   }
 }
 
+template <class Fuse>
 __global__ void __launch_bounds__(DEC_THREADS, 1) ctc_prefix_beam_shortlist_kernel(
-    const DecParams p, const int* __restrict__ shortlist, int L, int LS) {
+    const DecParams p, const int* __restrict__ shortlist, int L, int LS, const Fuse fu) {
   extern __shared__ unsigned char dec_smem[];
   const int b = blockIdx.x, tid = threadIdx.x;
   const int K = p.K, S = p.S, T = min(p.lens[b], p.T);
@@ -313,7 +443,7 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) ctc_prefix_beam_shortlist_kern
   __shared__ int rescan;
   const bool complete = L >= S - 1;        // every non-blank symbol is on the list
 
-  dec_begin(p, beams);
+  dec_begin<Fuse>(p, beams);
   const float* logp = p.logp + (size_t)b * p.T * S;
 
   for (int t = 0; t < T; ++t) {
@@ -322,6 +452,7 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) ctc_prefix_beam_shortlist_kern
     const float* lp = logp + (size_t)t * S;
     const int* sl = shortlist + ((size_t)b * p.T + t) * LS;
     const int nb = cur.size;
+    dec_frame(fu, cur, t);
     // ---- 1. score the shortlisted candidates ----
     for (int c = tid; c < ncand; c += DEC_THREADS) {
       double sc = d_neg_inf();
@@ -337,12 +468,12 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) ctc_prefix_beam_shortlist_kern
           }
           if (s >= 0 && s != p.blank) {
             fc = i * S + s;
-            ok = cand_value(cur, fc, lp, K, S, p.blank, sc, rk);
+            ok = cand_value(cur, fc, lp, K, S, p.blank, sc, rk, fu);
           }
         }
       } else {
         fc = K * S + (c - K * per);
-        ok = cand_value(cur, fc, lp, K, S, p.blank, sc, rk);
+        ok = cand_value(cur, fc, lp, K, S, p.blank, sc, rk, fu);
       }
       score[c] = sc;
       rank[c] = rk;
@@ -367,18 +498,28 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) ctc_prefix_beam_shortlist_kern
     // ---- 3. check that no left-out candidate can reach the selection ----
     if (!complete && tid < 32) {
       const double pmin = (double)lp[sl[L - 1]];
+      double qmax = pmin;
+      if constexpr (Fuse::kLm) qmax = pmin + (fu.alpha * fu.lm.lm_upper + fu.beta);
       double U = d_neg_inf();
-      if (tid < nb) U = lse3d(d_neg_inf(), cur.pb[tid] + pmin, cur.pnb[tid] + pmin);
+      if (tid < nb) U = lse3d(d_neg_inf(), cur.pb[tid] + qmax, cur.pnb[tid] + qmax);
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) U = fmax(U, __shfl_xor_sync(0xffffffffu, U, o));
       if (tid == 0) {
         bool ok = ns == K && last_s != d_neg_inf();
-        if (ok && U != d_neg_inf()) ok = last_s > U + 1e-12 * (1.0 + fabs(U));
+        if (ok && U != d_neg_inf()) {
+          if constexpr (Fuse::kLm)
+            ok = last_s > U + 1e-12 * (1.0 + fabs(U) + fabs(pmin) + fu.alpha * fu.lm.lm_abs +
+                                       fabs(fu.beta));
+          else
+            ok = last_s > U + 1e-12 * (1.0 + fabs(U));
+        }
         rescan = ok ? 0 : 1;
       }
     }
     __syncthreads();
     // ---- 3b. otherwise: full streamed scan of this frame ----
+    if constexpr (Fuse::kLm)
+      if (!complete && rescan && tid == 0) atomicAdd(&dec_lm_rescans, 1ull);
     if (!complete && rescan) {
       ns = 0;
       for (int r = 0; r < K; ++r) {
@@ -387,7 +528,7 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) ctc_prefix_beam_shortlist_kern
         for (int c = tid; c < K * S + K; c += DEC_THREADS) {
           double sc;
           int rk;
-          if (!cand_value(cur, c, lp, K, S, p.blank, sc, rk)) continue;
+          if (!cand_value(cur, c, lp, K, S, p.blank, sc, rk, fu)) continue;
           if (r > 0 && !beam_order(last_s, last_r, sc, rk)) continue;   // selected earlier
           if (beam_before(sc, rk, bs, br)) { bs = sc; br = rk; bc = c; }
         }
@@ -400,7 +541,7 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) ctc_prefix_beam_shortlist_kern
       }
     }
     // ---- 4. materialise the pruned beam ----
-    dec_commit(p, cur, nxt, mine, ns, lp, t);
+    dec_commit(p, cur, nxt, mine, ns, lp, t, fu);
   }
   dec_finish(p, beams[T & 1]);
 }
@@ -427,9 +568,14 @@ static size_t dec_full_smem(int S, int K) {
   return (size_t)(K * S + K) * (sizeof(double) + sizeof(int) + 1) + 16;
 }
 
+// Both routes with the fusion policy fu.  Every shape whose K*S + K full-scan candidates fit in
+// 200 KB of shared memory takes the full scan; the static shared memory of either instantiation
+// (5.8 KB at most, with the LM's contexts) leaves both sizes below the per-block limit.
+template <class Fuse>
 static int dec_entry(const float* logp, const int* lens, int B, int T, int S, int beam_size,
                      int blank, int* out_labels, int* out_lens, double* out_scores,
-                     void* workspace, size_t workspace_bytes, void* stream_, bool force_shortlist) {
+                     void* workspace, size_t workspace_bytes, void* stream_, bool force_shortlist,
+                     const Fuse& fu) {
   if (!logp || !lens || !out_labels || !out_lens || !out_scores || !workspace) return SB_ERR_INVALID;
   if (B <= 0 || T <= 0 || S <= 0 || blank < 0 || blank >= S || beam_size <= 0) return SB_ERR_INVALID;
   if (beam_size > DEC_MAX_BEAM) return SB_ERR_UNSUPPORTED;
@@ -454,11 +600,12 @@ static int dec_entry(const float* logp, const int* lens, int B, int T, int S, in
   const size_t full_smem = dec_full_smem(S, beam_size);
   if (!force_shortlist && full_smem <= 200 * 1024) {
     if (full_smem > 40 * 1024) {
-      if (cudaFuncSetAttribute(ctc_prefix_beam_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+      if (cudaFuncSetAttribute(ctc_prefix_beam_kernel<Fuse>,
+                               cudaFuncAttributeMaxDynamicSharedMemorySize,
                                (int)full_smem) != cudaSuccess)
         return SB_ERR_CUDA;
     }
-    ctc_prefix_beam_kernel<<<B, DEC_THREADS, full_smem, stream>>>(p);
+    ctc_prefix_beam_kernel<Fuse><<<B, DEC_THREADS, full_smem, stream>>>(p, fu);
     return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
   }
 
@@ -469,14 +616,14 @@ static int dec_entry(const float* logp, const int* lens, int B, int T, int S, in
   const int ncand = beam_size * (L + 1) + beam_size;
   const size_t smem = (size_t)ncand * (sizeof(double) + 2 * sizeof(int) + 1) + 16;
   if (smem > 40 * 1024) {
-    if (cudaFuncSetAttribute(ctc_prefix_beam_shortlist_kernel,
+    if (cudaFuncSetAttribute(ctc_prefix_beam_shortlist_kernel<Fuse>,
                              cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
       return SB_ERR_CUDA;
   }
   if (L > 0)
     ctc_shortlist_kernel<<<dim3(T, B), DEC_SL_THREADS, 0, stream>>>(logp, lens, shortlist, T, S,
                                                                      blank, L, LS);
-  ctc_prefix_beam_shortlist_kernel<<<B, DEC_THREADS, smem, stream>>>(p, shortlist, L, LS);
+  ctc_prefix_beam_shortlist_kernel<Fuse><<<B, DEC_THREADS, smem, stream>>>(p, shortlist, L, LS, fu);
   return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
 }
 
@@ -485,7 +632,7 @@ extern "C" int sb_ctc_prefix_beam(const float* logp, const int* lens, int B, int
                                   double* out_scores, void* workspace, size_t workspace_bytes,
                                   void* stream) {
   return dec_entry(logp, lens, B, T, S, beam_size, blank, out_labels, out_lens, out_scores,
-                   workspace, workspace_bytes, stream, false);
+                   workspace, workspace_bytes, stream, false, NoFuse{});
 }
 
 extern "C" int sb_ctc_prefix_beam_shortlist(const float* logp, const int* lens, int B, int T,
@@ -493,5 +640,60 @@ extern "C" int sb_ctc_prefix_beam_shortlist(const float* logp, const int* lens, 
                                             int* out_lens, double* out_scores, void* workspace,
                                             size_t workspace_bytes, void* stream) {
   return dec_entry(logp, lens, B, T, S, beam_size, blank, out_labels, out_lens, out_scores,
-                   workspace, workspace_bytes, stream, true);
+                   workspace, workspace_bytes, stream, true, NoFuse{});
+}
+
+// The LM needs no workspace of its own: each entry's context lives in shared memory.
+extern "C" int sb_ctc_prefix_beam_lm_workspace_size(int B, int T, int K, int order,
+                                                    size_t* bytes) {
+  if (order < 1) return SB_ERR_INVALID;
+  if (order > SB_LM_MAX_ORDER) return SB_ERR_UNSUPPORTED;
+  return sb_ctc_prefix_beam_workspace_size(B, T, K, bytes);
+}
+
+static int dec_lm_entry(const float* logp, const int* lens, int B, int T, int S, int beam_size,
+                        int blank, const SbNgramLm* lm, double lm_weight, double insertion_bonus,
+                        int* out_labels, int* out_lens, double* out_scores, void* workspace,
+                        size_t workspace_bytes, void* stream, bool force_shortlist) {
+  if (!lm || !lm->keys || !lm->vals || !lm->logp || !lm->bow || !lm->tok) return SB_ERR_INVALID;
+  if (!(lm_weight >= 0.0) || !isfinite(lm_weight) || !isfinite(insertion_bonus))
+    return SB_ERR_INVALID;
+  if (!isfinite(lm->lm_upper) || !isfinite(lm->lm_abs) || lm->num_classes < S) return SB_ERR_INVALID;
+  if (lm->blank != blank) return SB_ERR_INVALID;
+  if (lm->cap <= 0 || (lm->cap & (lm->cap - 1)) || lm->order < 1) return SB_ERR_INVALID;
+  if (lm->order > SB_LM_MAX_ORDER) return SB_ERR_UNSUPPORTED;
+  LmFuse fu;
+  fu.lm = *lm;
+  fu.alpha = lm_weight;
+  fu.beta = insertion_bonus;
+  return dec_entry(logp, lens, B, T, S, beam_size, blank, out_labels, out_lens, out_scores,
+                   workspace, workspace_bytes, stream, force_shortlist, fu);
+}
+
+extern "C" int sb_ctc_prefix_beam_lm(const float* logp, const int* lens, int B, int T, int S,
+                                     int beam_size, int blank, const SbNgramLm* lm,
+                                     double lm_weight, double insertion_bonus, int* out_labels,
+                                     int* out_lens, double* out_scores, void* workspace,
+                                     size_t workspace_bytes, void* stream) {
+  return dec_lm_entry(logp, lens, B, T, S, beam_size, blank, lm, lm_weight, insertion_bonus,
+                      out_labels, out_lens, out_scores, workspace, workspace_bytes, stream, false);
+}
+
+extern "C" int sb_ctc_prefix_beam_lm_shortlist(const float* logp, const int* lens, int B, int T,
+                                               int S, int beam_size, int blank,
+                                               const SbNgramLm* lm, double lm_weight,
+                                               double insertion_bonus, int* out_labels,
+                                               int* out_lens, double* out_scores, void* workspace,
+                                               size_t workspace_bytes, void* stream) {
+  return dec_lm_entry(logp, lens, B, T, S, beam_size, blank, lm, lm_weight, insertion_bonus,
+                      out_labels, out_lens, out_scores, workspace, workspace_bytes, stream, true);
+}
+
+extern "C" int sb_debug_ctc_lm_rescans(unsigned long long* frames) {
+  if (!frames) return SB_ERR_INVALID;
+  const unsigned long long zero = 0;
+  if (cudaMemcpyFromSymbol(frames, dec_lm_rescans, sizeof(zero)) != cudaSuccess ||
+      cudaMemcpyToSymbol(dec_lm_rescans, &zero, sizeof(zero)) != cudaSuccess)
+    return SB_ERR_CUDA;
+  return SB_OK;
 }

@@ -1,0 +1,384 @@
+"""Token-level backoff n-gram language model for shallow fusion in the CTC prefix beam search.
+
+The LM is over the acoustic model's own output classes (characters or subword units); the blank is
+never an LM token.  Orders 1..10, with a sentence start <s>, an end </s> and optionally <unk>.
+Values are held as the ARPA file's log10 numbers and converted once to natural log
+(`v10 * math.log(10)`) for lookup, so `from_arpa(to_arpa(lm))` reproduces every float64 value.
+
+    lm = NGramLM.from_arpa("chars.arpa", preproc.int_to_char)    # blank = last class
+    lm = NGramLM.train(transcripts, order=5, num_classes=V + 1, blank=V)
+    model.infer(batch, beam_size=8, lm=lm, lm_weight=0.8, insertion_bonus=1.5)
+
+lm(s | h) follows ARPA backoff: h is the prefix's last order-1 symbols, preceded by <s> where the
+prefix is shorter; when the n-gram (h, s) is stored its log-probability is used, otherwise the
+backoff weight of h (0 when h is not stored) is added and the oldest context token dropped.
+A class the LM does not know reads as <unk>.
+
+Device tables (csrc/decode.cu, SbNgramLm in include/speech_b200.h): one open-addressed map with
+two kinds of key, (context node, older token) -> context node and (context node, token) ->
+n-gram, over a trie of contexts read most recent token first.  They are built once and cached
+per device.
+"""
+import math
+from collections import Counter, defaultdict
+from collections.abc import Mapping
+
+import numpy as np
+
+LN10 = math.log(10.0)
+MAX_ORDER = 10
+BOS, EOS, UNK = "<s>", "</s>", "<unk>"
+_HASH_MUL = 0x9E3779B97F4A7C15
+_MASK64 = (1 << 64) - 1
+
+
+def _finite(v, what):
+    if not math.isfinite(v):
+        raise ValueError("n-gram LM: non-finite value %r in %s" % (v, what))
+    return v
+
+
+def _check_order(order):
+    if not isinstance(order, (int, np.integer)) or not 1 <= order <= MAX_ORDER:
+        raise ValueError("n-gram LM: order must be in 1..%d, got %r" % (MAX_ORDER, order))
+    return int(order)
+
+
+def _class_names(symbols, blank, num_classes):
+    """{class: symbol} of the non-blank classes, validated"""
+    names = {}
+    seen = {BOS: None, EOS: None, UNK: None}
+    for c in range(num_classes):
+        if c == blank:
+            continue
+        s = symbols[c] if symbols is not None else str(c)
+        if not isinstance(s, str) or s == "" or any(ch.isspace() for ch in s):
+            raise ValueError("n-gram LM: symbol %r of class %d is empty or has whitespace" % (s, c))
+        if s in seen:
+            raise ValueError("n-gram LM: symbol %r of class %d is a duplicate or reserved" % (s, c))
+        seen[s] = c
+        names[c] = s
+    return names
+
+
+def _as_list(symbols):
+    """symbols as a list indexed by class: a sequence, or a mapping class -> symbol (such as the
+    reference Preprocessor.int_to_char) with keys 0 .. len - 1"""
+    if isinstance(symbols, Mapping):
+        try:
+            return [symbols[c] for c in range(len(symbols))]
+        except KeyError:
+            raise ValueError("n-gram LM: a symbol mapping needs the keys 0 .. %d"
+                             % (len(symbols) - 1)) from None
+    return list(symbols)
+
+
+def _layout(symbols, blank):
+    """(num_classes, blank) of a symbol list: classes 0.. len(symbols) - 1, and the blank either
+    one of them (its entry is ignored) or, by default, the class after the last (CTC's convention)"""
+    symbols = _as_list(symbols)
+    if blank is None:
+        blank = len(symbols)
+    if not 0 <= blank <= len(symbols):
+        raise ValueError("n-gram LM: blank %r outside 0..%d" % (blank, len(symbols)))
+    return (len(symbols) + 1 if blank == len(symbols) else len(symbols)), int(blank), symbols
+
+
+class NGramLM:
+    """Backoff n-gram LM over class ids.  Tokens: class c -> c, <s> -> C, </s> -> C + 1,
+    <unk> -> C + 2 (C = num_classes).  Build with from_arpa or train."""
+
+    def __init__(self, order, num_classes, blank, ngrams):
+        # ngrams[n]: {token tuple: (log10 prob, log10 backoff or None)}, n = 1..order
+        self._order = order
+        self._num_classes = num_classes
+        self._blank = blank
+        self._ngrams = ngrams
+        self._bos, self._eos, self._unk = num_classes, num_classes + 1, num_classes + 2
+        uni = ngrams[1]
+        tok = np.full(num_classes, -1, np.int32)
+        for c in range(num_classes):
+            if c == blank:
+                continue
+            if (c,) in uni:
+                tok[c] = c
+            elif (self._unk,) in uni:
+                tok[c] = self._unk
+            else:
+                raise ValueError("n-gram LM: class %d is not in the LM and it has no %s" % (c, UNK))
+        self._tok = tok
+        self._host = None
+        self._dev = {}
+
+    @property
+    def order(self):
+        return self._order
+
+    @property
+    def num_classes(self):
+        return self._num_classes
+
+    @property
+    def blank(self):
+        return self._blank
+
+    # ------------------------------------------------------------------------------------------
+    # ARPA
+    # ------------------------------------------------------------------------------------------
+    @classmethod
+    def from_arpa(cls, path, symbols, blank=None):
+        """Read an ARPA file.  symbols[c] is the token string of class c (e.g. the reference
+        Preprocessor.int_to_char in id order); blank defaults to the class after the last symbol.
+        n-grams over words that are neither a class symbol nor <s>, </s>, <unk> are dropped."""
+        num_classes, blank, symbols = _layout(symbols, blank)
+        names = _class_names(symbols, blank, num_classes)
+        word_tok = {s: c for c, s in names.items()}
+        word_tok.update({BOS: num_classes, EOS: num_classes + 1, UNK: num_classes + 2})
+        with open(path, "r", encoding="utf-8") as fh:
+            lines = [ln.strip() for ln in fh]
+        lines = [ln for ln in lines if ln]
+        try:
+            i = lines.index("\\data\\")
+        except ValueError:
+            raise ValueError("n-gram LM: %s has no \\data\\ section" % path) from None
+        i += 1
+        counts = {}
+        while i < len(lines) and lines[i].startswith("ngram "):
+            key, _, val = lines[i][6:].partition("=")
+            try:
+                counts[int(key)] = int(val)
+            except ValueError:
+                raise ValueError("n-gram LM: bad count line %r" % lines[i]) from None
+            i += 1
+        if not counts:
+            raise ValueError("n-gram LM: %s declares no n-gram counts" % path)
+        order = max(counts)
+        _check_order(order)
+        if sorted(counts) != list(range(1, order + 1)) or any(v < 0 for v in counts.values()):
+            raise ValueError("n-gram LM: counts must be given for orders 1..%d" % order)
+        ngrams = {n: {} for n in range(1, order + 1)}
+        for n in range(1, order + 1):
+            header = "\\%d-grams:" % n
+            if i >= len(lines) or lines[i] != header:
+                raise ValueError("n-gram LM: missing section %s" % header)
+            i += 1
+            for _ in range(counts[n]):
+                if i >= len(lines) or lines[i].startswith("\\"):
+                    raise ValueError("n-gram LM: section %s has fewer than %d entries"
+                                     % (header, counts[n]))
+                f = lines[i].split()
+                i += 1
+                if len(f) not in (n + 1, n + 2):
+                    raise ValueError("n-gram LM: malformed %d-gram line %r" % (n, " ".join(f)))
+                try:
+                    p = float(f[0])
+                    b = float(f[n + 1]) if len(f) == n + 2 else None
+                except ValueError:
+                    raise ValueError("n-gram LM: malformed number in %r" % " ".join(f)) from None
+                _finite(p, "a %d-gram probability" % n)
+                if b is not None:
+                    _finite(b, "a %d-gram backoff" % n)
+                words = f[1:n + 1]
+                if any(w not in word_tok for w in words):
+                    continue
+                g = tuple(word_tok[w] for w in words)
+                if g in ngrams[n]:
+                    raise ValueError("n-gram LM: duplicate %d-gram %r" % (n, " ".join(words)))
+                ngrams[n][g] = (p, b)
+        if i >= len(lines) or lines[i] != "\\end\\":
+            raise ValueError("n-gram LM: %s: expected \\end\\ after the %d-grams (wrong counts?)"
+                             % (path, order))
+        return cls(order, num_classes, blank, ngrams)
+
+    def to_arpa(self, path, symbols=None):
+        """Write an ARPA file; str(c) names class c unless symbols are given (same layout as
+        from_arpa).  Values are written with repr, which reads back to the same float64."""
+        if symbols is not None:
+            symbols = _as_list(symbols)
+        if symbols is not None and len(symbols) < self._num_classes - (
+                self._blank == self._num_classes - 1):
+            raise ValueError("n-gram LM: symbols do not cover the LM's classes")
+        names = _class_names(symbols, self._blank, self._num_classes)
+        names.update({self._bos: BOS, self._eos: EOS, self._unk: UNK})
+        out = ["", "\\data\\"]
+        out += ["ngram %d=%d" % (n, len(self._ngrams[n])) for n in range(1, self._order + 1)]
+        for n in range(1, self._order + 1):
+            out += ["", "\\%d-grams:" % n]
+            for g, (p, b) in sorted(self._ngrams[n].items()):
+                line = "%r\t%s" % (p, " ".join(names[t] for t in g))
+                out.append(line if b is None else "%s\t%r" % (line, b))
+        out += ["", "\\end\\", ""]
+        with open(path, "w", encoding="utf-8") as fh:
+            fh.write("\n".join(out))
+
+    # ------------------------------------------------------------------------------------------
+    # training: interpolated Kneser-Ney in backoff form
+    # ------------------------------------------------------------------------------------------
+    @classmethod
+    def train(cls, sequences, order, num_classes, blank):
+        """Interpolated Kneser-Ney over label-id sequences (each read as <s> w1 .. wn </s>).
+
+        One discount per order, D = n1 / (n1 + 2 n2) (0.5 where that is undefined or outside
+        (0, 1)); lower orders use continuation counts, except n-grams that begin with <s>, which
+        keep raw counts; the unigram level is interpolated with the uniform distribution over the
+        classes and </s>.  Each seen n-gram stores its full interpolated probability and each
+        context its interpolation mass, which makes the backoff form the interpolated model."""
+        order = _check_order(order)
+        C = int(num_classes)
+        if C < 2 or not 0 <= blank < C:
+            raise ValueError("n-gram LM: need num_classes >= 2 and 0 <= blank < num_classes")
+        bos, eos = C, C + 1
+        raw = {n: Counter() for n in range(1, order + 1)}
+        for seq in sequences:
+            seq = [int(v) for v in seq]
+            if any(v < 0 or v >= C or v == blank for v in seq):
+                raise ValueError("n-gram LM: a training label is out of range or the blank")
+            w = [bos] + seq + [eos]
+            for n in range(1, order + 1):
+                for j in range(len(w) - n + 1):
+                    raw[n][tuple(w[j:j + n])] += 1
+        raw[1].pop((bos,), None)                            # <s> is never predicted
+        # KN counts: raw at the top order and for n-grams that begin with <s>, else the number of
+        # distinct tokens seen before the n-gram
+        kn = {order: raw[order]}
+        for n in range(order - 1, 0, -1):
+            left = Counter(g[1:] for g in raw[n + 1])
+            kn[n] = {g: (c if g[0] == bos else left[g]) for g, c in raw[n].items()}
+        disc, denom, types = {}, {}, {}
+        for n in range(1, order + 1):
+            n1 = sum(1 for c in kn[n].values() if c == 1)
+            n2 = sum(1 for c in kn[n].values() if c == 2)
+            d = n1 / (n1 + 2 * n2) if n1 + 2 * n2 else 0.0
+            disc[n] = d if 0.0 < d < 1.0 else 0.5
+            den, typ = defaultdict(int), defaultdict(int)
+            for g, c in kn[n].items():
+                den[g[:-1]] += c
+                typ[g[:-1]] += 1
+            denom[n], types[n] = den, typ
+
+        def gamma(n, h):
+            return disc[n] * types[n][h] / denom[n][h]
+
+        memo = {}
+
+        def prob(h, w):
+            """P_n(w | h), n = len(h) + 1"""
+            key = (h, w)
+            if key in memo:
+                return memo[key]
+            n = len(h) + 1
+            lower = prob(h[1:], w) if n > 1 else 1.0 / C
+            den = denom[n].get(h, 0)
+            if den == 0:
+                v = lower
+            else:
+                c = kn[n].get(h + (w,), 0)
+                v = max(c - disc[n], 0.0) / den + gamma(n, h) * lower
+            memo[key] = v
+            return v
+
+        vocab = [c for c in range(C) if c != blank] + [eos]
+        ngrams = {n: {} for n in range(1, order + 1)}
+        for w in vocab:
+            ngrams[1][(w,)] = (math.log10(prob((), w)), None)
+        ngrams[1][(bos,)] = (-99.0, None)
+        for n in range(2, order + 1):
+            for g in kn[n]:
+                ngrams[n][g] = (math.log10(prob(g[:-1], g[-1])), None)
+        for n in range(1, order):
+            for h in denom[n + 1]:
+                p, _ = ngrams[n][h]
+                ngrams[n][h] = (p, math.log10(gamma(n + 1, h)))
+        return cls(order, C, blank, ngrams)
+
+    # ------------------------------------------------------------------------------------------
+    # device tables
+    # ------------------------------------------------------------------------------------------
+    def host_tables(self):
+        """The tables of SbNgramLm as numpy arrays (built once): keys (uint64), vals (int32),
+        logp and bow (float64, natural log), tok (int32), and the scalars cap, order, bos,
+        lm_upper, lm_abs.  See include/speech_b200.h for the map's keys and hash."""
+        if self._host is not None:
+            return self._host
+        bos, eos = self._bos, self._eos
+        ctx = {(): 0}
+        entries = []                       # (key, value)
+        bow = [0.0]
+
+        def key(node, tok, kind):
+            return (node << 32) | ((tok + 1) << 1) | kind
+
+        def ctx_node(h):
+            """node of context h (oldest .. newest), created with backoff 0 when missing"""
+            if h in ctx:
+                return ctx[h]
+            parent = ctx_node(h[1:])
+            nid = len(bow)
+            ctx[h] = nid
+            bow.append(0.0)
+            entries.append((key(parent, h[0], 0), nid))
+            return nid
+
+        def usable(g):
+            # contexts: <s> only as the oldest token, never </s>
+            return all(t != eos for t in g) and all(t != bos for t in g[1:])
+
+        logp = []
+        upper_p, abs_p = -math.inf, 0.0
+        upper_b = [0.0] * (self._order + 1)
+        abs_b = [0.0] * (self._order + 1)
+        for n in range(1, self._order + 1):
+            for g, (p10, b10) in sorted(self._ngrams[n].items()):
+                p = p10 * LN10
+                if b10 is not None and n < self._order:
+                    b = b10 * LN10
+                    upper_b[n] = max(upper_b[n], b)
+                    abs_b[n] = max(abs_b[n], abs(b))
+                    if usable(g):
+                        bow[ctx_node(g)] = b
+                if g[-1] in (bos, eos) or not usable(g[:-1]):
+                    continue                # never looked up
+                upper_p, abs_p = max(upper_p, p), max(abs_p, abs(p))
+                entries.append((key(ctx_node(g[:-1]), g[-1], 1), len(logp)))
+                logp.append(p)
+        cap = 64
+        while cap < 2 * len(entries):
+            cap <<= 1
+        keys = np.zeros(cap, np.uint64)
+        vals = np.full(cap, -1, np.int32)
+        for k, v in entries:
+            h = ((k * _HASH_MUL) & _MASK64) >> 32 & (cap - 1)
+            while keys[h] != 0:
+                h = (h + 1) & (cap - 1)
+            keys[h] = k
+            vals[h] = v
+        self._host = {
+            "keys": keys, "vals": vals, "logp": np.array(logp or [0.0], np.float64),
+            "bow": np.array(bow, np.float64), "tok": self._tok.copy(), "cap": cap,
+            "order": self._order, "bos": bos,
+            "lm_upper": upper_p + sum(upper_b), "lm_abs": abs_p + sum(abs_b),
+        }
+        return self._host
+
+    def device_tables(self, device):
+        """(SbNgramLm ctypes struct, tensors it points into) on `device`, built once per device"""
+        import torch
+        from . import _lib
+        device = torch.device(device)
+        if device.type == "cuda" and device.index is None:
+            device = torch.device("cuda", torch.cuda.current_device())
+        if device not in self._dev:
+            h = self.host_tables()
+            t = {k: torch.from_numpy(h[k].view(np.int64) if k == "keys" else h[k]).to(device)
+                 for k in ("keys", "vals", "logp", "bow", "tok")}
+            st = _lib.SbNgramLm(t["keys"].data_ptr(), t["vals"].data_ptr(), t["logp"].data_ptr(),
+                                t["bow"].data_ptr(), t["tok"].data_ptr(), h["cap"], h["order"],
+                                self._num_classes, h["bos"], self._blank, h["lm_upper"],
+                                h["lm_abs"])
+            self._dev[device] = (st, t)
+        return self._dev[device]
+
+    def __getstate__(self):
+        d = dict(self.__dict__)
+        d["_dev"] = {}
+        return d

@@ -3,7 +3,7 @@ import numpy as np
 import torch
 
 from . import model
-from .ctc_decoder import decode, decode_batch
+from .ctc_decoder import check_lm, decode, decode_batch
 from ..functions import ctc
 
 
@@ -69,12 +69,16 @@ class CTC(model.Model):
     def collate(self, inputs, labels):
         return self.lattice_batch(inputs, labels)
 
-    def infer(self, batch, beam_size=1):
+    def infer(self, batch, beam_size=1, lm=None, lm_weight=0.0, insertion_bonus=0.0):
+        """Best label sequence of each utterance.  lm: an n-gram LM over this model's classes
+        (speech_b200.lm.NGramLM) fused into the beam search with lm_weight and insertion_bonus."""
+        check_lm(lm, lm_weight, insertion_bonus, self.blank + 1, self.blank)
         x, y, x_lens, y_lens = self._collated(batch)
         lens = self.exact_lens(x_lens)
         with torch.no_grad():
             probs = self._forward_impl(x, lens, softmax=True)
-        return decode_batch(probs, beam_size=beam_size, blank=self.blank, lens=lens)
+        return decode_batch(probs, beam_size=beam_size, blank=self.blank, lens=lens, lm=lm,
+                            lm_weight=lm_weight, insertion_bonus=insertion_bonus)
 
     @staticmethod
     def max_decode(pred, blank):

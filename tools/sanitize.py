@@ -17,6 +17,10 @@ for _ in range(2):
     opt.zero_grad(); loss = m.loss((inputs, labels)); loss.backward(); opt.step()
 print("ctc step ok", loss.item())
 print("infer", [len(p) for p in m.infer((inputs, labels), beam_size=4)])
+from speech_b200.lm import NGramLM
+lm = NGramLM.train(labels, 4, 29, 28)
+print("infer with LM", [len(p) for p in m.infer((inputs, labels), beam_size=4, lm=lm,
+                                                  lm_weight=0.5, insertion_bonus=1.0)])
 s = Seq2Seq(80, 30, cfg).cuda()
 lab2 = [[29] + l + [28] for l in labels]
 l2 = s.loss((inputs, lab2)); l2.backward()
@@ -139,6 +143,17 @@ _lib.check(lib.sb_ctc_prefix_beam_shortlist(lp.data_ptr(), lens.data_ptr(), 2, 3
                                             o_lab.data_ptr(), o_len.data_ptr(), o_sc.data_ptr(),
                                             ws.data_ptr(), nb.value, _lib.stream_ptr()),
            "sb_ctc_prefix_beam_shortlist")
+# the LM-fused shortlist kernel, forced, with a weight strong enough that its bound check fails
+# on some frames (so the rescan runs too)
+_lib.check(lib.sb_ctc_prefix_beam_lm_shortlist(lp.data_ptr(), lens.data_ptr(), 2, 30, 29, 4, 28,
+                                               ctypes.byref(lm.device_tables(lp.device)[0]), 2.0,
+                                               1.0, o_lab.data_ptr(), o_len.data_ptr(),
+                                               o_sc.data_ptr(), ws.data_ptr(), nb.value,
+                                               _lib.stream_ptr()),
+           "sb_ctc_prefix_beam_lm_shortlist")
+_resc = ctypes.c_ulonglong(0)
+_lib.check(lib.sb_debug_ctc_lm_rescans(ctypes.byref(_resc)), "sb_debug_ctc_lm_rescans")
+print("LM shortlist route ok", o_len.tolist(), "frames rescanned:", _resc.value)
 acts = torch.randn(2, 30, 29, device="cuda")
 nc = ctypes.c_size_t(0)
 lib.sb_ctc_compact_workspace_size(2, 30, 29, 3, ctypes.byref(nc))
