@@ -436,6 +436,33 @@ int sb_s2s_beam_select_split_batch(const float* logp, void* state, double* c_sco
                                    int* stop, int B, void* workspace, size_t workspace_bytes,
                                    void* stream);
 
+/* Attention beam search with shallow fusion of the n-gram LM (SbNgramLm above).
+ *   sb_s2s_beam_select_lm_batch        sb_s2s_beam_select_batch with the LM and its weights
+ *   sb_s2s_beam_select_split_lm_batch  sb_s2s_beam_select_split_batch with the LM and its weights
+ * Candidate (r, c), live row r extended by class c, has the float64 value
+ *   score_r + ((double)logp[r][c] + (lm_weight * lm(c | h_r) + beta_c)),
+ * evaluated in that order, with beta_c = insertion_bonus for c != end_tok and 0 for end_tok.  h_r
+ * is row r's last order-1 tokens; its root (the start token) reads as <s>, before which there is
+ * nothing.  The fused values are the hypothesis scores throughout: selection, completion, the stop
+ * rule and the final score.  With lm_weight = insertion_bonus = 0 the results equal the LM-less
+ * entry points' bit for bit.  The LM's classes are the model's vocabulary: lm->tok[end_tok] must
+ * be the token of </s> (the ABI cannot check this; speech_b200.lm.NGramLM with `end` builds such
+ * tables), and lm->blank is the start token, which must not be a class the search scores.
+ * SB_ERR_INVALID for a null LM or table pointer, lm_weight < 0, a non-finite weight or bound,
+ * lm->num_classes < C, 0 <= lm->blank < C, or a cap that is not a power of two;
+ * SB_ERR_UNSUPPORTED for order > SB_LM_MAX_ORDER; otherwise as the LM-less entry points. */
+int sb_s2s_beam_select_lm_batch(const float* logp, void* state, double* c_scores, int* nodes,
+                                int* parent_row, int* tok_next, int* out_tokens, int K, int C,
+                                int end_tok, int step, int max_len, int node_cap, int c_cap,
+                                int* stop, int B, const SbNgramLm* lm, double lm_weight,
+                                double insertion_bonus, void* stream);
+int sb_s2s_beam_select_split_lm_batch(const float* logp, void* state, double* c_scores,
+                                      int* nodes, int* parent_row, int* tok_next, int* out_tokens,
+                                      int K, int C, int end_tok, int step, int max_len,
+                                      int node_cap, int c_cap, int* stop, int B, void* workspace,
+                                      size_t workspace_bytes, const SbNgramLm* lm,
+                                      double lm_weight, double insertion_bonus, void* stream);
+
 /* ---------------------------------------------------------------------------------------
  * RNN-Transducer loss + gradient w.r.t. the log-probabilities.
  * Replaces: transducer.functions.transducer.TransducerLoss()(log_probs, labels, x_lens, y_lens)

@@ -101,6 +101,12 @@ SIGNATURES = {
     "sb_s2s_beam_select_split_batch": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_int, _c_int,
                                                 _c_int, _c_int, _c_int, _c_int, _c_int, _vp,
                                                 _c_int, _vp, _c_sz, _vp]),
+    "sb_s2s_beam_select_lm_batch": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_int, _c_int,
+                                             _c_int, _c_int, _c_int, _c_int, _c_int, _vp, _c_int,
+                                             _lmp, _db, _db, _vp]),
+    "sb_s2s_beam_select_split_lm_batch": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_int,
+                                                   _c_int, _c_int, _c_int, _c_int, _c_int, _c_int,
+                                                   _vp, _c_int, _vp, _c_sz, _lmp, _db, _db, _vp]),
     "sb_rnnt_workspace_size": (_c_int, [_c_int, _c_int, _c_int, ctypes.POINTER(_c_sz)]),
     "sb_rnnt_fwd_bwd": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int,
                                  _vp, _vp, _c_sz, _vp]),

@@ -16,6 +16,7 @@
 // Roofline: HBM-nominal (reads T*S floats per utterance), in practice latency-bound by the
 // T-serial beam update; decode is not on the training path.
 #include "beam.cuh"
+#include "ngram.cuh"
 #include <math.h>
 
 #include "../../include/speech_b200.h"
@@ -83,38 +84,17 @@ __device__ __forceinline__ LmShared& lm_shared() {
   return sh;
 }
 
-__device__ __forceinline__ int lm_find(const SbNgramLm& lm, int node, int tok, int kind) {
-  const unsigned long long key = ((unsigned long long)(unsigned int)node << 32) |
-                                 ((unsigned long long)(unsigned int)(tok + 1) << 1) |
-                                 (unsigned long long)kind;
-  unsigned int h = (unsigned int)((key * 0x9E3779B97F4A7C15ull) >> 32) & (lm.cap - 1);
-  for (int probe = 0; probe < lm.cap; ++probe) {
-    const unsigned long long k = __ldg(lm.keys + h);
-    if (k == key) return __ldg(lm.vals + h);
-    if (k == 0ull) return -1;
-    h = (h + 1) & (lm.cap - 1);
-  }
-  return -1;
-}
-
 struct LmFuse {
   static constexpr bool kLm = true;
   static constexpr int kMinBlocks = 1;
   SbNgramLm lm;
   double alpha, beta;
 
-  // lm(s | ctx_i): the longest stored context first, adding the backoff of each that misses
+  // lm(s | ctx_i)
   __device__ __forceinline__ double lm_logp(int i, int s) const {
     const LmShared& sh = lm_shared();
     const int t = __ldg(lm.tok + s);
-    double acc = 0.0;
-    for (int d = sh.depth[i]; d >= 0; --d) {
-      const int c = sh.ctx[i][d];
-      const int g = lm_find(lm, c, t, 1);
-      if (g >= 0) return acc + __ldg(lm.logp + g);
-      acc += __ldg(lm.bow + c);
-    }
-    return acc;   // not reached: every non-blank class maps to a token with a unigram
+    return lm_backoff(lm, sh.ctx[i], sh.depth[i], t);
   }
   __device__ __forceinline__ double q(int i, int s, double p) const {
     return p + (alpha * lm_logp(i, s) + beta);
@@ -126,17 +106,7 @@ __device__ __forceinline__ void lm_resolve(const LmFuse& fu, int par, int nb) {
   LmShared& sh = lm_shared();
   const int i = threadIdx.x;
   if (i >= nb) return;
-  int c = 0, d = 0;
-  sh.ctx[i][0] = 0;
-  for (int k = 0; k < fu.lm.order - 1; ++k) {
-    const int h = sh.hist[par][i][k];
-    const int nc = lm_find(fu.lm, c, h < 0 ? fu.lm.bos : __ldg(fu.lm.tok + h), 0);
-    if (nc < 0) break;
-    c = nc;
-    sh.ctx[i][++d] = c;
-    if (h < 0) break;
-  }
-  sh.depth[i] = d;
+  sh.depth[i] = lm_context(fu.lm, [&](int k) { return sh.hist[par][i][k]; }, sh.ctx[i]);
 }
 
 // value of the candidate "beam entry j keeps its prefix" at this frame

@@ -31,6 +31,7 @@
 // Everything is fp32 (the reference's arithmetic); roofline: L2 bandwidth on eh and the cell
 // weights per token (B*T*H*4 bytes forward, 3x that backward, + 24 H^2), in practice launch-bound.
 #include "beam.cuh"
+#include "ngram.cuh"
 #include <math.h>
 #include <stddef.h>
 #include <string.h>
@@ -909,8 +910,67 @@ struct BeamParams {
 SB_DEVINL void beam_bookkeep(const BeamParams& p, const int* sel_idx, const double* sel_sc,
                              int want);
 
+// ------------------------------------------------------------------------------------------------
+// Shallow fusion.  The selection is written once over a policy that gives the value of candidate
+// (r, c), live row r extended by class c:
+//   S2sNoFuse  score_r + logp[r][c] (the LM-less search, its arithmetic untouched);
+//   S2sLmFuse  score_r + ((double)logp[r][c] + (alpha * lm(c | h_r) + beta_c)), lm the backoff
+//              lookup of SbNgramLm (ngram.cuh), beta_c = beta but 0 for end_tok, whose LM token is
+//              </s>; with alpha = beta = 0 this is the LM-less value bit for bit.
+// h_r is row r's last order-1 tokens, read from its node up the parent links of the arena; the
+// root (the start token) reads as <s>.  Once per step each CTA resolves every live row's context
+// nodes into shared memory (resolve), so a candidate's lookup is at most `order` probes.  The
+// fused value is the hypothesis score everywhere after: selection, completion, stop rule, result.
+// ------------------------------------------------------------------------------------------------
+struct S2sNoFuse {
+  static constexpr bool kLm = false;
+  SB_DEVINL void resolve(const BeamParams&, const BeamState*, int) const {}
+  SB_DEVINL double value(const BeamParams& p, const BeamState* st, int r, int c) const {
+    return st->score[r] + (double)p.logp[(size_t)r * p.C + c];
+  }
+};
+
+struct S2sLmShared {
+  int ctx[BM_MAXK][SB_LM_MAX_ORDER];   // context nodes of each live row, [0] = root .. [depth]
+  int depth[BM_MAXK];
+};
+SB_DEVINL S2sLmShared& s2s_lm_shared() {
+  __shared__ S2sLmShared sh;
+  return sh;
+}
+
+struct S2sLmFuse {
+  static constexpr bool kLm = true;
+  SbNgramLm lm;
+  double alpha, beta;
+
+  // thread r < nl: row r's context nodes; the caller syncs
+  SB_DEVINL void resolve(const BeamParams& p, const BeamState* st, int nl) const {
+    const int r = threadIdx.x;
+    if (r >= nl) return;
+    S2sLmShared& sh = s2s_lm_shared();
+    int q = st->node[r];
+    // the k-th most recent token of row r's hypothesis, -1 (<s>) at the root
+    auto older = [&](int) {
+      const int up = p.nodes[2 * q];
+      if (up < 0) return -1;
+      const int t = p.nodes[2 * q + 1];
+      q = up;
+      return t;
+    };
+    sh.depth[r] = lm_context(lm, older, sh.ctx[r]);
+  }
+  SB_DEVINL double value(const BeamParams& p, const BeamState* st, int r, int c) const {
+    const S2sLmShared& sh = s2s_lm_shared();
+    const double l = lm_backoff(lm, sh.ctx[r], sh.depth[r], __ldg(lm.tok + c));
+    return st->score[r] +
+           ((double)p.logp[(size_t)r * p.C + c] + (alpha * l + (c == p.end_tok ? 0.0 : beta)));
+  }
+};
+
 // grid B: CTA b selects for utterance b
-__global__ void __launch_bounds__(256) s2s_beam_select_kernel(const BeamParams pb) {
+template <class Fuse>
+__global__ void __launch_bounds__(256) s2s_beam_select_kernel(const BeamParams pb, const Fuse fu) {
   extern __shared__ unsigned char bm_smem[];
   const BeamParams p = pb.of(blockIdx.x);
   double* sc = reinterpret_cast<double*>(bm_smem);       // [K * C]
@@ -920,9 +980,13 @@ __global__ void __launch_bounds__(256) s2s_beam_select_kernel(const BeamParams p
   BeamState* st = p.st;
   if (st->done) return;
   const int K = p.K, C = p.C, nl = st->nlive;
+  if constexpr (Fuse::kLm) {
+    fu.resolve(p, st, nl);
+    __syncthreads();
+  }
   for (int i = tid; i < K * C; i += 256) {
     const int r = i / C, c = i - r * C;
-    sc[i] = r < nl ? st->score[r] + (double)p.logp[(size_t)r * C + c] : nan("");
+    sc[i] = r < nl ? fu.value(p, st, r, c) : nan("");
   }
   __syncthreads();
   const int want = min(2 * K, nl * C);
@@ -943,14 +1007,18 @@ __global__ void __launch_bounds__(256) s2s_beam_select_kernel(const BeamParams p
 //   stage 2 (s2s_beam_merge): grid B, a CTA per utterance merges its tiles' sorted lists (a head
 //           per tile) into the first min(2K, nl*C) and runs the same bookkeeping.
 // The union of the top K and the first K non-ended candidates lies in the global top 2K (at most
-// K of the top K end in end_tok), so the 2K per tile lose nothing.
+// K of the top K end in end_tok), so the 2K per tile lose nothing.  The argument holds for any
+// candidate values, so for the fused ones too; with an LM every tile CTA resolves the live rows'
+// contexts itself (a few probes per row, next to the tile's 4096 lookups).
 // ------------------------------------------------------------------------------------------------
 static constexpr int BM_PER_THREAD = 16;
 static constexpr int BM_TILE = 256 * BM_PER_THREAD;
 
 // t_sc / t_idx [B][tiles][2K], t_cnt [B][tiles]
+template <class Fuse>
 __global__ void __launch_bounds__(256) s2s_beam_tiles_kernel(const BeamParams pb, double* t_sc,
-                                                             int* t_idx, int* t_cnt) {
+                                                             int* t_idx, int* t_cnt,
+                                                             const Fuse fu) {
   const BeamParams p = pb.of(blockIdx.y);
   const BeamState* st = p.st;
   if (st->done) return;
@@ -960,6 +1028,10 @@ __global__ void __launch_bounds__(256) s2s_beam_tiles_kernel(const BeamParams pb
   t_idx += u0 * K2;
   t_cnt += u0;
   const int n = st->nlive * C;
+  if constexpr (Fuse::kLm) {
+    fu.resolve(p, st, st->nlive);
+    __syncthreads();
+  }
   double v[BM_PER_THREAD];
 #pragma unroll
   for (int j = 0; j < BM_PER_THREAD; ++j) {
@@ -967,7 +1039,7 @@ __global__ void __launch_bounds__(256) s2s_beam_tiles_kernel(const BeamParams pb
     v[j] = nan("");
     if (i < n) {
       const int r = i / C, c = i - r * C;
-      v[j] = st->score[r] + (double)p.logp[(size_t)r * C + c];
+      v[j] = fu.value(p, st, r, c);
     }
   }
   int q = 0;
@@ -1333,10 +1405,11 @@ static int beam_params(sb::BeamParams* p, const float* logp, void* state, double
   return SB_OK;
 }
 
+template <class Fuse>
 static int beam_select(const float* logp, void* state, double* c_scores, int* nodes,
                        int* parent_row, int* tok_next, int* out_tokens, int K, int C, int end_tok,
                        int step, int max_len, int node_cap, int c_cap, int* stop, int B,
-                       void* stream_) {
+                       void* stream_, const Fuse& fu) {
   sb::BeamParams p;
   const int rc = beam_params(&p, logp, state, c_scores, nodes, parent_row, tok_next, out_tokens, K,
                              C, end_tok, step, max_len, node_cap, c_cap, stop, B);
@@ -1345,10 +1418,10 @@ static int beam_select(const float* logp, void* state, double* c_scores, int* no
   if (smem > 200 * 1024) return SB_ERR_UNSUPPORTED;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (smem > 40 * 1024 &&
-      cudaFuncSetAttribute(sb::s2s_beam_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                           (int)smem) != cudaSuccess)
+      cudaFuncSetAttribute(sb::s2s_beam_select_kernel<Fuse>,
+                           cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
     return SB_ERR_CUDA;
-  sb::s2s_beam_select_kernel<<<B, 256, smem, stream>>>(p);
+  sb::s2s_beam_select_kernel<Fuse><<<B, 256, smem, stream>>>(p, fu);
   return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
 }
 
@@ -1357,7 +1430,7 @@ extern "C" int sb_s2s_beam_select(const float* logp, void* state, double* c_scor
                                   int end_tok, int step, int max_len, int node_cap, int c_cap,
                                   void* stream_) {
   return beam_select(logp, state, c_scores, nodes, parent_row, tok_next, out_tokens, K, C, end_tok,
-                     step, max_len, node_cap, c_cap, nullptr, 1, stream_);
+                     step, max_len, node_cap, c_cap, nullptr, 1, stream_, sb::S2sNoFuse{});
 }
 
 extern "C" int sb_s2s_beam_select_batch(const float* logp, void* state, double* c_scores,
@@ -1367,7 +1440,7 @@ extern "C" int sb_s2s_beam_select_batch(const float* logp, void* state, double* 
                                         void* stream_) {
   if (!stop) return SB_ERR_INVALID;
   return beam_select(logp, state, c_scores, nodes, parent_row, tok_next, out_tokens, K, C, end_tok,
-                     step, max_len, node_cap, c_cap, stop, B, stream_);
+                     step, max_len, node_cap, c_cap, stop, B, stream_, sb::S2sNoFuse{});
 }
 
 extern "C" int sb_s2s_beam_select_fits(int K, int C) {
@@ -1391,11 +1464,12 @@ extern "C" int sb_s2s_beam_split_workspace_size(int K, int C, size_t* bytes) {
   return sb_s2s_beam_split_workspace_size_batch(K, C, 1, bytes);
 }
 
+template <class Fuse>
 static int beam_select_split(const float* logp, void* state, double* c_scores, int* nodes,
                              int* parent_row, int* tok_next, int* out_tokens, int K, int C,
                              int end_tok, int step, int max_len, int node_cap, int c_cap,
                              int* stop, int B, void* workspace, size_t workspace_bytes,
-                             void* stream_) {
+                             void* stream_, const Fuse& fu) {
   if (!workspace) return SB_ERR_INVALID;
   sb::BeamParams p;
   const int rc = beam_params(&p, logp, state, c_scores, nodes, parent_row, tok_next, out_tokens, K,
@@ -1417,7 +1491,7 @@ static int beam_select_split(const float* logp, void* state, double* c_scores, i
   double* t_sc = reinterpret_cast<double*>(workspace);
   int* t_idx = reinterpret_cast<int*>(t_sc + slots);
   int* t_cnt = t_idx + slots;
-  sb::s2s_beam_tiles_kernel<<<dim3(nt, B), 256, 0, stream>>>(p, t_sc, t_idx, t_cnt);
+  sb::s2s_beam_tiles_kernel<Fuse><<<dim3(nt, B), 256, 0, stream>>>(p, t_sc, t_idx, t_cnt, fu);
   sb::s2s_beam_merge_kernel<<<B, 256, smem, stream>>>(p, t_sc, t_idx, t_cnt, nt);
   return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
 }
@@ -1429,7 +1503,7 @@ extern "C" int sb_s2s_beam_select_split(const float* logp, void* state, double* 
                                         size_t workspace_bytes, void* stream_) {
   return beam_select_split(logp, state, c_scores, nodes, parent_row, tok_next, out_tokens, K, C,
                            end_tok, step, max_len, node_cap, c_cap, nullptr, 1, workspace,
-                           workspace_bytes, stream_);
+                           workspace_bytes, stream_, sb::S2sNoFuse{});
 }
 
 extern "C" int sb_s2s_beam_select_split_batch(const float* logp, void* state, double* c_scores,
@@ -1441,7 +1515,54 @@ extern "C" int sb_s2s_beam_select_split_batch(const float* logp, void* state, do
   if (!stop) return SB_ERR_INVALID;
   return beam_select_split(logp, state, c_scores, nodes, parent_row, tok_next, out_tokens, K, C,
                            end_tok, step, max_len, node_cap, c_cap, stop, B, workspace,
-                           workspace_bytes, stream_);
+                           workspace_bytes, stream_, sb::S2sNoFuse{});
+}
+
+// The fusion policy of an LM entry point, after the checks the header lists
+static int beam_lm_fuse(const SbNgramLm* lm, double lm_weight, double insertion_bonus, int C,
+                        sb::S2sLmFuse* fu) {
+  if (!lm || !lm->keys || !lm->vals || !lm->logp || !lm->bow || !lm->tok) return SB_ERR_INVALID;
+  if (!(lm_weight >= 0.0) || !isfinite(lm_weight) || !isfinite(insertion_bonus))
+    return SB_ERR_INVALID;
+  if (!isfinite(lm->lm_upper) || !isfinite(lm->lm_abs) || lm->num_classes < C) return SB_ERR_INVALID;
+  if (lm->blank >= 0 && lm->blank < C) return SB_ERR_INVALID;   // a scored class with no LM token
+  if (lm->cap <= 0 || (lm->cap & (lm->cap - 1)) || lm->order < 1) return SB_ERR_INVALID;
+  if (lm->order > SB_LM_MAX_ORDER) return SB_ERR_UNSUPPORTED;
+  fu->lm = *lm;
+  fu->alpha = lm_weight;
+  fu->beta = insertion_bonus;
+  return SB_OK;
+}
+
+extern "C" int sb_s2s_beam_select_lm_batch(const float* logp, void* state, double* c_scores,
+                                           int* nodes, int* parent_row, int* tok_next,
+                                           int* out_tokens, int K, int C, int end_tok, int step,
+                                           int max_len, int node_cap, int c_cap, int* stop, int B,
+                                           const SbNgramLm* lm, double lm_weight,
+                                           double insertion_bonus, void* stream_) {
+  if (!stop) return SB_ERR_INVALID;
+  sb::S2sLmFuse fu;
+  const int rc = beam_lm_fuse(lm, lm_weight, insertion_bonus, C, &fu);
+  if (rc != SB_OK) return rc;
+  return beam_select(logp, state, c_scores, nodes, parent_row, tok_next, out_tokens, K, C, end_tok,
+                     step, max_len, node_cap, c_cap, stop, B, stream_, fu);
+}
+
+extern "C" int sb_s2s_beam_select_split_lm_batch(const float* logp, void* state,
+                                                 double* c_scores, int* nodes, int* parent_row,
+                                                 int* tok_next, int* out_tokens, int K, int C,
+                                                 int end_tok, int step, int max_len, int node_cap,
+                                                 int c_cap, int* stop, int B, void* workspace,
+                                                 size_t workspace_bytes, const SbNgramLm* lm,
+                                                 double lm_weight, double insertion_bonus,
+                                                 void* stream_) {
+  if (!stop) return SB_ERR_INVALID;
+  sb::S2sLmFuse fu;
+  const int rc = beam_lm_fuse(lm, lm_weight, insertion_bonus, C, &fu);
+  if (rc != SB_OK) return rc;
+  return beam_select_split(logp, state, c_scores, nodes, parent_row, tok_next, out_tokens, K, C,
+                           end_tok, step, max_len, node_cap, c_cap, stop, B, workspace,
+                           workspace_bytes, stream_, fu);
 }
 
 extern "C" int sb_s2s_beam_gather_batch(const float* hx_in, const float* sx_in,

@@ -463,15 +463,19 @@ def beam_search(m, eh, start_tok, end_tok, beam_size, max_len):
     return beam_search_batch(m, _f(eh)[:1], start_tok, end_tok, beam_size, max_len)[0][0]
 
 
-def beam_search_batch(m, eh, start_tok, end_tok, beam_size, max_len, lens=None):
+def beam_search_batch(m, eh, start_tok, end_tok, beam_size, max_len, lens=None, lm=None,
+                      lm_weight=0.0, insertion_bonus=0.0):
     """Seq2Seq.beam_search (seq2seq.py:180-227) for each of the B utterances of eh (B, T, H) at
     once, device-resident.  Utterance b's K beam entries are rows b*K .. b*K+K-1 of the step
     kernels, which run over all B*K rows until every utterance has stopped; expand / prune /
     complete / stop run in one bookkeeping CTA per utterance and step (csrc/s2s.cu), and the
     hypotheses are back-tracked on the device.  Each utterance's search is the one it gets alone,
     bit for bit.  The host enqueues every step up front and reads all B results back in ONE copy.
-    lens (optional): frames each utterance attends over.  -> list of B (token tuple, float64
-    score of that hypothesis, steps that utterance's search ran)."""
+    lens (optional): frames each utterance attends over.  lm (optional): an NGramLM whose classes
+    are the vocabulary, blank the start token and end the end token (the caller checks), fused
+    into every candidate as logp + (lm_weight * lm + insertion_bonus, no bonus for the end token);
+    the scores are then the fused ones.  -> list of B (token tuple, float64 score of that
+    hypothesis, steps that utterance's search ran)."""
     lib = _lib.load()
     w = DecoderWeights(m)
     ehc = _f(eh)
@@ -512,6 +516,9 @@ def beam_search_batch(m, eh, start_tok, end_tok, beam_size, max_len, lens=None):
     p_state, p_c, p_nodes = state.data_ptr(), c_scores.data_ptr(), nodes.data_ptr()
     p_par, p_tok, p_out = parent.data_ptr(), tok.data_ptr(), out_tokens.data_ptr()
     p_stop = stop.data_ptr()
+    if lm is not None:
+        tables, _ = lm.device_tables(dev)
+        fusion = (tables, float(lm_weight), float(insertion_bonus))
     # buffers: [0] = state entering the step (gathered), [1] = state produced by the step
     for e in range(max_len):
         _cell_fwd(lib, w, p_tok, 1, sx[0] if e > 0 else None, hx[0], hx[1], None, None, done_ptr,
@@ -524,7 +531,17 @@ def beam_search_batch(m, eh, start_tok, end_tok, beam_size, max_len, lens=None):
                       done=done_ptr, with_fc=False, lens=ld)
             _fc_rows(lib, w, fc_ws, hx[1], sx[1], R, sp, logits=logp, done=done_ptr)
             _fc_logp(lib, w, fc_ws, logp, logp, R, sp, done=done_ptr)
-        if split:
+        if lm is not None and split:
+            ops._launch("s2s_beam_select_split_lm", 0.0,
+                        lambda: lib.sb_s2s_beam_select_split_lm_batch(
+                            logp.data_ptr(), p_state, p_c, p_nodes, p_par, p_tok, p_out, K, C,
+                            int(end_tok), e, max_len, node_cap, c_cap, p_stop, B,
+                            sel_ws.data_ptr(), sel_ws.numel(), *fusion, sp))
+        elif lm is not None:
+            ops._launch("s2s_beam_select_lm", 0.0, lambda: lib.sb_s2s_beam_select_lm_batch(
+                logp.data_ptr(), p_state, p_c, p_nodes, p_par, p_tok, p_out, K, C, int(end_tok), e,
+                max_len, node_cap, c_cap, p_stop, B, *fusion, sp))
+        elif split:
             ops._launch("s2s_beam_select_split", 0.0, lambda: lib.sb_s2s_beam_select_split_batch(
                 logp.data_ptr(), p_state, p_c, p_nodes, p_par, p_tok, p_out, K, C, int(end_tok), e,
                 max_len, node_cap, c_cap, p_stop, B, sel_ws.data_ptr(), sel_ws.numel(), sp))

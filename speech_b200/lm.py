@@ -1,7 +1,10 @@
-"""Token-level backoff n-gram language model for shallow fusion in the CTC prefix beam search.
+"""Token-level backoff n-gram language model for shallow fusion in the CTC prefix beam search and
+the attention model's beam search.
 
 The LM is over the acoustic model's own output classes (characters or subword units); the blank is
 never an LM token.  Orders 1..10, with a sentence start <s>, an end </s> and optionally <unk>.
+For the attention model, whose vocabulary has an end class and a start class, the end class is
+the LM's </s> and the start class takes the blank's place (it is never predicted):
 Values are held as the ARPA file's log10 numbers and converted once to natural log
 (`v10 * math.log(10)`) for lookup, so `from_arpa(to_arpa(lm))` reproduces every float64 value.
 
@@ -9,12 +12,17 @@ Values are held as the ARPA file's log10 numbers and converted once to natural l
     lm = NGramLM.train(transcripts, order=5, num_classes=V + 1, blank=V)
     model.infer(batch, beam_size=8, lm=lm, lm_weight=0.8, insertion_bonus=1.5)
 
+    lm = NGramLM.from_arpa("chars.arpa", preproc.int_to_char, blank=V - 1, end=V - 2)
+    lm = NGramLM.train([preproc.encode(t) for t in texts], order=5, num_classes=V, blank=V - 1,
+                       end=V - 2)
+    s2s_model.recognize(inputs, beam_size=8, lm=lm, lm_weight=0.5, insertion_bonus=0.5)
+
 lm(s | h) follows ARPA backoff: h is the prefix's last order-1 symbols, preceded by <s> where the
 prefix is shorter; when the n-gram (h, s) is stored its log-probability is used, otherwise the
 backoff weight of h (0 when h is not stored) is added and the oldest context token dropped.
 A class the LM does not know reads as <unk>.
 
-Device tables (csrc/decode.cu, SbNgramLm in include/speech_b200.h): one open-addressed map with
+Device tables (csrc/ngram.cuh, SbNgramLm in include/speech_b200.h): one open-addressed map with
 two kinds of key, (context node, older token) -> context node and (context node, token) ->
 n-gram, over a trie of contexts read most recent token first.  They are built once and cached
 per device.
@@ -44,12 +52,12 @@ def _check_order(order):
     return int(order)
 
 
-def _class_names(symbols, blank, num_classes):
-    """{class: symbol} of the non-blank classes, validated"""
+def _class_names(symbols, blank, num_classes, end=None):
+    """{class: symbol} of the classes but the blank and the end, validated"""
     names = {}
     seen = {BOS: None, EOS: None, UNK: None}
     for c in range(num_classes):
-        if c == blank:
+        if c == blank or c == end:
             continue
         s = symbols[c] if symbols is not None else str(c)
         if not isinstance(s, str) or s == "" or any(ch.isspace() for ch in s):
@@ -84,15 +92,28 @@ def _layout(symbols, blank):
     return (len(symbols) + 1 if blank == len(symbols) else len(symbols)), int(blank), symbols
 
 
+def _check_end(end, blank, num_classes):
+    """the end class (None: the LM has none), validated"""
+    if end is None:
+        return None
+    if not isinstance(end, (int, np.integer)) or not 0 <= end < num_classes:
+        raise ValueError("n-gram LM: end %r outside 0..%d" % (end, num_classes - 1))
+    if end == blank:
+        raise ValueError("n-gram LM: the end class %d is the blank" % end)
+    return int(end)
+
+
 class NGramLM:
     """Backoff n-gram LM over class ids.  Tokens: class c -> c, <s> -> C, </s> -> C + 1,
-    <unk> -> C + 2 (C = num_classes).  Build with from_arpa or train."""
+    <unk> -> C + 2 (C = num_classes); the end class, where there is one, -> </s>.  Build with
+    from_arpa or train."""
 
-    def __init__(self, order, num_classes, blank, ngrams):
+    def __init__(self, order, num_classes, blank, ngrams, end=None):
         # ngrams[n]: {token tuple: (log10 prob, log10 backoff or None)}, n = 1..order
         self._order = order
         self._num_classes = num_classes
         self._blank = blank
+        self._end = _check_end(end, blank, num_classes)
         self._ngrams = ngrams
         self._bos, self._eos, self._unk = num_classes, num_classes + 1, num_classes + 2
         uni = ngrams[1]
@@ -100,7 +121,11 @@ class NGramLM:
         for c in range(num_classes):
             if c == blank:
                 continue
-            if (c,) in uni:
+            if c == self._end:
+                if (self._eos,) not in uni:
+                    raise ValueError("n-gram LM: the end class %d needs a %s unigram" % (c, EOS))
+                tok[c] = self._eos
+            elif (c,) in uni:
                 tok[c] = c
             elif (self._unk,) in uni:
                 tok[c] = self._unk
@@ -122,16 +147,23 @@ class NGramLM:
     def blank(self):
         return self._blank
 
+    @property
+    def end(self):
+        """the class read as </s> (the attention model's END), or None"""
+        return self._end
+
     # ------------------------------------------------------------------------------------------
     # ARPA
     # ------------------------------------------------------------------------------------------
     @classmethod
-    def from_arpa(cls, path, symbols, blank=None):
+    def from_arpa(cls, path, symbols, blank=None, end=None):
         """Read an ARPA file.  symbols[c] is the token string of class c (e.g. the reference
         Preprocessor.int_to_char in id order); blank defaults to the class after the last symbol.
+        end (optional): the class that is the LM's </s>; its symbol, like the blank's, is ignored.
         n-grams over words that are neither a class symbol nor <s>, </s>, <unk> are dropped."""
         num_classes, blank, symbols = _layout(symbols, blank)
-        names = _class_names(symbols, blank, num_classes)
+        end = _check_end(end, blank, num_classes)
+        names = _class_names(symbols, blank, num_classes, end)
         word_tok = {s: c for c, s in names.items()}
         word_tok.update({BOS: num_classes, EOS: num_classes + 1, UNK: num_classes + 2})
         with open(path, "r", encoding="utf-8") as fh:
@@ -188,7 +220,7 @@ class NGramLM:
         if i >= len(lines) or lines[i] != "\\end\\":
             raise ValueError("n-gram LM: %s: expected \\end\\ after the %d-grams (wrong counts?)"
                              % (path, order))
-        return cls(order, num_classes, blank, ngrams)
+        return cls(order, num_classes, blank, ngrams, end)
 
     def to_arpa(self, path, symbols=None):
         """Write an ARPA file; str(c) names class c unless symbols are given (same layout as
@@ -198,7 +230,7 @@ class NGramLM:
         if symbols is not None and len(symbols) < self._num_classes - (
                 self._blank == self._num_classes - 1):
             raise ValueError("n-gram LM: symbols do not cover the LM's classes")
-        names = _class_names(symbols, self._blank, self._num_classes)
+        names = _class_names(symbols, self._blank, self._num_classes, self._end)
         names.update({self._bos: BOS, self._eos: EOS, self._unk: UNK})
         out = ["", "\\data\\"]
         out += ["ngram %d=%d" % (n, len(self._ngrams[n])) for n in range(1, self._order + 1)]
@@ -215,24 +247,32 @@ class NGramLM:
     # training: interpolated Kneser-Ney in backoff form
     # ------------------------------------------------------------------------------------------
     @classmethod
-    def train(cls, sequences, order, num_classes, blank):
+    def train(cls, sequences, order, num_classes, blank, end=None):
         """Interpolated Kneser-Ney over label-id sequences (each read as <s> w1 .. wn </s>).
+        With an end class, one leading blank and one trailing end are stripped from each sequence
+        where present (so Preprocessor.encode outputs, START .. END, go straight in); a blank or
+        an end anywhere else is an error.
 
         One discount per order, D = n1 / (n1 + 2 n2) (0.5 where that is undefined or outside
         (0, 1)); lower orders use continuation counts, except n-grams that begin with <s>, which
         keep raw counts; the unigram level is interpolated with the uniform distribution over the
-        classes and </s>.  Each seen n-gram stores its full interpolated probability and each
+        classes (but the blank and the end) and </s>.  Each seen n-gram stores its full interpolated probability and each
         context its interpolation mass, which makes the backoff form the interpolated model."""
         order = _check_order(order)
         C = int(num_classes)
         if C < 2 or not 0 <= blank < C:
             raise ValueError("n-gram LM: need num_classes >= 2 and 0 <= blank < num_classes")
+        end = _check_end(end, blank, C)
         bos, eos = C, C + 1
         raw = {n: Counter() for n in range(1, order + 1)}
         for seq in sequences:
             seq = [int(v) for v in seq]
-            if any(v < 0 or v >= C or v == blank for v in seq):
-                raise ValueError("n-gram LM: a training label is out of range or the blank")
+            if end is not None:
+                seq = seq[1:] if seq and seq[0] == blank else seq
+                seq = seq[:-1] if seq and seq[-1] == end else seq
+            if any(v < 0 or v >= C or v == blank or v == end for v in seq):
+                raise ValueError("n-gram LM: a training label is out of range, the blank or "
+                                 "the end")
             w = [bos] + seq + [eos]
             for n in range(1, order + 1):
                 for j in range(len(w) - n + 1):
@@ -259,6 +299,7 @@ class NGramLM:
         def gamma(n, h):
             return disc[n] * types[n][h] / denom[n][h]
 
+        vocab = [c for c in range(C) if c != blank and c != end] + [eos]
         memo = {}
 
         def prob(h, w):
@@ -267,7 +308,7 @@ class NGramLM:
             if key in memo:
                 return memo[key]
             n = len(h) + 1
-            lower = prob(h[1:], w) if n > 1 else 1.0 / C
+            lower = prob(h[1:], w) if n > 1 else 1.0 / len(vocab)
             den = denom[n].get(h, 0)
             if den == 0:
                 v = lower
@@ -277,7 +318,6 @@ class NGramLM:
             memo[key] = v
             return v
 
-        vocab = [c for c in range(C) if c != blank] + [eos]
         ngrams = {n: {} for n in range(1, order + 1)}
         for w in vocab:
             ngrams[1][(w,)] = (math.log10(prob((), w)), None)
@@ -289,7 +329,7 @@ class NGramLM:
             for h in denom[n + 1]:
                 p, _ = ngrams[n][h]
                 ngrams[n][h] = (p, math.log10(gamma(n + 1, h)))
-        return cls(order, C, blank, ngrams)
+        return cls(order, C, blank, ngrams, end)
 
     # ------------------------------------------------------------------------------------------
     # device tables
@@ -297,7 +337,8 @@ class NGramLM:
     def host_tables(self):
         """The tables of SbNgramLm as numpy arrays (built once): keys (uint64), vals (int32),
         logp and bow (float64, natural log), tok (int32), and the scalars cap, order, bos,
-        lm_upper, lm_abs.  See include/speech_b200.h for the map's keys and hash."""
+        lm_upper, lm_abs.  See include/speech_b200.h for the map's keys and hash.  With an end
+        class the n-grams that predict </s> are stored too (the attention search scores it)."""
         if self._host is not None:
             return self._host
         bos, eos = self._bos, self._eos
@@ -336,7 +377,7 @@ class NGramLM:
                     abs_b[n] = max(abs_b[n], abs(b))
                     if usable(g):
                         bow[ctx_node(g)] = b
-                if g[-1] in (bos, eos) or not usable(g[:-1]):
+                if g[-1] == bos or (g[-1] == eos and self._end is None) or not usable(g[:-1]):
                     continue                # never looked up
                 upper_p, abs_p = max(upper_p, p), max(abs_p, abs(p))
                 entries.append((key(ctx_node(g[:-1]), g[-1], 1), len(logp)))
@@ -382,3 +423,7 @@ class NGramLM:
         d = dict(self.__dict__)
         d["_dev"] = {}
         return d
+
+    def __setstate__(self, d):
+        d.setdefault("_end", None)          # pickled before LMs had an end class
+        self.__dict__.update(d)

@@ -25,6 +25,8 @@ def check_lm(lm, lm_weight, insertion_bonus, num_classes, blank):
         if lm_weight != 0.0 or insertion_bonus != 0.0:
             raise ValueError("lm_weight / insertion_bonus need an lm")
         return
+    if lm.end is not None:
+        raise ValueError("the LM reads class %d as </s>; the CTC search has no end class" % lm.end)
     if lm.num_classes != num_classes:
         raise ValueError("the LM covers %d classes, the model has %d"
                          % (lm.num_classes, num_classes))

@@ -10,6 +10,7 @@ Reference quirks kept on purpose: end-padding is part of the loss (:58-63), `hx`
 scheduled sampling draws from Python's `random` (:94), `beam_search` handles one utterance (:197)
 and needs the py3 fix list(filter(...)) (:211) - applied here.
 """
+import math
 import random
 
 import numpy as np
@@ -139,7 +140,7 @@ class Seq2Seq(model.Model):
             return [s2s.beam_search(self, x, start_tok, end_tok, beam_size, max_len)]
 
     def recognize(self, inputs, beam_size=10, max_len=200, start_tok=None, end_tok=None,
-                  return_scores=False):
+                  return_scores=False, lm=None, lm_weight=0.0, insertion_bonus=0.0):
         """Beam search of every utterance of a batch at once, from the audio alone.  inputs: the
         (T_i, F) arrays of batch[0].  Each utterance gets `beam_search`'s search on its own (float64
         scores, stable-descending tie order, the same completion and stop rules), bit for bit, and
@@ -148,7 +149,14 @@ class Seq2Seq(model.Model):
         the padded T' for every utterance, or its own conv_out_size(T_b) in the exact-lengths mode.
         Returns B token lists (START first; END last where a hypothesis completed, else the best
         live one), and their float64 scores with return_scores.  Device-resident
-        (functions/s2s.py: beam_search_batch)."""
+        (functions/s2s.py: beam_search_batch).
+
+        Shallow fusion: lm, a speech_b200.lm.NGramLM over the vocabulary with blank = start_tok and
+        end = end_tok (NGramLM.from_arpa(path, preproc.int_to_char, blank=V - 1, end=V - 2)).
+        Candidate c of a hypothesis h then scores logp(c) + (lm_weight * lm(c | h) +
+        insertion_bonus), where lm(end_tok | h) is lm(</s> | h) and the end token earns no bonus;
+        the context of h starts at <s>, its start token.  The returned scores are the fused ones.
+        With lm=None (the default) this is the LM-less search."""
         from ..functions import s2s
         V = self.embedding.num_embeddings
         start_tok = V - 1 if start_tok is None else int(start_tok)
@@ -164,14 +172,37 @@ class Seq2Seq(model.Model):
             raise ValueError("end_tok %d is not a class the model predicts (%d)" % (end_tok, V - 1))
         if len(inputs) == 0:
             raise ValueError("recognize needs at least one utterance")
+        self._check_lm(lm, lm_weight, insertion_bonus, V, start_tok, end_tok)
         lens = self.input_lens(inputs)
         x = self.stage_inputs(inputs)
         with torch.no_grad():
             x = self._encode(x, lens)
             res = s2s.beam_search_batch(self, x, start_tok, end_tok, int(beam_size), int(max_len),
-                                        lens)
+                                        lens, lm, lm_weight, insertion_bonus)
         labels = [list(r[0]) for r in res]
         return (labels, [r[1] for r in res]) if return_scores else labels
+
+    @staticmethod
+    def _check_lm(lm, lm_weight, insertion_bonus, V, start_tok, end_tok):
+        """ValueError unless the fusion arguments of recognize are usable"""
+        if lm is None:
+            if lm_weight != 0.0 or insertion_bonus != 0.0:
+                raise ValueError("lm_weight / insertion_bonus need an lm")
+            return
+        if not (math.isfinite(lm_weight) and lm_weight >= 0.0):
+            raise ValueError("lm_weight must be finite and >= 0, got %r" % (lm_weight,))
+        if not math.isfinite(insertion_bonus):
+            raise ValueError("insertion_bonus must be finite, got %r" % (insertion_bonus,))
+        if lm.num_classes != V:
+            raise ValueError("the LM covers %d classes, the vocabulary has %d" % (lm.num_classes, V))
+        if lm.blank != start_tok:
+            raise ValueError("the LM's blank is class %d, the start token is %d"
+                             % (lm.blank, start_tok))
+        if lm.end != end_tok:
+            raise ValueError("the LM's end class is %r, the end token is %d" % (lm.end, end_tok))
+        if start_tok < V - 1:
+            raise ValueError("with an LM the start token must be the class the model never "
+                             "predicts (%d), got %d" % (V - 1, start_tok))
 
     def collate(self, inputs, labels):
         return self.stage_inputs(inputs), torch.from_numpy(end_pad_concat(labels))

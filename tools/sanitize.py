@@ -27,6 +27,15 @@ l2 = s.loss((inputs, lab2)); l2.backward()
 print("seq2seq ok", l2.item(), [len(h) for h in s.infer((inputs, lab2), max_len=12)],
       s.beam_search(([inputs[0]], [lab2[0]]), beam_size=3, max_len=8))
 print("seq2seq recognize", [len(h) for h in s.recognize(inputs, beam_size=3, max_len=8)])
+lm2 = NGramLM.train(lab2, 3, 30, 29, end=28)
+print("seq2seq recognize with LM", [len(h) for h in s.recognize(
+    inputs, beam_size=3, max_len=8, lm=lm2, lm_weight=0.5, insertion_bonus=1.0)])
+from speech_b200.functions import s2s as s2s_fn
+fits = s2s_fn.beam_select_fits
+s2s_fn.beam_select_fits = lambda K, C: False     # the split selection with the LM
+print("seq2seq recognize with LM, split select", [len(h) for h in s.recognize(
+    inputs, beam_size=3, max_len=8, lm=lm2, lm_weight=0.5, insertion_bonus=1.0)])
+s2s_fn.beam_select_fits = fits
 t = Transducer(80, 28, cfg).cuda()
 l3 = t.loss((inputs, labels)); l3.backward()
 print("transducer ok", l3.item())
