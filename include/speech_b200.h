@@ -639,6 +639,39 @@ int sb_rnnt_pred_step(const float* emb, const int* sym, const float* x, const fl
                       const float* b_hh, float* h, void* y_bf16, int ldy, int R, int K, int Kin,
                       int H, void* stream);
 
+/* Label-free transducer beam search with shallow fusion of the n-gram LM (SbNgramLm above).
+ * The LM's classes are the model's: labels and the blank, no end class.  Per level the caller
+ * enqueues, after the acoustic rows lp (B, K, V) f32 of the frontier slots:
+ *   sb_rnnt_search_lm_rows   per live frontier slot (a workspace of the same search, read for the
+ *                            slots' hypotheses) the fused float64 values
+ *                              f_k = (double)lp_k + (lm_weight * lm(k | h) + insertion_bonus)
+ *                            for every label k, evaluated in that order, and f_blank = (double)
+ *                            lp_blank; written either as rows fused (B, K, V) f64 (full route) or,
+ *                            with fused NULL, as the kp best by (f desc, k asc): sl_val (B, K, kp)
+ *                            f64, sl_idx (B, K, kp) int32 (-inf / -1 padded) and sl_meta (B, K, 2)
+ *                            f64 = {f_blank, the (kp+1)-th f or -inf}
+ *   sb_rnnt_search_round_lm  sb_rnnt_search_round over those f64 rows or lists (same arguments)
+ * h is the hypothesis's last order-1 labels, preceded by <s> where it is shorter (the trie's root
+ * reads as <s>); there is no end-of-sentence term.  A blank emission scores score + f_blank; the
+ * fused values are the scores throughout: the selections, the merges into `done`, the next beam
+ * and out_scores of sb_rnnt_search_final.  With lm_weight = insertion_bonus = 0 the results equal
+ * the LM-less search's bit for bit.
+ * sb_rnnt_search_lm_rows returns SB_ERR_INVALID for a null LM or table pointer, lm_weight < 0, a
+ * non-finite weight or bound, lm->num_classes < V, lm->blank != blank, a cap that is not a power
+ * of two, or what sb_rnnt_search_round rejects (kp < beam_size on the shortlist route included);
+ * SB_ERR_UNSUPPORTED for order > SB_LM_MAX_ORDER or kp > 64.  sb_rnnt_search_round_lm returns
+ * what sb_rnnt_search_round returns. */
+int sb_rnnt_search_lm_rows(const float* lp, double* fused, double* sl_val, int* sl_idx,
+                           double* sl_meta, int kp, const int* tlens, int t, int level, int B,
+                           int T, int S, int V, int beam_size, int blank, const SbNgramLm* lm,
+                           double lm_weight, double insertion_bonus, void* workspace,
+                           size_t workspace_bytes, void* stream);
+int sb_rnnt_search_round_lm(const double* lp, const double* sl_val, const int* sl_idx,
+                            const double* sl_meta, int kp, const int* tlens, int t, int level,
+                            int max_len, int* par, int* sym, int* slot_lens, int B, int T, int S,
+                            int V, int beam_size, int blank, void* workspace,
+                            size_t workspace_bytes, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Scoring (SURVEY.md section 8f rank 4), HOST function: Levenshtein distance of two int32 token
  * sequences; replaces `editdistance.eval` in speech/utils/score.py:15-16.  Returns -1 on invalid

@@ -147,6 +147,12 @@ SIGNATURES = {
                                       _vp, _c_sz, _vp]),
     "sb_rnnt_pred_step": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_int,
                                    _c_int, _c_int, _c_int, _c_int, _vp]),
+    "sb_rnnt_search_lm_rows": (_c_int, [_vp, _vp, _vp, _vp, _vp, _c_int, _vp, _c_int, _c_int,
+                                        _c_int, _c_int, _c_int, _c_int, _c_int, _c_int, _lmp, _db,
+                                        _db, _vp, _c_sz, _vp]),
+    "sb_rnnt_search_round_lm": (_c_int, [_vp, _vp, _vp, _vp, _c_int, _vp, _c_int, _c_int, _c_int,
+                                         _vp, _vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int,
+                                         _c_int, _vp, _c_sz, _vp]),
     "sb_debug_gru_timeline": (_c_int, [_vp]),
     "sb_debug_gru_cluster": (_c_int, [_c_int]),
     "sb_debug_gru_ksplit": (_c_int, [_c_int]),

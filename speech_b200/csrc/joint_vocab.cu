@@ -16,6 +16,7 @@
 // Roofline of the row kernels: memory bandwidth (one fp32 read per logit, plus one bf16 write per
 // logit in the backward pass); the slab is read back from L2 when it fits there.
 #include "common.cuh"
+#include "shortlist.cuh"
 #include <math.h>
 
 #include "../../include/speech_b200.h"
@@ -135,37 +136,9 @@ joint_vocab_bwd_rows_kernel(const float* __restrict__ logits, long long ld,
 
 // ---- shortlist rows: one warp per row.  lp_k = v_k - lse is formed with the same fp32 expression
 // as the lp_full rows of joint_vocab_fwd_rows_kernel (or read as is when lse is NULL), so every
-// shortlisted value is bit-identical to the full tensor's entry.  The row streams through a
-// per-warp buffer of SL_CAP candidates: a class enters it when it ranks above the current
-// threshold by (lp desc, k asc) - ranking on the ROUNDED lp, since v - lse can map distinct logits
-// to equal log-probs - and a full buffer is sorted (bitonic) and cut to its P = kp + 1 best, whose
-// last entry becomes the threshold.  On a random row only O(P log(V1 / P)) classes ever enter.
-// -inf entries are ranked like any other value (the beam search treats them as live). ----
-static constexpr int SL_CAP = 256;     // >= SL_MAX_KP + 1 + 32: one cut leaves room for a warp's row
-static constexpr int SL_MAX_KP = 64;
-
-SB_DEVINL bool sl_better(float a, int ka, float b, int kb) { return a > b || (a == b && ka < kb); }
-
-// sorts bv / bi [0, SL_CAP) best first (entries past `cnt` are padded with the worst key first)
-SB_DEVINL void sl_sort(float* bv, int* bi, int cnt, int lane) {
-  for (int i = cnt + lane; i < SL_CAP; i += 32) { bv[i] = -INFINITY; bi[i] = 0x7fffffff; }
-  __syncwarp();
-  for (int k = 2; k <= SL_CAP; k <<= 1)
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      for (int i = lane; i < SL_CAP; i += 32) {
-        const int l = i ^ j;
-        if (l > i) {
-          const float a = bv[i], c = bv[l];
-          const int ka = bi[i], kc = bi[l];
-          if ((i & k) == 0 ? sl_better(c, kc, a, ka) : sl_better(a, ka, c, kc)) {
-            bv[i] = c; bi[i] = kc; bv[l] = a; bi[l] = ka;
-          }
-        }
-      }
-      __syncwarp();
-    }
-}
-
+// shortlisted value is bit-identical to the full tensor's entry.  The row streams through the
+// warp's top-P selection (shortlist.cuh, P = kp + 1), ranking on the ROUNDED lp, since v - lse can
+// map distinct logits to equal log-probs. ----
 __global__ void __launch_bounds__(256)
 rnnt_shortlist_rows_kernel(const float* __restrict__ v, long long ld, const float* __restrict__ lse,
                            int B, int T, int U1, int V1, int blank, int kp, long long n0,

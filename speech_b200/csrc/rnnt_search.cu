@@ -15,6 +15,18 @@
 // workspace between launches; an utterance past its frames, or whose frame has no live frontier
 // left, returns at once.
 //
+// With an n-gram LM (shallow fusion) the loop enqueues sb_rnnt_search_lm_rows between the rows and
+// the round: per live frontier slot it resolves the hypothesis's LM context once (the trie walked
+// up at most order - 1 labels; the root reads as <s>) and turns the acoustic f32 row into fused
+// float64 values f_k = (double)lp_k + (alpha * lm(k | h) + beta), f_blank = (double)lp_blank:
+// whole rows for the full route, or the kp best by (f desc, k asc) with the (kp+1)-th value for
+// the shortlist route, so that the lists are ranked by the value the search selects on.  One CTA
+// of RL_THREADS per slot spreads the row's lookups over the GPU; each warp streams its classes
+// through the top-P selection of shortlist.cuh and warp 0 merges the warps' lists.
+// sb_rnnt_search_round_lm is then the round over float64 rows / lists: the round kernel knows
+// nothing of the LM, and with alpha = beta = 0 (f = (double)lp exactly) it searches what the f32
+// round searches.
+//
 // Prediction states live in an arena of S + 2 blocks of B x K slots: block l (1 .. S) holds the
 // frontier of level l, blocks 0 and S + 1 take turns as the beam (`cur`) and the next beam.
 // A frontier slot is named by the code level * K + i.
@@ -23,6 +35,8 @@
 // s2s_cell_fwd (csrc/s2s.cu) with its structure (one warp per hidden unit, lanes over K, a group of
 // rows per CTA staged in shared memory), generalised to an input of any width (embedding_dim or H)
 // gathered by symbol, and a hidden state gathered from the parent's slot.
+#include "ngram.cuh"
+#include "shortlist.cuh"
 #include "tsearch.cuh"
 #include <math.h>
 
@@ -100,12 +114,14 @@ __global__ void __launch_bounds__(RS_THREADS) rnnt_search_init_kernel(RsWs w, in
   if (tid < K) slot_lens[b * K + tid] = 0;
 }
 
+// R: the value type of rows and lists, float (acoustic log-probabilities) or double (LM-fused)
+template <class R>
 struct RsRoundParams {
   RsWs w;
-  const float* lp;        // (B, K, V) rows of the level's frontier slots (full route)
-  const float* sl_val;    // (B, K, kp) shortlists of the same rows (shortlist route)
+  const R* lp;            // (B, K, V) rows of the level's frontier slots (full route)
+  const R* sl_val;        // (B, K, kp) shortlists of the same rows (shortlist route)
   const int* sl_idx;
-  const float* sl_meta;   // (B, K, 2)
+  const R* sl_meta;       // (B, K, 2)
   const int* tlens;
   int* par;               // (B, K) out: parent slot of each new frontier slot, -2 = none
   int* sym;               // (B, K) out: its symbol
@@ -113,8 +129,8 @@ struct RsRoundParams {
   int t, level, S, max_len, K, V, kp, blank;
 };
 
-template <bool SHORT>
-__global__ void __launch_bounds__(RS_THREADS, 1) rnnt_search_round_kernel(const RsRoundParams p) {
+template <bool SHORT, class R>
+__global__ void __launch_bounds__(RS_THREADS, 1) rnnt_search_round_kernel(const RsRoundParams<R> p) {
   extern __shared__ unsigned char rs_smem[];
   const int b = blockIdx.x, tid = threadIdx.x, K = p.K, V = p.V;
   __shared__ double fr_s[RS_MAX_BEAM], new_s[RS_MAX_BEAM];
@@ -160,9 +176,9 @@ __global__ void __launch_bounds__(RS_THREADS, 1) rnnt_search_round_kernel(const 
           reinterpret_cast<double*>(rs_smem), K, V, p.blank, nf, fr_s, fr_n, fr_l, can_extend,
           [&](int i, int k) { return p.lp[(row0 + i) * V + k]; }, trie, round_id, nw);
     } else {
-      nsel = ts_expand_shortlist(
+      nsel = ts_expand_shortlist<R>(
           K, V, p.kp, p.blank, nf, fr_s, fr_n, fr_l, can_extend,
-          [&](int i, const float** lv, const int** li, float* beta) {
+          [&](int i, const R** lv, const int** li, R* beta) {
             *lv = p.sl_val + (row0 + i) * p.kp;
             *li = p.sl_idx + (row0 + i) * p.kp;
             *beta = p.sl_meta[2 * (row0 + i) + 1];
@@ -184,6 +200,119 @@ __global__ void __launch_bounds__(RS_THREADS, 1) rnnt_search_round_kernel(const 
     st.ndone = ndone;
     st.round_id = round_id + (nsel >= 0 ? 1 : 0);
     st.nflag = nflag;
+  }
+}
+
+// ---- LM-fused rows --------------------------------------------------------------------------
+static constexpr int RL_THREADS = 256;
+static constexpr int RL_WARPS = RL_THREADS / 32;
+
+struct RsLmRowsParams {
+  RsWs w;
+  const float* lp;        // (B, K, V) acoustic rows of the level's frontier slots
+  double* fused;          // (B, K, V) out: fused rows (full route), or null
+  double* sl_val;         // (B, K, kp) out: fused shortlists (shortlist route)
+  int* sl_idx;
+  double* sl_meta;        // (B, K, 2) out: {blank lp, (kp+1)-th fused value or -inf}
+  const int* tlens;
+  SbNgramLm lm;
+  double alpha, beta;
+  int t, level, K, V, kp, blank;
+};
+
+// One CTA per frontier slot (b, i): grid B * K.
+__global__ void __launch_bounds__(RL_THREADS) rnnt_search_lm_rows_kernel(const RsLmRowsParams p) {
+  __shared__ double buf_v[RL_WARPS][SL_CAP];
+  __shared__ int buf_i[RL_WARPS][SL_CAP];
+  __shared__ int ctx[SB_LM_MAX_ORDER], cnt_w[RL_WARPS];
+  __shared__ int depth_s;
+  const int tid = threadIdx.x, lane = tid & 31, wp = tid >> 5;
+  const int b = blockIdx.x / p.K, i = blockIdx.x - b * p.K, V = p.V, blank = p.blank;
+  const RsState& st = p.w.st[b];
+  const int nf = p.t < p.tlens[b] ? (p.level == 0 ? st.nbeam : st.nfr) : 0;
+  if (i >= nf) return;                            // the round reads no row of this slot
+  if (tid == 0) {
+    const int* nodes = p.w.trie.of(b).nodes;
+    int q = p.level == 0 ? st.beam_n[i] : st.fr_n[i];
+    depth_s = lm_context(p.lm, [&](int) {         // labels most recent first, then <s>
+      if (q <= 0) return -1;
+      const int sym = nodes[2 * q + 1];
+      q = nodes[2 * q];
+      return sym;
+    }, ctx);
+  }
+  __syncthreads();
+  const int depth = depth_s;
+  const size_t row = (size_t)blockIdx.x;
+  const float* lp = p.lp + row * V;
+  const auto fuse = [&](int k, float x) {         // alpha * lm is not contracted into the + beta
+    const double l = lm_backoff(p.lm, ctx, depth, __ldg(p.lm.tok + k));
+    return (double)x + (__dmul_rn(p.alpha, l) + p.beta);
+  };
+  if (p.fused) {
+    for (int k = tid; k < V; k += RL_THREADS) {
+      const float x = lp[k];
+      p.fused[row * V + k] = k == blank ? (double)x : fuse(k, x);
+    }
+    return;
+  }
+  // shortlist route: each warp streams classes wp*128 + [0, 128), then every RL_WARPS*128
+  double* bv = buf_v[wp];
+  int* bi = buf_i[wp];
+  const int P = p.kp + 1;
+  // f_k <= (double)lp_k + bound (alpha >= 0, rounding is monotone): a class whose bound falls below
+  // the threshold cannot enter, and needs no lookup
+  const double bound = __dmul_rn(p.alpha, p.lm.lm_upper) + p.beta;
+  int cnt = 0, tk = 0;
+  bool thr = false;
+  double tv = 0.0;
+  for (int base = wp * 128; base < V; base += RL_WARPS * 128) {
+    double x[4];
+    bool q[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int j = base + e * 32 + lane;
+      q[e] = j < V && j != blank;
+      x[e] = 0.0;
+      if (q[e]) {
+        const float a = lp[j];
+        if (thr && (double)a + bound < tv) {
+          q[e] = false;
+        } else {
+          x[e] = fuse(j, a);
+          q[e] = !thr || sl_better(x[e], j, tv, tk);
+        }
+      }
+    }
+#pragma unroll
+    for (int e = 0; e < 4; ++e)
+      sl_push(bv, bi, cnt, thr, tv, tk, P, lane, q[e], x[e], base + e * 32 + lane);
+  }
+  sl_sort(bv, bi, cnt, lane);                     // each warp's P best first
+  if (lane == 0) cnt_w[wp] = min(cnt, P);
+  __syncthreads();
+  if (wp != 0) return;
+  // warp 0 merges the other warps' lists into its own
+  cnt = cnt_w[0];
+  thr = false;
+  for (int w = 1; w < RL_WARPS; ++w)
+    for (int c = 0; c < cnt_w[w]; c += 32) {
+      const int e = c + lane;
+      bool q = e < cnt_w[w];
+      const double xv = q ? buf_v[w][e] : 0.0;
+      const int k = q ? buf_i[w][e] : 0;
+      q = q && (!thr || sl_better(xv, k, tv, tk));
+      sl_push(bv, bi, cnt, thr, tv, tk, P, lane, q, xv, k);
+    }
+  sl_sort(bv, bi, cnt, lane);
+  const int kp = p.kp;
+  for (int e = lane; e < kp; e += 32) {
+    p.sl_val[row * kp + e] = e < cnt ? bv[e] : -INFINITY;
+    p.sl_idx[row * kp + e] = e < cnt ? bi[e] : -1;
+  }
+  if (lane == 0) {
+    p.sl_meta[2 * row] = (double)lp[blank];
+    p.sl_meta[2 * row + 1] = cnt > kp ? bv[kp] : -INFINITY;
   }
 }
 
@@ -369,12 +498,12 @@ extern "C" int sb_rnnt_search_init(int* slot_lens, int B, int T, int S, int beam
   return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
 }
 
-extern "C" int sb_rnnt_search_round(const float* lp, const float* sl_val, const int* sl_idx,
-                                    const float* sl_meta, int kp, const int* tlens, int t,
-                                    int level, int max_len, int* par, int* sym, int* slot_lens,
-                                    int B, int T, int S, int V, int beam_size, int blank,
-                                    void* workspace, size_t workspace_bytes, void* stream_) {
-  RsRoundParams p;
+template <class R>
+static int rs_round(const R* lp, const R* sl_val, const int* sl_idx, const R* sl_meta, int kp,
+                    const int* tlens, int t, int level, int max_len, int* par, int* sym,
+                    int* slot_lens, int B, int T, int S, int V, int beam_size, int blank,
+                    void* workspace, size_t workspace_bytes, void* stream_) {
+  RsRoundParams<R> p;
   const int rc = rs_ws(workspace, workspace_bytes, B, T, S, beam_size, &p.w);
   if (rc != SB_OK) return rc;
   const bool shortlist = lp == nullptr;
@@ -391,14 +520,63 @@ extern "C" int sb_rnnt_search_round(const float* lp, const float* sl_val, const 
   p.kp = shortlist ? kp : 0; p.blank = blank;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (shortlist) {
-    rnnt_search_round_kernel<true><<<B, RS_THREADS, 0, stream>>>(p);
+    rnnt_search_round_kernel<true, R><<<B, RS_THREADS, 0, stream>>>(p);
   } else {
     if (smem > 40 * 1024 &&
-        cudaFuncSetAttribute(rnnt_search_round_kernel<false>,
+        cudaFuncSetAttribute(rnnt_search_round_kernel<false, R>,
                              cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
       return SB_ERR_CUDA;
-    rnnt_search_round_kernel<false><<<B, RS_THREADS, smem, stream>>>(p);
+    rnnt_search_round_kernel<false, R><<<B, RS_THREADS, smem, stream>>>(p);
   }
+  return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
+}
+
+extern "C" int sb_rnnt_search_round(const float* lp, const float* sl_val, const int* sl_idx,
+                                    const float* sl_meta, int kp, const int* tlens, int t,
+                                    int level, int max_len, int* par, int* sym, int* slot_lens,
+                                    int B, int T, int S, int V, int beam_size, int blank,
+                                    void* workspace, size_t workspace_bytes, void* stream) {
+  return rs_round(lp, sl_val, sl_idx, sl_meta, kp, tlens, t, level, max_len, par, sym, slot_lens,
+                  B, T, S, V, beam_size, blank, workspace, workspace_bytes, stream);
+}
+
+extern "C" int sb_rnnt_search_round_lm(const double* lp, const double* sl_val, const int* sl_idx,
+                                       const double* sl_meta, int kp, const int* tlens, int t,
+                                       int level, int max_len, int* par, int* sym, int* slot_lens,
+                                       int B, int T, int S, int V, int beam_size, int blank,
+                                       void* workspace, size_t workspace_bytes, void* stream) {
+  return rs_round(lp, sl_val, sl_idx, sl_meta, kp, tlens, t, level, max_len, par, sym, slot_lens,
+                  B, T, S, V, beam_size, blank, workspace, workspace_bytes, stream);
+}
+
+extern "C" int sb_rnnt_search_lm_rows(const float* lp, double* fused, double* sl_val, int* sl_idx,
+                                      double* sl_meta, int kp, const int* tlens, int t, int level,
+                                      int B, int T, int S, int V, int beam_size, int blank,
+                                      const SbNgramLm* lm, double lm_weight,
+                                      double insertion_bonus, void* workspace,
+                                      size_t workspace_bytes, void* stream) {
+  RsLmRowsParams p;
+  const int rc = rs_ws(workspace, workspace_bytes, B, T, S, beam_size, &p.w);
+  if (rc != SB_OK) return rc;
+  const bool shortlist = fused == nullptr;
+  if (!lp || !tlens || V <= 0 || blank < 0 || blank >= V || t < 0 || t >= T || level < 0 ||
+      level > S)
+    return SB_ERR_INVALID;
+  if (shortlist && (!sl_val || !sl_idx || !sl_meta || kp < beam_size)) return SB_ERR_INVALID;
+  if (!lm || !lm->keys || !lm->vals || !lm->logp || !lm->bow || !lm->tok) return SB_ERR_INVALID;
+  if (!(lm_weight >= 0.0) || !isfinite(lm_weight) || !isfinite(insertion_bonus))
+    return SB_ERR_INVALID;
+  if (!isfinite(lm->lm_upper) || !isfinite(lm->lm_abs) || lm->num_classes < V) return SB_ERR_INVALID;
+  if (lm->blank != blank) return SB_ERR_INVALID;
+  if (lm->cap <= 0 || (lm->cap & (lm->cap - 1)) || lm->order < 1) return SB_ERR_INVALID;
+  if (lm->order > SB_LM_MAX_ORDER) return SB_ERR_UNSUPPORTED;
+  if (shortlist && kp > SL_MAX_KP) return SB_ERR_UNSUPPORTED;
+  if ((long long)B * beam_size > 0x7fffffffLL) return SB_ERR_UNSUPPORTED;
+  p.lp = lp; p.fused = fused; p.sl_val = sl_val; p.sl_idx = sl_idx; p.sl_meta = sl_meta;
+  p.tlens = tlens; p.lm = *lm; p.alpha = lm_weight; p.beta = insertion_bonus;
+  p.t = t; p.level = level; p.K = beam_size; p.V = V; p.kp = shortlist ? kp : 0; p.blank = blank;
+  rnnt_search_lm_rows_kernel<<<B * beam_size, RL_THREADS, 0,
+                               reinterpret_cast<cudaStream_t>(stream)>>>(p);
   return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
 }
 

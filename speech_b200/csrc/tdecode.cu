@@ -130,7 +130,7 @@ SB_DEVINL void td_search(const TdParams& p) {
             [&](int i, int k) { return lp[((size_t)t * p.U1 + fr_l[i]) * V + k]; }, trie,
             round_id, nw);
       } else {
-        nsel = ts_expand_shortlist(
+        nsel = ts_expand_shortlist<float>(
             K, V, p.kp, p.blank, nf, fr_s, fr_n, fr_l, can_extend,
             [&](int i, const float** lv, const int** li, float* beta) {
               const size_t node = node0 + (size_t)t * p.U1 + fr_l[i];

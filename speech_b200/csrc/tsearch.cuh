@@ -3,7 +3,21 @@
 // emissions into `done`, the two ways of selecting the K best label extensions, and the selection
 // of the next beam.  Where a row of log-probabilities comes from is the caller's: each function
 // takes it as a functor of the frontier entry.  The definition, the tie order and the exactness
-// argument of the shortlist route are in tdecode.cu's header comment.
+// argument of the shortlist route are in tdecode.cu's header comment, for float32 rows.
+//
+// Rows and lists may also hold float64 values: the LM-fused rows of the label-free search
+// (rnnt_search.cu), f_k = (double)lp_k + (alpha * lm(k | h) + beta), blank f = (double)lp_blank.
+// The full route computes fs + f_k, the fused candidate score, with no change.  The shortlist
+// route's argument carries over with float64 in place of float32: a list holds the kp best classes
+// by (f desc, k asc) and beta is the (kp+1)-th f, so a left-out class has f <= beta and, by the
+// monotonicity of fs + f, ties with a selection s only if fs + beta == s.  Given that, a left-out
+// class with f == beta follows every listed entry of value beta (safe when the selected value is
+// beta), and one with f < beta has f <= nextafter(beta, -inf) (the float64 neighbour), so it ties
+// only if fs + nextafter(beta, -inf) == s too.  A selection that fails either test is flagged and
+// its utterance is searched again from longer lists; an unflagged selection is the full route's.
+// Distinct fused values are closer than distinct float32 values can be, so flags are less rare
+// than on float32 lists, but they still need |fs| of about 2^52 times the gap of two classes'
+// fused values.
 //
 // Every function is called by all N threads of the block.  Frontier, beam and the "new" arrays are
 // the caller's shared memory; `done` and the trie may live anywhere.
@@ -23,6 +37,13 @@ SB_DEVINL float td_next_down(float x) {
   const int i = __float_as_int(x);
   if (x == 0.f) return -__int_as_float(1);                 // -(smallest subnormal)
   return __int_as_float(x > 0.f ? i - 1 : i + 1);
+}
+
+// nextafter(x, -inf) for finite x
+SB_DEVINL double td_next_down(double x) {
+  const long long i = __double_as_longlong(x);
+  if (x == 0.0) return -__longlong_as_double(1ll);         // -(smallest subnormal)
+  return __longlong_as_double(x > 0.0 ? i - 1 : i + 1);
 }
 
 // The new frontier of one round: scores, trie nodes, lengths, the frontier entry each extends and
@@ -105,10 +126,11 @@ SB_DEVINL int ts_expand_full(double* cand, int K, int V, int blank, int nf, cons
   return nsel;
 }
 
-// The same selection as a K-way merge of the frontier's shortlists (kp entries, by (lp desc, k
-// asc)), one lane per entry in warp 0.  list(i, &lv, &li, &beta) points at entry i's list and its
-// beta.  Unproven selections are added to *nflag (shared).  Returns as ts_expand_full.
-template <class CanExtend, class List>
+// The same selection as a K-way merge of the frontier's shortlists (kp entries of value type R,
+// float or double, by (value desc, k asc)), one lane per entry in warp 0.  list(i, &lv, &li,
+// &beta) points at entry i's list and its beta.  Unproven selections are added to *nflag
+// (shared).  Returns as ts_expand_full.
+template <class R, class CanExtend, class List>
 SB_DEVINL int ts_expand_shortlist(int K, int V, int kp, int blank, int nf, const double* fr_s,
                                   const int* fr_n, const int* fr_l, CanExtend can_extend, List list,
                                   const BeamTrie& trie, int round_id, TsNew nw, int* nflag) {
@@ -121,9 +143,9 @@ SB_DEVINL int ts_expand_shortlist(int K, int V, int kp, int blank, int nf, const
     const double fs = live ? fr_s[i] : 0.0;
     const bool all_tie = live && fs == -INFINITY;
     const int n = min(kp, V - 1);
-    const float* lv = nullptr;
+    const R* lv = nullptr;
     const int* li = nullptr;
-    float beta = -INFINITY;
+    R beta = -INFINITY;
     if (live && !all_tie) list(i, &lv, &li, &beta);
     const unsigned long long inlist = n >= 64 ? ~0ull : (1ull << n) - 1ull;
     unsigned long long used = 0ull;
@@ -156,7 +178,7 @@ SB_DEVINL int ts_expand_shortlist(int K, int V, int kp, int blank, int nf, const
           ++taken;
         } else {
           used |= 1ull << hq;
-          const float x = lv[hq];
+          const R x = lv[hq];
           if (fs + (double)beta == hs &&
               (x != beta || (beta != -INFINITY && fs + (double)td_next_down(beta) == hs)))
             ++nfl;

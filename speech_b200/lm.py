@@ -1,5 +1,5 @@
-"""Token-level backoff n-gram language model for shallow fusion in the CTC prefix beam search and
-the attention model's beam search.
+"""Token-level backoff n-gram language model for shallow fusion in the CTC prefix beam search, the
+attention model's beam search and the Transducer's label-free beam search.
 
 The LM is over the acoustic model's own output classes (characters or subword units); the blank is
 never an LM token.  Orders 1..10, with a sentence start <s>, an end </s> and optionally <unk>.
@@ -16,6 +16,13 @@ Values are held as the ARPA file's log10 numbers and converted once to natural l
     lm = NGramLM.train([preproc.encode(t) for t in texts], order=5, num_classes=V, blank=V - 1,
                        end=V - 2)
     s2s_model.recognize(inputs, beam_size=8, lm=lm, lm_weight=0.5, insertion_bonus=0.5)
+
+The Transducer's classes are laid out as CTC's (labels 0..V-1, the blank V last, no end class), so
+the same LM shape serves its label-free beam search:
+
+    lm = NGramLM.from_arpa("chars.arpa", preproc.int_to_char)    # blank = last class
+    lm = NGramLM.train(transcripts, order=5, num_classes=V + 1, blank=V)
+    transducer.recognize(inputs, beam_size=8, lm=lm, lm_weight=0.5, insertion_bonus=1.0)
 
 lm(s | h) follows ARPA backoff: h is the prefix's last order-1 symbols, preceded by <s> where the
 prefix is shorter; when the n-gram (h, s) is stored its log-probability is used, otherwise the

@@ -18,15 +18,16 @@ import torch
 from .. import _lib
 
 
-def check_lm(lm, lm_weight, insertion_bonus, num_classes, blank):
+def check_lm(lm, lm_weight, insertion_bonus, num_classes, blank, search="CTC"):
     """ValueError unless the fusion arguments are usable with a model of num_classes classes whose
-    blank is `blank`"""
+    blank is `blank`; `search` names the search in the refusal of an LM with an end class"""
     if lm is None:
         if lm_weight != 0.0 or insertion_bonus != 0.0:
             raise ValueError("lm_weight / insertion_bonus need an lm")
         return
     if lm.end is not None:
-        raise ValueError("the LM reads class %d as </s>; the CTC search has no end class" % lm.end)
+        raise ValueError("the LM reads class %d as </s>; the %s search has no end class"
+                         % (lm.end, search))
     if lm.num_classes != num_classes:
         raise ValueError("the LM covers %d classes, the model has %d"
                          % (lm.num_classes, num_classes))

@@ -17,6 +17,7 @@ from . import model
 from .. import ops
 from ..functions import transducer as transducer_fn
 from .. import _lib
+from .ctc_decoder import check_lm
 from ..transducer_decoders import (decode_static_batch, decode_static_fits, decode_static_shortlist,
                                    search_batch)
 
@@ -146,17 +147,25 @@ class Transducer(model.Model):
         return preds
 
     def recognize(self, inputs, beam_size=4, max_symbols_per_frame=4, max_len=None,
-                  return_scores=False):
+                  return_scores=False, lm=None, lm_weight=0.0, insertion_bonus=0.0):
         """Beam search from the audio alone: `infer`'s search with the row of each hypothesis
         computed by the prediction network reading the hypothesis's own labels (dropout off),
         instead of the reference transcript.  inputs: the (T_i, F) arrays of batch[0].  A frame
         emits at most max_symbols_per_frame labels; a hypothesis with max_len labels (default: no
         cap beyond frames * max_symbols_per_frame) is not extended.  Frames searched: the padded T'
         for every utterance, or its own conv_out_size(T_b) in the exact-lengths mode.
-        Returns the label lists (and their float64 log-probabilities with return_scores)."""
+        lm (optional): a speech_b200.lm.NGramLM over the model's V+1 classes (labels 0..V-1, the
+        blank V, no end class), fused into every label extension as lp + (lm_weight * lm(k | h) +
+        insertion_bonus), h the hypothesis's last order-1 labels after <s>; blank emissions keep
+        their log-probability.  Bad fusion arguments raise ValueError before any launch.
+        Returns the label lists (and their float64 scores with return_scores: log-probabilities,
+        or with an LM the fused scores)."""
+        check_lm(lm, lm_weight, insertion_bonus, self.fc2.fc.out_features, self.blank,
+                 search="Transducer")
         rows = PredictionRows(self, inputs)
         labels, scores = search_batch(rows, rows.tlens, beam_size, self.blank,
-                                      max_symbols_per_frame, max_len)
+                                      max_symbols_per_frame, max_len, lm, lm_weight,
+                                      insertion_bonus)
         return (labels, scores) if return_scores else labels
 
     def label_collate(self, labels):

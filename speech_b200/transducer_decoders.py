@@ -15,6 +15,8 @@ best non-blank classes, csrc/tdecode.cu), with the same results bit for bit: the
 selection the lists cannot prove, and flagged utterances are searched again from lists of
 SHORTLIST_RERUN entries.
 """
+import ctypes
+
 import torch
 
 from . import _lib, ops
@@ -154,24 +156,42 @@ def decode_static(lp, beam_size, blank=0):
 # Label-free search (csrc/rnnt_search.cu): decode_static's search with the row of hypothesis h at
 # frame t computed from h itself.  A row provider supplies the rows; Transducer.recognize passes the
 # prediction and joint networks (models/transducer_model.PredictionRows), tests pass a static
-# lattice.  Its CPU restatement is oracle/rnnt_search_ref.py.
+# lattice.  Its CPU restatement is oracle/rnnt_search_ref.py.  With an n-gram LM (shallow fusion)
+# each level's acoustic rows become fused float64 rows or shortlists on the device
+# (sb_rnnt_search_lm_rows) before the round reads them.
 # ------------------------------------------------------------------------------------------------
 class SearchSlots:
     """Device tensors of one search that a row provider reads: B, K, S, T, kp (None: full rows);
     par / sym / slot_lens (B, K) int32 (csrc/rnnt_search.cu), lp (B, K, V1) f32 or sl (the
-    shortlists, alloc_shortlists(B, 1, K, kp)) that rows() fills."""
+    shortlists, alloc_shortlists(B, 1, K, kp)) that rows() fills: whichever is not None.
+    With an LM (fused=True) rows() always fills the acoustic rows lp and sl is None; the search
+    writes the fused float64 values itself, into flp (B, K, V1) f64 on the full route or fsl =
+    (values (B, K, kp) f64, classes (B, K, kp) int32, {blank lp, next value} (B, K, 2) f64)."""
 
-    def __init__(self, B, K, S, T, V1, kp, dev):
+    def __init__(self, B, K, S, T, V1, kp, dev, fused=False):
         self.B, self.K, self.S, self.T, self.kp = B, K, S, T, kp
         self.par, self.sym, self.slot_lens = torch.zeros(3, B, K, dtype=torch.int32, device=dev)
-        self.lp = torch.empty(B, K, V1, dtype=torch.float32, device=dev) if kp is None else None
-        self.sl = None if kp is None else alloc_shortlists(B, 1, K, kp, dev)
+        full = kp is None or fused
+        self.lp = torch.empty(B, K, V1, dtype=torch.float32, device=dev) if full else None
+        self.sl = None if full else alloc_shortlists(B, 1, K, kp, dev)
+        self.flp = self.fsl = None
+        if fused and kp is None:
+            self.flp = torch.empty(B, K, V1, dtype=torch.float64, device=dev)
+        elif fused:
+            self.fsl = (torch.empty(B, K, kp, dtype=torch.float64, device=dev),
+                        torch.empty(B, K, kp, dtype=torch.int32, device=dev),
+                        torch.empty(B, K, 2, dtype=torch.float64, device=dev))
 
 
-def _search_once(provider, tl, T, K, S, max_len, L, blank, kp):
+def _search_once(provider, tl, T, K, S, max_len, L, blank, kp, fusion=None):
+    """one search at list length kp (None: full rows); fusion: None or (NGramLM, lm_weight,
+    insertion_bonus) -> (label lists, scores, flag counts)"""
     lib = _lib.load()
     B, V1, dev = provider.B, provider.V1, provider.device
-    slots = SearchSlots(B, K, S, T, V1, kp, dev)
+    slots = SearchSlots(B, K, S, T, V1, kp, dev, fused=fusion is not None)
+    if fusion is not None:
+        tables, _ = fusion[0].device_tables(dev)
+        weights = (float(fusion[1]), float(fusion[2]))
     nbytes = _lib.workspace_size(lib.sb_rnnt_search_workspace_size, B, T, S, K)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     tl_dev = torch.tensor(tl, dtype=torch.int32).pin_memory().to(dev, non_blocking=True)
@@ -192,11 +212,23 @@ def _search_once(provider, tl, T, K, S, max_len, L, blank, kp):
             for level in range(S + 1):
                 block = cur if level == 0 else level
                 provider.rows(t, block, slots)
-                ops._launch("rnnt_search", 0.0, lambda: lib.sb_rnnt_search_round(
-                    _lib.ptr(slots.lp), *(_lib.ptr(a) for a in (sl or (None,) * 3)), kp or 0,
-                    tl_dev.data_ptr(), t, level, max_len, slots.par.data_ptr(),
-                    slots.sym.data_ptr(), slots.slot_lens.data_ptr(), B, T, S, V1, K, blank,
-                    ws.data_ptr(), nbytes, sp))
+                if fusion is None:
+                    ops._launch("rnnt_search", 0.0, lambda: lib.sb_rnnt_search_round(
+                        _lib.ptr(slots.lp), *(_lib.ptr(a) for a in (sl or (None,) * 3)), kp or 0,
+                        tl_dev.data_ptr(), t, level, max_len, slots.par.data_ptr(),
+                        slots.sym.data_ptr(), slots.slot_lens.data_ptr(), B, T, S, V1, K, blank,
+                        ws.data_ptr(), nbytes, sp))
+                else:
+                    fsl = tuple(_lib.ptr(a) for a in (slots.fsl or (None,) * 3))
+                    ops._launch("rnnt_search_lm_rows", 0.0, lambda: lib.sb_rnnt_search_lm_rows(
+                        slots.lp.data_ptr(), _lib.ptr(slots.flp), *fsl, kp or 0,
+                        tl_dev.data_ptr(), t, level, B, T, S, V1, K, blank,
+                        ctypes.byref(tables), *weights, ws.data_ptr(), nbytes, sp))
+                    ops._launch("rnnt_search", 0.0, lambda: lib.sb_rnnt_search_round_lm(
+                        _lib.ptr(slots.flp), *fsl, kp or 0, tl_dev.data_ptr(), t, level,
+                        max_len, slots.par.data_ptr(), slots.sym.data_ptr(),
+                        slots.slot_lens.data_ptr(), B, T, S, V1, K, blank, ws.data_ptr(), nbytes,
+                        sp))
                 if level < S:
                     provider.extend(block, level + 1, slots)
             hid, layers, H, fy, Hj = provider.arenas()
@@ -215,21 +247,32 @@ def _search_once(provider, tl, T, K, S, max_len, L, blank, kp):
     return [lab[b, :n[b]].tolist() for b in range(B)], sc, fl
 
 
-def search_batch(provider, tlens, beam_size, blank, max_symbols_per_frame, max_len=None):
+def search_batch(provider, tlens, beam_size, blank, max_symbols_per_frame, max_len=None, lm=None,
+                 lm_weight=0.0, insertion_bonus=0.0):
     """Label-free beam search of a batch.  provider: B, T (frames available), V1, device, and
     begin(slots) (states of the empty hypothesis in block 0), rows(t, block, slots) (rows of the K
-    frontier slots of `block` at frame t into slots.lp or slots.sl), extend(src, dst, slots) (states
+    frontier slots of `block` at frame t into slots.lp and / or slots.sl, whichever is not None;
+    with an LM only slots.lp is given), extend(src, dst, slots) (states
     of the new frontier, slots.par / slots.sym, in block dst from block src), arenas() -> (hid,
     layers, H, fy, Hj) (None, 0, 0, None, 0 without states).  tlens: frames searched per utterance
     (clamped to T).  A frame emits at most max_symbols_per_frame labels; a hypothesis with max_len
     labels (default: frames * max_symbols_per_frame) is not extended.  Rows through shortlists
     where the full candidate list does not fit (decode_static_fits), with decode_static_shortlist's
     rerun of flagged utterances from SHORTLIST_RERUN-entry lists (the whole batch, so that every row
-    is computed as in the first pass).  Returns (list of label lists, list of float64 scores)."""
+    is computed as in the first pass).
+    lm (optional): a speech_b200.lm.NGramLM over the V1 classes with the search's blank and no end
+    class, fused into every label extension as lp_k + (lm_weight * lm(k | h) + insertion_bonus);
+    blank emissions keep lp_blank.  The fused values are the scores everywhere, the returned ones
+    included; lm_weight = insertion_bonus = 0 gives the LM-less search's results bit for bit.
+    Bad fusion arguments raise ValueError before any launch.
+    Returns (list of label lists, list of float64 scores)."""
+    from .models.ctc_decoder import check_lm
     B, T, V1 = provider.B, provider.T, provider.V1
     K, S = int(beam_size), int(max_symbols_per_frame)
     if K <= 0 or S <= 0:
         raise ValueError("beam_size and max_symbols_per_frame must be positive")
+    check_lm(lm, lm_weight, insertion_bonus, V1, blank, search="Transducer")
+    fusion = None if lm is None else (lm, lm_weight, insertion_bonus)
     tl = [max(0, min(int(t), T)) for t in tlens]
     if len(tl) != B:
         raise ValueError("tlens must have one entry per utterance")
@@ -238,12 +281,13 @@ def search_batch(provider, tlens, beam_size, blank, max_symbols_per_frame, max_l
     cap = T * S if max_len is None else min(int(max_len), T * S)
     L = max(1, cap)
     if decode_static_fits(K, V1):
-        labels, scores, _ = _search_once(provider, tl, T, K, S, cap, L, blank, None)
+        labels, scores, _ = _search_once(provider, tl, T, K, S, cap, L, blank, None, fusion)
         return labels, scores
-    labels, scores, flags = _search_once(provider, tl, T, K, S, cap, L, blank, K)
+    labels, scores, flags = _search_once(provider, tl, T, K, S, cap, L, blank, K, fusion)
     rerun = [b for b, f in enumerate(flags) if f]
     if rerun:
-        lab2, sc2, fl2 = _search_once(provider, tl, T, K, S, cap, L, blank, SHORTLIST_RERUN)
+        lab2, sc2, fl2 = _search_once(provider, tl, T, K, S, cap, L, blank, SHORTLIST_RERUN,
+                                      fusion)
         bad = [b for b in rerun if fl2[b]]
         if bad:
             raise _lib.SpeechB200Error(

@@ -195,3 +195,22 @@ for tm, V1, beam in ((t, 29, 4), (t2, 301, 32), (tv, 20001, 4)):
     tm.set_eval()
     print("recognize V+1=%d beam %d" % (V1, beam),
           [len(p) for p in tm.recognize(inputs[:3], beam_size=beam, max_symbols_per_frame=2)])
+# with an n-gram LM: the fused rows and the f64 rounds, full rows at V+1 = 29, shortlists at
+# V+1 = 301 (forced, as the split selection above) and 20001
+from speech_b200 import transducer_decoders as tdec
+lm_t = NGramLM.train(labels, 3, 29, 28)
+print("recognize with LM V+1=29", [len(p) for p in t.recognize(
+    inputs[:3], beam_size=4, max_symbols_per_frame=2, lm=lm_t, lm_weight=0.5,
+    insertion_bonus=1.0)])
+fits_t = tdec.decode_static_fits
+tdec.decode_static_fits = lambda K, V: False     # the shortlist route with the LM
+lm_t2 = NGramLM.train(labels2, 3, 301, 300)
+print("recognize with LM V+1=301, shortlists", [len(p) for p in t2.recognize(
+    inputs[:3], beam_size=4, max_symbols_per_frame=2, lm=lm_t2, lm_weight=0.5,
+    insertion_bonus=1.0)])
+tdec.decode_static_fits = fits_t
+lm_tv = NGramLM.train(labels4, 3, 20001, 20000)
+print("recognize with LM V+1=20001", [len(p) for p in tv.recognize(
+    inputs[:3], beam_size=4, max_symbols_per_frame=2, lm=lm_tv, lm_weight=0.5,
+    insertion_bonus=1.0)])
+torch.cuda.synchronize()
