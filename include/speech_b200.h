@@ -70,6 +70,32 @@ int sb_ctc_fwd_bwd_compact(const float* acts, float* grads, const int* labels,
                            int B, int T, int V, int blank, int max_label_len, float* costs,
                            void* workspace, size_t workspace_bytes, void* stream);
 
+/* CTC Viterbi (forced) alignment (csrc/ctc.cu): the single best path through the lattice the
+ * loss sums over.  Arguments as sb_ctc_fwd_bwd (raw logits, any V, max_label_len <= 1023).  Every
+ * frame is reduced by the compact path's kernels; the log-probability of a kept class at frame t
+ * is its compact column minus the frame's full-row log-sum-exp (float32).  The recursion runs in
+ * float64 over l' = (blank, y1, blank, ..., yL, blank), S = 2L+1:
+ *   d[0][0] = lp(0, blank), d[0][1] = lp(0, y1),
+ *   d[t][s] = max(d[t-1][s], d[t-1][s-1], d[t-1][s-2]) + lp(t, l'_s), the s-2 step only where
+ *   l'_s is not blank and l'_s != l'_{s-2}; the path ends in S-1 or S-2.
+ * Tie rule: on equal scores the predecessor s wins over s-1, and s-1 over s-2; at the end S-1
+ * wins over S-2.
+ *   path     (B, T) int32 out: the label index j (0-based) frame t is aligned to, -1 for blank,
+ *            -2 for frames >= act_lens[b]; all -2 where no alignment exists
+ *   scores   (B) float64 out: the path's log-probability; -inf where no alignment exists
+ *            (act_lens[b] < L + the number of adjacent repeats: the loss's +inf cost).  An empty
+ *            transcript aligns every frame to blank.
+ *   workspace >= sb_ctc_viterbi_workspace_size(...) bytes: the compact rows (B*T*(max_label_len+2)
+ *            floats), the row log-sum-exps, the column map and 2-bit backpointers (B * T *
+ *            ceil((2*max_label_len+1) / 256) * 64 bytes, the count rounded up to 1, 2, 4 or 8).
+ * Same argument checks and status codes as sb_ctc_fwd_bwd (path / scores non-NULL too); every
+ * SB_ERR_INVALID / SB_ERR_UNSUPPORTED is returned before any launch. */
+int sb_ctc_viterbi_workspace_size(int B, int T, int V, int max_label_len, size_t* bytes);
+int sb_ctc_viterbi(const float* acts, const int* labels, const int* label_offsets,
+                   const int* label_lens, const int* act_lens, int B, int T, int V, int blank,
+                   int max_label_len, int* path, double* scores, void* workspace,
+                   size_t workspace_bytes, void* stream);
+
 /* ---------------------------------------------------------------------------------------
  * Dense contraction on wgmma tensor cores:
  *     C[M,N] (f32)  (+)=  A[M,K] (bf16, row-major) * B[N,K]^T (bf16, row-major)  (+ bias[N])
@@ -487,6 +513,27 @@ int sb_rnnt_fwd_bwd_compact(const float* lat, float* garc, const int* labels,
                             const int* label_offsets, const int* label_lens, const int* act_lens,
                             int B, int T, int U1, int blank, float* costs, void* workspace,
                             size_t workspace_bytes, void* stream);
+
+/* Transducer Viterbi (forced) alignment over the same compact lattice (csrc/rnnt.cu): the single
+ * best path, in float64,
+ *   a[0][0] = 0,  a[t][u] = max(a[t-1][u] + blank(t-1, u), a[t][u-1] + label(t, u-1)),
+ *   score = a[T_b-1][U_b] + blank(T_b-1, U_b).
+ * Tie rule: where the two arcs into (t, u) score equal, the max takes the blank arc from (t-1, u),
+ * i.e. the path on which label u-1 was emitted at an earlier frame; read back from (T_b-1, U_b),
+ * each label is thus emitted at the earliest frame among equal paths, the last label first (on a
+ * lattice of equal values every label is emitted at frame 0).  Shapes as sb_rnnt_fwd_bwd_compact
+ * (U1 <= 1024); the labels are not read.
+ *   frames   (B, U1-1) int32 out: the frame at which label u is emitted; -1 past U_b, and
+ *            everywhere when the score is -inf
+ *   scores   (B) float64 out: the path's log-probability; -inf where act_lens[b] = 0
+ *   workspace >= sb_rnnt_viterbi_workspace_size(...) bytes: 1-bit backpointers by anti-diagonal,
+ *            B * (T + U1) * ceil(U1 / 256) * 32 bytes (the count rounded up to 1, 2 or 4), + 256.
+ * SB_ERR_INVALID for a NULL pointer or B, T, U1 <= 0; SB_ERR_UNSUPPORTED for U1 > 1024; both
+ * before any launch. */
+int sb_rnnt_viterbi_workspace_size(int B, int T, int U1, size_t* bytes);
+int sb_rnnt_viterbi(const float* lat, const int* labels, const int* label_offsets,
+                    const int* label_lens, const int* act_lens, int B, int T, int U1, int* frames,
+                    double* scores, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Fused RNN-T joint network: relu(fx[b,t,:] + fy[b,u,:]) -> fc2 -> log-softmax per lattice node,

@@ -39,6 +39,10 @@ SIGNATURES = {
                                                ctypes.POINTER(_c_sz)]),
     "sb_ctc_fwd_bwd_compact": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _c_int, _c_int, _c_int,
                                         _c_int, _c_int, _vp, _vp, _c_sz, _vp]),
+    "sb_ctc_viterbi_workspace_size": (_c_int, [_c_int, _c_int, _c_int, _c_int,
+                                               ctypes.POINTER(_c_sz)]),
+    "sb_ctc_viterbi": (_c_int, [_vp, _vp, _vp, _vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int,
+                                _vp, _vp, _vp, _c_sz, _vp]),
     "sb_gemm_bf16_tn": (_c_int, [_vp, _c_ll, _vp, _c_ll, _vp, _c_ll, _vp, _c_int, _c_int, _c_int,
                                  _c_int, _c_int, _c_int, _c_int, _c_int, _vp]),
     "sb_ctc_prefix_beam_workspace_size": (_c_int, [_c_int, _c_int, _c_int, ctypes.POINTER(_c_sz)]),
@@ -112,6 +116,9 @@ SIGNATURES = {
                                  _vp, _vp, _c_sz, _vp]),
     "sb_rnnt_fwd_bwd_compact": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _c_int, _c_int, _c_int, _c_int,
                                          _vp, _vp, _c_sz, _vp]),
+    "sb_rnnt_viterbi_workspace_size": (_c_int, [_c_int, _c_int, _c_int, ctypes.POINTER(_c_sz)]),
+    "sb_rnnt_viterbi": (_c_int, [_vp, _vp, _vp, _vp, _vp, _c_int, _c_int, _c_int, _vp, _vp, _vp,
+                                 _c_sz, _vp]),
     "sb_rnnt_joint_fwd": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_int, _c_int, _c_int, _c_int,
                                    _c_int, _c_int, _vp]),
     "sb_rnnt_joint_dlogits": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_int, _c_int,

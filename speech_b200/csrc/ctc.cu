@@ -642,6 +642,160 @@ static int ctc_run_compact(const CtcParams& full, int max_label_len, int ns, voi
   return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
 }
 
+// ------------------------------------------------------------------------------------------------
+// Viterbi alignment (sb_ctc_viterbi).  The compact path's column map and row kernels reduce every
+// frame first (any V); then one CTA of 256 threads per utterance runs the max-plus recursion over
+// the extended labels, states s = i + 256*q, two float64 rows ping-ponged in shared memory, one
+// barrier per frame.  Each warp packs its 32 states' 2-bit backpointers into one uint2 per frame
+// with two ballots (bit 0 in .x, bit 1 in .y); warp 0 then walks them back, 32 frames per batch of
+// loads: over 32 frames the state drops by at most 62, i.e. into the 3 words below and at its own.
+// ------------------------------------------------------------------------------------------------
+struct CtcViterbi {
+  const float* acts_c;   // (B, T, Vc) compact rows
+  const float* lse;      // (B, T) full-row log-sum-exp
+  const int* lab_c;      // labels as columns, utterance b at b * Lstride
+  const int* label_lens;
+  const int* act_lens;
+  uint2* bp;             // (B, T, NS * 8) backpointers
+  int* path;             // (B, T)
+  double* scores;        // (B)
+  int B, T, Vc, Lmax, Lstride;
+};
+
+template <int NS>
+__global__ void __launch_bounds__(CTC_SIDE) ctc_viterbi_kernel(const CtcViterbi p) {
+  constexpr int NW = NS * CTC_SIDE / 32;   // backpointer words per frame
+  __shared__ double rows[2][NS * CTC_SIDE + 2];
+  __shared__ int s_end;
+  const int b = blockIdx.x, i = threadIdx.x, warp = i >> 5, lane = i & 31;
+  const int Tb = max(0, min(p.act_lens[b], p.T));
+  const int L = max(0, min(p.label_lens[b], p.Lmax));
+  const int S = 2 * L + 1;
+  const int* lab = p.lab_c + (size_t)b * p.Lstride;
+  const float* ac = p.acts_c + (size_t)b * p.T * p.Vc;
+  const float* lz = p.lse + (size_t)b * p.T;
+  uint2* bp = p.bp + (size_t)b * p.T * NW;
+  int* path = p.path + (size_t)b * p.T;
+
+  int col[NS];
+  bool skip[NS], valid[NS];
+#pragma unroll
+  for (int q = 0; q < NS; ++q) {
+    const int s = i + CTC_SIDE * q;
+    valid[q] = s < S;
+    col[q] = 0;
+    skip[q] = false;
+    if (valid[q] && (s & 1)) {
+      const int j = (s - 1) >> 1;
+      col[q] = lab[j];
+      skip[q] = j > 0 && col[q] != 0 && lab[j - 1] != col[q];
+    }
+  }
+  for (int k = i; k < 2 * (NS * CTC_SIDE + 2); k += CTC_SIDE) (&rows[0][0])[k] = -INFINITY;
+  __syncthreads();
+
+  // log-probability of this thread's states at frame t: compact column minus the full row's
+  // log-sum-exp, in float32 as the compact loss path forms it
+  auto emit = [&](int t, float (&e)[NS]) {
+    const float z = __ldg(lz + t);
+#pragma unroll
+    for (int q = 0; q < NS; ++q) e[q] = valid[q] ? __ldg(ac + (size_t)t * p.Vc + col[q]) - z : 0.f;
+  };
+  float e[NS];
+  if (Tb > 0) emit(0, e);
+  for (int t = 0; t < Tb; ++t) {
+    float en[NS];
+    if (t + 1 < Tb) emit(t + 1, en);   // the next frame's loads overlap this frame's step
+    double* cur = rows[t & 1] + 2;
+    const double* prv = rows[(t & 1) ^ 1] + 2;
+#pragma unroll
+    for (int q = 0; q < NS; ++q) {
+      const int s = i + CTC_SIDE * q;
+      unsigned code = 0;   // predecessor s - code; ties keep the smaller code
+      if (valid[q]) {
+        double v = -INFINITY;
+        if (t == 0) {
+          if (s <= 1) v = (double)e[q];
+        } else {
+          double best = prv[s];
+          if (prv[s - 1] > best) { best = prv[s - 1]; code = 1; }
+          if (skip[q] && prv[s - 2] > best) { best = prv[s - 2]; code = 2; }
+          v = best + (double)e[q];
+        }
+        cur[s] = v;
+      }
+      const unsigned lo = __ballot_sync(0xffffffffu, code & 1u);
+      const unsigned hi = __ballot_sync(0xffffffffu, code >> 1);
+      if (lane == 0) bp[(size_t)t * NW + q * (CTC_SIDE / 32) + warp] = make_uint2(lo, hi);
+    }
+    __syncthreads();
+#pragma unroll
+    for (int q = 0; q < NS; ++q) e[q] = en[q];
+  }
+
+  if (i == 0) {
+    double sc = L == 0 ? 0.0 : -INFINITY;
+    int end = -1;
+    if (Tb > 0) {
+      const double* last = rows[(Tb - 1) & 1] + 2;
+      sc = last[S - 1];
+      end = S - 1;
+      if (S >= 2 && last[S - 2] > sc) { sc = last[S - 2]; end = S - 2; }
+    }
+    if (sc == -INFINITY) end = -1;
+    p.scores[b] = sc;
+    s_end = end;
+  }
+  __syncthreads();
+  const int end = s_end;
+  for (int t = (end < 0 ? 0 : Tb) + i; t < p.T; t += CTC_SIDE) path[t] = -2;
+  if (end < 0 || warp != 0) return;
+
+  int s = end;
+  for (int t1 = Tb - 1; t1 >= 0; t1 -= 32) {
+    const int w0 = s >> 5;
+    const int tl = t1 - lane;
+    uint2 wd[3] = {make_uint2(0u, 0u), make_uint2(0u, 0u), make_uint2(0u, 0u)};
+    if (tl >= 0) {
+#pragma unroll
+      for (int k = 0; k < 3; ++k)
+        if (w0 - k >= 0) wd[k] = __ldcg(bp + (size_t)tl * NW + w0 - k);
+    }
+    int mine = -2;
+    const int n = min(32, t1 + 1);
+    for (int k = 0; k < n; ++k) {
+      const int dw = w0 - (s >> 5);
+      const unsigned lo0 = __shfl_sync(0xffffffffu, wd[0].x, k), hi0 = __shfl_sync(0xffffffffu, wd[0].y, k);
+      const unsigned lo1 = __shfl_sync(0xffffffffu, wd[1].x, k), hi1 = __shfl_sync(0xffffffffu, wd[1].y, k);
+      const unsigned lo2 = __shfl_sync(0xffffffffu, wd[2].x, k), hi2 = __shfl_sync(0xffffffffu, wd[2].y, k);
+      const unsigned lo = dw == 0 ? lo0 : (dw == 1 ? lo1 : lo2);
+      const unsigned hi = dw == 0 ? hi0 : (dw == 1 ? hi1 : hi2);
+      if (lane == k) mine = (s & 1) ? (s - 1) >> 1 : -1;
+      s -= (int)(((lo >> (s & 31)) & 1u) | (((hi >> (s & 31)) & 1u) << 1));
+    }
+    if (lane < n) path[t1 - lane] = mine;
+  }
+}
+
+struct CtcViterbiLayout {
+  size_t acts_c, lse, lab_c, off_c, col_cls, ncols, bp, total;
+};
+static CtcViterbiLayout ctc_viterbi_layout(int B, int T, int max_label_len, int ns) {
+  const int Vc = max_label_len + 2;
+  const size_t rows = (size_t)B * T;
+  CtcViterbiLayout l;
+  size_t o = 256;   // slack for aligning the base pointer
+  l.acts_c = o;  o += align256(rows * Vc * sizeof(float));
+  l.lse = o;     o += align256(rows * sizeof(float));
+  l.lab_c = o;   o += align256((size_t)B * (max_label_len > 0 ? max_label_len : 1) * sizeof(int));
+  l.off_c = o;   o += align256((size_t)B * sizeof(int));
+  l.col_cls = o; o += align256((size_t)B * Vc * sizeof(int));
+  l.ncols = o;   o += align256((size_t)B * sizeof(int));
+  l.bp = o;      o += align256(rows * (size_t)(ns * CTC_SIDE / 32) * sizeof(uint2));
+  l.total = o;
+  return l;
+}
+
 }  // namespace sb
 
 using namespace sb;
@@ -709,4 +863,65 @@ extern "C" int sb_ctc_fwd_bwd_compact(const float* acts, float* grads, const int
                                       size_t workspace_bytes, void* stream) {
   return ctc_entry(acts, grads, labels_dev, label_offsets_dev, label_lens_dev, act_lens_dev, B, T,
                    V, blank, max_label_len, costs, workspace, workspace_bytes, stream, true);
+}
+
+extern "C" int sb_ctc_viterbi_workspace_size(int B, int T, int V, int max_label_len,
+                                             size_t* bytes) {
+  if (!bytes || B <= 0 || T < 0 || V <= 0 || max_label_len < 0) return SB_ERR_INVALID;
+  const int ns = ctc_ns_for(max_label_len);
+  if (ns < 0) return SB_ERR_UNSUPPORTED;
+  *bytes = ctc_viterbi_layout(B, T > 0 ? T : 1, max_label_len, ns).total;
+  return SB_OK;
+}
+
+extern "C" int sb_ctc_viterbi(const float* acts, const int* labels_dev,
+                              const int* label_offsets_dev, const int* label_lens_dev,
+                              const int* act_lens_dev, int B, int T, int V, int blank,
+                              int max_label_len, int* path, double* scores, void* workspace,
+                              size_t workspace_bytes, void* stream_) {
+  if (!acts || !labels_dev || !label_offsets_dev || !label_lens_dev || !act_lens_dev || !path ||
+      !scores || !workspace)
+    return SB_ERR_INVALID;
+  if (B <= 0 || T <= 0 || V <= 0 || blank < 0 || blank >= V || max_label_len < 0)
+    return SB_ERR_INVALID;
+  const int ns = ctc_ns_for(max_label_len);
+  if (ns < 0) return SB_ERR_UNSUPPORTED;
+  const CtcViterbiLayout l = ctc_viterbi_layout(B, T, max_label_len, ns);
+  if (workspace_bytes < l.total) return SB_ERR_WORKSPACE;
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  unsigned char* base = reinterpret_cast<unsigned char*>(
+      (reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255) - 256;
+
+  CtcCompact c;
+  c.acts = acts; c.grads = nullptr; c.labels = labels_dev; c.label_off = label_offsets_dev;
+  c.label_lens = label_lens_dev; c.act_lens = act_lens_dev; c.costs = nullptr;
+  c.acts_c = reinterpret_cast<float*>(base + l.acts_c);
+  c.grads_c = nullptr;
+  c.lse = reinterpret_cast<float*>(base + l.lse);
+  c.lab_c = reinterpret_cast<int*>(base + l.lab_c);
+  c.off_c = reinterpret_cast<int*>(base + l.off_c);
+  c.col_cls = reinterpret_cast<int*>(base + l.col_cls);
+  c.ncols = reinterpret_cast<int*>(base + l.ncols);
+  c.B = B; c.T = T; c.V = V; c.Vc = max_label_len + 2; c.blank = blank;
+  c.Lmax = max_label_len > 0 ? max_label_len : 1;
+
+  const size_t bits_smem = (size_t)((V + 31) / 32) * sizeof(unsigned);
+  if (ctc_bitmap_kernel_attr(ctc_compact_rows_kernel, bits_smem) != SB_OK) return SB_ERR_CUDA;
+  ctc_colmap_kernel<<<B, CTC_CMP_THREADS, 0, stream>>>(c);
+  ctc_compact_rows_kernel<<<dim3((T + CTC_CMP_ROWS - 1) / CTC_CMP_ROWS, B), CTC_CMP_THREADS,
+                            bits_smem, stream>>>(c);
+
+  CtcViterbi v;
+  v.acts_c = c.acts_c; v.lse = c.lse; v.lab_c = c.lab_c;
+  v.label_lens = label_lens_dev; v.act_lens = act_lens_dev;
+  v.bp = reinterpret_cast<uint2*>(base + l.bp);
+  v.path = path; v.scores = scores;
+  v.B = B; v.T = T; v.Vc = c.Vc; v.Lmax = max_label_len; v.Lstride = c.Lmax;
+  switch (ns) {
+    case 1: ctc_viterbi_kernel<1><<<B, CTC_SIDE, 0, stream>>>(v); break;
+    case 2: ctc_viterbi_kernel<2><<<B, CTC_SIDE, 0, stream>>>(v); break;
+    case 4: ctc_viterbi_kernel<4><<<B, CTC_SIDE, 0, stream>>>(v); break;
+    default: ctc_viterbi_kernel<8><<<B, CTC_SIDE, 0, stream>>>(v); break;
+  }
+  return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
 }

@@ -156,9 +156,171 @@ __global__ void __launch_bounds__(2 * RNNT_SIDE, 1) rnnt_fwd_bwd_kernel(const Rn
   }
 }
 
+// Viterbi alignment over the compact lattice (sb_rnnt_viterbi): the alpha side's anti-diagonal
+// wavefront above with max in place of log-sum-exp, 256 threads, column u on thread u % 256.  The
+// two arcs a node reads for the next diagonal are loaded while the current one is formed.  Each
+// warp packs its 32 columns' choice (1 = label arc) into one word per diagonal with a ballot; warp
+// 0 then walks back from (T_b-1, U_b), 32 diagonals per batch of loads: over 32 diagonals u drops
+// by at most 31, i.e. into the word below or its own.
+struct RnntViterbi {
+  const float* lat;       // (T, B, U1, 2)
+  const int* label_lens;
+  const int* act_lens;
+  unsigned* bits;         // (B, T + U1, NS * 8) backpointers by diagonal
+  int* frames;            // (B, U1 - 1)
+  double* scores;         // (B)
+  int B, T, U1;
+};
+
+template <int NS>
+__global__ void __launch_bounds__(RNNT_SIDE) rnnt_viterbi_kernel(const RnntViterbi p) {
+  constexpr int NW = NS * RNNT_SIDE / 32;   // backpointer words per diagonal
+  __shared__ double nb[2][NS * RNNT_SIDE + 1];   // [parity][u + 1]
+  __shared__ double s_score;
+  const int b = blockIdx.x, i = threadIdx.x, warp = i >> 5, lane = i & 31;
+  const int T = max(0, min(p.act_lens[b], p.T));
+  const int U = max(0, min(p.label_lens[b], p.U1 - 1));
+  const int U1 = p.U1;
+  const size_t tstr = (size_t)p.B * U1;
+  const float* lat = p.lat + (size_t)b * U1 * 2;
+  unsigned* bits = p.bits + (size_t)b * (p.T + U1) * NW;
+  int* frames = p.frames + (size_t)b * (U1 - 1);
+
+  for (int k = i; k < 2 * (NS * RNNT_SIDE + 1); k += RNNT_SIDE) (&nb[0][0])[k] = -INFINITY;
+  for (int u = U + i; u < U1 - 1; u += RNNT_SIDE) frames[u] = -1;
+  __syncthreads();
+  if (T <= 0) {
+    if (i == 0) p.scores[b] = -INFINITY;
+    for (int u = i; u < U; u += RNNT_SIDE) frames[u] = -1;
+    return;
+  }
+
+  // arcs into (t, u) = (d - u, u): blank of (t-1, u) and label of (t, u-1), -inf where absent
+  auto arcs = [&](int d, float (&bl)[NS], float (&lb)[NS]) {
+#pragma unroll
+    for (int q = 0; q < NS; ++q) {
+      const int u = i + RNNT_SIDE * q, t = d - u;
+      bl[q] = lb[q] = -INFINITY;
+      if (u <= U && t >= 0 && t < T) {
+        if (t > 0) bl[q] = __ldg(lat + ((size_t)(t - 1) * tstr + u) * 2);
+        if (u > 0) lb[q] = __ldg(lat + ((size_t)t * tstr + u - 1) * 2 + 1);
+      }
+    }
+  };
+  double own[NS];   // this thread's previous cell in column u
+  float bl[NS], lb[NS];
+#pragma unroll
+  for (int q = 0; q < NS; ++q) own[q] = -INFINITY;
+  arcs(0, bl, lb);
+  const int ndiag = T + U;
+  for (int d = 0; d < ndiag; ++d) {
+    float bln[NS], lbn[NS];
+    arcs(d + 1, bln, lbn);
+    double* cur = nb[d & 1] + 1;
+    const double* prv = nb[(d & 1) ^ 1] + 1;
+#pragma unroll
+    for (int q = 0; q < NS; ++q) {
+      const int u = i + RNNT_SIDE * q, t = d - u;
+      bool label = false;
+      if (u <= U && t >= 0 && t < T) {
+        double v = 0.0;
+        if (d > 0) {
+          const double a = own[q] + (double)bl[q];
+          const double c = prv[u - 1] + (double)lb[q];   // prv[-1] is the -inf pad
+          label = c > a;   // ties take the blank arc: the label came at an earlier frame
+          v = label ? c : a;
+        }
+        own[q] = v;
+        cur[u] = v;
+      }
+      const unsigned w = __ballot_sync(0xffffffffu, label);
+      if (lane == 0) bits[(size_t)d * NW + q * (RNNT_SIDE / 32) + warp] = w;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int q = 0; q < NS; ++q) { bl[q] = bln[q]; lb[q] = lbn[q]; }
+  }
+#pragma unroll
+  for (int q = 0; q < NS; ++q) {
+    if (i + RNNT_SIDE * q == U) {
+      const double sc = own[q] + (double)__ldg(lat + ((size_t)(T - 1) * tstr + U) * 2);
+      p.scores[b] = sc;
+      s_score = sc;
+    }
+  }
+  __syncthreads();
+  if (s_score == -INFINITY) {
+    for (int u = i; u < U; u += RNNT_SIDE) frames[u] = -1;
+    return;
+  }
+  if (warp != 0) return;
+
+  int t = T - 1, u = U;
+  for (int d1 = T - 1 + U; d1 > 0; d1 -= 32) {
+    const int w0 = u >> 5;
+    const int dl = d1 - lane;
+    unsigned w_own = 0u, w_below = 0u;
+    if (dl > 0) {
+      w_own = __ldcg(bits + (size_t)dl * NW + w0);
+      if (w0 > 0) w_below = __ldcg(bits + (size_t)dl * NW + w0 - 1);
+    }
+    const int n = min(32, d1);
+    for (int k = 0; k < n; ++k) {
+      const unsigned a = __shfl_sync(0xffffffffu, w_own, k);
+      const unsigned c = __shfl_sync(0xffffffffu, w_below, k);
+      const unsigned w = (u >> 5) == w0 ? a : c;
+      if ((w >> (u & 31)) & 1u) {
+        --u;
+        if (lane == 0) frames[u] = t;
+      } else {
+        --t;
+      }
+    }
+  }
+}
+
 }  // namespace sb
 
 using namespace sb;
+
+static int rnnt_viterbi_ns(int U1) {
+  const int ns = (U1 + RNNT_SIDE - 1) / RNNT_SIDE;
+  return ns <= 1 ? 1 : ns <= 2 ? 2 : ns <= 4 ? 4 : -1;
+}
+
+extern "C" int sb_rnnt_viterbi_workspace_size(int B, int T, int U1, size_t* bytes) {
+  if (!bytes || B <= 0 || T <= 0 || U1 <= 0) return SB_ERR_INVALID;
+  const int ns = rnnt_viterbi_ns(U1);
+  if (ns < 0) return SB_ERR_UNSUPPORTED;
+  *bytes = (size_t)B * (T + U1) * (ns * RNNT_SIDE / 32) * sizeof(unsigned) + 256;
+  return SB_OK;
+}
+
+extern "C" int sb_rnnt_viterbi(const float* lat, const int* labels, const int* label_offsets,
+                               const int* label_lens, const int* act_lens, int B, int T, int U1,
+                               int* frames, double* scores, void* workspace,
+                               size_t workspace_bytes, void* stream_) {
+  if (!lat || !labels || !label_offsets || !label_lens || !act_lens || !frames || !scores ||
+      !workspace)
+    return SB_ERR_INVALID;
+  if (B <= 0 || T <= 0 || U1 <= 0) return SB_ERR_INVALID;
+  size_t need = 0;
+  const int rc = sb_rnnt_viterbi_workspace_size(B, T, U1, &need);
+  if (rc != SB_OK) return rc;
+  if (workspace_bytes < need) return SB_ERR_WORKSPACE;
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  RnntViterbi p;
+  p.lat = lat; p.label_lens = label_lens; p.act_lens = act_lens;
+  p.bits = reinterpret_cast<unsigned*>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
+  p.frames = frames; p.scores = scores;
+  p.B = B; p.T = T; p.U1 = U1;
+  switch (rnnt_viterbi_ns(U1)) {
+    case 1: rnnt_viterbi_kernel<1><<<B, RNNT_SIDE, 0, stream>>>(p); break;
+    case 2: rnnt_viterbi_kernel<2><<<B, RNNT_SIDE, 0, stream>>>(p); break;
+    default: rnnt_viterbi_kernel<4><<<B, RNNT_SIDE, 0, stream>>>(p); break;
+  }
+  return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
+}
 
 extern "C" int sb_rnnt_workspace_size(int B, int T, int U1, size_t* bytes) {
   if (!bytes || B <= 0 || T <= 0 || U1 <= 0) return SB_ERR_INVALID;

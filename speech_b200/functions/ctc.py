@@ -46,6 +46,39 @@ def ctc_costs_and_grads(acts, labels, act_lens, label_lens, blank=None, need_gra
     return costs, grads
 
 
+def ctc_viterbi(acts, labels, act_lens, label_lens, blank=None):
+    """Viterbi (forced) alignment of each transcript to its logits: the best single path through
+    the lattice the loss sums over (sb_ctc_viterbi; same inputs as the loss, blank = last class by
+    default).  Returns, on the device, path (B, T) int32 -- the index of the label each frame is
+    aligned to, -1 for blank, -2 past act_lens[b] and everywhere for an utterance with no
+    alignment -- and scores (B,) float64, the path's log-probability (-inf without alignment)."""
+    _lib.require_cuda(acts, "acts")
+    lib = _lib.load()
+    if acts.dtype != torch.float32:
+        acts = acts.float()
+    acts = acts.contiguous()
+    B, T, V = acts.shape
+    if blank is None:
+        blank = V - 1
+    dev = acts.device
+    (d_lab, d_off, d_llen, d_alen), max_l = _lib.pack_labels(labels, label_lens, act_lens, B, dev,
+                                                            num_classes=V)
+    nbytes = _lib.workspace_size(lib.sb_ctc_viterbi_workspace_size, B, T, V, max_l)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    path = torch.empty(B, T, dtype=torch.int32, device=dev)
+    scores = torch.empty(B, dtype=torch.float64, device=dev)
+    # no labels in the batch: an empty tensor has no address, and no label is read
+    lab_ptr = d_lab.data_ptr() or d_off.data_ptr()
+    with torch.cuda.device(dev):
+        sp = _lib.stream_ptr()
+        ops._launch("ctc_viterbi", 0.0,
+                    lambda: lib.sb_ctc_viterbi(acts.data_ptr(), lab_ptr, d_off.data_ptr(),
+                                               d_llen.data_ptr(), d_alen.data_ptr(), B, T, V,
+                                               int(blank), max_l, path.data_ptr(),
+                                               scores.data_ptr(), ws.data_ptr(), nbytes, sp))
+    return path, scores
+
+
 class _CTCFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, acts, labels, act_lens, label_lens, blank, size_average):

@@ -246,6 +246,55 @@ def joint_shortlists(fx, fy, fc2, ymat, blank, kp):
     return sl
 
 
+def compact_lattice(fxc, fyc, w2b, b2c, ym, blank):
+    """The compact (T, B, U1, 2) lattice {log p(blank), log p(label)} the loss and the Viterbi
+    alignment read, from the joint's operands (as _joint_operands returns them): the fused joint
+    where fc2 stays resident, else the slab path.  -> lat (nodes, 2), and the slab path's per-node
+    log-sum-exp (None from the fused joint)."""
+    lib = _lib.load()
+    B, T, H = fxc.shape
+    U1 = fyc.shape[1]
+    V1 = w2b.shape[0]
+    if joint_uses_slabs(H, V1):
+        return joint_vocab_forward(fxc, fyc, w2b, b2c, ym, blank)
+    nodes = T * B * U1
+    lat = torch.empty(nodes, 2, dtype=torch.float32, device=fxc.device)
+    sp = _lib.stream_ptr()
+    ops._launch("rnnt_joint", 2.0 * nodes * H * V1,
+                lambda: lib.sb_rnnt_joint_fwd(fxc.data_ptr(), fyc.data_ptr(), w2b.data_ptr(),
+                                              b2c.data_ptr(), ym.data_ptr(), lat.data_ptr(), None,
+                                              B, T, U1, H, V1, int(blank), sp))
+    return lat, None
+
+
+def rnnt_viterbi(fx, fy, fc2, ymat, labels, x_lens, y_lens, blank):
+    """Viterbi (forced) alignment through the Transducer lattice of fx = fc1(x) (B,T,H) and
+    fy = fc1(pred) (B,U1,H) (sb_rnnt_viterbi on the loss's compact lattice); no autograd.
+    Returns, on the device, frames (B, U1-1) int32 -- the frame at which each label is emitted,
+    -1 past y_lens[b] -- and scores (B,) float64, the path's log-probability (-inf where
+    x_lens[b] = 0)."""
+    _lib.require_cuda(fx, "fx")
+    lib = _lib.load()
+    B, T = fx.shape[0], fx.shape[1]
+    U1 = fy.shape[1]
+    dev = fx.device
+    fxc, fyc, w2b, b2c, ym = _joint_operands(fx, fy, fc2, ymat)
+    (lab, offs, ylen, xlen), _ = _lib.pack_labels(labels, y_lens, x_lens, B, dev, lattice_rows=U1)
+    lat, _ = compact_lattice(fxc, fyc, w2b, b2c, ym, blank)
+    nbytes = _lib.workspace_size(lib.sb_rnnt_viterbi_workspace_size, B, T, U1)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    frames = torch.empty(B, max(U1 - 1, 1), dtype=torch.int32, device=dev)
+    scores = torch.empty(B, dtype=torch.float64, device=dev)
+    lab_ptr = lab.data_ptr() or offs.data_ptr()   # no labels in the batch: none is read
+    sp = _lib.stream_ptr()
+    ops._launch("rnnt_viterbi", 0.0,
+                lambda: lib.sb_rnnt_viterbi(lat.data_ptr(), lab_ptr, offs.data_ptr(),
+                                            ylen.data_ptr(), xlen.data_ptr(), B, T, U1,
+                                            frames.data_ptr(), scores.data_ptr(), ws.data_ptr(),
+                                            nbytes, sp))
+    return frames[:, :U1 - 1], scores
+
+
 class _JointLossFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, fx, fy, w2, b2, ymat, labels, x_lens, y_lens, blank, size_average):
@@ -262,17 +311,8 @@ class _JointLossFunction(torch.autograd.Function):
         (lab, offs, ylen, xlen), _ = _lib.pack_labels(labels, y_lens, x_lens, B, dev,
                                                       lattice_rows=U1)
         nodes = T * B * U1
-        lse = None
-        if joint_uses_slabs(H, V1):
-            lat, lse = joint_vocab_forward(fxc, fyc, w2b, b2c, ym, blank)
-            sp = _lib.stream_ptr()
-        else:
-            lat = torch.empty(nodes, 2, dtype=torch.float32, device=dev)
-            sp = _lib.stream_ptr()
-            ops._launch("rnnt_joint", 2.0 * nodes * H * V1,
-                        lambda: lib.sb_rnnt_joint_fwd(fxc.data_ptr(), fyc.data_ptr(), w2b.data_ptr(),
-                                                      b2c.data_ptr(), ym.data_ptr(), lat.data_ptr(),
-                                                      None, B, T, U1, H, V1, int(blank), sp))
+        lat, lse = compact_lattice(fxc, fyc, w2b, b2c, ym, blank)
+        sp = _lib.stream_ptr()
         need = any(ctx.needs_input_grad[:4])
         nbytes = _lib.workspace_size(lib.sb_rnnt_workspace_size, B, T, U1)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)

@@ -80,6 +80,34 @@ class CTC(model.Model):
         return decode_batch(probs, beam_size=beam_size, blank=self.blank, lens=lens, lm=lm,
                             lm_weight=lm_weight, insertion_bonus=insertion_bonus)
 
+    def align(self, batch, return_scores=False):
+        """Viterbi (forced) alignment of each transcript to its audio: the single best path through
+        the lattice `loss` sums over (functions.ctc.ctc_viterbi).  batch: what `loss` takes; the
+        timestamps of a hypothesis come from `align((inputs, hypotheses))`.  Frames searched: the
+        padded T', or each utterance's own conv_out_size(T_b) in the exact-lengths mode.
+        Returns, per utterance, a list of (first_frame, last_frame) encoder-frame pairs, one per
+        label, or None where no alignment exists (too few frames for the labels and their adjacent
+        repeats); with return_scores also the paths' float64 log-probabilities (-inf for None).
+        Encoder frame t starts at input frame t * prod(conv strides) (10 ms per input frame with
+        the reference featuriser)."""
+        x, y, x_lens, y_lens = self._collated(batch)
+        with torch.no_grad():
+            out = self._forward_impl(x, self.exact_lens(x_lens))
+        path, scores = ctc.ctc_viterbi(out, y, x_lens, y_lens, blank=self.blank)
+        path, scores = path.cpu().numpy(), scores.cpu().numpy()
+        spans = []
+        for b, n in enumerate(y_lens.tolist()):
+            if scores[b] == -np.inf:
+                spans.append(None)
+                continue
+            # a path visits labels 0..n-1 in order, each on at least one frame
+            t = np.flatnonzero(path[b] >= 0)
+            j, k = path[b][t], np.arange(n)
+            first = t[np.searchsorted(j, k, "left")]
+            last = t[np.searchsorted(j, k, "right") - 1]
+            spans.append(list(zip(first.tolist(), last.tolist())))
+        return (spans, scores) if return_scores else spans
+
     @staticmethod
     def max_decode(pred, blank):
         """Greedy collapse: merge repeats, then drop blanks (reference ctc_model.py:62-70)."""

@@ -10,6 +10,7 @@ vocabularies run the same computation a slab of frames at a time (GEMM logits + 
 csrc/joint_vocab.cu), so only one slab's logits ever exist.  Where the full lattice is too large
 for the beam search, `infer` decodes from per-node shortlists that the slab path writes instead.
 """
+import numpy as np
 import torch
 import torch.nn as nn
 
@@ -167,6 +168,32 @@ class Transducer(model.Model):
                                       max_symbols_per_frame, max_len, lm, lm_weight,
                                       insertion_bonus)
         return (labels, scores) if return_scores else labels
+
+    def align(self, batch, return_scores=False):
+        """Viterbi (forced) alignment of each transcript to its audio: the single best path through
+        the compact lattice `loss` sums over (functions.transducer.rnnt_viterbi).
+        batch: what `loss` takes; the timestamps of a hypothesis come from
+        `align((inputs, model.recognize(inputs)))`.  Frames searched: the padded T', or each
+        utterance's own conv_out_size(T_b) in the exact-lengths mode.  Returns, per utterance, the
+        encoder frame at which each label is emitted, or None where no alignment exists (no
+        frames); with return_scores also the paths' float64 log-probabilities (-inf for None).
+        Encoder frame t starts at input frame t * prod(conv strides) (10 ms per input frame with
+        the reference featuriser)."""
+        inputs, labels = batch
+        x, y, x_lens, y_lens = self.collate(inputs, labels)
+        # any filler past a row's own labels: fy at u <= U_b reads labels < u only
+        y_mat = self.label_collate([list(seq) or [0] for seq in labels])
+        with torch.no_grad():
+            if self.is_cuda:
+                x = x.cuda(non_blocking=True)
+                y_mat = y_mat.cuda(non_blocking=True)
+            fx, fy = self.joint_inputs(self._encode(x, self.exact_lens(x_lens)), y_mat)
+            frames, scores = transducer_fn.rnnt_viterbi(fx, fy, self.fc2.fc, y_mat, y, x_lens,
+                                                        y_lens, self.blank)
+        frames, scores = frames.cpu().numpy(), scores.cpu().numpy()
+        out = [None if scores[b] == -np.inf else frames[b, :n].tolist()
+               for b, n in enumerate(y_lens.tolist())]
+        return (out, scores) if return_scores else out
 
     def label_collate(self, labels):
         return torch.from_numpy(model.end_pad_labels(labels))

@@ -214,3 +214,29 @@ print("recognize with LM V+1=20001", [len(p) for p in tv.recognize(
     inputs[:3], beam_size=4, max_symbols_per_frame=2, lm=lm_tv, lm_weight=0.5,
     insertion_bonus=1.0)])
 torch.cuda.synchronize()
+# Viterbi alignments: CTC at V = 29 and at V = 20001 (the compact rows), with an infeasible
+# utterance; the Transducer on the resident joint (V+1 = 29) and the slab joint (V+1 = 301)
+print("ctc align", m.align((inputs, labels[:4] + [[3] * 60])))
+print("ctc align V=20001", cv.align((inputs, labels4)))
+for tm in (t, t2):
+    tm.set_eval()
+    print("transducer align", tm.align((inputs, labels if tm is t else labels2)))
+torch.cuda.synchronize()
+# long transcripts: the Viterbi kernels with 2, 4 and 8 states (CTC) and 2 and 4 columns (Transducer)
+# per thread
+from speech_b200.functions import ctc as ctc_fn, transducer as rnnt_fn
+for L in (200, 400, 900):
+    T = L + L // 2 + 10
+    lab = torch.from_numpy(np.random.randint(0, 28, L).astype(np.int32))
+    path, sc = ctc_fn.ctc_viterbi(torch.randn(2, T, 29, device="cuda"), torch.cat([lab, lab]),
+                                  torch.tensor([T, T - 5]), torch.tensor([L, L]))
+    print("ctc viterbi L=%d" % L, sc.tolist())
+fc2 = torch.nn.Linear(64, 29).cuda()
+for U in (300, 700):
+    ym = torch.from_numpy(np.random.randint(0, 28, (2, U)))
+    fr, sc = rnnt_fn.rnnt_viterbi(torch.randn(2, 40, 64, device="cuda"),
+                                  torch.randn(2, U + 1, 64, device="cuda"), fc2, ym,
+                                  ym.reshape(-1).int(), torch.tensor([40, 30]),
+                                  torch.tensor([U, U]), 28)
+    print("rnnt viterbi U=%d" % U, sc.tolist())
+torch.cuda.synchronize()
