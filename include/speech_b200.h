@@ -142,6 +142,21 @@ int sb_gru_fwd(const float* gi, const void* whh_bf16, const float* bhh, float* y
                float* gates, void* workspace, size_t workspace_bytes, int T, int Bp, int H,
                int ndir, void* stream);
 
+/* The forward recurrence resumed from a given state, for streaming: T new frames continue from
+ * h_{-1} = h0 instead of 0.  One direction only (SB_ERR_UNSUPPORTED for ndir = 2).
+ *   h0     [Bp][H] f32 and h0_bf16 [Bp][H] bf16: the state and the bf16 operand the first step's
+ *          W_hh product reads (the fp32 y and the bf16 xn of the previous call's last frame)
+ *   gi     [T*Bp][3H] f32 as for sb_gru_fwd
+ *   y, xn  [(T+1)*Bp][H]: frame 0 receives h0 / h0_bf16 (copied unless they already are frame 0),
+ *          frames 1..T are h_0 .. h_{T-1}
+ *   gates  [(T+1)*Bp][4][H] or NULL; frame 0 is left as it was
+ * Same workspace, constraints and kernel selection as sb_gru_fwd at (Bp, H, 1), and the same
+ * arithmetic: running frames [0, T1) with sb_gru_fwd and then [T1, T) from its last state gives
+ * y and xn bit-identical to one sb_gru_fwd over [0, T). */
+int sb_gru_fwd_h0(const float* gi, const void* whh_bf16, const float* bhh, const float* h0,
+                  const void* h0_bf16, float* y, void* xn_bf16, float* gates, void* workspace,
+                  size_t workspace_bytes, int T, int Bp, int H, int ndir, void* stream);
+
 /* "Parity mode" forward recurrence: the same time loop in plain fp32 on CUDA cores (fp32 weights
  * [ndir][3H][H], fp32 state, no bf16 rounding anywhere), csrc/gru_f32.cu.  It exists to measure
  * the bf16 tensor-core path against (SURVEY.md section 7), not to be fast.
@@ -281,6 +296,57 @@ int sb_ctc_prefix_beam_lm_shortlist(const float* logp, const int* lens, int B, i
                                     double lm_weight, double insertion_bonus, int* out_labels,
                                     int* out_lens, double* out_scores, void* workspace,
                                     size_t workspace_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------
+ * Resumable CTC prefix beam search, for streaming: B independent streams whose beams live in a
+ * device state buffer between calls, so that each call advances a stream by the frames that have
+ * arrived.  Frames [0, T) searched in any chunking give labels, lengths and float64 scores
+ * bit-identical to sb_ctc_prefix_beam[_lm] over [0, T): every call runs the same per-frame code,
+ * the tie and route rules are those of the offline search, and trie nodes are numbered by the
+ * absolute frame (1 + t*K + r), as one pass over the whole utterance numbers them.
+ *   sb_ctc_stream_state_size   bytes of the state of B streams of at most max_frames frames each
+ *       (order: 0 without an LM, else the LM's).  Layout: per stream, the beam (p_b, p_nb, trie
+ *       node, last symbol and parent node of each of <= K entries), the entries' LM contexts, the
+ *       frames consumed and an overflow flag; then the tries of the B streams, max_frames*K + 1
+ *       nodes each.
+ *   sb_ctc_stream_reset        streams [first, first + count) back to the empty prefix at frame 0;
+ *       the other streams are untouched.  Every stream must be reset before its first step.
+ *   sb_ctc_stream_step[_lm]    logp (B, T, S) float32 log-probabilities of the new frames, n (B)
+ *       int32 on the device: stream b advances by min(n[b], T) frames (0 leaves it as it was).  The
+ *       route is chosen as sb_ctc_prefix_beam chooses it; the _shortlist forms force the shortlist
+ *       search.  workspace >= sb_ctc_stream_workspace_size(B, T, beam_size): the shortlists.  The
+ *       LM arguments are those of sb_ctc_prefix_beam_lm; a state must be stepped with or without
+ *       an LM throughout, from its reset on.  A stream asked to pass max_frames is advanced only
+ *       to max_frames and its overflow flag is set (the caller, who knows every stream's frame
+ *       count, should refuse such a step instead).
+ *   sb_ctc_stream_best         each stream's best prefix so far: out_labels (B, max_frames) int32,
+ *       out_lens (B), out_scores (B) float64 -lse(p_b, p_nb) of beam entry 0, out_overflow (B).
+ * B, max_frames and beam_size must be the same in every call on one state.
+ * SB_ERR_INVALID for a null pointer, B, max_frames, T or beam_size <= 0, blank outside [0, S), and
+ * every LM argument sb_ctc_prefix_beam_lm refuses; SB_ERR_UNSUPPORTED for beam_size > 32 or
+ * order > SB_LM_MAX_ORDER; SB_ERR_WORKSPACE for a short workspace.  All before any CUDA call.
+ * ------------------------------------------------------------------------------------- */
+int sb_ctc_stream_state_size(int B, int max_frames, int beam_size, int order, size_t* bytes);
+int sb_ctc_stream_workspace_size(int B, int T, int beam_size, size_t* bytes);
+int sb_ctc_stream_reset(void* state, int B, int max_frames, int beam_size, int first, int count,
+                        void* stream);
+int sb_ctc_stream_step(const float* logp, const int* n, int B, int T, int S, int beam_size,
+                       int blank, int max_frames, void* state, void* workspace,
+                       size_t workspace_bytes, void* stream);
+int sb_ctc_stream_step_shortlist(const float* logp, const int* n, int B, int T, int S,
+                                 int beam_size, int blank, int max_frames, void* state,
+                                 void* workspace, size_t workspace_bytes, void* stream);
+int sb_ctc_stream_step_lm(const float* logp, const int* n, int B, int T, int S, int beam_size,
+                          int blank, const SbNgramLm* lm, double lm_weight,
+                          double insertion_bonus, int max_frames, void* state, void* workspace,
+                          size_t workspace_bytes, void* stream);
+int sb_ctc_stream_step_lm_shortlist(const float* logp, const int* n, int B, int T, int S,
+                                    int beam_size, int blank, const SbNgramLm* lm,
+                                    double lm_weight, double insertion_bonus, int max_frames,
+                                    void* state, void* workspace, size_t workspace_bytes,
+                                    void* stream);
+int sb_ctc_stream_best(const void* state, int B, int max_frames, int beam_size, int* out_labels,
+                       int* out_lens, double* out_scores, int* out_overflow, void* stream);
 /* Developer counter: frames the LM-fused shortlist search rescanned in full, over every call
  * since the last query (synchronous: waits for the device); resets it. */
 int sb_debug_ctc_lm_rescans(unsigned long long* frames);

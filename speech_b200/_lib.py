@@ -57,6 +57,18 @@ SIGNATURES = {
     "sb_ctc_prefix_beam_lm_shortlist": (_c_int, [_vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int,
                                                  _lmp, _db, _db, _vp, _vp, _vp, _vp, _c_sz, _vp]),
     "sb_debug_ctc_lm_rescans": (_c_int, [ctypes.POINTER(ctypes.c_ulonglong)]),
+    "sb_ctc_stream_state_size": (_c_int, [_c_int, _c_int, _c_int, _c_int, ctypes.POINTER(_c_sz)]),
+    "sb_ctc_stream_workspace_size": (_c_int, [_c_int, _c_int, _c_int, ctypes.POINTER(_c_sz)]),
+    "sb_ctc_stream_reset": (_c_int, [_vp, _c_int, _c_int, _c_int, _c_int, _c_int, _vp]),
+    "sb_ctc_stream_step": (_c_int, [_vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int, _c_int, _vp,
+                                    _vp, _c_sz, _vp]),
+    "sb_ctc_stream_step_shortlist": (_c_int, [_vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int,
+                                              _c_int, _vp, _vp, _c_sz, _vp]),
+    "sb_ctc_stream_step_lm": (_c_int, [_vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int, _lmp, _db,
+                                       _db, _c_int, _vp, _vp, _c_sz, _vp]),
+    "sb_ctc_stream_step_lm_shortlist": (_c_int, [_vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int,
+                                                 _lmp, _db, _db, _c_int, _vp, _vp, _c_sz, _vp]),
+    "sb_ctc_stream_best": (_c_int, [_vp, _c_int, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp]),
     "sb_conv_im2col": (_c_int, [_vp, _vp, _fl, _vp, _c_int, _c_int, _c_int, _c_int, _c_int, _c_int,
                                 _c_int, _c_int, _c_int, _vp]),
     "sb_conv_relu_to_bct": (_c_int, [_vp, _vp, _fl, _vp, _c_int, _c_int, _c_int, _c_int, _vp]),
@@ -177,6 +189,8 @@ SIGNATURES = {
     "sb_gru_fwd_workspace_size": (_c_int, [_c_int, _c_int, _c_int, ctypes.POINTER(_c_sz)]),
     "sb_gru_fwd": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_sz, _c_int, _c_int, _c_int,
                             _c_int, _vp]),
+    "sb_gru_fwd_h0": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_sz, _c_int, _c_int,
+                               _c_int, _c_int, _vp]),
     "sb_gru_fwd_f32": (_c_int, [_vp, _vp, _vp, _vp, _vp, _c_int, _c_int, _c_int, _c_int, _vp]),
     "sb_time_align": (_c_int, [_vp, _c_ll, _vp, _c_ll, _vp, _c_int, _c_int, _c_int, _c_int, _c_int,
                                _vp]),

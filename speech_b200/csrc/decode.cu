@@ -18,6 +18,7 @@
 #include "beam.cuh"
 #include "ngram.cuh"
 #include <math.h>
+#include <string.h>
 
 #include "../../include/speech_b200.h"
 
@@ -203,15 +204,20 @@ __device__ __forceinline__ int dec_take_first(const double* score, const int* ra
   return bc;
 }
 
+// the beam of the empty prefix (one thread)
+__device__ __forceinline__ void dec_empty(Beam& bm) {
+  bm.size = 1;
+  bm.pb[0] = 0.0;
+  bm.pnb[0] = d_neg_inf();
+  bm.node[0] = 0;
+  bm.last[0] = -1;
+  bm.parent[0] = -1;
+}
+
 template <class Fuse>
 __device__ __forceinline__ void dec_begin(const DecParams& p, Beam* beams) {
   if (threadIdx.x == 0) {
-    beams[0].size = 1;
-    beams[0].pb[0] = 0.0;
-    beams[0].pnb[0] = d_neg_inf();
-    beams[0].node[0] = 0;
-    beams[0].last[0] = -1;
-    beams[0].parent[0] = -1;
+    dec_empty(beams[0]);
     if constexpr (Fuse::kLm) lm_shared().hist[0][0][0] = -1;   // the empty prefix: <s>
   }
   p.trie.of(blockIdx.x).clear<DEC_THREADS>();
@@ -279,27 +285,96 @@ __device__ __forceinline__ void dec_finish(const DecParams& p, const Beam& fin) 
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// Where a search's beam comes from and goes to.  The kernels below run frames [t0, t0 + n) of
+// utterance b over a beam that begin() puts in beams[t0 & 1] (and, with an LM, the contexts in
+// hist[t0 & 1]); end() takes the beam of frame t0 + n.  Frame t of the utterance is row t - t0 of
+// the kernel's logp, and its trie nodes are numbered 1 + t*K + r, so that a resumed search names
+// every prefix as one pass over the whole utterance does.
+//   DecOffline  t0 = 0, n = lens[b]: a fresh beam and trie; the best prefix goes to the outputs.
+//   DecResume   t0 = the frames the slot has consumed: the beam, the contexts and the trie of a
+//               DecSlot (sb_ctc_stream_*), stored back at the end.
+// ------------------------------------------------------------------------------------------------
+struct DecOffline {
+  template <class Fuse>
+  __device__ __forceinline__ int begin(const DecParams& p, Beam* beams, int& n) const {
+    dec_begin<Fuse>(p, beams);
+    return 0;
+  }
+  template <class Fuse>
+  __device__ __forceinline__ void end(const DecParams& p, const Beam* beams, int t) const {
+    dec_finish(p, beams[t & 1]);
+  }
+};
+
+// One stream of the resumable search: the beam after frame `frames` - 1 and its entries' contexts.
+struct DecSlot {
+  Beam beam;
+  int hist[DEC_MAX_BEAM][SB_LM_MAX_ORDER - 1];
+  int frames;     // frames consumed since the last reset
+  int overflow;   // a step was asked for frames past max_frames (and clamped)
+};
+static constexpr size_t DEC_SLOT_BYTES = (sizeof(DecSlot) + 255) / 256 * 256;
+
+__device__ __forceinline__ DecSlot* dec_slot(void* base, int b) {
+  return reinterpret_cast<DecSlot*>(static_cast<unsigned char*>(base) + (size_t)b * DEC_SLOT_BYTES);
+}
+
+// copy `bytes` (a multiple of 4) with the whole block
+__device__ __forceinline__ void dec_copy(void* dst, const void* src, size_t bytes) {
+  for (size_t k = threadIdx.x; k < bytes / 4; k += DEC_THREADS)
+    static_cast<int*>(dst)[k] = static_cast<const int*>(src)[k];
+}
+
+struct DecResume {
+  void* slots;      // [B] DecSlot, DEC_SLOT_BYTES apart
+  int max_frames;
+
+  template <class Fuse>
+  __device__ __forceinline__ int begin(const DecParams& p, Beam* beams, int& n) const {
+    const DecSlot* sl = dec_slot(slots, blockIdx.x);
+    const int t0 = sl->frames;
+    if (n > max_frames - t0) {            // refused by the host; never past the trie's arena
+      n = max_frames - t0;
+      if (threadIdx.x == 0) dec_slot(slots, blockIdx.x)->overflow = 1;
+    }
+    dec_copy(&beams[t0 & 1], &sl->beam, sizeof(Beam));
+    if constexpr (Fuse::kLm) dec_copy(lm_shared().hist[t0 & 1], sl->hist, sizeof(sl->hist));
+    __syncthreads();
+    return t0;
+  }
+  template <class Fuse>
+  __device__ __forceinline__ void end(const DecParams& p, const Beam* beams, int t) const {
+    DecSlot* sl = dec_slot(slots, blockIdx.x);
+    dec_copy(&sl->beam, &beams[t & 1], sizeof(Beam));
+    if constexpr (Fuse::kLm) dec_copy(sl->hist, lm_shared().hist[t & 1], sizeof(sl->hist));
+    if (threadIdx.x == 0) sl->frames = t;
+  }
+};
+
 // kMinBlocks: 0 leaves the LM-less kernel's register allocation as it was; 1 lets the LM kernel
 // use 70 registers instead of 56 and an 8-byte spill (one CTA per utterance either way).
-template <class Fuse>
-__global__ void __launch_bounds__(DEC_THREADS, Fuse::kMinBlocks) ctc_prefix_beam_kernel(
-    const DecParams p, const Fuse fu) {
+template <class Fuse, class Io>
+__device__ __forceinline__ void ctc_prefix_beam_body(const DecParams p, const Fuse fu,
+                                                     const Io io) {
   extern __shared__ unsigned char dec_smem[];
   const int b = blockIdx.x, tid = threadIdx.x;
-  const int K = p.K, S = p.S, T = min(p.lens[b], p.T);
+  const int K = p.K, S = p.S;
+  int T = min(p.lens[b], p.T);
   const int ncand = K * S + K;
   double* score = reinterpret_cast<double*>(dec_smem);             // [ncand]
   int* rank = reinterpret_cast<int*>(score + ncand);               // [ncand]
   unsigned char* live = reinterpret_cast<unsigned char*>(rank + ncand);  // [ncand]
   __shared__ Beam beams[2];
 
-  dec_begin<Fuse>(p, beams);
+  const int t0 = io.template begin<Fuse>(p, beams, T);
   const float* logp = p.logp + (size_t)b * p.T * S;
 
-  for (int t = 0; t < T; ++t) {
+  for (int f = 0; f < T; ++f) {
+    const int t = t0 + f;
     const Beam& cur = beams[t & 1];
     Beam& nxt = beams[(t & 1) ^ 1];
-    const float* lp = logp + (size_t)t * S;
+    const float* lp = logp + (size_t)f * S;
     dec_frame(fu, cur, t);
     // ---- 1. score every candidate ----
     for (int c = tid; c < ncand; c += DEC_THREADS) {
@@ -323,7 +398,19 @@ __global__ void __launch_bounds__(DEC_THREADS, Fuse::kMinBlocks) ctc_prefix_beam
     // ---- 3. materialise the pruned beam ----
     dec_commit(p, cur, nxt, mine, ns, lp, t, fu);
   }
-  dec_finish(p, beams[T & 1]);
+  io.template end<Fuse>(p, beams, t0 + T);
+}
+
+template <class Fuse>
+__global__ void __launch_bounds__(DEC_THREADS, Fuse::kMinBlocks) ctc_prefix_beam_kernel(
+    const DecParams p, const Fuse fu) {
+  ctc_prefix_beam_body(p, fu, DecOffline{});
+}
+// The resumed kernel takes the LM kernel's bound in both forms: with 0 the LM-less one spills.
+template <class Fuse>
+__global__ void __launch_bounds__(DEC_THREADS, 1) ctc_stream_kernel(
+    const DecParams p, const Fuse fu, const DecResume io) {
+  ctc_prefix_beam_body(p, fu, io);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -397,12 +484,14 @@ __global__ void __launch_bounds__(DEC_SL_THREADS) ctc_shortlist_kernel(
   }
 }
 
-template <class Fuse>
-__global__ void __launch_bounds__(DEC_THREADS, 1) ctc_prefix_beam_shortlist_kernel(
-    const DecParams p, const int* __restrict__ shortlist, int L, int LS, const Fuse fu) {
+template <class Fuse, class Io>
+__device__ __forceinline__ void ctc_prefix_beam_shortlist_body(
+    const DecParams p, const int* __restrict__ shortlist, int L, int LS, const Fuse fu,
+    const Io io) {
   extern __shared__ unsigned char dec_smem[];
   const int b = blockIdx.x, tid = threadIdx.x;
-  const int K = p.K, S = p.S, T = min(p.lens[b], p.T);
+  const int K = p.K, S = p.S;
+  int T = min(p.lens[b], p.T);
   const int per = L + 1;                   // shortlist + last_i per entry
   const int ncand = K * per + K;
   double* score = reinterpret_cast<double*>(dec_smem);             // [ncand]
@@ -413,14 +502,15 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) ctc_prefix_beam_shortlist_kern
   __shared__ int rescan;
   const bool complete = L >= S - 1;        // every non-blank symbol is on the list
 
-  dec_begin<Fuse>(p, beams);
+  const int t0 = io.template begin<Fuse>(p, beams, T);
   const float* logp = p.logp + (size_t)b * p.T * S;
 
-  for (int t = 0; t < T; ++t) {
+  for (int f = 0; f < T; ++f) {
+    const int t = t0 + f;
     const Beam& cur = beams[t & 1];
     Beam& nxt = beams[(t & 1) ^ 1];
-    const float* lp = logp + (size_t)t * S;
-    const int* sl = shortlist + ((size_t)b * p.T + t) * LS;
+    const float* lp = logp + (size_t)f * S;
+    const int* sl = shortlist + ((size_t)b * p.T + f) * LS;
     const int nb = cur.size;
     dec_frame(fu, cur, t);
     // ---- 1. score the shortlisted candidates ----
@@ -513,7 +603,41 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) ctc_prefix_beam_shortlist_kern
     // ---- 4. materialise the pruned beam ----
     dec_commit(p, cur, nxt, mine, ns, lp, t, fu);
   }
-  dec_finish(p, beams[T & 1]);
+  io.template end<Fuse>(p, beams, t0 + T);
+}
+
+template <class Fuse>
+__global__ void __launch_bounds__(DEC_THREADS, 1) ctc_prefix_beam_shortlist_kernel(
+    const DecParams p, const int* __restrict__ shortlist, int L, int LS, const Fuse fu) {
+  ctc_prefix_beam_shortlist_body(p, shortlist, L, LS, fu, DecOffline{});
+}
+template <class Fuse>
+__global__ void __launch_bounds__(DEC_THREADS, 1) ctc_stream_shortlist_kernel(
+    const DecParams p, const int* __restrict__ shortlist, int L, int LS, const Fuse fu,
+    const DecResume io) {
+  ctc_prefix_beam_shortlist_body(p, shortlist, L, LS, fu, io);
+}
+
+// Slots first + blockIdx.x back to the empty prefix at frame 0, with an empty trie.
+__global__ void __launch_bounds__(DEC_THREADS) ctc_stream_reset_kernel(const BeamTrie trie,
+                                                                      void* slots, int first) {
+  const int b = first + blockIdx.x;
+  DecSlot* sl = dec_slot(slots, b);
+  if (threadIdx.x == 0) {
+    dec_empty(sl->beam);
+    sl->hist[0][0] = -1;
+    sl->frames = 0;
+    sl->overflow = 0;
+  }
+  trie.of(b).clear<DEC_THREADS>();
+}
+
+// Each slot's best prefix so far (dec_finish on the stored beam) and its overflow flag.
+__global__ void __launch_bounds__(32) ctc_stream_best_kernel(const DecParams p, const void* slots,
+                                                             int* out_overflow) {
+  const DecSlot* sl = dec_slot(const_cast<void*>(slots), blockIdx.x);
+  dec_finish(p, sl->beam);
+  if (threadIdx.x == 0 && out_overflow) out_overflow[blockIdx.x] = sl->overflow;
 }
 
 }  // namespace sb
@@ -538,63 +662,90 @@ static size_t dec_full_smem(int S, int K) {
   return (size_t)(K * S + K) * (sizeof(double) + sizeof(int) + 1) + 16;
 }
 
-// Both routes with the fusion policy fu.  Every shape whose K*S + K full-scan candidates fit in
-// 200 KB of shared memory takes the full scan; the static shared memory of either instantiation
-// (5.8 KB at most, with the LM's contexts) leaves both sizes below the per-block limit.
+// The trie arena of B utterances of node_cap nodes each at `base` (dec_shortlist_offset bytes).
+static BeamTrie dec_trie(void* base, int B, size_t node_cap) {
+  BeamTrie tr;
+  tr.node_cap = (int)node_cap;
+  tr.cap = beam_pow2_cap(2 * node_cap);
+  tr.nodes = reinterpret_cast<int*>((reinterpret_cast<uintptr_t>(base) + 255) & ~(uintptr_t)255);
+  tr.keys = reinterpret_cast<unsigned long long*>(
+      (reinterpret_cast<uintptr_t>(tr.nodes + (size_t)B * 2 * tr.node_cap) + 255) &
+      ~(uintptr_t)255);
+  tr.vals = reinterpret_cast<int*>(tr.keys + (size_t)B * tr.cap);
+  return tr;
+}
+
+// Both routes with the fusion policy fu, over a fresh beam (rs null) or resumed from the slots of
+// *rs.  Every shape whose K*S + K full-scan candidates fit in 200 KB of shared memory takes the
+// full scan; the static shared memory of either instantiation (5.8 KB at most, with the LM's
+// contexts) leaves both sizes below the per-block limit.  shortlist: B*T*(2K+1) ints.
+template <class Fuse>
+static int dec_launch(const DecParams& p, const Fuse& fu, const DecResume* rs, int* shortlist,
+                      bool force_shortlist, cudaStream_t stream) {
+  const int B = p.B, T = p.T, S = p.S, beam_size = p.K;
+  const size_t full_smem = dec_full_smem(S, beam_size);
+  if (!force_shortlist && full_smem <= 200 * 1024) {
+    const void* kern = rs ? (const void*)ctc_stream_kernel<Fuse>
+                          : (const void*)ctc_prefix_beam_kernel<Fuse>;
+    if (full_smem > 40 * 1024) {
+      if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               (int)full_smem) != cudaSuccess)
+        return SB_ERR_CUDA;
+    }
+    if (rs) ctc_stream_kernel<Fuse><<<B, DEC_THREADS, full_smem, stream>>>(p, fu, *rs);
+    else ctc_prefix_beam_kernel<Fuse><<<B, DEC_THREADS, full_smem, stream>>>(p, fu);
+    return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
+  }
+
+  const int LS = 2 * beam_size + 1;
+  const int L = S - 1 < LS ? S - 1 : LS;
+  const int ncand = beam_size * (L + 1) + beam_size;
+  const size_t smem = (size_t)ncand * (sizeof(double) + 2 * sizeof(int) + 1) + 16;
+  const void* kern = rs ? (const void*)ctc_stream_shortlist_kernel<Fuse>
+                        : (const void*)ctc_prefix_beam_shortlist_kernel<Fuse>;
+  if (smem > 40 * 1024) {
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) !=
+        cudaSuccess)
+      return SB_ERR_CUDA;
+  }
+  if (L > 0)
+    ctc_shortlist_kernel<<<dim3(T, B), DEC_SL_THREADS, 0, stream>>>(p.logp, p.lens, shortlist, T,
+                                                                     S, p.blank, L, LS);
+  if (rs)
+    ctc_stream_shortlist_kernel<Fuse><<<B, DEC_THREADS, smem, stream>>>(p, shortlist, L, LS, fu,
+                                                                       *rs);
+  else
+    ctc_prefix_beam_shortlist_kernel<Fuse><<<B, DEC_THREADS, smem, stream>>>(p, shortlist, L, LS,
+                                                                            fu);
+  return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
+}
+
+static int dec_check(int B, int T, int S, int beam_size, int blank) {
+  if (B <= 0 || T <= 0 || S <= 0 || blank < 0 || blank >= S || beam_size <= 0) return SB_ERR_INVALID;
+  if (beam_size > DEC_MAX_BEAM) return SB_ERR_UNSUPPORTED;
+  return SB_OK;
+}
+
 template <class Fuse>
 static int dec_entry(const float* logp, const int* lens, int B, int T, int S, int beam_size,
                      int blank, int* out_labels, int* out_lens, double* out_scores,
                      void* workspace, size_t workspace_bytes, void* stream_, bool force_shortlist,
                      const Fuse& fu) {
   if (!logp || !lens || !out_labels || !out_lens || !out_scores || !workspace) return SB_ERR_INVALID;
-  if (B <= 0 || T <= 0 || S <= 0 || blank < 0 || blank >= S || beam_size <= 0) return SB_ERR_INVALID;
-  if (beam_size > DEC_MAX_BEAM) return SB_ERR_UNSUPPORTED;
+  const int rc = dec_check(B, T, S, beam_size, blank);
+  if (rc != SB_OK) return rc;
   size_t need = 0;
   sb_ctc_prefix_beam_workspace_size(B, T, beam_size, &need);
   if (workspace_bytes < need) return SB_ERR_WORKSPACE;
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   DecParams p;
   p.logp = logp; p.lens = lens;
-  BeamTrie& tr = p.trie;
-  tr.node_cap = (int)dec_node_cap(T, beam_size);
-  tr.cap = beam_pow2_cap(2 * dec_node_cap(T, beam_size));
-  tr.nodes =
-      reinterpret_cast<int*>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
-  tr.keys = reinterpret_cast<unsigned long long*>(
-      (reinterpret_cast<uintptr_t>(tr.nodes + (size_t)B * 2 * tr.node_cap) + 255) &
-      ~(uintptr_t)255);
-  tr.vals = reinterpret_cast<int*>(tr.keys + (size_t)B * tr.cap);
+  p.trie = dec_trie(workspace, B, dec_node_cap(T, beam_size));
   p.out_labels = out_labels; p.out_lens = out_lens; p.out_scores = out_scores;
   p.B = B; p.T = T; p.S = S; p.K = beam_size; p.blank = blank;
-
-  const size_t full_smem = dec_full_smem(S, beam_size);
-  if (!force_shortlist && full_smem <= 200 * 1024) {
-    if (full_smem > 40 * 1024) {
-      if (cudaFuncSetAttribute(ctc_prefix_beam_kernel<Fuse>,
-                               cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               (int)full_smem) != cudaSuccess)
-        return SB_ERR_CUDA;
-    }
-    ctc_prefix_beam_kernel<Fuse><<<B, DEC_THREADS, full_smem, stream>>>(p, fu);
-    return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
-  }
-
-  const int LS = 2 * beam_size + 1;
-  const int L = S - 1 < LS ? S - 1 : LS;
   int* shortlist = reinterpret_cast<int*>(static_cast<unsigned char*>(workspace) +
                                           dec_shortlist_offset(B, T, beam_size));
-  const int ncand = beam_size * (L + 1) + beam_size;
-  const size_t smem = (size_t)ncand * (sizeof(double) + 2 * sizeof(int) + 1) + 16;
-  if (smem > 40 * 1024) {
-    if (cudaFuncSetAttribute(ctc_prefix_beam_shortlist_kernel<Fuse>,
-                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-      return SB_ERR_CUDA;
-  }
-  if (L > 0)
-    ctc_shortlist_kernel<<<dim3(T, B), DEC_SL_THREADS, 0, stream>>>(logp, lens, shortlist, T, S,
-                                                                     blank, L, LS);
-  ctc_prefix_beam_shortlist_kernel<Fuse><<<B, DEC_THREADS, smem, stream>>>(p, shortlist, L, LS, fu);
-  return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
+  return dec_launch(p, fu, nullptr, shortlist, force_shortlist,
+                    reinterpret_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int sb_ctc_prefix_beam(const float* logp, const int* lens, int B, int T, int S,
@@ -621,10 +772,9 @@ extern "C" int sb_ctc_prefix_beam_lm_workspace_size(int B, int T, int K, int ord
   return sb_ctc_prefix_beam_workspace_size(B, T, K, bytes);
 }
 
-static int dec_lm_entry(const float* logp, const int* lens, int B, int T, int S, int beam_size,
-                        int blank, const SbNgramLm* lm, double lm_weight, double insertion_bonus,
-                        int* out_labels, int* out_lens, double* out_scores, void* workspace,
-                        size_t workspace_bytes, void* stream, bool force_shortlist) {
+// The fusion policy of an LM and its weights, or the status that refuses them.
+static int dec_lm_fuse(int S, int blank, const SbNgramLm* lm, double lm_weight,
+                       double insertion_bonus, LmFuse* fu) {
   if (!lm || !lm->keys || !lm->vals || !lm->logp || !lm->bow || !lm->tok) return SB_ERR_INVALID;
   if (!(lm_weight >= 0.0) || !isfinite(lm_weight) || !isfinite(insertion_bonus))
     return SB_ERR_INVALID;
@@ -632,10 +782,19 @@ static int dec_lm_entry(const float* logp, const int* lens, int B, int T, int S,
   if (lm->blank != blank) return SB_ERR_INVALID;
   if (lm->cap <= 0 || (lm->cap & (lm->cap - 1)) || lm->order < 1) return SB_ERR_INVALID;
   if (lm->order > SB_LM_MAX_ORDER) return SB_ERR_UNSUPPORTED;
+  fu->lm = *lm;
+  fu->alpha = lm_weight;
+  fu->beta = insertion_bonus;
+  return SB_OK;
+}
+
+static int dec_lm_entry(const float* logp, const int* lens, int B, int T, int S, int beam_size,
+                        int blank, const SbNgramLm* lm, double lm_weight, double insertion_bonus,
+                        int* out_labels, int* out_lens, double* out_scores, void* workspace,
+                        size_t workspace_bytes, void* stream, bool force_shortlist) {
   LmFuse fu;
-  fu.lm = *lm;
-  fu.alpha = lm_weight;
-  fu.beta = insertion_bonus;
+  const int rc = dec_lm_fuse(S, blank, lm, lm_weight, insertion_bonus, &fu);
+  if (rc != SB_OK) return rc;
   return dec_entry(logp, lens, B, T, S, beam_size, blank, out_labels, out_lens, out_scores,
                    workspace, workspace_bytes, stream, force_shortlist, fu);
 }
@@ -657,6 +816,135 @@ extern "C" int sb_ctc_prefix_beam_lm_shortlist(const float* logp, const int* len
                                                size_t workspace_bytes, void* stream) {
   return dec_lm_entry(logp, lens, B, T, S, beam_size, blank, lm, lm_weight, insertion_bonus,
                       out_labels, out_lens, out_scores, workspace, workspace_bytes, stream, true);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Resumable search (sb_ctc_stream_*).  State: B DecSlots, then the trie arena of B streams of
+// max_frames * K + 1 nodes, laid out as the offline search's workspace lays out B utterances.
+// ------------------------------------------------------------------------------------------------
+static int dec_stream_check(int B, int max_frames, int beam_size) {
+  if (B <= 0 || max_frames <= 0 || beam_size <= 0) return SB_ERR_INVALID;
+  if (beam_size > DEC_MAX_BEAM) return SB_ERR_UNSUPPORTED;
+  return SB_OK;
+}
+
+static BeamTrie dec_stream_trie(void* state, int B, int max_frames, int beam_size) {
+  return dec_trie(static_cast<unsigned char*>(state) + (size_t)B * DEC_SLOT_BYTES, B,
+                  dec_node_cap(max_frames, beam_size));
+}
+
+extern "C" int sb_ctc_stream_state_size(int B, int max_frames, int beam_size, int order,
+                                        size_t* bytes) {
+  if (!bytes || order < 0) return SB_ERR_INVALID;
+  if (order > SB_LM_MAX_ORDER) return SB_ERR_UNSUPPORTED;
+  const int rc = dec_stream_check(B, max_frames, beam_size);
+  if (rc != SB_OK) return rc;
+  *bytes = (size_t)B * DEC_SLOT_BYTES + dec_shortlist_offset(B, max_frames, beam_size);
+  return SB_OK;
+}
+
+extern "C" int sb_ctc_stream_workspace_size(int B, int T, int beam_size, size_t* bytes) {
+  if (!bytes || B <= 0 || T <= 0 || beam_size <= 0) return SB_ERR_INVALID;
+  *bytes = (size_t)B * T * (2 * beam_size + 1) * sizeof(int);
+  return SB_OK;
+}
+
+extern "C" int sb_ctc_stream_reset(void* state, int B, int max_frames, int beam_size, int first,
+                                   int count, void* stream) {
+  if (!state) return SB_ERR_INVALID;
+  const int rc = dec_stream_check(B, max_frames, beam_size);
+  if (rc != SB_OK) return rc;
+  if (first < 0 || count <= 0 || count > B - first) return SB_ERR_INVALID;
+  ctc_stream_reset_kernel<<<count, DEC_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      dec_stream_trie(state, B, max_frames, beam_size), state, first);
+  return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
+}
+
+template <class Fuse>
+static int dec_stream_entry(const float* logp, const int* n, int B, int T, int S, int beam_size,
+                            int blank, int max_frames, void* state, void* workspace,
+                            size_t workspace_bytes, void* stream, bool force_shortlist,
+                            const Fuse& fu) {
+  if (!logp || !n || !state || !workspace) return SB_ERR_INVALID;
+  int rc = dec_check(B, T, S, beam_size, blank);
+  if (rc != SB_OK) return rc;
+  rc = dec_stream_check(B, max_frames, beam_size);
+  if (rc != SB_OK) return rc;
+  size_t need = 0;
+  sb_ctc_stream_workspace_size(B, T, beam_size, &need);
+  if (workspace_bytes < need) return SB_ERR_WORKSPACE;
+  DecParams p;
+  memset(&p, 0, sizeof(p));
+  p.logp = logp; p.lens = n;
+  p.trie = dec_stream_trie(state, B, max_frames, beam_size);
+  p.B = B; p.T = T; p.S = S; p.K = beam_size; p.blank = blank;
+  DecResume rs;
+  rs.slots = state;
+  rs.max_frames = max_frames;
+  return dec_launch(p, fu, &rs, static_cast<int*>(workspace), force_shortlist,
+                    reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int sb_ctc_stream_step(const float* logp, const int* n, int B, int T, int S,
+                                  int beam_size, int blank, int max_frames, void* state,
+                                  void* workspace, size_t workspace_bytes, void* stream) {
+  return dec_stream_entry(logp, n, B, T, S, beam_size, blank, max_frames, state, workspace,
+                          workspace_bytes, stream, false, NoFuse{});
+}
+
+extern "C" int sb_ctc_stream_step_shortlist(const float* logp, const int* n, int B, int T, int S,
+                                            int beam_size, int blank, int max_frames, void* state,
+                                            void* workspace, size_t workspace_bytes,
+                                            void* stream) {
+  return dec_stream_entry(logp, n, B, T, S, beam_size, blank, max_frames, state, workspace,
+                          workspace_bytes, stream, true, NoFuse{});
+}
+
+static int dec_stream_lm_entry(const float* logp, const int* n, int B, int T, int S,
+                               int beam_size, int blank, const SbNgramLm* lm, double lm_weight,
+                               double insertion_bonus, int max_frames, void* state,
+                               void* workspace, size_t workspace_bytes, void* stream,
+                               bool force_shortlist) {
+  LmFuse fu;
+  const int rc = dec_lm_fuse(S, blank, lm, lm_weight, insertion_bonus, &fu);
+  if (rc != SB_OK) return rc;
+  return dec_stream_entry(logp, n, B, T, S, beam_size, blank, max_frames, state, workspace,
+                          workspace_bytes, stream, force_shortlist, fu);
+}
+
+extern "C" int sb_ctc_stream_step_lm(const float* logp, const int* n, int B, int T, int S,
+                                     int beam_size, int blank, const SbNgramLm* lm,
+                                     double lm_weight, double insertion_bonus, int max_frames,
+                                     void* state, void* workspace, size_t workspace_bytes,
+                                     void* stream) {
+  return dec_stream_lm_entry(logp, n, B, T, S, beam_size, blank, lm, lm_weight, insertion_bonus,
+                             max_frames, state, workspace, workspace_bytes, stream, false);
+}
+
+extern "C" int sb_ctc_stream_step_lm_shortlist(const float* logp, const int* n, int B, int T,
+                                               int S, int beam_size, int blank,
+                                               const SbNgramLm* lm, double lm_weight,
+                                               double insertion_bonus, int max_frames,
+                                               void* state, void* workspace,
+                                               size_t workspace_bytes, void* stream) {
+  return dec_stream_lm_entry(logp, n, B, T, S, beam_size, blank, lm, lm_weight, insertion_bonus,
+                             max_frames, state, workspace, workspace_bytes, stream, true);
+}
+
+extern "C" int sb_ctc_stream_best(const void* state, int B, int max_frames, int beam_size,
+                                  int* out_labels, int* out_lens, double* out_scores,
+                                  int* out_overflow, void* stream) {
+  if (!state || !out_labels || !out_lens || !out_scores || !out_overflow) return SB_ERR_INVALID;
+  const int rc = dec_stream_check(B, max_frames, beam_size);
+  if (rc != SB_OK) return rc;
+  DecParams p;
+  memset(&p, 0, sizeof(p));
+  p.trie = dec_stream_trie(const_cast<void*>(state), B, max_frames, beam_size);
+  p.out_labels = out_labels; p.out_lens = out_lens; p.out_scores = out_scores;
+  p.B = B; p.T = max_frames; p.K = beam_size;
+  ctc_stream_best_kernel<<<B, 32, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p, state,
+                                                                              out_overflow);
+  return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
 }
 
 extern "C" int sb_debug_ctc_lm_rescans(unsigned long long* frames) {

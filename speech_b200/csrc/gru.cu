@@ -447,6 +447,13 @@ SB_DEVINL void gru_store_bwd(const GruBwdParams& p, long long m, int dir, int ju
   st_stream_bf16<UPT>(p.dghn + m * (p.ndir * H) + dir * H + ju, d.hn);
 }
 
+// Resumed forward (sb_gru_fwd_h0, one direction): step 0 publishes h_{-1}, which the caller put in
+// frame 0 of y and xn, instead of computing a state, and step s >= 1 reads gi frame s - 1.
+template <int UPT>
+SB_DEVINL void gru_load_h0(const GruFwdParams& p, int row, int ju, float (&h)[UPT]) {
+  ld_stream<UPT>(p.y + (long long)row * p.H + ju, h);
+}
+
 // ---- prologue pieces --------------------------------------------------------------------------
 SB_DEVINL void smem_zero(uint8_t* base, int bytes) {
   for (int k = threadIdx.x; k < bytes / 16; k += GRU_THREADS)
@@ -515,9 +522,9 @@ SB_DEVINL void init_ring_bars(uint64_t* full, uint64_t* empty, uint32_t csize) {
 // =============================================================================================
 // forward
 // =============================================================================================
-__global__ void __launch_bounds__(GRU_THREADS, 1)
-gru_fwd_kernel(const __grid_constant__ CUtensorMap tm_d0, const __grid_constant__ CUtensorMap tm_d1,
-               const GruFwdParams p) {
+template <bool H0>
+SB_DEVINL void gru_fwd_body(const CUtensorMap& tm_d0, const CUtensorMap& tm_d1,
+                            const GruFwdParams& p) {
   extern __shared__ uint8_t smem_raw[];
   const int H = p.H, Bp = p.Bp, T = p.T;
   const int nC = H / GRU_HC;
@@ -582,10 +589,16 @@ gru_fwd_kernel(const __grid_constant__ CUtensorMap tm_d0, const __grid_constant_
     float bias[3][GRU_UPT];
     gru_load_bias(s.scratch + uh * GRU_UPT, GRU_HC, bias);
     const bool active = row < Bp;
-    for (int step = 0; step < T; ++step) {
+    int step0 = 0;
+    if constexpr (H0) {
+      if (active) gru_load_h0(p, row, ju, hprev);
+      gru_publish(p, ctr, 0, false, false);
+      step0 = 1;
+    }
+    for (int step = step0; step < T; ++step) {
       const int t = dir == 0 ? step : (T - 1 - step);
       float gi[3][GRU_UPT];
-      if (active) gru_load_gi(p, t, row, dir, ju, gi);
+      if (active) gru_load_gi(p, t - step0, row, dir, ju, gi);
       float acc[3][GRU_UPT];
       if (step > 0) {
         mbar_wait(s.accfull, (step - 1) & 1);
@@ -617,6 +630,17 @@ gru_fwd_kernel(const __grid_constant__ CUtensorMap tm_d0, const __grid_constant_
 
   __syncthreads();
   cluster_sync_all();   // no CTA leaves while peers may still signal its barriers
+}
+
+__global__ void __launch_bounds__(GRU_THREADS, 1)
+gru_fwd_kernel(const __grid_constant__ CUtensorMap tm_d0, const __grid_constant__ CUtensorMap tm_d1,
+               const GruFwdParams p) {
+  gru_fwd_body<false>(tm_d0, tm_d1, p);
+}
+__global__ void __launch_bounds__(GRU_THREADS, 1)
+gru_fwd_h0_kernel(const __grid_constant__ CUtensorMap tm_d0,
+                  const __grid_constant__ CUtensorMap tm_d1, const GruFwdParams p) {
+  gru_fwd_body<true>(tm_d0, tm_d1, p);
 }
 
 // =============================================================================================
@@ -1066,10 +1090,9 @@ gru_bwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
 // until h_t is stored, 1.0-1.25 us more until the arrive.
 // Requires cluster size KS, H % (KS * 64) == 0, Bp <= 64.
 // =============================================================================================
-template <int KS>
-__global__ void __launch_bounds__(GRU_THREADS, 1)
-gru_fwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
-                  const __grid_constant__ CUtensorMap tm_d1, const GruFwdParams p) {
+template <int KS, bool H0>
+SB_DEVINL void gru_fwd_ks_body(const CUtensorMap& tm_d0, const CUtensorMap& tm_d1,
+                               const GruFwdParams& p) {
   static_assert(KS == 2 || KS == 4, "gru_fwd_ks_kernel: K split 2 or 4 ways");
   extern __shared__ uint8_t smem_raw[];
   const int H = p.H, Bp = p.Bp, T = p.T;
@@ -1174,10 +1197,16 @@ gru_fwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
     float bias[3][GRU_UPT];
     gru_load_bias(bias_s + uh * GRU_UPT, GRU_HC, bias);
 
-    for (int step = 0; step < T; ++step) {
+    int step0 = 0;
+    if constexpr (H0) {
+      if (active) gru_load_h0(p, row, ju, hprev);
+      gru_publish(p, ctr, 0, false, true);
+      step0 = 1;
+    }
+    for (int step = step0; step < T; ++step) {
       const int t = dir == 0 ? step : (T - 1 - step);
       float gi[3][GRU_UPT];
-      if (active) gru_load_gi(p, t, row, dir, ju, gi);
+      if (active) gru_load_gi(p, t - step0, row, dir, ju, gi);
       float acc[3][GRU_UPT] = {};
       if (step > 0) {
         mbar_wait(accfull, (step - 1) & 1);
@@ -1225,6 +1254,19 @@ gru_fwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
 
   __syncthreads();
   cluster_sync_all();
+}
+
+template <int KS>
+__global__ void __launch_bounds__(GRU_THREADS, 1)
+gru_fwd_ks_kernel(const __grid_constant__ CUtensorMap tm_d0,
+                  const __grid_constant__ CUtensorMap tm_d1, const GruFwdParams p) {
+  gru_fwd_ks_body<KS, false>(tm_d0, tm_d1, p);
+}
+template <int KS>
+__global__ void __launch_bounds__(GRU_THREADS, 1)
+gru_fwd_ks_h0_kernel(const __grid_constant__ CUtensorMap tm_d0,
+                     const __grid_constant__ CUtensorMap tm_d1, const GruFwdParams p) {
+  gru_fwd_ks_body<KS, true>(tm_d0, tm_d1, p);
 }
 
 // =============================================================================================
@@ -1344,10 +1386,9 @@ SB_DEVINL void bwd_kt_mma(uint8_t* ring, uint8_t* wtile, float* recv, float* sta
   }
 }
 
-template <int UPT>
-__global__ void __launch_bounds__(GRU_THREADS, 1)
-gru_fwd_kt_kernel(const __grid_constant__ CUtensorMap tm_d0,
-                  const __grid_constant__ CUtensorMap tm_d1, const GruFwdParams p) {
+template <int UPT, bool H0>
+SB_DEVINL void gru_fwd_kt_body(const CUtensorMap& tm_d0, const CUtensorMap& tm_d1,
+                               const GruFwdParams& p) {
   extern __shared__ uint8_t smem_raw[];
   const int H = p.H, Bp = p.Bp, T = p.T;
   const int nC = H / GRU_HC;
@@ -1435,10 +1476,16 @@ gru_fwd_kt_kernel(const __grid_constant__ CUtensorMap tm_d0,
     float bias[3][UPT] = {};
     if (active) gru_load_bias(bias_s + u0, GRU_HC, bias);
 
-    for (int step = 0; step < T; ++step) {
+    int step0 = 0;
+    if constexpr (H0) {
+      if (active) gru_load_h0(p, b, ju, hprev);
+      gru_publish(p, ctr, 0, false, true);
+      step0 = 1;
+    }
+    for (int step = step0; step < T; ++step) {
       const int t = dir == 0 ? step : (T - 1 - step);
       float gi[3][UPT];
-      if (active) gru_load_gi(p, t, b, dir, ju, gi);
+      if (active) gru_load_gi(p, t - step0, b, dir, ju, gi);
       float acc[3][UPT] = {};
       if (step > 0) {
         mbar_wait(accfull, (step - 1) & 1);
@@ -1471,6 +1518,19 @@ gru_fwd_kt_kernel(const __grid_constant__ CUtensorMap tm_d0,
 
   __syncthreads();
   cluster_sync_all();
+}
+
+template <int UPT>
+__global__ void __launch_bounds__(GRU_THREADS, 1)
+gru_fwd_kt_kernel(const __grid_constant__ CUtensorMap tm_d0,
+                  const __grid_constant__ CUtensorMap tm_d1, const GruFwdParams p) {
+  gru_fwd_kt_body<UPT, false>(tm_d0, tm_d1, p);
+}
+template <int UPT>
+__global__ void __launch_bounds__(GRU_THREADS, 1)
+gru_fwd_kt_h0_kernel(const __grid_constant__ CUtensorMap tm_d0,
+                     const __grid_constant__ CUtensorMap tm_d1, const GruFwdParams p) {
+  gru_fwd_kt_body<UPT, true>(tm_d0, tm_d1, p);
 }
 
 // =============================================================================================
@@ -1817,11 +1877,9 @@ SB_DEVINL void wide_setup(const WideSmem& s, int ring_bytes, int wbytes, uint32_
   });
 }
 
-template <int U, int NQ>
-__global__ void __launch_bounds__(GRU_THREADS, 1)
-gru_fwd_wide_kernel(const __grid_constant__ CUtensorMap tm_d0,
-                    const __grid_constant__ CUtensorMap tm_d1,
-                    const __grid_constant__ CUtensorMap tm_w, const GruFwdParams p) {
+template <int U, int NQ, bool H0>
+SB_DEVINL void gru_fwd_wide_body(const CUtensorMap& tm_d0, const CUtensorMap& tm_d1,
+                                 const CUtensorMap& tm_w, const GruFwdParams& p) {
   constexpr int NW = 3 * U;
   constexpr int WCHUNK = NW * 128;
   constexpr int RPT = 2048 / U;      // batch rows per pass of the 256 epilogue threads
@@ -1881,12 +1939,20 @@ gru_fwd_wide_kernel(const __grid_constant__ CUtensorMap tm_d0,
     float hprev[NQ][GRU_UPT] = {};
     float bias[3][GRU_UPT];
     gru_load_bias(s.scratch + uo, U, bias);
-    for (int step = 0; step < T; ++step) {
+    int step0 = 0;
+    if constexpr (H0) {
+#pragma unroll
+      for (int q = 0; q < NQ; ++q)
+        if (rsub + q * RPT < Bp) gru_load_h0(p, rsub + q * RPT, ju, hprev[q]);
+      gru_publish(p, ctr, 0, false, false);
+      step0 = 1;
+    }
+    for (int step = step0; step < T; ++step) {
       const int t = dir == 0 ? step : (T - 1 - step);
       float gi[NQ][3][GRU_UPT];
 #pragma unroll
       for (int q = 0; q < NQ; ++q)
-        if (rsub + q * RPT < Bp) gru_load_gi(p, t, rsub + q * RPT, dir, ju, gi[q]);
+        if (rsub + q * RPT < Bp) gru_load_gi(p, t - step0, rsub + q * RPT, dir, ju, gi[q]);
       if (step > 0) {
         mbar_wait(s.accfull, (step - 1) & 1);
         if (tid == 0) GRU_STAMP(3);
@@ -1919,6 +1985,21 @@ gru_fwd_wide_kernel(const __grid_constant__ CUtensorMap tm_d0,
 
   __syncthreads();
   cluster_sync_all();
+}
+
+template <int U, int NQ>
+__global__ void __launch_bounds__(GRU_THREADS, 1)
+gru_fwd_wide_kernel(const __grid_constant__ CUtensorMap tm_d0,
+                    const __grid_constant__ CUtensorMap tm_d1,
+                    const __grid_constant__ CUtensorMap tm_w, const GruFwdParams p) {
+  gru_fwd_wide_body<U, NQ, false>(tm_d0, tm_d1, tm_w, p);
+}
+template <int U, int NQ>
+__global__ void __launch_bounds__(GRU_THREADS, 1)
+gru_fwd_wide_h0_kernel(const __grid_constant__ CUtensorMap tm_d0,
+                       const __grid_constant__ CUtensorMap tm_d1,
+                       const __grid_constant__ CUtensorMap tm_w, const GruFwdParams p) {
+  gru_fwd_wide_body<U, NQ, true>(tm_d0, tm_d1, tm_w, p);
 }
 
 template <int U, int NQ>
@@ -2277,7 +2358,12 @@ static bool gru_wide_plan(int Bp, int H, int ndir, bool backward, bool no_reside
   return false;
 }
 
-static const void* gru_wide_kernel_fn(const GruWidePlan& w, int Bp, bool backward) {
+static const void* gru_wide_kernel_fn(const GruWidePlan& w, int Bp, bool backward,
+                                      bool h0 = false) {
+  if (h0)
+    return w.U == 16 ? (const void*)gru_fwd_wide_h0_kernel<16, 1>
+           : Bp > 64 ? (const void*)gru_fwd_wide_h0_kernel<32, 2>
+                     : (const void*)gru_fwd_wide_h0_kernel<32, 1>;
   if (backward)
     return w.U == 16 ? (const void*)gru_bwd_wide_kernel<16, 1>
            : Bp > 64 ? (const void*)gru_bwd_wide_kernel<32, 2>
@@ -2515,9 +2601,14 @@ extern "C" int sb_gru_fwd_workspace_size(int Bp, int H, int ndir, size_t* bytes)
   return SB_OK;
 }
 
-extern "C" int sb_gru_fwd(const float* gi, const void* whh_bf16, const float* bhh, float* y,
-                          void* xn_bf16, float* gates, void* workspace, size_t workspace_bytes,
-                          int T, int Bp, int H, int ndir, void* stream_) {
+// sb_gru_fwd, and with h0 (non-null) its resumed form sb_gru_fwd_h0, whose launch has T + 1 steps:
+// step 0 publishes h0, copied to frame 0 of y and xn.  The kernel selection depends on (Bp, H,
+// ndir) alone, so both forms of a shape run the same kernel.
+static int gru_fwd_entry(const float* gi, const void* whh_bf16, const float* bhh, const float* h0f,
+                         const void* h0_bf16, float* y, void* xn_bf16, float* gates,
+                         void* workspace, size_t workspace_bytes, int T, int Bp, int H, int ndir,
+                         void* stream_) {
+  const bool h0 = h0f != nullptr;
   GruWidePlan w;
   const bool wide = gru_check_shape(T, Bp, H, ndir) == SB_OK &&
                     gru_selects_wide(Bp, H, ndir, false, &w);
@@ -2534,6 +2625,16 @@ extern "C" int sb_gru_fwd(const float* gi, const void* whh_bf16, const float* bh
   uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
   unsigned int* barrier = reinterpret_cast<unsigned int*>(ws);
   gru_record_plan(0, nullptr);
+  if (h0) {
+    const size_t n = (size_t)Bp * H;
+    if ((static_cast<const void*>(h0f) != y &&
+         cudaMemcpyAsync(y, h0f, n * sizeof(float), cudaMemcpyDeviceToDevice, stream) !=
+             cudaSuccess) ||
+        (h0_bf16 != xn_bf16 && cudaMemcpyAsync(xn_bf16, h0_bf16, n * sizeof(bf16),
+                                               cudaMemcpyDeviceToDevice, stream) != cudaSuccess))
+      return SB_ERR_CUDA;
+    ++T;
+  }
 
   // ---- wide layers: U units per CTA, W_hh partly streamed from L2 (gru_fwd_wide_kernel) ----
   if (wide) {
@@ -2550,8 +2651,8 @@ extern "C" int sb_gru_fwd(const float* gi, const void* whh_bf16, const float* bh
     if (rc != SB_OK) return rc;
     void* args[] = {(void*)&tm[0], (void*)&tm[1], (void*)&tm[2], (void*)&p};
     const int nCw = H / w.U;
-    rc = gru_launch(gru_wide_kernel_fn(w, Bp, false), ndir * nCw, gru_cluster_size(nCw), w.smem,
-                    args, stream);
+    rc = gru_launch(gru_wide_kernel_fn(w, Bp, false, h0), ndir * nCw, gru_cluster_size(nCw),
+                    w.smem, args, stream);
     if (rc != SB_OK) return rc;
     gru_record_plan(0, &w);
     return gru_fwd_launched(GRU_FWD_WIDE);
@@ -2584,14 +2685,18 @@ extern "C" int sb_gru_fwd(const float* gi, const void* whh_bf16, const float* bh
       if (ks_smem <= 227 * 1024) {
         const size_t kt_smem = gru_fwd_kt_smem(Bp, H);
         if (gru_use_kt(Bp, false) && kt_smem <= 227 * 1024) {
-          const void* kt = Bp > 32   ? (const void*)gru_fwd_kt_kernel<4>
-                           : Bp > 16 ? (const void*)gru_fwd_kt_kernel<2>
-                                     : (const void*)gru_fwd_kt_kernel<1>;
+          const void* kt = h0 ? (Bp > 32   ? (const void*)gru_fwd_kt_h0_kernel<4>
+                                 : Bp > 16 ? (const void*)gru_fwd_kt_h0_kernel<2>
+                                           : (const void*)gru_fwd_kt_h0_kernel<1>)
+                              : (Bp > 32   ? (const void*)gru_fwd_kt_kernel<4>
+                                 : Bp > 16 ? (const void*)gru_fwd_kt_kernel<2>
+                                           : (const void*)gru_fwd_kt_kernel<1>);
           rc = gru_launch_exact(kt, ndir * nC, KS, kt_smem, kargs, stream);
           if (rc == SB_OK) return gru_fwd_launched(GRU_FWD_KT);
         }
-        rc = gru_launch_exact((const void*)gru_fwd_ks_kernel<KS>, ndir * nC, KS, ks_smem, kargs,
-                              stream);
+        rc = gru_launch_exact(h0 ? (const void*)gru_fwd_ks_h0_kernel<KS>
+                                 : (const void*)gru_fwd_ks_kernel<KS>,
+                              ndir * nC, KS, ks_smem, kargs, stream);
         if (rc == SB_OK) return gru_fwd_launched(GRU_FWD_KS4);
       }
     }
@@ -2602,8 +2707,9 @@ extern "C" int sb_gru_fwd(const float* gi, const void* whh_bf16, const float* bh
     const size_t ks2_smem = gru_fwd_ks_smem(2, Bp, H);
     if (ks2_smem <= 227 * 1024 && (H >= 512 || (g_gru_ablate & 1024))) {
       q.ring = H / 2 / 64;
-      rc = gru_launch_exact((const void*)gru_fwd_ks_kernel<2>, ndir * nC, 2, ks2_smem, kargs,
-                            stream);
+      rc = gru_launch_exact(h0 ? (const void*)gru_fwd_ks_h0_kernel<2>
+                               : (const void*)gru_fwd_ks_kernel<2>,
+                            ndir * nC, 2, ks2_smem, kargs, stream);
       if (rc == SB_OK) return gru_fwd_launched(GRU_FWD_KS2);
     }
   }
@@ -2620,9 +2726,26 @@ extern "C" int sb_gru_fwd(const float* gi, const void* whh_bf16, const float* bh
   rc = gru_dir_tmaps(tm, p.xn, H, (long long)T * Bp, H, (long long)ndir * H, ndir, Bp);
   if (rc != SB_OK) return rc;
   void* args[] = {(void*)&tm[0], (void*)&tm[1], (void*)&p};
-  rc = gru_launch((const void*)gru_fwd_kernel, ndir * nC, gru_cluster_size(nC), smem, args,
-                  stream);
+  rc = gru_launch(h0 ? (const void*)gru_fwd_h0_kernel : (const void*)gru_fwd_kernel, ndir * nC,
+                  gru_cluster_size(nC), smem, args, stream);
   return rc == SB_OK ? gru_fwd_launched(GRU_FWD_PLAIN) : rc;
+}
+
+extern "C" int sb_gru_fwd(const float* gi, const void* whh_bf16, const float* bhh, float* y,
+                          void* xn_bf16, float* gates, void* workspace, size_t workspace_bytes,
+                          int T, int Bp, int H, int ndir, void* stream) {
+  return gru_fwd_entry(gi, whh_bf16, bhh, nullptr, nullptr, y, xn_bf16, gates, workspace,
+                       workspace_bytes, T, Bp, H, ndir, stream);
+}
+
+extern "C" int sb_gru_fwd_h0(const float* gi, const void* whh_bf16, const float* bhh,
+                             const float* h0, const void* h0_bf16, float* y, void* xn_bf16,
+                             float* gates, void* workspace, size_t workspace_bytes, int T, int Bp,
+                             int H, int ndir, void* stream) {
+  if (ndir == 2) return SB_ERR_UNSUPPORTED;
+  if (!h0 || !h0_bf16) return SB_ERR_INVALID;
+  return gru_fwd_entry(gi, whh_bf16, bhh, h0, h0_bf16, y, xn_bf16, gates, workspace,
+                       workspace_bytes, T, Bp, H, ndir, stream);
 }
 
 // counters + the double-buffered exchange of dgh_t (Bp x 3H bf16 per direction and parity; the

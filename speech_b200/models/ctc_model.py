@@ -108,6 +108,16 @@ class CTC(model.Model):
             spans.append(list(zip(first.tolist(), last.tolist())))
         return (spans, scores) if return_scores else spans
 
+    def stream(self, num_streams, beam_size=1, max_frames=3000, lm=None, lm_weight=0.0,
+               insertion_bonus=0.0):
+        """Streaming recognition of num_streams (<= 128) utterances at once with a unidirectional
+        encoder: a speech_b200.streaming.CTCStream, whose push(chunks) feeds feature frames as
+        they arrive and partial() returns each stream's best labels so far; the final partial()
+        equals infer's search over the whole utterances (see that module).  max_frames caps the
+        encoder frames per stream between resets; lm, lm_weight, insertion_bonus: as infer."""
+        from ..streaming import CTCStream
+        return CTCStream(self, num_streams, beam_size, max_frames, lm, lm_weight, insertion_bonus)
+
     @staticmethod
     def max_decode(pred, blank):
         """Greedy collapse: merge repeats, then drop blanks (reference ctc_model.py:62-70)."""

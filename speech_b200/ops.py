@@ -437,6 +437,40 @@ def _workspace(nbytes, dev):
     return buf[off:off + nbytes]
 
 
+def gru_layer_operands(wl, l, Kl, ndir, H, Hp, dev):
+    """The recurrence's operands of GRU layer l at width Hp from its nn.GRU parameters wl (w_ih,
+    w_hh, b_ih, b_hh per direction) and an input of Kl columns: (wih_cat [ndir*3Hp][Kl] bf16,
+    whh [ndir][3Hp][Hp] bf16, bih_cat [ndir*3Hp] f32, bhh [ndir][3Hp] f32)."""
+    K3 = 3 * Hp
+    cached = _cached_gru_operands(wl[0], Kl) if Hp == H else None
+    if cached is not None:
+        # views of the optimizer's flat buffers (bf16 shadow written by sgd_clip_step)
+        return cached["wih"], cached["whh"], cached["bih"], cached["bhh"]
+    # (w_ih, w_hh, b_ih, b_hh) of each direction at the kernels' width
+    lw = [pad_gru_layer(*[q.detach() for q in wl[d * 4:d * 4 + 4]], H, Hp,
+                        ndir if l > 0 else 0) for d in range(ndir)]
+    In_l = lw[0][0].shape[1]
+    # bf16 operand copies of the master weights: one fused cast+copy per matrix
+    wih_cat = (torch.empty if Kl == In_l else torch.zeros)(
+        ndir * K3, Kl, dtype=torch.bfloat16, device=dev)
+    whh = torch.empty(ndir, K3, Hp, dtype=torch.bfloat16, device=dev)
+    for d in range(ndir):
+        wih_cat[d * K3:(d + 1) * K3, :In_l].copy_(lw[d][0])
+        whh[d].copy_(lw[d][1])
+    bih_cat = torch.cat([q[2] for q in lw]).float().contiguous()
+    bhh = torch.stack([q[3] for q in lw]).float().contiguous()
+    return wih_cat, whh, bih_cat, bhh
+
+
+def fc_operand(fc_w, ndir, H, Hp):
+    """[W | W] (one W per direction) bf16 at the layer width Hp: the B operand of the output
+    projection fused with the sum of the direction halves."""
+    wcat = fc_w.detach().to(torch.bfloat16)
+    if ndir == 2:
+        wcat = torch.cat([wcat, wcat], 1)
+    return pad_blocks(wcat, 1, ndir, H, Hp).contiguous()
+
+
 class GRUStackFunction(torch.autograd.Function):
     """Multi-layer (bi)directional GRU, semantics of nn.GRU(batch_first=True) with h0 = 0.
 
@@ -493,26 +527,7 @@ class GRUStackFunction(torch.autograd.Function):
         y = None
         for l in range(L):
             wl = weights[l * 4 * ndir:(l + 1) * 4 * ndir]
-            Kl = X.shape[1]
-            cached = _cached_gru_operands(wl[0], Kl) if Hp == H else None
-            if cached is not None:
-                # views of the optimizer's flat buffers (bf16 shadow written by sgd_clip_step)
-                wih_cat, whh = cached["wih"], cached["whh"]
-                bih_cat, bhh = cached["bih"], cached["bhh"]
-            else:
-                # (w_ih, w_hh, b_ih, b_hh) of each direction at the kernels' width
-                lw = [pad_gru_layer(*[q.detach() for q in wl[d * 4:d * 4 + 4]], H, Hp,
-                                    ndir if l > 0 else 0) for d in range(ndir)]
-                In_l = lw[0][0].shape[1]
-                # bf16 operand copies of the master weights: one fused cast+copy per matrix
-                wih_cat = (torch.empty if Kl == In_l else torch.zeros)(
-                    ndir * K3, Kl, dtype=torch.bfloat16, device=dev)
-                whh = torch.empty(ndir, K3, Hp, dtype=torch.bfloat16, device=dev)
-                for d in range(ndir):
-                    wih_cat[d * K3:(d + 1) * K3, :In_l].copy_(lw[d][0])
-                    whh[d].copy_(lw[d][1])
-                bih_cat = torch.cat([q[2] for q in lw]).float().contiguous()
-                bhh = torch.stack([q[3] for q in lw]).float().contiguous()
+            wih_cat, whh, bih_cat, bhh = gru_layer_operands(wl, l, X.shape[1], ndir, H, Hp, dev)
             if al is None:
                 gi = gemm_bf16_tn(X, wih_cat, bias=bih_cat)
             else:
@@ -558,10 +573,7 @@ class GRUStackFunction(torch.autograd.Function):
         ctx.fc = None
         if fc_w is not None:
             V = fc_w.shape[0]
-            wcat = fc_w.detach().to(torch.bfloat16)
-            if ndir == 2:
-                wcat = torch.cat([wcat, wcat], 1)
-            wcat = pad_blocks(wcat, 1, ndir, H, Hp).contiguous()
+            wcat = fc_operand(fc_w, ndir, H, Hp)
             out = gemm_bf16_tn(X, wcat, bias=fc_b.detach().float().contiguous(),
                                remap=(Bp, T, B)).view(B, T, V)
             ctx.fc = (fc_w, X)

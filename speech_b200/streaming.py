@@ -1,0 +1,256 @@
+"""Streaming recognition with a unidirectional CTC model: hypotheses while the audio arrives.
+
+    st = model.stream(num_streams, beam_size=8, lm=lm, lm_weight=0.5)
+    st.push([feats_0, feats_1, ...])      # (n_b, F) new feature frames per stream, n_b may be 0
+    hyps = st.partial()                   # best label list of each stream so far
+
+Every stage carries what the next chunk needs and nothing more:
+  * conv front-end: a stream keeps its input frames from next_b * prod(strides) onward, next_b its
+    next encoder frame, and runs the stack over that carry plus the chunk.  The stack is a valid
+    (unpadded) convolution, so its complete output frames are exactly the whole utterance's.
+  * GRU layers: the input projection, then the recurrence from each stream's carried state
+    (sb_gru_fwd_h0); the new state is the fp32 y and bf16 xn at the stream's last new frame.
+  * output: the fused projection, softmax and log as CTC.infer computes them, then one step of the
+    resumable prefix beam search (sb_ctc_stream_step[_lm]), whose beams stay on the device.
+With B streams, the final partial(return_scores=True) equals decode_batch(with_scores=True) on the
+logits of CTC.infer over the same B utterances in the exact-lengths mode, bit for bit: each stage
+computes the same values as the offline pass.  The recurrence kernel is selected by the number of
+batch rows, so against an offline batch of another size the results agree only to the GRU's
+rounding tolerance.
+"""
+import numpy as np
+import torch
+
+from . import _lib, features, ops
+from .models.ctc_decoder import check_lm
+
+MAX_STREAMS = ops.GRU_MAX_BATCH   # one recurrence launch per layer and push
+
+
+class CTCStream:
+    """B streams of one unidirectional CTC model (see the module docstring).  Built by
+    CTC.stream; the model's weights are read once, when the stream is built."""
+
+    def __init__(self, model, num_streams, beam_size=1, max_frames=3000, lm=None, lm_weight=0.0,
+                 insertion_bonus=0.0):
+        B = int(num_streams)
+        if not 1 <= B <= MAX_STREAMS:
+            raise ValueError("num_streams must lie in [1, %d], got %d" % (MAX_STREAMS, B))
+        if model.rnn.bidirectional:
+            raise ValueError("a bidirectional encoder cannot stream: it needs the whole utterance")
+        if getattr(model, "parity_mode", False):
+            raise ValueError("parity_mode has no streaming path")
+        if not 1 <= int(beam_size) <= 32:
+            raise ValueError("beam_size must lie in [1, 32], got %r" % (beam_size,))
+        if int(max_frames) < 1:
+            raise ValueError("max_frames must be >= 1, got %r" % (max_frames,))
+        check_lm(lm, lm_weight, insertion_bonus, model.blank + 1, model.blank)
+        if not model.is_cuda:
+            raise _lib.SpeechB200Error("CTC.stream needs the model on a CUDA device")
+        lib = _lib.load()
+        self.model = model
+        self.B, self.Bp = B, ops._round_up(B, 8)
+        self.K, self.max_frames = int(beam_size), int(max_frames)
+        self.lm, self.lm_weight, self.insertion_bonus = lm, float(lm_weight), float(insertion_bonus)
+        self.dev = dev = next(model.parameters()).device
+        self.stride = int(np.prod([c.stride[0] for c in model.conv.children()
+                                   if isinstance(c, torch.nn.Conv2d)]))
+        rnn = model.rnn
+        self.H = H = rnn.hidden_size
+        self.Hp = Hp = ops.gru_padded_width(self.Bp, H, 1)
+        _, weights = ops._gru_weights(rnn)
+        self.layers = []
+        with torch.no_grad():
+            Kl = ops._round_up(rnn.input_size, 8)
+            for l in range(rnn.num_layers):
+                self.layers.append(ops.gru_layer_operands(weights[l * 4:(l + 1) * 4], l, Kl, 1, H,
+                                                          Hp, dev))
+                Kl = Hp
+            self.fc_w = ops.fc_operand(model.fc.fc.weight, 1, H, Hp)
+            self.fc_b = model.fc.fc.bias.detach().float().contiguous()
+        self.ws_bytes = _lib.workspace_size(lib.sb_gru_fwd_workspace_size, self.Bp, Hp, 1)
+        self.ws = ops._workspace(self.ws_bytes, dev)
+        self.h = [torch.zeros(self.Bp, Hp, dtype=torch.float32, device=dev) for _ in self.layers]
+        self.hb = [torch.zeros(self.Bp, Hp, dtype=torch.bfloat16, device=dev) for _ in self.layers]
+        order = 0 if lm is None else lm.order
+        nbytes = _lib.workspace_size(lib.sb_ctc_stream_state_size, B, self.max_frames, self.K,
+                                     order)
+        self.state = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        self.carry = [None] * B                  # input frames from next_b * stride on
+        self.pcm = [np.zeros(0, np.int16) for _ in range(B)]    # push_audio's carried samples
+        self.next = [0] * B                      # encoder frames produced per stream
+        self._reset_search(0, B)
+
+    def _reset_search(self, first, count):
+        lib = _lib.load()
+        with torch.cuda.device(self.dev):
+            ops._launch("ctc_stream_reset",  0.0,
+                        lambda: lib.sb_ctc_stream_reset(self.state.data_ptr(), self.B,
+                                                        self.max_frames, self.K, first, count,
+                                                        _lib.stream_ptr()))
+
+    @property
+    def frames(self):
+        """encoder frames consumed per stream; frame t starts at input frame t * prod(strides)"""
+        return list(self.next)
+
+    def reset(self, b):
+        """start slot b afresh: conv carry, GRU states and search"""
+        b = int(b)
+        if not 0 <= b < self.B:
+            raise ValueError("stream %d out of range [0, %d)" % (b, self.B))
+        self.carry[b] = None
+        self.pcm[b] = np.zeros(0, np.int16)
+        self.next[b] = 0
+        for h, hb in zip(self.h, self.hb):
+            h[b].zero_()
+            hb[b].zero_()
+        self._reset_search(b, 1)
+
+    # ---- conv front-end ----
+    def _conv_inputs(self, chunks):
+        """the carry + chunk of each stream and the encoder frames it completes (host only)"""
+        if len(chunks) != self.B:
+            raise ValueError("push takes one chunk per stream (%d), got %d" % (self.B, len(chunks)))
+        xs, counts = [], []
+        for b, c in enumerate(chunks):
+            c = torch.as_tensor(c)
+            if c.dim() != 2:
+                raise ValueError("chunk %d must be (frames, features), got shape %s"
+                                 % (b, tuple(c.shape)))
+            c = c.to(self.dev, torch.float32)
+            x = c if self.carry[b] is None else torch.cat([self.carry[b], c], 0)
+            xs.append(x)
+            counts.append(max(0, self.model.conv_out_size(x.shape[0], 0)))
+        F = xs[0].shape[1]
+        if any(x.shape[1] != F for x in xs):
+            raise ValueError("every chunk must have the same number of features")
+        for b, n in enumerate(counts):
+            if self.next[b] + n > self.max_frames:
+                raise ValueError("stream %d would pass max_frames = %d (%d + %d encoder frames)"
+                                 % (b, self.max_frames, self.next[b], n))
+        return xs, counts
+
+    def push(self, chunks):
+        """Feed one (n_b, F) chunk of feature frames to every stream (n_b may be 0): runs the
+        encoder over the encoder frames the chunks complete and advances each stream's search."""
+        xs, counts = self._conv_inputs(chunks)
+        T = max(counts)
+        if T > 0:
+            with torch.no_grad():
+                logp = self._encode(xs, counts, T)
+            self._search(logp, counts)
+        self._advance(xs, counts)
+        return counts
+
+    def _advance(self, xs, counts):
+        """drop the input frames no later encoder frame reads: frame next_b starts at input frame
+        next_b * stride of the stream, and so every strided layer stays aligned"""
+        for b, n in enumerate(counts):
+            self.carry[b] = xs[b][n * self.stride:]
+            self.next[b] += n
+
+    def _encode(self, xs, counts, T):
+        """(B, T, S) log-probabilities of the new encoder frames (rows past counts[b] unused)"""
+        lib = _lib.load()
+        B, Bp, Hp, dev = self.B, self.Bp, self.Hp, self.dev
+        L = max(x.shape[0] for x in xs)
+        x = torch.zeros(B, L, xs[0].shape[1], dtype=torch.float32, device=dev)
+        for b, xb in enumerate(xs):
+            x[b, :xb.shape[0]] = xb
+        feats = ops.conv_stack(x, self.model.conv, False)[:, :T]       # (B, T, In)
+        In = feats.shape[2]
+        X = torch.zeros(T, Bp, ops._round_up(In, 8), dtype=torch.bfloat16, device=dev)
+        X[:, :B, :In] = feats.transpose(0, 1)
+        X = X.view(T * Bp, -1)
+        last = torch.tensor(counts + [0] * (Bp - B), dtype=torch.int64).to(dev) * Bp + \
+            torch.arange(Bp, device=dev)                                # frame counts[b] of y
+        sp = _lib.stream_ptr()
+        for l, (wih, whh, bih, bhh) in enumerate(self.layers):
+            gi = ops.gemm_bf16_tn(X, wih, bias=bih)
+            y = torch.empty((T + 1) * Bp, Hp, dtype=torch.float32, device=dev)
+            xn = torch.empty((T + 1) * Bp, Hp, dtype=torch.bfloat16, device=dev)
+            h, hb = self.h[l], self.hb[l]
+            ops._launch("gru_fwd", 2.0 * T * Bp * 3 * Hp * Hp,
+                        lambda: lib.sb_gru_fwd_h0(gi.data_ptr(), whh.data_ptr(), bhh.data_ptr(),
+                                                  h.data_ptr(), hb.data_ptr(), y.data_ptr(),
+                                                  xn.data_ptr(), None, self.ws.data_ptr(),
+                                                  self.ws_bytes, T, Bp, Hp, 1, sp))
+            h.copy_(y[last])
+            hb.copy_(xn[last])
+            X = xn[Bp:]
+        out = ops.gemm_bf16_tn(X, self.fc_w, bias=self.fc_b, remap=(Bp, T, B))
+        out = out.view(B, T, -1)
+        # CTC.infer: softmax over the classes, then decode_batch's float32 log
+        probs = torch.nn.functional.softmax(out, dim=2)
+        return torch.log(probs.float()).contiguous()
+
+    def _search(self, logp, counts):
+        lib = _lib.load()
+        B, T, S = logp.shape
+        n = torch.tensor(counts, dtype=torch.int32).to(self.dev)
+        ws_bytes = _lib.workspace_size(lib.sb_ctc_stream_workspace_size, B, T, self.K)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=self.dev)
+        args = (self.max_frames, self.state.data_ptr(), ws.data_ptr(), ws_bytes, _lib.stream_ptr())
+        with torch.cuda.device(self.dev):
+            if self.lm is None:
+                ops._launch("ctc_stream_step", 0.0,
+                            lambda: lib.sb_ctc_stream_step(logp.data_ptr(), n.data_ptr(), B, T, S,
+                                                           self.K, self.model.blank, *args))
+            else:
+                tables, _ = self.lm.device_tables(self.dev)
+                ops._launch("ctc_stream_step_lm", 0.0,
+                            lambda: lib.sb_ctc_stream_step_lm(
+                                logp.data_ptr(), n.data_ptr(), B, T, S, self.K, self.model.blank,
+                                tables, self.lm_weight, self.insertion_bonus, *args))
+
+    def partial(self, return_scores=False):
+        """Best label list of each stream so far (one device-to-host copy); with return_scores,
+        (labels, score) pairs, the score as decode_batch(with_scores=True) reports it."""
+        lib = _lib.load()
+        B, Tm = self.B, self.max_frames
+        off = B * Tm + 2 * B + (B * Tm) % 2          # float64 scores 8-byte aligned
+        buf = torch.empty(off + 2 * B, dtype=torch.int32, device=self.dev)
+        labels, lens, ovf = buf[:B * Tm], buf[B * Tm:B * Tm + B], buf[B * Tm + B:B * Tm + 2 * B]
+        scores = buf[off:].view(torch.float64)
+        with torch.cuda.device(self.dev):
+            ops._launch("ctc_stream_best", 0.0,
+                        lambda: lib.sb_ctc_stream_best(self.state.data_ptr(), B, Tm, self.K,
+                                                       labels.data_ptr(), lens.data_ptr(),
+                                                       scores.data_ptr(), ovf.data_ptr(),
+                                                       _lib.stream_ptr()))
+        host = buf.cpu()
+        lab = host[:B * Tm].view(B, Tm).numpy()
+        n = host[B * Tm:B * Tm + B].numpy()
+        sc = host[off:].view(torch.float64).numpy()
+        res = [tuple(int(v) for v in lab[b, :n[b]]) for b in range(B)]
+        return [(r, float(s)) for r, s in zip(res, sc)] if return_scores else res
+
+    def push_audio(self, pcm, sample_rate=16000, mean=None, std=None, window_size=20, step_size=10,
+                   eps=1e-10):
+        """Feed int16 PCM samples per stream: featurised by features.log_specgram_batch (same
+        arguments) over the samples carried from the last call plus the new ones, so that every
+        feature frame is the one the whole-utterance featuriser computes; then push."""
+        if len(pcm) != self.B:
+            raise ValueError("push_audio takes one array per stream (%d), got %d"
+                             % (self.B, len(pcm)))
+        nperseg = int(window_size * sample_rate / 1e3)
+        step = nperseg - int(step_size * sample_rate / 1e3)
+        audio = []
+        for b, a in enumerate(pcm):
+            a = np.asarray(a)
+            if a.dtype != np.int16 or a.ndim != 1:
+                raise ValueError("push_audio expects 1-D int16 arrays")
+            audio.append(np.concatenate([self.pcm[b], a]))
+        nf = [features.frame_count(len(a), nperseg, step) for a in audio]
+        if max(nf) > 0:
+            feats, _ = features.log_specgram_batch(audio, sample_rate, mean=mean, std=std,
+                                                   window_size=window_size, step_size=step_size,
+                                                   eps=eps, device=self.dev)
+            chunks = [feats[b, :nf[b]] for b in range(self.B)]
+        else:
+            chunks = [torch.zeros(0, nperseg // 2 + 1, device=self.dev) for _ in range(self.B)]
+        counts = self.push(chunks)
+        for b, a in enumerate(audio):
+            self.pcm[b] = a[nf[b] * step:]
+        return counts
