@@ -732,10 +732,25 @@ int sb_rnnt_decode_static_shortlist(const float* sl_val, const int* sl_idx, cons
  *   emb[sym[r]] (Kin = embedding width; sym[r] = -1 or sym NULL: zeros) or x[r] (Kin = H), hidden
  *   state h_prev[(r / K) * K + par[r]] (par[r] = -1 or par NULL: zeros; -2: row skipped) -> h[r],
  *   and bf16(h[r]) at y[r * ldy] if y is not NULL.  beam_size <= 32, kp <= 64.
+ * Streaming (speech_b200.streaming.TransducerStream): the same entry points resume a search across
+ * calls.  The workspace is sized and every call is made with T = max_frames, the most frames a
+ * stream is ever searched over (T only sizes the workspace's carve: trie node ids come from each
+ * utterance's own count of selection rounds, never from t); each push of n_b new frames runs the
+ * loop above for t = 0 .. max_b n_b - 1, local to the push, with tlens = the n_b, so that stream b
+ * takes its n_b frames and is left untouched by the others.  sb_rnnt_search_final does not change
+ * the state: it may be read after any push.  Default workspace, K = 8, S = 4, max_frames = 3000:
+ * 5120 + B * 3,915,748 bytes (about 3.7 MiB per stream).
+ * sb_rnnt_search_reset: utterances [first, first + count) back to sb_rnnt_search_init's state
+ *   (the empty hypothesis at frame 0: cleared trie, the root as the beam, zero counters and flag,
+ *   slot_lens rows zero), others untouched; sb_rnnt_search_init is the reset of [0, B).
+ *   SB_ERR_INVALID for a null slot_lens or workspace, bad sizes or a range outside [0, B),
+ *   SB_ERR_WORKSPACE for a short workspace, SB_ERR_UNSUPPORTED for beam_size > 32.
  * ------------------------------------------------------------------------------------- */
 int sb_rnnt_search_workspace_size(int B, int T, int S, int beam_size, size_t* bytes);
 int sb_rnnt_search_init(int* slot_lens, int B, int T, int S, int beam_size, void* workspace,
                         size_t workspace_bytes, void* stream);
+int sb_rnnt_search_reset(int* slot_lens, int B, int T, int S, int beam_size, int first, int count,
+                         void* workspace, size_t workspace_bytes, void* stream);
 int sb_rnnt_search_round(const float* lp, const float* sl_val, const int* sl_idx,
                          const float* sl_meta, int kp, const int* tlens, int t, int level,
                          int max_len, int* par, int* sym, int* slot_lens, int B, int T, int S,

@@ -156,6 +156,8 @@ SIGNATURES = {
     "sb_rnnt_search_workspace_size": (_c_int, [_c_int, _c_int, _c_int, _c_int,
                                                ctypes.POINTER(_c_sz)]),
     "sb_rnnt_search_init": (_c_int, [_vp, _c_int, _c_int, _c_int, _c_int, _vp, _c_sz, _vp]),
+    "sb_rnnt_search_reset": (_c_int, [_vp, _c_int, _c_int, _c_int, _c_int, _c_int, _c_int, _vp,
+                                      _c_sz, _vp]),
     "sb_rnnt_search_round": (_c_int, [_vp, _vp, _vp, _vp, _c_int, _vp, _c_int, _c_int, _c_int, _vp,
                                       _vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int, _c_int,
                                       _vp, _c_sz, _vp]),

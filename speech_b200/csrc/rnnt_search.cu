@@ -103,8 +103,10 @@ static RsWs rs_carve(void* workspace, int B, const RsSizes& sz) {
 
 // ---- search kernels --------------------------------------------------------------------------
 
-__global__ void __launch_bounds__(RS_THREADS) rnnt_search_init_kernel(RsWs w, int K, int* slot_lens) {
-  const int b = blockIdx.x, tid = threadIdx.x;
+// utterances first + blockIdx.x: the empty hypothesis at frame 0
+__global__ void __launch_bounds__(RS_THREADS) rnnt_search_init_kernel(RsWs w, int K, int* slot_lens,
+                                                                      int first) {
+  const int b = first + blockIdx.x, tid = threadIdx.x;
   w.trie.of(b).clear<RS_THREADS>();
   if (tid == 0) {
     RsState& s = w.st[b];
@@ -494,7 +496,19 @@ extern "C" int sb_rnnt_search_init(int* slot_lens, int B, int T, int S, int beam
   if (rc != SB_OK) return rc;
   if (!slot_lens) return SB_ERR_INVALID;
   rnnt_search_init_kernel<<<B, RS_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      w, beam_size, slot_lens);
+      w, beam_size, slot_lens, 0);
+  return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
+}
+
+extern "C" int sb_rnnt_search_reset(int* slot_lens, int B, int T, int S, int beam_size, int first,
+                                    int count, void* workspace, size_t workspace_bytes,
+                                    void* stream) {
+  if (!slot_lens || first < 0 || count <= 0 || count > B - first) return SB_ERR_INVALID;
+  RsWs w;
+  const int rc = rs_ws(workspace, workspace_bytes, B, T, S, beam_size, &w);
+  if (rc != SB_OK) return rc;
+  rnnt_search_init_kernel<<<count, RS_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      w, beam_size, slot_lens, first);
   return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
 }
 

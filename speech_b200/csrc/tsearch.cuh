@@ -19,6 +19,20 @@
 // than on float32 lists, but they still need |fs| of about 2^52 times the gap of two classes'
 // fused values.
 //
+// A search that cannot be rerun (the streaming search of rnnt_search.cu keeps no past rows) reads
+// lists of 64 entries from its first frame instead of kp = K lists plus a rerun, and gives the
+// offline search's answer wherever it is not flagged.  An unflagged selection is the full route's
+// at any kp, so until its first flag the stream is in the full route's state, as is the offline
+// kp = K pass until its first flag.  A flag at kp = 64 implies a flag at kp = K on the same state
+// (the kp = K list is the head of the kp = 64 one).  The selected value x sits at a list position
+// below K, so x >= beta_K >= beta_64, and fs + (.) is monotone, so fs + beta_64 == s forces
+// fs + beta_K == s.  Then either x > beta_K (the kp = K test holds outright), or x == beta_K and
+// beta_64 <= nextafter(beta_K, -inf) < beta_K (or beta_64 == beta_K), so fs + nextafter(beta_K,
+// -inf) == s as well.  Where the 64-entry list's tie scan picks an entry of equal sum at position
+// >= K, the kp = K list lacks it, selects an entry of larger value and so flags by the same
+// reasoning.  So a stream flags only where the offline search reruns and then raises, and it
+// reports the flag instead of an unproven hypothesis.
+//
 // Every function is called by all N threads of the block.  Frontier, beam and the "new" arrays are
 // the caller's shared memory; `done` and the trie may live anywhere.
 #pragma once

@@ -169,6 +169,14 @@ class Transducer(model.Model):
                                       insertion_bonus)
         return (labels, scores) if return_scores else labels
 
+    def stream(self, num_streams, beam_size=4, max_symbols_per_frame=4, max_frames=3000,
+               max_len=None, lm=None, lm_weight=0.0, insertion_bonus=0.0):
+        """Streaming recognition of num_streams utterances with a unidirectional encoder:
+        `recognize`'s search resumed chunk by chunk (speech_b200.streaming.TransducerStream)."""
+        from ..streaming import TransducerStream
+        return TransducerStream(self, num_streams, beam_size, max_symbols_per_frame, max_frames,
+                                max_len, lm, lm_weight, insertion_bonus)
+
     def align(self, batch, return_scores=False):
         """Viterbi (forced) alignment of each transcript to its audio: the single best path through
         the compact lattice `loss` sums over (functions.transducer.rnnt_viterbi).
@@ -199,33 +207,34 @@ class Transducer(model.Model):
         return torch.from_numpy(model.end_pad_labels(labels))
 
 
-class PredictionRows:
-    """Row provider of transducer_decoders.search_batch for a Transducer on a batch of inputs: the
-    encoder's fc1 outputs once (time-major, frame t = a contiguous (B, Hj) block), then per level
-    one sb_rnnt_pred_step per prediction-network layer and fc1 of the new states (the wgmma GEMM,
-    bf16 operands: the arithmetic of ops.linear with joint_inputs' padded weights) into an arena of
-    per-slot states, and the joint rows at frame t with `forward`'s kernels (fused at T = 1,
-    U1 = K where fc2 is resident, else one slab of the large-vocabulary joint)."""
+def fc1_operands(model):
+    """joint_inputs' fc1 weight and bias padded to Hj outputs: (w1 (Hj, H) f32, b1 (Hj) f32)"""
+    fc1 = model.fc1.fc
+    H = fc1.out_features
+    Hj = (H + 7) // 8 * 8
+    w1 = ops.pad_blocks(fc1.weight.detach(), 0, 1, H, Hj)
+    b1 = ops.pad_blocks(fc1.bias.detach(), 0, 1, H, Hj).float().contiguous()
+    return w1, b1
 
-    def __init__(self, model, inputs):
-        with torch.no_grad():
-            x = model.stage_inputs(inputs)
-            if model.exact_lengths:
-                tl = [max(0, model.conv_out_size(i.shape[0], 0)) for i in inputs]
-                enc = model._encode(x, torch.tensor(tl, dtype=torch.int32))
-            else:
-                enc = model._encode(x, None)
-            fc1 = model.fc1.fc
-            H = fc1.out_features
-            Hj = (H + 7) // 8 * 8
-            w1 = ops.pad_blocks(fc1.weight.detach(), 0, 1, H, Hj)
-            b1 = ops.pad_blocks(fc1.bias.detach(), 0, 1, H, Hj).float().contiguous()
-            fx = model.fc1(enc) if Hj == H else ops.linear(enc, w1, b1)
+
+class PredictionNet:
+    """The prediction and joint networks of a Transducer as a row provider of B utterances
+    (transducer_decoders.search_batch / StreamSearch): per level one sb_rnnt_pred_step per
+    prediction-network layer and fc1 of the new states (the wgmma GEMM, bf16 operands: the
+    arithmetic of ops.linear with joint_inputs' padded weights) into an arena of per-slot states,
+    and the joint rows at frame t with `forward`'s kernels (fused at T = 1, U1 = K where fc2 is
+    resident, else one slab of the large-vocabulary joint).  The encoder's fc1 rows are the
+    caller's: fxT, time-major, frame t a (>= B, Hj) float32 block whose first B rows are read."""
+
+    def __init__(self, model, B, device, w1=None, b1=None):
+        if w1 is None:
+            w1, b1 = fc1_operands(model)
+        H = model.fc1.fc.out_features
+        Hj = (H + 7) // 8 * 8
         self.model = model
-        self.B, self.T = fx.shape[0], fx.shape[1]
-        self.tlens = tl if model.exact_lengths else [self.T] * self.B
-        self.device = fx.device
-        self.fxT = fx.detach().float().transpose(0, 1).contiguous()        # (T', B, Hj)
+        self.B = B
+        self.device = device
+        self.fxT = None
         self.H, self.Hj, self.Hp = H, Hj, (H + 7) // 8 * 8
         self.w1 = torch.nn.functional.pad(w1.to(torch.bfloat16), (0, self.Hp - H)).contiguous()
         self.b1 = b1
@@ -312,3 +321,25 @@ class PredictionRows:
 
     def arenas(self):
         return self.hid, self.layers, self.H, self.fy, self.Hj
+
+
+class PredictionRows(PredictionNet):
+    """Row provider of transducer_decoders.search_batch for a Transducer on a batch of inputs: the
+    encoder's fc1 outputs once (time-major, frame t = a contiguous (B, Hj) block), then the rows of
+    PredictionNet."""
+
+    def __init__(self, model, inputs):
+        with torch.no_grad():
+            x = model.stage_inputs(inputs)
+            if model.exact_lengths:
+                tl = [max(0, model.conv_out_size(i.shape[0], 0)) for i in inputs]
+                enc = model._encode(x, torch.tensor(tl, dtype=torch.int32))
+            else:
+                enc = model._encode(x, None)
+            w1, b1 = fc1_operands(model)
+            H = model.fc1.fc.out_features
+            fx = model.fc1(enc) if w1.shape[0] == H else ops.linear(enc, w1, b1)
+            super().__init__(model, fx.shape[0], fx.device, w1, b1)
+        self.T = fx.shape[1]
+        self.tlens = tl if model.exact_lengths else [self.T] * self.B
+        self.fxT = fx.detach().float().transpose(0, 1).contiguous()        # (T', B, Hj)

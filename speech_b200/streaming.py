@@ -1,22 +1,38 @@
-"""Streaming recognition with a unidirectional CTC model: hypotheses while the audio arrives.
+"""Streaming recognition with a unidirectional encoder: hypotheses while the audio arrives.
 
-    st = model.stream(num_streams, beam_size=8, lm=lm, lm_weight=0.5)
+    st = model.stream(num_streams, beam_size=8, lm=lm, lm_weight=0.5)   # CTC or Transducer
     st.push([feats_0, feats_1, ...])      # (n_b, F) new feature frames per stream, n_b may be 0
     hyps = st.partial()                   # best label list of each stream so far
 
-Every stage carries what the next chunk needs and nothing more:
+Every stage carries what the next chunk needs and nothing more (EncoderStream, shared by both):
   * conv front-end: a stream keeps its input frames from next_b * prod(strides) onward, next_b its
     next encoder frame, and runs the stack over that carry plus the chunk.  The stack is a valid
     (unpadded) convolution, so its complete output frames are exactly the whole utterance's.
   * GRU layers: the input projection, then the recurrence from each stream's carried state
     (sb_gru_fwd_h0); the new state is the fp32 y and bf16 xn at the stream's last new frame.
-  * output: the fused projection, softmax and log as CTC.infer computes them, then one step of the
-    resumable prefix beam search (sb_ctc_stream_step[_lm]), whose beams stay on the device.
+CTCStream then runs the fused projection, softmax and log as CTC.infer computes them, and one step
+of the resumable prefix beam search (sb_ctc_stream_step[_lm]), whose beams stay on the device.
 With B streams, the final partial(return_scores=True) equals decode_batch(with_scores=True) on the
 logits of CTC.infer over the same B utterances in the exact-lengths mode, bit for bit: each stage
 computes the same values as the offline pass.  The recurrence kernel is selected by the number of
 batch rows, so against an offline batch of another size the results agree only to the GRU's
 rounding tolerance.
+
+TransducerStream runs fc1 on the top layer's bf16 xn of the new frames (the wgmma GEMM with the
+padded weights of transducer_model.PredictionNet, as the offline ops.linear does on the same
+values), then Transducer.recognize's label-free search resumed over them
+(transducer_decoders.StreamSearch): the search state, trie and prediction-state arenas stay on the
+device.  Between pushes every stream's beam states are in block 0 of the arenas: a push of n_b
+frames leaves stream b's beam in block 0 or S + 1 by the parity of n_b (the beam block flips once
+per frame for the whole batch), and one masked copy per arena moves the odd ones back.  After
+every push, partial(return_scores=True) equals Transducer.recognize(inputs_so_far, ...,
+return_scores=True) in the exact-lengths mode bit for bit, given two preconditions: the same B
+(as above), and an offline fc1 on the GEMM, which holds where B * T' >= 128 or H is not a multiple
+of 8 (below 128 rows LinearND runs fp32 nn.Linear; the GEMM picks its tile by N only and never
+splits K without accumulating, so a row's output does not depend on the number of rows).
+Where the search's candidates do not fit the full route (decode_static_fits), the stream reads
+64-entry lists from the first frame; partial raises for a stream whose lists flagged a selection,
+as recognize would after its rerun, until that stream is reset.
 """
 import numpy as np
 import torch
@@ -27,12 +43,13 @@ from .models.ctc_decoder import check_lm
 MAX_STREAMS = ops.GRU_MAX_BATCH   # one recurrence launch per layer and push
 
 
-class CTCStream:
-    """B streams of one unidirectional CTC model (see the module docstring).  Built by
-    CTC.stream; the model's weights are read once, when the stream is built."""
+class EncoderStream:
+    """The encoder half of a stream (see the module docstring): conv carry, per-layer GRU operands
+    and states, frames and push_audio.  Subclasses check their arguments, then call
+    _init_encoder."""
 
-    def __init__(self, model, num_streams, beam_size=1, max_frames=3000, lm=None, lm_weight=0.0,
-                 insertion_bonus=0.0):
+    @staticmethod
+    def _check(model, num_streams, beam_size, max_frames):
         B = int(num_streams)
         if not 1 <= B <= MAX_STREAMS:
             raise ValueError("num_streams must lie in [1, %d], got %d" % (MAX_STREAMS, B))
@@ -44,14 +61,15 @@ class CTCStream:
             raise ValueError("beam_size must lie in [1, 32], got %r" % (beam_size,))
         if int(max_frames) < 1:
             raise ValueError("max_frames must be >= 1, got %r" % (max_frames,))
-        check_lm(lm, lm_weight, insertion_bonus, model.blank + 1, model.blank)
+        return B
+
+    def _init_encoder(self, model, B, max_frames, what):
         if not model.is_cuda:
-            raise _lib.SpeechB200Error("CTC.stream needs the model on a CUDA device")
+            raise _lib.SpeechB200Error("%s needs the model on a CUDA device" % what)
         lib = _lib.load()
         self.model = model
         self.B, self.Bp = B, ops._round_up(B, 8)
-        self.K, self.max_frames = int(beam_size), int(max_frames)
-        self.lm, self.lm_weight, self.insertion_bonus = lm, float(lm_weight), float(insertion_bonus)
+        self.max_frames = int(max_frames)
         self.dev = dev = next(model.parameters()).device
         self.stride = int(np.prod([c.stride[0] for c in model.conv.children()
                                    if isinstance(c, torch.nn.Conv2d)]))
@@ -66,36 +84,20 @@ class CTCStream:
                 self.layers.append(ops.gru_layer_operands(weights[l * 4:(l + 1) * 4], l, Kl, 1, H,
                                                           Hp, dev))
                 Kl = Hp
-            self.fc_w = ops.fc_operand(model.fc.fc.weight, 1, H, Hp)
-            self.fc_b = model.fc.fc.bias.detach().float().contiguous()
         self.ws_bytes = _lib.workspace_size(lib.sb_gru_fwd_workspace_size, self.Bp, Hp, 1)
         self.ws = ops._workspace(self.ws_bytes, dev)
         self.h = [torch.zeros(self.Bp, Hp, dtype=torch.float32, device=dev) for _ in self.layers]
         self.hb = [torch.zeros(self.Bp, Hp, dtype=torch.bfloat16, device=dev) for _ in self.layers]
-        order = 0 if lm is None else lm.order
-        nbytes = _lib.workspace_size(lib.sb_ctc_stream_state_size, B, self.max_frames, self.K,
-                                     order)
-        self.state = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         self.carry = [None] * B                  # input frames from next_b * stride on
         self.pcm = [np.zeros(0, np.int16) for _ in range(B)]    # push_audio's carried samples
         self.next = [0] * B                      # encoder frames produced per stream
-        self._reset_search(0, B)
-
-    def _reset_search(self, first, count):
-        lib = _lib.load()
-        with torch.cuda.device(self.dev):
-            ops._launch("ctc_stream_reset",  0.0,
-                        lambda: lib.sb_ctc_stream_reset(self.state.data_ptr(), self.B,
-                                                        self.max_frames, self.K, first, count,
-                                                        _lib.stream_ptr()))
 
     @property
     def frames(self):
         """encoder frames consumed per stream; frame t starts at input frame t * prod(strides)"""
         return list(self.next)
 
-    def reset(self, b):
-        """start slot b afresh: conv carry, GRU states and search"""
+    def _reset_encoder(self, b):
         b = int(b)
         if not 0 <= b < self.B:
             raise ValueError("stream %d out of range [0, %d)" % (b, self.B))
@@ -105,7 +107,7 @@ class CTCStream:
         for h, hb in zip(self.h, self.hb):
             h[b].zero_()
             hb[b].zero_()
-        self._reset_search(b, 1)
+        return b
 
     # ---- conv front-end ----
     def _conv_inputs(self, chunks):
@@ -131,18 +133,6 @@ class CTCStream:
                                  % (b, self.max_frames, self.next[b], n))
         return xs, counts
 
-    def push(self, chunks):
-        """Feed one (n_b, F) chunk of feature frames to every stream (n_b may be 0): runs the
-        encoder over the encoder frames the chunks complete and advances each stream's search."""
-        xs, counts = self._conv_inputs(chunks)
-        T = max(counts)
-        if T > 0:
-            with torch.no_grad():
-                logp = self._encode(xs, counts, T)
-            self._search(logp, counts)
-        self._advance(xs, counts)
-        return counts
-
     def _advance(self, xs, counts):
         """drop the input frames no later encoder frame reads: frame next_b starts at input frame
         next_b * stride of the stream, and so every strided layer stays aligned"""
@@ -150,8 +140,9 @@ class CTCStream:
             self.carry[b] = xs[b][n * self.stride:]
             self.next[b] += n
 
-    def _encode(self, xs, counts, T):
-        """(B, T, S) log-probabilities of the new encoder frames (rows past counts[b] unused)"""
+    def _encoder(self, xs, counts, T):
+        """(T * Bp, Hp) bf16 xn of the top GRU layer at the new encoder frames (frame t of stream b
+        at row t * Bp + b; rows past counts[b] unused)"""
         lib = _lib.load()
         B, Bp, Hp, dev = self.B, self.Bp, self.Hp, self.dev
         L = max(x.shape[0] for x in xs)
@@ -179,6 +170,87 @@ class CTCStream:
             h.copy_(y[last])
             hb.copy_(xn[last])
             X = xn[Bp:]
+        return X
+
+    def push_audio(self, pcm, sample_rate=16000, mean=None, std=None, window_size=20, step_size=10,
+                   eps=1e-10):
+        """Feed int16 PCM samples per stream: featurised by features.log_specgram_batch (same
+        arguments) over the samples carried from the last call plus the new ones, so that every
+        feature frame is the one the whole-utterance featuriser computes; then push."""
+        if len(pcm) != self.B:
+            raise ValueError("push_audio takes one array per stream (%d), got %d"
+                             % (self.B, len(pcm)))
+        nperseg = int(window_size * sample_rate / 1e3)
+        step = nperseg - int(step_size * sample_rate / 1e3)
+        audio = []
+        for b, a in enumerate(pcm):
+            a = np.asarray(a)
+            if a.dtype != np.int16 or a.ndim != 1:
+                raise ValueError("push_audio expects 1-D int16 arrays")
+            audio.append(np.concatenate([self.pcm[b], a]))
+        nf = [features.frame_count(len(a), nperseg, step) for a in audio]
+        if max(nf) > 0:
+            feats, _ = features.log_specgram_batch(audio, sample_rate, mean=mean, std=std,
+                                                   window_size=window_size, step_size=step_size,
+                                                   eps=eps, device=self.dev)
+            chunks = [feats[b, :nf[b]] for b in range(self.B)]
+        else:
+            chunks = [torch.zeros(0, nperseg // 2 + 1, device=self.dev) for _ in range(self.B)]
+        counts = self.push(chunks)
+        for b, a in enumerate(audio):
+            self.pcm[b] = a[nf[b] * step:]
+        return counts
+
+
+class CTCStream(EncoderStream):
+    """B streams of one unidirectional CTC model (see the module docstring).  Built by
+    CTC.stream; the model's weights are read once, when the stream is built."""
+
+    def __init__(self, model, num_streams, beam_size=1, max_frames=3000, lm=None, lm_weight=0.0,
+                 insertion_bonus=0.0):
+        B = self._check(model, num_streams, beam_size, max_frames)
+        check_lm(lm, lm_weight, insertion_bonus, model.blank + 1, model.blank)
+        self._init_encoder(model, B, max_frames, "CTC.stream")
+        lib = _lib.load()
+        self.K = int(beam_size)
+        self.lm, self.lm_weight, self.insertion_bonus = lm, float(lm_weight), float(insertion_bonus)
+        with torch.no_grad():
+            self.fc_w = ops.fc_operand(model.fc.fc.weight, 1, self.H, self.Hp)
+            self.fc_b = model.fc.fc.bias.detach().float().contiguous()
+        order = 0 if lm is None else lm.order
+        nbytes = _lib.workspace_size(lib.sb_ctc_stream_state_size, B, self.max_frames, self.K,
+                                     order)
+        self.state = torch.empty(nbytes, dtype=torch.uint8, device=self.dev)
+        self._reset_search(0, B)
+
+    def _reset_search(self, first, count):
+        lib = _lib.load()
+        with torch.cuda.device(self.dev):
+            ops._launch("ctc_stream_reset",  0.0,
+                        lambda: lib.sb_ctc_stream_reset(self.state.data_ptr(), self.B,
+                                                        self.max_frames, self.K, first, count,
+                                                        _lib.stream_ptr()))
+
+    def reset(self, b):
+        """start slot b afresh: conv carry, GRU states and search"""
+        self._reset_search(self._reset_encoder(b), 1)
+
+    def push(self, chunks):
+        """Feed one (n_b, F) chunk of feature frames to every stream (n_b may be 0): runs the
+        encoder over the encoder frames the chunks complete and advances each stream's search."""
+        xs, counts = self._conv_inputs(chunks)
+        T = max(counts)
+        if T > 0:
+            with torch.no_grad():
+                logp = self._encode(xs, counts, T)
+            self._search(logp, counts)
+        self._advance(xs, counts)
+        return counts
+
+    def _encode(self, xs, counts, T):
+        """(B, T, S) log-probabilities of the new encoder frames (rows past counts[b] unused)"""
+        B, Bp = self.B, self.Bp
+        X = self._encoder(xs, counts, T)
         out = ops.gemm_bf16_tn(X, self.fc_w, bias=self.fc_b, remap=(Bp, T, B))
         out = out.view(B, T, -1)
         # CTC.infer: softmax over the classes, then decode_batch's float32 log
@@ -226,31 +298,56 @@ class CTCStream:
         res = [tuple(int(v) for v in lab[b, :n[b]]) for b in range(B)]
         return [(r, float(s)) for r, s in zip(res, sc)] if return_scores else res
 
-    def push_audio(self, pcm, sample_rate=16000, mean=None, std=None, window_size=20, step_size=10,
-                   eps=1e-10):
-        """Feed int16 PCM samples per stream: featurised by features.log_specgram_batch (same
-        arguments) over the samples carried from the last call plus the new ones, so that every
-        feature frame is the one the whole-utterance featuriser computes; then push."""
-        if len(pcm) != self.B:
-            raise ValueError("push_audio takes one array per stream (%d), got %d"
-                             % (self.B, len(pcm)))
-        nperseg = int(window_size * sample_rate / 1e3)
-        step = nperseg - int(step_size * sample_rate / 1e3)
-        audio = []
-        for b, a in enumerate(pcm):
-            a = np.asarray(a)
-            if a.dtype != np.int16 or a.ndim != 1:
-                raise ValueError("push_audio expects 1-D int16 arrays")
-            audio.append(np.concatenate([self.pcm[b], a]))
-        nf = [features.frame_count(len(a), nperseg, step) for a in audio]
-        if max(nf) > 0:
-            feats, _ = features.log_specgram_batch(audio, sample_rate, mean=mean, std=std,
-                                                   window_size=window_size, step_size=step_size,
-                                                   eps=eps, device=self.dev)
-            chunks = [feats[b, :nf[b]] for b in range(self.B)]
-        else:
-            chunks = [torch.zeros(0, nperseg // 2 + 1, device=self.dev) for _ in range(self.B)]
-        counts = self.push(chunks)
-        for b, a in enumerate(audio):
-            self.pcm[b] = a[nf[b] * step:]
+
+class TransducerStream(EncoderStream):
+    """B streams of one Transducer with a unidirectional encoder (see the module docstring).
+    Built by Transducer.stream; the model's weights are read once, when the stream is built.
+    beam_size, max_symbols_per_frame, max_len and the LM arguments are Transducer.recognize's;
+    max_frames caps the encoder frames per stream between resets (it sizes the search's trie)."""
+
+    def __init__(self, model, num_streams, beam_size=4, max_symbols_per_frame=4, max_frames=3000,
+                 max_len=None, lm=None, lm_weight=0.0, insertion_bonus=0.0):
+        from .models.transducer_model import PredictionNet
+        from .transducer_decoders import StreamSearch, check_stream_args
+        B = self._check(model, num_streams, beam_size, max_frames)
+        check_stream_args(beam_size, max_symbols_per_frame, max_frames, max_len,
+                          model.fc2.fc.out_features, model.blank, lm, lm_weight, insertion_bonus)
+        self._init_encoder(model, B, max_frames, "Transducer.stream")
+        with torch.no_grad():
+            self.pred = PredictionNet(model, B, self.dev)
+        self.Kr = ops._round_up(self.H, 8)     # the contraction of the offline ops.linear
+        self.search = StreamSearch(self.pred, beam_size, max_symbols_per_frame, max_frames,
+                                   model.blank, max_len, lm, lm_weight, insertion_bonus)
+
+    def reset(self, b):
+        """start slot b afresh: conv carry, GRU states, search and its prediction states"""
+        self.search.reset(self._reset_encoder(b))
+
+    def push(self, chunks):
+        """Feed one (n_b, F) chunk of feature frames to every stream (n_b may be 0): runs the
+        encoder over the encoder frames the chunks complete and advances each stream's search."""
+        xs, counts = self._conv_inputs(chunks)
+        T = max(counts)
+        if T > 0:
+            with torch.no_grad():
+                self._encode(xs, counts, T)
+            self.search.push(counts)
+        self._advance(xs, counts)
         return counts
+
+    def _encode(self, xs, counts, T):
+        """fc1 of the new encoder frames into the prediction network's fxT: (T, Bp, Hj), frame t
+        of stream b at [t, b].  xn's columns H .. Kr - 1 are zero (padded GRU units stay 0), as
+        the offline ops.linear's zero padding of bf16(y)."""
+        X = self._encoder(xs, counts, T)[:, :self.Kr]
+        fx = ops.gemm_bf16_tn(X, self.pred.w1, bias=self.pred.b1)
+        self.pred.fxT = fx.view(T, self.Bp, -1)
+
+    def partial(self, return_scores=False):
+        """Best label list of each stream so far (one device-to-host copy); with return_scores,
+        (labels, score) pairs, the float64 score as Transducer.recognize(return_scores=True)
+        reports it.  Raises SpeechB200Error naming the streams whose shortlists flagged a
+        selection (the large-vocabulary route only)."""
+        labels, scores = self.search.best()
+        res = [tuple(int(v) for v in lab) for lab in labels]
+        return list(zip(res, scores)) if return_scores else res

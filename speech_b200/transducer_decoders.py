@@ -183,15 +183,56 @@ class SearchSlots:
                         torch.empty(B, K, 2, dtype=torch.float64, device=dev))
 
 
+def _search_frame(lib, provider, slots, tl_dev, t, cur, max_len, blank, ws, nbytes, sp,
+                  lm_args=None):
+    """the launches of frame t: per level the provider's rows, the round (with an LM first the
+    fused rows, lm_args = (tables, lm_weight, insertion_bonus)) and the new frontier's states,
+    then frame_end into block S + 1 - cur.  slots.T sizes the workspace, t < slots.T."""
+    B, K, S, T, kp, V1 = slots.B, slots.K, slots.S, slots.T, slots.kp, provider.V1
+    sl = slots.sl
+    for level in range(S + 1):
+        block = cur if level == 0 else level
+        provider.rows(t, block, slots)
+        if lm_args is None:
+            ops._launch("rnnt_search", 0.0, lambda: lib.sb_rnnt_search_round(
+                _lib.ptr(slots.lp), *(_lib.ptr(a) for a in (sl or (None,) * 3)), kp or 0,
+                tl_dev.data_ptr(), t, level, max_len, slots.par.data_ptr(),
+                slots.sym.data_ptr(), slots.slot_lens.data_ptr(), B, T, S, V1, K, blank,
+                ws.data_ptr(), nbytes, sp))
+        else:
+            tables, weight, bonus = lm_args
+            fsl = tuple(_lib.ptr(a) for a in (slots.fsl or (None,) * 3))
+            ops._launch("rnnt_search_lm_rows", 0.0, lambda: lib.sb_rnnt_search_lm_rows(
+                slots.lp.data_ptr(), _lib.ptr(slots.flp), *fsl, kp or 0,
+                tl_dev.data_ptr(), t, level, B, T, S, V1, K, blank,
+                ctypes.byref(tables), weight, bonus, ws.data_ptr(), nbytes, sp))
+            ops._launch("rnnt_search", 0.0, lambda: lib.sb_rnnt_search_round_lm(
+                _lib.ptr(slots.flp), *fsl, kp or 0, tl_dev.data_ptr(), t, level,
+                max_len, slots.par.data_ptr(), slots.sym.data_ptr(),
+                slots.slot_lens.data_ptr(), B, T, S, V1, K, blank, ws.data_ptr(), nbytes,
+                sp))
+        if level < S:
+            provider.extend(block, level + 1, slots)
+    hid, layers, H, fy, Hj = provider.arenas()
+    ops._launch("rnnt_search", 0.0, lambda: lib.sb_rnnt_search_frame_end(
+        tl_dev.data_ptr(), t, slots.slot_lens.data_ptr(), _lib.ptr(hid), layers, H,
+        _lib.ptr(fy), Hj, cur, S + 1 - cur, B, T, S, K, ws.data_ptr(), nbytes, sp))
+
+
+def _lm_args(fusion, dev):
+    if fusion is None:
+        return None
+    tables, _ = fusion[0].device_tables(dev)
+    return tables, float(fusion[1]), float(fusion[2])
+
+
 def _search_once(provider, tl, T, K, S, max_len, L, blank, kp, fusion=None):
     """one search at list length kp (None: full rows); fusion: None or (NGramLM, lm_weight,
     insertion_bonus) -> (label lists, scores, flag counts)"""
     lib = _lib.load()
     B, V1, dev = provider.B, provider.V1, provider.device
     slots = SearchSlots(B, K, S, T, V1, kp, dev, fused=fusion is not None)
-    if fusion is not None:
-        tables, _ = fusion[0].device_tables(dev)
-        weights = (float(fusion[1]), float(fusion[2]))
+    lm_args = _lm_args(fusion, dev)
     nbytes = _lib.workspace_size(lib.sb_rnnt_search_workspace_size, B, T, S, K)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     tl_dev = torch.tensor(tl, dtype=torch.int32).pin_memory().to(dev, non_blocking=True)
@@ -201,7 +242,6 @@ def _search_once(provider, tl, T, K, S, max_len, L, blank, kp, fusion=None):
     out = torch.zeros(n_int + 2 * B, dtype=torch.int32, device=dev)
     labels, lens, flags = out[:B * L], out[B * L:B * L + B], out[B * L + B:B * L + 2 * B]
     scores = out[n_int:].view(torch.float64)
-    sl = slots.sl
     with torch.cuda.device(dev):
         sp = _lib.stream_ptr()
         provider.begin(slots)
@@ -209,32 +249,8 @@ def _search_once(provider, tl, T, K, S, max_len, L, blank, kp, fusion=None):
             slots.slot_lens.data_ptr(), B, T, S, K, ws.data_ptr(), nbytes, sp))
         cur = 0
         for t in range(T):
-            for level in range(S + 1):
-                block = cur if level == 0 else level
-                provider.rows(t, block, slots)
-                if fusion is None:
-                    ops._launch("rnnt_search", 0.0, lambda: lib.sb_rnnt_search_round(
-                        _lib.ptr(slots.lp), *(_lib.ptr(a) for a in (sl or (None,) * 3)), kp or 0,
-                        tl_dev.data_ptr(), t, level, max_len, slots.par.data_ptr(),
-                        slots.sym.data_ptr(), slots.slot_lens.data_ptr(), B, T, S, V1, K, blank,
-                        ws.data_ptr(), nbytes, sp))
-                else:
-                    fsl = tuple(_lib.ptr(a) for a in (slots.fsl or (None,) * 3))
-                    ops._launch("rnnt_search_lm_rows", 0.0, lambda: lib.sb_rnnt_search_lm_rows(
-                        slots.lp.data_ptr(), _lib.ptr(slots.flp), *fsl, kp or 0,
-                        tl_dev.data_ptr(), t, level, B, T, S, V1, K, blank,
-                        ctypes.byref(tables), *weights, ws.data_ptr(), nbytes, sp))
-                    ops._launch("rnnt_search", 0.0, lambda: lib.sb_rnnt_search_round_lm(
-                        _lib.ptr(slots.flp), *fsl, kp or 0, tl_dev.data_ptr(), t, level,
-                        max_len, slots.par.data_ptr(), slots.sym.data_ptr(),
-                        slots.slot_lens.data_ptr(), B, T, S, V1, K, blank, ws.data_ptr(), nbytes,
-                        sp))
-                if level < S:
-                    provider.extend(block, level + 1, slots)
-            hid, layers, H, fy, Hj = provider.arenas()
-            ops._launch("rnnt_search", 0.0, lambda: lib.sb_rnnt_search_frame_end(
-                tl_dev.data_ptr(), t, slots.slot_lens.data_ptr(), _lib.ptr(hid), layers, H,
-                _lib.ptr(fy), Hj, cur, S + 1 - cur, B, T, S, K, ws.data_ptr(), nbytes, sp))
+            _search_frame(lib, provider, slots, tl_dev, t, cur, max_len, blank, ws, nbytes, sp,
+                          lm_args)
             cur = S + 1 - cur
         ops._launch("rnnt_search", 0.0, lambda: lib.sb_rnnt_search_final(
             labels.data_ptr(), L, lens.data_ptr(), scores.data_ptr(), flags.data_ptr(), B, T, S,
@@ -296,3 +312,139 @@ def search_batch(provider, tlens, beam_size, blank, max_symbols_per_frame, max_l
         for b in rerun:
             labels[b], scores[b] = lab2[b], sc2[b]
     return labels, scores
+
+
+# ------------------------------------------------------------------------------------------------
+# Streaming (streaming.TransducerStream): search_batch's loop resumed push by push.  The workspace
+# is sized for T = max_frames and every launch passes that T; a push of counts[b] new frames per
+# stream runs frames t = 0 .. max(counts) - 1 of the push with tlens = counts, so stream b takes
+# its own frames and the kernels skip it after them.  The beam's prediction states sit in block
+# `cur` of the arenas, which flips once per frame for the whole batch: after the push, a stream
+# with an odd count has its beam in block S + 1, and settle_beams copies it to block 0, so that
+# between pushes every stream's beam is in block 0.
+# ------------------------------------------------------------------------------------------------
+def check_stream_args(beam_size, max_symbols_per_frame, max_frames, max_len, V1, blank, lm,
+                      lm_weight, insertion_bonus):
+    """the stream search's ValueErrors, raised before any launch"""
+    from .models.ctc_decoder import check_lm
+    if not 1 <= int(beam_size) <= 32:
+        raise ValueError("beam_size must lie in [1, 32], got %r" % (beam_size,))
+    if int(max_symbols_per_frame) < 1:
+        raise ValueError("max_symbols_per_frame must be >= 1, got %r" % (max_symbols_per_frame,))
+    if int(max_frames) < 1:
+        raise ValueError("max_frames must be >= 1, got %r" % (max_frames,))
+    if max_len is not None and int(max_len) < 1:
+        raise ValueError("max_len must be >= 1 or None, got %r" % (max_len,))
+    check_lm(lm, lm_weight, insertion_bonus, V1, blank, search="Transducer")
+
+
+def settle_beams(arenas, counts, K):
+    """Block S + 1 rows -> block 0 rows of every stream with an odd count, one masked copy per
+    arena.  arenas: tensors (S + 2, ..., B * K, width) or None; counts: (B,) frames of the push."""
+    odd = (counts.to(torch.int64) % 2 == 1).repeat_interleave(K).view(-1, 1)
+    for a in arenas:
+        if a is not None:
+            a[0].copy_(torch.where(odd.to(a.device), a[-1], a[0]))
+
+
+class StreamSearch:
+    """The label-free search of provider.B streams, resumed across pushes (see above).
+    provider: as search_batch's (B, V1, device, begin, rows, extend, arenas; T is not read), with
+    rows(t, block, slots) reading frame t of the current push.  Candidates go through the full rows
+    where they fit (decode_static_fits) and otherwise through SHORTLIST_RERUN-entry lists from the
+    first frame: a stream cannot rerun, and where those lists flag a selection the offline search
+    would rerun and flag it too (csrc/tsearch.cuh), so best() raises for it instead.  max_len None:
+    no cap beyond max_frames * max_symbols_per_frame, which never binds."""
+
+    def __init__(self, provider, beam_size, max_symbols_per_frame, max_frames, blank, max_len=None,
+                 lm=None, lm_weight=0.0, insertion_bonus=0.0):
+        B, V1, dev = provider.B, provider.V1, provider.device
+        check_stream_args(beam_size, max_symbols_per_frame, max_frames, max_len, V1, blank, lm,
+                          lm_weight, insertion_bonus)
+        lib = _lib.load()
+        self.provider, self.B, self.blank, self.dev = provider, B, int(blank), dev
+        self.K, self.S, self.Tm = K, S, Tm = (int(beam_size), int(max_symbols_per_frame),
+                                              int(max_frames))
+        self.max_len = Tm * S if max_len is None else min(int(max_len), Tm * S)
+        self.kp = None if decode_static_fits(K, V1) else SHORTLIST_RERUN
+        self.slots = SearchSlots(B, K, S, Tm, V1, self.kp, dev, fused=lm is not None)
+        self.lm_args = _lm_args(None if lm is None else (lm, lm_weight, insertion_bonus), dev)
+        self.nbytes = _lib.workspace_size(lib.sb_rnnt_search_workspace_size, B, Tm, S, K)
+        self.ws = torch.empty(self.nbytes, dtype=torch.uint8, device=dev)
+        self.frames = [0] * B
+        with torch.cuda.device(dev):
+            provider.begin(self.slots)
+            self._reset(0, B)
+        # the empty hypothesis's prediction state (the same in every row of block 0), for reset
+        hid, _, _, fy, _ = provider.arenas()
+        self.empty = [None if a is None else a[0].narrow(-2, 0, 1).clone() for a in (hid, fy)]
+
+    def _reset(self, first, count):
+        lib, s = _lib.load(), self.slots
+        ops._launch("rnnt_search", 0.0, lambda: lib.sb_rnnt_search_reset(
+            s.slot_lens.data_ptr(), self.B, self.Tm, self.S, self.K, first, count,
+            self.ws.data_ptr(), self.nbytes, _lib.stream_ptr()))
+
+    def reset(self, b):
+        """stream b back to the empty hypothesis at frame 0; the others are untouched"""
+        hid, _, _, fy, _ = self.provider.arenas()
+        with torch.cuda.device(self.dev):
+            self._reset(b, 1)
+            for a, e in zip((hid, fy), self.empty):
+                if a is not None:
+                    a[0].narrow(-2, b * self.K, self.K).copy_(e.expand_as(
+                        a[0].narrow(-2, 0, self.K)))
+        self.frames[b] = 0
+
+    def push(self, counts):
+        """search counts[b] more frames of stream b (the provider's frames 0 .. counts[b] - 1)"""
+        counts = [int(n) for n in counts]
+        if len(counts) != self.B:
+            raise ValueError("push takes one frame count per stream (%d), got %d"
+                             % (self.B, len(counts)))
+        if any(n < 0 or f + n > self.Tm for f, n in zip(self.frames, counts)):
+            raise ValueError("a push would take a stream past max_frames = %d" % self.Tm)
+        P = max(counts)
+        if P == 0:
+            return
+        lib, S = _lib.load(), self.S
+        tl_dev = torch.tensor(counts, dtype=torch.int32).pin_memory().to(self.dev,
+                                                                          non_blocking=True)
+        with torch.cuda.device(self.dev):
+            sp = _lib.stream_ptr()
+            cur = 0
+            for t in range(P):
+                _search_frame(lib, self.provider, self.slots, tl_dev, t, cur, self.max_len,
+                              self.blank, self.ws, self.nbytes, sp, self.lm_args)
+                cur = S + 1 - cur
+            if any(n % 2 for n in counts):
+                hid, _, _, fy, _ = self.provider.arenas()
+                settle_beams((hid, fy), tl_dev, self.K)
+        self.frames = [f + n for f, n in zip(self.frames, counts)]
+
+    def best(self):
+        """(label lists, float64 scores) of every stream's best hypothesis so far, one
+        device->host copy; raises where the shortlists flagged a selection of a stream"""
+        lib, B = _lib.load(), self.B
+        L = max(1, min(self.max_len, max(self.frames) * self.S))
+        n_int = B * (L + 2)
+        n_int += n_int % 2
+        out = torch.zeros(n_int + 2 * B, dtype=torch.int32, device=self.dev)
+        labels, lens, flags = out[:B * L], out[B * L:B * L + B], out[B * L + B:B * L + 2 * B]
+        scores = out[n_int:].view(torch.float64)
+        with torch.cuda.device(self.dev):
+            ops._launch("rnnt_search", 0.0, lambda: lib.sb_rnnt_search_final(
+                labels.data_ptr(), L, lens.data_ptr(), scores.data_ptr(), flags.data_ptr(), B,
+                self.Tm, self.S, self.K, self.ws.data_ptr(), self.nbytes, _lib.stream_ptr()))
+        host = out.cpu()
+        fl = host[B * L + B:B * L + 2 * B].tolist()
+        bad = [b for b, f in enumerate(fl) if f]
+        if bad:
+            raise _lib.SpeechB200Error(
+                "speech_b200: the shortlist beam search cannot order tied candidates of "
+                "stream(s) %s even from %d-entry lists (reset them to go on)"
+                % (bad, SHORTLIST_RERUN))
+        lab = host[:B * L].view(B, L)
+        n = host[B * L:B * L + B].tolist()
+        sc = host[n_int:].view(torch.float64).tolist()
+        return [lab[b, :n[b]].tolist() for b in range(B)], sc

@@ -240,3 +240,19 @@ for U in (300, 700):
                                   torch.tensor([U, U]), 28)
     print("rnnt viterbi U=%d" % U, sc.tolist())
 torch.cuda.synchronize()
+# Transducer streaming with an LM: the resumed search (reset, rounds over local frames, the
+# parity copy) on the full route (V+1 = 29) and the 64-entry shortlist route (V+1 = 20001)
+cfg_s = {"dropout": 0.0, "encoder": {"conv": [[8, 5, 8, 2], [8, 5, 8, 2]],
+                                     "rnn": {"dim": 64, "bidirectional": False, "layers": 2}},
+         "decoder": {"embedding_dim": 16, "layers": 1}}
+for V, lm_s in ((28, lm_t), (20000, lm_tv)):
+    ts = Transducer(80, V, cfg_s).cuda()
+    ts.set_eval()
+    st = ts.stream(3, beam_size=4, max_symbols_per_frame=2, max_frames=64, lm=lm_s,
+                   lm_weight=0.5, insertion_bonus=1.0)
+    for p, k in ((0, 17), (17, 5), (22, 40)):
+        st.push([x[p:p + k] for x in inputs[:3]])
+    st.reset(1)
+    st.push([inputs[0][:0], inputs[3][:30], inputs[2][:0]])
+    print("transducer stream V+1=%d" % (V + 1), st.frames, st.partial(return_scores=True))
+torch.cuda.synchronize()
