@@ -375,6 +375,25 @@ int sb_conv_dtop(const float* dY, const float* C, const void* mask_u8, float msc
 int sb_conv_col2im_relu(const float* dA, long long ldA, const float* Pprev,
                         const void* maskprev_u8, float mscale, void* dCprev_bf16, float* db, int B,
                         int Ti, int Fi, int Ci, int kh, int kw, int stride, void* stream);
+/* Direct convolution of a layer past the first (no patch matrix): the footprint of each output
+ * tile is staged in shared memory as im2col stages A (ReLU, dropout, bf16), so the operands equal
+ * the im2col path's.  Wp is the [Co][ldw] bf16 weight matrix of the im2col path (K order
+ * (i, j, ci)).  sb_conv_direct_ok: 1 when all three kernels take the layer (Ci, Co multiples of 8,
+ * Co <= 32, resident weights and footprint within shared memory), else 0 (use im2col).
+ *   sb_conv_fwd_direct    P (ReLU on read) -> C [M][Co] f32 = conv + bias
+ *   sb_conv_dgrad_direct  dC bf16 [M][Co] -> dC of the layer below, as sb_conv_col2im_relu
+ *   sb_conv_wgrad_direct  dWT [K][Co] f32 += sum over pixels of act * dC (fp32 atomics) */
+int sb_conv_direct_ok(int Fi, int Ci, int Co, int kh, int kw, int stride);
+int sb_conv_fwd_direct(const float* P, const void* mask_u8, float mscale, const void* Wp_bf16,
+                       int ldw, const float* bias, float* C, int B, int Ti, int Fi, int Ci, int Co,
+                       int kh, int kw, int stride, void* stream);
+int sb_conv_dgrad_direct(const void* dC_bf16, const void* Wp_bf16, int ldw, const float* Pprev,
+                         const void* maskprev_u8, float mscale, void* dCprev_bf16, float* db,
+                         int B, int Ti, int Fi, int Ci, int Co, int kh, int kw, int stride,
+                         void* stream);
+int sb_conv_wgrad_direct(const float* P, const void* mask_u8, float mscale, const void* dC_bf16,
+                         float* dWT, int B, int Ti, int Fi, int Ci, int Co, int kh, int kw,
+                         int stride, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Tail of the training step over flat fp32 buffers.

@@ -75,6 +75,11 @@ SIGNATURES = {
     "sb_conv_dtop": (_c_int, [_vp, _vp, _vp, _fl, _vp, _vp, _c_int, _c_int, _c_int, _c_int, _vp]),
     "sb_conv_col2im_relu": (_c_int, [_vp, _c_ll, _vp, _vp, _fl, _vp, _vp, _c_int, _c_int, _c_int,
                                      _c_int, _c_int, _c_int, _c_int, _vp]),
+    "sb_conv_direct_ok": (_c_int, [_c_int] * 6),
+    "sb_conv_fwd_direct": (_c_int, [_vp, _vp, _fl, _vp, _c_int, _vp, _vp] + [_c_int] * 8 + [_vp]),
+    "sb_conv_dgrad_direct": (_c_int, [_vp, _vp, _c_int, _vp, _vp, _fl, _vp, _vp] + [_c_int] * 8
+                             + [_vp]),
+    "sb_conv_wgrad_direct": (_c_int, [_vp, _vp, _fl, _vp, _vp] + [_c_int] * 8 + [_vp]),
     "sb_sumsq_workspace_size": (_c_int, [ctypes.POINTER(_c_sz)]),
     "sb_sumsq": (_c_int, [_vp, _c_ll, _vp, _vp, _vp]),
     "sb_sgd_clip_step": (_c_int, [_vp, _vp, _vp, _vp, _c_ll, _vp, _fl, _fl, _fl, _vp]),

@@ -73,9 +73,12 @@ def _apply_env_knobs():
     H = 1024; 256: that mode wherever the K-split backward kernel applies), SB_GEMM_FLAGS=<int>
     sets sb_debug_gemm_flags (bits: 1 = the 128 x 128 one-CTA GEMM kernel instead of the 128 x 256
     one over 2-CTA clusters; 2 = that kernel stores its output straight from the registers instead
-    of through shared memory and TMA; 4 = it stores no output at all, for timing only)."""
+    of through shared memory and TMA; 4 = it stores no output at all, for timing only),
+    SB_CONV_FLAGS=1 runs every conv layer on im2col + GEMM (no direct-convolution kernels)."""
     import os
+    global _conv_flags
     lib = _lib.load()
+    _conv_flags = int(os.environ.get("SB_CONV_FLAGS", "0"))
     if os.environ.get("SB_GRU_KSPLIT") is not None:
         lib.sb_debug_gru_ksplit(int(os.environ["SB_GRU_KSPLIT"]))
     if os.environ.get("SB_GRU_CLUSTER") is not None:
@@ -87,6 +90,14 @@ def _apply_env_knobs():
 
 
 _knobs_applied = False
+_conv_flags = 0
+
+
+def _ensure_knobs():
+    global _knobs_applied
+    if not _knobs_applied:
+        _knobs_applied = True
+        _apply_env_knobs()
 
 
 # ---- optional per-kernel timing (CUDA events on the launching stream; used by bench.py) ----
@@ -113,10 +124,7 @@ def profile_end():
 
 def _launch(name, flops, fn):
     """Run one C-ABI launch; counts it and, when profiling, brackets it with CUDA events."""
-    global _knobs_applied
-    if not _knobs_applied:
-        _knobs_applied = True
-        _apply_env_knobs()
+    _ensure_knobs()
     _lib.launch_count += 1
     if _prof is None:
         return _lib.check(fn(), name)
@@ -778,8 +786,24 @@ def gru_stack(x, rnn, dropout=0.0, lens=None):
         xc, ndir, rnn.hidden_size, float(dropout), None, None, lc, *weights))
 
 
+_direct_ok = {}
+
+
+def conv_direct_ok(Fi, Ci, Co, kh, kw, s):
+    """True when a conv layer past the first (input width Fi, Ci -> Co channels, kernel kh x kw,
+    stride s; channel counts as the kernels run them, multiples of 8) runs on the direct
+    convolution kernels: Co <= 32, and its resident weights and input footprint fit in shared
+    memory.  Every other layer runs on im2col + GEMM."""
+    key = (Fi, Ci, Co, kh, kw, s)
+    if key not in _direct_ok:
+        _direct_ok[key] = bool(_lib.load().sb_conv_direct_ok(*key))
+    return _direct_ok[key]
+
+
 class ConvStackFunction(torch.autograd.Function):
-    """Conv2d+ReLU stack as im2col + wgmma GEMM (csrc/conv.cu, csrc/gemm.cu).
+    """Conv2d+ReLU stack (csrc/conv.cu, csrc/gemm.cu): the first layer (one input channel) and any
+    layer outside conv_direct_ok as im2col + wgmma GEMM, the others as direct convolutions that
+    read their input activations straight from the previous layer's output (no patch matrix).
 
     forward(x (B,T,F) f32, specs ((kh,kw,s),...), w0, b0, w1, b1, ...) -> (B, T', C*F') f32 with
     the reference's channel-major feature order (model.py:66-71)."""
@@ -799,6 +823,7 @@ class ConvStackFunction(torch.autograd.Function):
         mscale = 1.0 / (1.0 - dropout) if dropout > 0.0 else 1.0
         need_grad = any(ctx.needs_input_grad)
         sp = _lib.stream_ptr()
+        _ensure_knobs()
         for l, (kh, kw, s_) in enumerate(specs):
             co_r, ci_r = params[2 * l].shape[:2]
             # zero filters up to the GEMM's multiple of 8 channels: a padded channel is
@@ -810,15 +835,26 @@ class ConvStackFunction(torch.autograd.Function):
             Kp = _round_up(K, 8)
             To, Fo = (Ti - kh) // s_ + 1, (Fi - kw) // s_ + 1
             M = B * To * Fo
-            A = torch.empty(M, Kp, dtype=torch.bfloat16, device=dev)
             src = cur
             mprev = masks[l - 1] if l > 0 else None
-            _launch("conv_im2col", 0.0,
-                    lambda: lib.sb_conv_im2col(src.data_ptr(), _lib.ptr(mprev), mscale, A.data_ptr(), B, Ti,
-                                               Fi, Ci, kh, kw, s_, Kp, 1 if l > 0 else 0, sp))
             Wp = torch.zeros(Co, Kp, dtype=torch.bfloat16, device=dev)
             Wp[:, :K] = w.detach().permute(0, 2, 3, 1).reshape(Co, K)
-            C = gemm_bf16_tn(A, Wp, bias=b.detach().float().contiguous())
+            bias = b.detach().float().contiguous()
+            if l > 0 and _conv_flags != 1 and conv_direct_ok(Fi, Ci, Co, kh, kw, s_):
+                A = None          # the backward re-reads the activations themselves
+                C = torch.empty(M, Co, dtype=torch.float32, device=dev)
+                _launch("conv_fwd_direct", 2.0 * M * Co * K,
+                        lambda: lib.sb_conv_fwd_direct(src.data_ptr(), _lib.ptr(mprev), mscale,
+                                                       Wp.data_ptr(), Kp, bias.data_ptr(),
+                                                       C.data_ptr(), B, Ti, Fi, Ci, Co, kh, kw,
+                                                       s_, sp))
+            else:
+                A = torch.empty(M, Kp, dtype=torch.bfloat16, device=dev)
+                _launch("conv_im2col", 0.0,
+                        lambda: lib.sb_conv_im2col(src.data_ptr(), _lib.ptr(mprev), mscale,
+                                                   A.data_ptr(), B, Ti, Fi, Ci, kh, kw, s_, Kp,
+                                                   1 if l > 0 else 0, sp))
+                C = gemm_bf16_tn(A, Wp, bias=bias)
             mask = None
             if dropout > 0.0:
                 mask = (torch.rand(M, Co, device=dev) >= dropout).to(torch.uint8)
@@ -868,11 +904,32 @@ class ConvStackFunction(torch.autograd.Function):
             # weight gradient: contraction over the M = B*To*Fo patch rows (split-K over all SMs)
             # dWp^T [Kp][Co] = A^T dC with both operands read token-major (MN-major UMMA)
             dWpT = torch.zeros(Kp, Co, dtype=torch.float32, device=dev)
-            gemm_bf16_tn(A, dC, out=dWpT, accumulate=True, a_mn=True, b_mn=True)
+            mprev = ctx.masks[l - 1] if l > 0 else None
+            if A is None:
+                dCw = dC
+                _launch("conv_wgrad_direct", 2.0 * M * Co * K,
+                        lambda: lib.sb_conv_wgrad_direct(Pprev.data_ptr(), _lib.ptr(mprev),
+                                                         ctx.mscale, dCw.data_ptr(),
+                                                         dWpT.data_ptr(), B, Ti, Fi, Ci, Co, kh,
+                                                         kw, s_, sp))
+            else:
+                gemm_bf16_tn(A, dC, out=dWpT, accumulate=True, a_mn=True, b_mn=True)
             dWp = dWpT.t()
             grads[2 * l] = dWp[:co_r, :K].reshape(co_r, kh, kw, Ci).permute(0, 3, 1, 2)[:, :ci_r] \
                 .contiguous()
-            if l > 0:
+            if l > 0 and A is None:
+                Mp = B * Ti * Fi
+                dCp = torch.empty(Mp, Ci, dtype=torch.bfloat16, device=dev)
+                db = torch.zeros(Ci, dtype=torch.float32, device=dev)
+                dCd = dC
+                _launch("conv_dgrad_direct", 2.0 * M * Co * K,
+                        lambda: lib.sb_conv_dgrad_direct(dCd.data_ptr(), Wp.data_ptr(), Kp,
+                                                         Pprev.data_ptr(), _lib.ptr(mprev),
+                                                         ctx.mscale, dCp.data_ptr(),
+                                                         db.data_ptr(), B, Ti, Fi, Ci, Co, kh,
+                                                         kw, s_, sp))
+                dC = dCp
+            elif l > 0:
                 dA = gemm_bf16_tn(dC, Wp, b_mn=True)            # [M][Kp] f32 patch gradient
                 Mp = B * Ti * Fi
                 dCp = torch.empty(Mp, Ci, dtype=torch.bfloat16, device=dev)
@@ -895,7 +952,8 @@ def conv_stack(x, conv, training):
 
     x (B, T, F) -> (B, T', C*F') with the reference's channel-major feature flattening
     (transpose(1,2) of (B,C,T',F') then view, model.py:66-71).  Runs on our im2col + wgmma
-    kernels, including the Dropout after each ReLU when training, for every stack the reference
+    kernels and, for the layers conv_direct_ok takes, on the direct-convolution kernels,
+    including the Dropout after each ReLU when training, for every stack the reference
     can express (model.py:21-23: square stride, no padding, dilation or groups, bias, one dropout
     rate); any other stack raises, there is no library fallback.  Any out_channels runs: a layer
     whose count is not a multiple of 8 gets zero filters up to the next multiple (exact: such a

@@ -256,3 +256,19 @@ for V, lm_s in ((28, lm_t), (20000, lm_tv)):
     st.push([inputs[0][:0], inputs[3][:30], inputs[2][:0]])
     print("transducer stream V+1=%d" % (V + 1), st.frames, st.partial(return_scores=True))
 torch.cuda.synchronize()
+# the direct-convolution kernels of the conv layers past the first (forward, data and weight
+# gradient): the benchmark's stack, a stride-3 layer and a stack with dropout
+from speech_b200 import ops
+for specs, B, T, F, p in (([[32, 5, 8, 2], [32, 5, 8, 2]], 2, 60, 80, 0.0),
+                          ([[16, 3, 4, 1], [8, 2, 3, 3]], 2, 33, 21, 0.0),
+                          ([[16, 5, 8, 2], [24, 3, 4, 1]], 2, 40, 40, 0.3)):
+    layers, in_c = [], 1
+    for out_c, kh, kw, st in specs:
+        layers += [torch.nn.Conv2d(in_c, out_c, (kh, kw), stride=(st, st)), torch.nn.ReLU(),
+                   torch.nn.Dropout(p)]
+        in_c = out_c
+    conv = torch.nn.Sequential(*layers).cuda()
+    ops.profile_begin()
+    y = ops.conv_stack(torch.randn(B, T, F, device="cuda"), conv, True)
+    y.sum().backward()
+    print("direct conv", specs, "dropout", p, sorted(n for n in ops.profile_end() if "direct" in n))
