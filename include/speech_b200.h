@@ -574,6 +574,56 @@ int sb_s2s_beam_select_split_lm_batch(const float* logp, void* state, double* c_
                                       size_t workspace_bytes, const SbNgramLm* lm,
                                       double lm_weight, double insertion_bonus, void* stream);
 
+/* Joint CTC/attention decoding of the attention model (Watanabe et al. 2017, Algorithm 2;
+ * csrc/s2s_ctc.cu): the batched beam search above with the CTC prefix scores of a CTC head.
+ * y (B, T, C) float32: the head's log-probabilities, C = the decoder's classes, blank C - 1, which
+ * is also end_tok; start_tok = C.  lambda = ctc_weight in (0, 1); M in [1, min(C, 128)] candidates
+ * per live row; lens (B) frames of each utterance (clamped to [1, T]) or null (all T).
+ * Per live row r the search keeps A_r (attention + LM part), psi_r = psi(h_r) and the CTC forward
+ * variables gn_t(h_r), gb_t(h_r), t < T_b; its score is S_r = A_r + lambda psi_r, used for
+ * selection, completion, the stop rule and the result.  The root has A = psi = 0, gn = -inf,
+ * gb_t = sum_{tau <= t} y_tau(blank).
+ *   P(r, c) = (1 - lambda) (double)logp[r][c] (+ (lm_weight lm(c | h_r) + beta_c) with an LM, as
+ *   in the LM entry points); row r's candidates are its M classes with the largest P (ties to the
+ *   lower class), in class order; value = (A_r + P) + lambda psi(h_r + c), in float64.
+ *   psi(h + END) = log(exp gn_{T_b-1}(h) + exp gb_{T_b-1}(h)); for a label c: gn_0(h + c) = y_0(c)
+ *   at the root, else -inf; gb_0 = -inf; psi = gn_0; for t = 1..T_b-1, Phi = gb_{t-1}(h) when c
+ *   is h's last label, else lse(gb_{t-1}(h), gn_{t-1}(h)); gn_t = lse(gn_{t-1}, Phi) + y_t(c);
+ *   gb_t = lse(gb_{t-1}, gn_{t-1}) + y_t(blank); psi = lse(psi, Phi + y_t(c)); lse(a, b) =
+ *   max + log1p(exp(min - max)), -inf when both are.
+ * Selection: the first min(2K, nl M) candidates by (value desc, (r, c) asc), and the bookkeeping
+ * of sb_s2s_beam_select_batch; a new live row gets A' = A_r + P and psi' = psi(h_r + c).
+ *   sb_s2s_ctc_state_size    bytes of the CTC buffer, R = B*K rows, carved in this order:
+ *                            A [R] double; the vectors [2][R][2][T] double (gn then gb of each
+ *                            row, buffer (step & 1) holding the rows entering step `step`); the
+ *                            rows' candidate lists [R][M] double values, [R][M] double A_r + P,
+ *                            [R][M] double psi(h_r + c), [R][M] int classes (ascending)
+ *   sb_s2s_ctc_init          after sb_s2s_beam_init_batch: every utterance's root
+ *   sb_s2s_ctc_candidates    per step after the attention step's logp: the rows' candidate lists;
+ *                            lm optional (null: lm_weight = insertion_bonus = 0), checked as in
+ *                            the LM entry points; a no-op once stop[1] is set
+ *   sb_s2s_ctc_select_batch  per step: selection, bookkeeping, the new rows' A (one CTA per
+ *                            utterance), then their vectors (one thread per new row); then
+ *                            sb_s2s_beam_gather_batch as usual
+ * SB_ERR_INVALID for a null pointer, K, T, B < 1, C < 2, M outside [1, C], lambda outside (0, 1),
+ * end_tok != C - 1 or start_tok != C; SB_ERR_UNSUPPORTED for K > 32, M > 128, B > 65535, or
+ * (candidates) C > 20480; SB_ERR_WORKSPACE for a CTC buffer below sb_s2s_ctc_state_size. */
+int sb_s2s_ctc_state_size(int K, int M, int T, int B, size_t* bytes);
+int sb_s2s_ctc_init(const float* ctc_logp, const int* lens, void* ctc_state,
+                    size_t ctc_state_bytes, int K, int C, int M, int T, int start_tok, int end_tok,
+                    double ctc_weight, int B, void* stream);
+int sb_s2s_ctc_candidates(const float* logp, const float* ctc_logp, const int* lens,
+                          const void* state, const int* nodes, int node_cap, void* ctc_state,
+                          size_t ctc_state_bytes, int K, int C, int M, int T, int start_tok,
+                          int end_tok, double ctc_weight, int step, const int* stop, int B,
+                          const SbNgramLm* lm, double lm_weight, double insertion_bonus,
+                          void* stream);
+int sb_s2s_ctc_select_batch(const float* ctc_logp, const int* lens, void* ctc_state,
+                            size_t ctc_state_bytes, void* state, double* c_scores, int* nodes,
+                            int* parent_row, int* tok_next, int* out_tokens, int K, int C, int M,
+                            int T, int start_tok, int end_tok, double ctc_weight, int step,
+                            int max_len, int node_cap, int c_cap, int* stop, int B, void* stream);
+
 /* ---------------------------------------------------------------------------------------
  * RNN-Transducer loss + gradient w.r.t. the log-probabilities.
  * Replaces: transducer.functions.transducer.TransducerLoss()(log_probs, labels, x_lens, y_lens)

@@ -464,7 +464,7 @@ def beam_search(m, eh, start_tok, end_tok, beam_size, max_len):
 
 
 def beam_search_batch(m, eh, start_tok, end_tok, beam_size, max_len, lens=None, lm=None,
-                      lm_weight=0.0, insertion_bonus=0.0):
+                      lm_weight=0.0, insertion_bonus=0.0, ctc=None):
     """Seq2Seq.beam_search (seq2seq.py:180-227) for each of the B utterances of eh (B, T, H) at
     once, device-resident.  Utterance b's K beam entries are rows b*K .. b*K+K-1 of the step
     kernels, which run over all B*K rows until every utterance has stopped; expand / prune /
@@ -474,8 +474,13 @@ def beam_search_batch(m, eh, start_tok, end_tok, beam_size, max_len, lens=None, 
     lens (optional): frames each utterance attends over.  lm (optional): an NGramLM whose classes
     are the vocabulary, blank the start token and end the end token (the caller checks), fused
     into every candidate as logp + (lm_weight * lm + insertion_bonus, no bonus for the end token);
-    the scores are then the fused ones.  -> list of B (token tuple, float64 score of that
-    hypothesis, steps that utterance's search ran)."""
+    the scores are then the fused ones.  ctc (optional): (y, ctc_weight, prebeam), joint
+    CTC/attention decoding (csrc/s2s_ctc.cu) with y the float32 CTC log-probabilities (B, T, C),
+    blank C - 1 = end_tok, start_tok = C: candidate c of row r is one of the row's `prebeam`
+    classes with the largest P = (1 - ctc_weight) logp[c] (+ the LM part), valued
+    (A_r + P) + ctc_weight * psi(h_r + c), psi the CTC prefix log-probability; the scores are then
+    A + ctc_weight * psi.  -> list of B (token tuple, float64 score of that hypothesis, steps that
+    utterance's search ran)."""
     lib = _lib.load()
     w = DecoderWeights(m)
     ehc = _f(eh)
@@ -484,6 +489,7 @@ def beam_search_batch(m, eh, start_tok, end_tok, beam_size, max_len, lens=None, 
     R = B * K
     dev = ehc.device
     ld = attn_lens(lens, B, T, dev)
+    ctc_ld = ld
     if ld is not None:
         ld = ld.repeat_interleave(K)
     S = _lib.workspace_size(lib.sb_s2s_beam_state_size)
@@ -509,16 +515,29 @@ def beam_search_batch(m, eh, start_tok, end_tok, beam_size, max_len, lens=None, 
                                           sp), "beam init")
     done_ptr = stop.data_ptr() + 4              # the no-op flag of the step kernels
     fc_ws = None if w.fused else fc_workspace(lib, R, C, dev)
-    split = not beam_select_fits(K, C)
+    split = ctc is None and not beam_select_fits(K, C)
     if split:
         sel_ws = torch.empty(_lib.workspace_size(lib.sb_s2s_beam_split_workspace_size_batch, K, C,
                                                  B), dtype=torch.uint8, device=dev)
     p_state, p_c, p_nodes = state.data_ptr(), c_scores.data_ptr(), nodes.data_ptr()
     p_par, p_tok, p_out = parent.data_ptr(), tok.data_ptr(), out_tokens.data_ptr()
     p_stop = stop.data_ptr()
+    fusion = (None, 0.0, 0.0)
     if lm is not None:
         tables, _ = lm.device_tables(dev)
         fusion = (tables, float(lm_weight), float(insertion_bonus))
+    if ctc is not None:
+        y, lam, M = ctc
+        if tuple(y.shape) != (B, T, C) or y.dtype != torch.float32 or y.device != ehc.device:
+            raise ValueError("ctc log-probabilities must be float32 (%d, %d, %d) on the encoder's "
+                             "device, got %s %s" % (B, T, C, y.dtype, tuple(y.shape)))
+        y = y.contiguous()
+        lam, M = float(lam), int(M)
+        cbuf = torch.empty(_lib.workspace_size(lib.sb_s2s_ctc_state_size, K, M, T, B),
+                           dtype=torch.uint8, device=dev)
+        cargs = (y.data_ptr(), _a(ctc_ld), cbuf.data_ptr(), cbuf.numel())
+        shape = (K, C, M, T, int(start_tok), int(end_tok), lam)
+        _lib.check(lib.sb_s2s_ctc_init(*cargs, *shape, B, sp), "ctc init")
     # buffers: [0] = state entering the step (gathered), [1] = state produced by the step
     for e in range(max_len):
         _cell_fwd(lib, w, p_tok, 1, sx[0] if e > 0 else None, hx[0], hx[1], None, None, done_ptr,
@@ -531,7 +550,14 @@ def beam_search_batch(m, eh, start_tok, end_tok, beam_size, max_len, lens=None, 
                       done=done_ptr, with_fc=False, lens=ld)
             _fc_rows(lib, w, fc_ws, hx[1], sx[1], R, sp, logits=logp, done=done_ptr)
             _fc_logp(lib, w, fc_ws, logp, logp, R, sp, done=done_ptr)
-        if lm is not None and split:
+        if ctc is not None:
+            ops._launch("s2s_ctc_candidates", 0.0, lambda: lib.sb_s2s_ctc_candidates(
+                logp.data_ptr(), cargs[0], cargs[1], p_state, p_nodes, node_cap, cargs[2],
+                cargs[3], *shape, e, p_stop, B, *fusion, sp))
+            ops._launch("s2s_ctc_select", 0.0, lambda: lib.sb_s2s_ctc_select_batch(
+                *cargs, p_state, p_c, p_nodes, p_par, p_tok, p_out, *shape, e, max_len, node_cap,
+                c_cap, p_stop, B, sp))
+        elif lm is not None and split:
             ops._launch("s2s_beam_select_split_lm", 0.0,
                         lambda: lib.sb_s2s_beam_select_split_lm_batch(
                             logp.data_ptr(), p_state, p_c, p_nodes, p_par, p_tok, p_out, K, C,

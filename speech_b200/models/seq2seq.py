@@ -22,6 +22,11 @@ from . import model
 
 class Seq2Seq(model.Model):
 
+    # Hybrid CTC/attention (config["decoder"]["ctc_weight"], default 0): a CTC head `ctc_fc` on
+    # the encoder, trained jointly and used by recognize(ctc_weight=...).  A class attribute, so
+    # that pickles written before the key existed read it as 0 (no head).
+    ctc_weight = 0.0
+
     def __init__(self, freq_dim, vocab_size, config):
         super().__init__(freq_dim, config)
         dec = config["decoder"]
@@ -33,6 +38,14 @@ class Seq2Seq(model.Model):
         self.scheduled_sampling = (self.sample_prob != 0)
         # the start-of-sequence token is never predicted: vocab_size - 1 classes (:32-34)
         self.fc = model.LinearND(rnn_dim, vocab_size - 1)
+        w = dec.get("ctc_weight", 0)
+        if isinstance(w, bool) or not isinstance(w, (int, float)) or not 0.0 <= w < 1.0:
+            raise ValueError("decoder ctc_weight must be a number in [0, 1), got %r" % (w,))
+        if w > 0:
+            # created after every reference module, so that they keep their initial values under
+            # a seed; classes 0..V-3 are the labels, V-2 the blank (END and START never occur)
+            self.ctc_weight = float(w)
+            self.ctc_fc = model.LinearND(rnn_dim, vocab_size - 1)
 
     def set_eval(self):
         self.eval()
@@ -58,6 +71,8 @@ class Seq2Seq(model.Model):
         return [max(0, self.conv_out_size(i.shape[0], 0)) for i in inputs]
 
     def loss(self, batch):
+        if self.ctc_weight > 0:
+            return self._joint_loss(batch)
         lens = self.input_lens(batch[0])
         x, y = self.collate(*batch)
         x, y = self._to_dev(x, y)
@@ -68,6 +83,43 @@ class Seq2Seq(model.Model):
                                              reduction="sum")
             # (1,)-shaped so that train.py:33 `loss.data[0]` works on current torch
             return (ce / bsz).reshape(1)
+
+    def _ctc_targets(self, labels):
+        """flat int32 CTC targets (each transcript without its START and END) and their lengths;
+        ValueError unless every transcript is [START, labels in 0..V-3, END]"""
+        V = self.embedding.num_embeddings
+        flat, lengths = [], []
+        for seq in labels:
+            seq = [int(t) for t in seq]
+            if len(seq) < 2 or seq[0] != V - 1 or seq[-1] != V - 2 or \
+                    any(not 0 <= t < V - 2 for t in seq[1:-1]):
+                raise ValueError("with a CTC head every transcript must be [START (%d), labels in "
+                                 "0..%d, END (%d)], got %r" % (V - 1, V - 3, V - 2, seq))
+            flat += seq[1:-1]
+            lengths.append(len(seq) - 2)
+        return torch.tensor(flat, dtype=torch.int32), torch.tensor(lengths, dtype=torch.int32)
+
+    def _joint_loss(self, batch):
+        """((1 - w) CE_sum + w CTC_sum) / B, w = ctc_weight: the encoder states feed both the
+        attention decoder and the CTC head (functions.ctc.CTCLoss, a sum, blank V-2), over the
+        padded T' frames or each utterance's own conv_out_size(T_b) in the exact-lengths mode"""
+        from ..functions import ctc
+        targets, target_lens = self._ctc_targets(batch[1])
+        lens = self.input_lens(batch[0])
+        x, y = self.collate(*batch)
+        x, y = self._to_dev(x, y)
+        with self._grad_ctx():
+            enc = self._encode(x, lens)
+            out, _ = self.decode(enc, y) if lens is None else self.decode(enc, y, lens)
+            bsz, _, out_dim = out.shape
+            ce = nn.functional.cross_entropy(out.reshape(-1, out_dim), y[:, 1:].reshape(-1),
+                                             reduction="sum")
+            logits = self.ctc_fc(enc)
+            frames = lens if lens is not None else [logits.shape[1]] * bsz
+            ctc_sum = ctc.CTCLoss()(logits, targets, torch.tensor(frames, dtype=torch.int32),
+                                    target_lens)
+            w = self.ctc_weight
+            return (((1.0 - w) * ce + w * ctc_sum.reshape(())) / bsz).reshape(1)
 
     def forward_impl(self, x, y, lens=None):
         x = self._encode(x, lens)
@@ -140,7 +192,8 @@ class Seq2Seq(model.Model):
             return [s2s.beam_search(self, x, start_tok, end_tok, beam_size, max_len)]
 
     def recognize(self, inputs, beam_size=10, max_len=200, start_tok=None, end_tok=None,
-                  return_scores=False, lm=None, lm_weight=0.0, insertion_bonus=0.0):
+                  return_scores=False, lm=None, lm_weight=0.0, insertion_bonus=0.0,
+                  ctc_weight=0.0, ctc_prebeam=None):
         """Beam search of every utterance of a batch at once, from the audio alone.  inputs: the
         (T_i, F) arrays of batch[0].  Each utterance gets `beam_search`'s search on its own (float64
         scores, stable-descending tie order, the same completion and stop rules), bit for bit, and
@@ -156,7 +209,16 @@ class Seq2Seq(model.Model):
         Candidate c of a hypothesis h then scores logp(c) + (lm_weight * lm(c | h) +
         insertion_bonus), where lm(end_tok | h) is lm(</s> | h) and the end token earns no bonus;
         the context of h starts at <s>, its start token.  The returned scores are the fused ones.
-        With lm=None (the default) this is the LM-less search."""
+        With lm=None (the default) this is the LM-less search.
+
+        Joint CTC/attention decoding (Watanabe et al. 2017, Algorithm 2): ctc_weight = w in
+        (0, 1) needs the CTC head (config["decoder"]["ctc_weight"] > 0) and the default START /
+        END.  Each live hypothesis h extends only by the ctc_prebeam classes c (default
+        min(V-1, 3 * beam_size // 2), at most 128) with the largest P = (1 - w) logp(c) (+ the LM
+        part above), and scores A_h + P + w * psi(h + c), psi the CTC prefix log-probability of
+        h + c over the head's log-softmax (the full CTC probability of h for END), A the attention
+        and LM part.  The returned scores are then A + w * psi.  With ctc_weight = 0 (the default)
+        this is the search above, untouched."""
         from ..functions import s2s
         V = self.embedding.num_embeddings
         start_tok = V - 1 if start_tok is None else int(start_tok)
@@ -173,14 +235,37 @@ class Seq2Seq(model.Model):
         if len(inputs) == 0:
             raise ValueError("recognize needs at least one utterance")
         self._check_lm(lm, lm_weight, insertion_bonus, V, start_tok, end_tok)
+        M = self._check_ctc(ctc_weight, ctc_prebeam, int(beam_size), V, start_tok, end_tok)
         lens = self.input_lens(inputs)
         x = self.stage_inputs(inputs)
         with torch.no_grad():
             x = self._encode(x, lens)
+            ctc = None
+            if ctc_weight > 0:
+                y = torch.log_softmax(self.ctc_fc(x).float(), dim=-1).contiguous()
+                ctc = (y, float(ctc_weight), M)
             res = s2s.beam_search_batch(self, x, start_tok, end_tok, int(beam_size), int(max_len),
-                                        lens, lm, lm_weight, insertion_bonus)
+                                        lens, lm, lm_weight, insertion_bonus, ctc)
         labels = [list(r[0]) for r in res]
         return (labels, [r[1] for r in res]) if return_scores else labels
+
+    def _check_ctc(self, ctc_weight, ctc_prebeam, beam_size, V, start_tok, end_tok):
+        """ValueError unless the joint-decoding arguments of recognize are usable; -> the
+        pre-beam width M"""
+        C = V - 1
+        if isinstance(ctc_weight, bool) or not isinstance(ctc_weight, (int, float)) or \
+                not 0.0 <= ctc_weight < 1.0:
+            raise ValueError("ctc_weight must be a number in [0, 1), got %r" % (ctc_weight,))
+        M = min(C, (3 * beam_size) // 2) if ctc_prebeam is None else ctc_prebeam
+        if isinstance(M, bool) or int(M) != M or not 1 <= M <= min(C, 128):
+            raise ValueError("ctc_prebeam must lie in [1, %d], got %r" % (min(C, 128), M))
+        if ctc_weight > 0:
+            if self.ctc_weight <= 0:
+                raise ValueError("ctc_weight > 0 needs a CTC head (config decoder ctc_weight > 0)")
+            if start_tok != V - 1 or end_tok != V - 2:
+                raise ValueError("joint CTC decoding needs START = %d and END = %d, got %d / %d"
+                                 % (V - 1, V - 2, start_tok, end_tok))
+        return int(M)
 
     @staticmethod
     def _check_lm(lm, lm_weight, insertion_bonus, V, start_tok, end_tok):

@@ -36,6 +36,12 @@ s2s_fn.beam_select_fits = lambda K, C: False     # the split selection with the 
 print("seq2seq recognize with LM, split select", [len(h) for h in s.recognize(
     inputs, beam_size=3, max_len=8, lm=lm2, lm_weight=0.5, insertion_bonus=1.0)])
 s2s_fn.beam_select_fits = fits
+sc = Seq2Seq(80, 30, dict(cfg, decoder={"embedding_dim": 256, "layers": 1, "ctc_weight": 0.3})).cuda()
+lc = sc.loss((inputs, lab2)); lc.backward()
+print("seq2seq joint CTC loss", lc.item(), "recognize", [len(h) for h in sc.recognize(
+    inputs, beam_size=3, max_len=8, ctc_weight=0.3)], "with LM", [len(h) for h in sc.recognize(
+    inputs, beam_size=3, max_len=8, lm=lm2, lm_weight=0.5, insertion_bonus=1.0, ctc_weight=0.5,
+    ctc_prebeam=29)])
 t = Transducer(80, 28, cfg).cuda()
 l3 = t.loss((inputs, labels)); l3.backward()
 print("transducer ok", l3.item())
