@@ -347,9 +347,94 @@ int sb_ctc_stream_step_lm_shortlist(const float* logp, const int* n, int B, int 
                                     void* stream);
 int sb_ctc_stream_best(const void* state, int B, int max_frames, int beam_size, int* out_labels,
                        int* out_lens, double* out_scores, int* out_overflow, void* stream);
-/* Developer counter: frames the LM-fused shortlist search rescanned in full, over every call
- * since the last query (synchronous: waits for the device); resets it. */
+/* Developer counter: frames the LM-fused shortlist search (character or word LM) rescanned in
+ * full, over every call since the last query (synchronous: waits for the device); resets it. */
 int sb_debug_ctc_lm_rescans(unsigned long long* frames);
+
+/* ---------------------------------------------------------------------------------------
+ * CTC prefix beam search with a word n-gram LM (Hannun et al. 2014, arXiv:1408.2873): the LM
+ * scores a word when the delimiter class that ends it (the space of a character model) is
+ * emitted, and a lexicon tracks the partial word.
+ * A prefix splits at every delimiter into completed words w_1..w_n and a partial word (the
+ * classes after the last delimiter).  Each beam entry carries its lexicon node (0 = the root,
+ * the empty partial word; -1 = the partial word has left the lexicon) and its last order-1
+ * completed words' tokens (most recent first, <s> before the first).  Extending entry i by class
+ * s != blank replaces p_s by q in every term of that extension, as the character LM does:
+ *   s the delimiter, partial word empty:      q = p_s (leading and repeated delimiters are free);
+ *   s the delimiter, partial word non-empty:  q = p_s + ((lm_weight * lm(w | ctx_i) +
+ *       insertion_bonus) + g_i) in float64, in that order.  w is the word at i's node, or <unk>
+ *       where the node is not a word or is -1; g_i = oov_penalty where the node is >= 1 and not a
+ *       word (an OOV word not charged yet), else 0.  The new entry's history is (w, older..) and
+ *       its node the root;
+ *   s any other class:  q = p_s + oov_penalty where i's node is >= 0 and has no child s (the new
+ *       node is -1: the word leaves the lexicon); otherwise q = p_s and the node becomes that
+ *       child, or stays -1.
+ * Blank terms and the repeated symbol that keeps the prefix use p_s.  lm(w | ctx) is the backoff
+ * lookup of the word n-gram, as sb_ctc_prefix_beam_lm's over tokens.
+ * End of utterance: each final entry scores final_i = lse(p_b, p_nb) + (e_i + lm_weight *
+ * lm(</s> | ctx'_i)), e_i the delimiter term above (0 for an empty partial word) and ctx'_i the
+ * history with the trailing word, if there is one.  The result is the entry with the largest
+ * final_i (ties: the lowest beam index) and its score -final_i: acoustic + lm_weight * (word LM
+ * with </s>) + insertion_bonus * words + oov_penalty * OOV words.
+ * oov_penalty <= 0: 0 is an open-vocabulary search scoring OOV words as <unk>, -inf a closed
+ * vocabulary.  With lm_weight = insertion_bonus = oov_penalty = 0 the results equal
+ * sb_ctc_prefix_beam's bit for bit.
+ * Shortlist route: each entry also scores the delimiter on every frame (as it scores its last
+ * symbol), and every other class has q <= p_s, so the LM-less bound check applies unchanged.
+ * Tables (built by speech_b200.lm.WordLM): the word n-gram in SbNgramLm's layout over tokens
+ * w -> w (0..W-1), <s> W, </s> W + 1, <unk> W + 2, with tok the identity over those W + 3 tokens
+ * and blank -1; the lexicon as a second map of the same hash and key layout,
+ *   (node << 32) | ((class + 1) << 1) | 0  -> child node,
+ * and lex_word[node], the word token ending at each node (-1 for none).
+ * ------------------------------------------------------------------------------------- */
+typedef struct SbWordLm {
+  SbNgramLm ngram;                 /* the word n-gram (orders 1 .. SB_LM_MAX_ORDER) */
+  const unsigned long long* lex_keys;  /* [lex_cap] lexicon map keys, 0 = empty (device) */
+  const int* lex_vals;             /* [lex_cap] child node (device) */
+  const int* lex_word;             /* [lexicon nodes] word token of each node or -1 (device) */
+  int lex_cap;                     /* power of two, at least twice the number of lexicon edges */
+  int num_words;                   /* W >= 1 */
+  int has_unk;                     /* the n-gram has a <unk> unigram; else oov_penalty = -inf */
+  int num_classes;                 /* classes the lexicon is spelled in; must be >= S */
+  int blank;                       /* must equal the search's */
+  int delimiter;                   /* the class that ends a word; in [0, S), not the blank */
+} SbWordLm;
+
+/*   sb_ctc_prefix_beam_wordlm            sb_ctc_prefix_beam's arguments, route choice and
+ *                                        workspace, plus the LM and its three weights
+ *   sb_ctc_prefix_beam_wordlm_shortlist  the shortlist search at any shape (same arguments)
+ *   sb_ctc_stream_step_wordlm[_shortlist]  sb_ctc_stream_step's arguments plus the LM and weights;
+ *       the state is sized with the LM's order and must be stepped with this LM from its reset on
+ *   sb_ctc_stream_best_wordlm            sb_ctc_stream_best with the end-of-utterance rule applied
+ *                                        to each stored beam (the same LM and weights)
+ * SB_ERR_INVALID for a null table, lm_weight < 0 or not finite, insertion_bonus not finite,
+ * oov_penalty > 0 or NaN, oov_penalty != -inf without <unk>, lm->num_classes < S, lm->blank !=
+ * blank, a delimiter outside [0, S) or equal to the blank, or order < 1;
+ * SB_ERR_UNSUPPORTED for order > SB_LM_MAX_ORDER or beam_size > 32.  All before any CUDA call. */
+int sb_ctc_prefix_beam_wordlm(const float* logp, const int* lens, int B, int T, int S,
+                              int beam_size, int blank, const SbWordLm* lm, double lm_weight,
+                              double insertion_bonus, double oov_penalty, int* out_labels,
+                              int* out_lens, double* out_scores, void* workspace,
+                              size_t workspace_bytes, void* stream);
+int sb_ctc_prefix_beam_wordlm_shortlist(const float* logp, const int* lens, int B, int T, int S,
+                                        int beam_size, int blank, const SbWordLm* lm,
+                                        double lm_weight, double insertion_bonus,
+                                        double oov_penalty, int* out_labels, int* out_lens,
+                                        double* out_scores, void* workspace,
+                                        size_t workspace_bytes, void* stream);
+int sb_ctc_stream_step_wordlm(const float* logp, const int* n, int B, int T, int S, int beam_size,
+                              int blank, const SbWordLm* lm, double lm_weight,
+                              double insertion_bonus, double oov_penalty, int max_frames,
+                              void* state, void* workspace, size_t workspace_bytes, void* stream);
+int sb_ctc_stream_step_wordlm_shortlist(const float* logp, const int* n, int B, int T, int S,
+                                        int beam_size, int blank, const SbWordLm* lm,
+                                        double lm_weight, double insertion_bonus,
+                                        double oov_penalty, int max_frames, void* state,
+                                        void* workspace, size_t workspace_bytes, void* stream);
+int sb_ctc_stream_best_wordlm(const void* state, int B, int max_frames, int beam_size,
+                              const SbWordLm* lm, double lm_weight, double insertion_bonus,
+                              double oov_penalty, int* out_labels, int* out_lens,
+                              double* out_scores, int* out_overflow, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Conv2d(+ReLU) front-end as im2col + sb_gemm_bf16_tn.

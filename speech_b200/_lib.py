@@ -24,7 +24,15 @@ class SbNgramLm(ctypes.Structure):
                 ("lm_upper", ctypes.c_double), ("lm_abs", ctypes.c_double)]
 
 
+class SbWordLm(ctypes.Structure):
+    """struct SbWordLm of include/speech_b200.h: device tables of a word n-gram LM and lexicon"""
+    _fields_ = [("ngram", SbNgramLm), ("lex_keys", _vp), ("lex_vals", _vp), ("lex_word", _vp),
+                ("lex_cap", _c_int), ("num_words", _c_int), ("has_unk", _c_int),
+                ("num_classes", _c_int), ("blank", _c_int), ("delimiter", _c_int)]
+
+
 _lmp = ctypes.POINTER(SbNgramLm)
+_wlmp = ctypes.POINTER(SbWordLm)
 _db = ctypes.c_double
 
 # name -> (restype, argtypes): every symbol include/speech_b200.h declares
@@ -69,6 +77,18 @@ SIGNATURES = {
     "sb_ctc_stream_step_lm_shortlist": (_c_int, [_vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int,
                                                  _lmp, _db, _db, _c_int, _vp, _vp, _c_sz, _vp]),
     "sb_ctc_stream_best": (_c_int, [_vp, _c_int, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp]),
+    "sb_ctc_prefix_beam_wordlm": (_c_int, [_vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int,
+                                           _wlmp, _db, _db, _db, _vp, _vp, _vp, _vp, _c_sz, _vp]),
+    "sb_ctc_prefix_beam_wordlm_shortlist": (_c_int, [_vp, _vp, _c_int, _c_int, _c_int, _c_int,
+                                                     _c_int, _wlmp, _db, _db, _db, _vp, _vp, _vp,
+                                                     _vp, _c_sz, _vp]),
+    "sb_ctc_stream_step_wordlm": (_c_int, [_vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int,
+                                           _wlmp, _db, _db, _db, _c_int, _vp, _vp, _c_sz, _vp]),
+    "sb_ctc_stream_step_wordlm_shortlist": (_c_int, [_vp, _vp, _c_int, _c_int, _c_int, _c_int,
+                                                     _c_int, _wlmp, _db, _db, _db, _c_int, _vp,
+                                                     _vp, _c_sz, _vp]),
+    "sb_ctc_stream_best_wordlm": (_c_int, [_vp, _c_int, _c_int, _c_int, _wlmp, _db, _db, _db,
+                                           _vp, _vp, _vp, _vp, _vp]),
     "sb_conv_im2col": (_c_int, [_vp, _vp, _fl, _vp, _c_int, _c_int, _c_int, _c_int, _c_int, _c_int,
                                 _c_int, _c_int, _c_int, _vp]),
     "sb_conv_relu_to_bct": (_c_int, [_vp, _vp, _fl, _vp, _c_int, _c_int, _c_int, _c_int, _vp]),

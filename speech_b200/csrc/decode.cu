@@ -65,12 +65,16 @@ struct Beam {
 // of beam entry i by symbol s scores with, from the acoustic log-probability p = p_s:
 //   NoFuse  q = p (the LM-less search, its arithmetic untouched);
 //   LmFuse  q = p + (alpha * lm(s | ctx_i) + beta), lm the backoff lookup of SbNgramLm.
-// Entry i's context is its last order-1 symbols, kept most recent first in LmShared::hist (-1
-// stands for <s>, before which there is nothing).  Once per frame each entry walks the context
-// trie along them (lm_resolve); a candidate's lookup is then at most `order` probes.
+//   WordLmFuse  the word LM of SbWordLm (include/speech_b200.h): the LM term only on the
+//           delimiter that ends a non-empty word, an OOV penalty where a word leaves the lexicon.
+// Entry i's context is its last order-1 symbols (LmFuse) or completed words (WordLmFuse), kept
+// most recent first in LmShared::hist (-1 stands for <s>, before which there is nothing).  Once per
+// frame each entry walks the context trie along them (lm_resolve); a candidate's lookup is then at
+// most `order` probes.
 // ------------------------------------------------------------------------------------------------
 struct NoFuse {
   static constexpr bool kLm = false;
+  static constexpr bool kWord = false;
   static constexpr int kMinBlocks = 0;
   __device__ __forceinline__ double q(int, int, double p) const { return p; }
 };
@@ -87,6 +91,7 @@ __device__ __forceinline__ LmShared& lm_shared() {
 
 struct LmFuse {
   static constexpr bool kLm = true;
+  static constexpr bool kWord = false;
   static constexpr int kMinBlocks = 1;
   SbNgramLm lm;
   double alpha, beta;
@@ -108,6 +113,81 @@ __device__ __forceinline__ void lm_resolve(const LmFuse& fu, int par, int nb) {
   const int i = threadIdx.x;
   if (i >= nb) return;
   sh.depth[i] = lm_context(fu.lm, [&](int k) { return sh.hist[par][i][k]; }, sh.ctx[i]);
+}
+
+// The word LM.  Per entry, besides its history of word tokens in LmShared::hist: its lexicon node
+// per beam buffer (WordShared::lex, 0 = the empty partial word, -1 = off the lexicon), and, for the
+// current frame, that node and the delimiter term d_i = (alpha * lm(w | ctx_i) + beta) + g_i
+// (word_resolve, thread i once per frame).  An extension by the delimiter then costs nothing more
+// and any other extension one lexicon probe.  kLm is false: the shortlist route keeps the LM-less
+// bound (see the comment above the shortlist body).
+struct WordShared {
+  int lex[2][DEC_MAX_BEAM];      // per beam buffer (t & 1) and entry
+  int node[DEC_MAX_BEAM];        // the current beam's nodes
+  double dterm[DEC_MAX_BEAM];    // the current beam's delimiter terms (entries with node != 0)
+  double fin[DEC_MAX_BEAM];      // end of utterance: final_i
+};
+__device__ __forceinline__ WordShared& word_shared() {
+  __shared__ WordShared sh;
+  return sh;
+}
+
+struct WordLmFuse {
+  static constexpr bool kLm = false;
+  static constexpr bool kWord = true;
+  static constexpr int kMinBlocks = 1;
+  SbWordLm lm;
+  double alpha, beta, gamma;
+
+  // the lexicon child of node (>= 0) by class s, -1 where there is none
+  __device__ __forceinline__ int child(int node, int s) const {
+    return map_find(LexMap{lm.lex_keys, lm.lex_vals, lm.lex_cap}, node, s, 0);
+  }
+  // the token of the word a delimiter ends at node (!= 0): the node's word or <unk>
+  __device__ __forceinline__ int word_tok(int node) const {
+    const int w = node > 0 ? __ldg(lm.lex_word + node) : -1;
+    return w >= 0 ? w : lm.ngram.bos + 2;
+  }
+  // the delimiter term of node (!= 0) against a history read by older (lm_context); ctx scratch
+  template <class Older>
+  __device__ __forceinline__ double dterm(int node, Older&& older, int* ctx) const {
+    const int w = node > 0 ? __ldg(lm.lex_word + node) : -1;
+    const double g = (node > 0 && w < 0) ? gamma : 0.0;   // an OOV word not charged yet
+    const int d = lm_context(lm.ngram, older, ctx);
+    return (alpha * lm_backoff(lm.ngram, ctx, d, w >= 0 ? w : lm.ngram.bos + 2) + beta) + g;
+  }
+  // e_i + alpha * lm(</s> | ctx'_i) of an entry at node with the history older
+  template <class Older>
+  __device__ __forceinline__ double end_term(int node, Older&& older, int* ctx) const {
+    const int eos = lm.ngram.bos + 1;
+    if (node == 0) {
+      const int d = lm_context(lm.ngram, older, ctx);
+      return 0.0 + alpha * lm_backoff(lm.ngram, ctx, d, eos);
+    }
+    const double e = dterm(node, older, ctx);
+    const int w = word_tok(node);
+    const int d = lm_context(lm.ngram, [&](int k) { return k == 0 ? w : older(k - 1); }, ctx);
+    return e + alpha * lm_backoff(lm.ngram, ctx, d, eos);
+  }
+  __device__ __forceinline__ double q(int i, int s, double p) const {
+    const WordShared& ws = word_shared();
+    const int node = ws.node[i];
+    if (s == lm.delimiter) return node == 0 ? p : p + ws.dterm[i];
+    if (node >= 0 && child(node, s) < 0) return p + gamma;
+    return p;
+  }
+};
+
+// entry i of the beam in buffer par: its node and delimiter term, thread i for i < nb; the caller
+// syncs
+__device__ __forceinline__ void word_resolve(const WordLmFuse& fu, int par, int nb) {
+  LmShared& sh = lm_shared();
+  WordShared& ws = word_shared();
+  const int i = threadIdx.x;
+  if (i >= nb) return;
+  const int node = ws.lex[par][i];
+  ws.node[i] = node;
+  if (node != 0) ws.dterm[i] = fu.dterm(node, [&](int k) { return sh.hist[par][i][k]; }, sh.ctx[i]);
 }
 
 // value of the candidate "beam entry j keeps its prefix" at this frame
@@ -218,7 +298,8 @@ template <class Fuse>
 __device__ __forceinline__ void dec_begin(const DecParams& p, Beam* beams) {
   if (threadIdx.x == 0) {
     dec_empty(beams[0]);
-    if constexpr (Fuse::kLm) lm_shared().hist[0][0][0] = -1;   // the empty prefix: <s>
+    if constexpr (Fuse::kLm || Fuse::kWord) lm_shared().hist[0][0][0] = -1;   // <s>
+    if constexpr (Fuse::kWord) word_shared().lex[0][0] = 0;
   }
   p.trie.of(blockIdx.x).clear<DEC_THREADS>();
 }
@@ -230,11 +311,17 @@ __device__ __forceinline__ void dec_frame(const Fuse& fu, const Beam& cur, int t
     lm_resolve(fu, t & 1, cur.size);
     __syncthreads();
   }
+  if constexpr (Fuse::kWord) {
+    word_resolve(fu, t & 1, cur.size);
+    __syncthreads();
+  }
 }
 
 // Materialise the pruned beam of frame t: thread r < ns holds the r-th selected candidate in `mine`
 // (full-scan numbering).  With an LM, an extension's context is its parent's shifted by one symbol
-// and an entry that stays copies its own.
+// and an entry that stays copies its own.  With a word LM, an extension by the delimiter shifts
+// the word it ends into the history (none for an empty word) and goes to the root; any other
+// extension moves the node to its child by s (-1 where there is none) and keeps the history.
 template <class Fuse>
 __device__ __forceinline__ void dec_commit(const DecParams& p, const Beam& cur, Beam& nxt, int mine,
                                            int ns, const float* lp, int t, const Fuse& fu) {
@@ -256,6 +343,18 @@ __device__ __forceinline__ void dec_commit(const DecParams& p, const Beam& cur, 
         for (int k = fu.lm.order - 2; k > 0; --k) sh.hist[par ^ 1][tid][k] = sh.hist[par][i][k - 1];
         if (fu.lm.order > 1) sh.hist[par ^ 1][tid][0] = s;
       }
+      if constexpr (Fuse::kWord) {
+        LmShared& sh = lm_shared();
+        WordShared& ws = word_shared();
+        const int par = t & 1, node = ws.node[i], n = fu.lm.ngram.order - 1;
+        if (s == fu.lm.delimiter && node != 0) {
+          for (int k = n - 1; k > 0; --k) sh.hist[par ^ 1][tid][k] = sh.hist[par][i][k - 1];
+          if (n > 0) sh.hist[par ^ 1][tid][0] = fu.word_tok(node);
+        } else {
+          for (int k = 0; k < n; ++k) sh.hist[par ^ 1][tid][k] = sh.hist[par][i][k];
+        }
+        ws.lex[par ^ 1][tid] = s == fu.lm.delimiter ? 0 : node < 0 ? -1 : fu.child(node, s);
+      }
     } else {
       const int j = c - K * S;
       double npb, npnb; int rk;
@@ -270,6 +369,14 @@ __device__ __forceinline__ void dec_commit(const DecParams& p, const Beam& cur, 
         const int par = t & 1;
         for (int k = 0; k < fu.lm.order - 1; ++k) sh.hist[par ^ 1][tid][k] = sh.hist[par][j][k];
       }
+      if constexpr (Fuse::kWord) {
+        LmShared& sh = lm_shared();
+        WordShared& ws = word_shared();
+        const int par = t & 1;
+        for (int k = 0; k < fu.lm.ngram.order - 1; ++k)
+          sh.hist[par ^ 1][tid][k] = sh.hist[par][j][k];
+        ws.lex[par ^ 1][tid] = ws.lex[par][j];
+      }
     }
   }
   if (tid == 0) nxt.size = ns;
@@ -282,6 +389,29 @@ __device__ __forceinline__ void dec_finish(const DecParams& p, const Beam& fin) 
     const int b = blockIdx.x;
     p.out_lens[b] = p.trie.of(b).backtrack(fin.node[0], p.out_labels + (size_t)b * p.T);
     p.out_scores[b] = -lse2d(fin.pb[0], fin.pnb[0]);
+  }
+}
+
+// With a word LM: the end-of-utterance rule over the final beam, whose entries' histories and
+// nodes are hist[i] and lex[i] (shared or global memory).  Thread i scores entry i; the largest
+// final_i wins, ties going to the lowest index.  Every thread of the block calls it.
+__device__ __forceinline__ void dec_finish_word(const DecParams& p, const WordLmFuse& fu,
+                                                const Beam& fin,
+                                                const int (*hist)[SB_LM_MAX_ORDER - 1],
+                                                const int* lex) {
+  WordShared& ws = word_shared();
+  const int i = threadIdx.x;
+  if (i < fin.size)
+    ws.fin[i] = lse2d(fin.pb[i], fin.pnb[i]) +
+                fu.end_term(lex[i], [&](int k) { return hist[i][k]; }, lm_shared().ctx[i]);
+  __syncthreads();
+  if (i == 0) {
+    int best = 0;
+    for (int j = 1; j < fin.size; ++j)
+      if (ws.fin[j] > ws.fin[best]) best = j;
+    const int b = blockIdx.x;
+    p.out_lens[b] = p.trie.of(b).backtrack(fin.node[best], p.out_labels + (size_t)b * p.T);
+    p.out_scores[b] = -ws.fin[best];
   }
 }
 
@@ -302,19 +432,26 @@ struct DecOffline {
     return 0;
   }
   template <class Fuse>
-  __device__ __forceinline__ void end(const DecParams& p, const Beam* beams, int t) const {
-    dec_finish(p, beams[t & 1]);
+  __device__ __forceinline__ void end(const DecParams& p, const Fuse& fu, const Beam* beams,
+                                      int t) const {
+    if constexpr (Fuse::kWord)
+      dec_finish_word(p, fu, beams[t & 1], lm_shared().hist[t & 1], word_shared().lex[t & 1]);
+    else
+      dec_finish(p, beams[t & 1]);
   }
 };
 
-// One stream of the resumable search: the beam after frame `frames` - 1 and its entries' contexts.
+// One stream of the resumable search: the beam after frame `frames` - 1 and its entries' contexts
+// (and, with a word LM, lexicon nodes).
 struct DecSlot {
   Beam beam;
   int hist[DEC_MAX_BEAM][SB_LM_MAX_ORDER - 1];
   int frames;     // frames consumed since the last reset
   int overflow;   // a step was asked for frames past max_frames (and clamped)
+  int lex[DEC_MAX_BEAM];
 };
 static constexpr size_t DEC_SLOT_BYTES = (sizeof(DecSlot) + 255) / 256 * 256;
+static_assert(DEC_SLOT_BYTES == 2304, "the lexicon nodes fit the slot's padding");
 
 __device__ __forceinline__ DecSlot* dec_slot(void* base, int b) {
   return reinterpret_cast<DecSlot*>(static_cast<unsigned char*>(base) + (size_t)b * DEC_SLOT_BYTES);
@@ -339,15 +476,20 @@ struct DecResume {
       if (threadIdx.x == 0) dec_slot(slots, blockIdx.x)->overflow = 1;
     }
     dec_copy(&beams[t0 & 1], &sl->beam, sizeof(Beam));
-    if constexpr (Fuse::kLm) dec_copy(lm_shared().hist[t0 & 1], sl->hist, sizeof(sl->hist));
+    if constexpr (Fuse::kLm || Fuse::kWord)
+      dec_copy(lm_shared().hist[t0 & 1], sl->hist, sizeof(sl->hist));
+    if constexpr (Fuse::kWord) dec_copy(word_shared().lex[t0 & 1], sl->lex, sizeof(sl->lex));
     __syncthreads();
     return t0;
   }
   template <class Fuse>
-  __device__ __forceinline__ void end(const DecParams& p, const Beam* beams, int t) const {
+  __device__ __forceinline__ void end(const DecParams& p, const Fuse& fu, const Beam* beams,
+                                      int t) const {
     DecSlot* sl = dec_slot(slots, blockIdx.x);
     dec_copy(&sl->beam, &beams[t & 1], sizeof(Beam));
-    if constexpr (Fuse::kLm) dec_copy(sl->hist, lm_shared().hist[t & 1], sizeof(sl->hist));
+    if constexpr (Fuse::kLm || Fuse::kWord)
+      dec_copy(sl->hist, lm_shared().hist[t & 1], sizeof(sl->hist));
+    if constexpr (Fuse::kWord) dec_copy(sl->lex, word_shared().lex[t & 1], sizeof(sl->lex));
     if (threadIdx.x == 0) sl->frames = t;
   }
 };
@@ -398,7 +540,7 @@ __device__ __forceinline__ void ctc_prefix_beam_body(const DecParams p, const Fu
     // ---- 3. materialise the pruned beam ----
     dec_commit(p, cur, nxt, mine, ns, lp, t, fu);
   }
-  io.template end<Fuse>(p, beams, t0 + T);
+  io.end(p, fu, beams, t0 + T);
 }
 
 template <class Fuse>
@@ -450,6 +592,14 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) ctc_stream_kernel(
 // is -inf exactly (the LM terms are finite), so U = -inf keeps its meaning.  A frame the check
 // cannot prove is rescanned as above, with the same fused arithmetic.
 //
+// With a word LM (WordLmFuse) each entry also scores the delimiter on every frame, next to its
+// last symbol (and deduplicated as that is), since the delimiter carries the word's LM term.
+// Every other class s has q_s = p_s or q_s = p_s + gamma, and gamma <= 0, so q_s <= p_s in exact
+// arithmetic and also as computed: floating-point addition rounds monotonically, so
+// fl(p_s + gamma) <= fl(p_s + 0) = p_s (and p_s + -inf = -inf).  A left-out class therefore has
+// q_s <= p_s <= p_min, and the LM-less bound U = max_i f_i(p_min) and margin apply unchanged: the
+// word LM causes no rescans of its own.
+//
 // The shortlist of every frame (2K + 1 ints, or S - 1 if fewer) comes from a pre-pass over the
 // B*T rows (ctc_shortlist_kernel, one CTA per frame).
 // ------------------------------------------------------------------------------------------------
@@ -492,7 +642,7 @@ __device__ __forceinline__ void ctc_prefix_beam_shortlist_body(
   const int b = blockIdx.x, tid = threadIdx.x;
   const int K = p.K, S = p.S;
   int T = min(p.lens[b], p.T);
-  const int per = L + 1;                   // shortlist + last_i per entry
+  const int per = L + 1 + (Fuse::kWord ? 1 : 0);   // shortlist + last_i (+ delimiter) per entry
   const int ncand = K * per + K;
   double* score = reinterpret_cast<double*>(dec_smem);             // [ncand]
   int* rank = reinterpret_cast<int*>(score + ncand);               // [ncand]
@@ -525,6 +675,14 @@ __device__ __forceinline__ void ctc_prefix_beam_shortlist_body(
           if (j == L) {
             for (int q = 0; q < L && s >= 0; ++q)
               if (sl[q] == s) s = -1;        // already scored as a shortlisted symbol
+          }
+          if constexpr (Fuse::kWord) {
+            if (j == L + 1) {                // the delimiter, unless scored above
+              s = fu.lm.delimiter;
+              for (int q = 0; q < L && s >= 0; ++q)
+                if (sl[q] == s) s = -1;
+              if (s == cur.last[i]) s = -1;
+            }
           }
           if (s >= 0 && s != p.blank) {
             fc = i * S + s;
@@ -578,7 +736,7 @@ __device__ __forceinline__ void ctc_prefix_beam_shortlist_body(
     }
     __syncthreads();
     // ---- 3b. otherwise: full streamed scan of this frame ----
-    if constexpr (Fuse::kLm)
+    if constexpr (Fuse::kLm || Fuse::kWord)
       if (!complete && rescan && tid == 0) atomicAdd(&dec_lm_rescans, 1ull);
     if (!complete && rescan) {
       ns = 0;
@@ -603,7 +761,7 @@ __device__ __forceinline__ void ctc_prefix_beam_shortlist_body(
     // ---- 4. materialise the pruned beam ----
     dec_commit(p, cur, nxt, mine, ns, lp, t, fu);
   }
-  io.template end<Fuse>(p, beams, t0 + T);
+  io.end(p, fu, beams, t0 + T);
 }
 
 template <class Fuse>
@@ -626,6 +784,7 @@ __global__ void __launch_bounds__(DEC_THREADS) ctc_stream_reset_kernel(const Bea
   if (threadIdx.x == 0) {
     dec_empty(sl->beam);
     sl->hist[0][0] = -1;
+    sl->lex[0] = 0;
     sl->frames = 0;
     sl->overflow = 0;
   }
@@ -637,6 +796,16 @@ __global__ void __launch_bounds__(32) ctc_stream_best_kernel(const DecParams p, 
                                                              int* out_overflow) {
   const DecSlot* sl = dec_slot(const_cast<void*>(slots), blockIdx.x);
   dec_finish(p, sl->beam);
+  if (threadIdx.x == 0 && out_overflow) out_overflow[blockIdx.x] = sl->overflow;
+}
+
+// The same with a word LM: the end-of-utterance rule over each stored beam (dec_finish_word).
+__global__ void __launch_bounds__(32) ctc_stream_best_wordlm_kernel(const DecParams p,
+                                                                    const void* slots,
+                                                                    int* out_overflow,
+                                                                    const WordLmFuse fu) {
+  const DecSlot* sl = dec_slot(const_cast<void*>(slots), blockIdx.x);
+  dec_finish_word(p, fu, sl->beam, sl->hist, sl->lex);
   if (threadIdx.x == 0 && out_overflow) out_overflow[blockIdx.x] = sl->overflow;
 }
 
@@ -677,8 +846,8 @@ static BeamTrie dec_trie(void* base, int B, size_t node_cap) {
 
 // Both routes with the fusion policy fu, over a fresh beam (rs null) or resumed from the slots of
 // *rs.  Every shape whose K*S + K full-scan candidates fit in 200 KB of shared memory takes the
-// full scan; the static shared memory of either instantiation (5.8 KB at most, with the LM's
-// contexts) leaves both sizes below the per-block limit.  shortlist: B*T*(2K+1) ints.
+// full scan; the static shared memory of any instantiation (6.7 KB at most, with a word LM's
+// contexts and nodes) leaves both sizes below the per-block limit.  shortlist: B*T*(2K+1) ints.
 template <class Fuse>
 static int dec_launch(const DecParams& p, const Fuse& fu, const DecResume* rs, int* shortlist,
                       bool force_shortlist, cudaStream_t stream) {
@@ -699,7 +868,7 @@ static int dec_launch(const DecParams& p, const Fuse& fu, const DecResume* rs, i
 
   const int LS = 2 * beam_size + 1;
   const int L = S - 1 < LS ? S - 1 : LS;
-  const int ncand = beam_size * (L + 1) + beam_size;
+  const int ncand = beam_size * (L + 1 + (Fuse::kWord ? 1 : 0)) + beam_size;
   const size_t smem = (size_t)ncand * (sizeof(double) + 2 * sizeof(int) + 1) + 16;
   const void* kern = rs ? (const void*)ctc_stream_shortlist_kernel<Fuse>
                         : (const void*)ctc_prefix_beam_shortlist_kernel<Fuse>;
@@ -954,4 +1123,123 @@ extern "C" int sb_debug_ctc_lm_rescans(unsigned long long* frames) {
       cudaMemcpyToSymbol(dec_lm_rescans, &zero, sizeof(zero)) != cudaSuccess)
     return SB_ERR_CUDA;
   return SB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Word LM (SbWordLm): the same routes and state over WordLmFuse.
+// ------------------------------------------------------------------------------------------------
+static int dec_wordlm_fuse(int S, int blank, const SbWordLm* lm, double lm_weight,
+                           double insertion_bonus, double oov_penalty, WordLmFuse* fu) {
+  if (!lm) return SB_ERR_INVALID;
+  const SbNgramLm& ng = lm->ngram;
+  if (!ng.keys || !ng.vals || !ng.logp || !ng.bow || !ng.tok || !lm->lex_keys || !lm->lex_vals ||
+      !lm->lex_word)
+    return SB_ERR_INVALID;
+  if (!(lm_weight >= 0.0) || !isfinite(lm_weight) || !isfinite(insertion_bonus))
+    return SB_ERR_INVALID;
+  if (isnan(oov_penalty) || oov_penalty > 0.0) return SB_ERR_INVALID;
+  if (!lm->has_unk && oov_penalty != -INFINITY) return SB_ERR_INVALID;
+  if (lm->num_classes < S || lm->blank != blank) return SB_ERR_INVALID;
+  if (lm->delimiter < 0 || lm->delimiter >= S || lm->delimiter == blank) return SB_ERR_INVALID;
+  if (ng.cap <= 0 || (ng.cap & (ng.cap - 1)) || lm->lex_cap <= 0 ||
+      (lm->lex_cap & (lm->lex_cap - 1)) || lm->num_words < 1 || ng.bos != lm->num_words ||
+      ng.order < 1)
+    return SB_ERR_INVALID;
+  if (ng.order > SB_LM_MAX_ORDER) return SB_ERR_UNSUPPORTED;
+  fu->lm = *lm;
+  fu->alpha = lm_weight;
+  fu->beta = insertion_bonus;
+  fu->gamma = oov_penalty;
+  return SB_OK;
+}
+
+static int dec_wordlm_entry(const float* logp, const int* lens, int B, int T, int S, int beam_size,
+                            int blank, const SbWordLm* lm, double lm_weight,
+                            double insertion_bonus, double oov_penalty, int* out_labels,
+                            int* out_lens, double* out_scores, void* workspace,
+                            size_t workspace_bytes, void* stream, bool force_shortlist) {
+  WordLmFuse fu;
+  const int rc = dec_wordlm_fuse(S, blank, lm, lm_weight, insertion_bonus, oov_penalty, &fu);
+  if (rc != SB_OK) return rc;
+  return dec_entry(logp, lens, B, T, S, beam_size, blank, out_labels, out_lens, out_scores,
+                   workspace, workspace_bytes, stream, force_shortlist, fu);
+}
+
+extern "C" int sb_ctc_prefix_beam_wordlm(const float* logp, const int* lens, int B, int T, int S,
+                                         int beam_size, int blank, const SbWordLm* lm,
+                                         double lm_weight, double insertion_bonus,
+                                         double oov_penalty, int* out_labels, int* out_lens,
+                                         double* out_scores, void* workspace,
+                                         size_t workspace_bytes, void* stream) {
+  return dec_wordlm_entry(logp, lens, B, T, S, beam_size, blank, lm, lm_weight, insertion_bonus,
+                          oov_penalty, out_labels, out_lens, out_scores, workspace,
+                          workspace_bytes, stream, false);
+}
+
+extern "C" int sb_ctc_prefix_beam_wordlm_shortlist(const float* logp, const int* lens, int B,
+                                                   int T, int S, int beam_size, int blank,
+                                                   const SbWordLm* lm, double lm_weight,
+                                                   double insertion_bonus, double oov_penalty,
+                                                   int* out_labels, int* out_lens,
+                                                   double* out_scores, void* workspace,
+                                                   size_t workspace_bytes, void* stream) {
+  return dec_wordlm_entry(logp, lens, B, T, S, beam_size, blank, lm, lm_weight, insertion_bonus,
+                          oov_penalty, out_labels, out_lens, out_scores, workspace,
+                          workspace_bytes, stream, true);
+}
+
+static int dec_stream_wordlm_entry(const float* logp, const int* n, int B, int T, int S,
+                                   int beam_size, int blank, const SbWordLm* lm, double lm_weight,
+                                   double insertion_bonus, double oov_penalty, int max_frames,
+                                   void* state, void* workspace, size_t workspace_bytes,
+                                   void* stream, bool force_shortlist) {
+  WordLmFuse fu;
+  const int rc = dec_wordlm_fuse(S, blank, lm, lm_weight, insertion_bonus, oov_penalty, &fu);
+  if (rc != SB_OK) return rc;
+  return dec_stream_entry(logp, n, B, T, S, beam_size, blank, max_frames, state, workspace,
+                          workspace_bytes, stream, force_shortlist, fu);
+}
+
+extern "C" int sb_ctc_stream_step_wordlm(const float* logp, const int* n, int B, int T, int S,
+                                         int beam_size, int blank, const SbWordLm* lm,
+                                         double lm_weight, double insertion_bonus,
+                                         double oov_penalty, int max_frames, void* state,
+                                         void* workspace, size_t workspace_bytes, void* stream) {
+  return dec_stream_wordlm_entry(logp, n, B, T, S, beam_size, blank, lm, lm_weight,
+                                 insertion_bonus, oov_penalty, max_frames, state, workspace,
+                                 workspace_bytes, stream, false);
+}
+
+extern "C" int sb_ctc_stream_step_wordlm_shortlist(const float* logp, const int* n, int B, int T,
+                                                   int S, int beam_size, int blank,
+                                                   const SbWordLm* lm, double lm_weight,
+                                                   double insertion_bonus, double oov_penalty,
+                                                   int max_frames, void* state, void* workspace,
+                                                   size_t workspace_bytes, void* stream) {
+  return dec_stream_wordlm_entry(logp, n, B, T, S, beam_size, blank, lm, lm_weight,
+                                 insertion_bonus, oov_penalty, max_frames, state, workspace,
+                                 workspace_bytes, stream, true);
+}
+
+extern "C" int sb_ctc_stream_best_wordlm(const void* state, int B, int max_frames, int beam_size,
+                                         const SbWordLm* lm, double lm_weight,
+                                         double insertion_bonus, double oov_penalty,
+                                         int* out_labels, int* out_lens, double* out_scores,
+                                         int* out_overflow, void* stream) {
+  if (!state || !out_labels || !out_lens || !out_scores || !out_overflow || !lm)
+    return SB_ERR_INVALID;
+  WordLmFuse fu;
+  int rc = dec_wordlm_fuse(lm->num_classes, lm->blank, lm, lm_weight, insertion_bonus,
+                           oov_penalty, &fu);
+  if (rc != SB_OK) return rc;
+  rc = dec_stream_check(B, max_frames, beam_size);
+  if (rc != SB_OK) return rc;
+  DecParams p;
+  memset(&p, 0, sizeof(p));
+  p.trie = dec_stream_trie(const_cast<void*>(state), B, max_frames, beam_size);
+  p.out_labels = out_labels; p.out_lens = out_lens; p.out_scores = out_scores;
+  p.B = B; p.T = max_frames; p.K = beam_size;
+  ctc_stream_best_wordlm_kernel<<<B, 32, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      p, state, out_overflow, fu);
+  return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
 }

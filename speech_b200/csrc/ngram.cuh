@@ -1,5 +1,6 @@
 // Device lookup of the backoff n-gram LM (SbNgramLm, include/speech_b200.h), shared by the searches
-// that fuse it: the CTC prefix beam search (decode.cu) and the attention beam search (s2s.cu).
+// that fuse it: the CTC prefix beam search (decode.cu, with a token or a word LM) and the attention
+// beam search (s2s.cu).
 // A search resolves each hypothesis' context once (lm_context: at most order - 1 probes), then
 // scores any number of next tokens against it (lm_backoff: at most order probes each).
 #pragma once
@@ -9,8 +10,10 @@
 
 namespace sb {
 
-// value of key (node, tok, kind) in the map, -1 where it is not stored
-__device__ __forceinline__ int lm_find(const SbNgramLm& lm, int node, int tok, int kind) {
+// value of key (node, tok, kind) in an open-addressed map of include/speech_b200.h's layout, -1
+// where it is not stored; Map has its keys, vals and cap: SbNgramLm, or a word LM's lexicon (LexMap)
+template <class Map>
+__device__ __forceinline__ int map_find(const Map& lm, int node, int tok, int kind) {
   const unsigned long long key = ((unsigned long long)(unsigned int)node << 32) |
                                  ((unsigned long long)(unsigned int)(tok + 1) << 1) |
                                  (unsigned long long)kind;
@@ -23,6 +26,17 @@ __device__ __forceinline__ int lm_find(const SbNgramLm& lm, int node, int tok, i
   }
   return -1;
 }
+
+__device__ __forceinline__ int lm_find(const SbNgramLm& lm, int node, int tok, int kind) {
+  return map_find(lm, node, tok, kind);
+}
+
+// the lexicon map of an SbWordLm: (node, class) -> child node
+struct LexMap {
+  const unsigned long long* keys;
+  const int* vals;
+  int cap;
+};
 
 // lm(t | context), t an LM token, ctx[0] = root .. ctx[depth] the context's nodes (lm_context):
 // the longest stored context first, adding the backoff of each that misses

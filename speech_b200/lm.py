@@ -1,5 +1,8 @@
-"""Token-level backoff n-gram language model for shallow fusion in the CTC prefix beam search, the
-attention model's beam search and the Transducer's label-free beam search.
+"""Backoff n-gram language models for shallow fusion: NGramLM over the model's own classes, for
+the CTC prefix beam search, the attention model's beam search and the Transducer's label-free beam
+search; WordLM over words spelled in a character model's classes, for the CTC prefix beam search
+(see WordLM).  Both read and write ARPA files and train interpolated Kneser-Ney models through the
+same module functions.
 
 The LM is over the acoustic model's own output classes (characters or subword units); the blank is
 never an LM token.  Orders 1..10, with a sentence start <s>, an end </s> and optionally <unk>.
@@ -110,6 +113,240 @@ def _check_end(end, blank, num_classes):
     return int(end)
 
 
+# ------------------------------------------------------------------------------------------------
+# ARPA files, Kneser-Ney training and the device tables, shared by NGramLM and WordLM.  An LM is
+# held as ngrams[n] = {token tuple: (log10 prob, log10 backoff or None)}, n = 1..order.
+# ------------------------------------------------------------------------------------------------
+def _read_arpa(path, vocabulary):
+    """(order, ngrams, dropped) of an ARPA file.  vocabulary(unigram words) -> {word: token} is
+    called once the 1-gram section is read; n-grams with a word it does not map are dropped and
+    counted."""
+    with open(path, "r", encoding="utf-8") as fh:
+        lines = [ln.strip() for ln in fh]
+    lines = [ln for ln in lines if ln]
+    try:
+        i = lines.index("\\data\\")
+    except ValueError:
+        raise ValueError("n-gram LM: %s has no \\data\\ section" % path) from None
+    i += 1
+    counts = {}
+    while i < len(lines) and lines[i].startswith("ngram "):
+        key, _, val = lines[i][6:].partition("=")
+        try:
+            counts[int(key)] = int(val)
+        except ValueError:
+            raise ValueError("n-gram LM: bad count line %r" % lines[i]) from None
+        i += 1
+    if not counts:
+        raise ValueError("n-gram LM: %s declares no n-gram counts" % path)
+    order = max(counts)
+    _check_order(order)
+    if sorted(counts) != list(range(1, order + 1)) or any(v < 0 for v in counts.values()):
+        raise ValueError("n-gram LM: counts must be given for orders 1..%d" % order)
+    ngrams = {n: {} for n in range(1, order + 1)}
+    dropped = 0
+    word_tok = None
+    for n in range(1, order + 1):
+        header = "\\%d-grams:" % n
+        if i >= len(lines) or lines[i] != header:
+            raise ValueError("n-gram LM: missing section %s" % header)
+        i += 1
+        section = []
+        for _ in range(counts[n]):
+            if i >= len(lines) or lines[i].startswith("\\"):
+                raise ValueError("n-gram LM: section %s has fewer than %d entries"
+                                 % (header, counts[n]))
+            f = lines[i].split()
+            i += 1
+            if len(f) not in (n + 1, n + 2):
+                raise ValueError("n-gram LM: malformed %d-gram line %r" % (n, " ".join(f)))
+            try:
+                p = float(f[0])
+                b = float(f[n + 1]) if len(f) == n + 2 else None
+            except ValueError:
+                raise ValueError("n-gram LM: malformed number in %r" % " ".join(f)) from None
+            _finite(p, "a %d-gram probability" % n)
+            if b is not None:
+                _finite(b, "a %d-gram backoff" % n)
+            section.append((f[1:n + 1], p, b))
+        if word_tok is None:
+            word_tok = vocabulary([words[0] for words, _, _ in section])
+        for words, p, b in section:
+            if any(w not in word_tok for w in words):
+                dropped += 1
+                continue
+            g = tuple(word_tok[w] for w in words)
+            if g in ngrams[n]:
+                raise ValueError("n-gram LM: duplicate %d-gram %r" % (n, " ".join(words)))
+            ngrams[n][g] = (p, b)
+    if i >= len(lines) or lines[i] != "\\end\\":
+        raise ValueError("n-gram LM: %s: expected \\end\\ after the %d-grams (wrong counts?)"
+                         % (path, order))
+    return order, ngrams, dropped
+
+
+def _write_arpa(path, order, ngrams, names):
+    """ARPA file of ngrams, names[token] the word of each token; values written with repr, which
+    reads back to the same float64"""
+    out = ["", "\\data\\"]
+    out += ["ngram %d=%d" % (n, len(ngrams[n])) for n in range(1, order + 1)]
+    for n in range(1, order + 1):
+        out += ["", "\\%d-grams:" % n]
+        for g, (p, b) in sorted(ngrams[n].items()):
+            line = "%r\t%s" % (p, " ".join(names[t] for t in g))
+            out.append(line if b is None else "%s\t%r" % (line, b))
+    out += ["", "\\end\\", ""]
+    with open(path, "w", encoding="utf-8") as fh:
+        fh.write("\n".join(out))
+
+
+def _kneser_ney(sequences, order, vocab, bos, eos):
+    """Interpolated Kneser-Ney in backoff form over token sequences (each read as <s> w1 .. wn
+    </s>); vocab: the tokens the unigram level spreads its uniform share over (</s> included)."""
+    raw = {n: Counter() for n in range(1, order + 1)}
+    for seq in sequences:
+        w = [bos] + list(seq) + [eos]
+        for n in range(1, order + 1):
+            for j in range(len(w) - n + 1):
+                raw[n][tuple(w[j:j + n])] += 1
+    raw[1].pop((bos,), None)                            # <s> is never predicted
+    # KN counts: raw at the top order and for n-grams that begin with <s>, else the number of
+    # distinct tokens seen before the n-gram
+    kn = {order: raw[order]}
+    for n in range(order - 1, 0, -1):
+        left = Counter(g[1:] for g in raw[n + 1])
+        kn[n] = {g: (c if g[0] == bos else left[g]) for g, c in raw[n].items()}
+    disc, denom, types = {}, {}, {}
+    for n in range(1, order + 1):
+        n1 = sum(1 for c in kn[n].values() if c == 1)
+        n2 = sum(1 for c in kn[n].values() if c == 2)
+        d = n1 / (n1 + 2 * n2) if n1 + 2 * n2 else 0.0
+        disc[n] = d if 0.0 < d < 1.0 else 0.5
+        den, typ = defaultdict(int), defaultdict(int)
+        for g, c in kn[n].items():
+            den[g[:-1]] += c
+            typ[g[:-1]] += 1
+        denom[n], types[n] = den, typ
+
+    def gamma(n, h):
+        return disc[n] * types[n][h] / denom[n][h]
+
+    memo = {}
+
+    def prob(h, w):
+        """P_n(w | h), n = len(h) + 1"""
+        key = (h, w)
+        if key in memo:
+            return memo[key]
+        n = len(h) + 1
+        lower = prob(h[1:], w) if n > 1 else 1.0 / len(vocab)
+        den = denom[n].get(h, 0)
+        if den == 0:
+            v = lower
+        else:
+            c = kn[n].get(h + (w,), 0)
+            v = max(c - disc[n], 0.0) / den + gamma(n, h) * lower
+        memo[key] = v
+        return v
+
+    ngrams = {n: {} for n in range(1, order + 1)}
+    for w in vocab:
+        ngrams[1][(w,)] = (math.log10(prob((), w)), None)
+    ngrams[1][(bos,)] = (-99.0, None)
+    for n in range(2, order + 1):
+        for g in kn[n]:
+            ngrams[n][g] = (math.log10(prob(g[:-1], g[-1])), None)
+    for n in range(1, order):
+        for h in denom[n + 1]:
+            p, _ = ngrams[n][h]
+            ngrams[n][h] = (p, math.log10(gamma(n + 1, h)))
+    return ngrams
+
+
+def _pack_map(entries):
+    """(keys, vals, cap) of the open-addressed map of include/speech_b200.h over (key, value)
+    pairs, inserted in order with linear probing"""
+    cap = 64
+    while cap < 2 * len(entries):
+        cap <<= 1
+    keys = [0] * cap
+    vals = [-1] * cap
+    mask = cap - 1
+    for k, v in entries:
+        h = ((k * _HASH_MUL) & _MASK64) >> 32 & mask
+        while keys[h] != 0:
+            h = (h + 1) & mask
+        keys[h] = k
+        vals[h] = v
+    return np.array(keys, np.uint64), np.array(vals, np.int32), cap
+
+
+def _map_key(node, tok, kind):
+    return (node << 32) | ((tok + 1) << 1) | kind
+
+
+def _backoff_tables(order, ngrams, bos, eos, with_eos):
+    """The n-gram tables of SbNgramLm but tok: keys, vals, logp, bow, cap, order, bos, lm_upper,
+    lm_abs.  with_eos: the n-grams that predict </s> are stored (a search scores it)."""
+    ctx = {(): 0}
+    entries = []                       # (key, value)
+    bow = [0.0]
+
+    def ctx_node(h):
+        """node of context h (oldest .. newest), created with backoff 0 when missing"""
+        if h in ctx:
+            return ctx[h]
+        parent = ctx_node(h[1:])
+        nid = len(bow)
+        ctx[h] = nid
+        bow.append(0.0)
+        entries.append((_map_key(parent, h[0], 0), nid))
+        return nid
+
+    def usable(g):
+        # contexts: <s> only as the oldest token, never </s>
+        return all(t != eos for t in g) and all(t != bos for t in g[1:])
+
+    logp = []
+    upper_p, abs_p = -math.inf, 0.0
+    upper_b = [0.0] * (order + 1)
+    abs_b = [0.0] * (order + 1)
+    for n in range(1, order + 1):
+        for g, (p10, b10) in sorted(ngrams[n].items()):
+            p = p10 * LN10
+            if b10 is not None and n < order:
+                b = b10 * LN10
+                upper_b[n] = max(upper_b[n], b)
+                abs_b[n] = max(abs_b[n], abs(b))
+                if usable(g):
+                    bow[ctx_node(g)] = b
+            if g[-1] == bos or (g[-1] == eos and not with_eos) or not usable(g[:-1]):
+                continue                # never looked up
+            upper_p, abs_p = max(upper_p, p), max(abs_p, abs(p))
+            entries.append((_map_key(ctx_node(g[:-1]), g[-1], 1), len(logp)))
+            logp.append(p)
+    keys, vals, cap = _pack_map(entries)
+    return {
+        "keys": keys, "vals": vals, "logp": np.array(logp or [0.0], np.float64),
+        "bow": np.array(bow, np.float64), "cap": cap, "order": order, "bos": bos,
+        "lm_upper": upper_p + sum(upper_b), "lm_abs": abs_p + sum(abs_b),
+    }
+
+
+def _device(device):
+    import torch
+    device = torch.device(device)
+    if device.type == "cuda" and device.index is None:
+        device = torch.device("cuda", torch.cuda.current_device())
+    return device
+
+
+def _to_device(h, names, device):
+    import torch
+    return {k: torch.from_numpy(h[k].view(np.int64) if h[k].dtype == np.uint64 else h[k])
+            .to(device) for k in names}
+
+
 class NGramLM:
     """Backoff n-gram LM over class ids.  Tokens: class c -> c, <s> -> C, </s> -> C + 1,
     <unk> -> C + 2 (C = num_classes); the end class, where there is one, -> </s>.  Build with
@@ -173,60 +410,7 @@ class NGramLM:
         names = _class_names(symbols, blank, num_classes, end)
         word_tok = {s: c for c, s in names.items()}
         word_tok.update({BOS: num_classes, EOS: num_classes + 1, UNK: num_classes + 2})
-        with open(path, "r", encoding="utf-8") as fh:
-            lines = [ln.strip() for ln in fh]
-        lines = [ln for ln in lines if ln]
-        try:
-            i = lines.index("\\data\\")
-        except ValueError:
-            raise ValueError("n-gram LM: %s has no \\data\\ section" % path) from None
-        i += 1
-        counts = {}
-        while i < len(lines) and lines[i].startswith("ngram "):
-            key, _, val = lines[i][6:].partition("=")
-            try:
-                counts[int(key)] = int(val)
-            except ValueError:
-                raise ValueError("n-gram LM: bad count line %r" % lines[i]) from None
-            i += 1
-        if not counts:
-            raise ValueError("n-gram LM: %s declares no n-gram counts" % path)
-        order = max(counts)
-        _check_order(order)
-        if sorted(counts) != list(range(1, order + 1)) or any(v < 0 for v in counts.values()):
-            raise ValueError("n-gram LM: counts must be given for orders 1..%d" % order)
-        ngrams = {n: {} for n in range(1, order + 1)}
-        for n in range(1, order + 1):
-            header = "\\%d-grams:" % n
-            if i >= len(lines) or lines[i] != header:
-                raise ValueError("n-gram LM: missing section %s" % header)
-            i += 1
-            for _ in range(counts[n]):
-                if i >= len(lines) or lines[i].startswith("\\"):
-                    raise ValueError("n-gram LM: section %s has fewer than %d entries"
-                                     % (header, counts[n]))
-                f = lines[i].split()
-                i += 1
-                if len(f) not in (n + 1, n + 2):
-                    raise ValueError("n-gram LM: malformed %d-gram line %r" % (n, " ".join(f)))
-                try:
-                    p = float(f[0])
-                    b = float(f[n + 1]) if len(f) == n + 2 else None
-                except ValueError:
-                    raise ValueError("n-gram LM: malformed number in %r" % " ".join(f)) from None
-                _finite(p, "a %d-gram probability" % n)
-                if b is not None:
-                    _finite(b, "a %d-gram backoff" % n)
-                words = f[1:n + 1]
-                if any(w not in word_tok for w in words):
-                    continue
-                g = tuple(word_tok[w] for w in words)
-                if g in ngrams[n]:
-                    raise ValueError("n-gram LM: duplicate %d-gram %r" % (n, " ".join(words)))
-                ngrams[n][g] = (p, b)
-        if i >= len(lines) or lines[i] != "\\end\\":
-            raise ValueError("n-gram LM: %s: expected \\end\\ after the %d-grams (wrong counts?)"
-                             % (path, order))
+        order, ngrams, _ = _read_arpa(path, lambda unigram_words: word_tok)
         return cls(order, num_classes, blank, ngrams, end)
 
     def to_arpa(self, path, symbols=None):
@@ -239,16 +423,7 @@ class NGramLM:
             raise ValueError("n-gram LM: symbols do not cover the LM's classes")
         names = _class_names(symbols, self._blank, self._num_classes, self._end)
         names.update({self._bos: BOS, self._eos: EOS, self._unk: UNK})
-        out = ["", "\\data\\"]
-        out += ["ngram %d=%d" % (n, len(self._ngrams[n])) for n in range(1, self._order + 1)]
-        for n in range(1, self._order + 1):
-            out += ["", "\\%d-grams:" % n]
-            for g, (p, b) in sorted(self._ngrams[n].items()):
-                line = "%r\t%s" % (p, " ".join(names[t] for t in g))
-                out.append(line if b is None else "%s\t%r" % (line, b))
-        out += ["", "\\end\\", ""]
-        with open(path, "w", encoding="utf-8") as fh:
-            fh.write("\n".join(out))
+        _write_arpa(path, self._order, self._ngrams, names)
 
     # ------------------------------------------------------------------------------------------
     # training: interpolated Kneser-Ney in backoff form
@@ -271,7 +446,7 @@ class NGramLM:
             raise ValueError("n-gram LM: need num_classes >= 2 and 0 <= blank < num_classes")
         end = _check_end(end, blank, C)
         bos, eos = C, C + 1
-        raw = {n: Counter() for n in range(1, order + 1)}
+        seqs = []
         for seq in sequences:
             seq = [int(v) for v in seq]
             if end is not None:
@@ -280,62 +455,9 @@ class NGramLM:
             if any(v < 0 or v >= C or v == blank or v == end for v in seq):
                 raise ValueError("n-gram LM: a training label is out of range, the blank or "
                                  "the end")
-            w = [bos] + seq + [eos]
-            for n in range(1, order + 1):
-                for j in range(len(w) - n + 1):
-                    raw[n][tuple(w[j:j + n])] += 1
-        raw[1].pop((bos,), None)                            # <s> is never predicted
-        # KN counts: raw at the top order and for n-grams that begin with <s>, else the number of
-        # distinct tokens seen before the n-gram
-        kn = {order: raw[order]}
-        for n in range(order - 1, 0, -1):
-            left = Counter(g[1:] for g in raw[n + 1])
-            kn[n] = {g: (c if g[0] == bos else left[g]) for g, c in raw[n].items()}
-        disc, denom, types = {}, {}, {}
-        for n in range(1, order + 1):
-            n1 = sum(1 for c in kn[n].values() if c == 1)
-            n2 = sum(1 for c in kn[n].values() if c == 2)
-            d = n1 / (n1 + 2 * n2) if n1 + 2 * n2 else 0.0
-            disc[n] = d if 0.0 < d < 1.0 else 0.5
-            den, typ = defaultdict(int), defaultdict(int)
-            for g, c in kn[n].items():
-                den[g[:-1]] += c
-                typ[g[:-1]] += 1
-            denom[n], types[n] = den, typ
-
-        def gamma(n, h):
-            return disc[n] * types[n][h] / denom[n][h]
-
+            seqs.append(seq)
         vocab = [c for c in range(C) if c != blank and c != end] + [eos]
-        memo = {}
-
-        def prob(h, w):
-            """P_n(w | h), n = len(h) + 1"""
-            key = (h, w)
-            if key in memo:
-                return memo[key]
-            n = len(h) + 1
-            lower = prob(h[1:], w) if n > 1 else 1.0 / len(vocab)
-            den = denom[n].get(h, 0)
-            if den == 0:
-                v = lower
-            else:
-                c = kn[n].get(h + (w,), 0)
-                v = max(c - disc[n], 0.0) / den + gamma(n, h) * lower
-            memo[key] = v
-            return v
-
-        ngrams = {n: {} for n in range(1, order + 1)}
-        for w in vocab:
-            ngrams[1][(w,)] = (math.log10(prob((), w)), None)
-        ngrams[1][(bos,)] = (-99.0, None)
-        for n in range(2, order + 1):
-            for g in kn[n]:
-                ngrams[n][g] = (math.log10(prob(g[:-1], g[-1])), None)
-        for n in range(1, order):
-            for h in denom[n + 1]:
-                p, _ = ngrams[n][h]
-                ngrams[n][h] = (p, math.log10(gamma(n + 1, h)))
+        ngrams = _kneser_ney(seqs, order, vocab, bos, eos)
         return cls(order, C, blank, ngrams, end)
 
     # ------------------------------------------------------------------------------------------
@@ -348,77 +470,18 @@ class NGramLM:
         class the n-grams that predict </s> are stored too (the attention search scores it)."""
         if self._host is not None:
             return self._host
-        bos, eos = self._bos, self._eos
-        ctx = {(): 0}
-        entries = []                       # (key, value)
-        bow = [0.0]
-
-        def key(node, tok, kind):
-            return (node << 32) | ((tok + 1) << 1) | kind
-
-        def ctx_node(h):
-            """node of context h (oldest .. newest), created with backoff 0 when missing"""
-            if h in ctx:
-                return ctx[h]
-            parent = ctx_node(h[1:])
-            nid = len(bow)
-            ctx[h] = nid
-            bow.append(0.0)
-            entries.append((key(parent, h[0], 0), nid))
-            return nid
-
-        def usable(g):
-            # contexts: <s> only as the oldest token, never </s>
-            return all(t != eos for t in g) and all(t != bos for t in g[1:])
-
-        logp = []
-        upper_p, abs_p = -math.inf, 0.0
-        upper_b = [0.0] * (self._order + 1)
-        abs_b = [0.0] * (self._order + 1)
-        for n in range(1, self._order + 1):
-            for g, (p10, b10) in sorted(self._ngrams[n].items()):
-                p = p10 * LN10
-                if b10 is not None and n < self._order:
-                    b = b10 * LN10
-                    upper_b[n] = max(upper_b[n], b)
-                    abs_b[n] = max(abs_b[n], abs(b))
-                    if usable(g):
-                        bow[ctx_node(g)] = b
-                if g[-1] == bos or (g[-1] == eos and self._end is None) or not usable(g[:-1]):
-                    continue                # never looked up
-                upper_p, abs_p = max(upper_p, p), max(abs_p, abs(p))
-                entries.append((key(ctx_node(g[:-1]), g[-1], 1), len(logp)))
-                logp.append(p)
-        cap = 64
-        while cap < 2 * len(entries):
-            cap <<= 1
-        keys = np.zeros(cap, np.uint64)
-        vals = np.full(cap, -1, np.int32)
-        for k, v in entries:
-            h = ((k * _HASH_MUL) & _MASK64) >> 32 & (cap - 1)
-            while keys[h] != 0:
-                h = (h + 1) & (cap - 1)
-            keys[h] = k
-            vals[h] = v
-        self._host = {
-            "keys": keys, "vals": vals, "logp": np.array(logp or [0.0], np.float64),
-            "bow": np.array(bow, np.float64), "tok": self._tok.copy(), "cap": cap,
-            "order": self._order, "bos": bos,
-            "lm_upper": upper_p + sum(upper_b), "lm_abs": abs_p + sum(abs_b),
-        }
+        self._host = _backoff_tables(self._order, self._ngrams, self._bos, self._eos,
+                                     self._end is not None)
+        self._host["tok"] = self._tok.copy()
         return self._host
 
     def device_tables(self, device):
         """(SbNgramLm ctypes struct, tensors it points into) on `device`, built once per device"""
-        import torch
         from . import _lib
-        device = torch.device(device)
-        if device.type == "cuda" and device.index is None:
-            device = torch.device("cuda", torch.cuda.current_device())
+        device = _device(device)
         if device not in self._dev:
             h = self.host_tables()
-            t = {k: torch.from_numpy(h[k].view(np.int64) if k == "keys" else h[k]).to(device)
-                 for k in ("keys", "vals", "logp", "bow", "tok")}
+            t = _to_device(h, ("keys", "vals", "logp", "bow", "tok"), device)
             st = _lib.SbNgramLm(t["keys"].data_ptr(), t["vals"].data_ptr(), t["logp"].data_ptr(),
                                 t["bow"].data_ptr(), t["tok"].data_ptr(), h["cap"], h["order"],
                                 self._num_classes, h["bos"], self._blank, h["lm_upper"],
@@ -434,3 +497,238 @@ class NGramLM:
     def __setstate__(self, d):
         d.setdefault("_end", None)          # pickled before LMs had an end class
         self.__dict__.update(d)
+
+
+class WordLM:
+    """Backoff word n-gram LM for the CTC prefix beam search of a character model (Hannun et al.
+    2014, arXiv:1408.2873): a word is scored when the delimiter class (the space) that ends it is
+    emitted, and a lexicon of the LM's words, spelled in the model's classes, tracks the partial
+    word.  Word tokens: the spellable words 0..W-1 in sorted order, <s> W, </s> W + 1, <unk> W + 2.
+    Build with from_arpa or train; the search semantics are in include/speech_b200.h (SbWordLm).
+
+        wlm = WordLM.from_arpa("3-gram.arpa", preproc.int_to_char)     # delimiter " ", blank last
+        model.infer(batch, beam_size=32, lm=wlm, lm_weight=0.8, insertion_bonus=1.0)
+
+    A class whose symbol is one character spells that character; the delimiter's and the blank's
+    symbols spell nothing.  oov_penalty (<= 0, settable) is added once per word that leaves the
+    lexicon: 0 scores such words as <unk>, -inf keeps the search to the lexicon.  An LM without an
+    <unk> unigram needs oov_penalty = -inf."""
+
+    def __init__(self, order, words, ngrams, symbols, num_classes, blank, delimiter, oov_penalty,
+                 dropped=0):
+        self._order = order
+        self._words = list(words)
+        self._ngrams = ngrams
+        self._num_classes, self._blank, self._delim = num_classes, blank, delimiter
+        self._symbols = list(symbols)
+        W = len(self._words)
+        self._bos, self._eos, self._unk = W, W + 1, W + 2
+        if (self._eos,) not in ngrams[1]:
+            raise ValueError("word LM: the LM has no %s unigram" % EOS)
+        self._dropped = int(dropped)
+        chars = _spelling(self._symbols, blank, delimiter)
+        self._spell = [tuple(chars[ch] for ch in w) for w in self._words]
+        self._oov = None
+        self.oov_penalty = oov_penalty
+        self._host = None
+        self._dev = {}
+
+    @property
+    def order(self):
+        return self._order
+
+    @property
+    def num_classes(self):
+        return self._num_classes
+
+    @property
+    def blank(self):
+        return self._blank
+
+    @property
+    def end(self):
+        """None: the search has no end class (check_lm reads it as NGramLM.end)"""
+        return None
+
+    @property
+    def delimiter(self):
+        """the class that ends a word"""
+        return self._delim
+
+    @property
+    def num_words(self):
+        return len(self._words)
+
+    @property
+    def words(self):
+        """the lexicon, word token w at index w"""
+        return list(self._words)
+
+    @property
+    def dropped(self):
+        """n-grams from_arpa left out because a word in them cannot be spelled"""
+        return self._dropped
+
+    @property
+    def has_unk(self):
+        return (self._unk,) in self._ngrams[1]
+
+    @property
+    def oov_penalty(self):
+        return self._oov
+
+    @oov_penalty.setter
+    def oov_penalty(self, v):
+        v = float(v)
+        if math.isnan(v) or v > 0.0:
+            raise ValueError("word LM: oov_penalty must be <= 0, got %r" % (v,))
+        if v != -math.inf and not self.has_unk:
+            raise ValueError("word LM: the LM has no %s unigram, so out-of-vocabulary words "
+                             "need oov_penalty = -inf, got %r" % (UNK, v))
+        self._oov = v
+
+    def spell(self, word):
+        """the classes of a word, or None where a character has no class"""
+        chars = _spelling(self._symbols, self._blank, self._delim)
+        if word == "" or any(ch not in chars for ch in word):
+            return None
+        return tuple(chars[ch] for ch in word)
+
+    # ------------------------------------------------------------------------------------------
+    # ARPA and training
+    # ------------------------------------------------------------------------------------------
+    @classmethod
+    def from_arpa(cls, path, symbols, delimiter=" ", blank=None, oov_penalty=0.0):
+        """Read an ARPA word LM.  symbols[c] is the string of class c (e.g. the reference
+        Preprocessor.int_to_char), blank defaults to the class after the last symbol, delimiter is
+        the symbol of the word boundary.  The lexicon is every unigram word spelled character by
+        character through the classes; n-grams with a word that cannot be spelled are dropped
+        (counted in `dropped`).  ValueError if no word can be spelled (such as an upper-case LM
+        against lower-case symbols)."""
+        num_classes, blank, symbols = _layout(symbols, blank)
+        delim = _delimiter_class(symbols, blank, delimiter)
+        chars = _spelling(symbols, blank, delim)
+        vocab = []
+
+        def vocabulary(unigram_words):
+            reserved = (BOS, EOS, UNK)
+            ws = sorted({w for w in unigram_words if w not in reserved and
+                         all(ch in chars for ch in w)})
+            if not ws:
+                raise ValueError("word LM: no word of %s can be spelled with the classes %r "
+                                 "(a case mismatch?)" % (path, sorted(chars)))
+            vocab.extend(ws)
+            tok = {w: t for t, w in enumerate(ws)}
+            tok.update({BOS: len(ws), EOS: len(ws) + 1, UNK: len(ws) + 2})
+            return tok
+
+        order, ngrams, dropped = _read_arpa(path, vocabulary)
+        return cls(order, vocab, ngrams, symbols, num_classes, blank, delim, oov_penalty, dropped)
+
+    def to_arpa(self, path):
+        """Write an ARPA file that from_arpa reads back to the same LM"""
+        names = self._words + [BOS, EOS, UNK]
+        _write_arpa(path, self._order, self._ngrams, names)
+
+    @classmethod
+    def train(cls, texts, order, symbols, delimiter=" ", blank=None, oov_penalty=0.0):
+        """Interpolated Kneser-Ney (as NGramLM.train) over the whitespace-split words of each text,
+        read as <s> w1 .. wn </s>.  The lexicon is the texts' spellable words; a word that cannot
+        be spelled is read as <unk>, and the unigram level spreads its uniform share over the
+        words, </s> and <unk>, so <unk> always has a unigram."""
+        order = _check_order(order)
+        num_classes, blank, symbols = _layout(symbols, blank)
+        delim = _delimiter_class(symbols, blank, delimiter)
+        chars = _spelling(symbols, blank, delim)
+        texts = [t.split() for t in texts]
+        words = sorted({w for t in texts for w in t if all(ch in chars for ch in w)})
+        if not words:
+            raise ValueError("word LM: no training word can be spelled with the classes %r"
+                             % sorted(chars))
+        W = len(words)
+        tok = {w: t for t, w in enumerate(words)}
+        seqs = [[tok.get(w, W + 2) for w in t] for t in texts]
+        ngrams = _kneser_ney(seqs, order, list(range(W)) + [W + 1, W + 2], W, W + 1)
+        return cls(order, words, ngrams, symbols, num_classes, blank, delim, oov_penalty)
+
+    # ------------------------------------------------------------------------------------------
+    # device tables
+    # ------------------------------------------------------------------------------------------
+    def host_tables(self):
+        """The tables of SbWordLm as numpy arrays (built once): the word n-gram's keys, vals,
+        logp, bow and tok (the identity over the W + 3 tokens) with its scalars, as
+        NGramLM.host_tables; the lexicon map lex_keys (uint64) / lex_vals (int32) of
+        (node, class) -> child node and lex_word (int32, the word token of each node, -1 where
+        none ends there), node 0 the empty word; lex_cap, and the counts."""
+        if self._host is not None:
+            return self._host
+        W = len(self._words)
+        h = _backoff_tables(self._order, self._ngrams, self._bos, self._eos, True)
+        h["tok"] = np.arange(W + 3, dtype=np.int32)
+        child = {}
+        lex_word = [-1]
+        entries = []
+        for w, spelling in enumerate(self._spell):
+            node = 0
+            for c in spelling:
+                nxt = child.get((node, c))
+                if nxt is None:
+                    nxt = child[(node, c)] = len(lex_word)
+                    lex_word.append(-1)
+                    entries.append((_map_key(node, c, 0), nxt))
+                node = nxt
+            lex_word[node] = w
+        h["lex_keys"], h["lex_vals"], h["lex_cap"] = _pack_map(entries)
+        h["lex_word"] = np.array(lex_word, np.int32)
+        self._host = h
+        return h
+
+    def device_tables(self, device):
+        """(SbWordLm ctypes struct, tensors it points into) on `device`, built once per device"""
+        from . import _lib
+        device = _device(device)
+        if device not in self._dev:
+            h = self.host_tables()
+            t = _to_device(h, ("keys", "vals", "logp", "bow", "tok", "lex_keys", "lex_vals",
+                               "lex_word"), device)
+            ng = _lib.SbNgramLm(t["keys"].data_ptr(), t["vals"].data_ptr(), t["logp"].data_ptr(),
+                                t["bow"].data_ptr(), t["tok"].data_ptr(), h["cap"], h["order"],
+                                len(self._words) + 3, h["bos"], -1, h["lm_upper"], h["lm_abs"])
+            st = _lib.SbWordLm(ng, t["lex_keys"].data_ptr(), t["lex_vals"].data_ptr(),
+                               t["lex_word"].data_ptr(), h["lex_cap"], len(self._words),
+                               int(self.has_unk), self._num_classes, self._blank, self._delim)
+            self._dev[device] = (st, t)
+        return self._dev[device]
+
+    def __getstate__(self):
+        d = dict(self.__dict__)
+        d["_dev"] = {}
+        return d
+
+    def __setstate__(self, d):
+        self.__dict__.update(d)
+
+
+def _delimiter_class(symbols, blank, delimiter):
+    """the one class but the blank whose symbol is `delimiter`"""
+    cs = [c for c, s in enumerate(symbols) if c != blank and s == delimiter]
+    if len(cs) != 1:
+        raise ValueError("word LM: %d classes have the delimiter symbol %r (need exactly one)"
+                         % (len(cs), delimiter))
+    return cs[0]
+
+
+def _spelling(symbols, blank, delim):
+    """{character: class} of the one-character symbols but the blank's and the delimiter's"""
+    chars = {}
+    for c, s in enumerate(symbols):
+        if c == blank or c == delim:
+            continue
+        if not isinstance(s, str) or s == "":
+            raise ValueError("word LM: symbol %r of class %d is not a string" % (s, c))
+        if len(s) == 1:
+            if s in chars or s.isspace():
+                raise ValueError("word LM: symbol %r of class %d is a duplicate or whitespace"
+                                 % (s, c))
+            chars[s] = c
+    return chars

@@ -5,10 +5,14 @@
 sb_ctc_prefix_beam (csrc/decode.cu), one CTA per utterance.  `decode_batch` is the batched
 entry CTC.infer uses (the reference loops over utterances in Python, ctc_model.py:59-60).
 
-Both take an optional n-gram LM (speech_b200.lm.NGramLM) for shallow fusion: an extension by
-symbol s scores p_s + (lm_weight * lm(s | prefix) + insertion_bonus) in place of p_s, and the
-returned score is the fused one (sb_ctc_prefix_beam_lm, include/speech_b200.h).  Without an LM
-the calls are the LM-less search.
+Both take an optional n-gram LM for shallow fusion, and the returned score is then the fused one:
+  * speech_b200.lm.NGramLM, over the model's classes: an extension by symbol s scores
+    p_s + (lm_weight * lm(s | prefix) + insertion_bonus) in place of p_s (sb_ctc_prefix_beam_lm);
+  * speech_b200.lm.WordLM, over words (Hannun et al. 2014): the delimiter that ends a word scores
+    p_s + ((lm_weight * lm(word | words) + insertion_bonus) + OOV penalty), so insertion_bonus is
+    per word; a word leaving the lexicon is charged the LM's oov_penalty once, and the end of the
+    utterance adds the trailing word and </s> (sb_ctc_prefix_beam_wordlm, include/speech_b200.h).
+Without an LM the calls are the LM-less search.
 """
 import math
 
@@ -16,6 +20,7 @@ import numpy as np
 import torch
 
 from .. import _lib
+from ..lm import WordLM
 
 
 def check_lm(lm, lm_weight, insertion_bonus, num_classes, blank, search="CTC"):
@@ -25,6 +30,9 @@ def check_lm(lm, lm_weight, insertion_bonus, num_classes, blank, search="CTC"):
         if lm_weight != 0.0 or insertion_bonus != 0.0:
             raise ValueError("lm_weight / insertion_bonus need an lm")
         return
+    if isinstance(lm, WordLM) and search != "CTC":
+        raise ValueError("a word LM fuses into the CTC search only; the %s search takes an NGramLM"
+                         % search)
     if lm.end is not None:
         raise ValueError("the LM reads class %d as </s>; the %s search has no end class"
                          % (lm.end, search))
@@ -43,7 +51,7 @@ def _run(logp, lens, beam_size, blank, lm=None, lm_weight=0.0, insertion_bonus=0
     lib = _lib.load()
     B, T, S = logp.shape
     dev = logp.device
-    if lm is None:
+    if lm is None or isinstance(lm, WordLM):
         nbytes = _lib.workspace_size(lib.sb_ctc_prefix_beam_workspace_size, B, T, beam_size)
     else:
         nbytes = _lib.workspace_size(lib.sb_ctc_prefix_beam_lm_workspace_size, B, T, beam_size,
@@ -59,6 +67,13 @@ def _run(logp, lens, beam_size, blank, lm=None, lm_weight=0.0, insertion_bonus=0
             _lib.check(lib.sb_ctc_prefix_beam(logp.data_ptr(), lens.data_ptr(), B, T, S,
                                               int(beam_size), int(blank), *outs),
                        "sb_ctc_prefix_beam")
+        elif isinstance(lm, WordLM):
+            tables, _ = lm.device_tables(dev)
+            _lib.check(lib.sb_ctc_prefix_beam_wordlm(logp.data_ptr(), lens.data_ptr(), B, T, S,
+                                                     int(beam_size), int(blank), tables,
+                                                     float(lm_weight), float(insertion_bonus),
+                                                     lm.oov_penalty, *outs),
+                       "sb_ctc_prefix_beam_wordlm")
         else:
             tables, _ = lm.device_tables(dev)
             _lib.check(lib.sb_ctc_prefix_beam_lm(logp.data_ptr(), lens.data_ptr(), B, T, S,
@@ -75,7 +90,9 @@ def decode_batch(probs, beam_size=10, blank=0, lens=None, with_scores=False, lm=
                  lm_weight=0.0, insertion_bonus=0.0):
     """probs (B, T, S) post-softmax CUDA tensor -> list of label tuples (one per utterance).
     lm: an NGramLM over the S classes, fused with lm_weight >= 0 and insertion_bonus; the scores
-    (with_scores) are then acoustic + lm_weight * LM + insertion_bonus * length."""
+    (with_scores) are then acoustic + lm_weight * LM + insertion_bonus * length.  Or a WordLM
+    spelled in the S classes: insertion_bonus is then per word, and the scores are acoustic +
+    lm_weight * word LM (</s> included) + insertion_bonus * words + oov_penalty * OOV words."""
     _lib.require_cuda(probs, "probs")
     check_lm(lm, lm_weight, insertion_bonus, probs.shape[-1], blank)
     logp = torch.log(probs.detach().float()).contiguous()

@@ -71,7 +71,9 @@ class CTC(model.Model):
 
     def infer(self, batch, beam_size=1, lm=None, lm_weight=0.0, insertion_bonus=0.0):
         """Best label sequence of each utterance.  lm: an n-gram LM over this model's classes
-        (speech_b200.lm.NGramLM) fused into the beam search with lm_weight and insertion_bonus."""
+        (speech_b200.lm.NGramLM) fused into the beam search with lm_weight and insertion_bonus,
+        or a word n-gram LM spelled in them (speech_b200.lm.WordLM), whose lm_weight scales the
+        word LM and whose insertion_bonus is per word (ctc_decoder)."""
         check_lm(lm, lm_weight, insertion_bonus, self.blank + 1, self.blank)
         x, y, x_lens, y_lens = self._collated(batch)
         lens = self.exact_lens(x_lens)

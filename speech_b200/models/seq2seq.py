@@ -18,6 +18,7 @@ import torch
 import torch.nn as nn
 
 from . import model
+from ..lm import WordLM
 
 
 class Seq2Seq(model.Model):
@@ -274,6 +275,9 @@ class Seq2Seq(model.Model):
             if lm_weight != 0.0 or insertion_bonus != 0.0:
                 raise ValueError("lm_weight / insertion_bonus need an lm")
             return
+        if isinstance(lm, WordLM):
+            raise ValueError("a word LM fuses into the CTC search only; the attention search "
+                             "takes an NGramLM")
         if not (math.isfinite(lm_weight) and lm_weight >= 0.0):
             raise ValueError("lm_weight must be finite and >= 0, got %r" % (lm_weight,))
         if not math.isfinite(insertion_bonus):

@@ -11,7 +11,8 @@ Every stage carries what the next chunk needs and nothing more (EncoderStream, s
   * GRU layers: the input projection, then the recurrence from each stream's carried state
     (sb_gru_fwd_h0); the new state is the fp32 y and bf16 xn at the stream's last new frame.
 CTCStream then runs the fused projection, softmax and log as CTC.infer computes them, and one step
-of the resumable prefix beam search (sb_ctc_stream_step[_lm]), whose beams stay on the device.
+of the resumable prefix beam search (sb_ctc_stream_step[_lm|_wordlm]), whose beams stay on the
+device.
 With B streams, the final partial(return_scores=True) equals decode_batch(with_scores=True) on the
 logits of CTC.infer over the same B utterances in the exact-lengths mode, bit for bit: each stage
 computes the same values as the offline pass.  The recurrence kernel is selected by the number of
@@ -38,6 +39,7 @@ import numpy as np
 import torch
 
 from . import _lib, features, ops
+from .lm import WordLM
 from .models.ctc_decoder import check_lm
 
 MAX_STREAMS = ops.GRU_MAX_BATCH   # one recurrence launch per layer and push
@@ -269,6 +271,13 @@ class CTCStream(EncoderStream):
                 ops._launch("ctc_stream_step", 0.0,
                             lambda: lib.sb_ctc_stream_step(logp.data_ptr(), n.data_ptr(), B, T, S,
                                                            self.K, self.model.blank, *args))
+            elif isinstance(self.lm, WordLM):
+                tables, _ = self.lm.device_tables(self.dev)
+                ops._launch("ctc_stream_step_wordlm", 0.0,
+                            lambda: lib.sb_ctc_stream_step_wordlm(
+                                logp.data_ptr(), n.data_ptr(), B, T, S, self.K, self.model.blank,
+                                tables, self.lm_weight, self.insertion_bonus, self.lm.oov_penalty,
+                                *args))
             else:
                 tables, _ = self.lm.device_tables(self.dev)
                 ops._launch("ctc_stream_step_lm", 0.0,
@@ -278,19 +287,28 @@ class CTCStream(EncoderStream):
 
     def partial(self, return_scores=False):
         """Best label list of each stream so far (one device-to-host copy); with return_scores,
-        (labels, score) pairs, the score as decode_batch(with_scores=True) reports it."""
+        (labels, score) pairs, the score as decode_batch(with_scores=True) reports it.  With a
+        WordLM the stored beams are ranked by the end-of-utterance rule, as if each stream ended
+        here (its partial word completed, then </s>)."""
         lib = _lib.load()
         B, Tm = self.B, self.max_frames
         off = B * Tm + 2 * B + (B * Tm) % 2          # float64 scores 8-byte aligned
         buf = torch.empty(off + 2 * B, dtype=torch.int32, device=self.dev)
         labels, lens, ovf = buf[:B * Tm], buf[B * Tm:B * Tm + B], buf[B * Tm + B:B * Tm + 2 * B]
         scores = buf[off:].view(torch.float64)
+        outs = (labels.data_ptr(), lens.data_ptr(), scores.data_ptr(), ovf.data_ptr(),
+                _lib.stream_ptr())
         with torch.cuda.device(self.dev):
-            ops._launch("ctc_stream_best", 0.0,
-                        lambda: lib.sb_ctc_stream_best(self.state.data_ptr(), B, Tm, self.K,
-                                                       labels.data_ptr(), lens.data_ptr(),
-                                                       scores.data_ptr(), ovf.data_ptr(),
-                                                       _lib.stream_ptr()))
+            if isinstance(self.lm, WordLM):
+                tables, _ = self.lm.device_tables(self.dev)
+                ops._launch("ctc_stream_best_wordlm", 0.0,
+                            lambda: lib.sb_ctc_stream_best_wordlm(
+                                self.state.data_ptr(), B, Tm, self.K, tables, self.lm_weight,
+                                self.insertion_bonus, self.lm.oov_penalty, *outs))
+            else:
+                ops._launch("ctc_stream_best", 0.0,
+                            lambda: lib.sb_ctc_stream_best(self.state.data_ptr(), B, Tm, self.K,
+                                                           *outs))
         host = buf.cpu()
         lab = host[:B * Tm].view(B, Tm).numpy()
         n = host[B * Tm:B * Tm + B].numpy()

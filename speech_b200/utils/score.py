@@ -26,3 +26,26 @@ def compute_cer(results):
     dist = sum(edit_distance(label, pred) for label, pred in results)
     total = sum(len(label) for label, _ in results)
     return dist / total
+
+
+def compute_wer(results, delimiter):
+    """results: list of (ground truth, prediction) label sequence pairs -> word error rate: the
+    total word edit distance divided by the total number of reference words.  A word is a maximal
+    run of labels other than `delimiter` (the space class of a character model)."""
+    def words(seq):
+        out, cur = [], []
+        for v in seq:
+            if v == delimiter:
+                if cur:
+                    out.append(tuple(cur))
+                cur = []
+            else:
+                cur.append(v)
+        if cur:
+            out.append(tuple(cur))
+        return out
+
+    pairs = [(words(label), words(pred)) for label, pred in results]
+    dist = sum(edit_distance(label, pred) for label, pred in pairs)
+    total = sum(len(label) for label, _ in pairs)
+    return dist / total

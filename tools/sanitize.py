@@ -278,3 +278,25 @@ for specs, B, T, F, p in (([[32, 5, 8, 2], [32, 5, 8, 2]], 2, 60, 80, 0.0),
     y = ops.conv_stack(torch.randn(B, T, F, device="cuda"), conv, True)
     y.sum().backward()
     print("direct conv", specs, "dropout", p, sorted(n for n in ops.profile_end() if "direct" in n))
+torch.cuda.synchronize()
+# word-LM fusion: sb_ctc_prefix_beam_wordlm on the full scan (infer) and the forced shortlist
+# route, and a CTC stream stepped with the word LM (stream step and best)
+from speech_b200.lm import WordLM
+wsyms = [chr(ord("a") + i) for i in range(26)] + ["'", " "]
+wlm = WordLM.train(["abc de f", "de abc", "f f abc", "b'c de"], 3, wsyms, oov_penalty=-2.0)
+print("infer with word LM", [len(p) for p in m.infer((inputs, labels), beam_size=4, lm=wlm,
+                                                       lm_weight=0.5, insertion_bonus=1.0)])
+_lib.check(lib.sb_ctc_prefix_beam_wordlm_shortlist(
+    lp.data_ptr(), lens.data_ptr(), 2, 30, 29, 4, 28, ctypes.byref(wlm.device_tables(lp.device)[0]),
+    0.5, 1.0, -2.0, o_lab.data_ptr(), o_len.data_ptr(), o_sc.data_ptr(), ws.data_ptr(), nb.value,
+    _lib.stream_ptr()), "sb_ctc_prefix_beam_wordlm_shortlist")
+print("word LM shortlist route ok", o_len.tolist())
+cs = CTC(80, 28, {"dropout": 0.0, "encoder": {"conv": [[8, 5, 8, 2], [8, 5, 8, 2]],
+                                              "rnn": {"dim": 64, "bidirectional": False,
+                                                      "layers": 2}}}).cuda()
+cs.set_eval()
+st = cs.stream(3, beam_size=4, max_frames=64, lm=wlm, lm_weight=0.5, insertion_bonus=1.0)
+for p, k in ((0, 17), (17, 5), (22, 40)):
+    st.push([x[p:p + k] for x in inputs[:3]])
+print("ctc stream with word LM", st.frames, st.partial(return_scores=True))
+torch.cuda.synchronize()
