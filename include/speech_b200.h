@@ -207,6 +207,39 @@ int sb_gru_plan(int Bp, int H, int ndir, int* Hp);
 int sb_time_align(const void* src, long long ld_src, void* dst, long long ld_dst, const int* lens,
                   int T, int Bp, int cols, int elem_bytes, int right, void* stream);
 
+/* Lookahead (row) convolution above a unidirectional GRU stack (Deep Speech 2, Amodei et al.
+ * 2016, section 3.5), csrc/lookahead.cu:  r[t, b, d] = sum_{j=0..tau} W[j][d] * h[t + j, b, d].
+ * Replaces: nothing in the reference; the model's nn.Conv1d(H, H, tau + 1, groups=H, bias=False)
+ * applied to the right-zero-padded top layer output.
+ *   h      [T*Bp][Hp] f32   top layer output y as sb_gru_fwd writes it (row t*Bp + b)
+ *   w      [tau+1][Hp] f32  taps, tap-major, zero for padded units
+ *   lens   (Bp) int32 valid frames per row (device; clamped to [0, T]) or NULL: T for every row
+ *   r      [T*Bp][Hp] f32 (out, may be NULL), rb [T*Bp][Hp] bf16 (out, may be NULL; not both)
+ * Arithmetic (streaming relies on it to reproduce the offline pass bit for bit):
+ *   - r[t, b, d] for t < len_b is one fp32 FMA chain from 0 over j = 0..tau in ascending order;
+ *   - a term with t + j >= len_b is skipped, not multiplied by zero;
+ *   - r = 0 at t >= len_b, and rb is the round-to-nearest-even bf16 of r.
+ * So r at frame t depends only on h[t .. min(t + tau, len_b - 1)] and on whether len_b cuts the
+ * window: a frame whose whole window lies below len_b has the same bits for any larger len_b.
+ *
+ * sb_lookahead_bwd, from dr = dL/dr [T*Bp][Hp] f32 (read once per tile, like h):
+ *   dh [T*Bp][Hp] f32 (out): dh[t] = sum_j W[j] dr[t - j] over t - j >= 0 (ascending j);
+ *                            dh = 0 at t >= len_b
+ *   dw [tau+1][Hp] f32 (out, overwritten): dW[j][d] = sum over rows b < Bp and t + j < len_b of
+ *                            dr[t, b, d] h[t + j, b, d], reduced deterministically: fixed
+ *                            per-CTA partials in the workspace, then a reduction of fixed shape,
+ *                            so two calls give identical bits
+ *   workspace  >= sb_lookahead_bwd_workspace_size(T, Bp, Hp, tau) bytes, 4-byte aligned
+ * Refusals, before any CUDA call: SB_ERR_INVALID for a NULL required pointer, T < 1, or both
+ * forward outputs NULL; SB_ERR_UNSUPPORTED for tau outside [1, 32], Bp not a multiple of 8 in
+ * [8, 128], or Hp not a positive multiple of 8; SB_ERR_WORKSPACE for a short workspace. */
+int sb_lookahead_fwd(const float* h, const float* w, const int* lens, float* r, void* rb_bf16,
+                     int T, int Bp, int Hp, int tau, void* stream);
+int sb_lookahead_bwd_workspace_size(int T, int Bp, int Hp, int tau, size_t* bytes);
+int sb_lookahead_bwd(const float* dr, const float* h, const float* w, const int* lens, float* dh,
+                     float* dw, void* workspace, size_t workspace_bytes, int T, int Bp, int Hp,
+                     int tau, void* stream);
+
 /* ---------------------------------------------------------------------------------------
  * CTC prefix beam search, one CTA per utterance.
  * Replaces: speech.models.ctc_decoder.decode(probs, beam_size, blank)

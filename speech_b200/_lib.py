@@ -230,6 +230,11 @@ SIGNATURES = {
     "sb_gru_fwd_f32": (_c_int, [_vp, _vp, _vp, _vp, _vp, _c_int, _c_int, _c_int, _c_int, _vp]),
     "sb_time_align": (_c_int, [_vp, _c_ll, _vp, _c_ll, _vp, _c_int, _c_int, _c_int, _c_int, _c_int,
                                _vp]),
+    "sb_lookahead_fwd": (_c_int, [_vp, _vp, _vp, _vp, _vp, _c_int, _c_int, _c_int, _c_int, _vp]),
+    "sb_lookahead_bwd_workspace_size": (_c_int, [_c_int, _c_int, _c_int, _c_int,
+                                                 ctypes.POINTER(_c_sz)]),
+    "sb_lookahead_bwd": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_sz, _c_int, _c_int, _c_int,
+                                  _c_int, _vp]),
     "sb_gru_bwd_workspace_size": (_c_int, [_c_int, _c_int, _c_int, ctypes.POINTER(_c_sz)]),
     "sb_gru_bwd": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_sz, _c_int, _c_int,
                             _c_int, _c_int, _vp]),

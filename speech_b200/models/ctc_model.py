@@ -13,6 +13,7 @@ class CTC(model.Model):
         super().__init__(freq_dim, config)
         self.blank = output_dim                      # blank is the LAST class (ctc_model.py:18)
         self.fc = model.LinearND(self.encoder_dim, output_dim + 1)
+        self._add_lookahead()
 
     def _collated(self, batch):
         """reference-style (inputs, labels) pair, or a loader.StagedBatch prepared ahead of time"""
@@ -49,12 +50,15 @@ class CTC(model.Model):
         if getattr(self, "parity_mode", False) and not torch.is_grad_enabled():
             if lens is not None:
                 raise NotImplementedError("parity_mode does not support exact_lengths")
+            if self.lookahead is not None:
+                raise NotImplementedError("parity_mode does not support a lookahead layer")
             # reference-precision forward (split-bf16 GEMMs, fp32 recurrence): a measuring stick
             # for the bf16 operand path, see ops.encode_logits_parity
             return ops.encode_logits_parity(x, self.conv, self.rnn, self.fc.fc)
         x = ops.conv_stack(x, self.conv, self.training)
         p = self.rnn.dropout if self.training else 0.0
-        return ops.gru_stack_logits(x, self.rnn, self.fc.fc, dropout=p, lens=lens)
+        return ops.gru_stack_logits(x, self.rnn, self.fc.fc, dropout=p, lens=lens,
+                                    lookahead=self.lookahead)
 
     def loss(self, batch):
         x, y, x_lens, y_lens = self._collated(batch)

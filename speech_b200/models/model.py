@@ -24,6 +24,23 @@ class Model(nn.Module):
     # so that pickles written before the key existed read it as False.
     exact_lengths = False
 
+    # Lookahead convolution (config["encoder"]["lookahead"] = tau; absent or 0 by default): Deep
+    # Speech 2's row convolution r[t, d] = sum_{j=0..tau} W[d, j] h[t + j, d] over the top layer
+    # of a unidirectional encoder, so every frame sees tau frames of future context.  Read through
+    # a property of the class, so that pickles written before the key existed read it as None; a
+    # plain class attribute would shadow the registered submodule.
+    @property
+    def lookahead(self):
+        return self._modules.get("lookahead")
+
+    @lookahead.setter
+    def lookahead(self, value):
+        # nn.Module.__setattr__ registers a module value itself; only None, on a model that has
+        # no layer, reaches here
+        if value is not None:
+            raise TypeError("lookahead must be an nn.Conv1d or None, got %r" % (value,))
+        self._modules["lookahead"] = None
+
     def __init__(self, input_dim, config):
         super().__init__()
         self.input_dim = input_dim
@@ -48,6 +65,21 @@ class Model(nn.Module):
         self._encoder_dim = rnn_cfg["dim"]
         self.volatile = False
         self.exact_lengths = bool(config.get("exact_lengths", False))
+        tau = enc.get("lookahead", 0)
+        if isinstance(tau, bool) or not isinstance(tau, int) or not 0 <= tau <= 32:
+            raise ValueError("encoder lookahead must be an int in [0, 32], got %r" % (tau,))
+        if tau > 0 and rnn_cfg["bidirectional"]:
+            raise ValueError("encoder lookahead needs a unidirectional encoder: a bidirectional "
+                             "one already sees the whole utterance")
+        self._lookahead_tau = tau
+
+    def _add_lookahead(self):
+        """Each family calls this after creating all its other modules, so that with the same
+        seed a model with a lookahead initialises every other parameter as one without."""
+        tau = self._lookahead_tau
+        if tau > 0:
+            H = self.encoder_dim
+            self.lookahead = nn.Conv1d(H, H, tau + 1, groups=H, bias=False)
 
     # reference: model.py:44-52 (valid convolution, ceil((n - k + 1) / s) per layer)
     def conv_out_size(self, n, dim):
@@ -73,7 +105,8 @@ class Model(nn.Module):
         _lib.require_cuda(x, "encode() input")
         x = ops.conv_stack(x, self.conv, self.training)          # (B, T', C*F') c-major features
         p = self.rnn.dropout if self.training else 0.0
-        x = ops.gru_stack(x, self.rnn, dropout=p, lens=lens)     # (B, T', ndir*H)
+        x = ops.gru_stack(x, self.rnn, dropout=p, lens=lens,     # (B, T', ndir*H)
+                          lookahead=self.lookahead)
         if self.rnn.bidirectional:
             half = x.shape[-1] // 2
             x = x[:, :, :half] + x[:, :, half:]

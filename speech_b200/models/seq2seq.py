@@ -47,6 +47,7 @@ class Seq2Seq(model.Model):
             # a seed; classes 0..V-3 are the labels, V-2 the blank (END and START never occur)
             self.ctc_weight = float(w)
             self.ctc_fc = model.LinearND(rnn_dim, vocab_size - 1)
+        self._add_lookahead()
 
     def set_eval(self):
         self.eval()

@@ -36,6 +36,7 @@ class Transducer(model.Model):
         self.blank = vocab_size                       # blank is the LAST class (:28)
         self.fc1 = model.LinearND(rnn_dim, rnn_dim)
         self.fc2 = model.LinearND(rnn_dim, vocab_size + 1)
+        self._add_lookahead()
 
     def forward(self, batch):
         x, y, x_lens, y_lens = self.collate(*batch)

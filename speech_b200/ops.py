@@ -499,10 +499,13 @@ class GRUStackFunction(torch.autograd.Function):
     """
 
     @staticmethod
-    def forward(ctx, x, ndir, H, dropout, fc_w, fc_b, lens, *weights):
+    def forward(ctx, x, ndir, H, dropout, fc_w, fc_b, lens, la_w, *weights):
         """fc_w/fc_b (optional): fuse `LinearND(sum of direction halves)` (reference
         model.py:75-77 + ctc_model.py:29) as ONE contraction on the bf16 top-layer output:
-        (h_f + h_b) W^T = [h_f | h_b] [W | W]^T, written batch-first by the GEMM epilogue."""
+        (h_f + h_b) W^T = [h_f | h_b] [W | W]^T, written batch-first by the GEMM epilogue.
+        la_w (optional, ndir = 1 only): the (H, 1, tau + 1) weight of a lookahead convolution
+        over the top layer's output (sb_lookahead_fwd, exact-lengths `lens` honoured); the fused
+        projection then reads its bf16 output, and the unfused path returns its fp32 output."""
         _lib.require_cuda(x, "x")
         lib = _lib.load()
         B, T, In = x.shape
@@ -518,6 +521,7 @@ class GRUStackFunction(torch.autograd.Function):
         need_grad = any(ctx.needs_input_grad)     # all False under torch.no_grad()
         lo = _lens_operands(lens, B, T, Bp, dev)
         al, valid = lo if lo is not None else (None, None)
+        la_lens = al
         if ndir == 1:
             al = None                             # the forward direction is causal
 
@@ -573,6 +577,21 @@ class GRUStackFunction(torch.autograd.Function):
             if need_grad:
                 saved.append((X, y_rec, gates, mask, wih_cat, whh, hb))
             X = xn
+        ctx.la = None
+        if la_w is not None:
+            # r over the top layer's fp32 states as the recurrence wrote them; frames >= len_b
+            # of each utterance are never read
+            tau = la_w.shape[2] - 1
+            taps = lookahead_taps(la_w, H, Hp)
+            r = None if fc_w is not None else torch.empty(M, Hp, dtype=torch.float32, device=dev)
+            rb = torch.empty(M, Hp, dtype=torch.bfloat16, device=dev) if fc_w is not None else None
+            lookahead_fwd(y_rec, taps, la_lens, r, rb, T, Bp, Hp, tau)
+            if need_grad:
+                ctx.la = (la_w, taps, la_lens, y_rec, tau)
+            if fc_w is not None:
+                X = rb
+            else:
+                y = r
         ctx.saved = saved
         ctx.announce = _announce
         ctx.weights = weights
@@ -631,6 +650,12 @@ class GRUStackFunction(torch.autograd.Function):
             dY = torch.zeros(T, Bp, D, dtype=torch.float32, device=dev)
             dY[:, :B] = pad_blocks(dout.transpose(0, 1), 2, ndir, H, Hp)
             dY = dY.view(M, D)
+        dla = None
+        if ctx.la is not None:
+            la_w, taps, la_lens, h_top, tau = ctx.la
+            dY, dla = lookahead_bwd(dY.contiguous(), h_top, taps, la_lens, T, Bp, Hp, tau)
+            dla = dla[:, :H].t().reshape(la_w.shape)
+            ctx.la = None
         nbytes = _lib.workspace_size(lib.sb_gru_bwd_workspace_size, Bp, Hp, ndir)
         ws = _workspace(nbytes, dev)
         grads = [None] * len(weights)
@@ -732,7 +757,46 @@ class GRUStackFunction(torch.autograd.Function):
         if ctx.needs_input_grad[0]:
             dx = dY.view(T, Bp, -1)[:, :B, :In].transpose(0, 1).contiguous()
         ctx.saved = None
-        return (dx, None, None, None, dfc_w, dfc_b, None) + tuple(grads)
+        return (dx, None, None, None, dfc_w, dfc_b, None, dla) + tuple(grads)
+
+
+def lookahead_taps(la_w, H, Hp):
+    """(H, 1, tau + 1) lookahead weight -> the kernels' [tau + 1][Hp] f32 taps (padded units 0)"""
+    taps = la_w.detach().float().reshape(H, -1).t()
+    return pad_blocks(taps, 1, 1, H, Hp).contiguous()
+
+
+def lookahead_fwd(h, taps, lens_dev, r, rb, T, Bp, Hp, tau):
+    """sb_lookahead_fwd of the time-major [T*Bp][Hp] f32 h into r (f32) and / or rb (bf16)"""
+    lib = _lib.load()
+    sp = _lib.stream_ptr()
+    _launch("lookahead_fwd", 2.0 * T * Bp * Hp * (tau + 1),
+            lambda: lib.sb_lookahead_fwd(h.data_ptr(), taps.data_ptr(), _lib.ptr(lens_dev),
+                                         _lib.ptr(r), _lib.ptr(rb), T, Bp, Hp, tau, sp))
+
+
+def lookahead_bwd(dr, h, taps, lens_dev, T, Bp, Hp, tau):
+    """sb_lookahead_bwd: -> (dh [T*Bp][Hp] f32, dW [tau + 1][Hp] f32)"""
+    lib = _lib.load()
+    dev = dr.device
+    dh = torch.empty(T * Bp, Hp, dtype=torch.float32, device=dev)
+    dw = torch.empty(tau + 1, Hp, dtype=torch.float32, device=dev)
+    nbytes = _lib.workspace_size(lib.sb_lookahead_bwd_workspace_size, T, Bp, Hp, tau)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    sp = _lib.stream_ptr()
+    _launch("lookahead_bwd", 4.0 * T * Bp * Hp * (tau + 1),
+            lambda: lib.sb_lookahead_bwd(dr.data_ptr(), h.data_ptr(), taps.data_ptr(),
+                                         _lib.ptr(lens_dev), dh.data_ptr(), dw.data_ptr(),
+                                         ws.data_ptr(), nbytes, T, Bp, Hp, tau, sp))
+    return dh, dw
+
+
+def _lookahead_weight(rnn, lookahead):
+    if lookahead is None:
+        return None
+    if rnn.bidirectional:
+        raise ValueError("a lookahead convolution needs a unidirectional GRU stack")
+    return lookahead.weight
 
 
 def _gru_weights(rnn):
@@ -767,23 +831,28 @@ def _batch_chunks(x, lens, fn):
         _announce = True
 
 
-def gru_stack_logits(x, rnn, fc, dropout=0.0, lens=None):
+def gru_stack_logits(x, rnn, fc, dropout=0.0, lens=None, lookahead=None):
     """GRU stack + sum of direction halves + output projection `fc` (an nn.Linear), fused:
     returns logits (B, T, V) - the encoder tail of CTC.forward_impl (ctc_model.py:25-32).
     lens (optional): valid frames per utterance (GRUStackFunction); logits are exact at frames
-    < lens[b]."""
+    < lens[b].  lookahead (optional, unidirectional rnn): the model's lookahead nn.Conv1d, run
+    between the top layer and fc."""
     ndir, weights = _gru_weights(rnn)
+    la_w = _lookahead_weight(rnn, lookahead)
     return _batch_chunks(x, lens, lambda xc, lc: GRUStackFunction.apply(
-        xc, ndir, rnn.hidden_size, float(dropout), fc.weight, fc.bias, lc, *weights))
+        xc, ndir, rnn.hidden_size, float(dropout), fc.weight, fc.bias, lc, la_w, *weights))
 
 
-def gru_stack(x, rnn, dropout=0.0, lens=None):
+def gru_stack(x, rnn, dropout=0.0, lens=None, lookahead=None):
     """Run the sm_90a GRU stack with the parameters of an nn.GRU module (batch_first, h0 = 0).
     lens (optional): valid frames per utterance, as nn.GRU over pack_padded_sequence followed by
-    pad_packed_sequence (GRUStackFunction)."""
+    pad_packed_sequence (GRUStackFunction).  lookahead (optional, unidirectional rnn): an
+    nn.Conv1d(H, H, tau + 1, groups=H, bias=False) over the top layer's output, zero-padded by
+    tau frames on the right (by lens[b] frames' end in the exact-lengths mode)."""
     ndir, weights = _gru_weights(rnn)
+    la_w = _lookahead_weight(rnn, lookahead)
     return _batch_chunks(x, lens, lambda xc, lc: GRUStackFunction.apply(
-        xc, ndir, rnn.hidden_size, float(dropout), None, None, lc, *weights))
+        xc, ndir, rnn.hidden_size, float(dropout), None, None, lc, la_w, *weights))
 
 
 _direct_ok = {}

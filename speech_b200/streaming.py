@@ -19,6 +19,14 @@ computes the same values as the offline pass.  The recurrence kernel is selected
 batch rows, so against an offline batch of another size the results agree only to the GRU's
 rounding tolerance.
 
+With a lookahead layer (config["encoder"]["lookahead"] = tau) a stream holds back, per stream, the
+top layer's fp32 states of its last <= tau frames (`pending`): a push runs sb_lookahead_fwd over
+[pending | new frames] with len_b = pending_b + n_b and searches the first
+max(0, pending_b + n_b - tau) of them, whose windows lie wholly below len_b and so carry the bits of
+the offline pass.  finish() runs the lookahead over the pending frames alone (len_b = pending_b),
+so the trailing frames see zeros as in the offline exact-lengths pass, and searches them; a
+finished stream takes no more frames until it is reset.  `frames` counts the frames searched.
+
 TransducerStream runs fc1 on the top layer's bf16 xn of the new frames (the wgmma GEMM with the
 padded weights of transducer_model.PredictionNet, as the offline ops.linear does on the same
 values), then Transducer.recognize's label-free search resumed over them
@@ -43,6 +51,15 @@ from .lm import WordLM
 from .models.ctc_decoder import check_lm
 
 MAX_STREAMS = ops.GRU_MAX_BATCH   # one recurrence launch per layer and push
+
+
+def lookahead_counts(pending, counts, tau, ends=()):
+    """With a lookahead of tau frames: the frames each stream searches, and the frames it holds
+    back, after counts[b] new encoder frames join its pending[b] ones.  A frame is searched once
+    its tau future frames are there, or when its stream ends (streams in `ends`)."""
+    tot = [p + n for p, n in zip(pending, counts)]
+    emit = [n if b in ends else max(0, n - tau) for b, n in enumerate(tot)]
+    return emit, [n - e for n, e in zip(tot, emit)]
 
 
 class EncoderStream:
@@ -93,11 +110,24 @@ class EncoderStream:
         self.carry = [None] * B                  # input frames from next_b * stride on
         self.pcm = [np.zeros(0, np.int16) for _ in range(B)]    # push_audio's carried samples
         self.next = [0] * B                      # encoder frames produced per stream
+        self.done = [False] * B                  # finished streams (until reset)
+        la = model.lookahead
+        self.tau = 0 if la is None else la.kernel_size[0] - 1
+        self.npend = [0] * B                     # top-layer frames held back for the lookahead
+        if self.tau:
+            with torch.no_grad():
+                self.taps = ops.lookahead_taps(la.weight, H, Hp)
+            self.pend = torch.zeros(B * self.tau, Hp, dtype=torch.float32, device=dev)
 
     @property
     def frames(self):
-        """encoder frames consumed per stream; frame t starts at input frame t * prod(strides)"""
-        return list(self.next)
+        """encoder frames searched per stream; frame t starts at input frame t * prod(strides)"""
+        return [n - p for n, p in zip(self.next, self.npend)]
+
+    @property
+    def pending(self):
+        """encoder frames per stream held back until the lookahead's future frames arrive"""
+        return list(self.npend)
 
     def _reset_encoder(self, b):
         b = int(b)
@@ -106,6 +136,8 @@ class EncoderStream:
         self.carry[b] = None
         self.pcm[b] = np.zeros(0, np.int16)
         self.next[b] = 0
+        self.done[b] = False
+        self.npend[b] = 0
         for h, hb in zip(self.h, self.hb):
             h[b].zero_()
             hb[b].zero_()
@@ -143,8 +175,8 @@ class EncoderStream:
             self.next[b] += n
 
     def _encoder(self, xs, counts, T):
-        """(T * Bp, Hp) bf16 xn of the top GRU layer at the new encoder frames (frame t of stream b
-        at row t * Bp + b; rows past counts[b] unused)"""
+        """(T * Bp, Hp) bf16 xn and f32 y of the top GRU layer at the new encoder frames (frame t
+        of stream b at row t * Bp + b; rows past counts[b] unused)"""
         lib = _lib.load()
         B, Bp, Hp, dev = self.B, self.Bp, self.Hp, self.dev
         L = max(x.shape[0] for x in xs)
@@ -172,7 +204,81 @@ class EncoderStream:
             h.copy_(y[last])
             hb.copy_(xn[last])
             X = xn[Bp:]
-        return X
+        return X, y[Bp:]
+
+    def _lookahead(self, Y, counts, T, ends):
+        """The lookahead over [pending | counts[b] new frames of Y] of every stream, len_b their
+        sum: -> (frames to search per stream, Te, (Te * Bp, Hp) bf16 operand of the projection).
+        A stream of `ends` searches all its frames, any other the frames whose window is complete;
+        the rest become its new pending frames."""
+        B, Bp, Hp, tau, dev = self.B, self.Bp, self.Hp, self.tau, self.dev
+        tot = [p + n for p, n in zip(self.npend, counts)]
+        Tl = max(tot)
+        emit, keep = lookahead_counts(self.npend, counts, tau, ends)
+        # one gather from [pending rows | Y rows | a zero row]
+        zero = B * tau + T * Bp
+        idx = np.full((Tl, Bp), zero, np.int64)
+        for b in range(B):
+            p = self.npend[b]
+            idx[:p, b] = b * tau + np.arange(p)
+            idx[p:tot[b], b] = B * tau + np.arange(counts[b]) * Bp + b
+        parts = [self.pend] + ([Y[:T * Bp]] if T else []) + [self.pend.new_zeros(1, Hp)]
+        src = torch.cat(parts)
+        h = src[torch.from_numpy(idx.reshape(-1)).to(dev)]
+        lens = torch.tensor(tot + [0] * (Bp - B), dtype=torch.int32).to(dev)
+        rb = torch.empty(Tl * Bp, Hp, dtype=torch.bfloat16, device=dev)
+        ops.lookahead_fwd(h, self.taps, lens, None, rb, Tl, Bp, Hp, tau)
+        pidx = np.full((B, tau), Tl * Bp, np.int64)
+        for b in range(B):
+            pidx[b, :keep[b]] = (emit[b] + np.arange(keep[b])) * Bp + b
+        self.npend = keep
+        self.pend = torch.cat([h, h.new_zeros(1, Hp)])[torch.from_numpy(pidx.reshape(-1)).to(dev)]
+        Te = max(emit)
+        return emit, Te, rb[:Te * Bp]
+
+    def push(self, chunks):
+        """Feed one (n_b, F) chunk of feature frames to every stream (n_b may be 0; a finished
+        stream takes none): runs the encoder over the encoder frames the chunks complete and
+        advances each stream's search over the frames it can search.  -> encoder frames completed
+        per stream."""
+        xs, counts = self._conv_inputs(chunks)
+        for b, c in enumerate(chunks):
+            if self.done[b] and len(c) > 0:
+                raise ValueError("stream %d is finished: reset(%d) before pushing to it" % (b, b))
+        T = max(counts)
+        if T > 0:
+            with torch.no_grad():
+                emit, Te, X = self._encode(xs, counts, T)
+                if Te > 0:
+                    self._decode(X, emit, Te)
+        self._advance(xs, counts)
+        return counts
+
+    def _encode(self, xs, counts, T):
+        """The encoder over counts[b] new encoder frames per stream (T = max(counts) > 0), and the
+        lookahead if the model has one: -> (frames to search per stream, Te = their maximum,
+        (Te * Bp, Hp) bf16 operand of the output projection, frame t of stream b at row
+        t * Bp + b)"""
+        X, Y = self._encoder(xs, counts, T)
+        if not self.tau:
+            return counts, T, X
+        return self._lookahead(Y, counts, T, ())
+
+    def finish(self, streams=None):
+        """End the listed streams (all when None): search their pending frames, the lookahead
+        seeing zeros past each utterance's end, and refuse further frames until reset(b).
+        Finishing a finished stream does nothing."""
+        bs = range(self.B) if streams is None else [int(b) for b in streams]
+        for b in bs:
+            if not 0 <= b < self.B:
+                raise ValueError("stream %d out of range [0, %d)" % (b, self.B))
+        ends = {b for b in bs if not self.done[b]}
+        if self.tau and any(self.npend[b] for b in ends):
+            with torch.no_grad():
+                emit, Te, X = self._lookahead(None, [0] * self.B, 0, ends)
+                self._decode(X, emit, Te)
+        for b in ends:
+            self.done[b] = True
 
     def push_audio(self, pcm, sample_rate=16000, mean=None, std=None, window_size=20, step_size=10,
                    eps=1e-10):
@@ -189,6 +295,8 @@ class EncoderStream:
             a = np.asarray(a)
             if a.dtype != np.int16 or a.ndim != 1:
                 raise ValueError("push_audio expects 1-D int16 arrays")
+            if self.done[b] and a.size > 0:
+                raise ValueError("stream %d is finished: reset(%d) before pushing to it" % (b, b))
             audio.append(np.concatenate([self.pcm[b], a]))
         nf = [features.frame_count(len(a), nperseg, step) for a in audio]
         if max(nf) > 0:
@@ -234,25 +342,16 @@ class CTCStream(EncoderStream):
                                                         _lib.stream_ptr()))
 
     def reset(self, b):
-        """start slot b afresh: conv carry, GRU states and search"""
+        """start slot b afresh: conv carry, GRU states, pending frames and search"""
         self._reset_search(self._reset_encoder(b), 1)
 
-    def push(self, chunks):
-        """Feed one (n_b, F) chunk of feature frames to every stream (n_b may be 0): runs the
-        encoder over the encoder frames the chunks complete and advances each stream's search."""
-        xs, counts = self._conv_inputs(chunks)
-        T = max(counts)
-        if T > 0:
-            with torch.no_grad():
-                logp = self._encode(xs, counts, T)
-            self._search(logp, counts)
-        self._advance(xs, counts)
-        return counts
+    def _decode(self, X, counts, T):
+        self._search(self._logp(X, T), counts)
 
-    def _encode(self, xs, counts, T):
-        """(B, T, S) log-probabilities of the new encoder frames (rows past counts[b] unused)"""
+    def _logp(self, X, T):
+        """(B, T, S) log-probabilities of the (T * Bp, Hp) bf16 top-layer operand X (rows past
+        each stream's frames unused)"""
         B, Bp = self.B, self.Bp
-        X = self._encoder(xs, counts, T)
         out = ops.gemm_bf16_tn(X, self.fc_w, bias=self.fc_b, remap=(Bp, T, B))
         out = out.view(B, T, -1)
         # CTC.infer: softmax over the classes, then decode_batch's float32 log
@@ -338,27 +437,19 @@ class TransducerStream(EncoderStream):
                                    model.blank, max_len, lm, lm_weight, insertion_bonus)
 
     def reset(self, b):
-        """start slot b afresh: conv carry, GRU states, search and its prediction states"""
+        """start slot b afresh: conv carry, GRU states, pending frames, search and its prediction
+        states"""
         self.search.reset(self._reset_encoder(b))
 
-    def push(self, chunks):
-        """Feed one (n_b, F) chunk of feature frames to every stream (n_b may be 0): runs the
-        encoder over the encoder frames the chunks complete and advances each stream's search."""
-        xs, counts = self._conv_inputs(chunks)
-        T = max(counts)
-        if T > 0:
-            with torch.no_grad():
-                self._encode(xs, counts, T)
-            self.search.push(counts)
-        self._advance(xs, counts)
-        return counts
+    def _decode(self, X, counts, T):
+        self._fc1(X, T)
+        self.search.push(counts)
 
-    def _encode(self, xs, counts, T):
-        """fc1 of the new encoder frames into the prediction network's fxT: (T, Bp, Hj), frame t
-        of stream b at [t, b].  xn's columns H .. Kr - 1 are zero (padded GRU units stay 0), as
-        the offline ops.linear's zero padding of bf16(y)."""
-        X = self._encoder(xs, counts, T)[:, :self.Kr]
-        fx = ops.gemm_bf16_tn(X, self.pred.w1, bias=self.pred.b1)
+    def _fc1(self, X, T):
+        """fc1 of the (T * Bp, Hp) bf16 top-layer operand X into the prediction network's fxT:
+        (T, Bp, Hj), frame t of stream b at [t, b].  X's columns H .. Kr - 1 are zero (padded GRU
+        units and lookahead taps stay 0), as the offline ops.linear's zero padding of bf16(y)."""
+        fx = ops.gemm_bf16_tn(X[:, :self.Kr], self.pred.w1, bias=self.pred.b1)
         self.pred.fxT = fx.view(T, self.Bp, -1)
 
     def partial(self, return_scores=False):

@@ -51,9 +51,11 @@ def run_stream(st, feats, chunk):
         e = events()
         e[0].record()
         with torch.no_grad():
-            logp = st._encode(xs, counts, T)
+            emit, Te, X = st._encode(xs, counts, T)
+            logp = st._logp(X, Te) if Te else None
         e[1].record()
-        st._search(logp, counts)
+        if Te:
+            st._search(logp, emit)
         e[2].record()
         e[2].synchronize()
         st._advance(xs, counts)

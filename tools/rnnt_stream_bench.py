@@ -69,9 +69,12 @@ def run_stream(st, feats, chunk, frames):
         e = events()
         e[0].record()
         with torch.no_grad():
-            st._encode(xs, counts, T)
+            emit, Te, X = st._encode(xs, counts, T)
+            if Te:
+                st._fc1(X, Te)
         e[1].record()
-        st.search.push(counts)
+        if Te:
+            st.search.push(emit)
         e[2].record()
         e[2].synchronize()
         st._advance(xs, counts)
