@@ -692,6 +692,61 @@ int sb_s2s_beam_select_split_lm_batch(const float* logp, void* state, double* c_
                                       size_t workspace_bytes, const SbNgramLm* lm,
                                       double lm_weight, double insertion_bonus, void* stream);
 
+/* Attention beam search with a word n-gram LM (SbWordLm below): the CTC word-LM contract moved onto
+ * the attention search's candidates.
+ *   sb_s2s_beam_select_wordlm_batch        sb_s2s_beam_select_batch with the LM, its three weights
+ *                                          and word_nodes
+ *   sb_s2s_beam_select_split_wordlm_batch  sb_s2s_beam_select_split_batch with the same
+ *   sb_s2s_ctc_candidates_wordlm           sb_s2s_ctc_candidates with the same (joint search)
+ * Candidate (r, c), live row r extended by class c, with p = (double)logp[r][c] and score_r the
+ * row's float64 score, is valued (float64, in this order):
+ *   c the delimiter, n_r = 0:      score_r + p (leading and repeated delimiters are free);
+ *   c the delimiter, n_r != 0:     score_r + (p + d_r), d_r = (lm_weight * lm(w | hist_r) +
+ *       insertion_bonus) + g_r exactly as in the CTC search: w the word at n_r, or <unk>; g_r =
+ *       oov_penalty where n_r >= 1 is not a word, else 0;
+ *   c = end_tok:                   score_r + (p + t_r), t_r = e_r + lm_weight * lm(</s> | hist'_r),
+ *       e_r = d_r, or 0.0 for an empty partial word, hist'_r the history with the trailing word
+ *       (the CTC search's end-of-utterance term);
+ *   any other c, n_r >= 0 with no lexicon child c:  score_r + (p + oov_penalty), the new row's node
+ *       -1;
+ *   any other c otherwise:         score_r + p.
+ * n_r is row r's lexicon node (0 the empty partial word; -1 the partial word has left the lexicon,
+ * its OOV penalty already charged); hist_r its last order-1 completed words, <s> before the first;
+ * the start token begins the history and spells nothing.  The fused value is the hypothesis score
+ * everywhere after: selection, the "first K may complete" rule, the stop rule, the chosen
+ * hypothesis and the returned score, which for a completed hypothesis is acoustic + lm_weight *
+ * (word LM with </s>) + insertion_bonus * words + oov_penalty * OOV words; a hypothesis returned
+ * live at max_len has no end term.  With lm_weight = insertion_bonus = oov_penalty = 0 the results
+ * equal the LM-less entry points' bit for bit.  Candidates valued -inf (oov_penalty = -inf) are
+ * ordinary values under the usual tie order.  In the joint search the LM part of P(r, c) is the
+ * term above (d_r, t_r, oov_penalty or 0) in place of lm_weight * lm(c | h_r) + beta_c.
+ * The LM's classes are the model's: lm->blank is the start token, no class the search scores, and
+ * end_tok is the LM's end class (speech_b200.lm.WordLM with `end` builds such tables).
+ * word_nodes: device int32 [B][node_cap][3], parallel to nodes, no initial contents needed: each
+ * step writes the word state of every live row's node (lexicon node, last completed word token or
+ * -1, a node holding the words before it), computed from its parent's with at most one lexicon
+ * probe, and reads the history up those links; a row's cost is O(order) probes, independent of the
+ * length of its words.  The same buffer must serve every step of a search.
+ * SB_ERR_INVALID for a null table or word_nodes, lm_weight < 0 or not finite, insertion_bonus not
+ * finite, oov_penalty > 0 or NaN, oov_penalty != -inf without <unk>, lm->num_classes < C, lm->blank
+ * in [0, C), a delimiter outside [0, C) or equal to end_tok, a cap that is not a power of two, or
+ * order < 1; SB_ERR_UNSUPPORTED for order > SB_LM_MAX_ORDER or K > 32; otherwise as the LM-less
+ * entry points.  All before any CUDA call. */
+int sb_s2s_beam_select_wordlm_batch(const float* logp, void* state, double* c_scores, int* nodes,
+                                    int* parent_row, int* tok_next, int* out_tokens, int K, int C,
+                                    int end_tok, int step, int max_len, int node_cap, int c_cap,
+                                    int* stop, int B, const SbWordLm* lm, double lm_weight,
+                                    double insertion_bonus, double oov_penalty, int* word_nodes,
+                                    void* stream);
+int sb_s2s_beam_select_split_wordlm_batch(const float* logp, void* state, double* c_scores,
+                                          int* nodes, int* parent_row, int* tok_next,
+                                          int* out_tokens, int K, int C, int end_tok, int step,
+                                          int max_len, int node_cap, int c_cap, int* stop, int B,
+                                          void* workspace, size_t workspace_bytes,
+                                          const SbWordLm* lm, double lm_weight,
+                                          double insertion_bonus, double oov_penalty,
+                                          int* word_nodes, void* stream);
+
 /* Joint CTC/attention decoding of the attention model (Watanabe et al. 2017, Algorithm 2;
  * csrc/s2s_ctc.cu): the batched beam search above with the CTC prefix scores of a CTC head.
  * y (B, T, C) float32: the head's log-probabilities, C = the decoder's classes, blank C - 1, which
@@ -736,6 +791,13 @@ int sb_s2s_ctc_candidates(const float* logp, const float* ctc_logp, const int* l
                           int end_tok, double ctc_weight, int step, const int* stop, int B,
                           const SbNgramLm* lm, double lm_weight, double insertion_bonus,
                           void* stream);
+int sb_s2s_ctc_candidates_wordlm(const float* logp, const float* ctc_logp, const int* lens,
+                                 const void* state, const int* nodes, int node_cap,
+                                 void* ctc_state, size_t ctc_state_bytes, int K, int C, int M,
+                                 int T, int start_tok, int end_tok, double ctc_weight, int step,
+                                 const int* stop, int B, const SbWordLm* lm, double lm_weight,
+                                 double insertion_bonus, double oov_penalty, int* word_nodes,
+                                 void* stream);
 int sb_s2s_ctc_select_batch(const float* ctc_logp, const int* lens, void* ctc_state,
                             size_t ctc_state_bytes, void* state, double* c_scores, int* nodes,
                             int* parent_row, int* tok_next, int* out_tokens, int K, int C, int M,

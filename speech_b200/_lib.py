@@ -148,12 +148,23 @@ SIGNATURES = {
     "sb_s2s_beam_select_split_lm_batch": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_int,
                                                    _c_int, _c_int, _c_int, _c_int, _c_int, _c_int,
                                                    _vp, _c_int, _vp, _c_sz, _lmp, _db, _db, _vp]),
+    "sb_s2s_beam_select_wordlm_batch": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_int,
+                                                 _c_int, _c_int, _c_int, _c_int, _c_int, _c_int,
+                                                 _vp, _c_int, _wlmp, _db, _db, _db, _vp, _vp]),
+    "sb_s2s_beam_select_split_wordlm_batch": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_int,
+                                                       _c_int, _c_int, _c_int, _c_int, _c_int,
+                                                       _c_int, _vp, _c_int, _vp, _c_sz, _wlmp,
+                                                       _db, _db, _db, _vp, _vp]),
     "sb_s2s_ctc_state_size": (_c_int, [_c_int, _c_int, _c_int, _c_int, ctypes.POINTER(_c_sz)]),
     "sb_s2s_ctc_init": (_c_int, [_vp, _vp, _vp, _c_sz, _c_int, _c_int, _c_int, _c_int, _c_int,
                                  _c_int, _db, _c_int, _vp]),
     "sb_s2s_ctc_candidates": (_c_int, [_vp, _vp, _vp, _vp, _vp, _c_int, _vp, _c_sz, _c_int,
                                        _c_int, _c_int, _c_int, _c_int, _c_int, _db, _c_int, _vp,
                                        _c_int, _lmp, _db, _db, _vp]),
+    "sb_s2s_ctc_candidates_wordlm": (_c_int, [_vp, _vp, _vp, _vp, _vp, _c_int, _vp, _c_sz,
+                                              _c_int, _c_int, _c_int, _c_int, _c_int, _c_int, _db,
+                                              _c_int, _vp, _c_int, _wlmp, _db, _db, _db, _vp,
+                                              _vp]),
     "sb_s2s_ctc_select_batch": (_c_int, [_vp, _vp, _vp, _c_sz, _vp, _vp, _vp, _vp, _vp, _vp,
                                          _c_int, _c_int, _c_int, _c_int, _c_int, _c_int, _db,
                                          _c_int, _c_int, _c_int, _c_int, _vp, _c_int, _vp]),

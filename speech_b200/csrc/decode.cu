@@ -132,43 +132,11 @@ __device__ __forceinline__ WordShared& word_shared() {
   return sh;
 }
 
-struct WordLmFuse {
+struct WordLmFuse : WordTerms {
   static constexpr bool kLm = false;
   static constexpr bool kWord = true;
   static constexpr int kMinBlocks = 1;
-  SbWordLm lm;
-  double alpha, beta, gamma;
 
-  // the lexicon child of node (>= 0) by class s, -1 where there is none
-  __device__ __forceinline__ int child(int node, int s) const {
-    return map_find(LexMap{lm.lex_keys, lm.lex_vals, lm.lex_cap}, node, s, 0);
-  }
-  // the token of the word a delimiter ends at node (!= 0): the node's word or <unk>
-  __device__ __forceinline__ int word_tok(int node) const {
-    const int w = node > 0 ? __ldg(lm.lex_word + node) : -1;
-    return w >= 0 ? w : lm.ngram.bos + 2;
-  }
-  // the delimiter term of node (!= 0) against a history read by older (lm_context); ctx scratch
-  template <class Older>
-  __device__ __forceinline__ double dterm(int node, Older&& older, int* ctx) const {
-    const int w = node > 0 ? __ldg(lm.lex_word + node) : -1;
-    const double g = (node > 0 && w < 0) ? gamma : 0.0;   // an OOV word not charged yet
-    const int d = lm_context(lm.ngram, older, ctx);
-    return (alpha * lm_backoff(lm.ngram, ctx, d, w >= 0 ? w : lm.ngram.bos + 2) + beta) + g;
-  }
-  // e_i + alpha * lm(</s> | ctx'_i) of an entry at node with the history older
-  template <class Older>
-  __device__ __forceinline__ double end_term(int node, Older&& older, int* ctx) const {
-    const int eos = lm.ngram.bos + 1;
-    if (node == 0) {
-      const int d = lm_context(lm.ngram, older, ctx);
-      return 0.0 + alpha * lm_backoff(lm.ngram, ctx, d, eos);
-    }
-    const double e = dterm(node, older, ctx);
-    const int w = word_tok(node);
-    const int d = lm_context(lm.ngram, [&](int k) { return k == 0 ? w : older(k - 1); }, ctx);
-    return e + alpha * lm_backoff(lm.ngram, ctx, d, eos);
-  }
   __device__ __forceinline__ double q(int i, int s, double p) const {
     const WordShared& ws = word_shared();
     const int node = ws.node[i];
@@ -1130,27 +1098,9 @@ extern "C" int sb_debug_ctc_lm_rescans(unsigned long long* frames) {
 // ------------------------------------------------------------------------------------------------
 static int dec_wordlm_fuse(int S, int blank, const SbWordLm* lm, double lm_weight,
                            double insertion_bonus, double oov_penalty, WordLmFuse* fu) {
-  if (!lm) return SB_ERR_INVALID;
-  const SbNgramLm& ng = lm->ngram;
-  if (!ng.keys || !ng.vals || !ng.logp || !ng.bow || !ng.tok || !lm->lex_keys || !lm->lex_vals ||
-      !lm->lex_word)
-    return SB_ERR_INVALID;
-  if (!(lm_weight >= 0.0) || !isfinite(lm_weight) || !isfinite(insertion_bonus))
-    return SB_ERR_INVALID;
-  if (isnan(oov_penalty) || oov_penalty > 0.0) return SB_ERR_INVALID;
-  if (!lm->has_unk && oov_penalty != -INFINITY) return SB_ERR_INVALID;
-  if (lm->num_classes < S || lm->blank != blank) return SB_ERR_INVALID;
-  if (lm->delimiter < 0 || lm->delimiter >= S || lm->delimiter == blank) return SB_ERR_INVALID;
-  if (ng.cap <= 0 || (ng.cap & (ng.cap - 1)) || lm->lex_cap <= 0 ||
-      (lm->lex_cap & (lm->lex_cap - 1)) || lm->num_words < 1 || ng.bos != lm->num_words ||
-      ng.order < 1)
-    return SB_ERR_INVALID;
-  if (ng.order > SB_LM_MAX_ORDER) return SB_ERR_UNSUPPORTED;
-  fu->lm = *lm;
-  fu->alpha = lm_weight;
-  fu->beta = insertion_bonus;
-  fu->gamma = oov_penalty;
-  return SB_OK;
+  return word_lm_terms(lm, lm_weight, insertion_bonus, oov_penalty, S,
+                       [&](const SbWordLm& l) { return l.blank == blank && l.delimiter != blank; },
+                       fu);
 }
 
 static int dec_wordlm_entry(const float* logp, const int* lens, int B, int T, int S, int beam_size,

@@ -851,7 +851,9 @@ __global__ void __launch_bounds__(32 * CELL_WARPS) s2s_cell_bwd_kernel(const Cel
 // root (the start token) reads as <s>.  Once per step each CTA resolves every live row's context
 // nodes into shared memory (resolve), so a candidate's lookup is at most `order` probes.  The
 // fused value is the hypothesis score everywhere after: selection, completion, stop rule, result.
-// The beam state, the bookkeeping and S2sLmFuse are in s2s_beam.cuh.
+//   S2sWordLmFuse  the word LM of SbWordLm: the LM term on the delimiter that ends a non-empty
+//              word and on end_tok, an OOV penalty where a word leaves the lexicon.
+// The beam state, the bookkeeping, S2sLmFuse and S2sWordLmFuse are in s2s_beam.cuh.
 // ------------------------------------------------------------------------------------------------
 struct S2sNoFuse {
   static constexpr bool kLm = false;
@@ -1374,6 +1376,39 @@ extern "C" int sb_s2s_beam_select_split_lm_batch(const float* logp, void* state,
   if (!stop) return SB_ERR_INVALID;
   sb::S2sLmFuse fu;
   const int rc = beam_lm_fuse(lm, lm_weight, insertion_bonus, C, &fu);
+  if (rc != SB_OK) return rc;
+  return beam_select_split(logp, state, c_scores, nodes, parent_row, tok_next, out_tokens, K, C,
+                           end_tok, step, max_len, node_cap, c_cap, stop, B, workspace,
+                           workspace_bytes, stream_, fu);
+}
+
+extern "C" int sb_s2s_beam_select_wordlm_batch(const float* logp, void* state, double* c_scores,
+                                               int* nodes, int* parent_row, int* tok_next,
+                                               int* out_tokens, int K, int C, int end_tok,
+                                               int step, int max_len, int node_cap, int c_cap,
+                                               int* stop, int B, const SbWordLm* lm,
+                                               double lm_weight, double insertion_bonus,
+                                               double oov_penalty, int* word_nodes,
+                                               void* stream_) {
+  if (!stop) return SB_ERR_INVALID;
+  sb::S2sWordLmFuse fu;
+  const int rc = beam_wordlm_fuse(lm, lm_weight, insertion_bonus, oov_penalty, C, end_tok,
+                                  word_nodes, nodes, &fu);
+  if (rc != SB_OK) return rc;
+  return beam_select(logp, state, c_scores, nodes, parent_row, tok_next, out_tokens, K, C, end_tok,
+                     step, max_len, node_cap, c_cap, stop, B, stream_, fu);
+}
+
+extern "C" int sb_s2s_beam_select_split_wordlm_batch(
+    const float* logp, void* state, double* c_scores, int* nodes, int* parent_row, int* tok_next,
+    int* out_tokens, int K, int C, int end_tok, int step, int max_len, int node_cap, int c_cap,
+    int* stop, int B, void* workspace, size_t workspace_bytes, const SbWordLm* lm,
+    double lm_weight, double insertion_bonus, double oov_penalty, int* word_nodes,
+    void* stream_) {
+  if (!stop) return SB_ERR_INVALID;
+  sb::S2sWordLmFuse fu;
+  const int rc = beam_wordlm_fuse(lm, lm_weight, insertion_bonus, oov_penalty, C, end_tok,
+                                  word_nodes, nodes, &fu);
   if (rc != SB_OK) return rc;
   return beam_select_split(logp, state, c_scores, nodes, parent_row, tok_next, out_tokens, K, C,
                            end_tok, step, max_len, node_cap, c_cap, stop, B, workspace,

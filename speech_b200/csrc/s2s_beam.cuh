@@ -120,6 +120,85 @@ struct S2sLmFuse {
   }
 };
 
+// The word LM (SbWordLm).  Each hypothesis node q carries its word state in the arena
+// word_nodes [B][node_cap][3]: the lexicon node of its partial word, the token of its last
+// completed word (-1: none, <s>), and a node whose state holds the words before that one.  The
+// state of a live row's node follows from its parent's, which was a live row resolved in the
+// previous step's launch, and its token: one lexicon probe or one word token at most; the root
+// (the start token) is the empty state.  Its history is then read up those links, at most order - 1
+// of them, so a row's resolve costs O(order) probes whatever the length of its words.  Several CTAs
+// resolving the same rows write the same values, and no row reads another's node of this step.
+struct S2sWordShared {
+  int hist[BM_MAXK][SB_LM_MAX_ORDER - 1];   // each live row's last order-1 words, most recent first
+  int ctx[BM_MAXK][SB_LM_MAX_ORDER];        // lm_context scratch
+  int node[BM_MAXK];                        // each live row's lexicon node n_r
+  double dterm[BM_MAXK];                    // d_r (rows with n_r != 0)
+  double eterm[BM_MAXK];                    // t_r
+};
+SB_DEVINL S2sWordShared& s2s_word_shared() {
+  __shared__ S2sWordShared sh;
+  return sh;
+}
+
+struct S2sWordLmFuse {
+  static constexpr bool kLm = true;
+  WordTerms wt;
+  int* word_nodes;          // [B][node_cap][3], parallel to BeamParams::nodes
+  const int* nodes0;        // utterance 0's nodes: p.nodes - nodes0 locates utterance b's arena
+
+  // thread r < nl: row r's word state (written to its node), history, d_r and t_r; the caller
+  // syncs
+  SB_DEVINL void resolve(const BeamParams& p, const BeamState* st, int nl) const {
+    const int r = threadIdx.x;
+    if (r >= nl) return;
+    S2sWordShared& sh = s2s_word_shared();
+    int* wn = word_nodes + (size_t)(p.nodes - nodes0) / 2 * 3;
+    const int q = st->node[r], u = p.nodes[2 * q], t = p.nodes[2 * q + 1];
+    int lex = 0, last = -1, before = -1;
+    if (u >= 0) {
+      const int nu = wn[3 * u];
+      last = wn[3 * u + 1];
+      before = wn[3 * u + 2];
+      if (t == wt.lm.delimiter) {
+        if (nu != 0) { last = wt.word_tok(nu); before = u; }
+      } else {
+        lex = nu < 0 ? -1 : wt.child(nu, t);
+      }
+    }
+    wn[3 * q] = lex;
+    wn[3 * q + 1] = last;
+    wn[3 * q + 2] = before;
+    const int n = wt.lm.ngram.order - 1;
+    for (int k = 0; k < n; ++k) {
+      sh.hist[r][k] = last;
+      if (last < 0) break;
+      last = wn[3 * before + 1];
+      before = wn[3 * before + 2];
+    }
+    auto older = [&](int k) { return sh.hist[r][k]; };
+    sh.node[r] = lex;
+    if (lex != 0) sh.dterm[r] = wt.dterm(lex, older, sh.ctx[r]);
+    sh.eterm[r] = wt.end_term(lex, older, sh.ctx[r]);
+  }
+  SB_DEVINL double value(const BeamParams& p, const BeamState* st, int r, int c) const {
+    const S2sWordShared& sh = s2s_word_shared();
+    const double lp = (double)p.logp[(size_t)r * p.C + c];
+    const int n = sh.node[r];
+    if (c == wt.lm.delimiter) return n == 0 ? st->score[r] + lp : st->score[r] + (lp + sh.dterm[r]);
+    if (c == p.end_tok) return st->score[r] + (lp + sh.eterm[r]);
+    if (n >= 0 && wt.child(n, c) < 0) return st->score[r] + (lp + wt.gamma);
+    return st->score[r] + lp;
+  }
+  // the LM part alone: d_r, t_r, gamma or 0 (the joint CTC/attention search's pre-beam)
+  SB_DEVINL double lm_part(const BeamParams& p, int r, int c) const {
+    const S2sWordShared& sh = s2s_word_shared();
+    const int n = sh.node[r];
+    if (c == wt.lm.delimiter) return n == 0 ? 0.0 : sh.dterm[r];
+    if (c == p.end_tok) return sh.eterm[r];
+    return (n >= 0 && wt.child(n, c) < 0) ? wt.gamma : 0.0;
+  }
+};
+
 // ---- the reference's bookkeeping of one utterance (p = BeamParams::of(b)), sequential (a handful
 // of entries): the first `want` candidates in (score desc, index asc) order -> complete / next
 // beam / stop rule / back-track; parent_row holds rows within the utterance.  A selected flat
@@ -203,4 +282,19 @@ static inline int beam_lm_fuse(const SbNgramLm* lm, double lm_weight, double ins
   fu->alpha = lm_weight;
   fu->beta = insertion_bonus;
   return SB_OK;
+}
+
+// The fusion policy of a word-LM entry point, after the checks the header lists (host): the blank
+// (the start token) is no scored class and the delimiter is not the end token
+static inline int beam_wordlm_fuse(const SbWordLm* lm, double lm_weight, double insertion_bonus,
+                                   double oov_penalty, int C, int end_tok, int* word_nodes,
+                                   const int* nodes, sb::S2sWordLmFuse* fu) {
+  if (!word_nodes) return SB_ERR_INVALID;
+  fu->word_nodes = word_nodes;
+  fu->nodes0 = nodes;
+  return word_lm_terms(lm, lm_weight, insertion_bonus, oov_penalty, C,
+                       [&](const SbWordLm& l) {
+                         return !(l.blank >= 0 && l.blank < C) && l.delimiter != end_tok;
+                       },
+                       &fu->wt);
 }

@@ -334,16 +334,17 @@ static int ctc_cand_launch(const CtcCandArgs<Fuse>& a, int K, int B, cudaStream_
   return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
 }
 
-extern "C" int sb_s2s_ctc_candidates(const float* logp, const float* ctc_logp, const int* lens,
-                                     const void* state, const int* nodes, int node_cap,
-                                     void* ctc_state, size_t ctc_state_bytes, int K, int C, int M,
-                                     int T, int start_tok, int end_tok, double ctc_weight,
-                                     int step, const int* stop, int B, const SbNgramLm* lm,
-                                     double lm_weight, double insertion_bonus, void* stream_) {
+// the checks and parameters of the candidate entry points, for the launch of a
+// CtcCandArgs<Fuse> a whose fusion policy the caller fills
+template <class Fuse>
+static int ctc_cand_args(CtcCandArgs<Fuse>* a, const float* logp, const float* ctc_logp,
+                         const int* lens, const void* state, const int* nodes, int node_cap,
+                         void* ctc_state, size_t ctc_state_bytes, int K, int C, int M, int T,
+                         int start_tok, int end_tok, double ctc_weight, int step, const int* stop,
+                         int B) {
   if (!logp || !state || !nodes || !stop || node_cap <= 0 || step < 0) return SB_ERR_INVALID;
-  CtcParams q;
-  int rc = ctc_params(&q, ctc_logp, lens, ctc_state, ctc_state_bytes, K, C, M, T, start_tok,
-                      end_tok, ctc_weight, B);
+  const int rc = ctc_params(&a->q, ctc_logp, lens, ctc_state, ctc_state_bytes, K, C, M, T,
+                            start_tok, end_tok, ctc_weight, B);
   if (rc != SB_OK) return rc;
   if ((size_t)C * sizeof(double) > CTC_MAX_PBYTES) return SB_ERR_UNSUPPORTED;
   BeamParams p = {};
@@ -351,18 +352,53 @@ extern "C" int sb_s2s_ctc_candidates(const float* logp, const float* ctc_logp, c
   p.st = reinterpret_cast<BeamState*>(const_cast<void*>(state));
   p.nodes = const_cast<int*>(nodes);
   p.node_cap = node_cap; p.K = K; p.C = C; p.end_tok = end_tok; p.step = step; p.B = B;
+  a->p = p;
+  a->done = stop + 1;
+  return SB_OK;
+}
+
+extern "C" int sb_s2s_ctc_candidates(const float* logp, const float* ctc_logp, const int* lens,
+                                     const void* state, const int* nodes, int node_cap,
+                                     void* ctc_state, size_t ctc_state_bytes, int K, int C, int M,
+                                     int T, int start_tok, int end_tok, double ctc_weight,
+                                     int step, const int* stop, int B, const SbNgramLm* lm,
+                                     double lm_weight, double insertion_bonus, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (lm) {
     CtcCandArgs<S2sLmFuse> a;
+    int rc = ctc_cand_args(&a, logp, ctc_logp, lens, state, nodes, node_cap, ctc_state,
+                           ctc_state_bytes, K, C, M, T, start_tok, end_tok, ctc_weight, step,
+                           stop, B);
+    if (rc != SB_OK) return rc;
     rc = beam_lm_fuse(lm, lm_weight, insertion_bonus, C, &a.fu);
     if (rc != SB_OK) return rc;
-    a.p = p; a.q = q; a.done = stop + 1;
     return ctc_cand_launch(a, K, B, stream);
   }
-  if (lm_weight != 0.0 || insertion_bonus != 0.0) return SB_ERR_INVALID;
   CtcCandArgs<S2sNoLm> a;
-  a.p = p; a.q = q; a.done = stop + 1;
+  const int rc = ctc_cand_args(&a, logp, ctc_logp, lens, state, nodes, node_cap, ctc_state,
+                               ctc_state_bytes, K, C, M, T, start_tok, end_tok, ctc_weight, step,
+                               stop, B);
+  if (rc != SB_OK) return rc;
+  if (lm_weight != 0.0 || insertion_bonus != 0.0) return SB_ERR_INVALID;
   return ctc_cand_launch(a, K, B, stream);
+}
+
+extern "C" int sb_s2s_ctc_candidates_wordlm(const float* logp, const float* ctc_logp,
+                                            const int* lens, const void* state, const int* nodes,
+                                            int node_cap, void* ctc_state, size_t ctc_state_bytes,
+                                            int K, int C, int M, int T, int start_tok,
+                                            int end_tok, double ctc_weight, int step,
+                                            const int* stop, int B, const SbWordLm* lm,
+                                            double lm_weight, double insertion_bonus,
+                                            double oov_penalty, int* word_nodes, void* stream_) {
+  CtcCandArgs<S2sWordLmFuse> a;
+  int rc = beam_wordlm_fuse(lm, lm_weight, insertion_bonus, oov_penalty, C, end_tok, word_nodes,
+                            nodes, &a.fu);
+  if (rc != SB_OK) return rc;
+  rc = ctc_cand_args(&a, logp, ctc_logp, lens, state, nodes, node_cap, ctc_state,
+                     ctc_state_bytes, K, C, M, T, start_tok, end_tok, ctc_weight, step, stop, B);
+  if (rc != SB_OK) return rc;
+  return ctc_cand_launch(a, K, B, reinterpret_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int sb_s2s_ctc_select_batch(const float* ctc_logp, const int* lens, void* ctc_state,

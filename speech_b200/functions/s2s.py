@@ -9,6 +9,7 @@ reads the final hypotheses back once.
 import torch
 
 from .. import _lib, ops
+from ..lm import WordLM
 
 
 def _f(t):
@@ -474,12 +475,16 @@ def beam_search_batch(m, eh, start_tok, end_tok, beam_size, max_len, lens=None, 
     lens (optional): frames each utterance attends over.  lm (optional): an NGramLM whose classes
     are the vocabulary, blank the start token and end the end token (the caller checks), fused
     into every candidate as logp + (lm_weight * lm + insertion_bonus, no bonus for the end token);
-    the scores are then the fused ones.  ctc (optional): (y, ctc_weight, prebeam), joint
-    CTC/attention decoding (csrc/s2s_ctc.cu) with y the float32 CTC log-probabilities (B, T, C),
-    blank C - 1 = end_tok, start_tok = C: candidate c of row r is one of the row's `prebeam`
-    classes with the largest P = (1 - ctc_weight) logp[c] (+ the LM part), valued
-    (A_r + P) + ctc_weight * psi(h_r + c), psi the CTC prefix log-probability; the scores are then
-    A + ctc_weight * psi.  -> list of B (token tuple, float64 score of that hypothesis, steps that
+    the scores are then the fused ones.  lm may instead be a WordLM with the same layout and a
+    delimiter class: the word-LM entry points (csrc/s2s_beam.cuh, S2sWordLmFuse) score each word
+    at its delimiter and the trailing word with </s> at the end token, insertion_bonus per word and
+    lm.oov_penalty per word that leaves the lexicon, with each node's word state in a
+    [B][node_cap][3] arena beside the hypothesis nodes.  ctc (optional): (y, ctc_weight,
+    prebeam), joint CTC/attention decoding (csrc/s2s_ctc.cu) with y the float32 CTC
+    log-probabilities (B, T, C), blank C - 1 = end_tok, start_tok = C: candidate c of row r is
+    one of the row's `prebeam` classes with the largest P = (1 - ctc_weight) logp[c] (+ the LM
+    part), valued (A_r + P) + ctc_weight * psi(h_r + c), psi the CTC prefix log-probability; the
+    scores are then A + ctc_weight * psi.  -> list of B (token tuple, float64 score of that hypothesis, steps that
     utterance's search ran)."""
     lib = _lib.load()
     w = DecoderWeights(m)
@@ -523,9 +528,13 @@ def beam_search_batch(m, eh, start_tok, end_tok, beam_size, max_len, lens=None, 
     p_par, p_tok, p_out = parent.data_ptr(), tok.data_ptr(), out_tokens.data_ptr()
     p_stop = stop.data_ptr()
     fusion = (None, 0.0, 0.0)
+    word = isinstance(lm, WordLM)
     if lm is not None:
         tables, _ = lm.device_tables(dev)
         fusion = (tables, float(lm_weight), float(insertion_bonus))
+    if word:
+        word_nodes = torch.empty(B, node_cap, 3, dtype=torch.int32, device=dev)
+        fusion += (float(lm.oov_penalty), word_nodes.data_ptr())
     if ctc is not None:
         y, lam, M = ctc
         if tuple(y.shape) != (B, T, C) or y.dtype != torch.float32 or y.device != ehc.device:
@@ -551,12 +560,23 @@ def beam_search_batch(m, eh, start_tok, end_tok, beam_size, max_len, lens=None, 
             _fc_rows(lib, w, fc_ws, hx[1], sx[1], R, sp, logits=logp, done=done_ptr)
             _fc_logp(lib, w, fc_ws, logp, logp, R, sp, done=done_ptr)
         if ctc is not None:
-            ops._launch("s2s_ctc_candidates", 0.0, lambda: lib.sb_s2s_ctc_candidates(
+            cand = lib.sb_s2s_ctc_candidates_wordlm if word else lib.sb_s2s_ctc_candidates
+            ops._launch("s2s_ctc_candidates", 0.0, lambda: cand(
                 logp.data_ptr(), cargs[0], cargs[1], p_state, p_nodes, node_cap, cargs[2],
                 cargs[3], *shape, e, p_stop, B, *fusion, sp))
             ops._launch("s2s_ctc_select", 0.0, lambda: lib.sb_s2s_ctc_select_batch(
                 *cargs, p_state, p_c, p_nodes, p_par, p_tok, p_out, *shape, e, max_len, node_cap,
                 c_cap, p_stop, B, sp))
+        elif word and split:
+            ops._launch("s2s_beam_select_split_wordlm", 0.0,
+                        lambda: lib.sb_s2s_beam_select_split_wordlm_batch(
+                            logp.data_ptr(), p_state, p_c, p_nodes, p_par, p_tok, p_out, K, C,
+                            int(end_tok), e, max_len, node_cap, c_cap, p_stop, B,
+                            sel_ws.data_ptr(), sel_ws.numel(), *fusion, sp))
+        elif word:
+            ops._launch("s2s_beam_select_wordlm", 0.0, lambda: lib.sb_s2s_beam_select_wordlm_batch(
+                logp.data_ptr(), p_state, p_c, p_nodes, p_par, p_tok, p_out, K, C, int(end_tok), e,
+                max_len, node_cap, c_cap, p_stop, B, *fusion, sp))
         elif lm is not None and split:
             ops._launch("s2s_beam_select_split_lm", 0.0,
                         lambda: lib.sb_s2s_beam_select_split_lm_batch(

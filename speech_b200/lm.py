@@ -1,8 +1,8 @@
 """Backoff n-gram language models for shallow fusion: NGramLM over the model's own classes, for
 the CTC prefix beam search, the attention model's beam search and the Transducer's label-free beam
 search; WordLM over words spelled in a character model's classes, for the CTC prefix beam search
-(see WordLM).  Both read and write ARPA files and train interpolated Kneser-Ney models through the
-same module functions.
+and the attention model's beam search (see WordLM).  Both read and write ARPA files and train
+interpolated Kneser-Ney models through the same module functions.
 
 The LM is over the acoustic model's own output classes (characters or subword units); the blank is
 never an LM token.  Orders 1..10, with a sentence start <s>, an end </s> and optionally <unk>.
@@ -500,14 +500,22 @@ class NGramLM:
 
 
 class WordLM:
-    """Backoff word n-gram LM for the CTC prefix beam search of a character model (Hannun et al.
-    2014, arXiv:1408.2873): a word is scored when the delimiter class (the space) that ends it is
-    emitted, and a lexicon of the LM's words, spelled in the model's classes, tracks the partial
-    word.  Word tokens: the spellable words 0..W-1 in sorted order, <s> W, </s> W + 1, <unk> W + 2.
+    """Backoff word n-gram LM for the CTC prefix beam search or the attention beam search of a
+    character model (Hannun et al. 2014, arXiv:1408.2873): a word is scored when the delimiter
+    class (the space) that ends it is emitted, and a lexicon of the LM's words, spelled in the
+    model's classes, tracks the partial word.  Word tokens: the spellable words 0..W-1 in sorted
+    order, <s> W, </s> W + 1, <unk> W + 2.
     Build with from_arpa or train; the search semantics are in include/speech_b200.h (SbWordLm).
 
         wlm = WordLM.from_arpa("3-gram.arpa", preproc.int_to_char)     # delimiter " ", blank last
         model.infer(batch, beam_size=32, lm=wlm, lm_weight=0.8, insertion_bonus=1.0)
+
+    The attention model's layout has START as the blank and an end class END, scored with the
+    trailing word and </s> where a hypothesis ends (include/speech_b200.h, the s2s word-LM entry
+    points); the CTC search refuses an LM with an end class:
+
+        wlm = WordLM.from_arpa("3-gram.arpa", preproc.int_to_char, blank=V - 1, end=V - 2)
+        s2s_model.recognize(inputs, beam_size=10, lm=wlm, lm_weight=0.8, insertion_bonus=1.0)
 
     A class whose symbol is one character spells that character; the delimiter's and the blank's
     symbols spell nothing.  oov_penalty (<= 0, settable) is added once per word that leaves the
@@ -515,18 +523,21 @@ class WordLM:
     <unk> unigram needs oov_penalty = -inf."""
 
     def __init__(self, order, words, ngrams, symbols, num_classes, blank, delimiter, oov_penalty,
-                 dropped=0):
+                 dropped=0, end=None):
         self._order = order
         self._words = list(words)
         self._ngrams = ngrams
         self._num_classes, self._blank, self._delim = num_classes, blank, delimiter
+        self._end = _check_end(end, blank, num_classes)
+        if self._end is not None and self._end == delimiter:
+            raise ValueError("word LM: the end class %d is the delimiter" % end)
         self._symbols = list(symbols)
         W = len(self._words)
         self._bos, self._eos, self._unk = W, W + 1, W + 2
         if (self._eos,) not in ngrams[1]:
             raise ValueError("word LM: the LM has no %s unigram" % EOS)
         self._dropped = int(dropped)
-        chars = _spelling(self._symbols, blank, delimiter)
+        chars = _spelling(self._symbols, blank, delimiter, self._end)
         self._spell = [tuple(chars[ch] for ch in w) for w in self._words]
         self._oov = None
         self.oov_penalty = oov_penalty
@@ -547,8 +558,9 @@ class WordLM:
 
     @property
     def end(self):
-        """None: the search has no end class (check_lm reads it as NGramLM.end)"""
-        return None
+        """the class that ends a hypothesis (the attention model's END), scored with </s> and the
+        trailing word, or None (the CTC search, which has no end class)"""
+        return self._end
 
     @property
     def delimiter(self):
@@ -589,7 +601,7 @@ class WordLM:
 
     def spell(self, word):
         """the classes of a word, or None where a character has no class"""
-        chars = _spelling(self._symbols, self._blank, self._delim)
+        chars = _spelling(self._symbols, self._blank, self._delim, self._end)
         if word == "" or any(ch not in chars for ch in word):
             return None
         return tuple(chars[ch] for ch in word)
@@ -598,16 +610,18 @@ class WordLM:
     # ARPA and training
     # ------------------------------------------------------------------------------------------
     @classmethod
-    def from_arpa(cls, path, symbols, delimiter=" ", blank=None, oov_penalty=0.0):
+    def from_arpa(cls, path, symbols, delimiter=" ", blank=None, oov_penalty=0.0, end=None):
         """Read an ARPA word LM.  symbols[c] is the string of class c (e.g. the reference
         Preprocessor.int_to_char), blank defaults to the class after the last symbol, delimiter is
         the symbol of the word boundary.  The lexicon is every unigram word spelled character by
         character through the classes; n-grams with a word that cannot be spelled are dropped
         (counted in `dropped`).  ValueError if no word can be spelled (such as an upper-case LM
-        against lower-case symbols)."""
+        against lower-case symbols).  end (optional): the class that ends a hypothesis, for the
+        attention model (blank=V - 1, end=V - 2); it spells nothing."""
         num_classes, blank, symbols = _layout(symbols, blank)
-        delim = _delimiter_class(symbols, blank, delimiter)
-        chars = _spelling(symbols, blank, delim)
+        end = _check_end(end, blank, num_classes)
+        delim = _delimiter_class(symbols, blank, delimiter, end)
+        chars = _spelling(symbols, blank, delim, end)
         vocab = []
 
         def vocabulary(unigram_words):
@@ -623,7 +637,8 @@ class WordLM:
             return tok
 
         order, ngrams, dropped = _read_arpa(path, vocabulary)
-        return cls(order, vocab, ngrams, symbols, num_classes, blank, delim, oov_penalty, dropped)
+        return cls(order, vocab, ngrams, symbols, num_classes, blank, delim, oov_penalty, dropped,
+                   end)
 
     def to_arpa(self, path):
         """Write an ARPA file that from_arpa reads back to the same LM"""
@@ -631,15 +646,16 @@ class WordLM:
         _write_arpa(path, self._order, self._ngrams, names)
 
     @classmethod
-    def train(cls, texts, order, symbols, delimiter=" ", blank=None, oov_penalty=0.0):
+    def train(cls, texts, order, symbols, delimiter=" ", blank=None, oov_penalty=0.0, end=None):
         """Interpolated Kneser-Ney (as NGramLM.train) over the whitespace-split words of each text,
         read as <s> w1 .. wn </s>.  The lexicon is the texts' spellable words; a word that cannot
         be spelled is read as <unk>, and the unigram level spreads its uniform share over the
-        words, </s> and <unk>, so <unk> always has a unigram."""
+        words, </s> and <unk>, so <unk> always has a unigram.  end: as in from_arpa."""
         order = _check_order(order)
         num_classes, blank, symbols = _layout(symbols, blank)
-        delim = _delimiter_class(symbols, blank, delimiter)
-        chars = _spelling(symbols, blank, delim)
+        end = _check_end(end, blank, num_classes)
+        delim = _delimiter_class(symbols, blank, delimiter, end)
+        chars = _spelling(symbols, blank, delim, end)
         texts = [t.split() for t in texts]
         words = sorted({w for t in texts for w in t if all(ch in chars for ch in w)})
         if not words:
@@ -649,7 +665,7 @@ class WordLM:
         tok = {w: t for t, w in enumerate(words)}
         seqs = [[tok.get(w, W + 2) for w in t] for t in texts]
         ngrams = _kneser_ney(seqs, order, list(range(W)) + [W + 1, W + 2], W, W + 1)
-        return cls(order, words, ngrams, symbols, num_classes, blank, delim, oov_penalty)
+        return cls(order, words, ngrams, symbols, num_classes, blank, delim, oov_penalty, end=end)
 
     # ------------------------------------------------------------------------------------------
     # device tables
@@ -706,23 +722,25 @@ class WordLM:
         return d
 
     def __setstate__(self, d):
+        d.setdefault("_end", None)          # pickled before word LMs had an end class
         self.__dict__.update(d)
 
 
-def _delimiter_class(symbols, blank, delimiter):
-    """the one class but the blank whose symbol is `delimiter`"""
-    cs = [c for c, s in enumerate(symbols) if c != blank and s == delimiter]
+def _delimiter_class(symbols, blank, delimiter, end=None):
+    """the one class but the blank and the end whose symbol is `delimiter`"""
+    cs = [c for c, s in enumerate(symbols) if c != blank and c != end and s == delimiter]
     if len(cs) != 1:
         raise ValueError("word LM: %d classes have the delimiter symbol %r (need exactly one)"
                          % (len(cs), delimiter))
     return cs[0]
 
 
-def _spelling(symbols, blank, delim):
-    """{character: class} of the one-character symbols but the blank's and the delimiter's"""
+def _spelling(symbols, blank, delim, end=None):
+    """{character: class} of the one-character symbols but the blank's, the delimiter's and the
+    end class's"""
     chars = {}
     for c, s in enumerate(symbols):
-        if c == blank or c == delim:
+        if c == blank or c == delim or c == end:
             continue
         if not isinstance(s, str) or s == "":
             raise ValueError("word LM: symbol %r of class %d is not a string" % (s, c))

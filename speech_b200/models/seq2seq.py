@@ -212,6 +212,13 @@ class Seq2Seq(model.Model):
         insertion_bonus), where lm(end_tok | h) is lm(</s> | h) and the end token earns no bonus;
         the context of h starts at <s>, its start token.  The returned scores are the fused ones.
         With lm=None (the default) this is the LM-less search.
+        lm may also be a speech_b200.lm.WordLM with the same layout (WordLM.from_arpa(path,
+        preproc.int_to_char, blank=V - 1, end=V - 2), the space its delimiter): a word is then
+        scored when the delimiter that ends it is chosen, lm_weight * lm(w | words) +
+        insertion_bonus (per word), and END adds the trailing word and lm(</s> | words); a class
+        that takes the partial word out of the lexicon adds lm.oov_penalty (include/speech_b200.h,
+        sb_s2s_beam_select_wordlm_batch).  The score of a completed hypothesis is acoustic +
+        lm_weight * (word LM with </s>) + insertion_bonus * words + oov_penalty * OOV words.
 
         Joint CTC/attention decoding (Watanabe et al. 2017, Algorithm 2): ctc_weight = w in
         (0, 1) needs the CTC head (config["decoder"]["ctc_weight"] > 0) and the default START /
@@ -276,9 +283,6 @@ class Seq2Seq(model.Model):
             if lm_weight != 0.0 or insertion_bonus != 0.0:
                 raise ValueError("lm_weight / insertion_bonus need an lm")
             return
-        if isinstance(lm, WordLM):
-            raise ValueError("a word LM fuses into the CTC search only; the attention search "
-                             "takes an NGramLM")
         if not (math.isfinite(lm_weight) and lm_weight >= 0.0):
             raise ValueError("lm_weight must be finite and >= 0, got %r" % (lm_weight,))
         if not math.isfinite(insertion_bonus):
@@ -290,6 +294,9 @@ class Seq2Seq(model.Model):
                              % (lm.blank, start_tok))
         if lm.end != end_tok:
             raise ValueError("the LM's end class is %r, the end token is %d" % (lm.end, end_tok))
+        if isinstance(lm, WordLM) and lm.delimiter in (start_tok, end_tok):
+            raise ValueError("the word LM's delimiter %d is the start or the end token"
+                             % lm.delimiter)
         if start_tok < V - 1:
             raise ValueError("with an LM the start token must be the class the model never "
                              "predicts (%d), got %d" % (V - 1, start_tok))

@@ -42,6 +42,18 @@ print("seq2seq joint CTC loss", lc.item(), "recognize", [len(h) for h in sc.reco
     inputs, beam_size=3, max_len=8, ctc_weight=0.3)], "with LM", [len(h) for h in sc.recognize(
     inputs, beam_size=3, max_len=8, lm=lm2, lm_weight=0.5, insertion_bonus=1.0, ctc_weight=0.5,
     ctc_prebeam=29)])
+from speech_b200.lm import WordLM
+wsyms = list("abcdefghijklmnopqrstuvwxyz") + [" ", "'", "</s>", "<s>"]
+wlm = WordLM.train(["the cat sat", "a cat", "the mat sat"], 3, wsyms, blank=29, end=28,
+                   oov_penalty=-2.0)
+wargs = dict(beam_size=3, max_len=8, lm=wlm, lm_weight=0.5, insertion_bonus=1.0)
+print("seq2seq recognize with a word LM", [len(h) for h in s.recognize(inputs, **wargs)])
+s2s_fn.beam_select_fits = lambda K, C: False     # the split selection with the word LM
+print("seq2seq recognize with a word LM, split select",
+      [len(h) for h in s.recognize(inputs, **wargs)])
+s2s_fn.beam_select_fits = fits
+print("seq2seq joint CTC with a word LM",
+      [len(h) for h in sc.recognize(inputs, ctc_weight=0.3, **wargs)])
 t = Transducer(80, 28, cfg).cuda()
 l3 = t.loss((inputs, labels)); l3.backward()
 print("transducer ok", l3.item())
