@@ -380,6 +380,23 @@ int sb_ctc_stream_step_lm_shortlist(const float* logp, const int* n, int B, int 
                                     void* stream);
 int sb_ctc_stream_best(const void* state, int B, int max_frames, int beam_size, int* out_labels,
                        int* out_lens, double* out_scores, int* out_overflow, void* stream);
+/*   sb_ctc_stream_nbest        every stored beam entry of every stream, the N-best of two-pass
+ *       decoding: out_count (B) int32 the n_b <= K entries of stream b's beam; entry i of stream b
+ *       has its labels at out_labels[(b*K + i) * max_frames ..] (B, K, max_frames) int32, its
+ *       length at out_lens[b*K + i] (B, K) int32 and c_i = lse(p_b, p_nb), the log-probability
+ *       itself (not negated), at out_scores[b*K + i] (B, K) float64.  Slots i >= n_b get length -1
+ *       and score -inf.  The order is the order the search stores: each frame's beam is taken as
+ *       the first K candidates by (score desc, first-touch rank asc), so entry 0 is the best
+ *       (sb_ctc_stream_best's result, whose score is -c_0), and the others follow by score, ties
+ *       in the search's first-touch order.  Changes no state.  Serves states stepped without an
+ *       LM: with a word LM the stored order is not the end-of-utterance order (that rule is
+ *       sb_ctc_stream_best_wordlm's); with a character LM c_i holds the fused scores.
+ *       The offline N-best is this same path: sb_ctc_stream_reset, one sb_ctc_stream_step over all
+ *       frames with n = each utterance's frames, then sb_ctc_stream_nbest; by the guarantee above
+ *       its entry 0 is sb_ctc_prefix_beam's result bit for bit.
+ *       SB_ERR_INVALID / SB_ERR_UNSUPPORTED as sb_ctc_stream_best, before any CUDA call. */
+int sb_ctc_stream_nbest(const void* state, int B, int max_frames, int beam_size, int* out_labels,
+                        int* out_lens, double* out_scores, int* out_count, void* stream);
 /* Developer counter: frames the LM-fused shortlist search (character or word LM) rescanned in
  * full, over every call since the last query (synchronous: waits for the device); resets it. */
 int sb_debug_ctc_lm_rescans(unsigned long long* frames);
@@ -589,6 +606,21 @@ int sb_s2s_cell_bwd(const float* d_gi, const float* d_gh, const float* d_hx_dire
                     const float* w_ihT, const float* w_hhT, float* d_ix, float* d_hx_prev, int B,
                     int H, void* stream);
 int sb_s2s_check_done(const int* end_count, int B, int* done, int* nsteps, int step1, void* stream);
+/* Attention rescoring (csrc/s2s_rescore.cu), the second pass of two-pass decoding: R rows, each a
+ * hypothesis forced through the step kernels above (row r attends over utterance r / K with
+ * eh_group = K).  Row r of tokens (R, ld) int32 is START, y_1 .. y_L with L = lens[r] <= ld - 1
+ * (lens (R) int32; L = -1 marks a row that scores nothing, an empty beam slot).
+ *   sb_s2s_score_tokens  after step u's log-softmax logp (R, C) float32: acc[r] += (double)
+ *       logp[r, y_{u+1}] where u < L, acc[r] += (double) logp[r, end_tok] where u == L, nothing
+ *       where u > L.  Called for u = 0, 1, .. in order, acc (R) float64 ends as
+ *       a = sum_{u=0..L} (double) l_u, summed in u order, l_u the float32 log-probability of the
+ *       u-th forced token; an empty hypothesis (L = 0) scores l(END | START).
+ *       Every token read must lie in [0, C) (the caller builds the matrix from
+ *       sb_ctc_stream_nbest's labels); the host sees only what it can check.
+ * SB_ERR_INVALID for a null pointer, R, C or ld <= 0, u < 0 or end_tok outside [0, C);
+ * SB_ERR_UNSUPPORTED for R past 2^31 - 1 blocks of rows.  Both before any CUDA call. */
+int sb_s2s_score_tokens(const float* logp, long long R, int C, const int* tokens, int ld,
+                        const int* lens, int u, int end_tok, double* acc, void* stream);
 /* The beam state is opaque but for the fields the host reads in place: `done` (int32) at byte 0
  * (0 while the search runs, then the number of steps it ran; for one utterance it doubles as the
  * `done` flag of the step kernels), the length of the final hypothesis in out_tokens (int32) at byte 4, and its

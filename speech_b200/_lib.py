@@ -77,6 +77,7 @@ SIGNATURES = {
     "sb_ctc_stream_step_lm_shortlist": (_c_int, [_vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int,
                                                  _lmp, _db, _db, _c_int, _vp, _vp, _c_sz, _vp]),
     "sb_ctc_stream_best": (_c_int, [_vp, _c_int, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp]),
+    "sb_ctc_stream_nbest": (_c_int, [_vp, _c_int, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp]),
     "sb_ctc_prefix_beam_wordlm": (_c_int, [_vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int,
                                            _wlmp, _db, _db, _db, _vp, _vp, _vp, _vp, _c_sz, _vp]),
     "sb_ctc_prefix_beam_wordlm_shortlist": (_c_int, [_vp, _vp, _c_int, _c_int, _c_int, _c_int,
@@ -113,6 +114,8 @@ SIGNATURES = {
     "sb_s2s_attn_bwd": (_c_int, [_vp] * 22 + [_c_int] * 5 + [_vp, _vp, _c_sz, _vp]),
     "sb_s2s_cell_bwd": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_int, _c_int, _vp]),
     "sb_s2s_check_done": (_c_int, [_vp, _c_int, _vp, _vp, _c_int, _vp]),
+    "sb_s2s_score_tokens": (_c_int, [_vp, _c_ll, _c_int, _vp, _c_int, _vp, _c_int, _c_int, _vp,
+                                     _vp]),
     "sb_s2s_beam_state_size": (_c_int, [ctypes.POINTER(_c_sz)]),
     "sb_s2s_beam_init": (_c_int, [_vp, _vp, _vp, _c_int, _vp]),
     "sb_s2s_beam_select": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_int, _c_int, _c_int,

@@ -777,6 +777,31 @@ __global__ void __launch_bounds__(32) ctc_stream_best_wordlm_kernel(const DecPar
   if (threadIdx.x == 0 && out_overflow) out_overflow[blockIdx.x] = sl->overflow;
 }
 
+// Every stored entry of each slot: thread i < K back-tracks entry i into out_labels[b][i] and
+// writes c_i = lse(p_b, p_nb); slots past the beam's size get length -1 and score -inf.
+__global__ void __launch_bounds__(DEC_MAX_BEAM) ctc_stream_nbest_kernel(const BeamTrie trie,
+                                                                        const void* slots, int K,
+                                                                        int max_frames,
+                                                                        int* out_labels,
+                                                                        int* out_lens,
+                                                                        double* out_scores,
+                                                                        int* out_count) {
+  const int b = blockIdx.x, i = threadIdx.x;
+  const DecSlot* sl = dec_slot(const_cast<void*>(slots), b);
+  const Beam& bm = sl->beam;
+  const int nb = bm.size;
+  if (i == 0) out_count[b] = nb;
+  if (i >= K) return;
+  const size_t e = (size_t)b * K + i;
+  if (i < nb) {
+    out_lens[e] = trie.of(b).backtrack(bm.node[i], out_labels + e * max_frames);
+    out_scores[e] = lse2d(bm.pb[i], bm.pnb[i]);
+  } else {
+    out_lens[e] = -1;
+    out_scores[e] = d_neg_inf();
+  }
+}
+
 }  // namespace sb
 
 using namespace sb;
@@ -1081,6 +1106,18 @@ extern "C" int sb_ctc_stream_best(const void* state, int B, int max_frames, int 
   p.B = B; p.T = max_frames; p.K = beam_size;
   ctc_stream_best_kernel<<<B, 32, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p, state,
                                                                               out_overflow);
+  return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
+}
+
+extern "C" int sb_ctc_stream_nbest(const void* state, int B, int max_frames, int beam_size,
+                                   int* out_labels, int* out_lens, double* out_scores,
+                                   int* out_count, void* stream) {
+  if (!state || !out_labels || !out_lens || !out_scores || !out_count) return SB_ERR_INVALID;
+  const int rc = dec_stream_check(B, max_frames, beam_size);
+  if (rc != SB_OK) return rc;
+  ctc_stream_nbest_kernel<<<B, DEC_MAX_BEAM, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      dec_stream_trie(const_cast<void*>(state), B, max_frames, beam_size), state, beam_size,
+      max_frames, out_labels, out_lens, out_scores, out_count);
   return cudaGetLastError() == cudaSuccess ? SB_OK : SB_ERR_CUDA;
 }
 

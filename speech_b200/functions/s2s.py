@@ -606,3 +606,154 @@ def beam_search_batch(m, eh, start_tok, end_tok, beam_size, max_len, lens=None, 
     toks = host[B * S:].view(torch.int32).view(B, out_cap)
     return [(tuple(toks[b, :int(n[b])].tolist()), float(score[b]), int(steps[b]))
             for b in range(B)]
+
+
+# ---- two-pass decoding: CTC prefix beam search N-best, then attention rescoring ----------------
+
+def ctc_nbest(state, B, max_frames, K, dev):
+    """Every stored beam entry of the B streams of a CTC stream state (sb_ctc_stream_nbest): ->
+    labels (B, K, max_frames) int32, lens (B, K) int32 (-1: empty slot), c (B, K) float64
+    log-probabilities lse(p_b, p_nb) (-inf: empty slot), in the search's stored order."""
+    lib = _lib.load()
+    labels = torch.empty(B, K, max_frames, dtype=torch.int32, device=dev)
+    lens = torch.empty(B, K, dtype=torch.int32, device=dev)
+    c = torch.empty(B, K, dtype=torch.float64, device=dev)
+    count = torch.empty(B, dtype=torch.int32, device=dev)
+    ops._launch("ctc_stream_nbest", 0.0, lambda: lib.sb_ctc_stream_nbest(
+        _a(state), B, max_frames, K, labels.data_ptr(), lens.data_ptr(), c.data_ptr(),
+        count.data_ptr(), _lib.stream_ptr()))
+    return labels, lens, c
+
+
+def ctc_stream_state(B, max_frames, K, dev):
+    """a fresh (reset) LM-less CTC stream state of B streams"""
+    lib = _lib.load()
+    state = torch.empty(_lib.workspace_size(lib.sb_ctc_stream_state_size, B, max_frames, K, 0),
+                        dtype=torch.uint8, device=dev)
+    ops._launch("ctc_stream_reset", 0.0, lambda: lib.sb_ctc_stream_reset(
+        state.data_ptr(), B, max_frames, K, 0, B, _lib.stream_ptr()))
+    return state
+
+
+def ctc_stream_step(state, y, n, K, blank, max_frames):
+    """advance the B streams of `state` by n[b] frames of y (B, T, C) float32 log-probabilities
+    (sb_ctc_stream_step, no LM)"""
+    lib = _lib.load()
+    B, T, C = y.shape
+    nd = torch.tensor(list(n), dtype=torch.int32).to(y.device)
+    ws_bytes = _lib.workspace_size(lib.sb_ctc_stream_workspace_size, B, T, K)
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=y.device)
+    ops._launch("ctc_stream_step", 0.0, lambda: lib.sb_ctc_stream_step(
+        y.data_ptr(), nd.data_ptr(), B, T, C, K, blank, max_frames, state.data_ptr(),
+        ws.data_ptr(), ws_bytes, _lib.stream_ptr()))
+
+
+def ctc_first_pass(y, frames, K):
+    """The first pass over whole utterances: y (B, T, C) float32 CTC log-probabilities (blank
+    C - 1), frames[b] <= T the frames of utterance b.  One reset, one step over all T frames and
+    one N-best read: the streaming path, whose entry 0 is sb_ctc_prefix_beam's result.
+    -> ctc_nbest's (labels, lens, c)."""
+    B, T, C = y.shape
+    state = ctc_stream_state(B, T, K, y.device)
+    ctc_stream_step(state, y, frames, K, C - 1, T)
+    return ctc_nbest(state, B, T, K, y.device)
+
+
+def score_batch(m, eh, tokens, lens, K, frame_lens=None):
+    """Teacher-forced attention scores of R = B*K hypotheses, K per utterance of eh (B, T, H):
+    tokens (R, ld) int32 on the device, row r START then its lens[r] labels (lens (R) int32 on the
+    device, -1 for a row that scores nothing); frame_lens (optional): frames each utterance
+    attends over.  Runs recognize's step sequence over the R rows (row r attends over utterance
+    r // K) for ld - 1 steps, sb_s2s_score_tokens after each step's log-softmax, with nothing
+    copied to the host.  -> a (R,) float64: sum over u = 0..lens[r] of the float32 log-probability
+    of the forced token (the next label, then END), as recognize's selection adds them."""
+    lib = _lib.load()
+    w = DecoderWeights(m)
+    ehc = _f(eh)
+    B, T, H = ehc.shape
+    R, ld = tokens.shape
+    C = w.C
+    dev = ehc.device
+    if R != B * K or tuple(lens.shape) != (R,):
+        raise ValueError("score_batch needs %d rows of tokens and lens, got %s / %s"
+                         % (B * K, tuple(tokens.shape), tuple(lens.shape)))
+    end_tok = m.embedding.num_embeddings - 2
+    tok = tokens.to(dev, torch.int32).contiguous()
+    ln = lens.to(dev, torch.int32).contiguous()
+    al = attn_lens(frame_lens, B, T, dev)
+    if al is not None:
+        al = al.repeat_interleave(K)
+    acc = torch.zeros(R, dtype=torch.float64, device=dev)
+    hx = [torch.zeros(R, H, dtype=torch.float32, device=dev) for _ in range(2)]
+    sx = [torch.empty(R, H, dtype=torch.float32, device=dev) for _ in range(2)]
+    ax = [torch.empty(R, T, dtype=torch.float32, device=dev) for _ in range(2)]
+    logp = torch.empty(R, C, dtype=torch.float32, device=dev)
+    sp = _lib.stream_ptr()
+    ws = attn_workspace(lib, R, T, H, dev)
+    fc_ws = None if w.fused else fc_workspace(lib, R, C, dev)
+    p_tok, p_ln, p_acc, p_logp = tok.data_ptr(), ln.data_ptr(), acc.data_ptr(), logp.data_ptr()
+    for u in range(ld - 1):
+        cur, prv = u & 1, (u & 1) ^ 1
+        _cell_fwd(lib, w, p_tok + 4 * u, ld, sx[prv] if u > 0 else None, hx[prv], hx[cur], None,
+                  None, None, R, sp)
+        if w.fused:
+            _attn_fwd(lib, w, ws, ehc, K, hx[cur], ax[prv] if u > 0 else None, sx[cur], ax[cur],
+                      R, T, sp, logp=logp, lens=al)
+        else:
+            _attn_fwd(lib, w, ws, ehc, K, hx[cur], ax[prv] if u > 0 else None, sx[cur], ax[cur],
+                      R, T, sp, with_fc=False, lens=al)
+            _fc_rows(lib, w, fc_ws, hx[cur], sx[cur], R, sp, logits=logp)
+            _fc_logp(lib, w, fc_ws, logp, logp, R, sp)
+        ops._launch("s2s_score_tokens", 0.0, lambda: lib.sb_s2s_score_tokens(
+            p_logp, R, C, p_tok, ld, p_ln, u, end_tok, p_acc, sp))
+    return acc
+
+
+def two_pass_select(a, c, valid, ctc_weight):
+    """The combination r = (1 - w) a + w c in float64 (both products rounded, then added) of the
+    (B, K) attention scores a and CTC log-probabilities c; slots where `valid` is False (empty
+    beam slots) get -inf.  -> (index of the largest r per row, the first on ties; r)."""
+    w = float(ctc_weight)
+    r = torch.mul(a, 1.0 - w).add_(torch.mul(c, w))
+    r = torch.where(valid, r, torch.full_like(r, -float("inf")))
+    return torch.argmax(r, dim=1), r
+
+
+def rescore(m, eh, nbest, frame_lens, K, ctc_weight, return_scores):
+    """The second pass over a first pass's N-best (ctc_nbest's output, utterance b's entries over
+    eh[b]) and the selection: -> B token lists [START] + y + [END] (and their float64 scores r).
+    Reads the longest hypothesis's length before the step loop and the chosen hypotheses once at
+    the end: two device-to-host copies per call."""
+    labels, lens, c = nbest
+    B, _, Lcap = labels.shape
+    dev = labels.device
+    V = m.embedding.num_embeddings
+    start, end = V - 1, V - 2
+    L = max(0, int(lens.max()))
+    R = B * K
+    col = torch.arange(L, device=dev, dtype=torch.int32)
+    body = torch.where(col < lens.view(R, 1), labels.view(R, Lcap)[:, :L],
+                       torch.full((1, 1), end, dtype=torch.int32, device=dev))
+    tokens = torch.cat([torch.full((R, 1), start, dtype=torch.int32, device=dev), body,
+                        torch.full((R, 1), end, dtype=torch.int32, device=dev)], 1)
+    a = score_batch(m, eh, tokens, lens.view(R), K, frame_lens).view(B, K)
+    best, r = two_pass_select(a, c, lens >= 0, ctc_weight)
+    rows = torch.arange(B, device=dev) * K + best
+    # [B float64 scores | B lengths | B rows of L labels] as int32, the scores 8-byte aligned
+    out = torch.cat([r.gather(1, best.view(B, 1)).view(torch.int32).reshape(-1),
+                     lens.view(R)[rows], body[rows].reshape(-1)])
+    host = out.cpu()                            # the chosen hypotheses, in one copy
+    score = host[:2 * B].view(torch.float64).tolist()
+    n = host[2 * B:3 * B].tolist()
+    lab = host[3 * B:].view(B, L)
+    res = [[start] + lab[b, :n[b]].tolist() + [end] for b in range(B)]
+    return (res, score) if return_scores else res
+
+
+def recognize_two_pass(m, eh, y, frame_lens, K, ctc_weight, return_scores):
+    """Two-pass decoding of whole utterances: eh (B, T, H) encoder states, y (B, T, C) float32
+    CTC log-probabilities; frame_lens (optional) the frames of each utterance (default T)."""
+    B, T, _ = y.shape
+    frames = [T] * B if frame_lens is None else [int(f) for f in frame_lens]
+    nbest = ctc_first_pass(y.contiguous(), frames, K)
+    return rescore(m, eh, nbest, frame_lens, K, ctc_weight, return_scores)

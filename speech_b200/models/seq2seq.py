@@ -258,6 +258,50 @@ class Seq2Seq(model.Model):
         labels = [list(r[0]) for r in res]
         return (labels, [r[1] for r in res]) if return_scores else labels
 
+    def recognize_two_pass(self, inputs, beam_size=10, ctc_weight=0.5, return_scores=False):
+        """Two-pass decoding (attention rescoring, Zhang et al. 2020, arXiv:2012.05481) of every
+        utterance of a batch: the CTC head's prefix beam search (beam_size, no LM) gives each
+        utterance an N-best of n_b <= beam_size entries y_i with log-probabilities c_i; the
+        attention decoder then scores each one teacher-forced, a_i = sum of the float32
+        log-softmax values of y_i's labels and END after START, summed in float64 in order.  The
+        result is the entry with the largest r_i = (1 - w) a_i + w c_i (float64, w = ctc_weight
+        in [0, 1]; ties to the lower beam index) as [START] + y + [END], and r with
+        return_scores.  w = 1 gives the first pass's best, w = 0 the N-best entry the attention
+        prefers.  Needs the CTC head (config["decoder"]["ctc_weight"] > 0).  Frames: the padded
+        T' for every utterance, or its own conv_out_size(T_b) in the exact-lengths mode."""
+        from ..functions import s2s
+        self._check_two_pass(beam_size, ctc_weight)
+        if len(inputs) == 0:
+            raise ValueError("recognize_two_pass needs at least one utterance")
+        lens = self.input_lens(inputs)
+        x = self.stage_inputs(inputs)
+        with torch.no_grad():
+            x = self._encode(x, lens)
+            y = torch.log_softmax(self.ctc_fc(x).float(), dim=-1).contiguous()
+            return s2s.recognize_two_pass(self, x, y, lens, int(beam_size), float(ctc_weight),
+                                          return_scores)
+
+    def stream(self, num_streams, beam_size=10, max_frames=3000, ctc_weight=0.5):
+        """Two-pass recognition as the audio arrives (speech_b200.streaming.Seq2SeqStream): the CTC
+        head's prefix beam search advances with every push (partial()), and rescored() runs the
+        attention over each stream's N-best as recognize_two_pass does.  Needs a unidirectional
+        encoder and the CTC head."""
+        from ..streaming import Seq2SeqStream
+        return Seq2SeqStream(self, num_streams, beam_size, max_frames, ctc_weight)
+
+    def _check_two_pass(self, beam_size, ctc_weight):
+        """ValueError unless two-pass decoding can run with these arguments"""
+        from ..functions import s2s
+        if self.ctc_weight <= 0:
+            raise ValueError("two-pass decoding needs a CTC head (config decoder ctc_weight > 0)")
+        if isinstance(beam_size, bool) or int(beam_size) != beam_size or \
+                not 1 <= int(beam_size) <= s2s.BEAM_MAX_WIDTH:
+            raise ValueError("beam_size must lie in [1, %d], got %r"
+                             % (s2s.BEAM_MAX_WIDTH, beam_size))
+        if isinstance(ctc_weight, bool) or not isinstance(ctc_weight, (int, float)) or \
+                not 0.0 <= ctc_weight <= 1.0:
+            raise ValueError("ctc_weight must be a number in [0, 1], got %r" % (ctc_weight,))
+
     def _check_ctc(self, ctc_weight, ctc_prebeam, beam_size, V, start_tok, end_tok):
         """ValueError unless the joint-decoding arguments of recognize are usable; -> the
         pre-beam width M"""

@@ -65,7 +65,10 @@ def lookahead_counts(pending, counts, tau, ends=()):
 class EncoderStream:
     """The encoder half of a stream (see the module docstring): conv carry, per-layer GRU operands
     and states, frames and push_audio.  Subclasses check their arguments, then call
-    _init_encoder."""
+    _init_encoder.  keep_f32: _decode also finds the fp32 top-layer states of the frames it
+    searches (post-lookahead) in self.y32, laid out as its bf16 operand."""
+
+    keep_f32 = False
 
     @staticmethod
     def _check(model, num_streams, beam_size, max_frames):
@@ -114,6 +117,7 @@ class EncoderStream:
         la = model.lookahead
         self.tau = 0 if la is None else la.kernel_size[0] - 1
         self.npend = [0] * B                     # top-layer frames held back for the lookahead
+        self.y32 = None              # with keep_f32: fp32 top-layer states of the frames searched
         if self.tau:
             with torch.no_grad():
                 self.taps = ops.lookahead_taps(la.weight, H, Hp)
@@ -227,13 +231,15 @@ class EncoderStream:
         h = src[torch.from_numpy(idx.reshape(-1)).to(dev)]
         lens = torch.tensor(tot + [0] * (Bp - B), dtype=torch.int32).to(dev)
         rb = torch.empty(Tl * Bp, Hp, dtype=torch.bfloat16, device=dev)
-        ops.lookahead_fwd(h, self.taps, lens, None, rb, Tl, Bp, Hp, tau)
+        r = torch.empty(Tl * Bp, Hp, dtype=torch.float32, device=dev) if self.keep_f32 else None
+        ops.lookahead_fwd(h, self.taps, lens, r, rb, Tl, Bp, Hp, tau)
         pidx = np.full((B, tau), Tl * Bp, np.int64)
         for b in range(B):
             pidx[b, :keep[b]] = (emit[b] + np.arange(keep[b])) * Bp + b
         self.npend = keep
         self.pend = torch.cat([h, h.new_zeros(1, Hp)])[torch.from_numpy(pidx.reshape(-1)).to(dev)]
         Te = max(emit)
+        self.y32 = None if r is None else r[:Te * Bp]
         return emit, Te, rb[:Te * Bp]
 
     def push(self, chunks):
@@ -261,6 +267,7 @@ class EncoderStream:
         t * Bp + b)"""
         X, Y = self._encoder(xs, counts, T)
         if not self.tau:
+            self.y32 = Y if self.keep_f32 else None
             return counts, T, X
         return self._lookahead(Y, counts, T, ())
 
@@ -460,3 +467,105 @@ class TransducerStream(EncoderStream):
         labels, scores = self.search.best()
         res = [tuple(int(v) for v in lab) for lab in labels]
         return list(zip(res, scores)) if return_scores else res
+
+
+class Seq2SeqStream(EncoderStream):
+    """B streams of two-pass recognition with one hybrid CTC/attention Seq2Seq (unidirectional
+    encoder, CTC head).  Built by Seq2Seq.stream; the model's weights are read once, when the
+    stream is built.
+
+    First pass, per push: the CTC head (ctc_fc with bias) on the top layer's new bf16 states, on
+    the wgmma GEMM with the padded weights of the offline ops.linear, a float32 log_softmax, and one
+    step of the resumable prefix beam search (sb_ctc_stream_step, blank V - 2, no LM).  The fp32
+    top-layer states of the frames searched (post-lookahead: the values Seq2Seq._encode returns)
+    are appended to a per-stream arena of B * max_frames * H * 4 bytes.
+    partial() is the first pass's best so far; rescored() reads every stream's N-best
+    (sb_ctc_stream_nbest) and runs the attention rescoring of Seq2Seq.recognize_two_pass over the
+    frames searched so far.  After finish(), rescored(return_scores=True) equals
+    recognize_two_pass(inputs, return_scores=True) bit for bit in the exact-lengths mode with the
+    same B, where the offline ctc_fc runs on the GEMM (B * T' >= 128 or H not a multiple of 8, as
+    for TransducerStream)."""
+
+    keep_f32 = True
+
+    def __init__(self, model, num_streams, beam_size=10, max_frames=3000, ctc_weight=0.5):
+        B = self._check(model, num_streams, beam_size, max_frames)
+        model._check_two_pass(beam_size, ctc_weight)
+        self._init_encoder(model, B, max_frames, "Seq2Seq.stream")
+        from .functions import s2s
+        self.K, self.ctc_weight = int(beam_size), float(ctc_weight)
+        self.blank = model.embedding.num_embeddings - 2
+        self.Kr = ops._round_up(self.H, 8)     # the contraction of the offline ops.linear
+        with torch.no_grad():
+            fc = model.ctc_fc.fc
+            self.fc_w = torch.nn.functional.pad(fc.weight.detach().to(torch.bfloat16),
+                                                (0, self.Kr - self.H)).contiguous()
+            self.fc_b = fc.bias.detach().float().contiguous()
+        self.arena = torch.zeros(B, self.max_frames, self.H, dtype=torch.float32, device=self.dev)
+        self.searched = [0] * B
+        self.state = s2s.ctc_stream_state(B, self.max_frames, self.K, self.dev)
+
+    def reset(self, b):
+        """start slot b afresh: conv carry, GRU states, pending frames, search and arena"""
+        lib = _lib.load()
+        b = self._reset_encoder(b)
+        self.searched[b] = 0
+        self.arena[b].zero_()
+        with torch.cuda.device(self.dev):
+            ops._launch("ctc_stream_reset", 0.0,
+                        lambda: lib.sb_ctc_stream_reset(self.state.data_ptr(), self.B,
+                                                        self.max_frames, self.K, b, 1,
+                                                        _lib.stream_ptr()))
+
+    def _decode(self, X, counts, T):
+        from .functions import s2s
+        B, Bp, H = self.B, self.Bp, self.H
+        logits = ops.gemm_bf16_tn(X[:, :self.Kr], self.fc_w, bias=self.fc_b)
+        y = logits.view(T, Bp, -1)[:, :B].transpose(0, 1).contiguous()
+        y = torch.log_softmax(y.float(), dim=-1).contiguous()
+        with torch.cuda.device(self.dev):
+            s2s.ctc_stream_step(self.state, y, counts, self.K, self.blank, self.max_frames)
+        src, dst = [], []
+        for b, n in enumerate(counts):
+            src += [t * Bp + b for t in range(n)]
+            dst += [b * self.max_frames + self.searched[b] + t for t in range(n)]
+            self.searched[b] += n
+        if src:
+            rows = self.y32[torch.tensor(src, device=self.dev), :H]
+            self.arena.view(-1, H).index_copy_(0, torch.tensor(dst, device=self.dev), rows)
+
+    def partial(self, return_scores=False):
+        """Best label list of each stream so far, the first pass alone (one device-to-host copy);
+        with return_scores, (labels, score) pairs, the score -c_0 as CTCStream.partial reports it."""
+        lib = _lib.load()
+        B, Tm = self.B, self.max_frames
+        off = B * Tm + 2 * B + (B * Tm) % 2          # float64 scores 8-byte aligned
+        buf = torch.empty(off + 2 * B, dtype=torch.int32, device=self.dev)
+        labels, lens, ovf = buf[:B * Tm], buf[B * Tm:B * Tm + B], buf[B * Tm + B:B * Tm + 2 * B]
+        scores = buf[off:].view(torch.float64)
+        with torch.cuda.device(self.dev):
+            ops._launch("ctc_stream_best", 0.0,
+                        lambda: lib.sb_ctc_stream_best(self.state.data_ptr(), B, Tm, self.K,
+                                                       labels.data_ptr(), lens.data_ptr(),
+                                                       scores.data_ptr(), ovf.data_ptr(),
+                                                       _lib.stream_ptr()))
+        host = buf.cpu()
+        lab = host[:B * Tm].view(B, Tm).numpy()
+        n = host[B * Tm:B * Tm + B].numpy()
+        sc = host[off:].view(torch.float64).numpy()
+        res = [tuple(int(v) for v in lab[b, :n[b]]) for b in range(B)]
+        return [(r, float(s)) for r, s in zip(res, sc)] if return_scores else res
+
+    def rescored(self, return_scores=False):
+        """The second pass over every stream's frames searched so far: each stream's N-best
+        rescored by the attention as Seq2Seq.recognize_two_pass does; -> its output.  Raises
+        ValueError while a stream has searched no frame (the attention needs one)."""
+        from .functions import s2s
+        empty = [b for b, f in enumerate(self.searched) if f == 0]
+        if empty:
+            raise ValueError("streams %s have searched no frame yet" % empty)
+        T = max(self.searched)
+        with torch.no_grad(), torch.cuda.device(self.dev):
+            nbest = s2s.ctc_nbest(self.state, self.B, self.max_frames, self.K, self.dev)
+            return s2s.rescore(self.model, self.arena[:, :T], nbest, list(self.searched), self.K,
+                               self.ctc_weight, return_scores)

@@ -36,7 +36,8 @@ s2s_fn.beam_select_fits = lambda K, C: False     # the split selection with the 
 print("seq2seq recognize with LM, split select", [len(h) for h in s.recognize(
     inputs, beam_size=3, max_len=8, lm=lm2, lm_weight=0.5, insertion_bonus=1.0)])
 s2s_fn.beam_select_fits = fits
-sc = Seq2Seq(80, 30, dict(cfg, decoder={"embedding_dim": 256, "layers": 1, "ctc_weight": 0.3})).cuda()
+sc_dec = {"embedding_dim": 256, "layers": 1, "ctc_weight": 0.3}
+sc = Seq2Seq(80, 30, dict(cfg, decoder=sc_dec)).cuda()
 lc = sc.loss((inputs, lab2)); lc.backward()
 print("seq2seq joint CTC loss", lc.item(), "recognize", [len(h) for h in sc.recognize(
     inputs, beam_size=3, max_len=8, ctc_weight=0.3)], "with LM", [len(h) for h in sc.recognize(
@@ -54,6 +55,14 @@ print("seq2seq recognize with a word LM, split select",
 s2s_fn.beam_select_fits = fits
 print("seq2seq joint CTC with a word LM",
       [len(h) for h in sc.recognize(inputs, ctc_weight=0.3, **wargs)])
+scu = Seq2Seq(80, 30, dict(cfg, encoder=dict(cfg["encoder"], lookahead=2, rnn=dict(
+    cfg["encoder"]["rnn"], bidirectional=False)), decoder=sc_dec)).cuda()
+print("seq2seq two-pass", [len(h) for h in scu.recognize_two_pass(inputs, beam_size=4)])
+sst = scu.stream(2, beam_size=4, max_frames=100)
+for k in range(0, 60, 20):
+    sst.push([inputs[0][k:k + 20], inputs[1][k:k + 20]])
+sst.finish()
+print("seq2seq two-pass stream", sst.partial(), [len(h) for h in sst.rescored()])
 t = Transducer(80, 28, cfg).cuda()
 l3 = t.loss((inputs, labels)); l3.backward()
 print("transducer ok", l3.item())
