@@ -9,7 +9,8 @@ reads the final hypotheses back once.
 import torch
 
 from .. import _lib, ops
-from ..lm import WordLM
+from ..lm import NGramLM, WordLM, fusion_args, fusion_kind
+from ..models.ctc_decoder import StreamSearch
 
 
 def _f(t):
@@ -28,6 +29,19 @@ DOUT_MAX_CLASSES = 8192
 BEAM_DONE_OFFSET = 0
 BEAM_OUT_LEN_OFFSET = 4
 BEAM_MAX_WIDTH = 32
+# the beam search's per-step entry point by route and LM kind: (ops._launch name, symbol).  On the
+# joint CTC/attention route it builds the candidates, and sb_s2s_ctc_select_batch selects.
+_SELECT = {
+    ("single", None): ("s2s_beam_select", "sb_s2s_beam_select_batch"),
+    ("single", NGramLM): ("s2s_beam_select_lm", "sb_s2s_beam_select_lm_batch"),
+    ("single", WordLM): ("s2s_beam_select_wordlm", "sb_s2s_beam_select_wordlm_batch"),
+    ("split", None): ("s2s_beam_select_split", "sb_s2s_beam_select_split_batch"),
+    ("split", NGramLM): ("s2s_beam_select_split_lm", "sb_s2s_beam_select_split_lm_batch"),
+    ("split", WordLM): ("s2s_beam_select_split_wordlm", "sb_s2s_beam_select_split_wordlm_batch"),
+    ("ctc", None): ("s2s_ctc_candidates", "sb_s2s_ctc_candidates"),
+    ("ctc", NGramLM): ("s2s_ctc_candidates", "sb_s2s_ctc_candidates"),
+    ("ctc", WordLM): ("s2s_ctc_candidates", "sb_s2s_ctc_candidates_wordlm"),
+}
 
 
 def fc_fused(H, C):
@@ -527,14 +541,11 @@ def beam_search_batch(m, eh, start_tok, end_tok, beam_size, max_len, lens=None, 
     p_state, p_c, p_nodes = state.data_ptr(), c_scores.data_ptr(), nodes.data_ptr()
     p_par, p_tok, p_out = parent.data_ptr(), tok.data_ptr(), out_tokens.data_ptr()
     p_stop = stop.data_ptr()
-    fusion = (None, 0.0, 0.0)
-    word = isinstance(lm, WordLM)
-    if lm is not None:
-        tables, _ = lm.device_tables(dev)
-        fusion = (tables, float(lm_weight), float(insertion_bonus))
-    if word:
+    kind = fusion_kind(lm)
+    fusion = fusion_args(lm, lm_weight, insertion_bonus, dev)
+    if kind is WordLM:
         word_nodes = torch.empty(B, node_cap, 3, dtype=torch.int32, device=dev)
-        fusion += (float(lm.oov_penalty), word_nodes.data_ptr())
+        fusion += (word_nodes.data_ptr(),)
     if ctc is not None:
         y, lam, M = ctc
         if tuple(y.shape) != (B, T, C) or y.dtype != torch.float32 or y.device != ehc.device:
@@ -547,6 +558,15 @@ def beam_search_batch(m, eh, start_tok, end_tok, beam_size, max_len, lens=None, 
         cargs = (y.data_ptr(), _a(ctc_ld), cbuf.data_ptr(), cbuf.numel())
         shape = (K, C, M, T, int(start_tok), int(end_tok), lam)
         _lib.check(lib.sb_s2s_ctc_init(*cargs, *shape, B, sp), "ctc init")
+        # the joint candidates take a null LM where there is none
+        head = (cargs[0], cargs[1], p_state, p_nodes, node_cap, cargs[2], cargs[3], *shape)
+        tail = (p_stop, B, *(fusion or (None, 0.0, 0.0)))
+    else:
+        head = (p_state, p_c, p_nodes, p_par, p_tok, p_out, K, C, int(end_tok))
+        tail = (max_len, node_cap, c_cap, p_stop, B,
+                *((sel_ws.data_ptr(), sel_ws.numel()) if split else ()), *fusion)
+    name, symbol = _SELECT["ctc" if ctc is not None else "split" if split else "single", kind]
+    select = getattr(lib, symbol)
     # buffers: [0] = state entering the step (gathered), [1] = state produced by the step
     for e in range(max_len):
         _cell_fwd(lib, w, p_tok, 1, sx[0] if e > 0 else None, hx[0], hx[1], None, None, done_ptr,
@@ -559,42 +579,11 @@ def beam_search_batch(m, eh, start_tok, end_tok, beam_size, max_len, lens=None, 
                       done=done_ptr, with_fc=False, lens=ld)
             _fc_rows(lib, w, fc_ws, hx[1], sx[1], R, sp, logits=logp, done=done_ptr)
             _fc_logp(lib, w, fc_ws, logp, logp, R, sp, done=done_ptr)
+        ops._launch(name, 0.0, lambda: select(logp.data_ptr(), *head, e, *tail, sp))
         if ctc is not None:
-            cand = lib.sb_s2s_ctc_candidates_wordlm if word else lib.sb_s2s_ctc_candidates
-            ops._launch("s2s_ctc_candidates", 0.0, lambda: cand(
-                logp.data_ptr(), cargs[0], cargs[1], p_state, p_nodes, node_cap, cargs[2],
-                cargs[3], *shape, e, p_stop, B, *fusion, sp))
             ops._launch("s2s_ctc_select", 0.0, lambda: lib.sb_s2s_ctc_select_batch(
                 *cargs, p_state, p_c, p_nodes, p_par, p_tok, p_out, *shape, e, max_len, node_cap,
                 c_cap, p_stop, B, sp))
-        elif word and split:
-            ops._launch("s2s_beam_select_split_wordlm", 0.0,
-                        lambda: lib.sb_s2s_beam_select_split_wordlm_batch(
-                            logp.data_ptr(), p_state, p_c, p_nodes, p_par, p_tok, p_out, K, C,
-                            int(end_tok), e, max_len, node_cap, c_cap, p_stop, B,
-                            sel_ws.data_ptr(), sel_ws.numel(), *fusion, sp))
-        elif word:
-            ops._launch("s2s_beam_select_wordlm", 0.0, lambda: lib.sb_s2s_beam_select_wordlm_batch(
-                logp.data_ptr(), p_state, p_c, p_nodes, p_par, p_tok, p_out, K, C, int(end_tok), e,
-                max_len, node_cap, c_cap, p_stop, B, *fusion, sp))
-        elif lm is not None and split:
-            ops._launch("s2s_beam_select_split_lm", 0.0,
-                        lambda: lib.sb_s2s_beam_select_split_lm_batch(
-                            logp.data_ptr(), p_state, p_c, p_nodes, p_par, p_tok, p_out, K, C,
-                            int(end_tok), e, max_len, node_cap, c_cap, p_stop, B,
-                            sel_ws.data_ptr(), sel_ws.numel(), *fusion, sp))
-        elif lm is not None:
-            ops._launch("s2s_beam_select_lm", 0.0, lambda: lib.sb_s2s_beam_select_lm_batch(
-                logp.data_ptr(), p_state, p_c, p_nodes, p_par, p_tok, p_out, K, C, int(end_tok), e,
-                max_len, node_cap, c_cap, p_stop, B, *fusion, sp))
-        elif split:
-            ops._launch("s2s_beam_select_split", 0.0, lambda: lib.sb_s2s_beam_select_split_batch(
-                logp.data_ptr(), p_state, p_c, p_nodes, p_par, p_tok, p_out, K, C, int(end_tok), e,
-                max_len, node_cap, c_cap, p_stop, B, sel_ws.data_ptr(), sel_ws.numel(), sp))
-        else:
-            ops._launch("s2s_beam_select", 0.0, lambda: lib.sb_s2s_beam_select_batch(
-                logp.data_ptr(), p_state, p_c, p_nodes, p_par, p_tok, p_out, K, C, int(end_tok), e,
-                max_len, node_cap, c_cap, p_stop, B, sp))
         ops._launch("s2s_beam_gather", 0.0, lambda: lib.sb_s2s_beam_gather_batch(
             hx[1].data_ptr(), sx[1].data_ptr(), ax[1].data_ptr(), hx[0].data_ptr(),
             sx[0].data_ptr(), ax[0].data_ptr(), p_par, p_state, K, H, T, B, sp))
@@ -610,53 +599,15 @@ def beam_search_batch(m, eh, start_tok, end_tok, beam_size, max_len, lens=None, 
 
 # ---- two-pass decoding: CTC prefix beam search N-best, then attention rescoring ----------------
 
-def ctc_nbest(state, B, max_frames, K, dev):
-    """Every stored beam entry of the B streams of a CTC stream state (sb_ctc_stream_nbest): ->
-    labels (B, K, max_frames) int32, lens (B, K) int32 (-1: empty slot), c (B, K) float64
-    log-probabilities lse(p_b, p_nb) (-inf: empty slot), in the search's stored order."""
-    lib = _lib.load()
-    labels = torch.empty(B, K, max_frames, dtype=torch.int32, device=dev)
-    lens = torch.empty(B, K, dtype=torch.int32, device=dev)
-    c = torch.empty(B, K, dtype=torch.float64, device=dev)
-    count = torch.empty(B, dtype=torch.int32, device=dev)
-    ops._launch("ctc_stream_nbest", 0.0, lambda: lib.sb_ctc_stream_nbest(
-        _a(state), B, max_frames, K, labels.data_ptr(), lens.data_ptr(), c.data_ptr(),
-        count.data_ptr(), _lib.stream_ptr()))
-    return labels, lens, c
-
-
-def ctc_stream_state(B, max_frames, K, dev):
-    """a fresh (reset) LM-less CTC stream state of B streams"""
-    lib = _lib.load()
-    state = torch.empty(_lib.workspace_size(lib.sb_ctc_stream_state_size, B, max_frames, K, 0),
-                        dtype=torch.uint8, device=dev)
-    ops._launch("ctc_stream_reset", 0.0, lambda: lib.sb_ctc_stream_reset(
-        state.data_ptr(), B, max_frames, K, 0, B, _lib.stream_ptr()))
-    return state
-
-
-def ctc_stream_step(state, y, n, K, blank, max_frames):
-    """advance the B streams of `state` by n[b] frames of y (B, T, C) float32 log-probabilities
-    (sb_ctc_stream_step, no LM)"""
-    lib = _lib.load()
-    B, T, C = y.shape
-    nd = torch.tensor(list(n), dtype=torch.int32).to(y.device)
-    ws_bytes = _lib.workspace_size(lib.sb_ctc_stream_workspace_size, B, T, K)
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=y.device)
-    ops._launch("ctc_stream_step", 0.0, lambda: lib.sb_ctc_stream_step(
-        y.data_ptr(), nd.data_ptr(), B, T, C, K, blank, max_frames, state.data_ptr(),
-        ws.data_ptr(), ws_bytes, _lib.stream_ptr()))
-
-
 def ctc_first_pass(y, frames, K):
     """The first pass over whole utterances: y (B, T, C) float32 CTC log-probabilities (blank
     C - 1), frames[b] <= T the frames of utterance b.  One reset, one step over all T frames and
     one N-best read: the streaming path, whose entry 0 is sb_ctc_prefix_beam's result.
-    -> ctc_nbest's (labels, lens, c)."""
+    -> ctc_decoder.StreamSearch.nbest's (labels, lens, c)."""
     B, T, C = y.shape
-    state = ctc_stream_state(B, T, K, y.device)
-    ctc_stream_step(state, y, frames, K, C - 1, T)
-    return ctc_nbest(state, B, T, K, y.device)
+    search = StreamSearch(B, T, K, C - 1, y.device)
+    search.push(y, frames)
+    return search.nbest()
 
 
 def score_batch(m, eh, tokens, lens, K, frame_lens=None):
@@ -720,8 +671,9 @@ def two_pass_select(a, c, valid, ctc_weight):
 
 
 def rescore(m, eh, nbest, frame_lens, K, ctc_weight, return_scores):
-    """The second pass over a first pass's N-best (ctc_nbest's output, utterance b's entries over
-    eh[b]) and the selection: -> B token lists [START] + y + [END] (and their float64 scores r).
+    """The second pass over a first pass's N-best (StreamSearch.nbest's output, utterance b's
+    entries over eh[b]) and the selection: -> B token lists [START] + y + [END] (and their float64
+    scores r).
     Reads the longest hypothesis's length before the step loop and the chosen hypotheses once at
     the end: two device-to-host copies per call."""
     labels, lens, c = nbest

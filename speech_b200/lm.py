@@ -726,6 +726,23 @@ class WordLM:
         self.__dict__.update(d)
 
 
+def fusion_kind(lm):
+    """None, NGramLM or WordLM: the key of each search's table of entry points"""
+    return None if lm is None else WordLM if isinstance(lm, WordLM) else NGramLM
+
+
+def fusion_args(lm, lm_weight, insertion_bonus, device):
+    """The C arguments of shallow fusion with `lm` on `device`, as every fused entry point takes
+    them: () without an LM, (SbNgramLm, lm_weight, insertion_bonus) for an NGramLM and
+    (SbWordLm, lm_weight, insertion_bonus, oov_penalty) for a WordLM.  The tables are built once
+    per device; oov_penalty is read at each call, since it is settable."""
+    if lm is None:
+        return ()
+    tables, _ = lm.device_tables(device)
+    args = (tables, float(lm_weight), float(insertion_bonus))
+    return args + (float(lm.oov_penalty),) if isinstance(lm, WordLM) else args
+
+
 def _delimiter_class(symbols, blank, delimiter, end=None):
     """the one class but the blank and the end whose symbol is `delimiter`"""
     cs = [c for c, s in enumerate(symbols) if c != blank and c != end and s == delimiter]

@@ -13,14 +13,28 @@ Both take an optional n-gram LM for shallow fusion, and the returned score is th
     per word; a word leaving the lexicon is charged the LM's oov_penalty once, and the end of the
     utterance adds the trailing word and </s> (sb_ctc_prefix_beam_wordlm, include/speech_b200.h).
 Without an LM the calls are the LM-less search.
+
+`StreamSearch` owns the state of the resumable search (sb_ctc_stream_*) that CTC.stream,
+Seq2Seq.stream and the attention model's two-pass first pass advance frame by frame.
 """
 import math
 
 import numpy as np
 import torch
 
-from .. import _lib
-from ..lm import WordLM
+from .. import _lib, ops
+from ..lm import NGramLM, WordLM, fusion_args, fusion_kind
+
+# entry points by LM kind, and the stream's with their ops._launch profile names
+_OFFLINE = {None: "sb_ctc_prefix_beam", NGramLM: "sb_ctc_prefix_beam_lm",
+            WordLM: "sb_ctc_prefix_beam_wordlm"}
+_STREAM_STEP = {None: ("ctc_stream_step", "sb_ctc_stream_step"),
+                NGramLM: ("ctc_stream_step_lm", "sb_ctc_stream_step_lm"),
+                WordLM: ("ctc_stream_step_wordlm", "sb_ctc_stream_step_wordlm")}
+# only a word LM changes the ranking at the end (the partial word and </s>)
+_STREAM_BEST = {None: ("ctc_stream_best", "sb_ctc_stream_best"),
+                NGramLM: ("ctc_stream_best", "sb_ctc_stream_best"),
+                WordLM: ("ctc_stream_best_wordlm", "sb_ctc_stream_best_wordlm")}
 
 
 def check_lm(lm, lm_weight, insertion_bonus, num_classes, blank, search="CTC"):
@@ -51,35 +65,23 @@ def _run(logp, lens, beam_size, blank, lm=None, lm_weight=0.0, insertion_bonus=0
     lib = _lib.load()
     B, T, S = logp.shape
     dev = logp.device
-    if lm is None or isinstance(lm, WordLM):
-        nbytes = _lib.workspace_size(lib.sb_ctc_prefix_beam_workspace_size, B, T, beam_size)
-    else:
+    kind = fusion_kind(lm)
+    if kind is NGramLM:
         nbytes = _lib.workspace_size(lib.sb_ctc_prefix_beam_lm_workspace_size, B, T, beam_size,
                                      lm.order)
+    else:
+        nbytes = _lib.workspace_size(lib.sb_ctc_prefix_beam_workspace_size, B, T, beam_size)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     out_labels = torch.empty(B, T, dtype=torch.int32, device=dev)
     out_lens = torch.empty(B, dtype=torch.int32, device=dev)
     out_scores = torch.empty(B, dtype=torch.float64, device=dev)
     outs = (out_labels.data_ptr(), out_lens.data_ptr(), out_scores.data_ptr(), ws.data_ptr(),
             nbytes, _lib.stream_ptr())
+    name = _OFFLINE[kind]
     with torch.cuda.device(dev):
-        if lm is None:
-            _lib.check(lib.sb_ctc_prefix_beam(logp.data_ptr(), lens.data_ptr(), B, T, S,
-                                              int(beam_size), int(blank), *outs),
-                       "sb_ctc_prefix_beam")
-        elif isinstance(lm, WordLM):
-            tables, _ = lm.device_tables(dev)
-            _lib.check(lib.sb_ctc_prefix_beam_wordlm(logp.data_ptr(), lens.data_ptr(), B, T, S,
-                                                     int(beam_size), int(blank), tables,
-                                                     float(lm_weight), float(insertion_bonus),
-                                                     lm.oov_penalty, *outs),
-                       "sb_ctc_prefix_beam_wordlm")
-        else:
-            tables, _ = lm.device_tables(dev)
-            _lib.check(lib.sb_ctc_prefix_beam_lm(logp.data_ptr(), lens.data_ptr(), B, T, S,
-                                                 int(beam_size), int(blank), tables,
-                                                 float(lm_weight), float(insertion_bonus), *outs),
-                       "sb_ctc_prefix_beam_lm")
+        fusion = fusion_args(lm, lm_weight, insertion_bonus, dev)
+        _lib.check(getattr(lib, name)(logp.data_ptr(), lens.data_ptr(), B, T, S, int(beam_size),
+                                      int(blank), *fusion, *outs), name)
     labels = out_labels.cpu().numpy()
     n = out_lens.cpu().numpy()
     scores = out_scores.cpu().numpy()
@@ -122,3 +124,87 @@ def decode(probs, beam_size=10, blank=0, lm=None, lm_weight=0.0, insertion_bonus
     lp = torch.from_numpy(np.ascontiguousarray(logp, dtype=np.float32))[None].cuda()
     lens = torch.full((1,), lp.shape[1], dtype=torch.int32, device=lp.device)
     return _run(lp, lens, beam_size, blank, lm, lm_weight, insertion_bonus)[0]
+
+
+class StreamSearch:
+    """The resumable prefix beam search of B streams (sb_ctc_stream_*): each stream's beam stays
+    on the device between pushes, for up to max_frames frames per stream between resets.  lm,
+    lm_weight, insertion_bonus: as decode_batch (the caller checks them); a WordLM's oov_penalty
+    is read at each launch."""
+
+    def __init__(self, B, max_frames, beam_size, blank, device, lm=None, lm_weight=0.0,
+                 insertion_bonus=0.0):
+        lib = _lib.load()
+        self.B, self.Tm, self.K, self.blank, self.dev = (int(B), int(max_frames), int(beam_size),
+                                                         int(blank), device)
+        self.lm, self.lm_weight, self.insertion_bonus = lm, lm_weight, insertion_bonus
+        self.kind = fusion_kind(lm)
+        nbytes = _lib.workspace_size(lib.sb_ctc_stream_state_size, self.B, self.Tm, self.K,
+                                     0 if lm is None else lm.order)
+        self.state = torch.empty(nbytes, dtype=torch.uint8, device=device)
+        self.reset(0, self.B)
+
+    def _fusion(self):
+        return fusion_args(self.lm, self.lm_weight, self.insertion_bonus, self.dev)
+
+    def reset(self, first, count):
+        """streams first .. first + count - 1 back to the empty prefix at frame 0"""
+        lib = _lib.load()
+        with torch.cuda.device(self.dev):
+            ops._launch("ctc_stream_reset", 0.0, lambda: lib.sb_ctc_stream_reset(
+                self.state.data_ptr(), self.B, self.Tm, self.K, first, count, _lib.stream_ptr()))
+
+    def push(self, logp, counts):
+        """advance stream b by counts[b] frames of logp (B, T, S), contiguous float32
+        log-probabilities"""
+        lib = _lib.load()
+        B, T, S = logp.shape
+        n = torch.tensor(list(counts), dtype=torch.int32).to(self.dev)
+        ws_bytes = _lib.workspace_size(lib.sb_ctc_stream_workspace_size, B, T, self.K)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=self.dev)
+        name, symbol = _STREAM_STEP[self.kind]
+        with torch.cuda.device(self.dev):
+            fusion = self._fusion()
+            ops._launch(name, 0.0, lambda: getattr(lib, symbol)(
+                logp.data_ptr(), n.data_ptr(), B, T, S, self.K, self.blank, *fusion, self.Tm,
+                self.state.data_ptr(), ws.data_ptr(), ws_bytes, _lib.stream_ptr()))
+
+    def best(self, return_scores=False):
+        """Best label tuple of each stream so far (one device-to-host copy); with return_scores,
+        (labels, score) pairs, the score as decode_batch(with_scores=True) reports it.  With a
+        WordLM the stored beams are ranked by the end-of-utterance rule, as if each stream ended
+        here (its partial word completed, then </s>)."""
+        lib = _lib.load()
+        B, Tm = self.B, self.Tm
+        off = B * Tm + 2 * B + (B * Tm) % 2          # float64 scores 8-byte aligned
+        buf = torch.empty(off + 2 * B, dtype=torch.int32, device=self.dev)
+        labels, lens, ovf = buf[:B * Tm], buf[B * Tm:B * Tm + B], buf[B * Tm + B:B * Tm + 2 * B]
+        scores = buf[off:].view(torch.float64)
+        name, symbol = _STREAM_BEST[self.kind]
+        with torch.cuda.device(self.dev):
+            fusion = self._fusion() if self.kind is WordLM else ()
+            ops._launch(name, 0.0, lambda: getattr(lib, symbol)(
+                self.state.data_ptr(), B, Tm, self.K, *fusion, labels.data_ptr(), lens.data_ptr(),
+                scores.data_ptr(), ovf.data_ptr(), _lib.stream_ptr()))
+        host = buf.cpu()
+        lab = host[:B * Tm].view(B, Tm).numpy()
+        n = host[B * Tm:B * Tm + B].numpy()
+        sc = host[off:].view(torch.float64).numpy()
+        res = [tuple(int(v) for v in lab[b, :n[b]]) for b in range(B)]
+        return [(r, float(s)) for r, s in zip(res, sc)] if return_scores else res
+
+    def nbest(self):
+        """Every stored beam entry of every stream (sb_ctc_stream_nbest), on the device: labels
+        (B, K, max_frames) int32, lens (B, K) int32 (-1: empty slot), c (B, K) float64
+        log-probabilities lse(p_b, p_nb) (-inf: empty slot), in the search's stored order"""
+        lib = _lib.load()
+        B, Tm, K, dev = self.B, self.Tm, self.K, self.dev
+        labels = torch.empty(B, K, Tm, dtype=torch.int32, device=dev)
+        lens = torch.empty(B, K, dtype=torch.int32, device=dev)
+        c = torch.empty(B, K, dtype=torch.float64, device=dev)
+        count = torch.empty(B, dtype=torch.int32, device=dev)
+        with torch.cuda.device(dev):
+            ops._launch("ctc_stream_nbest", 0.0, lambda: lib.sb_ctc_stream_nbest(
+                self.state.data_ptr(), B, Tm, K, labels.data_ptr(), lens.data_ptr(),
+                c.data_ptr(), count.data_ptr(), _lib.stream_ptr()))
+        return labels, lens, c

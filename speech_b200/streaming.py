@@ -11,7 +11,7 @@ Every stage carries what the next chunk needs and nothing more (EncoderStream, s
   * GRU layers: the input projection, then the recurrence from each stream's carried state
     (sb_gru_fwd_h0); the new state is the fp32 y and bf16 xn at the stream's last new frame.
 CTCStream then runs the fused projection, softmax and log as CTC.infer computes them, and one step
-of the resumable prefix beam search (sb_ctc_stream_step[_lm|_wordlm]), whose beams stay on the
+of the resumable prefix beam search (models.ctc_decoder.StreamSearch), whose beams stay on the
 device.
 With B streams, the final partial(return_scores=True) equals decode_batch(with_scores=True) on the
 logits of CTC.infer over the same B utterances in the exact-lengths mode, bit for bit: each stage
@@ -47,8 +47,7 @@ import numpy as np
 import torch
 
 from . import _lib, features, ops
-from .lm import WordLM
-from .models.ctc_decoder import check_lm
+from .models.ctc_decoder import StreamSearch, check_lm
 
 MAX_STREAMS = ops.GRU_MAX_BATCH   # one recurrence launch per layer and push
 
@@ -328,32 +327,18 @@ class CTCStream(EncoderStream):
         B = self._check(model, num_streams, beam_size, max_frames)
         check_lm(lm, lm_weight, insertion_bonus, model.blank + 1, model.blank)
         self._init_encoder(model, B, max_frames, "CTC.stream")
-        lib = _lib.load()
-        self.K = int(beam_size)
-        self.lm, self.lm_weight, self.insertion_bonus = lm, float(lm_weight), float(insertion_bonus)
         with torch.no_grad():
             self.fc_w = ops.fc_operand(model.fc.fc.weight, 1, self.H, self.Hp)
             self.fc_b = model.fc.fc.bias.detach().float().contiguous()
-        order = 0 if lm is None else lm.order
-        nbytes = _lib.workspace_size(lib.sb_ctc_stream_state_size, B, self.max_frames, self.K,
-                                     order)
-        self.state = torch.empty(nbytes, dtype=torch.uint8, device=self.dev)
-        self._reset_search(0, B)
-
-    def _reset_search(self, first, count):
-        lib = _lib.load()
-        with torch.cuda.device(self.dev):
-            ops._launch("ctc_stream_reset",  0.0,
-                        lambda: lib.sb_ctc_stream_reset(self.state.data_ptr(), self.B,
-                                                        self.max_frames, self.K, first, count,
-                                                        _lib.stream_ptr()))
+        self.search = StreamSearch(B, self.max_frames, beam_size, model.blank, self.dev, lm,
+                                   lm_weight, insertion_bonus)
 
     def reset(self, b):
         """start slot b afresh: conv carry, GRU states, pending frames and search"""
-        self._reset_search(self._reset_encoder(b), 1)
+        self.search.reset(self._reset_encoder(b), 1)
 
     def _decode(self, X, counts, T):
-        self._search(self._logp(X, T), counts)
+        self.search.push(self._logp(X, T), counts)
 
     def _logp(self, X, T):
         """(B, T, S) log-probabilities of the (T * Bp, Hp) bf16 top-layer operand X (rows past
@@ -365,62 +350,12 @@ class CTCStream(EncoderStream):
         probs = torch.nn.functional.softmax(out, dim=2)
         return torch.log(probs.float()).contiguous()
 
-    def _search(self, logp, counts):
-        lib = _lib.load()
-        B, T, S = logp.shape
-        n = torch.tensor(counts, dtype=torch.int32).to(self.dev)
-        ws_bytes = _lib.workspace_size(lib.sb_ctc_stream_workspace_size, B, T, self.K)
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=self.dev)
-        args = (self.max_frames, self.state.data_ptr(), ws.data_ptr(), ws_bytes, _lib.stream_ptr())
-        with torch.cuda.device(self.dev):
-            if self.lm is None:
-                ops._launch("ctc_stream_step", 0.0,
-                            lambda: lib.sb_ctc_stream_step(logp.data_ptr(), n.data_ptr(), B, T, S,
-                                                           self.K, self.model.blank, *args))
-            elif isinstance(self.lm, WordLM):
-                tables, _ = self.lm.device_tables(self.dev)
-                ops._launch("ctc_stream_step_wordlm", 0.0,
-                            lambda: lib.sb_ctc_stream_step_wordlm(
-                                logp.data_ptr(), n.data_ptr(), B, T, S, self.K, self.model.blank,
-                                tables, self.lm_weight, self.insertion_bonus, self.lm.oov_penalty,
-                                *args))
-            else:
-                tables, _ = self.lm.device_tables(self.dev)
-                ops._launch("ctc_stream_step_lm", 0.0,
-                            lambda: lib.sb_ctc_stream_step_lm(
-                                logp.data_ptr(), n.data_ptr(), B, T, S, self.K, self.model.blank,
-                                tables, self.lm_weight, self.insertion_bonus, *args))
-
     def partial(self, return_scores=False):
         """Best label list of each stream so far (one device-to-host copy); with return_scores,
         (labels, score) pairs, the score as decode_batch(with_scores=True) reports it.  With a
         WordLM the stored beams are ranked by the end-of-utterance rule, as if each stream ended
         here (its partial word completed, then </s>)."""
-        lib = _lib.load()
-        B, Tm = self.B, self.max_frames
-        off = B * Tm + 2 * B + (B * Tm) % 2          # float64 scores 8-byte aligned
-        buf = torch.empty(off + 2 * B, dtype=torch.int32, device=self.dev)
-        labels, lens, ovf = buf[:B * Tm], buf[B * Tm:B * Tm + B], buf[B * Tm + B:B * Tm + 2 * B]
-        scores = buf[off:].view(torch.float64)
-        outs = (labels.data_ptr(), lens.data_ptr(), scores.data_ptr(), ovf.data_ptr(),
-                _lib.stream_ptr())
-        with torch.cuda.device(self.dev):
-            if isinstance(self.lm, WordLM):
-                tables, _ = self.lm.device_tables(self.dev)
-                ops._launch("ctc_stream_best_wordlm", 0.0,
-                            lambda: lib.sb_ctc_stream_best_wordlm(
-                                self.state.data_ptr(), B, Tm, self.K, tables, self.lm_weight,
-                                self.insertion_bonus, self.lm.oov_penalty, *outs))
-            else:
-                ops._launch("ctc_stream_best", 0.0,
-                            lambda: lib.sb_ctc_stream_best(self.state.data_ptr(), B, Tm, self.K,
-                                                           *outs))
-        host = buf.cpu()
-        lab = host[:B * Tm].view(B, Tm).numpy()
-        n = host[B * Tm:B * Tm + B].numpy()
-        sc = host[off:].view(torch.float64).numpy()
-        res = [tuple(int(v) for v in lab[b, :n[b]]) for b in range(B)]
-        return [(r, float(s)) for r, s in zip(res, sc)] if return_scores else res
+        return self.search.best(return_scores)
 
 
 class TransducerStream(EncoderStream):
@@ -476,11 +411,11 @@ class Seq2SeqStream(EncoderStream):
 
     First pass, per push: the CTC head (ctc_fc with bias) on the top layer's new bf16 states, on
     the wgmma GEMM with the padded weights of the offline ops.linear, a float32 log_softmax, and one
-    step of the resumable prefix beam search (sb_ctc_stream_step, blank V - 2, no LM).  The fp32
+    step of the resumable prefix beam search (StreamSearch, blank V - 2, no LM).  The fp32
     top-layer states of the frames searched (post-lookahead: the values Seq2Seq._encode returns)
     are appended to a per-stream arena of B * max_frames * H * 4 bytes.
     partial() is the first pass's best so far; rescored() reads every stream's N-best
-    (sb_ctc_stream_nbest) and runs the attention rescoring of Seq2Seq.recognize_two_pass over the
+    (StreamSearch.nbest) and runs the attention rescoring of Seq2Seq.recognize_two_pass over the
     frames searched so far.  After finish(), rescored(return_scores=True) equals
     recognize_two_pass(inputs, return_scores=True) bit for bit in the exact-lengths mode with the
     same B, where the offline ctc_fc runs on the GEMM (B * T' >= 128 or H not a multiple of 8, as
@@ -492,9 +427,7 @@ class Seq2SeqStream(EncoderStream):
         B = self._check(model, num_streams, beam_size, max_frames)
         model._check_two_pass(beam_size, ctc_weight)
         self._init_encoder(model, B, max_frames, "Seq2Seq.stream")
-        from .functions import s2s
         self.K, self.ctc_weight = int(beam_size), float(ctc_weight)
-        self.blank = model.embedding.num_embeddings - 2
         self.Kr = ops._round_up(self.H, 8)     # the contraction of the offline ops.linear
         with torch.no_grad():
             fc = model.ctc_fc.fc
@@ -503,28 +436,22 @@ class Seq2SeqStream(EncoderStream):
             self.fc_b = fc.bias.detach().float().contiguous()
         self.arena = torch.zeros(B, self.max_frames, self.H, dtype=torch.float32, device=self.dev)
         self.searched = [0] * B
-        self.state = s2s.ctc_stream_state(B, self.max_frames, self.K, self.dev)
+        self.search = StreamSearch(B, self.max_frames, self.K,
+                                   model.embedding.num_embeddings - 2, self.dev)
 
     def reset(self, b):
         """start slot b afresh: conv carry, GRU states, pending frames, search and arena"""
-        lib = _lib.load()
         b = self._reset_encoder(b)
         self.searched[b] = 0
         self.arena[b].zero_()
-        with torch.cuda.device(self.dev):
-            ops._launch("ctc_stream_reset", 0.0,
-                        lambda: lib.sb_ctc_stream_reset(self.state.data_ptr(), self.B,
-                                                        self.max_frames, self.K, b, 1,
-                                                        _lib.stream_ptr()))
+        self.search.reset(b, 1)
 
     def _decode(self, X, counts, T):
-        from .functions import s2s
         B, Bp, H = self.B, self.Bp, self.H
         logits = ops.gemm_bf16_tn(X[:, :self.Kr], self.fc_w, bias=self.fc_b)
         y = logits.view(T, Bp, -1)[:, :B].transpose(0, 1).contiguous()
         y = torch.log_softmax(y.float(), dim=-1).contiguous()
-        with torch.cuda.device(self.dev):
-            s2s.ctc_stream_step(self.state, y, counts, self.K, self.blank, self.max_frames)
+        self.search.push(y, counts)
         src, dst = [], []
         for b, n in enumerate(counts):
             src += [t * Bp + b for t in range(n)]
@@ -537,24 +464,7 @@ class Seq2SeqStream(EncoderStream):
     def partial(self, return_scores=False):
         """Best label list of each stream so far, the first pass alone (one device-to-host copy);
         with return_scores, (labels, score) pairs, the score -c_0 as CTCStream.partial reports it."""
-        lib = _lib.load()
-        B, Tm = self.B, self.max_frames
-        off = B * Tm + 2 * B + (B * Tm) % 2          # float64 scores 8-byte aligned
-        buf = torch.empty(off + 2 * B, dtype=torch.int32, device=self.dev)
-        labels, lens, ovf = buf[:B * Tm], buf[B * Tm:B * Tm + B], buf[B * Tm + B:B * Tm + 2 * B]
-        scores = buf[off:].view(torch.float64)
-        with torch.cuda.device(self.dev):
-            ops._launch("ctc_stream_best", 0.0,
-                        lambda: lib.sb_ctc_stream_best(self.state.data_ptr(), B, Tm, self.K,
-                                                       labels.data_ptr(), lens.data_ptr(),
-                                                       scores.data_ptr(), ovf.data_ptr(),
-                                                       _lib.stream_ptr()))
-        host = buf.cpu()
-        lab = host[:B * Tm].view(B, Tm).numpy()
-        n = host[B * Tm:B * Tm + B].numpy()
-        sc = host[off:].view(torch.float64).numpy()
-        res = [tuple(int(v) for v in lab[b, :n[b]]) for b in range(B)]
-        return [(r, float(s)) for r, s in zip(res, sc)] if return_scores else res
+        return self.search.best(return_scores)
 
     def rescored(self, return_scores=False):
         """The second pass over every stream's frames searched so far: each stream's N-best
@@ -566,6 +476,5 @@ class Seq2SeqStream(EncoderStream):
             raise ValueError("streams %s have searched no frame yet" % empty)
         T = max(self.searched)
         with torch.no_grad(), torch.cuda.device(self.dev):
-            nbest = s2s.ctc_nbest(self.state, self.B, self.max_frames, self.K, self.dev)
-            return s2s.rescore(self.model, self.arena[:, :T], nbest, list(self.searched), self.K,
-                               self.ctc_weight, return_scores)
+            return s2s.rescore(self.model, self.arena[:, :T], self.search.nbest(),
+                               list(self.searched), self.K, self.ctc_weight, return_scores)

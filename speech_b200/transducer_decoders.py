@@ -15,11 +15,10 @@ best non-blank classes, csrc/tdecode.cu), with the same results bit for bit: the
 selection the lists cannot prove, and flagged utterances are searched again from lists of
 SHORTLIST_RERUN entries.
 """
-import ctypes
-
 import torch
 
 from . import _lib, ops
+from .lm import fusion_args
 
 SHORTLIST_RERUN = 64      # list length of the second search of flagged utterances (the maximum)
 
@@ -184,28 +183,27 @@ class SearchSlots:
 
 
 def _search_frame(lib, provider, slots, tl_dev, t, cur, max_len, blank, ws, nbytes, sp,
-                  lm_args=None):
+                  lm_args=()):
     """the launches of frame t: per level the provider's rows, the round (with an LM first the
-    fused rows, lm_args = (tables, lm_weight, insertion_bonus)) and the new frontier's states,
-    then frame_end into block S + 1 - cur.  slots.T sizes the workspace, t < slots.T."""
+    fused rows, lm_args = lm.fusion_args(...)) and the new frontier's states, then frame_end into
+    block S + 1 - cur.  slots.T sizes the workspace, t < slots.T."""
     B, K, S, T, kp, V1 = slots.B, slots.K, slots.S, slots.T, slots.kp, provider.V1
     sl = slots.sl
     for level in range(S + 1):
         block = cur if level == 0 else level
         provider.rows(t, block, slots)
-        if lm_args is None:
+        if not lm_args:
             ops._launch("rnnt_search", 0.0, lambda: lib.sb_rnnt_search_round(
                 _lib.ptr(slots.lp), *(_lib.ptr(a) for a in (sl or (None,) * 3)), kp or 0,
                 tl_dev.data_ptr(), t, level, max_len, slots.par.data_ptr(),
                 slots.sym.data_ptr(), slots.slot_lens.data_ptr(), B, T, S, V1, K, blank,
                 ws.data_ptr(), nbytes, sp))
         else:
-            tables, weight, bonus = lm_args
             fsl = tuple(_lib.ptr(a) for a in (slots.fsl or (None,) * 3))
             ops._launch("rnnt_search_lm_rows", 0.0, lambda: lib.sb_rnnt_search_lm_rows(
                 slots.lp.data_ptr(), _lib.ptr(slots.flp), *fsl, kp or 0,
-                tl_dev.data_ptr(), t, level, B, T, S, V1, K, blank,
-                ctypes.byref(tables), weight, bonus, ws.data_ptr(), nbytes, sp))
+                tl_dev.data_ptr(), t, level, B, T, S, V1, K, blank, *lm_args, ws.data_ptr(),
+                nbytes, sp))
             ops._launch("rnnt_search", 0.0, lambda: lib.sb_rnnt_search_round_lm(
                 _lib.ptr(slots.flp), *fsl, kp or 0, tl_dev.data_ptr(), t, level,
                 max_len, slots.par.data_ptr(), slots.sym.data_ptr(),
@@ -219,20 +217,13 @@ def _search_frame(lib, provider, slots, tl_dev, t, cur, max_len, blank, ws, nbyt
         _lib.ptr(fy), Hj, cur, S + 1 - cur, B, T, S, K, ws.data_ptr(), nbytes, sp))
 
 
-def _lm_args(fusion, dev):
-    if fusion is None:
-        return None
-    tables, _ = fusion[0].device_tables(dev)
-    return tables, float(fusion[1]), float(fusion[2])
-
-
 def _search_once(provider, tl, T, K, S, max_len, L, blank, kp, fusion=None):
     """one search at list length kp (None: full rows); fusion: None or (NGramLM, lm_weight,
     insertion_bonus) -> (label lists, scores, flag counts)"""
     lib = _lib.load()
     B, V1, dev = provider.B, provider.V1, provider.device
     slots = SearchSlots(B, K, S, T, V1, kp, dev, fused=fusion is not None)
-    lm_args = _lm_args(fusion, dev)
+    lm_args = () if fusion is None else fusion_args(*fusion, dev)
     nbytes = _lib.workspace_size(lib.sb_rnnt_search_workspace_size, B, T, S, K)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     tl_dev = torch.tensor(tl, dtype=torch.int32).pin_memory().to(dev, non_blocking=True)
@@ -368,7 +359,7 @@ class StreamSearch:
         self.max_len = Tm * S if max_len is None else min(int(max_len), Tm * S)
         self.kp = None if decode_static_fits(K, V1) else SHORTLIST_RERUN
         self.slots = SearchSlots(B, K, S, Tm, V1, self.kp, dev, fused=lm is not None)
-        self.lm_args = _lm_args(None if lm is None else (lm, lm_weight, insertion_bonus), dev)
+        self.lm_args = fusion_args(lm, lm_weight, insertion_bonus, dev)
         self.nbytes = _lib.workspace_size(lib.sb_rnnt_search_workspace_size, B, Tm, S, K)
         self.ws = torch.empty(self.nbytes, dtype=torch.uint8, device=dev)
         self.frames = [0] * B

@@ -114,13 +114,14 @@ def test_nbest_equals_the_reference_beam(cuda_lib, K):
 
 
 @pytest.mark.parametrize("C,K", [(12, 4), (12, 32), (5000, 4)])
-def test_nbest_of_uneven_chunks_is_the_same(cuda_lib, C, K):
+def test_stream_search_nbest_of_uneven_chunks_is_the_same(cuda_lib, C, K):
     from speech_b200.functions import s2s
+    from speech_b200.models.ctc_decoder import StreamSearch
     B, T = 3, 40
     logp = _logp(B, T, C, 7 + K)
     lens = [T, 29, 17]
     whole = s2s.ctc_first_pass(logp, lens, K)
-    state = s2s.ctc_stream_state(B, T, K, logp.device)
+    search = StreamSearch(B, T, K, C - 1, logp.device)
     rng = np.random.RandomState(K)
     pos = [0] * B
     while any(p < n for p, n in zip(pos, lens)):
@@ -129,9 +130,9 @@ def test_nbest_of_uneven_chunks_is_the_same(cuda_lib, C, K):
         chunk = torch.zeros(B, Tc, C, device="cuda")
         for b in range(B):
             chunk[b, :step[b]] = logp[b, pos[b]:pos[b] + step[b]]
-        s2s.ctc_stream_step(state, chunk.contiguous(), step, K, C - 1, T)
+        search.push(chunk.contiguous(), step)
         pos = [p + s for p, s in zip(pos, step)]
-    got = s2s.ctc_nbest(state, B, T, K, logp.device)
+    got = search.nbest()
     ln = whole[1].cpu()
     assert torch.equal(got[1].cpu(), ln)
     assert torch.equal(got[2].cpu(), whole[2].cpu())

@@ -55,7 +55,7 @@ def run_stream(st, feats, chunk):
             logp = st._logp(X, Te) if Te else None
         e[1].record()
         if Te:
-            st._search(logp, emit)
+            st.search.push(logp, emit)
         e[2].record()
         e[2].synchronize()
         st._advance(xs, counts)
